@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py -- env steps/sec of the Anakin ff_ppo training step (BASELINE.json metric) on N B200s.
+"""bench.py -- env steps/sec of the Anakin ff_ppo training step (BASELINE.json metric) on N H100s.
 
-  python bench.py --gpus N --steps K --warmup W            (N>1: launched under torchrun by the driver)
+  python bench.py --gpus N --steps K --warmup W            (N>1: launch under torchrun)
   python bench.py --impl reference ...                     CPU arm: the torch-CPU port of the same step
+  python bench.py ... --dump-outputs DIR                   also write the last timed step's outputs as DIR/<name>.npy
 
 One "step" = one Anakin update step per GPU: T=128 env steps of E=4096 envs (rollout with the
 actor/critic MLP[256,256] forwards on synthetic Box obs_dim=64 observations), the GAE scan, and
@@ -10,7 +11,8 @@ actor/critic MLP[256,256] forwards on synthetic Box obs_dim=64 observations), th
 value = N * T * E * K / time (whole-job env steps/s), timed with CUDA events on the stream the work
 runs on, barrier + synchronize on both sides, MAX over ranks.  Working set per step (trajectory obs +
 next_obs = 2 x 128 MiB fp32, or 2 x 64 MiB bf16) exceeds L2 together with weights/activations, so no
-explicit L2 flush is needed between steps (stated in config.l2).
+explicit L2 flush is needed between steps (stated in config.l2).  The inputs are seeded (arch.seed): the same arguments
+give the same inputs on every run, so --dump-outputs of two builds can be compared array by array.
 """
 from __future__ import annotations
 
@@ -26,7 +28,7 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-METRIC = "env steps/sec Anakin PPO at 1/2/4/8 B200; GAE-scan HBM GB/s vs roofline"
+METRIC = "env steps/sec Anakin PPO at 1/2/4/8 H100; GAE-scan HBM GB/s vs roofline"
 E_PER_GPU, T, D, A, HIDDEN, EPOCHS, NMB = 4096, 128, 64, 8, (256, 256), 4, 16
 
 
@@ -67,11 +69,12 @@ def load_peaks():
     if os.path.exists(path):
         p = json.load(open(path))
         return {"hbm_gbs": p["hbm_gbs"], "bf16_tflops": p["bf16_tflops"], "bf16_tflops_sustained": p.get("bf16_tflops_sustained", p["bf16_tflops"]), "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback"}
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s -- a denominator, not a measured rate
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0, "source": "datasheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (read-only queries)."""
 
     Q = "clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -136,7 +139,7 @@ def run_reference(args):
 def workload_config(n, precision):
     return {"workload": f"ff_ppo Anakin, synthetic Box obs_dim={D}, MLP{list(HIDDEN)}, num_envs={E_PER_GPU}/GPU, rollout_len={T}, actions={A}, epochs={EPOCHS}, minibatches={NMB}",
             "total_num_envs": E_PER_GPU * n, "parallelism": f"dp{n}", "precision": precision,
-            "l2": "per-step working set (2x trajectory obs >= 128 MiB + activations) exceeds the 126 MB L2; no explicit flush"}
+            "l2": "per-step working set (2x trajectory obs >= 128 MiB + activations) exceeds the 50 MB L2; no explicit flush"}
 
 
 def _pick_threads():
@@ -239,6 +242,35 @@ def _one_minibatch(model, tr, perm, i, mb):
 
 
 # ----------------------------------------------------------------------------------------------------
+DUMP_SAMPLE = 1 << 20  # at most this many entries per array (a fixed, seeded sample of larger ones): 4 MB of float32 each
+
+
+def dump_outputs(path, out):
+    """What the timed path returned in its last step -- parameters, optimiser moments, training and episode metrics --
+    as <path>/<name>.npy (float32), for output-by-output comparison of two builds on the same seeded inputs."""
+    import numpy as np
+
+    os.makedirs(path, exist_ok=True)
+    ls = out.learner_state
+    arrays = {}
+    for net in ("actor", "critic"):
+        tree = getattr(ls.params, f"{net}_params")
+        arrays[f"{net}_params"] = tree.flat
+        arrays[f"{net}_params_bf16"] = tree.flat_bf16
+    arrays["adam_mu"], arrays["adam_nu"] = ls.params.actor_params.arena_mu, ls.params.actor_params.arena_nu
+    for name, v in out.train_metrics.items():
+        arrays[f"train_{name}"] = v
+    for name, v in out.episode_metrics.items():
+        arrays[f"episode_{name}"] = v
+    for name, v in arrays.items():
+        if v is None:
+            continue
+        a = v.detach().float().cpu().numpy().reshape(-1)
+        if a.size > DUMP_SAMPLE:
+            a = a[np.sort(np.random.default_rng(0).choice(a.size, DUMP_SAMPLE, replace=False))]
+        np.save(os.path.join(path, f"{name}.npy"), a.astype(np.float32))
+
+
 def run_ours(args):
     # Libraries (NCCL prints its version banner on stdout) must not pollute the ONE JSON line: everything
     # written to fd 1 during the run goes to stderr; the JSON line is written to the real stdout at the end.
@@ -310,12 +342,16 @@ def run_ours(args):
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     barrier()
     ev0.record()
+    out = None
     for _ in range(args.steps):
-        state = learn(state).learner_state
+        out = learn(state)
+        state = out.learner_state
     ev1.record()
     barrier()
     dt = ev0.elapsed_time(ev1) * 1e-3
     progress(f"timed region A done {dt:.3f}s")
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, out)
 
     # ---- spread: the same K-step region nine more times (median / min / max beside the contract's single region) ----
     region_ms = [dt / args.steps * 1e3]
@@ -376,7 +412,7 @@ def run_ours(args):
             ts = []
             for _ in range(5):
                 a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                if name == "gae":  # the GAE inputs (11.5 MB) would sit in L2: flush so HBM is what is measured
+                if name == "gae":  # the GAE inputs (11.5 MB) would sit in the 50 MB L2: flush so HBM is what is measured
                     ops._zeros_scratch(("flush",), 256 << 20, torch.device("cuda", local)).fill_(1)
                 a.record()
                 g.replay()
@@ -388,8 +424,8 @@ def run_ours(args):
         roll_f, upd_f = flops_per_env_step()
         upd_exec = executed_update_flops_per_env_step()
         upd_tflops = upd_f * T * E_PER_GPU / (phase_ms["update"] * 1e-3) / 1e12
-        # the timed region is a sub-second burst at (or near) the maximum SM clock with no power cap: the BURST cuBLAS
-        # figure is the honest denominator; the sustained one (seconds under the 1 kW cap) is given beside it
+        # with a MEASURED_PEAKS.json the burst figure is the denominator of a sub-second region without power capping and the
+        # sustained one otherwise; without it both are the data-sheet figure
         burst = (dt < 1.0) and not (set(clocks.get("reasons", [])) & {"sw_power_cap"})
         peak = peaks["bf16_tflops"] if burst else peaks["bf16_tflops_sustained"]
         traffic, traffic_src = committed_k3_traffic() if precision == "bf16" else (None, None)
@@ -398,7 +434,7 @@ def run_ours(args):
                     "frac_of_sustained_peak": upd_tflops / peaks["bf16_tflops_sustained"],
                     "frac_of_burst_peak": upd_tflops / peaks["bf16_tflops"],
                     "traffic": traffic, "traffic_unit": "dram bytes per minibatch step (K3a+K3b)", "traffic_source": traffic_src,
-                    "peak_source": f"{peaks['source']} ({'burst' if burst else 'sustained'} bf16 cuBLAS)",
+                    "peak_source": f"{peaks['source']} ({'burst' if burst else 'sustained'} bf16)",
                     "flops_per_env_step": upd_f, "flops_per_env_step_executed": upd_exec,
                     "achieved_executed": upd_exec * T * E_PER_GPU / (phase_ms["update"] * 1e-3) / 1e12}
         gae_gbs = 22.0 * T * E_PER_GPU / (phase_ms["gae"] * 1e-3) / 1e9
@@ -417,7 +453,7 @@ def run_ours(args):
                     ops.gae_ppo(rr, vv, bb, dd, tt, 0.99, 0.95, 1.0, 1, out=(oa, ot))
                 ts = []
                 reps = 5             # launches per event pair: behind the first one the queue is never empty, so the pair times the
-                for _ in range(7):   # GPU, not the Python call; inputs (1.9 GB) + outputs (1.1 GB) >> 126 MB L2: no flush needed
+                for _ in range(7):   # GPU, not the Python call; inputs (1.9 GB) + outputs (1.1 GB) >> 50 MB L2: no flush needed
                     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                     a.record()
                     for _ in range(reps):
@@ -471,6 +507,8 @@ def main():
     ap.add_argument("--precision", default=os.environ.get("STX_BENCH_PRECISION", "bf16"), choices=["f32", "bf16"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--nccl-allreduce", action="store_true", help="N>1: NCCL all-reduce + K4 instead of the fused NVLink all-reduce/optimiser kernel")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (float32, <= 64 MB)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,5 +1,5 @@
 /*
- * stx.h -- C ABI of libstoixb200.so: the B200-native kernels behind Stoix's Anakin ff_ppo hot path.
+ * stx.h -- C ABI of libstoixb200.so: the H100-native (sm_90a) kernels behind Stoix's Anakin ff_ppo hot path.
  *
  * The reference (EdanToledo/Stoix) has no FFI/plugin registry: its boundary is Python-level
  * (SURVEY.md section 8b).  This header is the C boundary a maintainer binds (ctypes stub in
@@ -39,7 +39,7 @@ extern "C" {
 
 /* Compute precision of the MLP GEMMs. */
 #define STX_PREC_F32 0  /* fp32 CUDA-core GEMMs: the parity path (reference is fp32 everywhere) */
-#define STX_PREC_BF16 1 /* bf16 operands on tcgen05 tensor cores, fp32 accumulate, fp32 master weights */
+#define STX_PREC_BF16 1 /* bf16 operands on wgmma tensor cores, fp32 accumulate, fp32 master weights */
 
 /* Torso activation (stoix/networks/utils.py:9-24; flax.linen functions).  STX_PREC_BF16 kernels implement RELU only. */
 #define STX_ACT_RELU 0
@@ -159,11 +159,11 @@ int stx_tc_debug_forward(const StxMlp* mlp, const void* x, int64_t ldx, int64_t 
  * kernel leaves idle) instead of queueing CTAs behind it.  Host-side state, read at launch time. */
 void stx_tc_set_forward_ctas(int n);
 
-/* Profiling hook: device buffer of >= 32 int64 that K3a's CTA 0 fills with clock64() stamps of its second
- * tile (MMA-warp slots 0..9, first epilogue warp slots 16..27); NULL disables.  Synchronous (not for capture). */
+/* Profiling hook kept for ABI compatibility: the K3a kernel of this build records no clock64() stamps, so the
+ * buffer is left untouched.  Synchronous (not for capture). */
 int stx_tc_debug_set_clock_buffer(long long* buf);
-/* Profiling hook of the fused K3 launch: device buffer of [148][8] int64 filled per CTA with
- * {role, total cycles, wait/stall breakdown ...} (see stx_tc_ppo.cu g_prof_buf); NULL disables. */
+/* Profiling hook of the K3 launches: device buffer of [gridDim][8] int64 filled per CTA of K3a / K3b with
+ * {role, total cycles, -, tiles (K3a) / -, -, chunks (K3b)} (see stx_tc_ppo.cu g_prof_buf); NULL disables. */
 int stx_tc_debug_set_prof_buffer(long long* buf);
 
 /* Categorical head ops on logits (E, A) -- tfd.Categorical (stoix/networks/heads.py:41) as used at

@@ -210,7 +210,7 @@ def init_mlp(rng, sizes: Sequence[int], head_scale: float, dtype=np.float64) -> 
 
 
 def _bf16_round(x: np.ndarray) -> np.ndarray:
-    """Round-to-nearest-even to bfloat16 precision (emulates the tcgen05 operand format).
+    """Round-to-nearest-even to bfloat16 precision (emulates the tensor-core operand format).
     uint32 arithmetic throughout (the carry of the rounding add never leaves 32 bits for finite inputs)."""
     x32 = np.ascontiguousarray(x, dtype=np.float32)
     u = x32.view(np.uint32)
@@ -233,7 +233,7 @@ def mlp_forward(p: MLPParams, x: np.ndarray, bf16_operands: bool = False):
     n = len(p.W)
     for i in range(n):
         if i < n - 1 and p.has_ln(i):
-            assert not bf16_operands, "the bf16 emulation covers the relu / no-LayerNorm networks of the tcgen05 path"
+            assert not bf16_operands, "the bf16 emulation covers the relu / no-LayerNorm networks of the bf16 tensor-core path"
             u = h @ p.W[i]                                          # Dense(use_bias=False), torso.py:26
             mean = u.mean(axis=-1, keepdims=True)
             rstd = 1.0 / np.sqrt(((u - mean) ** 2).mean(axis=-1, keepdims=True) + LN_EPS)

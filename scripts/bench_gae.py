@@ -27,7 +27,7 @@ def bench(T, E, quads=0, iters=20, flush=True):
     for _ in range(iters):
         if flush:
             flush_buf.fill_(1)
-        # traffic >> L2 (126 MB): several launches per event pair, so that the pair times the GPU and not the Python call that
+        # traffic >> L2 (50 MB): several launches per event pair, so that the pair times the GPU and not the Python call that
         # precedes the first launch on an idle queue (~50 us); smaller shapes: one launch per pair (L2 flushed in between)
         reps = 5 if 22.0 * T * E > 1e9 else 1
         s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)

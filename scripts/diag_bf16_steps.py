@@ -1,4 +1,4 @@
-"""Per-optimiser-step diagnosis of the bf16 (tcgen05) update against the bf16-rounding oracle in the LEARNER setting
+"""Per-optimiser-step diagnosis of the bf16 (wgmma) update against the bf16-rounding oracle in the LEARNER setting
 (real rollout values / GAE targets instead of independent random inputs).  For every minibatch step the gradient is
 taken from the kernels' CURRENT parameters on both sides, so trajectory divergence cannot hide (or fake) an error:
 

@@ -1,4 +1,4 @@
-"""Summarise an `ncu --set full` report (any kernels) into the profiles/ text format: per launch the duration, DRAM bytes,
+"""Summarise an `ncu --set full` report (any kernels) into a text summary: per launch the duration, DRAM bytes,
 DRAM / tensor / issue utilisation, occupancy, registers, grid.   python scripts/ncu_summary.py report.ncu-rep [note]"""
 import csv
 import subprocess

@@ -1,8 +1,8 @@
 """Driver for `ncu --set full`: ONE launch of every kernel of the hot path at the benchmark shapes (BASELINE config 2:
 E=4096, T=128, D=64, A=8, mb=32768), after a warm-up launch of each.  Summarise the report with
-scripts/ncu_summary.py -> profiles/rNN_kernels_ncu.txt.
+scripts/ncu_summary.py.
 
-    ncu --set full --clock-control none --import-source on --nvtx --nvtx-include "measure/" -o gpurun_out/all python scripts/profile_all.py
+    ncu --set full --clock-control none --import-source on --nvtx --nvtx-include "measure/" -o out/all python scripts/profile_all.py
 """
 import sys
 

@@ -1,8 +1,8 @@
 """Driver for `ncu --set full`: ONE launch of every kernel of the ff_sac update epoch (and the Sebulba / fp32 path's GEMMs) at the
 BASELINE configs[3] shapes (obs 17, act 6, batch 256 and 4096, actor MLP[256x4] silu, twin-Q MLP[256x4] LayerNorm silu, replay
-ring 1e6), after a warm-up launch of each.  Summarise with scripts/ncu_summary.py -> profiles/r02_sac_kernels_ncu.txt.
+ring 1e6), after a warm-up launch of each.  Summarise with scripts/ncu_summary.py.
 
-    ncu --set full --clock-control none --nvtx --nvtx-include "measure/" -o gpurun_out/sac python scripts/profile_sac_kernels.py [batch]
+    ncu --set full --clock-control none --nvtx --nvtx-include "measure/" -o out/sac python scripts/profile_sac_kernels.py [batch]
 """
 import sys
 

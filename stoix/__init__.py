@@ -1,4 +1,4 @@
-"""`stoix` import path of the B200 build: every `stoix.<module>` resolves to `stoix_b200.<module>` (same module object),
+"""`stoix` import path of this build: every `stoix.<module>` resolves to `stoix_b200.<module>` (same module object),
 so code written against the reference -- `from stoix.systems.ppo.anakin.ff_ppo import learner_setup`,
 `from stoix.utils.multistep import batch_truncated_generalized_advantage_estimation`, Hydra `_target_: stoix.networks...`
 strings -- runs on this framework unchanged.  The script-style launches of the reference

@@ -1,7 +1,7 @@
-"""In-tree build of libstoixb200.so (sm_100a only) with nvcc.
+"""In-tree build of libstoixb200.so (sm_90a, H100) with nvcc.
 
 `python -m stoix_b200.build` or `__graft_entry__.build()`.  Objects go to stoix_b200/lib/obj, the
-shared library to stoix_b200/lib/libstoixb200.so (git-ignored, but shipped to the GPU box).
+shared library to stoix_b200/lib/libstoixb200.so (git-ignored build products).
 nvcc cross-compiles without a GPU.
 """
 from __future__ import annotations
@@ -20,7 +20,7 @@ LIBDIR = ROOT / "lib"
 OBJDIR = LIBDIR / "obj"
 LIB = LIBDIR / "libstoixb200.so"
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -45,7 +45,7 @@ def _digest() -> str:
 
 
 def build_library(force: bool = False, verbose: bool = False) -> Path:
-    """Compile every .cu under csrc/ for sm_100a and link the C-ABI shared library."""
+    """Compile every .cu under csrc/ for sm_90a and link the C-ABI shared library."""
     OBJDIR.mkdir(parents=True, exist_ok=True)
     stamp = LIBDIR / "build.stamp"
     digest = _digest()

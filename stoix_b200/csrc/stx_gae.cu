@@ -214,7 +214,7 @@ __global__ void standardize_inplace_kernel(float* __restrict__ adv, int64_t n,
 // so the HBM read stream never stops.  The arithmetic is the code above, reading its inputs from shared memory.
 // Tile shapes: 32 envs x 128 timesteps (4 timesteps per thread, the association order of gae_scan_kernel) or 64 x 64 (2 per
 // thread, two segments per 128-step rollout): half as many distinct rows -- hence 2 MB pages -- in flight per tile, which is what
-// matters once the row pitch E * 4 B exceeds the page size (measured at E = 1 048 576: see profiles/r02_gae_bench.txt).
+// matters once the row pitch E * 4 B exceeds the page size .
 constexpr int kGStages = 3;
 template <int kGE, int kGT>
 struct GaeStageT {
@@ -443,8 +443,8 @@ int launch_gae_tma_shape(const PpoIn& in, int T, int E, int want, float* adv, fl
 int launch_gae_tma(const PpoIn& in, int T, int E, int want, float* adv, float* tgt, float* stats, double2* partials, unsigned int* counter,
                    cudaStream_t st) {
   if (E % 16 != 0 || !aligned16(in.done) || !aligned16(in.trunc)) return 1;  // TMA: 16-byte aligned rows of the byte arrays
-  // measured (profiles/r02_gae_bench.txt): 32 x 128 tiles up to E = 32768, 64 x 64 from E = 65536 (0.87 of the copy peak at
-  // E = 1 048 576 where 32 x 128 gets 0.72); code 502 = 128 x 32 tiles
+  // 32 x 128 tiles up to E = 32768, 64 x 64 from E = 65536: once the row pitch exceeds the page size, 64 x 64 tiles halve the
+  // rows (pages) in flight per tile; code 502 = 128 x 32 tiles
   if (g_quads_override == 502) return launch_gae_tma_shape<128, 32>(in, T, E, want, adv, tgt, stats, partials, counter, st);
   const bool wide = g_quads_override == 501 || (g_quads_override != 500 && E >= 65536);
   return wide ? launch_gae_tma_shape<64, 64>(in, T, E, want, adv, tgt, stats, partials, counter, st)
@@ -493,7 +493,7 @@ int launch_gae(const In& in, int T, int E, bool vec4, int standardize, float* ad
   } else if (vec4) {
     const int quads_total = E / 4;
     // Small E is latency-bound: more, smaller blocks.  Large E: 128-byte rows per warp access.
-    // measured on B200 (profiles/r01_gae_bench.txt): wider rows per block win once the grid is large
+    // wider rows per block once the grid is large
     int quads = quads_total >= 65536 ? 32 : (quads_total >= 8 * kNumSMs * 2 ? 8 : (quads_total >= 4 * kNumSMs ? 4 : 2));
     if (g_quads_override == 2 || g_quads_override == 4 || g_quads_override == 8 || g_quads_override == 16 ||
         g_quads_override == 32)

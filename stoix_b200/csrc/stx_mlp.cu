@@ -1,5 +1,5 @@
 // K1 (fp32 path) MLP forward, categorical head ops, and K3 (fp32 path) PPO minibatch gradients.
-// The bf16 tcgen05 implementations live in stx_tc_mlp.cu and are dispatched from here by precision.
+// The bf16 wgmma implementations live in stx_tc_mlp.cu and are dispatched from here by precision.
 #include "stx_common.cuh"
 #include "stx_ppo_loss.cuh"
 #include "stx_simt_gemm.cuh"

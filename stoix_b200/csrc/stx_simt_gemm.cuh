@@ -1,7 +1,7 @@
 // fp32 CUDA-core GEMM family for the parity path (STX_PREC_F32).
 //
 // The reference is fp32 everywhere (SURVEY.md "facts"), so this path keeps every product and
-// accumulation in fp32 and is what the tight-tolerance parity tests run.  The bf16 tcgen05 path
+// accumulation in fp32 and is what the tight-tolerance parity tests run.  The bf16 wgmma path
 // (stx_tc_*.cu) is the throughput path.  Three flavours of one 64x64x16 register-tiled kernel:
 //   FWD : U[m,n]  = sum_k H_prev[row(m),k] * W[k,n] (+ b[n])                nn.Dense, torso.py:26
 //   DX  : dU_prev[m,k] = (sum_n dY[m,n] * W[k,n]) * f'(U_prev[m,k])         backward through the activation (no-LayerNorm torso)
@@ -102,7 +102,7 @@ __device__ __forceinline__ void store_out(const GemmArgs& g, int64_t m, int n, f
 }
 
 // Register-tiled GEMM, one shared-memory stage + register prefetch: the global loads of step k+1 are issued before the products
-// of step k and land in registers while the FFMA2s run; (BM, BN, BK, TM, TN) = (64, 64, 16, 4, 4) for mid-size grids and
+// of step k and land in registers while the FMAs run; (BM, BN, BK, TM, TN) = (64, 64, 16, 4, 4) for mid-size grids and
 // (128, 128, 8, 8, 8) -- 64 accumulators per thread, 4 shared loads per 32 packed FMAs -- when that still fills the GPU.
 template <int MODE, int BM_, int BN_, int BK_, int TM_, int TN_>
 __global__ void __launch_bounds__((BM_ / TM_) * (BN_ / TN_)) gemm_kernel(GemmArgs g) {
@@ -204,7 +204,7 @@ __global__ void __launch_bounds__((BM_ / TM_) * (BN_ / TN_)) gemm_kernel(GemmArg
 #pragma unroll
       for (int i = 0; i < TM_; ++i)
 #pragma unroll
-        for (int j = 0; j < TN_ / 2; ++j) fma2(acc[i][j], a[i], make_float2(b[2 * j], b[2 * j + 1]));   // FFMA2: same bits as two FFMAs
+        for (int j = 0; j < TN_ / 2; ++j) fma2(acc[i][j], a[i], make_float2(b[2 * j], b[2 * j + 1]));
       if (MODE == DW) {
 #pragma unroll
         for (int j = 0; j < TN_; ++j) dbacc[j] += b[j];
@@ -359,7 +359,7 @@ __global__ void __launch_bounds__(kPanelThreads) gemm_panel_kernel(GemmArgs g) {
     for (int kk = half; kk < kc; kk += 2) {
       const float2 a = *reinterpret_cast<const float2*>(As + kk * kAsLd + ty * PTM);
       const float4 b = *reinterpret_cast<const float4*>(Bs + kk * kBsLd + tx * PTN);
-      fma2(acc2[0][0], a.x, make_float2(b.x, b.y)), fma2(acc2[0][1], a.x, make_float2(b.z, b.w));   // FFMA2: 4 instructions for the 2x4 tile
+      fma2(acc2[0][0], a.x, make_float2(b.x, b.y)), fma2(acc2[0][1], a.x, make_float2(b.z, b.w));
       fma2(acc2[1][0], a.y, make_float2(b.x, b.y)), fma2(acc2[1][1], a.y, make_float2(b.z, b.w));
       if (MODE == DW) dbacc[0] += b.x, dbacc[1] += b.y, dbacc[2] += b.z, dbacc[3] += b.w;
     }
@@ -425,14 +425,13 @@ __global__ void __launch_bounds__(kPanelThreads) gemm_panel_kernel(GemmArgs g) {
 }
 
 // One entry point for the three GEMM flavours: picks the tiling from the grid the 64x64 kernel would get.
-constexpr int kPanelBelowCtas = 148;
+constexpr int kPanelBelowCtas = kNumSMs;
 template <int MODE>
 inline cudaError_t launch_gemm(const GemmArgs& g, int splits, cudaStream_t st) {
   const int64_t out_rows = (MODE == DW) ? g.K : g.M;
   const int64_t ctas64 = ((out_rows + BM - 1) / BM) * ((g.N + BN - 1) / BN) * (MODE == DW ? splits : 1);
   const int64_t ctas128 = ((out_rows + 127) / 128) * ((g.N + 127) / 128) * (MODE == DW ? splits : 1);
-  // 128x128x8 tiles with 8x8 outputs per thread need ~136 registers -> one 256-thread block per SM, and measured SLOWER than the
-  // 64x64x16 tiles on every workload here (fp32 PPO update 97 -> 145 ms, recurrent update +10 %): kept for reference, not dispatched
+  // 128x128x8 tiles with 8x8 outputs per thread need ~136 registers -> one 256-thread block per SM; not dispatched by default
   // (STX_GEMM_128=1 enables it).
   static const bool big_tiles = [] { const char* e = getenv("STX_GEMM_128"); return e && e[0] == '1'; }();
   if (big_tiles && ctas128 >= kPanelBelowCtas) {

@@ -1,20 +1,18 @@
-// K1 (bf16 path): fused 3-layer MLP forward on tcgen05 tensor cores.
+// K1 (bf16 path): fused 3-layer MLP forward on Hopper tensor cores (wgmma).
 //
 // Reference semantics: FeedForwardActor / FeedForwardCritic.apply with an MLPTorso[256,256] and a Dense
 // head (stoix/networks/base.py:18-59, torso.py:24-33, heads.py:36,134):  out = (relu(relu(x W0 + b0) W1 +
 // b1)) W2 + b2.  The reference runs three XLA GEMMs + fusions per apply; here ONE persistent kernel keeps
 // all weights of the network resident in shared memory (W0 32 KB + W1 128 KB + W2 8 KB, bf16) and chains
-// the three GEMMs of a 128-row tile through tensor memory:
+// the three GEMMs of a 64-row tile through registers:
 //
-//   TMA(X tile, 128B swizzle) -> smem --tcgen05.mma SS--> D0 (TMEM, fp32) --epilogue: +b0, relu, bf16-->
-//   A1 (TMEM, packed bf16) --tcgen05.mma TS (A from TMEM)--> D1 --epilogue--> A2 --TS--> D2 --> +b2 -> HBM
+//   TMA(X tile, 128B swizzle) -> smem --wgmma SS--> acc (fp32 regs) --+b0, relu, bf16--> A1 (regs)
+//   --wgmma RS (A from registers)--> acc --epilogue--> A2 --RS--> head --> +b2 -> HBM
 //
 // so hidden activations never leave the SM (SURVEY.md 7 "Keeping activations out of HBM").
-// Warp roles (576 threads): warp 0 = TMA producer, warp 1 = MMA issuer (one elected lane) + TMEM
-// allocator, warps 2-17 = epilogue (warp w owns TMEM lanes 32*(w%4)..+31, one row per thread, 2 column chunks).
-// Operand layouts: X K-major SW128; W0/W1 row-major (in,out) loaded by TMA as [rows x 64-col] blocks =
-// MN-major SW128 B operands (the same image serves as the K-major B operand of the backward pass);
-// W2 (256 x A<=16) is staged by hand in the un-swizzled core-matrix layout.
+// Two warpgroups per CTA, each running its own sequence of 64-row tiles (one TMA X ring of 2 stages per warpgroup), so
+// the epilogue math of one warpgroup overlaps the MMAs of the other.  256-wide layers run as two N=128 halves to keep
+// the accumulator at 64 registers per thread.  Weight images: stx_tc_ptx.cuh.
 // Shapes: hidden = [256,256] exactly, input dim D <= 64 (multiple of 8; zero-filled by TMA), head <= 16.
 #include <cuda.h>
 
@@ -24,20 +22,16 @@
 namespace stx {
 namespace tc {
 
-constexpr int kTileM = 128;
+constexpr int kTileM = 64;
 constexpr int kH = 256;
-constexpr int kXStages = 2;
-constexpr int kEpiWarps = 16;                 // 4 per TMEM lane quarter: hides the tcgen05.ld / pack latencies
-constexpr int kThreads = 32 * (2 + kEpiWarps);  // warp 0 TMA, warp 1 MMA, warps 2.. epilogue
+constexpr int kWG = 2;
+constexpr int kThreads = 128 * kWG;
 
-// shared-memory map (bytes from a 1024-aligned base)
-constexpr uint32_t kOffW1 = 0;                         // 4 x [256 rows x 128 B]
-constexpr uint32_t kOffW0 = 131072;                    // 4 x [ 64 rows x 128 B]
-constexpr uint32_t kOffW2 = 163840;                    // 32 x 2 core matrices of 128 B
-constexpr uint32_t kOffX = 172032;                     // kXStages x [128 rows x 128 B]
-constexpr uint32_t kOffBias = kOffX + kXStages * 16384;  // b0[256] b1[256] b2[16]
+// shared-memory map (bytes from a 1024-aligned base): weight images, then per warpgroup 2 X stages of 8 KB
+constexpr uint32_t kOffX = kImgWBytes;
+constexpr uint32_t kOffBias = kOffX + kWG * 2 * 8192;  // b0[256] b1[256] b2[16]
 constexpr uint32_t kOffBar = kOffBias + (256 + 256 + 16) * 4;
-constexpr uint32_t kSmemBytes = kOffBar + 128 + 1024;  // + alignment slack
+constexpr uint32_t kSmemBytes = kOffBar + 64 + 1024;  // + alignment slack
 
 struct FwdParams {
   const __nv_bfloat16* w2;  // [256 x A] row-major (bf16 shadow arena)
@@ -50,6 +44,17 @@ struct FwdParams {
   int num_tiles;
 };
 
+__device__ __forceinline__ void store_dbg(float* dbg, const uint32_t (&a)[64], int64_t row, int64_t M, int lane) {
+#pragma unroll
+  for (int i = 0; i < 64; ++i) {
+    const int64_t rr = row + 8 * (i & 1);
+    if (rr < M) {
+      const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(&a[i]);
+      *reinterpret_cast<float2*>(dbg + rr * kH + 8 * (i >> 1) + 2 * (lane & 3)) = make_float2(__bfloat162float(v.x), __bfloat162float(v.y));
+    }
+  }
+}
+
 __global__ void __launch_bounds__(kThreads, 1)
     tc_mlp_fwd_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW0,
                       const __grid_constant__ CUtensorMap tmW1, const FwdParams p) {
@@ -61,207 +66,64 @@ __global__ void __launch_bounds__(kThreads, 1)
   float* s_b1 = s_b0 + 256;
   float* s_b2 = s_b1 + 256;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBar);
-  uint64_t* x_full = bars;             // [kXStages]
-  uint64_t* x_empty = bars + 2;        // [kXStages]
-  uint64_t* w_full = bars + 4;
-  uint64_t* d_ready = bars + 5;      // [4] MMA -> epilogue: 64-column part p of the current layer's accumulator is complete
-  uint64_t* chunk_done = bars + 9;   // [4] epilogue -> MMA: part p consumed and its slice of the next A operand written
-  uint64_t* head_ready = bars + 13;  // head GEMM complete
-  uint64_t* head_done = bars + 14;   // head read out of tensor memory
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 15);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint64_t* w_full = bars;
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127, warp = t >> 5, lane = threadIdx.x & 31;
+  uint64_t* x_full = bars + 1 + 2 * wg;  // [2] per warpgroup
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < kXStages; ++s) {
-      mbar_init(&x_full[s], 1);
-      mbar_init(&x_empty[s], 1);
-    }
     mbar_init(w_full, 1);
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(&d_ready[i], 1);
-      mbar_init(&chunk_done[i], 8);  // 4 lane quarters x 2 chunks of 32 columns
-    }
-    mbar_init(head_ready, 1);
-    mbar_init(head_done, 4);
+    for (int i = 0; i < 2 * kWG; ++i) mbar_init(&bars[1 + i], 1);
     fence_barrier_init();
     tma_prefetch_desc(&tmX);
-    tma_prefetch_desc(&tmW0);
-    tma_prefetch_desc(&tmW1);
+    mbar_arrive_expect_tx(w_full, 32768 + 131072);
+    for (int j = 0; j < 4; ++j) tma_load_2d(smem + kImgW0 + j * 8192, &tmW0, w_full, j * 64, 0);
+    for (int j = 0; j < 4; ++j) tma_load_2d(smem + kImgW1 + j * 32768, &tmW1, w_full, j * 64, 0);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  // W2 image: element (j, n) at (j/8)*256 + (n/8)*128 + (j%8)*16 + (n%8)*2, zero for n >= A
-  {
-    // one thread per W2 row: all of its (<=16) loads are independent and in flight together
-    uint8_t* w2s = smem + kOffW2;
-    for (int j = threadIdx.x; j < kH; j += kThreads) {
-      uint32_t pk[8];
-      if (p.A == 8 && (reinterpret_cast<uintptr_t>(p.w2) & 15) == 0) {
-        const uint4 v = *reinterpret_cast<const uint4*>(p.w2 + j * 8);
-        pk[0] = v.x, pk[1] = v.y, pk[2] = v.z, pk[3] = v.w, pk[4] = pk[5] = pk[6] = pk[7] = 0u;
-      } else {
-        unsigned short e[16];
-#pragma unroll
-        for (int n = 0; n < 16; ++n) e[n] = n < p.A ? reinterpret_cast<const unsigned short*>(p.w2)[j * p.A + n] : (unsigned short)0;
-#pragma unroll
-        for (int n = 0; n < 8; ++n) pk[n] = (uint32_t)e[2 * n] | ((uint32_t)e[2 * n + 1] << 16);
-      }
-      uint8_t* dst = w2s + (j >> 3) * 256 + (j & 7) * 16;   // element (j, n) at (j/8)*256 + (n/8)*128 + (j%8)*16 + (n%8)*2
-      *reinterpret_cast<uint4*>(dst) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-      *reinterpret_cast<uint4*>(dst + 128) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-    }
-    for (int i = threadIdx.x; i < 256; i += kThreads) s_b0[i] = p.b0[i], s_b1[i] = p.b1[i];
-    if (threadIdx.x < 16) s_b2[threadIdx.x] = threadIdx.x < p.A ? p.b2[threadIdx.x] : 0.f;
-    fence_async_proxy();  // generic-proxy smem writes -> visible to the tensor-core (async) proxy
-  }
-  tc_fence_before();
+  stage_w2_bias(smem, p.w2, p.b0, p.b1, p.b2, p.A, s_b0, s_b1, s_b2);
+  fence_async_proxy();  // generic-proxy smem writes -> visible to the tensor-core (async) proxy
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  const int my_tiles = (p.num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    if (elect_one()) {
-      mbar_arrive_expect_tx(w_full, 32768 + 131072);
-      for (int j = 0; j < 4; ++j) tma_load_2d(smem + kOffW0 + j * 8192, &tmW0, w_full, j * 64, 0);
-      for (int j = 0; j < 4; ++j) tma_load_2d(smem + kOffW1 + j * 32768, &tmW1, w_full, j * 64, 0);
-      for (int it = 0; it < my_tiles; ++it) {
-        const int s = it % kXStages;
-        if (it >= kXStages) mbar_wait(&x_empty[s], ((it / kXStages) & 1) ^ 1, 1);
-        const int tile = blockIdx.x + it * gridDim.x;
-        mbar_arrive_expect_tx(&x_full[s], 16384);
-        tma_load_2d(smem + kOffX + s * 16384, &tmX, &x_full[s], 0, tile * kTileM);
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    // Every 256-wide GEMM is issued as four N=64 column parts; part p of the NEXT layer only needs D part p consumed
-    // and the K-chunks of its A operand written (chunk_done[]), so the tensor pipe trails the epilogue part by part
-    // (same scheme as K3a in stx_tc_ppo.cu).  h1 and h2 live in separate TMEM regions for that reason.
-    constexpr uint32_t idesc_n64 = idesc_bf16(128, 64, 0, 1);
-    constexpr uint32_t idesc_n16 = idesc_bf16(128, 16, 0, 1);
-    const uint32_t tmem_d = tmem, tmem_a1 = tmem + 256, tmem_a2 = tmem + 384;
-    // rolled part/group loops with incremental descriptors (see stx_tc_ppo.cu: code size / instruction cache)
-    auto adv = [](uint64_t desc, uint32_t bytes) { return desc + (uint64_t)(bytes >> 4); };
-    const uint64_t dW0 = smem_desc(sbase + kOffW0, 8192, 1024, SWIZZLE_128B), dW1 = smem_desc(sbase + kOffW1, 32768, 1024, SWIZZLE_128B);
-    const uint64_t dW2 = smem_desc(sbase + kOffW2, 256, 128, SWIZZLE_NONE);
-    mbar_wait(w_full, 0, 2);
-    for (int it = 0; it < my_tiles; ++it) {
-      const int s = it % kXStages;
-      mbar_wait(&x_full[s], (it / kXStages) & 1, 3);
-      if (it > 0) mbar_wait(head_done, (it - 1) & 1, 4);  // the previous tile's head has left D columns 0..15
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t dX = smem_desc(sbase + kOffX + s * 16384, 16, 1024, SWIZZLE_128B);
-#pragma unroll 1
-        for (int pt = 0; pt < 4; ++pt) {  // layer 0: D0 = X (K-major SW128) * W0 (MN-major SW128), K = 64
-          const uint64_t b0 = adv(dW0, pt * 8192);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) mma_ss(tmem_d + pt * 64, adv(dX, k * 32), adv(b0, k * 2048), idesc_n64, k > 0);
-          mma_commit(&d_ready[pt]);
-        }
-        mma_commit(&x_empty[s]);
-      }
-      __syncwarp();
-#pragma unroll 1
-      for (int j = 0; j < 4; ++j) {  // layer 1: D1 = A1 (TMEM) * W1, K = 256, trailing E0
-        mbar_wait(&chunk_done[j], 0, 34);
-        tc_fence_after();
-        if (elect_one()) {
-#pragma unroll 1
-          for (int pt = 0; pt <= j; ++pt) {
-#pragma unroll 1
-            for (int g = (pt == j ? 0 : j); g <= j; ++g) {  // K steps 4g .. 4g+3
-              const uint64_t b0 = adv(dW1, pt * 32768 + g * 8192);
-              const uint32_t a0 = tmem_a1 + g * 32;
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk) mma_ts(tmem_d + pt * 64, a0 + kk * 8, adv(b0, kk * 2048), idesc_n64, (g | kk) != 0);
-            }
-            if (j == 3) mma_commit(&d_ready[pt]);
-          }
-        }
-        __syncwarp();
-      }
-#pragma unroll 1
-      for (int j = 0; j < 4; ++j) {  // head: D2 = A2 (TMEM) * W2 (un-swizzled core matrices), N = 16, trailing E1
-        mbar_wait(&chunk_done[j], 1, 35);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t b0 = adv(dW2, j * 2048);
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) mma_ts(tmem_d, tmem_a2 + j * 32 + kk * 8, adv(b0, kk * 512), idesc_n16, (j | kk) != 0);
-          if (j == 3) mma_commit(head_ready);
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-    // ===================== epilogue warps: lane quarter q = warp % 4, `sub` picks the column chunk of a step =============
-    // step cc handles the 32-column chunks cc*kSub + sub (kSub warps per lane quarter): two 64-column parts per step
-    constexpr int kSub = kEpiWarps / 4, kSteps = 8 / kSub;
-    const int q = warp & 3, sub = (warp - 2) >> 2;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const uint32_t tmem_d = tmem + lane_addr, tmem_a1 = tmem + lane_addr + 256, tmem_a2 = tmem + lane_addr + 384;
-    for (int it = 0; it < my_tiles; ++it) {
-      const int tile = blockIdx.x + it * gridDim.x;
-      const int64_t row = (int64_t)tile * kTileM + q * 32 + lane;
-#pragma unroll 1
-      for (int layer = 0; layer < 2; ++layer) {
-        const float* bias = layer == 0 ? s_b0 : s_b1;
-        float* dbg = layer == 0 ? p.dbg_h1 : p.dbg_h2;
-        const uint32_t ta = layer == 0 ? tmem_a1 : tmem_a2;
-#pragma unroll 1
-        for (int cc = 0; cc < kSteps; ++cc) {
-          const int c = cc * kSub + sub, part = c >> 1;
-          mbar_wait(&d_ready[part], layer, 7 + layer);  // layer 0 / 1 are the 1st / 2nd completion of d_ready per tile
-          tc_fence_after();
-          uint32_t r[32], pk[16];
-          tmem_ld32(tmem_d + c * 32, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            pk[j] = bias_relu_pack_bf16(r[2 * j], r[2 * j + 1], *reinterpret_cast<const float2*>(bias + c * 32 + 2 * j));
-          }
-          tmem_st16(ta + c * 16, pk);
-          tmem_st_wait();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&chunk_done[part]);
-          if (dbg != nullptr && row < p.M) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              __nv_bfloat162 h = *reinterpret_cast<__nv_bfloat162*>(&pk[j]);
-              dbg[row * kH + c * 32 + 2 * j] = __bfloat162float(h.x);
-              dbg[row * kH + c * 32 + 2 * j + 1] = __bfloat162float(h.y);
-            }
-          }
-        }
-      }
-      // head (one row per thread: the sub == 0 warps)
-      if (sub == 0) {
-        mbar_wait(head_ready, it & 1, 9);
-        tc_fence_after();
-        uint32_t r[16];
-        tmem_ld16(tmem_d, r);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(head_done);  // the head is in registers: layer 0 of the next tile may overwrite D
-        if (row < p.M) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-            if (j < p.A) p.out[row * p.A + j] = __uint_as_float(r[j]) + s_b2[j];
-        }
-      }
-    }
+  const int n_wg = (int)gridDim.x * kWG, g = (int)blockIdx.x * kWG + wg;
+  const int my_tiles = g < p.num_tiles ? (p.num_tiles - g + n_wg - 1) / n_wg : 0;
+  uint8_t* xs = smem + kOffX + wg * 16384;
+  if (t == 0 && my_tiles > 0) {
+    mbar_arrive_expect_tx(&x_full[0], 8192);
+    tma_load_2d(xs, &tmX, &x_full[0], 0, g * kTileM);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 512);
+  mbar_wait(w_full, 0, 1);
+  for (int it = 0; it < my_tiles; ++it) {
+    const int s = it & 1, tile = g + it * n_wg;
+    wg_sync(1 + wg);  // every warp of this warpgroup is done with stage s ^ 1 (tile it - 1)
+    if (t == 0 && it + 1 < my_tiles) {
+      mbar_arrive_expect_tx(&x_full[s ^ 1], 8192);
+      tma_load_2d(xs + (s ^ 1) * 8192, &tmX, &x_full[s ^ 1], 0, (tile + n_wg) * kTileM);
+    }
+    mbar_wait(&x_full[s], (it >> 1) & 1, 2);
+    const int64_t row = (int64_t)tile * kTileM + warp * 16 + (lane >> 2);
+    float acc[64];
+    uint32_t a1[64], a2[64];
+    wg_zero(acc);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      gemm_x_w0(acc, smem_u32(xs + s * 8192), sbase, h);
+      epi_bias_relu(acc, s_b0, h, a1, lane);
+    }
+    if (p.dbg_h1 != nullptr) store_dbg(p.dbg_h1, a1, row, p.M, lane);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      gemm_a_w1(acc, a1, sbase, h);
+      epi_bias_relu(acc, s_b1, h, a2, lane);
+    }
+    if (p.dbg_h2 != nullptr) store_dbg(p.dbg_h2, a2, row, p.M, lane);
+    float z[8];
+    wg_zero(z);
+    gemm_a_w2(z, a2, sbase);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {  // z[i]: row + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (lane % 4) + (i & 1)
+      const int64_t rr = row + 8 * ((i >> 1) & 1);
+      const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
+      if (rr < p.M && col < p.A) p.out[rr * p.A + col] = z[i] + s_b2[col];
+    }
   }
 }
 
@@ -306,14 +168,14 @@ int make_map_2d_pub(CUtensorMap* m, const void* base, uint64_t rows, uint64_t co
 
 // Tiled activation matrix [tiles*128 rows x 8*colgroups] (layout of stx_tc_ppo.cu::tiled_ptr) seen as a 2D
 // array of 8-byte words: inner = the 2 KB (128 rows x 16 B) block of one (tile, column group), outer =
-// tile*colgroups + group.  Box = 64 rows (128 words) x all column groups, no swizzle.
-int make_map_tiled(CUtensorMap* m, const void* base, uint64_t tiles, uint32_t colgroups) {
+// tile*colgroups + group.  Box = 64 rows (128 words) x box_cg column groups, no swizzle.
+int make_map_tiled(CUtensorMap* m, const void* base, uint64_t tiles, uint32_t colgroups, uint32_t box_cg) {
   EncodeTiledFn enc = get_encode();
   STX_REQUIRE(enc != nullptr, STX_E_UNSUPPORTED, "cuTensorMapEncodeTiled is not available from this driver");
   STX_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0, STX_E_ALIGN, "TMA source must be 16-byte aligned");
   cuuint64_t dims[2] = {256, tiles * colgroups};
   cuuint64_t strides[1] = {2048};
-  cuuint32_t box[2] = {128, colgroups};
+  cuuint32_t box[2] = {128, box_cg};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT64, 2, const_cast<void*>(base), dims, strides, box, estr,
                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -355,7 +217,8 @@ int tc_forward_impl(const StxMlp* m, const void* x, int64_t ldx, int64_t M, floa
     attr_set = true;
   }
   const int cap = (g_forward_ctas > 0 && g_forward_ctas < kNumSMs) ? g_forward_ctas : kNumSMs;
-  const int grid = p.num_tiles < cap ? p.num_tiles : cap;
+  const int want = (p.num_tiles + kWG - 1) / kWG;
+  const int grid = want < cap ? want : cap;
   tc_mlp_fwd_kernel<<<grid, kThreads, kSmemBytes, st>>>(tmX, tmW0, tmW1, p);
   STX_LAUNCH_OK();
   return STX_OK;

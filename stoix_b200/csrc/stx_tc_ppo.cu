@@ -1,26 +1,23 @@
-// K3 (bf16 path): the PPO minibatch gradient step on tcgen05 tensor cores.
+// K3 (bf16 path): the PPO minibatch gradient step on Hopper tensor cores (wgmma).
 //
 // Reference semantics: _actor_loss_fn / _critic_loss_fn + jax.grad for one minibatch
 // (stoix/systems/ppo/anakin/ff_ppo.py:184-247; losses stoix/utils/loss.py:17-32,68-78).  Three launches:
 //
 //  tc_ppo_fwd_bwd_kernel (K3a)  one persistent CTA per SM; CTAs [0, n_a) run the actor, the rest the critic.
-//      Per 128-row tile (rows gathered through the shuffle permutation straight into 128B-swizzled smem):
+//      Two warpgroups per CTA, each running its own sequence of 64-row tiles (rows gathered through the shuffle
+//      permutation straight into 128B-swizzled smem):
 //        G0 X*W0 -> E0 h1=relu(.+b0) -> G1 h1*W1 -> E1 h2 -> G2 h2*W2 -> E2 loss + d(logits|value) ->
 //        G3 dz*W2^T -> E3 dh2 = .*(h2>0) -> G4 dh2*W1^T -> E4 dh1 = .*(h1>0)
-//      All five GEMMs run on tcgen05 with the hidden activations resident in tensor memory (A operand
-//      from TMEM); W1's single smem image serves as MN-major B (forward) and K-major B (backward).
-//      Every 256-wide GEMM is issued as four N=64 column parts with their own mbarriers, so the tensor pipe
-//      trails the epilogue part by part (TMEM is full: two tiles cannot be in flight).
-//      Epilogue warps also emit h1, h2, dh2, dh1, dz (bf16) for the weight-gradient GEMMs -- deferred, one
-//      512-byte store at a time between the column groups of the next chunk, because the SM's store path
-//      (32 B/clk) is this kernel's roofline --, reduce the layer-1 / head bias gradients with a shuffle
-//      butterfly and accumulate the loss metrics.
+//      All five GEMMs run on wgmma with the activations resident in registers (A operand from registers: the
+//      accumulator of one GEMM packed to bf16 is the A operand of the next); W1's single smem image serves as
+//      MN-major B (forward) and K-major B (backward).  256-wide GEMMs run as two N=128 halves (64 accumulator
+//      registers).  The epilogues also emit h1, h2, dh2, dh1, dz (bf16) for the weight-gradient GEMMs, reduce the
+//      bias gradients (quad butterfly + per-warp smem slices, fixed order) and accumulate the loss metrics.
 //  tc_dw_kernel (K3b)  split-K GEMMs dW = A^T * B over the minibatch rows with both operands MN-major,
-//      3-stage TMA/mbarrier pipeline, 256 x N fp32 accumulators in TMEM:
-//        dW1 = h1^T dh2 (N=256), dW2 = h2^T dz (N=16), dW0^T = dh1^T x (N=64) + db0 = dh1^T 1 (ones-operand MMA).
+//      4-stage TMA/mbarrier pipeline (one producer warp), two consumer warpgroups with 128 x N fp32 accumulators each:
+//        dW1 = h1^T dh2 (two jobs of N=128), dW2 = h2^T dz (N=16), dW0^T = dh1^T x (N=64).
 //      The activations travel K3a -> K3b in a tiled layout [tile of 128 rows][8-column group][row][8]:
-//      a warp of K3a (one row per thread) stores 512 contiguous bytes per instruction, and one TMA box of
-//      K3b lands 64 rows of every column group as un-swizzled UMMA core matrices (8 rows x 16 B).
+//      one TMA box of K3b lands 64 rows of every column group as un-swizzled core matrices (8 rows x 16 B).
 //  tc_reduce_kernel     fixed-order reduction of the per-CTA partials into the flat fp32 gradient arena
 //      (deterministic; also the bias gradients and the six loss metrics); optionally fused with clip + Adam
 //      (stx_ppo_minibatch_update).
@@ -39,37 +36,22 @@ namespace tc {
 
 int make_map_2d_pub(CUtensorMap* m, const void* base, uint64_t rows, uint64_t cols, uint64_t pitch_elems, uint32_t box_rows,
                     uint32_t box_cols);  // stx_tc_mlp.cu (SWIZZLE_128B bf16)
-int make_map_tiled(CUtensorMap* m, const void* base, uint64_t tiles, uint32_t colgroups);  // stx_tc_mlp.cu
+int make_map_tiled(CUtensorMap* m, const void* base, uint64_t tiles, uint32_t colgroups, uint32_t box_cg);  // stx_tc_mlp.cu
 
-// optional timeline instrumentation (scripts/profile_k3_timeline.py): clock64 stamps of CTA 0, tile 1
+// optional instrumentation hooks of the C ABI (stx_tc_debug_set_*_buffer): [gridDim][8] per-CTA cycle counts
 __device__ long long* g_clock_buf = nullptr;
-#define STX_STAMP_AT(slot, cond)                                   \
-  do {                                                             \
-    if (clk_buf != nullptr && (cond)) clk_buf[slot] = clock64();   \
-  } while (0)
-#define STX_STAMP(slot) STX_STAMP_AT(slot, it == 1 && lane == 0)
-// optional per-CTA cycle accounting of the fused launch (scripts/profile_k3_fused.py): [gridDim][8] long long
-//   K3a CTAs: 0 role id (1), 1 total, 2 cycles inside flag_signal (epilogue warp 5), 3 tiles
-//   dW CTAs:  0 role id (2 + job), 1 total, 2 TMA thread waiting for flags, 3 TMA thread waiting for a free stage,
-//             4 MMA thread waiting for a full stage, 5 pipeline iterations
 __device__ long long* g_prof_buf = nullptr;
 
-constexpr int kTileM = 128;
 constexpr int kH = 256;
-// warps 0..3 gather producers (one row per thread), warp 4 MMA, warps 5.. epilogue (8 or 16 of them)
-constexpr int fb_threads(int nepi) { return 32 * (5 + nepi); }
-constexpr int kFbMmaWarp = 4;
+constexpr int kWTile = 64;               // rows per warpgroup tile
+constexpr int kFbThreads = 256;          // two warpgroups
 
 // ---- K3a shared-memory map ------------------------------------------------------------------------
-constexpr uint32_t kOffW1 = 0;
-constexpr uint32_t kOffW0 = 131072;
-constexpr uint32_t kOffW2 = 163840;
-constexpr uint32_t kOffX = 172032;                 // 2 stages x 16 KB
-constexpr uint32_t kOffDz = kOffX + 2 * 16384;     // 4 KB: dz tile, K-major core matrices
-constexpr uint32_t kOffBias = kOffDz + 4096;       // b0[256] b1[256] b2[16]
-constexpr uint32_t kOffDb = kOffBias + 528 * 4;    // [4 lane quarters][db0[256] db1[256] db2[16]] accumulators
-constexpr uint32_t kOffBar = kOffDb + 4 * 528 * 4;
-constexpr uint32_t kFbSmemBytes = kOffBar + 128 + 1024;
+constexpr uint32_t kOffX = kImgWBytes;               // 2 warpgroups x 8 KB
+constexpr uint32_t kOffBias = kOffX + 2 * 8192;      // b0[256] b1[256] b2[16]
+constexpr uint32_t kOffDb = kOffBias + 528 * 4;      // [8 warps][db0[256] db1[256] db2[16]] accumulators
+constexpr uint32_t kOffBar = kOffDb + 8 * 528 * 4;
+constexpr uint32_t kFbSmemBytes = kOffBar + 64 + 1024;
 
 struct FbNet {
   const __nv_bfloat16* w2;   // [256 x A] bf16
@@ -94,86 +76,89 @@ struct FbParams {
   int D;
   int mb;
   float clip_eps, ent_coef, vf_coef;
-  // fused launch (tc_ppo_fused_kernel): per-tile completion counters polled by the weight-gradient CTAs (nullptr: none)
-  uint32_t* flag_t;   // [2][tiles] every activation (h1, h2, dz, dh2, dh1) of (net, tile) stored -> kFlagEpi arrivals (one per epilogue warp)
-  uint32_t* flag_x;   // [tiles]    gathered input rows xg of tile stored                         -> kFlagGather arrivals (actor CTAs)
   int act_policy;     // L2 policy of the activation stores: 0 evict_first (read once, after a kernel boundary), 1 normal, 2 evict_last
-  int ring_tiles;     // activation workspace = ring of this many tile slots per network (tile t -> slot t % ring_tiles); 0: one slot per tile
 };
-constexpr uint32_t kFlagEpi = 8, kFlagGather = 4;
-
-// Release "this warp's stores of the tile are issued" to the consumer CTAs: the warp barrier orders the other lanes' stores
-// before lane 0's gpu-scope fence (the same barrier + single-thread fence pattern cooperative-groups grid.sync relies on).
-__device__ __forceinline__ void flag_signal(uint32_t* f, int lane) {
-  __syncwarp();
-  if (lane == 0) {
-    __threadfence();
-    asm volatile("red.relaxed.gpu.global.add.u32 [%0], %1;" ::"l"(f), "r"(1u) : "memory");
-  }
-}
-__device__ __forceinline__ void flag_signal_timed(uint32_t* f, int lane, long long& acc) {
-  const long long t0 = clock64();
-  flag_signal(f, lane);
-  acc += clock64() - t0;
-}
-__device__ __forceinline__ uint32_t ld_acquire_gpu(const uint32_t* f) {
-  uint32_t v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(f) : "memory");
-  return v;
-}
-__device__ __forceinline__ void fence_proxy_async_global() { asm volatile("fence.proxy.async.global;" ::: "memory"); }
 
 // Tiled activation layout shared by K3a (writer) and K3b (reader): element (row, col) of a [mb x 8*CG]
 // matrix lives at ((row/128 * CG + col/8) * 128 + row%128) * 8 + col%8.
-__device__ __forceinline__ uint4* tiled_ptr(__nv_bfloat16* base, int64_t row, int cg, int CG) {
-  return reinterpret_cast<uint4*>(base + (((row >> 7) * CG + cg) * 128 + (row & 127)) * 8);
+__device__ __forceinline__ __nv_bfloat16* tiled_ptr(__nv_bfloat16* base, int64_t row, int col, int CG) {
+  return base + (((row >> 7) * CG + (col >> 3)) * 128 + (row & 127)) * 8 + (col & 7);
 }
 
-// sum over the 32 lanes of a warp of v[i], i = 0..31: afterwards v[0] of lane l holds the total of
-// column l (reduce-scatter butterfly: 31 shuffles instead of 32 x 5).
-__device__ __forceinline__ float warp_colsum32(float (&v)[32], int lane) {
+// Stores half h of a packed 64 x 256 register operand (rows row0, row0 + 8 of the thread; see stx_tc_ptx.cuh) to the tiled layout.
+__device__ __forceinline__ void store_act(__nv_bfloat16* base, const uint32_t (&a)[64], int h, int64_t row0, int lane, uint64_t pol) {
 #pragma unroll
-  for (int s = 16; s >= 1; s >>= 1) {
+  for (int i = 32 * h; i < 32 * h + 32; ++i)
+    st_hint(reinterpret_cast<uint32_t*>(tiled_ptr(base, row0 + 8 * (i & 1), 8 * (i >> 1) + 2 * (lane & 3), 32)), a[i], pol);
+}
+
+// Column sums over the 64 rows of a warpgroup tile, half h: x = accumulator-layout values of this thread.  The 8 lanes that
+// share lane % 4 hold the same columns; a reduce-scatter butterfly leaves lane l with the totals of its entries 4 (l/4) .. +3.
+// dst: this warp's slice (every column written by exactly one lane of the warp: fixed order, no atomics).
+__device__ __forceinline__ void colsum_half(const float (&x)[64], float* dst, int h, int lane) {
+  float v[32];
 #pragma unroll
-    for (int i = 0; i < s; ++i) {
+  for (int j = 0; j < 16; ++j) {
+    v[2 * j] = x[4 * j] + x[4 * j + 2];
+    v[2 * j + 1] = x[4 * j + 1] + x[4 * j + 3];
+  }
+#pragma unroll
+  for (int s = 16; s >= 4; s >>= 1) {
+    const int n = 2 * s;  // values still held: 32, 16, 8 -> keep half of them
+#pragma unroll
+    for (int i = 0; i < n / 2; ++i) {
       const bool hi = (lane & s) != 0;
-      const float send = hi ? v[i] : v[i + s];
-      const float keep = hi ? v[i + s] : v[i];
+      const float send = hi ? v[i] : v[i + n / 2];
+      const float keep = hi ? v[i + n / 2] : v[i];
       v[i] = keep + __shfl_xor_sync(0xffffffffu, send, s);
     }
   }
-  return v[0];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int m = 4 * (lane >> 2) + k;
+    dst[128 * h + 8 * (m >> 1) + 2 * (lane & 3) + (m & 1)] += v[k];
+  }
 }
 
-// Actor head of one row: softmax statistics with ONE exponential per logit (e_j = exp(z_j - zmax), p_j = e_j / sum(e),
-// log p_j = (z_j - zmax) - log(sum(e))), the clipped-surrogate loss and d(loss)/d(logits) incl. the entropy bonus.
-// Fast intrinsics: this path carries bf16-level error anyway.  NA = compile-time bound on the action count.
-template <int NA>
-__device__ __forceinline__ void actor_head(const uint32_t (&r)[16], const float* s_b2, int A, int a, float logp_old, float adv,
-                                           float clip_eps, float ent_coef, float inv_m, float (&dz)[16], float& loss,
-                                           float& ent_out) {
-  float zs[NA], ex[NA], zmax = -INFINITY;
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+// Actor head of one row, spread over the 4 lanes of a quad (zz: this lane's 4 logits incl. bias, columns col[k]):
+// softmax statistics with ONE exponential per logit (e_j = exp(z_j - zmax), p_j = e_j / sum(e), log p_j = (z_j - zmax) -
+// log(sum(e))), the clipped-surrogate loss and d(loss)/d(logits) incl. the entropy bonus.  Fast intrinsics: this path
+// carries bf16-level error anyway.  Loss and entropy come out identical in the 4 lanes.
+__device__ __forceinline__ void actor_head_quad(float (&zz)[4], const int (&col)[4], int A, int a, float logp_old, float adv,
+                                                float clip_eps, float ent_coef, float inv_m, float (&dz)[4], float& loss, float& ent_out) {
+  float zmax = -INFINITY;
 #pragma unroll
-  for (int j = 0; j < NA; ++j) {
-    zs[j] = __uint_as_float(r[j]) + s_b2[j];
-    if (j < A) zmax = fmaxf(zmax, zs[j]);
-  }
-  float se = 0.f;
+  for (int k = 0; k < 4; ++k)
+    if (col[k] < A) zmax = fmaxf(zmax, zz[k]);
+  zmax = quad_max(zmax);
+  float ex[4], se = 0.f;
 #pragma unroll
-  for (int j = 0; j < NA; ++j) {
-    zs[j] -= zmax;
-    ex[j] = j < A ? __expf(zs[j]) : 0.f;
-    se += ex[j];
+  for (int k = 0; k < 4; ++k) {
+    zz[k] -= zmax;
+    ex[k] = col[k] < A ? __expf(zz[k]) : 0.f;
+    se += ex[k];
   }
+  se = quad_sum(se);
   const float lse = __logf(se), inv_se = 1.0f / se;
   float ent = 0.f, logp_a = 0.f;
 #pragma unroll
-  for (int j = 0; j < NA; ++j)
-    if (j < A) {
-      const float lp = zs[j] - lse;
-      ent -= ex[j] * inv_se * lp;
-      if (j == a) logp_a = lp;
+  for (int k = 0; k < 4; ++k)
+    if (col[k] < A) {
+      const float lp = zz[k] - lse;
+      ent -= ex[k] * inv_se * lp;
+      if (col[k] == a) logp_a = lp;
     }
+  ent = quad_sum(ent);
+  logp_a = quad_sum(logp_a);
   const float ratio = __expf(logp_a - logp_old);
   const float l1 = ratio * adv;
   const float l2 = fminf(fmaxf(ratio, 1.0f - clip_eps), 1.0f + clip_eps) * adv;
@@ -181,462 +166,212 @@ __device__ __forceinline__ void actor_head(const uint32_t (&r)[16], const float*
   const float dlogp = ((l1 < l2) || in_band) ? -adv * ratio * inv_m : 0.f;
   const float ce = ent_coef * inv_m;
 #pragma unroll
-  for (int j = 0; j < NA; ++j)
-    if (j < A) {
-      const float lp = zs[j] - lse, pr = ex[j] * inv_se;
-      dz[j] = dlogp * ((j == a ? 1.f : 0.f) - pr) + ce * pr * (lp + ent);
-    }
+  for (int k = 0; k < 4; ++k) {
+    const float lp = zz[k] - lse, pr = ex[k] * inv_se;
+    dz[k] = col[k] < A ? dlogp * ((col[k] == a ? 1.f : 0.f) - pr) + ce * pr * (lp + ent) : 0.f;
+  }
   loss = -fminf(l1, l2);
   ent_out = ent;
 }
 
-// The K3a CTA: called by tc_ppo_fwd_bwd_kernel (split launches) and by the producer CTAs of tc_ppo_fused_kernel.
-template <int NEPI>
-__device__ __forceinline__ void fb_role(uint8_t* smem_raw, const CUtensorMap& tmW0a, const CUtensorMap& tmW1a, const CUtensorMap& tmW0c,
-                                        const CUtensorMap& tmW1c, const FbParams& p) {
+__global__ void __launch_bounds__(kFbThreads, 1)
+    tc_ppo_fwd_bwd_kernel(const __grid_constant__ CUtensorMap tmW0a, const __grid_constant__ CUtensorMap tmW1a,
+                          const __grid_constant__ CUtensorMap tmW0c, const __grid_constant__ CUtensorMap tmW1c,
+                          const FbParams p) {
+  extern __shared__ uint8_t smem_raw[];
   // align by OFFSET (not through an integer cast) so that the compiler keeps the shared address space: LDS/STS, not generic LD/ST
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const uint32_t sbase = smem_u32(smem);
   const long long prof_t0 = clock64();
-  long long* const clk_buf = blockIdx.x == 0 ? g_clock_buf : nullptr;  // one load; the stamps themselves stay cheap
-  STX_STAMP_AT(56, threadIdx.x == 0);
   float* s_b0 = reinterpret_cast<float*>(smem + kOffBias);
   float* s_b1 = s_b0 + 256;
   float* s_b2 = s_b1 + 256;
-  float* s_db = reinterpret_cast<float*>(smem + kOffDb);  // [4][528]: one slice per lane quarter -> no atomics, fixed order
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBar);
-  uint64_t* x_full = bars;       // [2]
-  uint64_t* x_empty = bars + 2;  // [2]
-  uint64_t* w_full = bars + 4;
-  uint64_t* d_ready = bars + 5;      // [4] MMA -> epilogue: column part p of the current GEMM is complete
-  uint64_t* chunk_done = bars + 9;   // [4] epilogue -> MMA: part p consumed (and its slice of the next A operand written)
-  uint64_t* head_ready = bars + 13;  // G2 complete
-  uint64_t* head_done = bars + 14;   // dz tile in smem
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 15);
+  float* s_db = reinterpret_cast<float*>(smem + kOffDb);  // [8][528]: one slice per warp -> no atomics, fixed order
+  uint64_t* w_full = reinterpret_cast<uint64_t*>(smem + kOffBar);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7, t = threadIdx.x & 127, warp = threadIdx.x >> 5, wq = warp & 3, lane = threadIdx.x & 31;
+  const int q4 = lane & 3;
   const uint64_t pol_stream = l2_policy(p.act_policy);  // default evict_first: the activations are written once and read once (by K3b)
   const int which = (int)blockIdx.x < p.n_cta[0] ? 0 : 1;
   const FbNet& net = p.net[which];
   const int cta_in_net = which == 0 ? (int)blockIdx.x : (int)blockIdx.x - p.n_cta[0];
-  const int ncta = p.n_cta[which];
-  const int num_tiles = p.mb / kTileM;
-  const int ring = p.ring_tiles > 0 ? p.ring_tiles : (num_tiles > 0 ? num_tiles : 1);
-  const int my_tiles = cta_in_net < num_tiles ? (num_tiles - cta_in_net + ncta - 1) / ncta : 0;
+  const int n_wg = 2 * p.n_cta[which], g = 2 * cta_in_net + wg;
+  const int num_tiles = p.mb / kWTile;
+  const int my_tiles = g < num_tiles ? (num_tiles - g + n_wg - 1) / n_wg : 0;
   const CUtensorMap* tmW0 = which == 0 ? &tmW0a : &tmW0c;
   const CUtensorMap* tmW1 = which == 0 ? &tmW1a : &tmW1c;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&x_full[s], 4);  // one arrival per producer warp
-      mbar_init(&x_empty[s], 1);
-    }
     mbar_init(w_full, 1);
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(&d_ready[i], 1);
-      mbar_init(&chunk_done[i], 8);  // 4 lane quarters x 2 column halves
-    }
-    mbar_init(head_ready, 1);
-    mbar_init(head_done, 4);
     fence_barrier_init();
     tma_prefetch_desc(tmW0);
     tma_prefetch_desc(tmW1);
   }
   griddep_launch();  // K3b cannot co-reside with this CTA anyway; lets its launch be queued early
-  if (warp == kFbMmaWarp) tmem_alloc(tmem_slot, 512);
-  for (int i = threadIdx.x; i < 4 * 528; i += fb_threads(NEPI)) s_db[i] = 0.f;
+  for (int i = threadIdx.x; i < 8 * 528; i += kFbThreads) s_db[i] = 0.f;
   griddep_wait();  // everything above overlapped the previous optimiser kernel; the weights below are its output
-  // Start every long-latency fetch of the prologue at once: the 160 KB of W0/W1 (TMA), the first shuffle indices of the
-  // gather and loss-input rows, then the W2 / bias staging below; all of them are in flight together.
   if (threadIdx.x == 0) {
     mbar_arrive_expect_tx(w_full, 32768 + 131072);
-    const uint64_t pol_keep = l2_evict_last();  // the bf16 weights (K4's output) stay L2-resident for all 148 CTAs and the next step
-    for (int j = 0; j < 4; ++j) tma_load_2d_hint(smem + kOffW0 + j * 8192, tmW0, w_full, j * 64, 0, pol_keep);
-    for (int j = 0; j < 4; ++j) tma_load_2d_hint(smem + kOffW1 + j * 32768, tmW1, w_full, j * 64, 0, pol_keep);
+    const uint64_t pol_keep = l2_evict_last();  // the bf16 weights (K4's output) stay L2-resident for all CTAs and the next step
+    for (int j = 0; j < 4; ++j) tma_load_2d_hint(smem + kImgW0 + j * 8192, tmW0, w_full, j * 64, 0, pol_keep);
+    for (int j = 0; j < 4; ++j) tma_load_2d_hint(smem + kImgW1 + j * 32768, tmW1, w_full, j * 64, 0, pol_keep);
   }
-  int32_t idx_first = 0;  // producers: row of tile 0 owned by this thread; epilogue (sub 0): its loss-input row of tile 0
-  if (p.idx != nullptr && my_tiles > 0) {
-    if (warp < 4) idx_first = p.idx[(int64_t)cta_in_net * kTileM + threadIdx.x];
-    else if (warp >= 5 && warp < 9) idx_first = p.idx[(int64_t)cta_in_net * kTileM + (warp & 3) * 32 + lane];
-  }
-  {
-    // one thread per W2 row: all of its (<=16) loads are independent and in flight together
-    uint8_t* w2s = smem + kOffW2;
-    for (int j = threadIdx.x; j < kH; j += fb_threads(NEPI)) {
-      uint32_t pk[8];
-      if (net.A == 8 && (reinterpret_cast<uintptr_t>(net.w2) & 15) == 0) {
-        const uint4 v = *reinterpret_cast<const uint4*>(net.w2 + j * 8);
-        pk[0] = v.x, pk[1] = v.y, pk[2] = v.z, pk[3] = v.w, pk[4] = pk[5] = pk[6] = pk[7] = 0u;
-      } else {
-        unsigned short e[16];
-#pragma unroll
-        for (int n = 0; n < 16; ++n) e[n] = n < net.A ? reinterpret_cast<const unsigned short*>(net.w2)[j * net.A + n] : (unsigned short)0;
-#pragma unroll
-        for (int n = 0; n < 8; ++n) pk[n] = (uint32_t)e[2 * n] | ((uint32_t)e[2 * n + 1] << 16);
-      }
-      uint8_t* dst = w2s + (j >> 3) * 256 + (j & 7) * 16;   // element (j, n) at (j/8)*256 + (n/8)*128 + (j%8)*16 + (n%8)*2
-      *reinterpret_cast<uint4*>(dst) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-      *reinterpret_cast<uint4*>(dst + 128) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-    }
-    for (int i = threadIdx.x; i < 256; i += fb_threads(NEPI)) s_b0[i] = net.b0[i], s_b1[i] = net.b1[i];
-    if (threadIdx.x < 16) s_b2[threadIdx.x] = threadIdx.x < net.A ? net.b2[threadIdx.x] : 0.f;
-    fence_async_proxy();
-  }
-  tc_fence_before();
+  stage_w2_bias(smem, net.w2, net.b0, net.b1, net.b2, net.A, s_b0, s_b1, s_b2);
+  fence_async_proxy();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  STX_STAMP_AT(57, threadIdx.x == 0);
 
   float m_acc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};  // actor_loss, entropy, value_loss, adv, pred value, target
+  float* dbw = s_db + warp * 528;
+  uint8_t* xs = smem + kOffX + wg * 8192;
+  const float inv_m = 1.0f / (float)p.mb;
+  float adv_mean = 0.f, adv_rstd = 1.f;
+  if (p.adv_stats) adv_mean = p.adv_stats[0], adv_rstd = p.adv_stats[1];
+  const int dchunks = p.D >> 3;  // 16-byte chunks per observation row
+  mbar_wait(w_full, 0, 2);
 
-  if (warp < 4) {
-    // ===================== producers: X rows gathered one row per thread =====================
-    const int dchunks = p.D >> 3;  // 16-byte chunks per observation row
-    const int r = threadIdx.x;     // row of the tile owned by this thread
-    int32_t gidx = idx_first;      // shuffle index of this thread's row: fetched one tile ahead, kept raw until used
-    for (int it = 0; it < my_tiles; ++it) {
-      const int s = it & 1;
-      const int tile = cta_in_net + it * ncta;
-      const int64_t mrow = (int64_t)tile * kTileM + r;
-      const int64_t src = p.idx ? (int64_t)gidx : p.row0 + mrow;
-      if (p.idx && it + 1 < my_tiles) gidx = p.idx[mrow + (int64_t)ncta * kTileM];
-      uint4 v[8];
+  for (int it = 0; it < my_tiles; ++it) {
+    const int tile = g + it * n_wg;
+    // ---------------- gather: two threads per row, 4 chunks of 16 bytes each ----------------
+    {
+      const int r = t >> 1, hf = t & 1;
+      const int64_t mrow = (int64_t)tile * kWTile + r;
+      const int64_t src = p.idx ? (int64_t)p.idx[mrow] : p.row0 + mrow;
+      uint4 v[4];
 #pragma unroll
-      for (int c = 0; c < 8; ++c)  // 8 independent 16-byte loads in flight per thread
-        v[c] = c < dchunks ? *reinterpret_cast<const uint4*>(p.obs + src * p.D + c * 8) : make_uint4(0u, 0u, 0u, 0u);
-      if (warp == 0) STX_STAMP(48);
-      if (it >= 2) mbar_wait(&x_empty[s], ((it >> 1) & 1) ^ 1, 1);
-      if (warp == 0) STX_STAMP(49);
-      uint8_t* xs = smem + kOffX + s * 16384 + r * 128;
-#pragma unroll
-      for (int c = 0; c < 8; ++c) *reinterpret_cast<uint4*>(xs + ((c ^ (r & 7)) << 4)) = v[c];  // Swizzle<3,4,3>
-      if (which == 0) {
-#pragma unroll
-        for (int c = 0; c < 8; ++c) st_hint(tiled_ptr(p.xg, (int64_t)(tile % ring) * kTileM + r, c, 8), v[c], pol_stream);
+      for (int cc = 0; cc < 4; ++cc) {
+        const int c = hf * 4 + cc;
+        v[cc] = c < dchunks ? *reinterpret_cast<const uint4*>(p.obs + src * p.D + c * 8) : make_uint4(0u, 0u, 0u, 0u);
       }
-      if (warp == 0) STX_STAMP(50);
+      wg_sync(1 + wg);  // every warp of this warpgroup has finished layer 0 of the previous tile (X stage free)
+#pragma unroll
+      for (int cc = 0; cc < 4; ++cc) {
+        const int c = hf * 4 + cc;
+        *reinterpret_cast<uint4*>(xs + r * 128 + ((c ^ (r & 7)) << 4)) = v[cc];  // Swizzle<3,4,3>
+        if (which == 0) st_hint(reinterpret_cast<uint4*>(tiled_ptr(p.xg, mrow, 8 * c, 8)), v[cc], pol_stream);
+      }
       fence_async_proxy();
-      if (warp == 0) STX_STAMP(51);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&x_full[s]);
-      if (which == 0 && p.flag_x != nullptr) flag_signal(p.flag_x + tile, lane);  // xg rows of this warp are on their way
+      wg_sync(1 + wg);
     }
-  } else if (warp == kFbMmaWarp) {
-    // ===================== MMA issuer =====================
-    // Every 256-wide GEMM is issued as four N=64 column parts.  Part p of the NEXT GEMM only needs (a) D part p
-    // consumed by the running epilogue and (b) the K-chunks of its A operand written, both announced per part
-    // through chunk_done[]; so the tensor pipe trails the epilogue part by part instead of waiting for all of it.
-    // Code shape: groups of four K steps are unrolled (the issuing thread must stay ahead of the 33 cycles an N=64 MMA
-    // takes), the loops over parts and groups are rolled and the descriptors advance by adding byte offsets: fully
-    // unrolled, the ~200 MMA issues of a tile were a third of the kernel's code and the instruction-cache misses at
-    // every phase change stalled the SM for ~2.5k cycles per tile; fully rolled, the issue itself became the bottleneck.
-    constexpr uint32_t idesc_fwd = idesc_bf16(128, 64, 0, 1);    // B = W (in,out) image as MN-major
-    constexpr uint32_t idesc_head = idesc_bf16(128, 16, 0, 1);
-    constexpr uint32_t idesc_bwd = idesc_bf16(128, 64, 0, 0);    // B = same images read as K-major
-    constexpr uint32_t idesc_bwd_full = idesc_bf16(128, 256, 0, 0);
-    const uint32_t tmem_d = tmem, tmem_a1 = tmem + 256, tmem_a2 = tmem + 384;
-    auto adv = [](uint64_t desc, uint32_t bytes) { return desc + (uint64_t)(bytes >> 4); };  // start-address field, no carry (< 256 KB)
-    const uint64_t dW0 = smem_desc(sbase + kOffW0, 8192, 1024, SWIZZLE_128B);
-    const uint64_t dW1f = smem_desc(sbase + kOffW1, 32768, 1024, SWIZZLE_128B);  // forward: MN-major
-    const uint64_t dW1b = smem_desc(sbase + kOffW1, 16, 1024, SWIZZLE_128B);     // backward: K-major
-    const uint64_t dW2f = smem_desc(sbase + kOffW2, 256, 128, SWIZZLE_NONE);
-    mbar_wait(w_full, 0, 2);
-    STX_STAMP_AT(58, lane == 0);
-    for (int it = 0; it < my_tiles; ++it) {
-      const int s = it & 1;
-      STX_STAMP(0);
-      mbar_wait(&x_full[s], (it >> 1) & 1, 3);
-      const uint64_t dX = smem_desc(sbase + kOffX + s * 16384, 16, 1024, SWIZZLE_128B);
-#pragma unroll 1
-      for (int pt = 0; pt < 4; ++pt) {  // G0: D = X * W0, trailing E4 of the previous tile
-        if (it > 0) mbar_wait(&chunk_done[pt], 1, 4);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t b0 = adv(dW0, pt * 8192);
+    // ---------------- per-row loss inputs of rows row0 and row0 + 8 (consumed in E2) ----------------
+    const int64_t row0 = (int64_t)tile * kWTile + wq * 16 + (lane >> 2);
+    int pf_a[2] = {0, 0};
+    float pf_0[2] = {0.f, 0.f}, pf_1[2] = {0.f, 0.f};
 #pragma unroll
-          for (int k = 0; k < 4; ++k) mma_ss(tmem_d + pt * 64, adv(dX, k * 32), adv(b0, k * 2048), idesc_fwd, k > 0);
-          mma_commit(&d_ready[pt]);
-          if (pt == 3) mma_commit(&x_empty[s]);
-        }
-        __syncwarp();
-      }
-      STX_STAMP(1);
-#pragma unroll 1
-      for (int j = 0; j < 4; ++j) {  // G1: D = h1 * W1, trailing E0
-        mbar_wait(&chunk_done[j], 0, 5);
-        tc_fence_after();
-        if (elect_one()) {
-#pragma unroll 1
-          for (int pt = 0; pt <= j; ++pt) {
-#pragma unroll 1
-            for (int g = (pt == j ? 0 : j); g <= j; ++g) {  // K steps 4g .. 4g+3
-              const uint64_t b0 = adv(dW1f, pt * 32768 + g * 8192);
-              const uint32_t a0 = tmem_a1 + g * 32;
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk) mma_ts(tmem_d + pt * 64, a0 + kk * 8, adv(b0, kk * 2048), idesc_fwd, (g | kk) != 0);
-            }
-            if (j == 3) mma_commit(&d_ready[pt]);
-          }
-        }
-        __syncwarp();
-      }
-      STX_STAMP(3);
-#pragma unroll 1
-      for (int j = 0; j < 4; ++j) {  // G2: D[:, :16] = h2 * W2, trailing E1 (columns 0..15 are free after its first part)
-        mbar_wait(&chunk_done[j], 1, 6);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t b0 = adv(dW2f, j * 2048);
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) mma_ts(tmem_d, tmem_a2 + j * 32 + kk * 8, adv(b0, kk * 512), idesc_head, (j | kk) != 0);
-          if (j == 3) mma_commit(head_ready);
-        }
-        __syncwarp();
-      }
-      STX_STAMP(5);
-      mbar_wait(head_done, it & 1, 7);
-      tc_fence_after();
-      if (elect_one()) {  // G3: D = dz (smem, K-major core matrices) * W2^T (same W2 image, K-major)
-        mma_ss(tmem_d, smem_desc(sbase + kOffDz, 128, 256, SWIZZLE_NONE), smem_desc(sbase + kOffW2, 128, 256, SWIZZLE_NONE),
-               idesc_bwd_full, 0);
-#pragma unroll
-        for (int pt = 0; pt < 4; ++pt) mma_commit(&d_ready[pt]);
-      }
-      __syncwarp();
-      STX_STAMP(7);
-#pragma unroll 1
-      for (int j = 0; j < 4; ++j) {  // G4: D = dh2 * W1^T, trailing E3  (W1 image as K-major SW128: 4 K-blocks of 64)
-        mbar_wait(&chunk_done[j], 0, 8);
-        tc_fence_after();
-        if (elect_one()) {
-#pragma unroll 1
-          for (int pt = 0; pt <= j; ++pt) {
-#pragma unroll 1
-            for (int g = (pt == j ? 0 : j); g <= j; ++g) {  // K steps 4g .. 4g+3 = the g-th 64-wide K block of the image
-              const uint64_t b0 = adv(dW1b, g * 32768 + pt * 8192);
-              const uint32_t a0 = tmem_a2 + g * 32;
-#pragma unroll
-              for (int kk = 0; kk < 4; ++kk) mma_ts(tmem_d + pt * 64, a0 + kk * 8, adv(b0, kk * 32), idesc_bwd, (g | kk) != 0);
-            }
-            if (j == 3) mma_commit(&d_ready[pt]);
-          }
-        }
-        __syncwarp();
-      }
-      STX_STAMP(9);
+    for (int rr = 0; rr < 2; ++rr) {
+      const int64_t m = row0 + 8 * rr;
+      const int64_t src = p.idx ? (int64_t)p.idx[m] : p.row0 + m;
+      if (net.is_actor) pf_a[rr] = p.action[src], pf_0[rr] = p.logp_old[src], pf_1[rr] = p.adv[src];
+      else pf_0[rr] = p.v_old[src], pf_1[rr] = p.tgt[src];
     }
-  } else {
-    // ===================== epilogue warps 5..: lane quarter q = warp % 4, column position `sub` =====================
-    // Time step cc of an epilogue handles the 32-column chunks cc*kSub + sub (kSub = NEPI/4 warps per lane quarter), so
-    // the 64-column parts complete in order and are handed to the MMA warp one by one (NEPI=8: one part per step,
-    // NEPI=16: two parts per step).
-    constexpr int kSub = NEPI / 4, kSteps = 8 / kSub;
-    const int q = warp & 3, sub = (warp - 5) >> 2;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const uint32_t tmem_d = tmem + lane_addr, tmem_a1 = tmem + lane_addr + 256, tmem_a2 = tmem + lane_addr + 384;
-    const float inv_m = 1.0f / (float)p.mb;
-    float adv_mean = 0.f, adv_rstd = 1.f;
-    if (p.adv_stats) adv_mean = p.adv_stats[0], adv_rstd = p.adv_stats[1];
-    // source row of this thread's row in the NEXT tile: loaded one tile ahead so that the dependent per-row
-    // loads below never wait on the index (two chained DRAM latencies would otherwise open every tile)
-    // (kept RAW: a conversion right behind the load would stall this in-order warp for the full memory latency)
-    int32_t idx_next = idx_first;  // (tile 0: requested in the prologue)
-    // Deferred activation stores.  The SM's global-store path moves 32 B/clk (tools/store_bw.cu): the 2 KB a warp
-    // produces per chunk occupy it for 64 cycles, and all 8 warps finish a chunk at about the same time.  Issued in one
-    // burst, the later stores of a warp block it behind the other warps' bursts; so the four 512-byte stores of a chunk
-    // are issued one at a time between the four column groups of the NEXT chunk this warp processes (whatever phase
-    // that chunk belongs to), where the store path has long drained.
-    long long prof_sig = 0;
-    uint32_t pend[16];
-    uint4* pend_ptr = nullptr;
+    float acc[64];
+    uint32_t a1[64], a2[64];
+    wg_zero(acc);
+    // ---------------- G0 / E0, G1 / E1: hidden layers ----------------
 #pragma unroll
-    for (int j = 0; j < 16; ++j) pend[j] = 0u;
-#define STX_FLUSH_PENDING(g)                                                                                           \
-  do {                                                                                                                 \
-    if (pend_ptr != nullptr)                                                                                           \
-      st_hint(pend_ptr + (g) * 128, make_uint4(pend[4 * (g)], pend[4 * (g) + 1], pend[4 * (g) + 2], pend[4 * (g) + 3]), pol_stream); \
-  } while (0)
-    for (int it = 0; it < my_tiles; ++it) {
-      const int tile = cta_in_net + it * ncta;
-      const int64_t mrow = (int64_t)tile * kTileM + q * 32 + lane;  // row inside the minibatch
-      const int64_t srow = (int64_t)(tile % ring) * kTileM + q * 32 + lane;  // its row in the activation workspace (slot of the tile)
-      // per-row loss inputs: issued now, consumed in E2 (their latency hides behind E0/E1)
-      int pf_a = 0;
-      float pf_0 = 0.f, pf_1 = 0.f;
-      if (sub == 0) {
-        const int64_t src = p.idx ? (int64_t)idx_next : p.row0 + mrow;
-        if (net.is_actor) pf_a = p.action[src], pf_0 = p.logp_old[src], pf_1 = p.adv[src];
-        else pf_0 = p.v_old[src], pf_1 = p.tgt[src];
-        if (it + 1 < my_tiles && p.idx) idx_next = p.idx[mrow + (int64_t)ncta * kTileM];
-      }
-      // ---------------- E0 / E1: hidden layers ----------------
-      STX_STAMP_AT(32 + 4 * it, warp == 5 && lane == 0 && it < 4);  // 32, 36, 40, 44: E0 start of tile it
-#pragma unroll 1
-      for (int layer = 0; layer < 2; ++layer) {
-        if (warp == 5) STX_STAMP(16 + 2 * layer);
-        const float* bias = layer == 0 ? s_b0 : s_b1;
-        const uint32_t ta = layer == 0 ? tmem_a1 : tmem_a2;
-        __nv_bfloat16* hout = layer == 0 ? net.h1 : net.h2;
-#pragma unroll 1
-        for (int cc = 0; cc < kSteps; ++cc) {
-          const int c = cc * kSub + sub, part = c >> 1;
-          mbar_wait(&d_ready[part], layer, 10 + layer);  // G0 / G1 are the 1st / 2nd completion of d_ready per tile
-          tc_fence_after();
-          if (warp == 5 && cc == 0) STX_STAMP(17 + 2 * layer);
-          uint32_t r[32], pk[16];
-          tmem_ld32(tmem_d + c * 32, r);
-          tmem_ld_wait();
+    for (int h = 0; h < 2; ++h) {
+      gemm_x_w0(acc, smem_u32(xs), sbase, h);
+      epi_bias_relu(acc, s_b0, h, a1, lane);
+      store_act(net.h1, a1, h, row0, lane, pol_stream);
+    }
 #pragma unroll
-          for (int g = 0; g < 4; ++g) {
+    for (int h = 0; h < 2; ++h) {
+      gemm_a_w1(acc, a1, sbase, h);
+      epi_bias_relu(acc, s_b1, h, a2, lane);
+      store_act(net.h2, a2, h, row0, lane, pol_stream);
+    }
+    // ---------------- G2 / E2: head + loss + d(head) ----------------
+    float z[8];
+    wg_zero(z);
+    gemm_a_w2(z, a2, sbase);
+    float dz[8];  // accumulator layout: dz[i] = row0 + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 q4 + (i & 1)
 #pragma unroll
-            for (int j = 4 * g; j < 4 * g + 4; ++j) {
-              pk[j] = bias_relu_pack_bf16(r[2 * j], r[2 * j + 1], *reinterpret_cast<const float2*>(bias + c * 32 + 2 * j));
-            }
-            STX_FLUSH_PENDING(g);  // one 512-byte store of the previous chunk (32 lanes = 32 consecutive rows)
-          }
-          tmem_st16(ta + c * 16, pk);
-          tmem_st_wait();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&chunk_done[part]);  // this chunk of D consumed, its K-chunks of the next A operand written
-          // the flushes above issued this warp's last stores (dh1) of the PREVIOUS tile: that tile's activations are complete
-          if (layer == 0 && cc == 0 && it > 0 && p.flag_t != nullptr) flag_signal_timed(p.flag_t + which * num_tiles + (tile - ncta), lane, prof_sig);
+    for (int rr = 0; rr < 2; ++rr) {
+      const int ix[4] = {2 * rr, 2 * rr + 1, 4 + 2 * rr, 5 + 2 * rr};
+      const int col[4] = {2 * q4, 2 * q4 + 1, 8 + 2 * q4, 9 + 2 * q4};
+      if (net.is_actor) {
+        float zz[4], d4[4], loss, ent;
 #pragma unroll
-          for (int j = 0; j < 16; ++j) pend[j] = pk[j];
-          pend_ptr = tiled_ptr(hout, srow, c * 4, 32);
-        }
-      }
-      // ---------------- E2: head + loss + d(head) ----------------
-      if (warp == 5) STX_STAMP(20);
-      STX_STAMP_AT(32 + 4 * it + 1, warp == 5 && lane == 0 && it < 4);  // E2 start of tile it
-      if (sub == 0) {
-        mbar_wait(head_ready, it & 1, 12);
-        tc_fence_after();
-        if (warp == 5) STX_STAMP(21);
-        uint32_t r[16];
-        tmem_ld16(tmem_d, r);
-        tmem_ld_wait();
-        float dz[16];
+        for (int k = 0; k < 4; ++k) zz[k] = z[ix[k]] + s_b2[col[k]];
+        const float adv = (pf_1[rr] - adv_mean) * adv_rstd;
+        actor_head_quad(zz, col, net.A, pf_a[rr], pf_0[rr], adv, p.clip_eps, p.ent_coef, inv_m, d4, loss, ent);
 #pragma unroll
-        for (int j = 0; j < 16; ++j) dz[j] = 0.f;
-        if (net.is_actor) {
-          const float adv = (pf_1 - adv_mean) * adv_rstd;
-          float loss, ent;
-          if (net.A <= 8) actor_head<8>(r, s_b2, net.A, pf_a, pf_0, adv, p.clip_eps, p.ent_coef, inv_m, dz, loss, ent);
-          else actor_head<16>(r, s_b2, net.A, pf_a, pf_0, adv, p.clip_eps, p.ent_coef, inv_m, dz, loss, ent);
-          m_acc[0] += loss, m_acc[1] += ent, m_acc[3] += adv;
-        } else {
-          const float v = __uint_as_float(r[0]) + s_b2[0], vo = pf_0, tg = pf_1;
+        for (int k = 0; k < 4; ++k) dz[ix[k]] = d4[k];
+        if (q4 == 0) m_acc[0] += loss, m_acc[1] += ent, m_acc[3] += adv;
+      } else {
+#pragma unroll
+        for (int k = 0; k < 4; ++k) dz[ix[k]] = 0.f;
+        if (q4 == 0) {  // the value is column 0
+          const float v = z[2 * rr] + s_b2[0], vo = pf_0[rr], tg = pf_1[rr];
           const float diff = v - vo;
           const float vclip = vo + fminf(fmaxf(diff, -p.clip_eps), p.clip_eps);
           const float e1 = v - tg, e2 = vclip - tg, q1 = e1 * e1, q2 = e2 * e2;
           const float g2 = (fabsf(diff) < p.clip_eps) ? e2 : 0.f;
           const float dv = q1 > q2 ? e1 : (q1 < q2 ? g2 : 0.5f * (e1 + g2));
-          dz[0] = p.vf_coef * dv * inv_m;
+          dz[2 * rr] = p.vf_coef * dv * inv_m;
           m_acc[2] += 0.5f * fmaxf(q1, q2), m_acc[4] += v, m_acc[5] += tg;
         }
-        if (warp == 5) STX_STAMP(41);
-        // dz -> bf16: smem A operand (core-matrix K-major) + global (padded row of 64)
-        uint32_t pk[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) pk[j] = pack_bf16(dz[2 * j], dz[2 * j + 1]);
-        const int mr = q * 32 + lane;
-        uint8_t* dzs = smem + kOffDz + (mr >> 3) * 256 + (mr & 7) * 16;
-        *reinterpret_cast<uint4*>(dzs) = make_uint4(pk[0], pk[1], pk[2], pk[3]);        // k = 0..7
-        *reinterpret_cast<uint4*>(dzs + 128) = make_uint4(pk[4], pk[5], pk[6], pk[7]);  // k = 8..15
-        fence_async_proxy();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(head_done);
-        if (warp == 5) STX_STAMP(44);
-        st_hint(tiled_ptr(net.dz, srow, 0, 2), make_uint4(pk[0], pk[1], pk[2], pk[3]), pol_stream);
-        st_hint(tiled_ptr(net.dz, srow, 1, 2), make_uint4(pk[4], pk[5], pk[6], pk[7]), pol_stream);
-        // bias gradient of the head (off the critical path: G3 is already running): column sums over the 32 rows
-        // of this warp; fold the two half-warps first (1 shuffle per column), then the 16-lane butterfly
-        {
-          float t[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) t[j] = dz[j] + __shfl_xor_sync(0xffffffffu, dz[j], 16);
-#pragma unroll
-          for (int s2 = 8; s2 >= 1; s2 >>= 1) {
-#pragma unroll
-            for (int i = 0; i < s2; ++i) {
-              const bool hi = (lane & s2) != 0;
-              const float send = hi ? t[i] : t[i + s2];
-              const float keep = hi ? t[i + s2] : t[i];
-              t[i] = keep + __shfl_xor_sync(0xffffffffu, send, s2);
-            }
-          }
-          if (lane < 16) s_db[q * 528 + 512 + lane] += t[0];  // lanes 0..15 hold columns 0..15
-        }
-      }
-      // ---------------- E3 / E4: dh2 = D * (h2 > 0) ; dh1 = D * (h1 > 0) ----------------
-#pragma unroll 1
-      for (int layer = 1; layer >= 0; --layer) {
-        if (warp == 5) STX_STAMP(22 + 2 * (1 - layer));
-        const uint32_t ta = layer == 1 ? tmem_a2 : tmem_a1;  // packed h of this layer (mask source)
-        __nv_bfloat16* dout = layer == 1 ? net.dh2 : net.dh1;
-        float* dbacc = s_db + q * 528 + (layer == 1 ? 256 : 0);
-#pragma unroll 1
-        for (int cc = 0; cc < kSteps; ++cc) {
-          const int c = cc * kSub + sub, part = c >> 1;
-          mbar_wait(&d_ready[part], 1 - layer, 13 + layer);  // G3 / G4 are the 3rd / 4th completion per tile
-          tc_fence_after();
-          uint32_t r[32], hm[16], pk[16];
-          tmem_ld32(tmem_d + c * 32, r);
-          tmem_ld16(ta + c * 16, hm);
-          tmem_ld_wait();
-          float dv[32];
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-#pragma unroll
-            for (int j = 4 * g; j < 4 * g + 4; ++j) {
-              // h is post-relu (>= 0): positive <=> bf16 bit pattern non-zero (and not -0)
-              const bool p0 = (hm[j] & 0x7FFFu) != 0u, p1 = (hm[j] & 0x7FFF0000u) != 0u;
-              dv[2 * j] = p0 ? __uint_as_float(r[2 * j]) : 0.f;
-              dv[2 * j + 1] = p1 ? __uint_as_float(r[2 * j + 1]) : 0.f;
-              pk[j] = pack_bf16(dv[2 * j], dv[2 * j + 1]);
-            }
-            STX_FLUSH_PENDING(g);
-          }
-          if (layer == 1) {  // dh2 replaces h2 as the A operand of G4
-            tmem_st16(ta + c * 16, pk);
-            tmem_st_wait();
-          }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&chunk_done[part]);  // E3: -> G4 ; E4: D columns free for the next tile's G0
-#pragma unroll
-          for (int j = 0; j < 16; ++j) pend[j] = pk[j];
-          pend_ptr = tiled_ptr(dout, srow, c * 4, 32);
-          if (layer == 1) {  // db1; db0 = column sums of dh1 comes out of K3b's dW0 job for free (ones-operand MMA)
-            const float cs = warp_colsum32(dv, lane);
-            dbacc[c * 32 + lane] += cs;  // this (quarter, column) is touched by this warp only
-          }
-        }
-        if (warp == 5) STX_STAMP(26 + (1 - layer));
-        STX_STAMP_AT(32 + 4 * it + 2 + (1 - layer), warp == 5 && lane == 0 && it < 4);  // E3 / E4 end of tile it
       }
     }
+    uint32_t dzp[4];  // dz as the A operand of G3 (K = 16)
 #pragma unroll
-    for (int g = 0; g < 4; ++g) STX_FLUSH_PENDING(g);  // the last chunk of the last tile
-    if (my_tiles > 0 && p.flag_t != nullptr) flag_signal_timed(p.flag_t + which * num_tiles + cta_in_net + (my_tiles - 1) * ncta, lane, prof_sig);
-#undef STX_FLUSH_PENDING
-    STX_STAMP_AT(61, warp == 5 && lane == 0);
-    if (g_prof_buf != nullptr && warp == 5 && lane == 0) {
-      long long* pb = g_prof_buf + (int64_t)blockIdx.x * 8;
-      pb[0] = 1, pb[1] = clock64() - prof_t0, pb[2] = prof_sig, pb[3] = my_tiles;
+    for (int k = 0; k < 4; ++k) dzp[k] = pack_bf16(dz[2 * k], dz[2 * k + 1]);
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      st_hint(reinterpret_cast<uint32_t*>(tiled_ptr(net.dz, row0 + 8 * (k & 1), 8 * (k >> 1) + 2 * q4, 2)), dzp[k], pol_stream);
+    {  // head bias gradient: column sums of dz over the tile rows of this warp
+      float cs[4];
+#pragma unroll
+      for (int k = 0; k < 4; ++k) cs[k] = dz[(k >> 1) * 4 + (k & 1)] + dz[(k >> 1) * 4 + 2 + (k & 1)];
+#pragma unroll
+      for (int s = 4; s <= 16; s <<= 1)
+#pragma unroll
+        for (int k = 0; k < 4; ++k) cs[k] += __shfl_xor_sync(0xffffffffu, cs[k], s);
+      if (lane < 4)
+#pragma unroll
+        for (int k = 0; k < 4; ++k) dbw[512 + 8 * (k >> 1) + 2 * lane + (k & 1)] += cs[k];
+    }
+    // ---------------- G3 / E3: dh2 = (dz W2^T) * (h2 > 0), replaces h2 as the A operand of G4 ----------------
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      gemm_dz_w2t(acc, dzp, sbase, h);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        // h is post-relu (>= 0): positive <=> bf16 bit pattern non-zero (and not -0)
+        const uint32_t hm = a2[32 * h + i];
+        acc[2 * i] = (hm & 0x7FFFu) != 0u ? acc[2 * i] : 0.f;
+        acc[2 * i + 1] = (hm & 0x7FFF0000u) != 0u ? acc[2 * i + 1] : 0.f;
+        a2[32 * h + i] = pack_bf16(acc[2 * i], acc[2 * i + 1]);
+      }
+      store_act(net.dh2, a2, h, row0, lane, pol_stream);
+      colsum_half(acc, dbw + 256, h, lane);  // db1
+    }
+    // ---------------- G4 / E4: dh1 = (dh2 W1^T) * (h1 > 0) ----------------
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      gemm_a_w1t(acc, a2, sbase, h);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const uint32_t hm = a1[32 * h + i];
+        const uint32_t pk = pack_bf16((hm & 0x7FFFu) != 0u ? acc[2 * i] : 0.f, (hm & 0x7FFF0000u) != 0u ? acc[2 * i + 1] : 0.f);
+        a1[32 * h + i] = pk;
+        const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(&pk);
+        acc[2 * i] = __bfloat162float(v.x), acc[2 * i + 1] = __bfloat162float(v.y);  // db0 sums the bf16 dh1 that K3b's dW0 uses
+      }
+      store_act(net.dh1, a1, h, row0, lane, pol_stream);
+      colsum_half(acc, dbw, h, lane);  // db0
     }
   }
   // ---- teardown: bias-gradient and metric partials of this CTA ----
-  tc_fence_before();
   __syncthreads();
-  const uint64_t pol_keep = l2_evict_last();  // read by the reduce kernel after K3b has streamed ~140 MB through L2
-  for (int i = threadIdx.x; i < 528; i += fb_threads(NEPI))
-    st_hint(&net.db_part[(int64_t)cta_in_net * 528 + i], (s_db[i] + s_db[528 + i]) + (s_db[2 * 528 + i] + s_db[3 * 528 + i]), pol_keep);
+  const uint64_t pol_keep = l2_evict_last();  // read by the reduce kernel after K3b has streamed the activations through L2
+  for (int i = threadIdx.x; i < 528; i += kFbThreads) {
+    float acc = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) acc += s_db[w * 528 + i];
+    st_hint(&net.db_part[(int64_t)cta_in_net * 528 + i], acc, pol_keep);
+  }
   {
-    __shared__ float s_mw[fb_threads(NEPI) / 32][6];
+    __shared__ float s_mw[kFbThreads / 32][6];
 #pragma unroll
     for (int k = 0; k < 6; ++k) {
       const float w = warp_sum(m_acc[k]);
@@ -646,285 +381,151 @@ __device__ __forceinline__ void fb_role(uint8_t* smem_raw, const CUtensorMap& tm
     if (threadIdx.x < 8) {
       float acc = 0.f;
       if (threadIdx.x < 6)
-        for (int w = 0; w < fb_threads(NEPI) / 32; ++w) acc += s_mw[w][threadIdx.x];
+        for (int w = 0; w < kFbThreads / 32; ++w) acc += s_mw[w][threadIdx.x];
       st_hint(&p.metric_part[(int64_t)blockIdx.x * 8 + threadIdx.x], acc, pol_keep);
     }
   }
-  if (warp == kFbMmaWarp) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 512);
+  if (g_prof_buf != nullptr && threadIdx.x == 0) {
+    long long* pb = g_prof_buf + (int64_t)blockIdx.x * 8;
+    pb[0] = 1, pb[1] = clock64() - prof_t0, pb[3] = my_tiles;
   }
-  STX_STAMP_AT(62, threadIdx.x == 0);
-}
-
-template <int NEPI>
-__global__ void __launch_bounds__(fb_threads(NEPI), 1)
-    tc_ppo_fwd_bwd_kernel(const __grid_constant__ CUtensorMap tmW0a, const __grid_constant__ CUtensorMap tmW1a,
-                          const __grid_constant__ CUtensorMap tmW0c, const __grid_constant__ CUtensorMap tmW1c,
-                          const FbParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  fb_role<NEPI>(smem_raw, tmW0a, tmW1a, tmW0c, tmW1c, p);
 }
 
 // =============================== K3b: dW = A^T * B ===============================================
-constexpr int kDwThreads = 192;  // warp 0 TMA, warp 1 MMA, warps 2..5 epilogue
-constexpr int kDwStages = 3;
-constexpr uint32_t kDwStageBytes = 65536;  // A [64 x 256] 32 KB + B [64 x <=256] 32 KB
-constexpr uint32_t kDwOffOnes = kDwStages * kDwStageBytes;  // 2 KB: B tile [2 column groups][64 rows][16 B] of bf16 1.0
-constexpr uint32_t kDwOffBar = kDwOffOnes + 2048;
-constexpr uint32_t kDwSmemBytes = kDwOffBar + 128 + 1024;
-constexpr int kMaxJobs = 6;
-constexpr int kMaxSubs = 2;
+constexpr int kDwThreads = 288;  // warps 0..7: two consumer warpgroups (hidden units [128 w, 128 w + 128)), warp 8: TMA
+constexpr int kDwStages = 4;
+constexpr uint32_t kDwStageBytes = 49152;  // A [64 x 256] 32 KB + B [64 x <=128] 16 KB
+constexpr uint32_t kDwOffBar = kDwStages * kDwStageBytes;
+constexpr uint32_t kDwSmemBytes = kDwOffBar + 64 + 1024;
+constexpr int kMaxJobs = 8;
 
-// One weight-gradient GEMM of a job: dW = A^T * B over the rows this CTA is given.
-struct DwSub {
-  float* part;     // [n_cta][256 x N] fp32 partial outputs
-  float* colsum;   // nullable: [n_cta][256] per-CTA sums over the rows of every A column (A^T * 1): the bias gradient that
-                   // belongs to A = dh1, obtained from one extra N=16 MMA per K step against an all-ones B tile
-  int N;           // 16, 64 or 256 (= 8 * column groups of B)
-  int map;         // index of the (A, B) tensor-map pair in DwMaps
-  int tmem_col;    // accumulator columns [tmem_col, tmem_col + N (+16 with colsum)) of each 256-column half
-  int wait_x;      // fused launch: 1 = the B operand is xg (written by the ACTOR CTAs: its own completion counter)
-};
-// A job = the CTAs [cta_begin, cta_begin + n_cta) running the same 1..2 GEMMs over an interleaved share of the 64-row chunks.
+// One weight-gradient GEMM: part = A^T * B[:, 8 b_cg0 .. 8 b_cg0 + N) over the rows this CTA is given.
 struct DwJob {
-  DwSub sub[kMaxSubs];
-  int n_sub;
-  int cta_begin;   // first CTA of this job (relative to the first weight-gradient CTA of the launch)
+  float* part;     // [n_cta][256 x N] fp32 partial outputs
+  int N;           // 16, 64 or 128
+  int map;         // index of the (A, B) tensor-map pair in DwMaps
+  int b_cg;        // column groups of the whole B matrix
+  int b_cg0;       // first column group of B taken by this job
+  int cta_begin;   // first CTA of this job
   int n_cta;
   int num_chunks;  // mb / 64
-  int net;
 };
 struct DwParams {
   DwJob job[kMaxJobs];
   int n_jobs;
-  int num_tiles;
-  // fused launch: completion counters written by the K3a CTAs of the same grid (nullptr: operands are complete at entry)
-  const uint32_t* flag_t;  // [2][tiles]
-  const uint32_t* flag_x;  // [tiles]
-  int ring_tiles;  // see FbParams
   int act_policy;
 };
 struct DwMaps {
   CUtensorMap a[kMaxJobs];  // tiled [mb x 256]: 2D u64 view {256 per (tile, colgroup), tiles*32}, box {128, 32}
-  CUtensorMap b[kMaxJobs];  // tiled [mb x N]:   box {128, N/8}
+  CUtensorMap b[kMaxJobs];  // tiled [mb x 8 b_cg]: box {128, N/8}
 };
 
-// The K3b CTA (warps 0..5 of the block work; further warps of a fused launch only join the block barriers).
-// `cta` counts from the first weight-gradient CTA of the launch.
-__device__ __forceinline__ void dw_role(uint8_t* smem_raw, const DwMaps& maps, const DwParams& p, const int cta_abs, const bool fused) {
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+template <int N>
+__device__ __forceinline__ void dw_consume(uint8_t* smem, uint64_t* full, uint64_t* empty, const DwJob& job, int cta, int my_chunks) {
   const uint32_t sbase = smem_u32(smem);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kDwOffBar);
-  uint64_t* full = bars;                 // [kDwStages]
-  uint64_t* empty = bars + kDwStages;    // [kDwStages]
-  uint64_t* acc_done = bars + 2 * kDwStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * kDwStages + 1);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long long prof_t0 = clock64();
-  long long* const prof = g_prof_buf ? g_prof_buf + (int64_t)blockIdx.x * 8 : nullptr;
-
-  int j = 0;
-  while (j + 1 < p.n_jobs && cta_abs >= p.job[j + 1].cta_begin) ++j;
-  const DwJob& job = p.job[j];
-  const int cta = cta_abs - job.cta_begin;
-  const int my_chunks = cta < job.num_chunks ? (job.num_chunks - cta + job.n_cta - 1) / job.n_cta : 0;
-  const int n_sub = job.n_sub;
-  const int my_iters = my_chunks * n_sub;  // pipeline slots: (chunk, sub-GEMM) pairs in order
-  bool any_colsum = false;
-  for (int sj = 0; sj < n_sub; ++sj) any_colsum |= job.sub[sj].colsum != nullptr;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kDwStages; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    mbar_init(acc_done, 1);
-    fence_barrier_init();
-    for (int sj = 0; sj < n_sub; ++sj) {
-      tma_prefetch_desc(&maps.a[job.sub[sj].map]);
-      tma_prefetch_desc(&maps.b[job.sub[sj].map]);
-    }
-  }
-  griddep_launch();
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  if (any_colsum) {  // all-ones B operand (every layout of a constant tile is the same tile)
-    for (int i = threadIdx.x; i < 512; i += blockDim.x) reinterpret_cast<uint32_t*>(smem + kDwOffOnes)[i] = 0x3F803F80u;
-    fence_async_proxy();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
-  griddep_wait();  // the activations are K3a's output; the partials written below were read by the previous reduce
-
-  if (warp == 0) {
-    if (elect_one()) {
-      const uint64_t pol_stream = l2_policy(p.act_policy);  // default evict_first: every activation tile is read exactly once
-      long long w_flag = 0, w_empty = 0;
-      int k = 0;
-      bool need_x = false;
-      for (int sj = 0; sj < n_sub; ++sj) need_x |= job.sub[sj].wait_x != 0;
-      // Completion of this CTA's chunks is polled a WINDOW at a time: one batch of independent acquire loads (one L2 round
-      // trip) and ONE generic->async proxy fence cover up to kWin chunks, instead of a dependent round trip + fence in front
-      // of every TMA issue (measured: ~900 cycles per pipeline slot, which made the loads, not the MMAs, the pace).
-      constexpr int kWin = 8;
-      int known = fused ? 0 : my_chunks;  // chunks [0, known) of this CTA's sequence have their operands in memory
-      for (int it = 0; it < my_chunks; ++it) {
-        // split launches: newest rows first (K3a wrote the last tiles most recently, so they are the likeliest L2 residents);
-        // fused launch: in the order the K3a CTAs of this grid finish their tiles
-        const int ci = cta + it * job.n_cta;
-        const int chunk = fused ? ci : job.num_chunks - 1 - ci;  // 64 rows: half of a 128-row tile
-        const int tile = chunk >> 1, r0 = (chunk & 1) * 64;
-        if (it >= known) {
-          const long long tq = clock64();
-          uint32_t spins = 0;
-          unsigned long long t0 = 0ull;
-          for (;;) {
-            uint32_t vt[kWin], vx[kWin];
+  const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  float acc[2][N / 2];
+  wg_zero(acc[0]);
+  wg_zero(acc[1]);
+  for (int k = 0; k < my_chunks; ++k) {
+    const int s = k % kDwStages;
+    mbar_wait(&full[s], (k / kDwStages) & 1, 21);
+    const uint32_t a0 = sbase + s * kDwStageBytes, b0 = a0 + 32768;
+    wg_fence_acc(acc[0]);
+    wg_fence_acc(acc[1]);
+    wg_fence();
 #pragma unroll
-            for (int w = 0; w < kWin; ++w) {
-              const int tw = (cta + (it + w) * job.n_cta) >> 1;
-              const bool in = it + w < my_chunks;
-              vt[w] = in ? ld_acquire_gpu(p.flag_t + job.net * p.num_tiles + tw) : 0u;
-              vx[w] = (in && need_x) ? ld_acquire_gpu(p.flag_x + tw) : kFlagGather;
-            }
-            int ok = 0;
+    for (int ks = 0; ks < 4; ++ks) {  // 16 rows (K) per step = two core-matrix row groups of 128 B
+      const uint64_t db = wg_desc(b0 + ks * 256, 128, 1024, WG_INTERLEAVE);
 #pragma unroll
-            for (int w = 0; w < kWin; ++w)
-              if (ok == w && it + w < my_chunks && vt[w] >= kFlagEpi && vx[w] >= kFlagGather) ok = w + 1;
-            if (ok > 0) {
-              known = it + ok;
-              break;
-            }
-            spin_guard(spins, t0, "K3 activations of a tile");
-          }
-          fence_proxy_async_global();  // the TMA (async proxy) reads below must observe what the acquire loads observed
-          w_flag += clock64() - tq;
-        }
-        for (int sj = 0; sj < n_sub; ++sj, ++k) {
-          const DwSub& sub = job.sub[sj];
-          const int s = k % kDwStages;
-          const long long tq = clock64();
-          if (k >= kDwStages) mbar_wait(&empty[s], ((k / kDwStages) & 1) ^ 1, 20);
-          w_empty += clock64() - tq;
-          uint8_t* st = smem + s * kDwStageBytes;
-          mbar_arrive_expect_tx(&full[s], 32768 + (uint32_t)sub.N * 128);
-          // one box = rows r0..r0+63 of every column group: smem image [colgroup][row][16 B]
-          const int slot = p.ring_tiles > 0 ? tile % p.ring_tiles : tile;
-          tma_load_2d_hint(st, &maps.a[sub.map], &full[s], r0 * 2, slot * 32, pol_stream);
-          tma_load_2d_hint(st + 32768, &maps.b[sub.map], &full[s], r0 * 2, slot * (sub.N >> 3), pol_stream);
-        }
-      }
-      if (prof) prof[0] = 2 + j, prof[2] = w_flag, prof[3] = w_empty, prof[5] = my_iters;
-    }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc_ones = idesc_bf16(128, 16, 1, 1);
-    long long w_full = 0;
-    int k = 0;
-    for (int it = 0; it < my_chunks; ++it) {
-      for (int sj = 0; sj < n_sub; ++sj, ++k) {
-        const DwSub& sub = job.sub[sj];
-        const uint32_t idesc = idesc_bf16(128, sub.N, 1, 1);  // both operands MN-major
-        const bool colsum = sub.colsum != nullptr;
-        const int s = k % kDwStages;
-        const long long tq = clock64();
-        mbar_wait(&full[s], (k / kDwStages) & 1, 21);
-        w_full += clock64() - tq;
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t a0 = sbase + s * kDwStageBytes, b0 = a0 + 32768;
-          const uint32_t acc = (it > 0) ? 1u : 0u;
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {      // 16 rows (K) per step = two core-matrix row groups of 128 B
-#pragma unroll
-            for (int h = 0; h < 2; ++h)      // M halves: hidden units [128 h, 128 h + 128) = column groups 16 h ..
-              mma_ss(tmem + h * 256 + sub.tmem_col, smem_desc(a0 + h * 16384 + ks * 256, 128, 1024, SWIZZLE_NONE),
-                     smem_desc(b0 + ks * 256, 128, 1024, SWIZZLE_NONE), idesc, (acc | (uint32_t)(ks > 0)));
-            if (colsum) {
-#pragma unroll
-              for (int h = 0; h < 2; ++h)  // columns [N, N+16) behind the GEMM's: A^T * ones (every column holds the same sums)
-                mma_ss(tmem + h * 256 + sub.tmem_col + sub.N, smem_desc(a0 + h * 16384 + ks * 256, 128, 1024, SWIZZLE_NONE),
-                       smem_desc(sbase + kDwOffOnes, 128, 1024, SWIZZLE_NONE), idesc_ones, (acc | (uint32_t)(ks > 0)));
-            }
-          }
-          mma_commit(&empty[s]);
-        }
-        __syncwarp();
+      for (int m = 0; m < 2; ++m) {  // M blocks of 64 hidden units = 8 column groups of A
+        const uint64_t da = wg_desc(a0 + (2 * wg + m) * 8192 + ks * 256, 128, 1024, WG_INTERLEAVE);
+        const uint32_t accum = (k > 0 || ks > 0) ? 1u : 0u;
+        if constexpr (N == 128) wg_mma_ss_n128<1, 1>(acc[m], da, db, accum);
+        else if constexpr (N == 64) wg_mma_ss_n64<1, 1>(acc[m], da, db, accum);
+        else wg_mma_ss_n16<1, 1>(acc[m], da, db, accum);
       }
     }
-    if (elect_one()) mma_commit(acc_done);
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(acc[0]);
+    wg_fence_acc(acc[1]);
     __syncwarp();
-    if (prof && lane == 0) prof[4] = w_full;
-  } else if (warp < 6) {
-    const int q = warp & 3;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const uint64_t pol_keep = l2_evict_last();  // the reduce kernel reads these next: keep them in L2 under the activation stream
-    if (my_iters > 0) {
-      mbar_wait(acc_done, 0, 22);
-      tc_fence_after();
-    }
-    for (int sj = 0; sj < n_sub; ++sj) {
-      const DwSub& sub = job.sub[sj];
-      // partial layout [N/4][256 rows][4]: the 32 lanes of a warp (= 32 consecutive rows) write 512 contiguous bytes
-      float4* out = reinterpret_cast<float4*>(sub.part + (int64_t)cta * 256 * sub.N);
-      for (int h = 0; h < 2; ++h) {
-        const int m = h * 128 + q * 32 + lane;
-        for (int c = 0; c < sub.N / 16; ++c) {
-          uint32_t r[16];
-          if (my_iters > 0) {
-            tmem_ld16(tmem + lane_addr + h * 256 + sub.tmem_col + c * 16, r);
-            tmem_ld_wait();
-          } else {
-#pragma unroll
-            for (int i = 0; i < 16; ++i) r[i] = 0u;
-          }
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-            st_hint(&out[(int64_t)(c * 4 + i) * 256 + m],
-                    make_float4(__uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1]), __uint_as_float(r[4 * i + 2]), __uint_as_float(r[4 * i + 3])),
-                    pol_keep);
-        }
-        if (sub.colsum != nullptr) {
-          uint32_t r[16];
-          r[0] = 0u;
-          if (my_iters > 0) {
-            tmem_ld16(tmem + lane_addr + h * 256 + sub.tmem_col + sub.N, r);
-            tmem_ld_wait();
-          }
-          st_hint(&sub.colsum[(int64_t)cta * 256 + m], __uint_as_float(r[0]), pol_keep);
-        }
-      }
-    }
+    if (lane == 0) mbar_arrive(&empty[s]);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (prof && threadIdx.x == 0) prof[1] = clock64() - prof_t0;
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 512);
+  // partial layout [N/4][256 rows][4]: element (m, c) at ((c/4) * 256 + m) * 4 + c % 4
+  const uint64_t pol_keep = l2_evict_last();  // the reduce kernel reads these next: keep them in L2 under the activation stream
+  float* out = job.part + (int64_t)cta * 256 * N;
+#pragma unroll
+  for (int m = 0; m < 2; ++m) {
+    const int r = (2 * wg + m) * 64 + wq * 16 + (lane >> 2);
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int c = 8 * j + 2 * (lane & 3);
+        float* dst = out + ((int64_t)(c >> 2) * 256 + r + 8 * rr) * 4 + (c & 3);
+        st_hint(reinterpret_cast<uint2*>(dst), make_uint2(__float_as_uint(acc[m][4 * j + 2 * rr]), __float_as_uint(acc[m][4 * j + 2 * rr + 1])), pol_keep);
+      }
   }
 }
 
 __global__ void __launch_bounds__(kDwThreads, 1) tc_dw_kernel(const __grid_constant__ DwMaps maps, const DwParams p) {
   extern __shared__ uint8_t smem_raw[];
-  dw_role(smem_raw, maps, p, (int)blockIdx.x, false);
-}
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kDwOffBar);
+  uint64_t* full = bars;                 // [kDwStages]
+  uint64_t* empty = bars + kDwStages;    // [kDwStages]
+  const int warp = threadIdx.x >> 5;
+  const long long prof_t0 = clock64();
 
-// ONE launch for K3a + K3b: the first n_cta[0] + n_cta[1] CTAs are K3a CTAs (fb_role), the rest weight-gradient CTAs
-// (dw_role) that consume the activation tiles as the K3a CTAs of the same grid complete them (flag_t / flag_x),
-// through L2 instead of after a kernel boundary.  All CTAs are co-resident (grid <= 148, one CTA per SM); a consumer only
-// ever waits for K3a CTAs, which wait for nobody outside their own CTA, so the launch cannot deadlock.  The assignment of
-// tiles to CTAs is static => the partial sums keep a fixed association order (run-to-run deterministic gradients).
-template <int NEPI>
-__global__ void __launch_bounds__(fb_threads(NEPI), 1)
-    tc_ppo_fused_kernel(const __grid_constant__ CUtensorMap tmW0a, const __grid_constant__ CUtensorMap tmW1a,
-                        const __grid_constant__ CUtensorMap tmW0c, const __grid_constant__ CUtensorMap tmW1c,
-                        const FbParams p, const __grid_constant__ DwMaps maps, const DwParams dp) {
-  extern __shared__ uint8_t smem_raw[];
-  const int n_fb = p.n_cta[0] + p.n_cta[1];
-  if ((int)blockIdx.x < n_fb) fb_role<NEPI>(smem_raw, tmW0a, tmW1a, tmW0c, tmW1c, p);
-  else dw_role(smem_raw, maps, dp, (int)blockIdx.x - n_fb, true);
+  int j = 0;
+  while (j + 1 < p.n_jobs && (int)blockIdx.x >= p.job[j + 1].cta_begin) ++j;
+  const DwJob& job = p.job[j];
+  const int cta = (int)blockIdx.x - job.cta_begin;
+  const int my_chunks = cta < job.num_chunks ? (job.num_chunks - cta + job.n_cta - 1) / job.n_cta : 0;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kDwStages; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 8);  // one arrival per consumer warp
+    }
+    fence_barrier_init();
+    tma_prefetch_desc(&maps.a[job.map]);
+    tma_prefetch_desc(&maps.b[job.map]);
+  }
+  griddep_launch();
+  __syncthreads();
+  griddep_wait();  // the activations are K3a's output; the partials written below were read by the previous reduce
+
+  if (warp == 8) {
+    if (elect_one()) {
+      const uint64_t pol_stream = l2_policy(p.act_policy);  // default evict_first: every activation tile is read exactly once
+      for (int it = 0; it < my_chunks; ++it) {
+        // newest rows first (K3a wrote the last tiles most recently, so they are the likeliest L2 residents)
+        const int chunk = job.num_chunks - 1 - (cta + it * job.n_cta);  // 64 rows: half of a 128-row tile
+        const int tile = chunk >> 1, r0 = (chunk & 1) * 64;
+        const int s = it % kDwStages;
+        if (it >= kDwStages) mbar_wait(&empty[s], ((it / kDwStages) & 1) ^ 1, 20);
+        uint8_t* st = smem + s * kDwStageBytes;
+        mbar_arrive_expect_tx(&full[s], 32768 + (uint32_t)job.N * 128);
+        // one box = rows r0..r0+63 of the column groups: smem image [colgroup][row][16 B]
+        tma_load_2d_hint(st, &maps.a[job.map], &full[s], r0 * 2, tile * 32, pol_stream);
+        tma_load_2d_hint(st + 32768, &maps.b[job.map], &full[s], r0 * 2, tile * job.b_cg + job.b_cg0, pol_stream);
+      }
+    }
+  } else if (job.N == 128) {
+    dw_consume<128>(smem, full, empty, job, cta, my_chunks);
+  } else if (job.N == 64) {
+    dw_consume<64>(smem, full, empty, job, cta, my_chunks);
+  } else {
+    dw_consume<16>(smem, full, empty, job, cta, my_chunks);
+  }
+  __syncthreads();
+  if (g_prof_buf != nullptr && threadIdx.x == 0) {
+    long long* prof = g_prof_buf + (int64_t)blockIdx.x * 8;
+    prof[0] = 2 + j, prof[1] = clock64() - prof_t0, prof[5] = my_chunks;
+  }
 }
 
 // =============================== reduce partials -> gradient arena ================================
@@ -942,7 +543,7 @@ struct RedSeg {
   int items;            // rows*cols/4 (vec) or rows*cols
 };
 struct RedParams {
-  RedSeg seg[12];
+  RedSeg seg[14];
   int n_seg;
   int total_items;
   const float* metric_part;  // [n_cta_total][8]
@@ -953,12 +554,10 @@ struct RedParams {
   int overwrite;
   double* sumsq;             // nullable: [2][gridDim] block partials of sum((weight*g)^2) per optimiser segment
   unsigned long long* sumsq_count;  // where the number of block partials per segment (= gridDim) is published
-  uint32_t* flags;           // nullable: the fused launch's tile counters, cleared here for the next optimiser step
-  int n_flags;
 };
 
-constexpr int kRedThreads = 288;  // x 592 blocks >= the ~168k gradient entries of the benchmark networks: one element per thread
-constexpr int kRedMaxBlocks = 4 * kNumSMs;  // the optimiser scratch holds 8 x 148 doubles = 2 segments x 592 block partials
+constexpr int kRedThreads = 352;  // x 528 blocks >= the ~173k gradient entries of the benchmark networks: one element per thread
+constexpr int kRedMaxBlocks = 4 * kNumSMs;  // the optimiser scratch holds 8 x 132 doubles = 2 segments x 528 block partials
 
 // Optimiser context of the fused variant (stx_ppo_minibatch_update): clip_by_global_norm + Adam of stx_adam.cu applied
 // by the thread that reduced the gradient entry.  scratch layout = stx_adam.cu's AdamScratch.
@@ -986,12 +585,10 @@ struct FusedOpt {
 // and the thread applies clip + Adam + the bf16 shadow update to its entry: K4 without its launch, its gradient
 // re-read and its own ramp-up.
 template <bool FUSED>
-__global__ void __launch_bounds__(kRedThreads) tc_reduce_kernel(const RedParams p, float* __restrict__ grad, const FusedOpt f) {
+__global__ void __launch_bounds__(kRedThreads, 4) tc_reduce_kernel(const RedParams p, float* __restrict__ grad, const FusedOpt f) {
   griddep_launch();
   griddep_wait();
   const uint64_t pol_keep = l2_evict_last();  // partials and gradients: small, reused every step, latency-critical
-  if (p.flags != nullptr && blockIdx.x == gridDim.x - 1)  // the fused K3 launch that counted them up has completed
-    for (int i = threadIdx.x; i < p.n_flags; i += blockDim.x) p.flags[i] = 0u;
   double sq0 = 0.0, sq1 = 0.0;
   int64_t my_dst = -1;  // FUSED: arena index, value and optimiser segment of this thread's entry
   float my_g = 0.f;
@@ -1129,47 +726,28 @@ inline size_t al(size_t x) { return (x + 255) / 256 * 256; }
 
 struct TcWs {
   __nv_bfloat16 *h1[2], *h2[2], *dh1[2], *dh2[2], *dz[2], *xg;
-  float *part_w1[2], *part_w2[2], *part_w0[2], *db_part[2], *db0_part[2], *metric_part;
-  uint32_t* flags;  // [2][tiles] tile counters, [tiles] xg counters  (fused launch)
+  float *part_w1[2][2], *part_w2[2], *part_w0[2], *db_part[2], *metric_part;
   size_t bytes;
 };
 
-constexpr int kCtaPerNet = kNumSMs / 2;              // 74
-// Launch plan, per network (x 2 networks = 148 CTAs).
-//  split (default): K3a on 74 CTAs, then K3b with 35/18/21 split-K CTAs for dW1 / dW2 / dW0 -- proportional to the
-//    bytes each job streams (dW1: h1 + dh2, dW2: h2 + dz, dW0: dh1 + x): K3b alone is HBM-bound, so the CTAs should finish together.
-//  fused (STX_K3_FUSED=1, experimental): ONE launch; 64 K3a CTAs (256 tiles of the benchmark minibatch = exactly 4 each),
-//    6 CTAs accumulate dW1 and 4 CTAs dW2 + dW0 + db0 behind per-tile flags.  Parity-green, but MEASURED SLOWER on B200
-//    (profiles/r02_k3_fused_accounting.txt: 267 us per minibatch step at 64/6/4, 131 us at 40/21/13, split 113 us in the
-//    same eager loop): with the full-size activation workspace the stream still goes through HBM (145 MB written + 145 MB
-//    read per step), and a weight-gradient CTA with 192 KB of TMA loads in flight sustains only ~44 B/clk against that
-//    saturated memory system (1.45k cycles per 64 KB stage against 1.0k of MMA; the 33-40 KB stages of the dW2/dW0 job are
-//    pure latency: 1.6k cycles each).  It needs an L2-resident ring of tile slots to pay off; kept for that experiment.
-//  Tuning switches: STX_DW_SPLIT="w1,w2,w0" (split), STX_K3_SPLIT="fb,w1,w02" (fused), each summing to 74.
+constexpr int kCtaPerNet = kNumSMs / 2;              // 66
+// Launch plan, per network (x 2 networks = 132 CTAs): K3a on 66 CTAs, then K3b with 19 + 19 / 13 / 15 split-K CTAs for
+// the two column halves of dW1 / dW2 / dW0 -- proportional to the bytes each job streams (dW1 half: h1 + half of dh2,
+// dW2: h2 + dz, dW0: dh1 + x): K3b is memory-bound, so the CTAs should finish together.
+// Tuning switches: STX_DW_SPLIT="w1,w2,w0" (CTAs per dW1 half, dW2, dW0; 2 w1 + w2 + w0 = 66), STX_K3_POLICY (L2 policy
+// of the activation stream: 0 evict_first, 1 normal, 2 evict_last).
 struct K3Plan {
-  int w1 = 35, w2 = 18, w0 = 21;   // split
-  bool fused = false;
-  int fb = 64, fw1 = 6, fw02 = 4;  // fused
-  int act_policy = 0;              // L2 policy of the activation stream (STX_K3_POLICY: 0 evict_first, 1 normal, 2 evict_last)
-  int ring = 0;                    // fused: tile slots per network of the activation ring (STX_K3_RING; 0 = one slot per tile)
+  int w1 = 19, w2 = 13, w0 = 15;
+  int act_policy = 0;
   K3Plan() {
     int a, b, c;
     const char* e = getenv("STX_DW_SPLIT");
-    if (e && sscanf(e, "%d,%d,%d", &a, &b, &c) == 3 && a > 0 && b > 0 && c > 0 && a + b + c == kCtaPerNet) w1 = a, w2 = b, w0 = c;
-    e = getenv("STX_K3_SPLIT");
-    if (e && sscanf(e, "%d,%d,%d", &a, &b, &c) == 3 && a > 0 && b > 0 && c > 0 && a + b + c == kCtaPerNet) fb = a, fw1 = b, fw02 = c;
-    e = getenv("STX_K3_FUSED");
-    if (e) fused = e[0] == '1';
-    e = getenv("STX_K3_RING");
-    if (e) ring = atoi(e);
+    if (e && sscanf(e, "%d,%d,%d", &a, &b, &c) == 3 && a > 0 && b > 0 && c > 0 && 2 * a + b + c == kCtaPerNet) w1 = a, w2 = b, w0 = c;
     e = getenv("STX_K3_POLICY");
     if (e) act_policy = atoi(e);
   }
 };
 static const K3Plan g_plan;
-#define kDwCtaW1 (g_plan.w1)
-#define kDwCtaW2 (g_plan.w2)
-#define kDwCtaW0 (g_plan.w0)
 
 TcWs carve_tc(int64_t mb, char* base) {
   TcWs w{};
@@ -1179,21 +757,16 @@ TcWs carve_tc(int64_t mb, char* base) {
     o += al(bytes);
     return q;
   };
-  const int tiles = (int)(mb / 128);
-  w.flags = (uint32_t*)take((size_t)3 * tiles * 4);  // first: the caller zero-fills the workspace once, the reduce kernel re-zeroes
-  const int n_w1 = g_plan.fused ? g_plan.fw1 : g_plan.w1, n_w2 = g_plan.fused ? g_plan.fw02 : g_plan.w2,
-            n_w0 = g_plan.fused ? g_plan.fw02 : g_plan.w0;
   for (int n = 0; n < 2; ++n) {
     w.h1[n] = (__nv_bfloat16*)take((size_t)mb * 256 * 2);
     w.h2[n] = (__nv_bfloat16*)take((size_t)mb * 256 * 2);
     w.dh1[n] = (__nv_bfloat16*)take((size_t)mb * 256 * 2);
     w.dh2[n] = (__nv_bfloat16*)take((size_t)mb * 256 * 2);
     w.dz[n] = (__nv_bfloat16*)take((size_t)mb * 16 * 2);
-    w.part_w1[n] = (float*)take((size_t)n_w1 * 65536 * 4);
-    w.part_w2[n] = (float*)take((size_t)n_w2 * 256 * 16 * 4);
-    w.part_w0[n] = (float*)take((size_t)n_w0 * 256 * 64 * 4);
+    for (int hh = 0; hh < 2; ++hh) w.part_w1[n][hh] = (float*)take((size_t)g_plan.w1 * 256 * 128 * 4);
+    w.part_w2[n] = (float*)take((size_t)g_plan.w2 * 256 * 16 * 4);
+    w.part_w0[n] = (float*)take((size_t)g_plan.w0 * 256 * 64 * 4);
     w.db_part[n] = (float*)take((size_t)kCtaPerNet * 528 * 4);
-    w.db0_part[n] = (float*)take((size_t)n_w0 * 256 * 4);
   }
   w.xg = (__nv_bfloat16*)take((size_t)mb * 64 * 2);
   w.metric_part = (float*)take((size_t)kNumSMs * 8 * 4);
@@ -1239,9 +812,7 @@ int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxP
   int64_t aoff, coff, total;
   stx_ppo_arena_offsets(actor, critic, &aoff, &coff, &total);
   const int64_t noff[2] = {aoff, coff};
-  const bool fused = g_plan.fused;
-  const int num_tiles = (int)(mb / 128);
-  const int n_fb = fused ? g_plan.fb : kCtaPerNet;  // K3a CTAs per network
+  const int n_fb = kCtaPerNet;  // K3a CTAs per network
 
   // ---- K3a parameters ----
   FbParams fp{};
@@ -1268,64 +839,39 @@ int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxP
   fp.adv_stats = h->standardize_advantages ? b->adv_stats : nullptr;
   fp.metric_part = ws.metric_part;
   fp.D = D, fp.mb = (int)mb, fp.clip_eps = h->clip_eps, fp.ent_coef = h->ent_coef, fp.vf_coef = h->vf_coef;
-  const int ring_tiles = (fused && g_plan.ring > 0 && g_plan.ring < num_tiles) ? g_plan.ring : 0;
-  if (fused) fp.flag_t = ws.flags, fp.flag_x = ws.flags + 2 * num_tiles;
-  fp.ring_tiles = ring_tiles, fp.act_policy = g_plan.act_policy;
+  fp.act_policy = g_plan.act_policy;
 
   // ---- K3b parameters ----
   DwMaps maps;
   DwParams dp{};
-  int cta = 0, jn = 0, mi = 0;
+  int cta = 0, jn = 0;
   const int chunks = (int)(mb / 64);
-  const uint64_t tiles = (uint64_t)(ring_tiles > 0 ? ring_tiles : num_tiles);
-  int n_w1 = 0, n_w2 = 0, n_w0 = 0;  // partials per network of each weight gradient (for the reduce below)
+  const uint64_t tiles = (uint64_t)(mb / 128);
   for (int n = 0; n < 2; ++n) {
-    // tensor-map pairs of this network: m1 (h1, dh2) -> dW1, m2 (h2, dz) -> dW2, m0 (dh1, xg) -> dW0^T (+ db0 = dh1^T * 1)
-    const int m1 = mi++, m2 = mi++, m0 = mi++;
-    if (int rc = make_map_tiled(&maps.a[m1], ws.h1[n], tiles, 32)) return rc;
-    if (int rc = make_map_tiled(&maps.b[m1], ws.dh2[n], tiles, 32)) return rc;
-    if (int rc = make_map_tiled(&maps.a[m2], ws.h2[n], tiles, 32)) return rc;
-    if (int rc = make_map_tiled(&maps.b[m2], ws.dz[n], tiles, 2)) return rc;
-    if (int rc = make_map_tiled(&maps.a[m0], ws.dh1[n], tiles, 32)) return rc;
-    if (int rc = make_map_tiled(&maps.b[m0], ws.xg, tiles, 8)) return rc;
-    const DwSub s1{ws.part_w1[n], nullptr, 256, m1, 0, 0};
-    const DwSub s2{ws.part_w2[n], nullptr, 16, m2, fused ? 96 : 0, 0};
-    const DwSub s0{ws.part_w0[n], ws.db0_part[n], 64, m0, 0, 1};
-    auto add_job = [&](int n_cta, int n_sub, DwSub a, DwSub c) {
-      DwJob& j = dp.job[jn++];
-      j.sub[0] = a, j.sub[1] = c, j.n_sub = n_sub, j.cta_begin = cta, j.n_cta = n_cta, j.num_chunks = chunks, j.net = n;
-      cta += n_cta;
+    auto add_job = [&](float* part, int N, const __nv_bfloat16* a, const __nv_bfloat16* bm, int b_cg, int b_cg0, int n_cta) -> int {
+      DwJob& j = dp.job[jn];
+      if (int rc = make_map_tiled(&maps.a[jn], a, tiles, 32, 32)) return rc;
+      if (int rc = make_map_tiled(&maps.b[jn], bm, tiles, (uint32_t)b_cg, (uint32_t)(N / 8))) return rc;
+      j.part = part, j.N = N, j.map = jn, j.b_cg = b_cg, j.b_cg0 = b_cg0, j.cta_begin = cta, j.n_cta = n_cta, j.num_chunks = chunks;
+      cta += n_cta, ++jn;
+      return STX_OK;
     };
-    if (fused) {
-      add_job(g_plan.fw1, 1, s1, s1);
-      add_job(g_plan.fw02, 2, s2, s0);  // per chunk: dW2 (operands complete after E3) first, then dW0 (needs dh1)
-      n_w1 = g_plan.fw1, n_w2 = n_w0 = g_plan.fw02;
-    } else {
-      add_job(kDwCtaW1, 1, s1, s1);
-      add_job(kDwCtaW2, 1, s2, s2);
-      add_job(kDwCtaW0, 1, s0, s0);
-      n_w1 = kDwCtaW1, n_w2 = kDwCtaW2, n_w0 = kDwCtaW0;
-    }
+    // dW1 = h1^T dh2 (two column halves), dW2 = h2^T dz, dW0^T = dh1^T xg
+    if (int rc = add_job(ws.part_w1[n][0], 128, ws.h1[n], ws.dh2[n], 32, 0, g_plan.w1)) return rc;
+    if (int rc = add_job(ws.part_w1[n][1], 128, ws.h1[n], ws.dh2[n], 32, 16, g_plan.w1)) return rc;
+    if (int rc = add_job(ws.part_w2[n], 16, ws.h2[n], ws.dz[n], 2, 0, g_plan.w2)) return rc;
+    if (int rc = add_job(ws.part_w0[n], 64, ws.dh1[n], ws.xg, 8, 0, g_plan.w0)) return rc;
   }
-  dp.n_jobs = jn, dp.num_tiles = num_tiles, dp.ring_tiles = ring_tiles, dp.act_policy = g_plan.act_policy;
-  if (fused) dp.flag_t = fp.flag_t, dp.flag_x = fp.flag_x;
+  dp.n_jobs = jn, dp.act_policy = g_plan.act_policy;
 
   // ---- launches ----
-  // 8 epilogue warps: 16 (two parts per step, 80 registers) measured 5 % slower (profiles/README.md)
-  if (fused) {
-    if (int rc = opt_in_smem(tc_ppo_fused_kernel<8>, kFbSmemBytes > kDwSmemBytes ? kFbSmemBytes : kDwSmemBytes, 2)) return rc;
-    STX_CUDA_OK(launch_pdl(tc_ppo_fused_kernel<8>, dim3(2 * n_fb + cta), dim3(fb_threads(8)),
-                           kFbSmemBytes > kDwSmemBytes ? kFbSmemBytes : kDwSmemBytes, st, tmW0[0], tmW1[0], tmW0[1], tmW1[1], fp, maps, dp));
-    STX_LAUNCH_OK();
-  } else {
-    if (int rc = opt_in_smem(tc_ppo_fwd_bwd_kernel<8>, kFbSmemBytes, 0)) return rc;
-    if (int rc = opt_in_smem(tc_dw_kernel, kDwSmemBytes, 1)) return rc;
-    STX_CUDA_OK(launch_pdl(tc_ppo_fwd_bwd_kernel<8>, dim3(2 * n_fb), dim3(fb_threads(8)), kFbSmemBytes, st, tmW0[0], tmW1[0], tmW0[1],
-                           tmW1[1], fp));
-    STX_LAUNCH_OK();
-    STX_CUDA_OK(launch_pdl(tc_dw_kernel, dim3(cta), dim3(kDwThreads), kDwSmemBytes, st, maps, dp));
-    STX_LAUNCH_OK();
-  }
+  if (int rc = opt_in_smem(tc_ppo_fwd_bwd_kernel, kFbSmemBytes, 0)) return rc;
+  if (int rc = opt_in_smem(tc_dw_kernel, kDwSmemBytes, 1)) return rc;
+  STX_CUDA_OK(launch_pdl(tc_ppo_fwd_bwd_kernel, dim3(2 * n_fb), dim3(kFbThreads), kFbSmemBytes, st, tmW0[0], tmW1[0], tmW0[1],
+                         tmW1[1], fp));
+  STX_LAUNCH_OK();
+  STX_CUDA_OK(launch_pdl(tc_dw_kernel, dim3(cta), dim3(kDwThreads), kDwSmemBytes, st, maps, dp));
+  STX_LAUNCH_OK();
 
   // ---- reduce ----
   RedParams rp{};
@@ -1344,10 +890,11 @@ int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxP
     const int A = nets[n]->sizes[3];
     const int64_t o_w0 = noff[n], o_b0 = o_w0 + (int64_t)D * kH, o_w1 = o_b0 + kH, o_b1 = o_w1 + (int64_t)kH * kH, o_w2 = o_b1 + kH,
                   o_b2 = o_w2 + (int64_t)kH * A;
-    add_seg(ws.part_w1[n], 65536, n_w1, kH, kH, 256, 0, kH, o_w1, n, 1);           // dW1[in][out]
-    add_seg(ws.part_w0[n], 256 * 64, n_w0, kH, D, 64, 1, kH, o_w0, n, 1);          // part(j, d) -> W0[d][j]
-    add_seg(ws.part_w2[n], 256 * 16, n_w2, kH, A, 16, 0, A, o_w2, n, 1);           // dW2[j][a]
-    add_seg(ws.db0_part[n], 256, n_w0, 1, kH, 256, 0, kH, o_b0, n, 0);             // db0 from K3b (column sums of dh1)
+    add_seg(ws.part_w1[n][0], 256 * 128, g_plan.w1, kH, 128, 128, 0, kH, o_w1, n, 1);         // dW1[in][out], out 0..127
+    add_seg(ws.part_w1[n][1], 256 * 128, g_plan.w1, kH, 128, 128, 0, kH, o_w1 + 128, n, 1);   // out 128..255
+    add_seg(ws.part_w0[n], 256 * 64, g_plan.w0, kH, D, 64, 1, kH, o_w0, n, 1);      // part(j, d) -> W0[d][j]
+    add_seg(ws.part_w2[n], 256 * 16, g_plan.w2, kH, A, 16, 0, A, o_w2, n, 1);       // dW2[j][a]
+    add_seg(ws.db_part[n], 528, n_fb, 1, kH, 528, 0, kH, o_b0, n, 0);
     add_seg(ws.db_part[n] + 256, 528, n_fb, 1, kH, 528, 0, kH, o_b1, n, 0);
     add_seg(ws.db_part[n] + 512, 528, n_fb, 1, A, 528, 0, A, o_b2, n, 0);
   }
@@ -1355,7 +902,6 @@ int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxP
   rp.metric_part = ws.metric_part, rp.n_cta_total = 2 * n_fb, rp.metrics = metrics;
   rp.weight = grad_weight, rp.inv_mb = 1.0f / (float)mb;
   rp.overwrite = opt ? 1 : h->overwrite_grads;
-  if (fused) rp.flags = ws.flags, rp.n_flags = 3 * num_tiles;
   // side output for the fused optimiser: partials[seg][block] right after the 16-byte header of its scratch
   void* adam_scratch = opt ? opt->scratch : h->adam_scratch;
   rp.sumsq = (rp.overwrite && adam_scratch) ? reinterpret_cast<double*>(reinterpret_cast<char*>(adam_scratch) + 16) : nullptr;
@@ -1373,7 +919,7 @@ int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxP
     fo.P = opt->param_arena, fo.MU = opt->mu, fo.NU = opt->nu, fo.counts = opt->counts, fo.segs = opt->segs, fo.h = opt->hyper;
     fo.P16 = reinterpret_cast<__nv_bfloat16*>(opt->params_bf16), fo.gnorm_out = opt->gnorm_out;
     char* sc = reinterpret_cast<char*>(opt->scratch);
-    // own ticket words (stx_adam.cu keeps its barrier / last-block tickets for a 148-block grid in the same scratch: the
+    // own ticket words (stx_adam.cu keeps its barrier / last-block tickets for a kNumSMs-block grid in the same scratch: the
     // modulo arithmetic of a ticket is only valid for one grid size)
     char* tail = sc + 16 + sizeof(double) * 8 * kNumSMs;  // = sizeof(AdamScratch) + partials; 64 spare bytes follow
     fo.arrive = reinterpret_cast<unsigned long long*>(tail + 24);

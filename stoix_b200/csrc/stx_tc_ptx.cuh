@@ -1,7 +1,6 @@
-// Thin inline-PTX wrappers for the Blackwell (sm_100a) tensor-core path: mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 alloc / mma / commit / ld / st / fences, and the UMMA shared-memory
-// and instruction descriptors.  Bit layouts follow the PTX ISA "tcgen05" chapter (the same fields as
-// cute/arch/mma_sm100_desc.hpp in CUTLASS 4.x, used here only as a reference for the encoding).
+// Thin inline-PTX wrappers for the Hopper (sm_90a) tensor-core path: mbarrier, TMA (cp.async.bulk.tensor),
+// warpgroup MMA (wgmma.mma_async) and its shared-memory matrix descriptors.  Bit layouts follow the PTX ISA
+// "Asynchronous Warpgroup Level Matrix Multiply-Accumulate" chapter.
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -78,116 +77,95 @@ __device__ __forceinline__ void tma_load_2d_hint(void* smem_dst, const CUtensorM
       : "memory");
 }
 
-// ---- tcgen05: TMEM allocation -------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// ---- wgmma ------------------------------------------------------------------------------------
+// A warpgroup (4 consecutive warps, first warp index a multiple of 4) computes D[64 x N] (+)= A[64 x 16] * B[16 x N] per
+// instruction.  D lives in registers: thread t = 32 w + l holds rows 16 w + l/4 and 16 w + l/4 + 8; for every 8-column
+// block j it holds d[4j + {0,1}] = (row, 8j + 2(l%4) + {0,1}) and d[4j + {2,3}] = (row + 8, same columns).  An A operand
+// in registers has the same shape per 16-wide K block, so packing consecutive accumulator pairs to bf16x2 turns the
+// output of one GEMM into the A operand of the next without leaving the registers.
+enum : uint32_t { WG_INTERLEAVE = 0, WG_SW128 = 1 };
 
-// ---- descriptors ------------------------------------------------------------------------------
-enum : uint32_t { SWIZZLE_NONE = 0, SWIZZLE_128B = 2, SWIZZLE_64B = 4, SWIZZLE_32B = 6 };
-
-// Shared-memory matrix descriptor (64-bit).  Byte quantities are given in bytes (must be multiples of 16).
-__device__ __forceinline__ uint64_t smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
+// Shared-memory matrix descriptor (64-bit), LBO / SBO in bytes (multiples of 16), canonical layouts of the PTX ISA:
+//   K-major, no swizzle:  SBO = stride of 8-row groups (M/N), LBO = stride of 8-element core matrices along K
+//   K-major, 128B swizzle: SBO = stride of 8-row groups (1024 for packed rows), LBO unused
+//   MN-major, no swizzle: SBO = stride of 8-element core matrices along M/N, LBO = stride of 8-row groups along K
+//   MN-major, 128B swizzle: LBO = stride of 64-element blocks along M/N, SBO = stride of 8-row groups along K
+__device__ __forceinline__ uint64_t wg_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFFu);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;              // descriptor version (Blackwell)
-  d |= (uint64_t)(layout & 7u) << 61;  // swizzle mode
+  d |= (uint64_t)(layout & 3u) << 62;
   return d;
 }
+__device__ __forceinline__ uint64_t wg_adv(uint64_t desc, uint32_t bytes) { return desc + (uint64_t)(bytes >> 4); }  // start field, no carry
 
-// Instruction descriptor for kind::f16 with BF16 inputs and FP32 accumulation.
-// a_mn / b_mn: 1 = the operand is MN-major ("transposed"), 0 = K-major.
-__host__ __device__ constexpr uint32_t idesc_bf16(int M, int N, int a_mn, int b_mn) {
-  return (1u << 4)                      // D format F32
-         | (1u << 7)                    // A format BF16
-         | (1u << 10)                   // B format BF16
-         | ((uint32_t)a_mn << 15) | ((uint32_t)b_mn << 16)
-         | ((uint32_t)(N >> 3) << 17)   // N / 8
-         | ((uint32_t)(M >> 4) << 24);  // M / 16
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMA
+template <int R>
+__device__ __forceinline__ void wg_fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
+// named barrier of the 128 threads of one warpgroup (ids 1.. ; 0 is __syncthreads)
+__device__ __forceinline__ void wg_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
-// ---- tcgen05.mma (single elected thread) -------------------------------------------------------
-// D[tmem] (+)= A[smem] * B[smem]
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+// SS form: A and B from shared memory (TA / TB: 1 = the operand is MN-major); RS form: A from registers (4 x bf16x2).
+template <int TA, int TB>
+__device__ __forceinline__ void wg_mma_ss_n16(float (&d)[8], uint64_t da, uint64_t db, uint32_t acc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
 }
-// D[tmem] (+)= A[tmem] * B[smem]   (A: 128 lanes x K/2 packed-bf16 columns)
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+template <int TA, int TB>
+__device__ __forceinline__ void wg_mma_ss_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t acc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, %35, %36;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
 }
-// All previously issued MMAs of this thread arrive on `bar` when complete (implies fence::before_thread_sync).
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// ---- TMEM <-> registers (warp w may only touch lanes 32*(w%4) .. +31) --------------------------
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {  // 32 consecutive columns of this thread's lane
+template <int TA, int TB>
+__device__ __forceinline__ void wg_mma_ss_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, %67, %68;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
 }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
+template <int TB>
+__device__ __forceinline__ void wg_mma_rs_n16(float (&d)[8], const uint32_t* a, uint64_t db, uint32_t acc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1, %14;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc), "n"(TB));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
+template <int TB>
+__device__ __forceinline__ void wg_mma_rs_n128(float (&d)[64], const uint32_t* a, uint64_t db, uint32_t acc) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64,%65,%66,%67}, %68, p, 1, 1, %70;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc), "n"(TB));
 }
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};"
-               ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1,%2,%3,%4};" ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]) : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);  // .x = lo (low 16 bits), .y = hi
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
-// bf16x2( relu(acc0 + b.x), relu(acc1 + b.y) ): one packed add (FADD2) + one convert with the ReLU folded in
-// (cvt.rn.relu.bf16x2.f32: negative inputs give +0, the rest rounds to nearest even) -- 2 instructions per pair instead of
-// 2 FADD + 2 FMNMX + 1 CVT; the same bits as fmaxf(acc + b, 0) followed by the rounding (rounding keeps the sign).
+// bf16x2( relu(acc0 + b.x), relu(acc1 + b.y) ): two adds + one convert with the ReLU folded in (cvt.rn.relu.bf16x2.f32:
+// negative inputs give +0, the rest rounds to nearest even); the same bits as fmaxf(acc + b, 0) followed by the rounding.
 __device__ __forceinline__ uint32_t bias_relu_pack_bf16(uint32_t acc0, uint32_t acc1, float2 b) {
-  const float2 v = __fadd2_rn(make_float2(__uint_as_float(acc0), __uint_as_float(acc1)), b);
+  const float v0 = __fadd_rn(__uint_as_float(acc0), b.x), v1 = __fadd_rn(__uint_as_float(acc1), b.y);
   uint32_t d;
-  asm("cvt.rn.relu.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(v.y), "f"(v.x));  // first source -> upper half
+  asm("cvt.rn.relu.bf16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(v1), "f"(v0));  // first source -> upper half
   return d;
 }
 
@@ -199,6 +177,101 @@ __device__ __forceinline__ bool elect_one() {
       "selp.u32 %0, 1, 0, p;\n\t}"
       : "=r"(pred));
   return pred != 0;
+}
+
+// ---- MLP[D<=64, 256, 256, A<=16] building blocks (one warpgroup, one 64-row tile) ----------------------------------
+// Shared-memory images of the weights (the same images serve the forward and the backward pass):
+//   W1 (256 x 256, row-major (in, out)): 4 TMA boxes [256 rows x 64 columns] of 128B-swizzled rows at kImgW1 + 32768 j
+//      (j = column block): MN-major B operand of the forward, K-major B operand of the backward (W1^T).
+//   W0 (D x 256): 4 boxes [64 rows x 64 columns] at kImgW0 + 8192 j (rows >= D zero-filled by TMA).
+//   W2 (256 x A): element (j, n) at kImgW2 + (j/8)*256 + (n/8)*128 + (j%8)*16 + (n%8)*2, zero for n >= A (no swizzle).
+//   X  (64 rows x 64 columns, bf16): 128B-swizzled rows, 16-byte chunk c of row r at r*128 + ((c ^ (r%8)) << 4).
+constexpr uint32_t kImgW1 = 0, kImgW0 = 131072, kImgW2 = 163840, kImgWBytes = 172032;
+
+// W2 image and biases staged by all threads of the block (generic proxy; the caller fences and synchronises)
+__device__ __forceinline__ void stage_w2_bias(uint8_t* smem, const __nv_bfloat16* w2, const float* b0, const float* b1, const float* b2,
+                                              int A, float* s_b0, float* s_b1, float* s_b2) {
+  for (int j = threadIdx.x; j < 256; j += blockDim.x) {  // one thread per W2 row: its (<=16) loads are in flight together
+    uint32_t pk[8];
+    unsigned short e[16];
+#pragma unroll
+    for (int n = 0; n < 16; ++n) e[n] = n < A ? reinterpret_cast<const unsigned short*>(w2)[j * A + n] : (unsigned short)0;
+#pragma unroll
+    for (int n = 0; n < 8; ++n) pk[n] = (uint32_t)e[2 * n] | ((uint32_t)e[2 * n + 1] << 16);
+    uint8_t* dst = smem + kImgW2 + (j >> 3) * 256 + (j & 7) * 16;
+    *reinterpret_cast<uint4*>(dst) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+    *reinterpret_cast<uint4*>(dst + 128) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
+  }
+  for (int i = threadIdx.x; i < 256; i += blockDim.x) s_b0[i] = b0[i], s_b1[i] = b1[i];
+  if (threadIdx.x < 16) s_b2[threadIdx.x] = threadIdx.x < A ? b2[threadIdx.x] : 0.f;
+}
+
+template <int R>
+__device__ __forceinline__ void wg_zero(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) d[i] = 0.f;
+}
+
+// acc = X * W0[:, 128 h .. 128 h + 127]   (K = 64)
+__device__ __forceinline__ void gemm_x_w0(float (&acc)[64], uint32_t s_x, uint32_t sbase, int h) {
+  const uint64_t dx = wg_desc(s_x, 16, 1024, WG_SW128), db = wg_desc(sbase + kImgW0 + h * 16384, 8192, 1024, WG_SW128);
+  wg_fence_acc(acc);
+  wg_fence();
+#pragma unroll
+  for (int k = 0; k < 4; ++k) wg_mma_ss_n128<0, 1>(acc, wg_adv(dx, k * 32), wg_adv(db, k * 2048), k > 0);
+  wg_commit();
+  wg_wait<0>();
+  wg_fence_acc(acc);
+}
+// acc = A * W1[:, 128 h ..]   (A: 64 x 256 in registers, 16 K blocks of 4 bf16x2)
+__device__ __forceinline__ void gemm_a_w1(float (&acc)[64], const uint32_t (&a)[64], uint32_t sbase, int h) {
+  const uint64_t db = wg_desc(sbase + kImgW1 + h * 65536, 32768, 1024, WG_SW128);
+  wg_fence_acc(acc);
+  wg_fence();
+#pragma unroll
+  for (int kb = 0; kb < 16; ++kb) wg_mma_rs_n128<1>(acc, &a[4 * kb], wg_adv(db, kb * 2048), kb > 0);
+  wg_commit();
+  wg_wait<0>();
+  wg_fence_acc(acc);
+}
+// acc = A * W1^T[:, 128 h ..]  (the W1 image read K-major: K = output unit, N = input unit)
+__device__ __forceinline__ void gemm_a_w1t(float (&acc)[64], const uint32_t (&a)[64], uint32_t sbase, int h) {
+  const uint64_t db = wg_desc(sbase + kImgW1 + h * 16384, 16, 1024, WG_SW128);
+  wg_fence_acc(acc);
+  wg_fence();
+#pragma unroll
+  for (int kb = 0; kb < 16; ++kb) wg_mma_rs_n128<0>(acc, &a[4 * kb], wg_adv(db, (kb >> 2) * 32768 + (kb & 3) * 32), kb > 0);
+  wg_commit();
+  wg_wait<0>();
+  wg_fence_acc(acc);
+}
+// z = A * W2   (64 x 16; columns >= A are zero)
+__device__ __forceinline__ void gemm_a_w2(float (&z)[8], const uint32_t (&a)[64], uint32_t sbase) {
+  const uint64_t db = wg_desc(sbase + kImgW2, 256, 128, WG_INTERLEAVE);
+  wg_fence_acc(z);
+  wg_fence();
+#pragma unroll
+  for (int kb = 0; kb < 16; ++kb) wg_mma_rs_n16<1>(z, &a[4 * kb], wg_adv(db, kb * 512), kb > 0);
+  wg_commit();
+  wg_wait<0>();
+  wg_fence_acc(z);
+}
+// acc = dZ * W2^T[:, 128 h ..]  (dZ: 64 x 16 in registers, the W2 image read K-major)
+__device__ __forceinline__ void gemm_dz_w2t(float (&acc)[64], const uint32_t (&dz)[4], uint32_t sbase, int h) {
+  wg_fence_acc(acc);
+  wg_fence();
+  wg_mma_rs_n128<0>(acc, dz, wg_desc(sbase + kImgW2 + h * 4096, 128, 256, WG_INTERLEAVE), 0);
+  wg_commit();
+  wg_wait<0>();
+  wg_fence_acc(acc);
+}
+// half h of a hidden layer's epilogue: a[32 h + i] = bf16x2(relu(acc[2i] + b), relu(acc[2i+1] + b)), the A operand of the next GEMM
+__device__ __forceinline__ void epi_bias_relu(const float (&acc)[64], const float* bias, int h, uint32_t (&a)[64], int lane) {
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {
+    const float2 b = *reinterpret_cast<const float2*>(bias + 128 * h + 8 * (i >> 1) + 2 * (lane & 3));
+    a[32 * h + i] = bias_relu_pack_bf16(__float_as_uint(acc[2 * i]), __float_as_uint(acc[2 * i + 1]), b);
+  }
 }
 
 }  // namespace tc

@@ -1,20 +1,20 @@
-// Fused persistent rollout for the synthetic Box environment (bf16 / tcgen05 path).
+// Fused persistent rollout for the synthetic Box environment (bf16 / wgmma path).
 //
 // Reference semantics: the T-step lax.scan of _env_step (stoix/systems/ppo/anakin/ff_ppo.py:81-140) for
 // the actor side: logits = actor(obs_t) -> action ~ Categorical -> log_prob -> env.step.  (value /
 // bootstrap_value are evaluated afterwards in two batched critic launches, see ff_ppo.py in this repo.)
 //
-// One CTA owns 128 environments for the WHOLE rollout (grid = E/128), so the actor's weights are loaded into
+// One CTA owns 64 environments for the WHOLE rollout (grid = E/64), so the actor's weights are loaded into
 // shared memory once per rollout instead of once per step, and the T sequential steps cost one launch.
 // Warp roles:
-//   warps 0..7   environment producers (2 threads per env row): SyntheticBoxEnv's dynamics do not depend on
+//   warps 0..3   one warpgroup: the layer chain of stx_tc_mlp.cu on wgmma (activations in registers), then
+//                Gumbel-max sampling + log-prob of the logits (same Philox counters as stx_categorical =>
+//                identical actions for identical logits).
+//   warps 4..5   environment producers (one thread per env row): SyntheticBoxEnv's dynamics do not depend on
 //                the action (stx_env.cu), so the producers run one step AHEAD of the policy: while the
 //                tensor cores evaluate step t they draw step t's outcome and observation t+1 (same Philox
 //                streams as stx_synth_env_step => bit-identical trajectory), write the trajectory rows and
 //                drop the next observation tile straight into 128B-swizzled shared memory.
-//   warp 8       tcgen05.mma issuer (layer chain through tensor memory, as in stx_tc_mlp.cu)
-//   warps 9..16  epilogue: bias+relu+bf16 (TMEM->TMEM), then Gumbel-max sampling + log-prob in the head
-//                epilogue (same Philox counters as stx_categorical => identical actions).
 // Environments whose dynamics depend on the action use the unfused per-step path.
 #include <cuda.h>
 
@@ -29,14 +29,14 @@ int make_map_2d_pub(CUtensorMap* m, const void* base, uint64_t rows, uint64_t co
 
 namespace ro {
 
-constexpr int kTileM = 128, kH = 256;
-constexpr int kProdWarps = 8, kMmaWarp = 8, kEpiWarp0 = 9;
-constexpr int kThreads = 32 * (kProdWarps + 1 + 8);  // 544
+constexpr int kTileM = 64, kH = 256;
+constexpr int kProdWarps = 2;
+constexpr int kThreads = 128 + 32 * kProdWarps;  // 192
 
-constexpr uint32_t kOffW1 = 0, kOffW0 = 131072, kOffW2 = 163840, kOffX = 172032;
-constexpr uint32_t kOffBias = kOffX + 2 * 16384;
+constexpr uint32_t kOffX = kImgWBytes;  // 2 stages x 8 KB
+constexpr uint32_t kOffBias = kOffX + 2 * 8192;
 constexpr uint32_t kOffBar = kOffBias + 528 * 4;
-constexpr uint32_t kSmemBytes = kOffBar + 128 + 1024;
+constexpr uint32_t kSmemBytes = kOffBar + 64 + 1024;
 
 constexpr uint32_t kTagObs = 0x4f425331u, kTagReset = 0x52535431u, kTagStep = 0x53545031u, kTagCat = 0x43415447u;
 
@@ -75,62 +75,30 @@ __global__ void __launch_bounds__(kThreads, 1)
   float* s_b1 = s_b0 + 256;
   float* s_b2 = s_b1 + 256;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBar);
-  uint64_t* x_full = bars;
-  uint64_t* x_empty = bars + 2;
+  uint64_t* x_full = bars;       // [2] producers -> MMA: observation tile of the step in the stage
+  uint64_t* x_empty = bars + 2;  // [2] MMA -> producers: layer 0 has read the stage
   uint64_t* w_full = bars + 4;
-  uint64_t* d_ready = bars + 5;      // [4] MMA -> epilogue: 64-column part p of the current layer's accumulator is complete
-  uint64_t* chunk_done = bars + 9;   // [4] epilogue -> MMA: part p consumed and its slice of the next A operand written
-  uint64_t* head_ready = bars + 13;  // logits complete
-  uint64_t* head_done = bars + 14;   // logits read out of tensor memory
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 15);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t tile_row0 = (int64_t)blockIdx.x * kTileM;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < 2; ++s) {
       mbar_init(&x_full[s], kProdWarps);
-      mbar_init(&x_empty[s], 1);
+      mbar_init(&x_empty[s], 4);  // one arrival per MMA warp
     }
     mbar_init(w_full, 1);
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(&d_ready[i], 1);
-      mbar_init(&chunk_done[i], 8);  // 4 lane quarters x 2 chunks of 32 columns
-    }
-    mbar_init(head_ready, 1);
-    mbar_init(head_done, 4);
     fence_barrier_init();
-    tma_prefetch_desc(&tmW0);
-    tma_prefetch_desc(&tmW1);
     mbar_arrive_expect_tx(w_full, 32768 + 131072);
-    for (int j = 0; j < 4; ++j) tma_load_2d(smem + kOffW0 + j * 8192, &tmW0, w_full, j * 64, 0);
-    for (int j = 0; j < 4; ++j) tma_load_2d(smem + kOffW1 + j * 32768, &tmW1, w_full, j * 64, 0);
+    for (int j = 0; j < 4; ++j) tma_load_2d(smem + kImgW0 + j * 8192, &tmW0, w_full, j * 64, 0);
+    for (int j = 0; j < 4; ++j) tma_load_2d(smem + kImgW1 + j * 32768, &tmW1, w_full, j * 64, 0);
   }
-  if (warp == kMmaWarp) tmem_alloc(tmem_slot, 512);
-  {
-    uint8_t* w2s = smem + kOffW2;
-    for (int j = threadIdx.x; j < kH; j += kThreads) {
-      uint32_t pk[8];
-      unsigned short e[16];
-#pragma unroll
-      for (int n = 0; n < 16; ++n) e[n] = n < p.A ? reinterpret_cast<const unsigned short*>(p.w2)[j * p.A + n] : (unsigned short)0;
-#pragma unroll
-      for (int n = 0; n < 8; ++n) pk[n] = (uint32_t)e[2 * n] | ((uint32_t)e[2 * n + 1] << 16);
-      uint8_t* dst = w2s + (j >> 3) * 256 + (j & 7) * 16;
-      *reinterpret_cast<uint4*>(dst) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-      *reinterpret_cast<uint4*>(dst + 128) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-    }
-    for (int i = threadIdx.x; i < 256; i += kThreads) s_b0[i] = p.b0[i], s_b1[i] = p.b1[i];
-    if (threadIdx.x < 16) s_b2[threadIdx.x] = threadIdx.x < p.A ? p.b2[threadIdx.x] : 0.f;
-    fence_async_proxy();
-  }
-  tc_fence_before();
+  stage_w2_bias(smem, p.w2, p.b0, p.b1, p.b2, p.A, s_b0, s_b1, s_b2);
+  fence_async_proxy();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
-  if (warp < kProdWarps) {
-    // ===================== environment producers: 2 threads per env row =====================
-    const int r = threadIdx.x >> 1, hf = threadIdx.x & 1;
+  if (warp >= 4) {
+    // ===================== environment producers: one thread per env row =====================
+    const int r = threadIdx.x - 128;
     const int64_t e = tile_row0 + r;
     const int dchunks = p.D >> 3;
     const uint64_t step0 = p.env_step + (p.env_counter ? *p.env_counter : 0ull);
@@ -141,8 +109,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     {
       uint8_t* xs = smem + kOffX + r * 128;
 #pragma unroll
-      for (int cc = 0; cc < 4; ++cc) {
-        const int c = hf * 4 + cc;
+      for (int c = 0; c < 8; ++c) {
         uint4 v = make_uint4(0u, 0u, 0u, 0u);
         if (c < dchunks) v = *reinterpret_cast<const uint4*>(p.obs + e * p.D + c * 8);
         *reinterpret_cast<uint4*>(xs + ((c ^ (r & 7)) << 4)) = v;
@@ -159,11 +126,15 @@ __global__ void __launch_bounds__(kThreads, 1)
       const bool term = u01(rs.z) < p.p_term;
       const bool trunc = !term && (u01(rs.w) < p.p_trunc);
       const bool last = term || trunc;
-      uint4 nx[4], ob[4];
-#pragma unroll
-      for (int cc = 0; cc < 4; ++cc) {
-        const int c = hf * 4 + cc;
-        nx[cc] = make_uint4(0u, 0u, 0u, 0u);
+      __nv_bfloat16* nrow = p.next_obs + ((int64_t)t * p.E + e) * p.D;
+      __nv_bfloat16* orow = p.obs + ((int64_t)(t + 1) * p.E + e) * p.D;
+      const int s = (t + 1) & 1;
+      const bool fill = t + 1 < p.T;  // next observation tile -> smem stage (t+1)&1 (consumed by the forward of step t+1)
+      if (fill && t >= 1) mbar_wait(&x_empty[s], (((t - 1) >> 1) & 1), 30);  // layer 0 of step t-1 has read this stage
+      uint8_t* xs = smem + kOffX + s * 8192 + r * 128;
+#pragma unroll 1
+      for (int c = 0; c < 8; ++c) {
+        uint4 nx = make_uint4(0u, 0u, 0u, 0u), ob;
         if (c < dchunks) {
           uint32_t w[4];
 #pragma unroll
@@ -174,9 +145,9 @@ __global__ void __launch_bounds__(kThreads, 1)
             w[2 * g2] = pack_bf16(a.x, a.y);
             w[2 * g2 + 1] = pack_bf16(b.x, b.y);
           }
-          nx[cc] = make_uint4(w[0], w[1], w[2], w[3]);
+          nx = make_uint4(w[0], w[1], w[2], w[3]);
         }
-        ob[cc] = nx[cc];
+        ob = nx;
         if (last && c < dchunks) {
           uint32_t w[4];
 #pragma unroll
@@ -187,21 +158,15 @@ __global__ void __launch_bounds__(kThreads, 1)
             w[2 * g2] = pack_bf16(a.x, a.y);
             w[2 * g2 + 1] = pack_bf16(b.x, b.y);
           }
-          ob[cc] = make_uint4(w[0], w[1], w[2], w[3]);
+          ob = make_uint4(w[0], w[1], w[2], w[3]);
         }
-      }
-      // trajectory rows (global)
-      __nv_bfloat16* nrow = p.next_obs + ((int64_t)t * p.E + e) * p.D;
-      __nv_bfloat16* orow = p.obs + ((int64_t)(t + 1) * p.E + e) * p.D;
-#pragma unroll
-      for (int cc = 0; cc < 4; ++cc) {
-        const int c = hf * 4 + cc;
-        if (c < dchunks) {
-          *reinterpret_cast<uint4*>(nrow + c * 8) = nx[cc];
-          *reinterpret_cast<uint4*>(orow + c * 8) = ob[cc];
+        if (c < dchunks) {  // trajectory rows (global)
+          *reinterpret_cast<uint4*>(nrow + c * 8) = nx;
+          *reinterpret_cast<uint4*>(orow + c * 8) = ob;
         }
+        if (fill) *reinterpret_cast<uint4*>(xs + ((c ^ (r & 7)) << 4)) = ob;
       }
-      if (hf == 0) {
+      {
         const float rwd = normal2(rs.x, rs.y).x;
         const int64_t o = (int64_t)t * p.E + e;
         const float ret = run_ret + rwd;
@@ -215,131 +180,58 @@ __global__ void __launch_bounds__(kThreads, 1)
         run_ret = last ? 0.f : ret;
         run_len = last ? 0 : len;
       }
-      // next observation tile -> smem stage (t+1)&1 (consumed by the forward of step t+1)
-      if (t + 1 < p.T) {
-        const int s = (t + 1) & 1;
-        if (t >= 1) mbar_wait(&x_empty[s], (((t - 1) >> 1) & 1), 30);  // G0 of step t-1 has read this stage
-        uint8_t* xs = smem + kOffX + s * 16384 + r * 128;
-#pragma unroll
-        for (int cc = 0; cc < 4; ++cc) {
-          const int c = hf * 4 + cc;
-          *reinterpret_cast<uint4*>(xs + ((c ^ (r & 7)) << 4)) = ob[cc];
-        }
+      if (fill) {
         fence_async_proxy();
         __syncwarp();
         if (lane == 0) mbar_arrive(&x_full[s]);
       }
     }
-    if (hf == 0) p.run_return[e] = run_ret, p.run_length[e] = run_len;
-  } else if (warp == kMmaWarp) {
-    // ===================== MMA issuer =====================
-    // Every 256-wide GEMM is issued as four N=64 column parts; part p of the NEXT layer only needs D part p consumed
-    // and the K-chunks of its A operand written (chunk_done[]), so the tensor pipe trails the epilogue part by part
-    // (same scheme as K3a in stx_tc_ppo.cu).  h1 and h2 live in separate TMEM regions for that reason.
-    constexpr uint32_t idesc_n64 = idesc_bf16(128, 64, 0, 1);
-    constexpr uint32_t idesc_n16 = idesc_bf16(128, 16, 0, 1);
-    const uint32_t tmem_d = tmem, tmem_a1 = tmem + 256, tmem_a2 = tmem + 384;
-    // rolled part/group loops with incremental descriptors (see stx_tc_ppo.cu: code size / instruction cache)
-    auto adv = [](uint64_t desc, uint32_t bytes) { return desc + (uint64_t)(bytes >> 4); };
-    const uint64_t dW0 = smem_desc(sbase + kOffW0, 8192, 1024, SWIZZLE_128B), dW1 = smem_desc(sbase + kOffW1, 32768, 1024, SWIZZLE_128B);
-    const uint64_t dW2 = smem_desc(sbase + kOffW2, 256, 128, SWIZZLE_NONE);
+    p.run_return[e] = run_ret, p.run_length[e] = run_len;
+  } else {
+    // ===================== the MMA warpgroup =====================
+    const int q4 = lane & 3;
+    const int row = warp * 16 + (lane >> 2);  // rows row and row + 8 of the tile; lanes q4 = 0 / 1 sample them
+    const int64_t e = tile_row0 + row + 8 * (q4 & 1);
+    const uint64_t call0 = p.cat_offset + (p.cat_counter ? *p.cat_counter : 0ull);
+    const uint2 ckey = make_uint2((uint32_t)p.cat_seed, (uint32_t)(p.cat_seed >> 32));
     mbar_wait(w_full, 0, 31);
     for (int t = 0; t < p.T; ++t) {
       const int s = t & 1;
       mbar_wait(&x_full[s], (t >> 1) & 1, 32);
-      if (t > 0) mbar_wait(head_done, (t - 1) & 1, 33);  // the logits of step t-1 have left D columns 0..15
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t dX = smem_desc(sbase + kOffX + s * 16384, 16, 1024, SWIZZLE_128B);
-#pragma unroll 1
-        for (int pt = 0; pt < 4; ++pt) {  // layer 0: D0 = X (K-major SW128) * W0 (MN-major SW128), K = 64
-          const uint64_t b0 = adv(dW0, pt * 8192);
+      float acc[64];
+      uint32_t a1[64], a2[64];
+      wg_zero(acc);
 #pragma unroll
-          for (int k = 0; k < 4; ++k) mma_ss(tmem_d + pt * 64, adv(dX, k * 32), adv(b0, k * 2048), idesc_n64, k > 0);
-          mma_commit(&d_ready[pt]);
-        }
-        mma_commit(&x_empty[s]);
+      for (int h = 0; h < 2; ++h) {
+        gemm_x_w0(acc, sbase + kOffX + s * 8192, sbase, h);
+        if (h == 1 && lane == 0) mbar_arrive(&x_empty[s]);  // both halves of layer 0 have read the stage
+        epi_bias_relu(acc, s_b0, h, a1, lane);
       }
-      __syncwarp();
-#pragma unroll 1
-      for (int j = 0; j < 4; ++j) {  // layer 1: D1 = A1 (TMEM) * W1, K = 256, trailing E0
-        mbar_wait(&chunk_done[j], 0, 34);
-        tc_fence_after();
-        if (elect_one()) {
-#pragma unroll 1
-          for (int pt = 0; pt <= j; ++pt) {
-#pragma unroll 1
-            for (int g = (pt == j ? 0 : j); g <= j; ++g) {  // K steps 4g .. 4g+3
-              const uint64_t b0 = adv(dW1, pt * 32768 + g * 8192);
-              const uint32_t a0 = tmem_a1 + g * 32;
 #pragma unroll
-              for (int kk = 0; kk < 4; ++kk) mma_ts(tmem_d + pt * 64, a0 + kk * 8, adv(b0, kk * 2048), idesc_n64, (g | kk) != 0);
-            }
-            if (j == 3) mma_commit(&d_ready[pt]);
-          }
-        }
-        __syncwarp();
+      for (int h = 0; h < 2; ++h) {
+        gemm_a_w1(acc, a1, sbase, h);
+        epi_bias_relu(acc, s_b1, h, a2, lane);
       }
-#pragma unroll 1
-      for (int j = 0; j < 4; ++j) {  // head: D2 = A2 (TMEM) * W2 (un-swizzled core matrices), N = 16, trailing E1
-        mbar_wait(&chunk_done[j], 1, 35);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t b0 = adv(dW2, j * 2048);
+      float zr[8];
+      wg_zero(zr);
+      gemm_a_w2(zr, a2, sbase);
+      // the 16 logits of row (q4 = 0) / row + 8 (q4 = 1), gathered from the 4 lanes of the quad
+      float z[16];
 #pragma unroll
-          for (int kk = 0; kk < 4; ++kk) mma_ts(tmem_d, tmem_a2 + j * 32 + kk * 8, adv(b0, kk * 512), idesc_n16, (j | kk) != 0);
-          if (j == 3) mma_commit(head_ready);
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-    // ===================== epilogue warps =====================
-    // step cc of a layer epilogue: chunk 2cc (half-0 warps) and 2cc+1 (half-1 warps) = the 64-column part cc
-    const int q = warp & 3, half = (warp - kEpiWarp0) >> 2;
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const uint32_t tmem_d = tmem + lane_addr, tmem_a1 = tmem + lane_addr + 256, tmem_a2 = tmem + lane_addr + 384;
-    const int64_t e = tile_row0 + q * 32 + lane;
-    const uint64_t call0 = p.cat_offset + (p.cat_counter ? *p.cat_counter : 0ull);
-    const uint2 ckey = make_uint2((uint32_t)p.cat_seed, (uint32_t)(p.cat_seed >> 32));
-    for (int t = 0; t < p.T; ++t) {
-#pragma unroll 1
-      for (int layer = 0; layer < 2; ++layer) {
-        const float* bias = layer == 0 ? s_b0 : s_b1;
-        const uint32_t ta = layer == 0 ? tmem_a1 : tmem_a2;
-#pragma unroll 1
-        for (int cc = 0; cc < 4; ++cc) {
-          const int c = cc * 2 + half;
-          mbar_wait(&d_ready[cc], layer, 36 + layer);  // layer 0 / 1 are the 1st / 2nd completion of d_ready per step
-          tc_fence_after();
-          uint32_t r[32], pk[16];
-          tmem_ld32(tmem_d + c * 32, r);
-          tmem_ld_wait();
+      for (int src = 0; src < 4; ++src) {
+        const int sl = (lane & ~3) | src;
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            pk[j] = bias_relu_pack_bf16(r[2 * j], r[2 * j + 1], *reinterpret_cast<const float2*>(bias + c * 32 + 2 * j));
-          }
-          tmem_st16(ta + c * 16, pk);
-          tmem_st_wait();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&chunk_done[cc]);
+        for (int i = 0; i < 8; ++i) {  // zr[i]: row + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 src + (i & 1)
+          const float v = __shfl_sync(0xffffffffu, zr[i], sl);
+          if (((i >> 1) & 1) == (q4 & 1)) z[8 * (i >> 2) + 2 * src + (i & 1)] = v;
         }
       }
-      if (half == 0) {
-        mbar_wait(head_ready, t & 1, 38);
-        tc_fence_after();
-        uint32_t r[16];
-        tmem_ld16(tmem_d, r);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(head_done);  // the logits are in registers: layer 0 of the next step may overwrite D
+      if (q4 < 2) {
         const int A = p.A;
-        float z[16], zmax = -INFINITY;
+        float zmax = -INFINITY;
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
-          z[j] = __uint_as_float(r[j]) + s_b2[j];
+          z[j] += s_b2[j];
           if (j < A) zmax = fmaxf(zmax, z[j]);
         }
         float se = 0.f;
@@ -371,12 +263,6 @@ __global__ void __launch_bounds__(kThreads, 1)
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    tc_fence_after();
-    tmem_dealloc(tmem, 512);
-  }
 }
 
 }  // namespace ro
@@ -398,7 +284,7 @@ extern "C" int stx_tc_rollout_synth(const StxMlp* actor, void* obs, void* next_o
                   actor->sizes[0] % 8 == 0 && actor->sizes[3] >= 1 && actor->sizes[3] <= 16 && actor->activation == STX_ACT_RELU &&
                   !actor->use_layer_norm,
               STX_E_SHAPE, "stx_tc_rollout_synth: actor must be MLP [D<=64 (mult of 8), 256, 256, A<=16]");
-  STX_REQUIRE(E > 0 && E % 128 == 0 && T > 0, STX_E_SHAPE, "stx_tc_rollout_synth: num_envs (%lld) must be a multiple of 128", (long long)E);
+  STX_REQUIRE(E > 0 && E % 64 == 0 && T > 0, STX_E_SHAPE, "stx_tc_rollout_synth: num_envs (%lld) must be a multiple of 64", (long long)E);
   STX_REQUIRE(actor->params_bf16 != nullptr, STX_E_ARG, "stx_tc_rollout_synth needs the bf16 shadow arena");
   const int D = actor->sizes[0], A = actor->sizes[3];
   const __nv_bfloat16* w = reinterpret_cast<const __nv_bfloat16*>(actor->params_bf16);
@@ -420,7 +306,7 @@ extern "C" int stx_tc_rollout_synth(const StxMlp* actor, void* obs, void* next_o
     STX_CUDA_OK(cudaFuncSetAttribute(ro::tc_rollout_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ro::kSmemBytes));
     attr_set = true;
   }
-  ro::tc_rollout_kernel<<<(unsigned)(E / 128), ro::kThreads, ro::kSmemBytes, (cudaStream_t)stream>>>(tmW0, tmW1, p);
+  ro::tc_rollout_kernel<<<(unsigned)(E / ro::kTileM), ro::kThreads, ro::kSmemBytes, (cudaStream_t)stream>>>(tmW0, tmW1, p);
   STX_LAUNCH_OK();
   return STX_OK;
 }

@@ -56,7 +56,7 @@ def _seed_to_int(seed) -> int:
 class CategoricalHead:
     def __init__(self, action_dim: Union[int, Sequence[int]], kernel_init: Optional[float] = None):
         if not isinstance(action_dim, (int, np.integer)):
-            raise NotImplementedError("factorised action_dim is outside the B200 hot path")
+            raise NotImplementedError("factorised action_dim is outside the hot path of this build")
         self.action_dim = int(action_dim)
         self.out_dim = self.action_dim
         self.kernel_init_scale = 0.01 if kernel_init is None else float(kernel_init)  # heads.py:32

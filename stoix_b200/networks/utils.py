@@ -1,6 +1,6 @@
 """Activation lookup (stoix/networks/utils.py:7-25).  A torso here is a description, so the parser returns the NAME; the
 fp32 CUDA path implements relu, tanh, silu / swish, elu, gelu (flax default: tanh approximation), sigmoid, softplus and
-identity / none (csrc/stx_simt_gemm.cuh); the bf16 tcgen05 kernels implement relu.  The remaining names of the reference's
+identity / none (csrc/stx_simt_gemm.cuh); the bf16 tensor-core (wgmma) kernels implement relu.  The remaining names of the reference's
 table are not elementwise torso activations (normalise, softmax, log_softmax) or unused (log_sigmoid) and raise."""
 
 _SUPPORTED = {"relu", "tanh", "silu", "swish", "elu", "gelu", "sigmoid", "softplus", "identity", "none"}

@@ -206,7 +206,7 @@ def mlp_forward(spec: MlpSpec, params: torch.Tensor, x: torch.Tensor, row_idx: O
     return out
 
 
-NUM_SMS = 148
+NUM_SMS = 132  # H100 SXM
 
 
 def set_forward_cta_budget(n: int) -> None:
@@ -460,9 +460,8 @@ class PeerGradBuffers:
         self.gsum2.zero_()
         self.gsum2_handle = symm_mem.rendezvous(self.gsum2, group)
         self.gsum2_ptrs = (C.c_void_p * self.world)(*[int(p) for p in self.gsum2_handle.buffer_ptrs])
-        # 1 = one-shot (default), 2 = two-shot.  Measured at N=2 (profiles/r02_allreduce_modes.txt): one-shot 6.48 ms / update
-        # phase, two-shot 7.04 ms -- its second cross-GPU hand-shake (fence.sys after the peer stores, last-block norm, signal
-        # flight) costs more than the (W-1) extra arenas of 0.67 MB it saves.
+        # 1 = one-shot (default), 2 = two-shot: the second cross-GPU hand-shake of two-shot (fence.sys after the peer stores,
+        # last-block norm, signal flight) can cost more than the (W-1) extra arenas of 0.67 MB it saves.
         self.mode = int(os.environ.get("STX_ALLREDUCE_MODE", "1"))
         if self.total % 4 != 0:
             self.mode = 1

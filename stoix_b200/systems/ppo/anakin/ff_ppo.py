@@ -1,10 +1,10 @@
-"""Anakin feed-forward PPO on B200 -- drop-in for stoix/systems/ppo/anakin/ff_ppo.py.
+"""Anakin feed-forward PPO on H100 -- drop-in for stoix/systems/ppo/anakin/ff_ppo.py.
 
 Same entry points and signatures (get_learner_fn :49-54, learner_setup :424-426, run_experiment :554,
 hydra_entry_point :709-727) and the same state / output contracts (stoix_b200/base_types.py), but a
 different machine underneath:
 
-  reference (JAX)                                 here (B200)
+  reference (JAX)                                 here (H100)
   ----------------------------------------------  -------------------------------------------------
   pmap over devices                               one process per GPU (torchrun), rank = device index
   lax.scan over T env steps, 3 MLP applies/step   T x (actor MLP kernel + sample kernel + env kernel);
@@ -230,7 +230,7 @@ def get_learner_fn(
                  and getattr(env, "fused_rollout_supported", False) and b["rs"] is None)
         # The two critic evaluations of _env_step (value = critic(obs_t), bootstrap_value = critic(next_obs_t), ff_ppo.py:99,
         # 113-116) depend only on the observations, so they are batched over (steps x envs) rows.  With the fused rollout
-        # (E/128 of the 148 SMs busy) the scan is cut into chunks and the critic of chunk c runs on a second stream on the
+        # (E/64 of the 132 SMs busy: one CTA per 64 envs) the scan is cut into chunks and the critic of chunk c runs on a second stream on the
         # idle SMs while the rollout kernel produces chunk c+1; only the last chunk's critic is left after the scan.
         chunks = max(int(arch.get("rollout_chunks", 8)), 1) if fused else 1
         while T % chunks != 0:  # largest divisor of T not above the request
@@ -257,7 +257,7 @@ def get_learner_fn(
                         with torch.cuda.stream(side):
                             # leave the rollout's SMs alone: a persistent forward CTA that has to wait for one of them
                             # would hold its share of the tiles back until the rollout chunk ends
-                            ops.set_forward_cta_budget(ops.NUM_SMS - E // 128 if c + 1 < chunks else 0)
+                            ops.set_forward_cta_budget(ops.NUM_SMS - E // 64 if c + 1 < chunks else 0)
                             critic_rows(sh, c * Tc, (c + 1) * Tc)
                             ops.set_forward_cta_budget(0)
                 if side is not None:
@@ -296,7 +296,7 @@ def get_learner_fn(
     def _shuffle_phase(state: OnPolicyLearnerState) -> None:
         """SHUFFLE MINIBATCHES (ff_ppo.py:294-307) for ALL epochs of this update: one keyed permutation of the flat index per
         (shard, epoch).  They depend on the key and the device-resident stream counter only, not on the rollout, so the
-        update step issues them on a side stream underneath the rollout (which occupies E/128 of the 148 SMs)."""
+        update step issues them on a side stream underneath the rollout (which occupies E/64 of the 132 SMs)."""
         b = built
         for u in range(U):
             sh = b["shards"][u]

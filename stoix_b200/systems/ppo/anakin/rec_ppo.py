@@ -1,4 +1,4 @@
-"""Anakin recurrent PPO on B200 -- drop-in for stoix/systems/ppo/anakin/rec_ppo.py (SURVEY.md 8f row 3), fp32.
+"""Anakin recurrent PPO on H100 -- drop-in for stoix/systems/ppo/anakin/rec_ppo.py (SURVEY.md 8f row 3), fp32.
 
 Same entry points (get_learner_fn :38, learner_setup :431, run_experiment :593, hydra_entry_point) and state contracts
 (RNNLearnerState, RNNPPOTransition, ActorCriticHiddenStates).  Behaviour restated from the reference, including its details:
@@ -6,7 +6,7 @@ the hidden state is reset where the PREVIOUS transition ended (done | truncated)
 its step and the losses re-run the networks from `hstates[0]` of the chunk; GAE goes through the `values=` interface with
 discount_t = (1 - last_done_t) * gamma; minibatches are column subsets of the batch reshaped to (chunk, num_envs * num_chunks).
 
-  reference (JAX)                                   here (B200)
+  reference (JAX)                                   here (H100)
   ------------------------------------------------  -----------------------------------------------------------------------
   nn.scan of GRUCell over T inside jax.grad         pre-torso + input projections of ALL steps as one MLP launch chain,
                                                     stx_gru_sequence_forward / _backward for the recurrence (BPTT with the saved

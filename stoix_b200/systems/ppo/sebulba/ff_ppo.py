@@ -1,11 +1,11 @@
-"""Sebulba feed-forward PPO on B200 -- drop-in for stoix/systems/ppo/sebulba/ff_ppo.py (MLP torso).
+"""Sebulba feed-forward PPO on H100 -- drop-in for stoix/systems/ppo/sebulba/ff_ppo.py (MLP torso).
 
 Same entry points (get_act_fn :123, get_rollout_fn :145, get_actor_thread :336, get_learner_step_fn :378,
 get_learner_rollout_fn :568, get_learner_thread :661, learner_setup :703, run_experiment :801, hydra_entry_point :1026)
 and the same thread topology: N actor threads per actor GPU stepping CPU environments, one learner thread, one evaluator
 thread, joined by ParameterServer / OnPolicyPipeline queues (stoix_b200/utils/sebulba_utils.py).
 
-  reference (JAX)                                     here (B200)
+  reference (JAX)                                     here (H100)
   --------------------------------------------------  -------------------------------------------------------------
   act_fn = jit(actor+critic apply, sample) per step    batched INFERENCE SERVER per actor thread: the thread's env batch
   obs -> device by an implicit transfer, action back   goes pinned-host -> cudaMemcpyAsync on the thread's own stream ->

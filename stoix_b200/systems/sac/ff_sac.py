@@ -1,9 +1,9 @@
-"""Anakin feed-forward SAC on B200 -- drop-in for stoix/systems/sac/ff_sac.py (SURVEY.md 8f row 4, fp32).
+"""Anakin feed-forward SAC on H100 -- drop-in for stoix/systems/sac/ff_sac.py (SURVEY.md 8f row 4, fp32).
 
 Same entry points and signatures (get_warmup_fn :40-92, get_learner_fn :95-344, learner_setup :347-513, run_experiment :516,
 hydra_entry_point) and the same state / output contracts (sac_types.py), on a different machine:
 
-  reference (JAX)                                      here (B200)
+  reference (JAX)                                      here (H100)
   ---------------------------------------------------  ------------------------------------------------------------------
   flashbax item buffer (add / sample, host-traced)      device ring buffer, write position in HBM (stx_replay_add / _sample):
                                                         ONE launch lays the sampled batch out as the three network inputs

@@ -39,4 +39,4 @@ def make(config) -> Tuple[Environment, Environment]:
         from ..envs.cartpole import CartPoleEnv
 
         return CartPoleEnv(device=device, seed=seed + 7919 * rank), CartPoleEnv(device=device, seed=seed + 1 + 7919 * rank)
-    raise NotImplementedError(f"environment suite '{name}' is outside the B200 hot path build")
+    raise NotImplementedError(f"environment suite '{name}' is outside the hot path of this build")

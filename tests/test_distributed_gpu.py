@@ -5,7 +5,7 @@ gradient arena per minibatch step) on the GPU, checked against the ORACLE:
   (`stx_allreduce2_clip_adam_step`, the default) and one-shot (`stx_allreduce_clip_adam_step`), driven through the C ABI with
   W = 2 / 4 / 8 "virtual ranks" whose gradient arenas and signal pads are plain buffers of the same device; every virtual rank's parameters / moments must equal
   `oracle.clip_adam_step(mean of the W gradients)` and be bit-identical to each other.
-* `test_two_rank_update_matches_oracle` (needs >= 2 GPUs; `gpurun --gpus 2`): two torchrun ranks run three whole update
+* `test_two_rank_update_matches_oracle` (needs >= 2 GPUs): two torchrun ranks run three whole update
   steps (eager, graph capture, graph replay); each rank replays its own trajectory through `oracle.ppo_update` with the
   gradient exchange as `grad_sync` (a gloo all-reduce between the two oracle instances: SUM, then 1/world) and compares its
   post-update optimiser state and parameters with the oracle's, for the fused NVLink all-reduce and for NCCL.
@@ -104,7 +104,7 @@ for upd in range(n_upd):   # eager, graph capture, graph replay
     pu = per_update[-1]
     mu_err, nu_err, p_err = max(pu["mu_a"], pu["mu_c"]), max(pu["nu_a"], pu["nu_c"]), max(pu["p_a"], pu["p_c"])
     # Every update is checked on its own: afterwards the oracle continues from the kernels' parameters and moments.  Bounds:
-    #  bf16 (tcgen05 path vs the bf16-rounding oracle): the end-state bounds of the single-device whole-update test
+    #  bf16 (tensor-core path vs the bf16-rounding oracle): the end-state bounds of the single-device whole-update test
     #       (tests/test_tc_gpu.py: mu 0.3, nu 0.1, params 0.15 -- trajectory drift under Adam normalisation; the strict check
     #       of that path is the per-step teacher-forced gradient test there, 5e-3);
     #  f32  (CUDA-core path vs the fp64 oracle): per-step gradients agree to 3e-7 (scripts/diag_bf16_steps.py ... f32), but over

@@ -1,4 +1,4 @@
-"""bf16 tensor-core path (tcgen05): fused MLP forward vs the oracle with bf16-rounded GEMM operands
+"""bf16 tensor-core path (wgmma): fused MLP forward vs the oracle with bf16-rounded GEMM operands
 (weights, inputs and hidden activations rounded to bf16, fp32 accumulate -- oracle.mlp_forward(
 bf16_operands=True)).  Tolerance: the only differences left are fp32 accumulation order and rare
 1-ulp bf16 rounding flips of a hidden activation: rtol 2e-3 / atol 2e-3 on outputs; vs the pure fp32
@@ -156,7 +156,7 @@ def test_tc_ppo_minibatch_grads_vs_bf16_oracle(B, mb_off, mb, D, A, use_perm):
     (4096, 128, 16),   # BASELINE config 2: the exact update step bench.py times (mb = 32 768, 64 optimiser steps)
 ])
 def test_learner_bf16_update_tracks_bf16_oracle(E, T, nmb):
-    """One whole Anakin update step with arch.precision=bf16 (tcgen05 rollout, batched critic, K3 on tensor
+    """One whole Anakin update step with arch.precision=bf16 (tensor-core rollout, batched critic, K3 on tensor
     cores, bf16 weight shadows refreshed by the fused Adam) vs the oracle run with the same bf16 operand
     rounding, actions and permutations injected.
 

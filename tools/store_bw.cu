@@ -58,22 +58,22 @@ int main() {
   long long* out;
   uint8_t* gbuf;
   const size_t big = (size_t)4 << 20;  // 4 MB per CTA -> 592 MB total
-  cudaMalloc(&out, 148 * 8);
-  cudaMalloc(&gbuf, 148 * big);
+  cudaMalloc(&out, 132 * 8);
+  cudaMalloc(&gbuf, 132 * big);
   cudaFuncSetAttribute(k<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 32768);
   const int iters = 4000;
-  for (int grid : {148, 74, 32, 8})
+  for (int grid : {132, 66, 32, 8})
   for (size_t cta_bytes : {(size_t)65536, big})
     for (int mode = 0; mode < 2; ++mode)
       for (int warps : {8}) {
-        if (grid != 148 && mode == 1) continue;
+        if (grid != 132 && mode == 1) continue;
         for (int rep = 0; rep < 2; ++rep) {
           if (mode == 0) k<0><<<grid, warps * 32>>>(iters, cta_bytes, gbuf, out);
           if (mode == 1) k<1><<<grid, warps * 32, 32768>>>(iters, cta_bytes, gbuf, out);
           cudaError_t e = cudaDeviceSynchronize();
           if (e != cudaSuccess) { printf("error %s\n", cudaGetErrorString(e)); return 1; }
         }
-        long long h[148];
+        long long h[132];
         cudaMemcpy(h, out, sizeof(h), cudaMemcpyDeviceToHost);
         long long mx = 0;
         for (int i = 0; i < grid; ++i) mx = h[i] > mx ? h[i] : mx;
