@@ -320,6 +320,21 @@ def test_learner_bf16_per_step_gradients_match_oracle(E, T, nmb, check_steps):
 def test_fused_rollout_is_bit_identical_to_per_step_path():
     """stx_tc_rollout_synth (one persistent launch for the T-step scan) must reproduce the per-step path
     (forward kernel + stx_categorical + stx_synth_env_step per step) exactly: same Philox streams, same GEMMs."""
+    _fused_vs_per_step_rollout(256, 12, 64, 8, 2)
+
+
+@pytest.mark.parametrize("E,T,D,A,nmb", [
+    (128, 13, 8, 16, 1),    # T prime: the rollout runs in one chunk; D = 8 and a 16-column head
+    (8704, 4, 24, 9, 2),    # 136 rollout CTAs (> 132 SMs); the critic's forward CTA budget 132 - 136 is negative
+])
+def test_fused_rollout_is_bit_identical_at_edge_shapes(E, T, D, A, nmb):
+    """The same comparison at shapes where the rollout's chunking, tile count or head width differ from the default."""
+    _fused_vs_per_step_rollout(E, T, D, A, nmb)
+
+
+def _fused_vs_per_step_rollout(E, T, D, A, nmb):
+    """Two update steps with the fused rollout and two with the per-step path: every trajectory field and the updated
+    actor arena must be bit-identical."""
     from stoix_b200 import random as srandom
     from stoix_b200.config import compose
     from stoix_b200.systems.ppo.anakin import ff_ppo
@@ -327,11 +342,11 @@ def test_fused_rollout_is_bit_identical_to_per_step_path():
     from stoix_b200.utils.total_timestep_checker import check_total_timesteps
 
     def run(fused):
-        E, T = 256, 12
         cfg = compose("default_ff_ppo", ["env=synthetic/box", f"arch.total_num_envs={E}", f"system.rollout_length={T}",
-                                         "system.num_minibatches=2", f"arch.total_timesteps={E * T * 2}", "arch.num_evaluation=1",
+                                         f"system.num_minibatches={nmb}", f"arch.total_timesteps={E * T * 2}", "arch.num_evaluation=1",
                                          "arch.precision=bf16", f"arch.fused_rollout={fused}", "logger.use_console=False",
-                                         "env.kwargs.p_term=0.05", "env.kwargs.p_trunc=0.05"])
+                                         "env.kwargs.p_term=0.05", "env.kwargs.p_trunc=0.05", f"env.kwargs.obs_dim={D}",
+                                         f"env.kwargs.num_actions={A}"])
         cfg.num_devices, cfg.rank = 1, 0
         cfg = check_total_timesteps(cfg, quiet=True)
         env, _ = make_env.make(cfg)
