@@ -444,6 +444,53 @@ int stx_ppo_head_grads(const float* logits, const float* value, const int32_t* i
                        const float* v_old, const float* adv, const float* targets, const float* adv_stats, int64_t mb, int A, float clip_eps,
                        float ent_coef, float vf_coef, float* d_logits, float* d_value, float* metrics, float weight, void* scratch, void* stream);
 
+/* ------------------------------------------------------------------ continuous-action PPO (fp32) ---------------
+ * The tanh-Normal head (NormalAffineTanhDistributionHead, heads.py:44-65; head_out[M][2A] = loc | scale pre-activation,
+ * sigma = softplus(raw) + min_scale) under the PPO losses of stoix/systems/ppo/anakin/ff_ppo_continuous.py.
+ * stx_tanh_normal_log_prob: log_prob of GIVEN actions (row stride ld_action) by the inverse path of
+ *   AffineTanhTransformedDistribution.log_prob (distributions.py:56-80): the event is clipped to [min + 1e-3, max - 1e-3],
+ *   the tails score log Phi((u_lo - loc)/sigma) - log 1e-3 and log Phi(-(u_hi - loc)/sigma) - log 1e-3, the band the Normal
+ *   density of atanh((a - shift)/s) plus the inverse log-det of tanh and the scale; summed over the A dims.  The gradient
+ *   entries below score the stored actions with the same device function.
+ * Entropy: the reference's one-sample estimate entropy(seed) (distributions.py:85-88) per row,
+ *   H = sum_j [1/2 + log sqrt(2 pi) + log sigma_j + log s + fldj(loc_j + sigma_j eps'_j)], fldj(x) = 2 (log 2 - x - softplus(-2x)),
+ *   with eps' held fixed under the gradient.  eps' of minibatch row m, dims 4g..4g+3: Philox4x32-10 with
+ *     key     = (seed & 0xffffffff, seed >> 32)
+ *     counter = (m & 0xffffffff, call & 0xffffffff, (call >> 32) ^ (g << 20) ^ ((m >> 32) << 8), 0x50504f45)
+ *   call = offset + *dev_counter (dev_counter nullable); words (x, y) -> dims 4g, 4g+1 and (z, w) -> 4g+2, 4g+3 through
+ *   Box-Muller (r = sqrt(-2 log u01(x)), (r cos 2 pi u01(y), r sin 2 pi u01(y))), u01 as for the other Philox draws.
+ *   eps_in (nullable, (mb, A)) replaces the draw; eps_out (nullable, (mb, A)) records the noise used.
+ * stx_ppo_tanh_normal_head_grads: the actor half of _update_minibatch (ff_ppo_continuous.py:191-213) on head outputs already
+ *   computed: row m of head_out pairs with batch row idx[m] (or row0 + m) of action / logp_old / adv (standardised on load when
+ *   adv_stats is given).  Writes d(ppo_clip_loss - ent_coef * mean H)/d(head_out) and accumulates metrics[0] actor_loss,
+ *   metrics[1] entropy, metrics[3] mean advantage (with `weight`).  scratch: stx_ppo_head_scratch_bytes(mb), zeroed once.
+ * stx_ppo_continuous_minibatch_grads: stx_ppo_minibatch_grads for the tanh-Normal actor: actor forward, the kernel above and
+ *   the actor backward, then the critic half the discrete fp32 path runs.  STX_PREC_F32 only; A <= 32; scalar critic; the
+ *   batch's int32 `action` is unused (the head's float actions replace it).  Workspace: stx_ppo_workspace_bytes(F32). */
+typedef struct StxTanhNormalPpo {
+  const float* action;          /* (B, A) stored actions, traj_batch.action */
+  const float* eps_in;          /* (mb, A) injected entropy noise, or NULL: Philox */
+  float* eps_out;               /* (mb, A) noise used, or NULL */
+  const uint64_t* dev_counter;  /* device RNG stream position added to `offset`, or NULL */
+  uint64_t seed;
+  uint64_t offset;
+  float minimum, maximum;       /* action bounds of the head */
+  float min_scale;
+  int32_t reserved;
+} StxTanhNormalPpo;
+int stx_tanh_normal_log_prob(const float* head_out, int64_t M, int A, const float* action, int64_t ld_action, float minimum, float maximum,
+                             float min_scale, float* log_prob, void* stream);
+/* stx_tanh_normal_entropy: the per-row estimate H above for head_out rows 0..M-1 (row r draws as minibatch row r). */
+int stx_tanh_normal_entropy(const float* head_out, int64_t M, int A, const float* eps_in, uint64_t seed, uint64_t offset,
+                            const uint64_t* dev_counter, float minimum, float maximum, float min_scale, float* entropy, float* eps_out,
+                            void* stream);
+int stx_ppo_tanh_normal_head_grads(const float* head_out, const int32_t* idx, int64_t row0, const StxTanhNormalPpo* head, const float* logp_old,
+                                   const float* adv, const float* adv_stats, int64_t mb, int A, float clip_eps, float ent_coef, float* d_head_out,
+                                   float* metrics, float weight, void* scratch, void* stream);
+int stx_ppo_continuous_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxPpoBatch* batch, const StxTanhNormalPpo* head,
+                                       int64_t mb_off, int64_t mb, const StxPpoHyper* hyper, float grad_weight, float* grad_arena, float* metrics,
+                                       int precision, void* workspace, size_t workspace_bytes, void* stream);
+
 /* Utility casts used by the bf16 path (obs / weight shadows). */
 int stx_cast_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream);
 

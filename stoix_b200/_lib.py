@@ -109,6 +109,21 @@ class StxPpoBatch(C.Structure):
     ]
 
 
+class StxTanhNormalPpo(C.Structure):
+    _fields_ = [
+        ("action", C.c_void_p),
+        ("eps_in", C.c_void_p),
+        ("eps_out", C.c_void_p),
+        ("dev_counter", C.c_void_p),
+        ("seed", C.c_uint64),
+        ("offset", C.c_uint64),
+        ("minimum", C.c_float),
+        ("maximum", C.c_float),
+        ("min_scale", C.c_float),
+        ("reserved", C.c_int32),
+    ]
+
+
 _P = C.c_void_p
 _SIGNATURES = {
     # name: (restype, argtypes)
@@ -174,6 +189,12 @@ _SIGNATURES = {
     "stx_running_stats_accumulate": (C.c_int, [_P, _P, C.c_int64, C.c_int, _P, _P, _P, _P]),
     "stx_running_stats_finalize": (C.c_int, [_P, C.c_int, _P, _P, _P, _P, C.c_float, C.c_float, _P]),
     "stx_obs_normalize": (C.c_int, [_P, C.c_int64, C.c_int, _P, _P, C.c_float, _P, C.c_int, _P]),
+    "stx_tanh_normal_log_prob": (C.c_int, [_P, C.c_int64, C.c_int, _P, C.c_int64, C.c_float, C.c_float, C.c_float, _P, _P]),
+    "stx_tanh_normal_entropy": (C.c_int, [_P, C.c_int64, C.c_int, _P, C.c_uint64, C.c_uint64, _P, C.c_float, C.c_float, C.c_float, _P, _P, _P]),
+    "stx_ppo_tanh_normal_head_grads": (C.c_int, [_P, _P, C.c_int64, C.POINTER(StxTanhNormalPpo), _P, _P, _P, C.c_int64, C.c_int, C.c_float,
+                                                 C.c_float, _P, _P, C.c_float, _P, _P]),
+    "stx_ppo_continuous_minibatch_grads": (C.c_int, [C.POINTER(StxMlp), C.POINTER(StxMlp), C.POINTER(StxPpoBatch), C.POINTER(StxTanhNormalPpo),
+                                                     C.c_int64, C.c_int64, C.POINTER(StxPpoHyper), C.c_float, _P, _P, C.c_int, _P, C.c_size_t, _P]),
 }
 
 _lib = None

@@ -1,6 +1,7 @@
 // K1 (fp32 path) MLP forward, categorical head ops, and K3 (fp32 path) PPO minibatch gradients.
 // The bf16 wgmma implementations live in stx_tc_mlp.cu and are dispatched from here by precision.
 #include "stx_common.cuh"
+#include "stx_ppo_halves.cuh"
 #include "stx_ppo_loss.cuh"
 #include "stx_simt_gemm.cuh"
 
@@ -270,6 +271,44 @@ int simt_backward(const StxMlp* m, const float* x, int64_t ldx, const int32_t* r
 }
 
 }  // namespace
+
+// ---- halves of the fp32 PPO minibatch shared with other policy heads (stx_ppo_continuous.cu) ----
+// Both carve `workspace` exactly as stx_ppo_minibatch_grads does, so one stx_ppo_workspace_bytes() workspace serves either net.
+int simt_check_mlp(const StxMlp* m, const char* who) { return check_mlp(m, who); }
+
+int simt_net_forward(const StxMlp* m, const float* x, int64_t ldx, const int32_t* idx, int64_t mb, void* workspace, SimtHeadBufs* out,
+                     cudaStream_t st) {
+  SimtPpoWs ws = carve(m, mb, reinterpret_cast<char*>(workspace));
+  out->head = ws.head, out->dhead = ws.dhead, out->loss_partials = ws.loss_partials, out->counter = ws.counter;
+  return simt_forward(m, x, ldx, idx, mb, ws.acts, ws.hacts, ws.stats, ws.head, st);
+}
+
+int simt_net_backward(const StxMlp* m, const float* x, int64_t ldx, const int32_t* idx, int64_t mb, void* workspace, float grad_weight,
+                      float* net_grad, int overwrite, cudaStream_t st) {
+  SimtPpoWs ws = carve(m, mb, reinterpret_cast<char*>(workspace));
+  return simt_backward(m, x, ldx, idx, mb, ws, grad_weight, net_grad, overwrite, st);
+}
+
+// Critic half of _update_minibatch (ff_ppo.py:215-235, 244-247): forward, clipped value loss, backward into grad_arena + coff.
+int simt_ppo_critic_grads(const StxMlp* critic, const StxPpoBatch* b, int64_t mb_off, int64_t mb, const StxPpoHyper* h, float grad_weight,
+                          float* net_grad, float* metrics, void* workspace, cudaStream_t st) {
+  const int D = critic->sizes[0];
+  const float* obs = reinterpret_cast<const float*>(b->obs);
+  const int32_t* idx = b->perm ? b->perm + mb_off : nullptr;
+  const float* x = idx ? obs : obs + mb_off * (int64_t)D;  // without a permutation: the contiguous row range from mb_off
+  SimtPpoWs ws = carve(critic, mb, reinterpret_cast<char*>(workspace));
+  if (int rc = simt_forward(critic, x, D, idx, mb, ws.acts, ws.hacts, ws.stats, ws.head, st)) return rc;
+  LossArgs g{};
+  g.logits = nullptr, g.value = ws.head, g.value_ld = 1, g.idx = idx, g.row0 = mb_off;
+  g.action = b->action, g.logp_old = b->log_prob, g.v_old = b->value, g.adv = b->advantages, g.tgt = b->targets;
+  g.adv_stats = h->standardize_advantages ? b->adv_stats : nullptr, g.dlogits = nullptr, g.dvalue = ws.dhead, g.mb = mb, g.A = 0;
+  g.clip_eps = h->clip_eps, g.ent_coef = h->ent_coef, g.vf_coef = h->vf_coef;
+  g.partials = ws.loss_partials, g.counter = ws.counter, g.metrics = metrics, g.weight = grad_weight;
+  ppo_loss_grad_kernel<<<(unsigned)((mb + 255) / 256), 256, 0, st>>>(g);
+  STX_LAUNCH_OK();
+  return simt_backward(critic, x, D, idx, mb, ws, grad_weight, net_grad, h->overwrite_grads, st);
+}
+
 }  // namespace stx
 
 using namespace stx;
@@ -469,18 +508,5 @@ extern "C" int stx_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic
     if (int rc = simt_backward(actor, x, D, idx, mb, ws, grad_weight, grad_arena + aoff, h->overwrite_grads, st)) return rc;
   }
   // ---- critic: forward, loss, backward (ff_ppo.py:215-235, 244-247) ----
-  {
-    SimtPpoWs ws = carve(critic, mb, reinterpret_cast<char*>(workspace));
-    if (int rc = simt_forward(critic, x, D, idx, mb, ws.acts, ws.hacts, ws.stats, ws.head, st)) return rc;
-    LossArgs g{};
-    g.logits = nullptr, g.value = ws.head, g.value_ld = 1, g.idx = idx, g.row0 = mb_off;
-    g.action = b->action, g.logp_old = b->log_prob, g.v_old = b->value, g.adv = b->advantages, g.tgt = b->targets;
-    g.adv_stats = stats, g.dlogits = nullptr, g.dvalue = ws.dhead, g.mb = mb, g.A = 0;
-    g.clip_eps = h->clip_eps, g.ent_coef = h->ent_coef, g.vf_coef = h->vf_coef;
-    g.partials = ws.loss_partials, g.counter = ws.counter, g.metrics = metrics, g.weight = grad_weight;
-    ppo_loss_grad_kernel<<<(unsigned)((mb + 255) / 256), 256, 0, st>>>(g);
-    STX_LAUNCH_OK();
-    if (int rc = simt_backward(critic, x, D, idx, mb, ws, grad_weight, grad_arena + coff, h->overwrite_grads, st)) return rc;
-  }
-  return STX_OK;
+  return simt_ppo_critic_grads(critic, b, mb_off, mb, h, grad_weight, grad_arena + coff, metrics, workspace, st);
 }

@@ -9,35 +9,12 @@
 // 2 (log 2 - x - softplus(-2x)).  The networks themselves (silu MLPs, LayerNorm twin-Q) run on the generic train-mode MLP
 // entry points of stx_mlp.cu; everything here is elementwise / row-wise and HBM- or latency-bound.
 #include "stx_common.cuh"
+#include "stx_tanh_normal.cuh"
 
 namespace stx {
 namespace {
 
-constexpr float kLogSqrt2Pi = 0.9189385332046727f;
 constexpr uint32_t kTagSac = 0x53414331u;
-
-__device__ __forceinline__ float softplusf(float x) { return fmaxf(x, 0.f) + log1pf(expf(-fabsf(x))); }
-__device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
-// log Phi(z) = log(0.5 erfc(-z / sqrt 2)); erfcx keeps the far tail finite
-__device__ __forceinline__ float log_ndtrf(float z) {
-  const float t = -z * 0.70710678118654752f;
-  if (t < 3.f) return logf(0.5f * erfcf(t));
-  return logf(0.5f * erfcxf(t)) - t * t;
-}
-// phi(z) / Phi(z)
-__device__ __forceinline__ float mills(float z) { return expf(-0.5f * z * z - kLogSqrt2Pi - log_ndtrf(z)); }
-
-struct HeadGeom {
-  float s, sh, lo, hi, u_lo, u_hi, log_s, log_eps;
-};
-__device__ __forceinline__ HeadGeom head_geom(float minimum, float maximum, float epsilon) {
-  HeadGeom g;
-  g.s = 0.5f * (maximum - minimum), g.sh = 0.5f * (minimum + maximum);
-  g.lo = minimum + epsilon, g.hi = maximum - epsilon;
-  g.u_lo = atanhf((g.lo - g.sh) / g.s), g.u_hi = atanhf((g.hi - g.sh) / g.s);
-  g.log_s = logf(g.s), g.log_eps = logf(epsilon);
-  return g;
-}
 
 // One thread per row: action = shift + s tanh(loc + sigma eps) and log_prob (sum over the action dims).
 // eps_in == nullptr: eps ~ N(0,1) from Philox keyed by (seed; row, call = offset + *counter, dim pair); eps_out keeps it.

@@ -1,0 +1,65 @@
+// Device arithmetic of the tanh-Normal policy head (NormalAffineTanhDistributionHead, stoix/networks/heads.py:44-65, on
+// AffineTanhTransformedDistribution, stoix/networks/distributions.py:19-89), shared by the SAC kernels (stx_sac.cu) and the
+// continuous PPO kernels (stx_ppo_continuous.cu).  tfp pieces restated from their published definitions: Normal.log_prob,
+// log_cdf / log_survival_function, bijectors.Tanh.forward_log_det_jacobian(x) = 2 (log 2 - x - softplus(-2x)).
+#pragma once
+#include "stx_common.cuh"
+
+namespace stx {
+
+constexpr float kLogSqrt2Pi = 0.9189385332046727f;
+constexpr float kTanhNormalEpsilon = 1e-3f;  // the clip band of AffineTanhTransformedDistribution (distributions.py:28)
+
+__device__ __forceinline__ float softplusf(float x) { return fmaxf(x, 0.f) + log1pf(expf(-fabsf(x))); }
+__device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
+// log Phi(z) = log(0.5 erfc(-z / sqrt 2)); erfcx keeps the far tail finite
+__device__ __forceinline__ float log_ndtrf(float z) {
+  const float t = -z * 0.70710678118654752f;
+  if (t < 3.f) return logf(0.5f * erfcf(t));
+  return logf(0.5f * erfcxf(t)) - t * t;
+}
+// phi(z) / Phi(z)
+__device__ __forceinline__ float mills(float z) { return expf(-0.5f * z * z - kLogSqrt2Pi - log_ndtrf(z)); }
+// forward log-det-Jacobian of tanh at x
+__device__ __forceinline__ float tanh_fldj(float x) { return 2.f * (0.6931471805599453f - x - softplusf(-2.f * x)); }
+
+struct HeadGeom {
+  float s, sh, lo, hi, u_lo, u_hi, log_s, log_eps;
+};
+__device__ __forceinline__ HeadGeom head_geom(float minimum, float maximum, float epsilon) {
+  HeadGeom g;
+  g.s = 0.5f * (maximum - minimum), g.sh = 0.5f * (minimum + maximum);
+  g.lo = minimum + epsilon, g.hi = maximum - epsilon;
+  g.u_lo = atanhf((g.lo - g.sh) / g.s), g.u_hi = atanhf((g.hi - g.sh) / g.s);
+  g.log_s = logf(g.s), g.log_eps = logf(epsilon);
+  return g;
+}
+
+// One action dimension of log_prob(a) for a GIVEN event a (the inverse path, distributions.py:56-80) and its derivatives
+// with respect to loc and sigma (the event held fixed).  The event is clipped to [lo, hi]:
+//   a <= lo:  log Phi((u_lo - loc) / sigma) - log eps            d/dloc = -m / sigma, d/dsigma = -m z / sigma
+//   a >= hi:  log Phi(-(u_hi - loc) / sigma) - log eps           d/dloc =  m / sigma, d/dsigma = -m z / sigma
+//   else:     u = atanh((a - shift) / s), z = (u - loc) / sigma,
+//             -z^2/2 - log sigma - log sqrt(2 pi) - fldj(u) - log s    d/dloc = z / sigma, d/dsigma = (z^2 - 1) / sigma
+// with m = phi(z) / Phi(z) at the tail's own z.  Callers that only need the value let the compiler drop the rest.
+struct TanhNormalDim {
+  float lp, d_loc, d_sigma;
+};
+__device__ __forceinline__ TanhNormalDim tanh_normal_log_prob_given(float loc, float sigma, float a, const HeadGeom& g) {
+  TanhNormalDim r;
+  const float ev = fminf(fmaxf(a, g.lo), g.hi);
+  if (ev <= g.lo) {
+    const float z = (g.u_lo - loc) / sigma, m = mills(z);
+    r.lp = log_ndtrf(z) - g.log_eps, r.d_loc = -m / sigma, r.d_sigma = -m * z / sigma;
+  } else if (ev >= g.hi) {
+    const float z = -(g.u_hi - loc) / sigma, m = mills(z);
+    r.lp = log_ndtrf(z) - g.log_eps, r.d_loc = m / sigma, r.d_sigma = -m * z / sigma;
+  } else {
+    const float u = atanhf((ev - g.sh) / g.s), z = (u - loc) / sigma;
+    r.lp = -0.5f * z * z - logf(sigma) - kLogSqrt2Pi - tanh_fldj(u) - g.log_s;
+    r.d_loc = z / sigma, r.d_sigma = (z * z - 1.f) / sigma;
+  }
+  return r;
+}
+
+}  // namespace stx

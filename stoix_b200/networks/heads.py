@@ -85,11 +85,24 @@ class AffineTanhNormal:
         self._last = (a, lp, eps)
         return a
 
+    def _rows(self) -> torch.Tensor:
+        return self.head_out.reshape(-1, self.head_out.shape[-1]).contiguous()
+
     def log_prob(self, action: torch.Tensor) -> torch.Tensor:
-        if self._last is None or self._last[0] is not action:
-            raise NotImplementedError("log_prob is available for the action this distribution object has just sampled "
-                                      "(the only use in the SAC systems, ff_sac.py:165-167, 187-188, 217-218)")
-        return self._last[1]
+        """log_prob of `action` (distributions.py:56-80).  The action this object has just sampled returns the value the sampler
+        computed with it (ff_sac.py:165-167); any other action is scored by stx_tanh_normal_log_prob."""
+        if self._last is not None and self._last[0] is action:
+            return self._last[1]
+        A = self.head_out.shape[-1] // 2
+        a = action.to(torch.float32).reshape(-1, A).contiguous()
+        return ops.tanh_normal_log_prob(self._rows(), a, self.minimum, self.maximum, self.min_scale).view(self.head_out.shape[:-1])
+
+    def entropy(self, seed=None, offset: int = 0, dev_counter: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The reference's seeded one-sample estimate entropy(seed) (distributions.py:85-88) per row: Normal entropy plus the
+        log-det-Jacobian of the Shift / Scale / Tanh chain at a Normal sample drawn with `seed`."""
+        ent, _ = ops.tanh_normal_entropy(self._rows(), self.minimum, self.maximum, self.min_scale, seed=_seed_to_int(seed), offset=offset,
+                                         dev_counter=dev_counter)
+        return ent.view(self.head_out.shape[:-1])
 
     def mode(self) -> torch.Tensor:
         A = self.head_out.shape[-1] // 2

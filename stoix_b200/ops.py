@@ -692,6 +692,111 @@ def tanh_normal_backward(head_out: torch.Tensor, eps: torch.Tensor, minimum: flo
     return out
 
 
+def tanh_normal_log_prob(head_out: torch.Tensor, action: torch.Tensor, minimum: float, maximum: float, min_scale: float = 1e-3,
+                         out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """log_prob of GIVEN actions (M, A) under the tanh-Normal head on head_out (M, 2A) (distributions.py:56-80, the inverse path
+    with the clipped tails).  `action` may be a column block of a wider matrix (unit column stride)."""
+    dev = _need_cuda(head_out, out)
+    M, A2 = head_out.shape
+    A = A2 // 2
+    if not action.is_cuda or action.dtype != torch.float32 or action.shape != (M, A) or action.stride(1) != 1:
+        raise StxError("tanh_normal_log_prob: action must be a CUDA float32 (M, A) matrix with unit column stride")
+    if out is None:
+        out = torch.empty(M, dtype=torch.float32, device=dev)
+    _lib.check(_lib.load().stx_tanh_normal_log_prob(_p(head_out), M, A, _p(action), action.stride(0), float(minimum), float(maximum),
+                                                    float(min_scale), _p(out), _stream()), "stx_tanh_normal_log_prob")
+    return out
+
+
+def tanh_normal_entropy(head_out: torch.Tensor, minimum: float, maximum: float, min_scale: float = 1e-3, eps: Optional[torch.Tensor] = None,
+                        seed: int = 0, offset: int = 0, dev_counter: Optional[torch.Tensor] = None,
+                        want_eps: bool = False) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """The seeded one-sample entropy estimate of the tanh-Normal head per row (distributions.py:85-88).  Returns (entropy, eps)."""
+    dev = _need_cuda(head_out, eps, dev_counter)
+    M, A2 = head_out.shape
+    ent = torch.empty(M, dtype=torch.float32, device=dev)
+    eps_out = torch.empty(M, A2 // 2, dtype=torch.float32, device=dev) if (want_eps and eps is None) else None
+    _lib.check(_lib.load().stx_tanh_normal_entropy(_p(head_out), M, A2 // 2, _p(eps), int(seed) & (2**64 - 1), int(offset), _p(dev_counter),
+                                                   float(minimum), float(maximum), float(min_scale), _p(ent), _p(eps_out), _stream()),
+               "stx_tanh_normal_entropy")
+    return ent, (eps if eps is not None else eps_out)
+
+
+def _tanh_normal_ppo(action,minimum, maximum, min_scale, seed, offset, dev_counter, eps_in, eps_out) -> _lib.StxTanhNormalPpo:
+    _need_cuda(action, eps_in, eps_out, dev_counter)
+    for t, name in ((action, "action"), (eps_in, "eps_in"), (eps_out, "eps_out")):
+        if t is not None and t.dtype != torch.float32:
+            raise StxError(f"tanh-Normal PPO head: {name} must be float32")
+    if dev_counter is not None and dev_counter.dtype != torch.int64:
+        raise StxError("tanh-Normal PPO head: dev_counter must be an int64 tensor (used as uint64)")
+    return _lib.StxTanhNormalPpo(_p(action), _p(eps_in), _p(eps_out), _p(dev_counter), int(seed) & (2**64 - 1), int(offset), float(minimum),
+                                 float(maximum), float(min_scale), 0)
+
+
+def ppo_tanh_normal_head_grads(head_out: torch.Tensor, idx: Optional[torch.Tensor], action: torch.Tensor, logp_old: torch.Tensor,
+                               adv: torch.Tensor, adv_stats: Optional[torch.Tensor], clip_eps: float, ent_coef: float, minimum: float,
+                               maximum: float, min_scale: float = 1e-3, seed: int = 0, offset: int = 0,
+                               dev_counter: Optional[torch.Tensor] = None, eps_in: Optional[torch.Tensor] = None,
+                               eps_out: Optional[torch.Tensor] = None, d_head_out: Optional[torch.Tensor] = None,
+                               metrics: Optional[torch.Tensor] = None, weight: float = 1.0, row0: int = 0,
+                               scratch_key: str = "ppo_tanh_normal_head") -> Tuple[torch.Tensor, torch.Tensor]:
+    """The actor half of continuous PPO's _update_minibatch on head outputs computed elsewhere (stx_ppo_tanh_normal_head_grads):
+    row m of head_out (mb, 2A) pairs with batch row idx[m] (or row0 + m) of action (B, A) / logp_old / adv.
+    Returns (d_head_out, metrics[6]); metrics slots 0, 1, 3 = actor_loss, entropy, mean advantage."""
+    dev = _need_cuda(head_out, idx, action, logp_old, adv, adv_stats, d_head_out, metrics)
+    mb, A2 = head_out.shape
+    if idx is not None and idx.dtype != torch.int32:
+        raise StxError("ppo_tanh_normal_head_grads: idx must be int32")
+    if action.ndim != 2 or action.shape[1] != A2 // 2:
+        raise StxError("ppo_tanh_normal_head_grads: action must be (B, A) with 2A = head_out.shape[1]")
+    if d_head_out is None:
+        d_head_out = torch.empty(mb, A2, dtype=torch.float32, device=dev)
+    if metrics is None:
+        metrics = torch.zeros(6, dtype=torch.float32, device=dev)
+    hd = _tanh_normal_ppo(action, minimum, maximum, min_scale, seed, offset, dev_counter, eps_in, eps_out)
+    lib = _lib.load()
+    scratch = _zeros_scratch((scratch_key,), lib.stx_ppo_head_scratch_bytes(mb), dev)
+    _lib.check(lib.stx_ppo_tanh_normal_head_grads(_p(head_out), _p(idx), int(row0), C.byref(hd), _p(logp_old), _p(adv), _p(adv_stats), mb, A2 // 2,
+                                                  float(clip_eps), float(ent_coef), _p(d_head_out), _p(metrics), float(weight), _p(scratch),
+                                                  _stream()), "stx_ppo_tanh_normal_head_grads")
+    return d_head_out, metrics
+
+
+def ppo_continuous_minibatch_grads(actor: MlpSpec, critic: MlpSpec, param_arena: torch.Tensor, batch: PpoBatch, mb_off: int, mb: int,
+                                   clip_eps: float, ent_coef: float, vf_coef: float, standardize: bool, grad_arena: torch.Tensor,
+                                   metrics: torch.Tensor, workspace: torch.Tensor, minimum: float, maximum: float, min_scale: float = 1e-3,
+                                   seed: int = 0, offset: int = 0, dev_counter: Optional[torch.Tensor] = None,
+                                   eps_in: Optional[torch.Tensor] = None, eps_out: Optional[torch.Tensor] = None,
+                                   precision: int = STX_PREC_F32, grad_weight: float = 1.0, overwrite: bool = False) -> None:
+    """ppo_minibatch_grads for a tanh-Normal actor (ff_ppo_continuous.py:184-247): batch.action holds the float (B, A) actions.
+    Entropy noise from Philox (seed, minibatch row, offset + *dev_counter) unless eps_in (mb, A) is given; eps_out records it."""
+    _need_cuda(param_arena, batch.obs, batch.action, batch.log_prob, batch.value, batch.advantages, batch.targets, batch.adv_stats, batch.perm,
+               grad_arena, metrics, workspace)
+    if batch.perm is not None and batch.perm.dtype != torch.int32:
+        raise StxError("ppo_continuous_minibatch_grads: perm must be int32")
+    if batch.obs.dtype != torch.float32:
+        raise StxError("ppo_continuous_minibatch_grads: obs must be float32 (the tanh-Normal head runs on the fp32 path)")
+    _, coff, total = arena_offsets(actor, critic)
+    if param_arena.numel() < total or grad_arena.numel() < total or metrics.numel() < 6:
+        raise StxError("ppo_continuous_minibatch_grads: arena or metrics too small")
+    B = int(batch.log_prob.numel())
+    if batch.action.shape != (B, actor.sizes[-1] // 2):
+        raise StxError(f"ppo_continuous_minibatch_grads: action must be float32 ({B}, {actor.sizes[-1] // 2})")
+    hd = _tanh_normal_ppo(batch.action, minimum, maximum, min_scale, seed, offset, dev_counter, eps_in, eps_out)
+    lib = _lib.load()
+    a = actor.c_struct(param_arena)
+    c = critic.c_struct(param_arena[coff:])
+    b = batch.c_struct()
+    b.action, b.B = None, B
+    h = _lib.StxPpoHyper(float(clip_eps), float(ent_coef), float(vf_coef), int(bool(standardize)), int(bool(overwrite)), 0, None)
+    _lib.check(
+        lib.stx_ppo_continuous_minibatch_grads(C.byref(a), C.byref(c), C.byref(b), C.byref(hd), int(mb_off), int(mb), C.byref(h),
+                                               float(grad_weight), _p(grad_arena), _p(metrics), int(precision), _p(workspace),
+                                               workspace.numel(), _stream()),
+        "stx_ppo_continuous_minibatch_grads",
+    )
+
+
 def sac_actor_seed(q1, q2, log_prob, log_alpha, dq1, dq2, metrics=None, weight: float = 1.0) -> None:
     _need_cuda(q1, q2, log_prob, log_alpha, dq1, dq2, metrics)
     _lib.check(_lib.load().stx_sac_actor_seed(_p(q1), _p(q2), _p(log_prob), _p(log_alpha), q1.numel(), _p(dq1), _p(dq2), _p(metrics), float(weight),

@@ -51,6 +51,7 @@ from stoix_b200.envs.base import Environment, StepOut, TimeStep
 from stoix_b200.networks.base import FeedForwardActor as Actor
 from stoix_b200.networks.base import FeedForwardCritic as Critic
 from stoix_b200.networks.base import build_param_tree
+from stoix_b200.networks.heads import NormalAffineTanhDistributionHead
 from stoix_b200.systems.ppo.ppo_types import PPOTransition
 from stoix_b200.utils import make_env as environments
 from stoix_b200.utils.logger import LogEvent, StoixLogger
@@ -69,7 +70,7 @@ def _world() -> Tuple[int, int]:
 class _Shard:
     """Trajectory buffers of one (device, update-batch) shard: PPOTransition fields, time-major."""
 
-    def __init__(self, T: int, E: int, D: int, A: int, obs_dtype, device, normalize: bool = False):
+    def __init__(self, T: int, E: int, D: int, A: int, obs_dtype, device, normalize: bool = False, act_dim: int = 0):
         z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=device)
         self.obs = z(T + 1, E, D, dt=obs_dtype)      # row t = last_timestep.observation of step t
         self.next_obs = z(T, E, D, dt=obs_dtype)     # timestep.extras["next_obs"]   (ff_ppo.py:113)
@@ -77,7 +78,8 @@ class _Shard:
         # ff_ppo.py:145-162) and obs / next_obs above hold the normalised copies every network kernel reads (:90-94,113-115)
         self.obs_raw = z(T + 1, E, D) if normalize else None
         self.next_obs_raw = z(T, E, D) if normalize else None
-        self.action = z(T, E, dt=torch.int32)
+        # Categorical: (T, E) int32 action indices; tanh-Normal (act_dim > 0): (T, E, act_dim) float32 actions
+        self.action = z(T, E, act_dim) if act_dim > 0 else z(T, E, dt=torch.int32)
         self.log_prob = z(T, E)
         self.value = z(T, E)
         self.bootstrap_value = z(T, E)
@@ -89,7 +91,7 @@ class _Shard:
         self.is_terminal_step = z(T, E, dt=torch.uint8)
         self.advantages = z(T, E)
         self.targets = z(T, E)
-        self.logits = z(E, A)
+        self.logits = z(E, A)                        # actor head output of one step: logits, or loc | scale pre-activation
         self.perms = None  # (epochs, T*E) int32 shuffles of this update, allocated by the learner
         self.adv_stats: Optional[torch.Tensor] = None
 
@@ -146,6 +148,12 @@ def get_learner_fn(
     precision = ops.STX_PREC_BF16 if str(arch.get("precision", "f32")) == "bf16" else ops.STX_PREC_F32
     use_graph = bool(arch.get("cuda_graph", True))
     has_step_into = hasattr(env, "step_into")
+    # The actor head decides the action buffer, the rollout sampler, the gradient entry and the entropy RNG; everything else
+    # (GAE, shuffles, shards, all-reduce, observation normalisation, graph capture) is shared.
+    tanh_head = actor_net.action_head if isinstance(actor_net.action_head, NormalAffineTanhDistributionHead) else None
+    if tanh_head is not None and precision == ops.STX_PREC_BF16:
+        raise ValueError("arch.precision=bf16 is not available with a tanh-Normal actor (NormalAffineTanhDistributionHead): the bf16 "
+                         "tensor-core PPO kernels implement the Categorical head only; use arch.precision=f32")
 
     built: Dict[str, Any] = {}
 
@@ -158,7 +166,8 @@ def get_learner_fn(
         D, A = sa.sizes[0], sa.sizes[-1]
         obs_dtype = torch.bfloat16 if precision == ops.STX_PREC_BF16 else torch.float32
         rs = getattr(state, "running_statistics", None)
-        shards = [_Shard(T, E, D, A, obs_dtype, dev, normalize=rs is not None) for _ in range(U)]
+        act_dim = tanh_head.action_dim if tanh_head is not None else 0
+        shards = [_Shard(T, E, D, A, obs_dtype, dev, normalize=rs is not None, act_dim=act_dim) for _ in range(U)]
         decay = bool(sysc.decay_learning_rates)
         plan = ops.AdamPlan(
             [(0, sa.param_count, actor_opt.init_lr, actor_opt.max_grad_norm),
@@ -186,6 +195,7 @@ def get_learner_fn(
             peers=None,
             roll_ctr=torch.zeros(1, dtype=torch.int64, device=dev),   # categorical call index
             perm_ctr=torch.zeros(1, dtype=torch.int64, device=dev),   # shuffle stream index
+            ent_ctr=torch.zeros(1, dtype=torch.int64, device=dev),    # tanh-Normal entropy noise: minibatch call index
             side_stream=torch.cuda.Stream(device=dev),                # the shuffles run here, underneath the rollout
             critic_stream=torch.cuda.Stream(device=dev),              # chunked critic evaluation underneath the fused rollout
             rs=rs, rs_sums=torch.zeros(2 * D + 1, dtype=torch.float64, device=dev) if rs is not None else None,
@@ -201,7 +211,13 @@ def get_learner_fn(
             ops.obs_normalize(sh.obs_raw[t], b["rs"].mean, b["rs"].std, out=sh.obs[t])
         # SELECT ACTION (ff_ppo.py:97-101): logits -> sample -> log_prob
         ops.mlp_forward(b["sa"], a_tree.flat, sh.obs[t], precision=precision, params_bf16=a_tree.flat_bf16, out=sh.logits, ws_key="learner")
-        ops.categorical(sh.logits, None, seeds[0] + u, t, b["roll_ctr"], out=(sh.action[t], sh.log_prob[t]))
+        if tanh_head is None:
+            ops.categorical(sh.logits, None, seeds[0] + u, t, b["roll_ctr"], out=(sh.action[t], sh.log_prob[t]))
+        else:  # sample, then score the stored action by the inverse path the loss uses (ff_ppo_continuous.py:98-101)
+            lo, hi, ms = tanh_head.minimum, tanh_head.maximum, tanh_head.min_scale
+            ops.tanh_normal_sample(sh.logits, lo, hi, ms, seed=seeds[0] + u, offset=t, dev_counter=b["roll_ctr"], action_out=sh.action[t],
+                                   want_eps=False)
+            ops.tanh_normal_log_prob(sh.logits, sh.action[t], lo, hi, ms, out=sh.log_prob[t])
         # STEP ENVIRONMENT (ff_ppo.py:104-116)
         if has_step_into:
             env.step_into(state.env_state[u], sh.action[t], sh.step_out(t), t)
@@ -321,7 +337,8 @@ def get_learner_fn(
             batches = []
             for u in range(U):
                 sh = b["shards"][u]
-                batches.append(ops.PpoBatch(sh.obs[:T].view(B, D), sh.action.view(B), sh.log_prob.view(B), sh.value.view(B),
+                batches.append(ops.PpoBatch(sh.obs[:T].view(B, D), sh.action.view(B, -1) if tanh_head is not None else sh.action.view(B),
+                                            sh.log_prob.view(B), sh.value.view(B),
                                             sh.advantages.view(B), sh.targets.view(B), sh.adv_stats, sh.perms[ep]))
             # single shard on a single device: the gradient reduction can hand sum(g^2) straight to the fused
             # optimiser (no separate norm pass / grid barrier); otherwise the all-reduce sits in between.
@@ -339,6 +356,14 @@ def get_learner_fn(
                                              b["plan"], a_tree.arena_mu, a_tree.arena_nu, b["arena_bf16"])
                     continue
                 for u in range(U):  # vmap over "batch" + pmean("batch") (ff_ppo.py:253-256); first shard overwrites
+                    if tanh_head is not None:
+                        # entropy noise of this minibatch: (shard seed, row, call = ep * nmb + i + *ent_ctr)
+                        ops.ppo_continuous_minibatch_grads(sa, sc, b["arena"], batches[u], i * mb, mb, float(sysc.clip_eps), float(sysc.ent_coef),
+                                                           float(sysc.vf_coef), bool(sysc.standardize_advantages), grads, metrics[ep, i], b["ws"],
+                                                           tanh_head.minimum, tanh_head.maximum, tanh_head.min_scale, seed=seeds[0] + u,
+                                                           offset=ep * nmb + i, dev_counter=b["ent_ctr"], grad_weight=1.0 / U,
+                                                           overwrite=(u == 0))
+                        continue
                     ops.ppo_minibatch_grads(sa, sc, b["arena"], batches[u], i * mb, mb, float(sysc.clip_eps),
                                             float(sysc.ent_coef), float(sysc.vf_coef), bool(sysc.standardize_advantages),
                                             grads, metrics[ep, i], b["ws"], precision, 1.0 / U, b["arena_bf16"],
@@ -373,6 +398,8 @@ def get_learner_fn(
                 env.advance(state.env_state[u], T)
         ops.counter_add(b["roll_ctr"], T)
         ops.counter_add(b["perm_ctr"], epochs)
+        if tanh_head is not None:
+            ops.counter_add(b["ent_ctr"], epochs * nmb)
 
     def _update_step(state: OnPolicyLearnerState) -> None:
         """A single update of the network (ff_ppo.py:61-341), in place on the learner state."""
@@ -448,23 +475,43 @@ def get_learner_fn(
     return learner_fn
 
 
+def _discrete_action_head_kwargs(env: Environment, config: DictConfig) -> Dict[str, Any]:
+    """Get number/dimension of actions (ff_ppo.py:432-433)."""
+    num_actions = int(env.action_space().num_values)
+    config.system.action_dim = num_actions
+    return {"action_dim": num_actions}
+
+
+def _uniform_discrete_actions(config: DictConfig, E: int, gen: torch.Generator, dev) -> torch.Tensor:
+    return torch.randint(0, int(config.system.action_dim), (E,), device=dev, generator=gen, dtype=torch.int32)
+
+
 def learner_setup(
     env: Environment, keys: Tuple[int, int, int], config: DictConfig
 ) -> Tuple[LearnerFn[OnPolicyLearnerState], Actor, OnPolicyLearnerState]:
     """Initialise learner_fn, network, optimiser, environment and states (ff_ppo.py:424-551)."""
+    return build_learner(env, keys, config, _discrete_action_head_kwargs, _uniform_discrete_actions)
+
+
+def build_learner(
+    env: Environment, keys: Tuple[int, int, int], config: DictConfig,
+    action_head_kwargs: Callable[[Environment, DictConfig], Dict[str, Any]],
+    random_actions: Callable[[DictConfig, int, torch.Generator, Any], torch.Tensor],
+) -> Tuple[LearnerFn[OnPolicyLearnerState], Actor, OnPolicyLearnerState]:
+    """The body of learner_setup shared by the PPO variants.  `action_head_kwargs(env, config)` reads the action space, records
+    it in config.system and returns the action head's constructor arguments; `random_actions(config, E, gen, device)` draws the
+    uniform actions of the observation-normalisation warm-up."""
     rank, world = _world()
     device = torch.device("cuda", torch.cuda.current_device())
     n_devices = world
 
-    # Get number/dimension of actions (ff_ppo.py:432-433).
-    num_actions = int(env.action_space().num_values)
-    config.system.action_dim = num_actions
+    head_kwargs = action_head_kwargs(env, config)
 
     key, actor_net_key, critic_net_key = keys
 
     # Define network and optimiser (ff_ppo.py:439-463).
     actor_torso = instantiate(config.network.actor_network.pre_torso)
-    actor_action_head = instantiate(config.network.actor_network.action_head, action_dim=num_actions)
+    actor_action_head = instantiate(config.network.actor_network.action_head, **head_kwargs)
     critic_torso = instantiate(config.network.critic_network.pre_torso)
     critic_head = instantiate(config.network.critic_network.critic_head)
 
@@ -542,13 +589,13 @@ def learner_setup(
     if config.system.normalize_observations:
         from stoix_b200.utils import running_statistics as rstat
 
-        warmup_observations = _collect_obs_norm_rollouts(env, key, config)
+        warmup_observations = _collect_obs_norm_rollouts(env, key, config, random_actions)
         running_statistics = rstat.initialize_statistics_from_data(init_x[0], warmup_observations)
         init_learner_state = rstat.create_with_running_statistics(init_learner_state, running_statistics)
     return learn, actor_network, init_learner_state
 
 
-def _collect_obs_norm_rollouts(env: Environment, key: int, config: DictConfig) -> torch.Tensor:
+def _collect_obs_norm_rollouts(env: Environment, key: int, config: DictConfig, random_actions=_uniform_discrete_actions) -> torch.Tensor:
     """Collect observations for observation normalisation by taking uniformly random actions for
     system.obs_norm_warmup_steps steps (ff_ppo.py:375-421); not counted in the timestep budget.
     Returns (warmup_steps + 1, num_envs, *obs_shape) raw observations of this rank's env shard."""
@@ -565,7 +612,7 @@ def _collect_obs_norm_rollouts(env: Environment, key: int, config: DictConfig) -
     gen.manual_seed(int(keys[E]) & ((1 << 62) - 1))
     obs = [ts.observation.float().clone()]
     for _ in range(steps):
-        action = torch.randint(0, int(config.system.action_dim), (E,), device=dev, generator=gen, dtype=torch.int32)
+        action = random_actions(config, E, gen, dev)
         env_state, ts = env.step(env_state, action)
         obs.append(ts.observation.float().clone())
     return torch.stack(obs, 0)
@@ -581,6 +628,11 @@ def get_final_step_metrics(metrics: Dict[str, torch.Tensor]) -> Tuple[Dict[str, 
 
 def run_experiment(_config: DictConfig) -> float:
     """Runs experiment (ff_ppo.py:554-706)."""
+    return run_with(_config, learner_setup)
+
+
+def run_with(_config: DictConfig, setup: Callable) -> float:
+    """The body of run_experiment shared by the PPO variants; `setup` is the variant's learner_setup."""
     from stoix_b200.evaluator import evaluator_setup, get_distribution_act_fn
 
     config = copy.deepcopy(_config)
@@ -595,7 +647,7 @@ def run_experiment(_config: DictConfig) -> float:
     env, eval_env = environments.make(config=config)
 
     key, key_e, actor_net_key, critic_net_key = srandom.split(srandom.PRNGKey(config.arch.seed), num=4)
-    learn, actor_network, learner_state = learner_setup(env, (key, actor_net_key, critic_net_key), config)
+    learn, actor_network, learner_state = setup(env, (key, actor_net_key, critic_net_key), config)
 
     evaluator, absolute_metric_evaluator = evaluator_setup(
         eval_env=eval_env, key_e=key_e, eval_act_fn=get_distribution_act_fn(config, actor_network.apply), config=config,
@@ -675,13 +727,18 @@ def run_experiment(_config: DictConfig) -> float:
 def hydra_entry_point(cfg: Optional[DictConfig] = None, overrides: Optional[List[str]] = None) -> float:
     """Experiment entry point (ff_ppo.py:709-727).  Without hydra-core the composition happens here:
     `python -m stoix_b200.systems.ppo.anakin.ff_ppo env=synthetic/box arch.total_num_envs=4096 ...`"""
+    return entry_with(cfg, overrides, "default_ff_ppo", run_experiment)
+
+
+def entry_with(cfg: Optional[DictConfig], overrides: Optional[List[str]], config_name: str, run: Callable[[DictConfig], float]) -> float:
+    """The body of hydra_entry_point shared by the PPO variants."""
     if cfg is None:
-        cfg = compose("default_ff_ppo", overrides if overrides is not None else sys.argv[1:], config_dir="default/anakin")
+        cfg = compose(config_name, overrides if overrides is not None else sys.argv[1:], config_dir="default/anakin")
     if "RANK" in os.environ and not dist.is_initialized():
         torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", 0)))
         dist.init_process_group("nccl")
     t0 = time.time()
-    eval_performance = run_experiment(cfg)
+    eval_performance = run(cfg)
     if _world()[0] == 0:
         print(f"PPO experiment completed in {time.time() - t0:.2f} seconds.")
     return eval_performance
