@@ -11,11 +11,14 @@
 //      All five GEMMs run on wgmma with the activations resident in registers (A operand from registers: the
 //      accumulator of one GEMM packed to bf16 is the A operand of the next); W1's single smem image serves as
 //      MN-major B (forward) and K-major B (backward).  256-wide GEMMs run as two N=128 halves (64 accumulator
-//      registers).  The epilogues also emit h1, h2, dh2, dh1, dz (bf16) for the weight-gradient GEMMs, reduce the
-//      bias gradients (quad butterfly + per-warp smem slices, fixed order) and accumulate the loss metrics.
-//  tc_dw_kernel (K3b)  split-K GEMMs dW = A^T * B over the minibatch rows with both operands MN-major,
-//      4-stage TMA/mbarrier pipeline (one producer warp), two consumer warpgroups with 128 x N fp32 accumulators each:
-//        dW1 = h1^T dh2 (two jobs of N=128), dW2 = h2^T dz (N=16), dW0^T = dh1^T x (N=64).
+//      registers).  The epilogues also emit h2, dh1, dz (bf16) and the h2 > 0 sign mask for the weight-gradient GEMMs,
+//      reduce the bias gradients (quad butterfly + per-warp smem slices, fixed order) and accumulate the loss metrics.
+//  tc_dw_kernel (K3b)  split-K GEMMs dW = A^T * B over the minibatch rows with both operands MN-major, two consumer
+//      warpgroups with fp32 register accumulators and a third warpgroup that feeds them:
+//        dW2 = h2^T dz (N=16), dW0^T = dh1^T x (N=64): 4-stage TMA/mbarrier ring of A and B (one producer warp);
+//        dW1 = h1^T dh2 in two jobs of 128 hidden units (N=256): the third warpgroup rebuilds h1[:, half] = relu(x W0 + b0)
+//        and dh2 = (dz W2^T) * mask per 64-row chunk from x, dz and the mask (12 KB instead of 96 KB of stored h1 and dh2)
+//        with K3a's own instruction sequences, into double-buffered smem images that the consumers multiply.
 //      The activations travel K3a -> K3b in a tiled layout [tile of 128 rows][8-column group][row][8]:
 //      one TMA box of K3b lands 64 rows of every column group as un-swizzled core matrices (8 rows x 16 B).
 //  tc_reduce_kernel     fixed-order reduction of the per-CTA partials into the flat fp32 gradient arena
@@ -56,8 +59,9 @@ constexpr uint32_t kFbSmemBytes = kOffBar + 64 + 1024;
 struct FbNet {
   const __nv_bfloat16* w2;   // [256 x A] bf16
   const float *b0, *b1, *b2;
-  __nv_bfloat16 *h1, *h2, *dh1, *dh2;  // [mb x 256], tiled layout (see tiled_ptr)
+  __nv_bfloat16 *h2, *dh1;            // [mb x 256], tiled layout (see tiled_ptr)
   __nv_bfloat16* dz;                   // [mb x 16] tiled (columns >= A are zero)
+  uint4* mask;                         // [mb / 64][128]: h2 > 0 bits of each 64-row tile in fragment order (see mask_bit)
   float* db_part;                      // [n_cta_of_net][528]
   int A;
   int is_actor;
@@ -84,6 +88,13 @@ struct FbParams {
 __device__ __forceinline__ __nv_bfloat16* tiled_ptr(__nv_bfloat16* base, int64_t row, int col, int CG) {
   return base + (((row >> 7) * CG + (col >> 3)) * 128 + (row & 127)) * 8 + (col & 7);
 }
+
+// Sign mask of h2 in fragment order: thread t of the warpgroup that owns a 64-row tile keeps the bits of its register operand
+// a2[64] (rows 16 (t / 32) + (t % 32) / 4 (+ 8), see stx_tc_ptx.cuh) in one uint4: element e of a2[32 h + i] is bit
+// 2 (i % 16) + e of word 2 h + i / 16.  K3b's rebuild of dh2 runs the same MMA with the same thread <-> (row, column) mapping,
+// so each thread reads back exactly its own 16 bytes.
+__device__ __forceinline__ int mask_word(int h, int i) { return 2 * h + (i >> 4); }
+__device__ __forceinline__ uint32_t mask_bit(int i, int e) { return (uint32_t)(2 * (i & 15) + e); }
 
 // Stores half h of a packed 64 x 256 register operand (rows row0, row0 + 8 of the thread; see stx_tc_ptx.cuh) to the tiled layout.
 __device__ __forceinline__ void store_act(__nv_bfloat16* base, const uint32_t (&a)[64], int h, int64_t row0, int lane, uint64_t pol) {
@@ -271,7 +282,6 @@ __global__ void __launch_bounds__(kFbThreads, 1)
     for (int h = 0; h < 2; ++h) {
       gemm_x_w0(acc, smem_u32(xs), sbase, h);
       epi_bias_relu(acc, s_b0, h, a1, lane);
-      store_act(net.h1, a1, h, row0, lane, pol_stream);
     }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -331,6 +341,7 @@ __global__ void __launch_bounds__(kFbThreads, 1)
         for (int k = 0; k < 4; ++k) dbw[512 + 8 * (k >> 1) + 2 * lane + (k & 1)] += cs[k];
     }
     // ---------------- G3 / E3: dh2 = (dz W2^T) * (h2 > 0), replaces h2 as the A operand of G4 ----------------
+    uint32_t mw[4] = {0u, 0u, 0u, 0u};  // h2 > 0 (fragment order): K3b rebuilds dh2 for dW1 from dz and this mask
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       gemm_dz_w2t(acc, dzp, sbase, h);
@@ -338,13 +349,15 @@ __global__ void __launch_bounds__(kFbThreads, 1)
       for (int i = 0; i < 32; ++i) {
         // h is post-relu (>= 0): positive <=> bf16 bit pattern non-zero (and not -0)
         const uint32_t hm = a2[32 * h + i];
-        acc[2 * i] = (hm & 0x7FFFu) != 0u ? acc[2 * i] : 0.f;
-        acc[2 * i + 1] = (hm & 0x7FFF0000u) != 0u ? acc[2 * i + 1] : 0.f;
+        const bool p0 = (hm & 0x7FFFu) != 0u, p1 = (hm & 0x7FFF0000u) != 0u;
+        mw[mask_word(h, i)] |= ((uint32_t)p0 << mask_bit(i, 0)) | ((uint32_t)p1 << mask_bit(i, 1));
+        acc[2 * i] = p0 ? acc[2 * i] : 0.f;
+        acc[2 * i + 1] = p1 ? acc[2 * i + 1] : 0.f;
         a2[32 * h + i] = pack_bf16(acc[2 * i], acc[2 * i + 1]);
       }
-      store_act(net.dh2, a2, h, row0, lane, pol_stream);
       colsum_half(acc, dbw + 256, h, lane);  // db1
     }
+    st_hint(net.mask + (int64_t)tile * 128 + t, make_uint4(mw[0], mw[1], mw[2], mw[3]), pol_stream);
     // ---------------- G4 / E4: dh1 = (dh2 W1^T) * (h1 > 0) ----------------
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -392,23 +405,45 @@ __global__ void __launch_bounds__(kFbThreads, 1)
 }
 
 // =============================== K3b: dW = A^T * B ===============================================
-constexpr int kDwThreads = 288;  // warps 0..7: two consumer warpgroups (hidden units [128 w, 128 w + 128)), warp 8: TMA
+constexpr int kDwThreads = 384;  // warpgroups 0, 1: MMA consumers; warpgroup 2: TMA producer (warp 8) / dW1 operand rebuild
 constexpr int kDwStages = 4;
 constexpr uint32_t kDwStageBytes = 49152;  // A [64 x 256] 32 KB + B [64 x <=128] 16 KB
 constexpr uint32_t kDwOffBar = kDwStages * kDwStageBytes;
-constexpr uint32_t kDwSmemBytes = kDwOffBar + 64 + 1024;
+constexpr uint32_t kDwSmemBytes = kDwOffBar + 128 + 1024;
 constexpr int kMaxJobs = 8;
 
-// One weight-gradient GEMM: part = A^T * B[:, 8 b_cg0 .. 8 b_cg0 + N) over the rows this CTA is given.
+// dW1 role shared-memory map (inside the ring area of the other roles): a 4-stage ring of the chunk inputs (x 8 KB, dz 2 KB,
+// mask 2 KB), two buffers of the rebuilt operands (h1 half [16 colgroups][64 rows][8] 16 KB, dh2 [32][64][8] 32 KB, the tiled
+// core-matrix layout that K3b's MMAs read), the W0 column half (2 SW128 boxes), the W2 image, b0 of the half.
+constexpr uint32_t kW1StageBytes = 12288;
+constexpr uint32_t kW1OffImg = kDwStages * kW1StageBytes;
+constexpr uint32_t kW1ImgBytes = 49152;
+constexpr uint32_t kW1OffW0 = kW1OffImg + 2 * kW1ImgBytes;
+constexpr uint32_t kW1OffW2 = kW1OffW0 + 16384;
+constexpr uint32_t kW1OffB0 = kW1OffW2 + 8192;
+static_assert(kW1OffB0 + 128 * 4 <= kDwOffBar, "dW1 role smem exceeds the ring area");
+
+// One weight-gradient GEMM over the rows this CTA is given.
+//   rebuild == 0: part = A^T * B[:, 8 b_cg0 .. 8 b_cg0 + N), A and B streamed from K3a's tiled activations.
+//   rebuild == 1: rows [m0, m0 + 128) of dW1 = h1^T dh2 (N = 256): h1[:, m0 ..] = relu(x W0 + b0) and dh2 = (dz W2^T) * mask are
+//                 rebuilt per 64-row chunk from x (map a), dz (map b) and the h2 sign mask with K3a's own instruction sequences,
+//                 so the operands are bit-identical to what K3a computed.
 struct DwJob {
-  float* part;     // [n_cta][256 x N] fp32 partial outputs
-  int N;           // 16, 64 or 128
+  float* part;     // [n_cta][256 x N] fp32 partials; rebuild: the two [n_cta][256 x 128] arrays of output halves, back to back
+  int N;           // 16, 64 or 128 (rebuild: 256)
   int map;         // index of the (A, B) tensor-map pair in DwMaps
   int b_cg;        // column groups of the whole B matrix
   int b_cg0;       // first column group of B taken by this job
   int cta_begin;   // first CTA of this job
   int n_cta;
   int num_chunks;  // mb / 64
+  int rebuild;
+  int m0;          // rebuild: first hidden unit (0 or 128)
+  int net;         // rebuild: index of the network's W0 map in DwMaps
+  int A;           // rebuild: head width
+  const uint4* mask;         // rebuild: K3a's h2 sign mask
+  const __nv_bfloat16* w2;   // rebuild: [256 x A] bf16
+  const float* b0;           // rebuild: [256] fp32 (as K3a reads it)
 };
 struct DwParams {
   DwJob job[kMaxJobs];
@@ -418,6 +453,7 @@ struct DwParams {
 struct DwMaps {
   CUtensorMap a[kMaxJobs];  // tiled [mb x 256]: 2D u64 view {256 per (tile, colgroup), tiles*32}, box {128, 32}
   CUtensorMap b[kMaxJobs];  // tiled [mb x 8 b_cg]: box {128, N/8}
+  CUtensorMap w0[2];        // per network: W0 bf16 [D x 256], SW128 boxes [64 x 64] (as K3a)
 };
 
 template <int N>
@@ -441,8 +477,7 @@ __device__ __forceinline__ void dw_consume(uint8_t* smem, uint64_t* full, uint64
       for (int m = 0; m < 2; ++m) {  // M blocks of 64 hidden units = 8 column groups of A
         const uint64_t da = wg_desc(a0 + (2 * wg + m) * 8192 + ks * 256, 128, 1024, WG_INTERLEAVE);
         const uint32_t accum = (k > 0 || ks > 0) ? 1u : 0u;
-        if constexpr (N == 128) wg_mma_ss_n128<1, 1>(acc[m], da, db, accum);
-        else if constexpr (N == 64) wg_mma_ss_n64<1, 1>(acc[m], da, db, accum);
+        if constexpr (N == 64) wg_mma_ss_n64<1, 1>(acc[m], da, db, accum);
         else wg_mma_ss_n16<1, 1>(acc[m], da, db, accum);
       }
     }
@@ -470,12 +505,124 @@ __device__ __forceinline__ void dw_consume(uint8_t* smem, uint64_t* full, uint64
   }
 }
 
+// dW1 consumers: warpgroup w owns hidden units m0 + 64 w .. + 63 and all 256 output columns (two N=128 accumulators).  Per chunk
+// the products run in the order of the column-split kernel this replaces (16-row steps ks, then chunks), and the partials land
+// in its layout ([output half][n_cta][N/4 = 32][256 rows][4]), so the reduce and its summation order are unchanged.
+__device__ __forceinline__ void dw1_consume(uint8_t* smem, uint64_t* img_full, uint64_t* img_empty, const DwJob& job, int cta,
+                                            int my_chunks) {
+  const uint32_t sbase = smem_u32(smem);
+  const int wg = threadIdx.x >> 7, wq = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  float acc[2][64];
+  wg_zero(acc[0]);
+  wg_zero(acc[1]);
+  for (int k = 0; k < my_chunks; ++k) {
+    const int b = k & 1;
+    mbar_wait(&img_full[b], (k >> 1) & 1, 23);
+    const uint32_t h1 = sbase + kW1OffImg + b * kW1ImgBytes, dh2 = h1 + 16384;
+    wg_fence_acc(acc[0]);
+    wg_fence_acc(acc[1]);
+    wg_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      const uint64_t da = wg_desc(h1 + wg * 8192 + ks * 256, 128, 1024, WG_INTERLEAVE);
+#pragma unroll
+      for (int nh = 0; nh < 2; ++nh)
+        wg_mma_ss_n128<1, 1>(acc[nh], da, wg_desc(dh2 + nh * 16384 + ks * 256, 128, 1024, WG_INTERLEAVE), (k > 0 || ks > 0) ? 1u : 0u);
+    }
+    wg_commit();
+    wg_wait<0>();
+    wg_fence_acc(acc[0]);
+    wg_fence_acc(acc[1]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&img_empty[b]);
+  }
+  const uint64_t pol_keep = l2_evict_last();
+  const int r = job.m0 + wg * 64 + wq * 16 + (lane >> 2);
+#pragma unroll
+  for (int nh = 0; nh < 2; ++nh) {
+    float* out = job.part + (int64_t)(nh * job.n_cta + cta) * 256 * 128;
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const int c = 8 * j + 2 * (lane & 3);
+        float* dst = out + ((int64_t)(c >> 2) * 256 + r + 8 * rr) * 4 + (c & 3);
+        st_hint(reinterpret_cast<uint2*>(dst), make_uint2(__float_as_uint(acc[nh][4 * j + 2 * rr]), __float_as_uint(acc[nh][4 * j + 2 * rr + 1])), pol_keep);
+      }
+  }
+}
+
+// dW1 operand rebuild (warpgroup 2): thread t plays K3a's thread t of the warpgroup that ran the chunk's 64-row tile.  Chunk k's
+// operands go to image buffer k % 2 while the consumers multiply chunk k - 1 out of the other buffer.  Thread 0 also keeps the
+// input ring full.
+__device__ __forceinline__ void dw1_rebuild(uint8_t* smem, uint64_t* full, uint64_t* img_full, uint64_t* img_empty, uint64_t* w_full,
+                                            const CUtensorMap* map_x, const CUtensorMap* map_dz, const DwJob& job, int cta,
+                                            int my_chunks, uint64_t pol_stream) {
+  const uint32_t sbase = smem_u32(smem);
+  const int t = threadIdx.x & 127, wq = t >> 5, lane = t & 31, q4 = lane & 3;
+  const float* s_b0 = reinterpret_cast<const float*>(smem + kW1OffB0);
+  auto load_chunk = [&](int it) {
+    // newest rows first, as the streamed jobs (K3a wrote the last tiles most recently)
+    const int chunk = job.num_chunks - 1 - (cta + it * job.n_cta);
+    const int tile = chunk >> 1, r0 = (chunk & 1) * 64, s = it % kDwStages;
+    uint8_t* st = smem + s * kW1StageBytes;
+    mbar_arrive_expect_tx(&full[s], kW1StageBytes);
+    tma_load_2d_hint(st, map_x, &full[s], r0 * 2, tile * 8, pol_stream);
+    tma_load_2d_hint(st + 8192, map_dz, &full[s], r0 * 2, tile * 2, pol_stream);
+    bulk_load_hint(st + 10240, job.mask + (int64_t)chunk * 128, 2048, &full[s], pol_stream);
+  };
+  if (t == 0)
+    for (int it = 0; it < kDwStages && it < my_chunks; ++it) load_chunk(it);
+  mbar_wait(w_full, 0, 24);
+  for (int it = 0; it < my_chunks; ++it) {
+    const int s = it % kDwStages, b = it & 1;
+    mbar_wait(&full[s], (it / kDwStages) & 1, 25);
+    uint8_t* st = smem + s * kW1StageBytes;
+    uint8_t* h1img = smem + kW1OffImg + b * kW1ImgBytes;
+    uint8_t* dh2img = h1img + 16384;
+    const int r = wq * 16 + (lane >> 2);  // rows r and r + 8 of the chunk
+    float acc[64];
+    uint32_t a[64];
+    // h1[:, m0 ..] = relu(x W0[:, m0 ..] + b0[m0 ..]): K3a's G0 / E0 with x K-major from the tiled layout ([colgroup][row][8])
+    gemm_x_w0_at(acc, wg_desc(smem_u32(st), 1024, 128, WG_INTERLEAVE), 2048, sbase + kW1OffW0, 0);
+    epi_bias_relu(acc, s_b0, 0, a, lane);
+    if (it >= 2) mbar_wait(&img_empty[b], ((it >> 1) - 1) & 1, 26);
+#pragma unroll
+    for (int i = 0; i < 32; ++i)
+      *reinterpret_cast<uint32_t*>(h1img + (i >> 1) * 1024 + (r + 8 * (i & 1)) * 16 + 4 * q4) = a[i];
+    // dh2 = (dz W2^T) * (h2 > 0): K3a's G3 / E3 with dz in the A-fragment layout and the mask words this thread wrote there
+    uint32_t dzp[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) dzp[k] = *reinterpret_cast<const uint32_t*>(st + 8192 + (k >> 1) * 1024 + (r + 8 * (k & 1)) * 16 + 4 * q4);
+    const uint4 m4 = *reinterpret_cast<const uint4*>(st + 10240 + 16 * t);
+    const uint32_t mw[4] = {m4.x, m4.y, m4.z, m4.w};
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      gemm_dz_w2t_at(acc, dzp, sbase + kW1OffW2, h);
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const uint32_t w = mw[mask_word(h, i)];
+        acc[2 * i] = (w >> mask_bit(i, 0)) & 1u ? acc[2 * i] : 0.f;
+        acc[2 * i + 1] = (w >> mask_bit(i, 1)) & 1u ? acc[2 * i + 1] : 0.f;
+        *reinterpret_cast<uint32_t*>(dh2img + (16 * h + (i >> 1)) * 1024 + (r + 8 * (i & 1)) * 16 + 4 * q4) = pack_bf16(acc[2 * i], acc[2 * i + 1]);
+      }
+    }
+    fence_async_proxy();  // generic-proxy image stores -> visible to the consumers' wgmma
+    mbar_arrive(&img_full[b]);
+    wg_sync(3);  // every thread of this warpgroup is done with ring stage s
+    if (t == 0 && it + kDwStages < my_chunks) load_chunk(it + kDwStages);
+  }
+}
+
 __global__ void __launch_bounds__(kDwThreads, 1) tc_dw_kernel(const __grid_constant__ DwMaps maps, const DwParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kDwOffBar);
   uint64_t* full = bars;                 // [kDwStages]
   uint64_t* empty = bars + kDwStages;    // [kDwStages]
+  uint64_t* img_full = bars + 2 * kDwStages;   // [2] dW1 role
+  uint64_t* img_empty = img_full + 2;          // [2]
+  uint64_t* w_full = img_empty + 2;
   const int warp = threadIdx.x >> 5;
   const long long prof_t0 = clock64();
 
@@ -490,6 +637,11 @@ __global__ void __launch_bounds__(kDwThreads, 1) tc_dw_kernel(const __grid_const
       mbar_init(&full[s], 1);
       mbar_init(&empty[s], 8);  // one arrival per consumer warp
     }
+    for (int b = 0; b < 2; ++b) {
+      mbar_init(&img_full[b], 128);  // every rebuild thread, after its own proxy fence
+      mbar_init(&img_empty[b], 8);
+    }
+    mbar_init(w_full, 1);
     fence_barrier_init();
     tma_prefetch_desc(&maps.a[job.map]);
     tma_prefetch_desc(&maps.b[job.map]);
@@ -498,9 +650,26 @@ __global__ void __launch_bounds__(kDwThreads, 1) tc_dw_kernel(const __grid_const
   __syncthreads();
   griddep_wait();  // the activations are K3a's output; the partials written below were read by the previous reduce
 
-  if (warp == 8) {
-    if (elect_one()) {
-      const uint64_t pol_stream = l2_policy(p.act_policy);  // default evict_first: every activation tile is read exactly once
+  const uint64_t pol_stream = l2_policy(p.act_policy);  // default evict_first: every activation tile is read exactly once
+  if (job.rebuild) {
+    // weights of the job's network (after griddep_wait: the previous optimiser step wrote them), as K3a stages them
+    if (threadIdx.x == 256) {
+      mbar_arrive_expect_tx(w_full, 16384);
+      const uint64_t pol_keep = l2_evict_last();
+      for (int jb = 0; jb < 2; ++jb) tma_load_2d_hint(smem + kW1OffW0 + jb * 8192, &maps.w0[job.net], w_full, job.m0 + 64 * jb, 0, pol_keep);
+    }
+    stage_w2(smem + kW1OffW2, job.w2, job.A);
+    if (threadIdx.x < 128) reinterpret_cast<float*>(smem + kW1OffB0)[threadIdx.x] = job.b0[job.m0 + threadIdx.x];
+    fence_async_proxy();
+    __syncthreads();
+  }
+  // 384 threads x 168 registers: the consumers' 128 accumulators + addressing need more than 168, the producer / rebuild
+  // warpgroup fewer (2 x 128 x 200 + 128 x 104 = 384 x 168)
+  if (warp >= 8) {
+    setmaxnreg_dec<104>();
+    if (job.rebuild) {
+      dw1_rebuild(smem, full, img_full, img_empty, w_full, &maps.a[job.map], &maps.b[job.map], job, cta, my_chunks, pol_stream);
+    } else if (warp == 8 && elect_one()) {
       for (int it = 0; it < my_chunks; ++it) {
         // newest rows first (K3a wrote the last tiles most recently, so they are the likeliest L2 residents)
         const int chunk = job.num_chunks - 1 - (cta + it * job.n_cta);  // 64 rows: half of a 128-row tile
@@ -514,12 +683,11 @@ __global__ void __launch_bounds__(kDwThreads, 1) tc_dw_kernel(const __grid_const
         tma_load_2d_hint(st + 32768, &maps.b[job.map], &full[s], r0 * 2, tile * job.b_cg + job.b_cg0, pol_stream);
       }
     }
-  } else if (job.N == 128) {
-    dw_consume<128>(smem, full, empty, job, cta, my_chunks);
-  } else if (job.N == 64) {
-    dw_consume<64>(smem, full, empty, job, cta, my_chunks);
   } else {
-    dw_consume<16>(smem, full, empty, job, cta, my_chunks);
+    setmaxnreg_inc<200>();
+    if (job.rebuild) dw1_consume(smem, img_full, img_empty, job, cta, my_chunks);
+    else if (job.N == 64) dw_consume<64>(smem, full, empty, job, cta, my_chunks);
+    else dw_consume<16>(smem, full, empty, job, cta, my_chunks);
   }
   __syncthreads();
   if (g_prof_buf != nullptr && threadIdx.x == 0) {
@@ -725,15 +893,16 @@ __global__ void __launch_bounds__(kRedThreads, 4) tc_reduce_kernel(const RedPara
 inline size_t al(size_t x) { return (x + 255) / 256 * 256; }
 
 struct TcWs {
-  __nv_bfloat16 *h1[2], *h2[2], *dh1[2], *dh2[2], *dz[2], *xg;
+  __nv_bfloat16 *h2[2], *dh1[2], *dz[2], *xg;
+  uint4* mask[2];
   float *part_w1[2][2], *part_w2[2], *part_w0[2], *db_part[2], *metric_part;
   size_t bytes;
 };
 
 constexpr int kCtaPerNet = kNumSMs / 2;              // 66
 // Launch plan, per network (x 2 networks = 132 CTAs): K3a on 66 CTAs, then K3b with 19 + 19 / 13 / 15 split-K CTAs for
-// the two column halves of dW1 / dW2 / dW0 -- proportional to the bytes each job streams (dW1 half: h1 + half of dh2,
-// dW2: h2 + dz, dW0: dh1 + x): K3b is memory-bound, so the CTAs should finish together.
+// the two row halves of dW1 / dW2 / dW0.  Each dW1 CTA sums the same rows in the same order as the column-split jobs that
+// first set this plan, so the default keeps the gradients' rounding; the split decides which rows each partial holds.
 // Tuning switches: STX_DW_SPLIT="w1,w2,w0" (CTAs per dW1 half, dW2, dW0; 2 w1 + w2 + w0 = 66), STX_K3_POLICY (L2 policy
 // of the activation stream: 0 evict_first, 1 normal, 2 evict_last).
 struct K3Plan {
@@ -758,11 +927,11 @@ TcWs carve_tc(int64_t mb, char* base) {
     return q;
   };
   for (int n = 0; n < 2; ++n) {
-    w.h1[n] = (__nv_bfloat16*)take((size_t)mb * 256 * 2);
     w.h2[n] = (__nv_bfloat16*)take((size_t)mb * 256 * 2);
     w.dh1[n] = (__nv_bfloat16*)take((size_t)mb * 256 * 2);
-    w.dh2[n] = (__nv_bfloat16*)take((size_t)mb * 256 * 2);
     w.dz[n] = (__nv_bfloat16*)take((size_t)mb * 16 * 2);
+    w.mask[n] = (uint4*)take((size_t)mb * 256 / 8);
+    // the dW1 half-jobs write both output halves: [1] must follow [0] directly (the size is a multiple of the alignment)
     for (int hh = 0; hh < 2; ++hh) w.part_w1[n][hh] = (float*)take((size_t)g_plan.w1 * 256 * 128 * 4);
     w.part_w2[n] = (float*)take((size_t)g_plan.w2 * 256 * 16 * 4);
     w.part_w0[n] = (float*)take((size_t)g_plan.w0 * 256 * 64 * 4);
@@ -827,7 +996,7 @@ int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxP
     FbNet& fn = fp.net[n];
     fn.w2 = w + off_w2;
     fn.b0 = m->params + (int64_t)D * kH, fn.b1 = m->params + off_w1 + (int64_t)kH * kH, fn.b2 = m->params + off_w2 + (int64_t)kH * A;
-    fn.h1 = ws.h1[n], fn.h2 = ws.h2[n], fn.dh1 = ws.dh1[n], fn.dh2 = ws.dh2[n], fn.dz = ws.dz[n];
+    fn.h2 = ws.h2[n], fn.dh1 = ws.dh1[n], fn.dz = ws.dz[n], fn.mask = ws.mask[n];
     fn.db_part = ws.db_part[n], fn.A = A, fn.is_actor = (n == 0);
     fp.n_cta[n] = n_fb;
   }
@@ -844,6 +1013,7 @@ int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxP
   // ---- K3b parameters ----
   DwMaps maps;
   DwParams dp{};
+  maps.w0[0] = tmW0[0], maps.w0[1] = tmW0[1];
   int cta = 0, jn = 0;
   const int chunks = (int)(mb / 64);
   const uint64_t tiles = (uint64_t)(mb / 128);
@@ -856,9 +1026,15 @@ int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxP
       cta += n_cta, ++jn;
       return STX_OK;
     };
-    // dW1 = h1^T dh2 (two column halves), dW2 = h2^T dz, dW0^T = dh1^T xg
-    if (int rc = add_job(ws.part_w1[n][0], 128, ws.h1[n], ws.dh2[n], 32, 0, g_plan.w1)) return rc;
-    if (int rc = add_job(ws.part_w1[n][1], 128, ws.h1[n], ws.dh2[n], 32, 16, g_plan.w1)) return rc;
+    // dW1 = h1^T dh2 (two row halves, operands rebuilt from xg, dz and the mask), dW2 = h2^T dz, dW0^T = dh1^T xg
+    for (int hh = 0; hh < 2; ++hh) {
+      DwJob& j = dp.job[jn];
+      if (int rc = make_map_tiled(&maps.a[jn], ws.xg, tiles, 8, 8)) return rc;
+      if (int rc = make_map_tiled(&maps.b[jn], ws.dz[n], tiles, 2, 2)) return rc;
+      j.part = ws.part_w1[n][0], j.N = 256, j.map = jn, j.cta_begin = cta, j.n_cta = g_plan.w1, j.num_chunks = chunks;
+      j.rebuild = 1, j.m0 = 128 * hh, j.net = n, j.A = fp.net[n].A, j.mask = ws.mask[n], j.w2 = fp.net[n].w2, j.b0 = fp.net[n].b0;
+      cta += g_plan.w1, ++jn;
+    }
     if (int rc = add_job(ws.part_w2[n], 16, ws.h2[n], ws.dz[n], 2, 0, g_plan.w2)) return rc;
     if (int rc = add_job(ws.part_w0[n], 64, ws.dh1[n], ws.xg, 8, 0, g_plan.w0)) return rc;
   }

@@ -77,6 +77,14 @@ __device__ __forceinline__ void tma_load_2d_hint(void* smem_dst, const CUtensorM
       : "memory");
 }
 
+// 1D bulk copy global -> shared (bytes: multiple of 16, both addresses 16-byte aligned) with an L2 cache-policy operand
+__device__ __forceinline__ void bulk_load_hint(void* smem_dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t policy) {
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(smem_u32(bar)), "l"(policy)
+      : "memory");
+}
+
 // ---- wgmma ------------------------------------------------------------------------------------
 // A warpgroup (4 consecutive warps, first warp index a multiple of 4) computes D[64 x N] (+)= A[64 x 16] * B[16 x N] per
 // instruction.  D lives in registers: thread t = 32 w + l holds rows 16 w + l/4 and 16 w + l/4 + 8; for every 8-column
@@ -169,6 +177,12 @@ __device__ __forceinline__ uint32_t bias_relu_pack_bf16(uint32_t acc0, uint32_t 
   return d;
 }
 
+// per-warpgroup register budget (every thread of the warpgroup executes it): hand registers from a producer warpgroup to the others
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -188,9 +202,8 @@ __device__ __forceinline__ bool elect_one() {
 //   X  (64 rows x 64 columns, bf16): 128B-swizzled rows, 16-byte chunk c of row r at r*128 + ((c ^ (r%8)) << 4).
 constexpr uint32_t kImgW1 = 0, kImgW0 = 131072, kImgW2 = 163840, kImgWBytes = 172032;
 
-// W2 image and biases staged by all threads of the block (generic proxy; the caller fences and synchronises)
-__device__ __forceinline__ void stage_w2_bias(uint8_t* smem, const __nv_bfloat16* w2, const float* b0, const float* b1, const float* b2,
-                                              int A, float* s_b0, float* s_b1, float* s_b2) {
+// W2 image (layout above, at img) staged by all threads of the block (generic proxy; the caller fences and synchronises)
+__device__ __forceinline__ void stage_w2(uint8_t* img, const __nv_bfloat16* w2, int A) {
   for (int j = threadIdx.x; j < 256; j += blockDim.x) {  // one thread per W2 row: its (<=16) loads are in flight together
     uint32_t pk[8];
     unsigned short e[16];
@@ -198,10 +211,15 @@ __device__ __forceinline__ void stage_w2_bias(uint8_t* smem, const __nv_bfloat16
     for (int n = 0; n < 16; ++n) e[n] = n < A ? reinterpret_cast<const unsigned short*>(w2)[j * A + n] : (unsigned short)0;
 #pragma unroll
     for (int n = 0; n < 8; ++n) pk[n] = (uint32_t)e[2 * n] | ((uint32_t)e[2 * n + 1] << 16);
-    uint8_t* dst = smem + kImgW2 + (j >> 3) * 256 + (j & 7) * 16;
+    uint8_t* dst = img + (j >> 3) * 256 + (j & 7) * 16;
     *reinterpret_cast<uint4*>(dst) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
     *reinterpret_cast<uint4*>(dst + 128) = make_uint4(pk[4], pk[5], pk[6], pk[7]);
   }
+}
+// W2 image and biases staged by all threads of the block (generic proxy; the caller fences and synchronises)
+__device__ __forceinline__ void stage_w2_bias(uint8_t* smem, const __nv_bfloat16* w2, const float* b0, const float* b1, const float* b2,
+                                              int A, float* s_b0, float* s_b1, float* s_b2) {
+  stage_w2(smem + kImgW2, w2, A);
   for (int i = threadIdx.x; i < 256; i += blockDim.x) s_b0[i] = b0[i], s_b1[i] = b1[i];
   if (threadIdx.x < 16) s_b2[threadIdx.x] = threadIdx.x < A ? b2[threadIdx.x] : 0.f;
 }
@@ -212,16 +230,21 @@ __device__ __forceinline__ void wg_zero(float (&d)[R]) {
   for (int i = 0; i < R; ++i) d[i] = 0.f;
 }
 
-// acc = X * W0[:, 128 h .. 128 h + 127]   (K = 64)
-__device__ __forceinline__ void gemm_x_w0(float (&acc)[64], uint32_t s_x, uint32_t sbase, int h) {
-  const uint64_t dx = wg_desc(s_x, 16, 1024, WG_SW128), db = wg_desc(sbase + kImgW0 + h * 16384, 8192, 1024, WG_SW128);
+// acc = X * W0[:, 128 h .. 128 h + 127]   (K = 64).  dx: K-major descriptor of the 64 x 64 X tile, advanced by x_kstep bytes
+// per 16 columns; w0_img: W0 image (layout above).
+__device__ __forceinline__ void gemm_x_w0_at(float (&acc)[64], uint64_t dx, uint32_t x_kstep, uint32_t w0_img, int h) {
+  const uint64_t db = wg_desc(w0_img + h * 16384, 8192, 1024, WG_SW128);
   wg_fence_acc(acc);
   wg_fence();
 #pragma unroll
-  for (int k = 0; k < 4; ++k) wg_mma_ss_n128<0, 1>(acc, wg_adv(dx, k * 32), wg_adv(db, k * 2048), k > 0);
+  for (int k = 0; k < 4; ++k) wg_mma_ss_n128<0, 1>(acc, wg_adv(dx, k * x_kstep), wg_adv(db, k * 2048), k > 0);
   wg_commit();
   wg_wait<0>();
   wg_fence_acc(acc);
+}
+// X as the 128B-swizzled tile of the layout above
+__device__ __forceinline__ void gemm_x_w0(float (&acc)[64], uint32_t s_x, uint32_t sbase, int h) {
+  gemm_x_w0_at(acc, wg_desc(s_x, 16, 1024, WG_SW128), 32, sbase + kImgW0, h);
 }
 // acc = A * W1[:, 128 h ..]   (A: 64 x 256 in registers, 16 K blocks of 4 bf16x2)
 __device__ __forceinline__ void gemm_a_w1(float (&acc)[64], const uint32_t (&a)[64], uint32_t sbase, int h) {
@@ -256,14 +279,17 @@ __device__ __forceinline__ void gemm_a_w2(float (&z)[8], const uint32_t (&a)[64]
   wg_wait<0>();
   wg_fence_acc(z);
 }
-// acc = dZ * W2^T[:, 128 h ..]  (dZ: 64 x 16 in registers, the W2 image read K-major)
-__device__ __forceinline__ void gemm_dz_w2t(float (&acc)[64], const uint32_t (&dz)[4], uint32_t sbase, int h) {
+// acc = dZ * W2^T[:, 128 h ..]  (dZ: 64 x 16 in registers, the W2 image at w2_img read K-major)
+__device__ __forceinline__ void gemm_dz_w2t_at(float (&acc)[64], const uint32_t (&dz)[4], uint32_t w2_img, int h) {
   wg_fence_acc(acc);
   wg_fence();
-  wg_mma_rs_n128<0>(acc, dz, wg_desc(sbase + kImgW2 + h * 4096, 128, 256, WG_INTERLEAVE), 0);
+  wg_mma_rs_n128<0>(acc, dz, wg_desc(w2_img + h * 4096, 128, 256, WG_INTERLEAVE), 0);
   wg_commit();
   wg_wait<0>();
   wg_fence_acc(acc);
+}
+__device__ __forceinline__ void gemm_dz_w2t(float (&acc)[64], const uint32_t (&dz)[4], uint32_t sbase, int h) {
+  gemm_dz_w2t_at(acc, dz, sbase + kImgW2, h);
 }
 // half h of a hidden layer's epilogue: a[32 h + i] = bf16x2(relu(acc[2i] + b), relu(acc[2i+1] + b)), the A operand of the next GEMM
 __device__ __forceinline__ void epi_bias_relu(const float (&acc)[64], const float* bias, int h, uint32_t (&a)[64], int lane) {
