@@ -107,6 +107,13 @@ const char* stx_last_error_string(void);
 /* Kernel launches enqueued by this library in this process so far (host-side count; launches replayed
  * from a captured CUDA graph are counted once, at capture). */
 unsigned long long stx_launch_count(void);
+/* "" or where a tensor-core kernel's bounded mbarrier wait timed out before it trapped (a synchronisation protocol bug):
+ * block, thread, wait tag and phase parity of the first thread to time out in this process.  Host memory: readable after
+ * the trap has made the CUDA context unusable. */
+const char* stx_tc_trap_message(void);
+/* Test hook: out[0] += the number of fp32 bit patterns in [lo, hi] where the call-free device reciprocal (fn 0) or square
+ * root (fn 1) differs in any bit from 1.0f / x or sqrtf(x) on the device; out[1] = min(out[1], the first such pattern). */
+int stx_debug_callfree_math(int fn, uint32_t lo, uint32_t hi, unsigned long long* out, void* stream);
 /* Floats in one network arena (no padding). */
 int64_t stx_mlp_param_count(const StxMlp* mlp);
 

@@ -130,6 +130,8 @@ _SIGNATURES = {
     "stx_version": (C.c_int, []),
     "stx_last_error_string": (C.c_char_p, []),
     "stx_launch_count": (C.c_ulonglong, []),
+    "stx_tc_trap_message": (C.c_char_p, []),
+    "stx_debug_callfree_math": (C.c_int, [C.c_int, C.c_uint32, C.c_uint32, _P, _P]),
     "stx_mlp_param_count": (C.c_int64, [C.POINTER(StxMlp)]),
     "stx_gae_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "stx_gae_set_tuning": (None, [C.c_int]),
@@ -235,4 +237,5 @@ def load():
 def check(rc: int, what: str) -> None:
     if rc != 0:
         msg = load().stx_last_error_string()
-        raise StxError(f"{what} failed (rc={rc}): {msg.decode() if msg else ''}")
+        trap = load().stx_tc_trap_message()
+        raise StxError(f"{what} failed (rc={rc}): {msg.decode() if msg else ''}" + (f" [{trap.decode()}]" if trap else ""))

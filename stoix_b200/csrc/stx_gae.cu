@@ -433,6 +433,7 @@ int launch_gae_tma_shape(const PpoIn& in, int T, int E, int want, float* adv, fl
     STX_CUDA_OK(cudaFuncSetAttribute(gae_tma_kernel<kGE, kGT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGaeSmemBytes));
     if (dev < 64) opted |= 1ull << dev;
   }
+  if (int rc = tc::use_trap_record(st)) return rc;
   const int n_tiles = (E + kGE - 1) / kGE;
   const int grid = n_tiles < kNumSMs ? n_tiles : kNumSMs;
   gae_tma_kernel<kGE, kGT><<<grid, kGE / 4 * kChunks, kGaeSmemBytes, st>>>(mr, mv, mvt, mdn, mtr, in.gamma, in.lambda, in.reward_scale, T, E, adv, tgt,

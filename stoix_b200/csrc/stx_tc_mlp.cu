@@ -216,6 +216,7 @@ int tc_forward_impl(const StxMlp* m, const void* x, int64_t ldx, int64_t M, floa
     STX_CUDA_OK(cudaFuncSetAttribute(tc_mlp_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
     attr_set = true;
   }
+  if (int rc = use_trap_record(st)) return rc;
   const int cap = (g_forward_ctas > 0 && g_forward_ctas < kNumSMs) ? g_forward_ctas : kNumSMs;
   const int want = (p.num_tiles + kWG - 1) / kWG;
   const int grid = want < cap ? want : cap;

@@ -79,6 +79,7 @@ struct FbParams {
   float* metric_part;       // [gridDim][8]
   int D;
   int mb;
+  float inv_m;              // 1 / mb, computed on the host (a device division would be a library call in this kernel)
   float clip_eps, ent_coef, vf_coef;
   int act_policy;     // L2 policy of the activation stores: 0 evict_first (read once, after a kernel boundary), 1 normal, 2 evict_last
 };
@@ -103,31 +104,39 @@ __device__ __forceinline__ void store_act(__nv_bfloat16* base, const uint32_t (&
     st_hint(reinterpret_cast<uint32_t*>(tiled_ptr(base, row0 + 8 * (i & 1), 8 * (i >> 1) + 2 * (lane & 3), 32)), a[i], pol);
 }
 
+// One reduce-scatter step of colsum_half at lane distance S, on entries k, k + 4, k + 8, ... of one class (v[j] = entry k + 4 j):
+// of the 2 S entries still held, lane l keeps half (l & S) and adds its partner's copy of it.  S is a template parameter so
+// that every index into v is a compile-time constant (a loop over S leaves the inner loop rolled and v in local memory).
+template <int S>
+__device__ __forceinline__ void colsum_step(float (&v)[8], int lane) {
+  const bool hi = (lane & S) != 0;
+#pragma unroll
+  for (int j = 0; j < S / 4; ++j) {
+    const float send = hi ? v[j] : v[j + S / 4];
+    const float keep = hi ? v[j + S / 4] : v[j];
+    v[j] = keep + __shfl_xor_sync(0xffffffffu, send, S);
+  }
+}
+
 // Column sums over the 64 rows of a warpgroup tile, half h: x = accumulator-layout values of this thread.  The 8 lanes that
-// share lane % 4 hold the same columns; a reduce-scatter butterfly leaves lane l with the totals of its entries 4 (l/4) .. +3.
+// share lane % 4 hold the same columns; a reduce-scatter butterfly over the 32 row-pair sums e (e = 2 j + b: x[4 j + b] +
+// x[4 j + b + 2]) leaves lane l with the totals of its entries 4 (l/4) + k, k < 4.  The butterfly pairs e with e + 16, e + 8,
+// e + 4, so the four classes e % 4 = k reduce independently: one class at a time keeps 8 partial sums live instead of 32.
 // dst: this warp's slice (every column written by exactly one lane of the warp: fixed order, no atomics).
 __device__ __forceinline__ void colsum_half(const float (&x)[64], float* dst, int h, int lane) {
-  float v[32];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    v[2 * j] = x[4 * j] + x[4 * j + 2];
-    v[2 * j + 1] = x[4 * j + 1] + x[4 * j + 3];
-  }
-#pragma unroll
-  for (int s = 16; s >= 4; s >>= 1) {
-    const int n = 2 * s;  // values still held: 32, 16, 8 -> keep half of them
-#pragma unroll
-    for (int i = 0; i < n / 2; ++i) {
-      const bool hi = (lane & s) != 0;
-      const float send = hi ? v[i] : v[i + n / 2];
-      const float keep = hi ? v[i + n / 2] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, s);
-    }
-  }
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
+    float v[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int e = k + 4 * j, i = 4 * (e >> 1) + (e & 1);
+      v[j] = x[i] + x[i + 2];
+    }
+    colsum_step<16>(v, lane);
+    colsum_step<8>(v, lane);
+    colsum_step<4>(v, lane);
     const int m = 4 * (lane >> 2) + k;
-    dst[128 * h + 8 * (m >> 1) + 2 * (lane & 3) + (m & 1)] += v[k];
+    dst[128 * h + 8 * (m >> 1) + 2 * (lane & 3) + (m & 1)] += v[0];
   }
 }
 
@@ -159,7 +168,7 @@ __device__ __forceinline__ void actor_head_quad(float (&zz)[4], const int (&col)
     se += ex[k];
   }
   se = quad_sum(se);
-  const float lse = __logf(se), inv_se = 1.0f / se;
+  const float lse = __logf(se), inv_se = rcp_rn_callfree(se);  // se in [1, 16]
   float ent = 0.f, logp_a = 0.f;
 #pragma unroll
   for (int k = 0; k < 4; ++k)
@@ -234,7 +243,7 @@ __global__ void __launch_bounds__(kFbThreads, 1)
   float m_acc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};  // actor_loss, entropy, value_loss, adv, pred value, target
   float* dbw = s_db + warp * 528;
   uint8_t* xs = smem + kOffX + wg * 8192;
-  const float inv_m = 1.0f / (float)p.mb;
+  const float inv_m = p.inv_m;
   float adv_mean = 0.f, adv_rstd = 1.f;
   if (p.adv_stats) adv_mean = p.adv_stats[0], adv_rstd = p.adv_stats[1];
   const int dchunks = p.D >> 3;  // 16-byte chunks per observation row
@@ -1007,7 +1016,7 @@ int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxP
   fp.action = b->action, fp.logp_old = b->log_prob, fp.v_old = b->value, fp.adv = b->advantages, fp.tgt = b->targets;
   fp.adv_stats = h->standardize_advantages ? b->adv_stats : nullptr;
   fp.metric_part = ws.metric_part;
-  fp.D = D, fp.mb = (int)mb, fp.clip_eps = h->clip_eps, fp.ent_coef = h->ent_coef, fp.vf_coef = h->vf_coef;
+  fp.D = D, fp.mb = (int)mb, fp.inv_m = 1.0f / (float)mb, fp.clip_eps = h->clip_eps, fp.ent_coef = h->ent_coef, fp.vf_coef = h->vf_coef;
   fp.act_policy = g_plan.act_policy;
 
   // ---- K3b parameters ----
@@ -1043,6 +1052,7 @@ int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxP
   // ---- launches ----
   if (int rc = opt_in_smem(tc_ppo_fwd_bwd_kernel, kFbSmemBytes, 0)) return rc;
   if (int rc = opt_in_smem(tc_dw_kernel, kDwSmemBytes, 1)) return rc;
+  if (int rc = use_trap_record(st)) return rc;
   STX_CUDA_OK(launch_pdl(tc_ppo_fwd_bwd_kernel, dim3(2 * n_fb), dim3(kFbThreads), kFbSmemBytes, st, tmW0[0], tmW1[0], tmW0[1],
                          tmW1[1], fp));
   STX_LAUNCH_OK();

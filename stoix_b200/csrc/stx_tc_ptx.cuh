@@ -6,6 +6,8 @@
 #include <cuda_bf16.h>
 #include <stdint.h>
 
+#include "stx_common.cuh"
+
 namespace stx {
 namespace tc {
 
@@ -46,15 +48,43 @@ __device__ __forceinline__ bool mbar_test_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug traps (with a message) instead of hanging the GPU.
+// This translation unit's pointer to the process-wide TrapRecord (stx_common.cuh); set by use_trap_record().
+static __device__ TrapRecord* g_trap_record = nullptr;
+
+// Bounded wait: a protocol bug traps instead of hanging the GPU.  The first thread to time out records where in the host-
+// mapped TrapRecord, which _lib.py reports with the error.  No printf: a call would serialise every wgmma of the kernel.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, int tag) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
     if (++spins > (1u << 26)) {
-      printf("[stx tc] mbarrier wait timeout: block %d thread %d tag %d parity %u\n", blockIdx.x, threadIdx.x, tag, parity);
+      volatile TrapRecord* r = g_trap_record;
+      if (r != nullptr && atomicCAS_system(const_cast<uint32_t*>(&r->claimed), 0u, 1u) == 0u) {
+        r->block = blockIdx.x, r->thread = threadIdx.x, r->tag = (uint32_t)tag, r->parity = parity;
+        __threadfence_system();
+      }
       __trap();
     }
   }
+}
+
+// Host: points g_trap_record of the calling translation unit at the process-wide record, once per device.  Skipped while
+// `st` is being captured (a synchronous copy is not allowed then); the pointer is device state, so the next eager call
+// also covers the kernels of graphs captured before it.
+static inline int use_trap_record(cudaStream_t st) {
+  static unsigned long long done = 0;  // bit d: set on device d
+  int dev = 0;
+  STX_CUDA_OK(cudaGetDevice(&dev));
+  if (dev < 64 && ((done >> dev) & 1ull)) return STX_OK;
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  STX_CUDA_OK(cudaStreamIsCapturing(st, &cs));
+  if (cs != cudaStreamCaptureStatusNone) return STX_OK;
+  TrapRecord* host = trap_record();
+  STX_REQUIRE(host != nullptr, STX_E_UNSUPPORTED, "could not allocate the host-mapped mbarrier timeout record");
+  TrapRecord* dptr = nullptr;
+  STX_CUDA_OK(cudaHostGetDevicePointer(reinterpret_cast<void**>(&dptr), host, 0));
+  STX_CUDA_OK(cudaMemcpyToSymbol(g_trap_record, &dptr, sizeof(dptr)));
+  if (dev < 64) done |= 1ull << dev;
+  return STX_OK;
 }
 
 // ---- TMA -------------------------------------------------------------------------------------

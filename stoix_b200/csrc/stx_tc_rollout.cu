@@ -306,6 +306,7 @@ extern "C" int stx_tc_rollout_synth(const StxMlp* actor, void* obs, void* next_o
     STX_CUDA_OK(cudaFuncSetAttribute(ro::tc_rollout_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ro::kSmemBytes));
     attr_set = true;
   }
+  if (int rc = use_trap_record((cudaStream_t)stream)) return rc;
   ro::tc_rollout_kernel<<<(unsigned)(E / ro::kTileM), ro::kThreads, ro::kSmemBytes, (cudaStream_t)stream>>>(tmW0, tmW1, p);
   STX_LAUNCH_OK();
   return STX_OK;
