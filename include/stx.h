@@ -498,6 +498,60 @@ int stx_ppo_continuous_minibatch_grads(const StxMlp* actor, const StxMlp* critic
                                        int64_t mb_off, int64_t mb, const StxPpoHyper* hyper, float grad_weight, float* grad_arena, float* metrics,
                                        int precision, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------ PPO variants: KL penalty and DPO (fp32) --------
+ * Each variant replaces only the actor loss of _update_minibatch; the critic half, the networks' forward / backward, the
+ * workspace (stx_ppo_workspace_bytes(F32)) and the metric reduction are the clip path's.  No ratio clipping in either.
+ * KL penalty (ppo_penalty_loss, stoix/utils/loss.py:35-47; ff_ppo_penalty.py:150-178, ff_ppo_penalty_continuous.py:150-179):
+ *   actor_loss = -mean(ratio A) + kl_coef * mean(KL_i), KL_i = KL(behaviour_i || pi_i), no gradient into the behaviour policy.
+ *   The behaviour policy is the actor at the start of the update (:137); its head outputs are supplied per batch row in
+ *   `behaviour` ((B, A) logits or (B, 2A) loc | scale pre-activation), read as behaviour[idx[m]] like the other batch fields.
+ *   Categorical KL = sum_j pb_j (log pb_j - log p_j); tanh-Normal KL = the KL of the base Normals summed over the dims,
+ *   sum_j [log(s_j / sb_j) + (sb_j^2 + (mb_j - m_j)^2) / (2 s_j^2) - 1/2] (the shared affine-tanh bijector cancels).
+ * DPO (dpo_loss, loss.py:50-65; ff_dpo_continuous.py:160-170), tanh-Normal only:
+ *   ld = logp - logp_old, x1 = (e^ld - 1) A, x2 = ld A, drift = 1[A>=0] relu(x1 - alpha tanh(x1/alpha)) + 1[A<0] relu(x2 - beta tanh(x2/beta)),
+ *   actor_loss = -mean(e^ld A - drift).
+ * Entropy: exact for the Categorical, the seeded estimate of the continuous section (same noise layout) for the tanh-Normal;
+ *   total = actor_loss - ent_coef * mean H.
+ * Metrics accumulated with `weight`: [0] actor_loss, [1] entropy, [6] kl_divergence (KL penalty only); the minibatch entries
+ *   add [2] value_loss, [4] pred_value, [5] target_value from the critic half.  metrics must hold 7 floats.
+ * STX_PREC_BF16 returns STX_E_UNSUPPORTED: the bf16 tensor-core kernels implement the clipped Categorical loss only. */
+#define STX_PPO_KL_PENALTY 1
+#define STX_PPO_DPO 2
+typedef struct StxPpoVariant {
+  const float* behaviour;  /* (B, head width) behaviour head outputs, STX_PPO_KL_PENALTY; NULL for STX_PPO_DPO */
+  int32_t kind;            /* STX_PPO_KL_PENALTY or STX_PPO_DPO */
+  float kl_coef;           /* beta of ppo_penalty_loss (system.kl_penalty_coef) */
+  float dpo_alpha;         /* alpha of dpo_loss (system.alpha) */
+  float dpo_beta;          /* beta of dpo_loss (system.beta) */
+} StxPpoVariant;
+/* Per-row KL(p || q): tfd.Categorical.kl_divergence (logits (M, A)) and the tanh-Normal head's (head outputs (M, 2A)). */
+int stx_categorical_kl(const float* logits_p, const float* logits_q, int64_t M, int A, float* kl, void* stream);
+int stx_tanh_normal_kl(const float* head_p, const float* head_q, int64_t M, int A, float min_scale, float* kl, void* stream);
+/* Value faces (loss.py:35-47, 50-65) with stx_loss_scratch_bytes() scratch: stx_ppo_penalty_loss writes out[0] = the actor loss
+ * and out[1] = mean(kl) from per-row kl; stx_dpo_loss writes out[0]. */
+int stx_ppo_penalty_loss(const float* pi_log_prob_t, const float* b_pi_log_prob_t, const float* gae_t, const float* kl, int64_t n, float beta,
+                         float* out, void* scratch, void* stream);
+int stx_dpo_loss(const float* pi_log_prob_t, const float* b_pi_log_prob_t, const float* gae_t, int64_t n, float alpha, float beta, float* out,
+                 void* scratch, void* stream);
+/* Actor halves on head outputs computed elsewhere: row m pairs with batch row idx[m] (or row0 + m); A <= 32; scratch:
+ * stx_ppo_head_scratch_bytes(mb), zeroed once.  stx_ppo_penalty_head_grads is the Categorical KL penalty (v->kind must be
+ * STX_PPO_KL_PENALTY); stx_ppo_variant_tanh_normal_head_grads serves both kinds. */
+int stx_ppo_penalty_head_grads(const float* logits, const int32_t* idx, int64_t row0, const StxPpoVariant* v, const int32_t* action,
+                               const float* logp_old, const float* adv, const float* adv_stats, int64_t mb, int A, float ent_coef, float* d_logits,
+                               float* metrics, float weight, void* scratch, void* stream);
+int stx_ppo_variant_tanh_normal_head_grads(const float* head_out, const int32_t* idx, int64_t row0, const StxTanhNormalPpo* head,
+                                           const StxPpoVariant* v, const float* logp_old, const float* adv, const float* adv_stats, int64_t mb,
+                                           int A, float ent_coef, float* d_head_out, float* metrics, float weight, void* scratch, void* stream);
+/* Minibatch entries (like stx_ppo_minibatch_grads / stx_ppo_continuous_minibatch_grads): actor forward, the variant's loss
+ * kernel, actor backward, critic half.  hyper->clip_eps clips only the value loss. */
+int stx_ppo_penalty_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxPpoBatch* batch, const StxPpoVariant* v, int64_t mb_off,
+                                    int64_t mb, const StxPpoHyper* hyper, float grad_weight, float* grad_arena, float* metrics, int precision,
+                                    void* workspace, size_t workspace_bytes, void* stream);
+int stx_ppo_variant_continuous_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxPpoBatch* batch, const StxTanhNormalPpo* head,
+                                               const StxPpoVariant* v, int64_t mb_off, int64_t mb, const StxPpoHyper* hyper, float grad_weight,
+                                               float* grad_arena, float* metrics, int precision, void* workspace, size_t workspace_bytes,
+                                               void* stream);
+
 /* Utility casts used by the bf16 path (obs / weight shadows). */
 int stx_cast_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream);
 

@@ -124,6 +124,20 @@ class StxTanhNormalPpo(C.Structure):
     ]
 
 
+STX_PPO_KL_PENALTY = 1
+STX_PPO_DPO = 2
+
+
+class StxPpoVariant(C.Structure):
+    _fields_ = [
+        ("behaviour", C.c_void_p),
+        ("kind", C.c_int32),
+        ("kl_coef", C.c_float),
+        ("dpo_alpha", C.c_float),
+        ("dpo_beta", C.c_float),
+    ]
+
+
 _P = C.c_void_p
 _SIGNATURES = {
     # name: (restype, argtypes)
@@ -197,6 +211,19 @@ _SIGNATURES = {
                                                  C.c_float, _P, _P, C.c_float, _P, _P]),
     "stx_ppo_continuous_minibatch_grads": (C.c_int, [C.POINTER(StxMlp), C.POINTER(StxMlp), C.POINTER(StxPpoBatch), C.POINTER(StxTanhNormalPpo),
                                                      C.c_int64, C.c_int64, C.POINTER(StxPpoHyper), C.c_float, _P, _P, C.c_int, _P, C.c_size_t, _P]),
+    "stx_categorical_kl": (C.c_int, [_P, _P, C.c_int64, C.c_int, _P, _P]),
+    "stx_tanh_normal_kl": (C.c_int, [_P, _P, C.c_int64, C.c_int, C.c_float, _P, _P]),
+    "stx_ppo_penalty_loss": (C.c_int, [_P, _P, _P, _P, C.c_int64, C.c_float, _P, _P, _P]),
+    "stx_dpo_loss": (C.c_int, [_P, _P, _P, C.c_int64, C.c_float, C.c_float, _P, _P, _P]),
+    "stx_ppo_penalty_head_grads": (C.c_int, [_P, _P, C.c_int64, C.POINTER(StxPpoVariant), _P, _P, _P, _P, C.c_int64, C.c_int, C.c_float, _P, _P,
+                                             C.c_float, _P, _P]),
+    "stx_ppo_variant_tanh_normal_head_grads": (C.c_int, [_P, _P, C.c_int64, C.POINTER(StxTanhNormalPpo), C.POINTER(StxPpoVariant), _P, _P, _P,
+                                                         C.c_int64, C.c_int, C.c_float, _P, _P, C.c_float, _P, _P]),
+    "stx_ppo_penalty_minibatch_grads": (C.c_int, [C.POINTER(StxMlp), C.POINTER(StxMlp), C.POINTER(StxPpoBatch), C.POINTER(StxPpoVariant),
+                                                  C.c_int64, C.c_int64, C.POINTER(StxPpoHyper), C.c_float, _P, _P, C.c_int, _P, C.c_size_t, _P]),
+    "stx_ppo_variant_continuous_minibatch_grads": (C.c_int, [C.POINTER(StxMlp), C.POINTER(StxMlp), C.POINTER(StxPpoBatch),
+                                                             C.POINTER(StxTanhNormalPpo), C.POINTER(StxPpoVariant), C.c_int64, C.c_int64,
+                                                             C.POINTER(StxPpoHyper), C.c_float, _P, _P, C.c_int, _P, C.c_size_t, _P]),
 }
 
 _lib = None

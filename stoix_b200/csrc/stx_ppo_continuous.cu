@@ -12,7 +12,6 @@
 namespace stx {
 namespace {
 
-constexpr uint32_t kTagPpoEntropy = 0x50504f45u;  // "PPOE"
 constexpr int kMaxTanhNormalDims = 32;
 
 // Rollout / face: log_prob of given actions, one thread per row.
@@ -46,26 +45,6 @@ struct TnLossArgs {
   float* metrics;         // slots 0 (actor_loss), 1 (entropy), 3 (advantages) accumulated with weight
   float weight;
 };
-
-// Entropy noise eps' of row m, dims j0..j0+3 (layout in include/stx.h); eps_in (nullable, (rows, A)) replaces the draw.
-__device__ __forceinline__ void entropy_noise(const float* __restrict__ eps_in, int A, uint64_t seed, int64_t m, uint64_t call, int j0, float e[4]) {
-  if (eps_in) {
-#pragma unroll
-    for (int k = 0; k < 4; ++k) e[k] = j0 + k < A ? eps_in[m * A + j0 + k] : 0.f;
-    return;
-  }
-  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
-  const uint4 w = Philox::rand4(make_uint4((uint32_t)m, (uint32_t)call,
-                                           (uint32_t)(call >> 32) ^ ((uint32_t)(j0 >> 2) << 20) ^ ((uint32_t)((uint64_t)m >> 32) << 8),
-                                           kTagPpoEntropy), key);
-  const float2 n0 = normal2(w.x, w.y), n1 = normal2(w.z, w.w);
-  e[0] = n0.x, e[1] = n0.y, e[2] = n1.x, e[3] = n1.y;
-}
-
-// One dimension of the entropy estimate: Normal entropy + fldj of the Shift / Scale / Tanh chain at the Normal sample.
-__device__ __forceinline__ float tanh_normal_entropy_dim(float loc, float sigma, float e, const HeadGeom& g) {
-  return 0.5f + kLogSqrt2Pi + logf(sigma) + g.log_s + tanh_fldj(loc + sigma * e);
-}
 
 // Face of the estimate (AffineTanhNormal.entropy(seed)): one thread per row, noise keyed by the row index.
 __global__ void tanh_normal_entropy_kernel(const float* __restrict__ head, int64_t M, int A, const float* __restrict__ eps_in, uint64_t seed,

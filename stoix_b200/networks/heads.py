@@ -40,6 +40,12 @@ class Categorical:
         _, _, ent = ops.categorical(self._flat, a, want_entropy=True)
         return ent.view(self._lead)
 
+    def kl_divergence(self, other: "Categorical") -> torch.Tensor:
+        """KL(self || other) per row (tfd.Categorical.kl_divergence, as ppo_penalty_loss calls it, loss.py:44)."""
+        if not isinstance(other, Categorical) or other._flat.shape != self._flat.shape:
+            raise TypeError("Categorical.kl_divergence: `other` must be a Categorical over the same shape")
+        return ops.categorical_kl(self._flat, other._flat).view(self._lead)
+
     def mode(self) -> torch.Tensor:
         return torch.argmax(self.logits, dim=-1).to(torch.int32)
 
@@ -103,6 +109,16 @@ class AffineTanhNormal:
         ent, _ = ops.tanh_normal_entropy(self._rows(), self.minimum, self.maximum, self.min_scale, seed=_seed_to_int(seed), offset=offset,
                                          dev_counter=dev_counter)
         return ent.view(self.head_out.shape[:-1])
+
+    def kl_divergence(self, other: "AffineTanhNormal") -> torch.Tensor:
+        """KL(self || other) per row.  Both transform their base Normal by the same affine-tanh bijector, and a KL is invariant
+        under a shared bijection, so it is the KL of the base Normals summed over the action dimensions (the registration tfp
+        applies to Independent / TransformedDistribution pairs, loss.py:44)."""
+        if not isinstance(other, AffineTanhNormal) or other.head_out.shape != self.head_out.shape:
+            raise TypeError("AffineTanhNormal.kl_divergence: `other` must be an AffineTanhNormal over the same shape")
+        if (other.minimum, other.maximum, other.min_scale) != (self.minimum, self.maximum, self.min_scale):
+            raise ValueError("AffineTanhNormal.kl_divergence: both distributions must share the bounds and min_scale")
+        return ops.tanh_normal_kl(self._rows(), other._rows(), self.min_scale).view(self.head_out.shape[:-1])
 
     def mode(self) -> torch.Tensor:
         A = self.head_out.shape[-1] // 2

@@ -797,6 +797,191 @@ def ppo_continuous_minibatch_grads(actor: MlpSpec, critic: MlpSpec, param_arena:
     )
 
 
+# ------------------------------------------------------------------------------------------------
+# PPO variants: KL penalty (ff_ppo_penalty*, loss.py:35-47) and DPO (ff_dpo_continuous, loss.py:50-65)
+# ------------------------------------------------------------------------------------------------
+
+STX_PPO_KL_PENALTY, STX_PPO_DPO = _lib.STX_PPO_KL_PENALTY, _lib.STX_PPO_DPO
+METRIC_SLOT_KL = 6  # metrics slot of kl_divergence (0 actor_loss, 1 entropy, 2 value_loss, 3-5 as on the clip path)
+
+
+def _variant(kind: int, behaviour: Optional[torch.Tensor], kl_coef: float, dpo_alpha: float, dpo_beta: float) -> _lib.StxPpoVariant:
+    _need_cuda(behaviour)
+    if behaviour is not None and behaviour.dtype != torch.float32:
+        raise StxError("PPO variant: behaviour head outputs must be float32")
+    if kind == STX_PPO_KL_PENALTY and behaviour is None:
+        raise StxError("PPO variant: the KL penalty needs the behaviour head outputs")
+    return _lib.StxPpoVariant(_p(behaviour), int(kind), float(kl_coef), float(dpo_alpha), float(dpo_beta))
+
+
+def categorical_kl(logits_p: torch.Tensor, logits_q: torch.Tensor) -> torch.Tensor:
+    """KL(Categorical(logits_p) || Categorical(logits_q)) per row of (M, A) logits."""
+    dev = _need_cuda(logits_p, logits_q)
+    if logits_p.shape != logits_q.shape or logits_p.dtype != torch.float32 or logits_q.dtype != torch.float32 or logits_p.ndim != 2:
+        raise StxError("categorical_kl: expected two float32 (M, A) logit matrices of the same shape")
+    out = torch.empty(logits_p.shape[0], dtype=torch.float32, device=dev)
+    _lib.check(_lib.load().stx_categorical_kl(_p(logits_p), _p(logits_q), logits_p.shape[0], logits_p.shape[1], _p(out), _stream()),
+               "stx_categorical_kl")
+    return out
+
+
+def tanh_normal_kl(head_p: torch.Tensor, head_q: torch.Tensor, min_scale: float = 1e-3) -> torch.Tensor:
+    """KL(p || q) per row of two tanh-Normal heads (M, 2A) with the same bounds: the KL of the base Normals summed over the dims."""
+    dev = _need_cuda(head_p, head_q)
+    if head_p.shape != head_q.shape or head_p.dtype != torch.float32 or head_q.dtype != torch.float32 or head_p.ndim != 2 or head_p.shape[1] % 2:
+        raise StxError("tanh_normal_kl: expected two float32 (M, 2A) head outputs of the same shape")
+    out = torch.empty(head_p.shape[0], dtype=torch.float32, device=dev)
+    _lib.check(_lib.load().stx_tanh_normal_kl(_p(head_p), _p(head_q), head_p.shape[0], head_p.shape[1] // 2, float(min_scale), _p(out), _stream()),
+               "stx_tanh_normal_kl")
+    return out
+
+
+def _flat_f32(*ts: torch.Tensor, what: str) -> None:
+    _need_cuda(*ts)
+    if any(t.dtype != torch.float32 for t in ts) or len({t.numel() for t in ts}) != 1:
+        raise StxError(f"{what}: expected float32 tensors of equal size")
+
+
+def ppo_penalty_loss_value(pi_log_prob_t, b_pi_log_prob_t, gae_t, kl, beta: float) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(-mean(ratio A) + beta mean(kl), mean(kl)) of ppo_penalty_loss (loss.py:35-47) from per-row KL values."""
+    _flat_f32(pi_log_prob_t, b_pi_log_prob_t, gae_t, kl, what="ppo_penalty_loss_value")
+    lib = _lib.load()
+    out = torch.empty(2, dtype=torch.float32, device=gae_t.device)
+    scratch = _zeros_scratch(("loss",), lib.stx_loss_scratch_bytes(), gae_t.device)
+    _lib.check(lib.stx_ppo_penalty_loss(_p(pi_log_prob_t), _p(b_pi_log_prob_t), _p(gae_t), _p(kl), gae_t.numel(), float(beta), _p(out), _p(scratch),
+                                        _stream()), "stx_ppo_penalty_loss")
+    return out[0], out[1]
+
+
+def dpo_loss_value(pi_log_prob_t, b_pi_log_prob_t, gae_t, alpha: float, beta: float) -> torch.Tensor:
+    """-mean(ratio A - drift) of dpo_loss (loss.py:50-65)."""
+    _flat_f32(pi_log_prob_t, b_pi_log_prob_t, gae_t, what="dpo_loss_value")
+    lib = _lib.load()
+    out = torch.empty(1, dtype=torch.float32, device=gae_t.device)
+    scratch = _zeros_scratch(("loss",), lib.stx_loss_scratch_bytes(), gae_t.device)
+    _lib.check(lib.stx_dpo_loss(_p(pi_log_prob_t), _p(b_pi_log_prob_t), _p(gae_t), gae_t.numel(), float(alpha), float(beta), _p(out), _p(scratch),
+                                _stream()), "stx_dpo_loss")
+    return out[0]
+
+
+def ppo_penalty_head_grads(logits: torch.Tensor, idx: Optional[torch.Tensor], behaviour: torch.Tensor, action: torch.Tensor, logp_old: torch.Tensor,
+                           adv: torch.Tensor, adv_stats: Optional[torch.Tensor], kl_coef: float, ent_coef: float,
+                           d_logits: Optional[torch.Tensor] = None, metrics: Optional[torch.Tensor] = None, weight: float = 1.0, row0: int = 0,
+                           scratch_key: str = "ppo_penalty_head") -> Tuple[torch.Tensor, torch.Tensor]:
+    """The actor half of ff_ppo_penalty's _update_minibatch on logits (mb, A) computed elsewhere: row m pairs with batch row idx[m]
+    (or row0 + m) of behaviour (B, A) / action / logp_old / adv.  Returns (d_logits, metrics[8]); slots 0, 1, 6 = actor_loss,
+    entropy, kl_divergence."""
+    dev = _need_cuda(logits, idx, behaviour, action, logp_old, adv, adv_stats, d_logits, metrics)
+    mb, A = logits.shape
+    if (idx is not None and idx.dtype != torch.int32) or action.dtype != torch.int32:
+        raise StxError("ppo_penalty_head_grads: idx / action must be int32")
+    if behaviour.ndim != 2 or behaviour.shape[1] != A:
+        raise StxError("ppo_penalty_head_grads: behaviour must be (B, A) with A = logits.shape[1]")
+    d_logits = torch.empty(mb, A, dtype=torch.float32, device=dev) if d_logits is None else d_logits
+    metrics = torch.zeros(8, dtype=torch.float32, device=dev) if metrics is None else metrics
+    if metrics.numel() < 7:
+        raise StxError("ppo_penalty_head_grads: metrics must hold at least 7 floats")
+    v = _variant(STX_PPO_KL_PENALTY, behaviour, kl_coef, 0.0, 0.0)
+    lib = _lib.load()
+    scratch = _zeros_scratch((scratch_key,), lib.stx_ppo_head_scratch_bytes(mb), dev)
+    _lib.check(lib.stx_ppo_penalty_head_grads(_p(logits), _p(idx), int(row0), C.byref(v), _p(action), _p(logp_old), _p(adv), _p(adv_stats), mb, A,
+                                              float(ent_coef), _p(d_logits), _p(metrics), float(weight), _p(scratch), _stream()),
+               "stx_ppo_penalty_head_grads")
+    return d_logits, metrics
+
+
+def ppo_variant_tanh_normal_head_grads(head_out: torch.Tensor, idx: Optional[torch.Tensor], kind: int, action: torch.Tensor, logp_old: torch.Tensor,
+                                       adv: torch.Tensor, adv_stats: Optional[torch.Tensor], ent_coef: float, minimum: float, maximum: float,
+                                       min_scale: float = 1e-3, behaviour: Optional[torch.Tensor] = None, kl_coef: float = 0.0,
+                                       dpo_alpha: float = 2.0, dpo_beta: float = 0.6, seed: int = 0, offset: int = 0,
+                                       dev_counter: Optional[torch.Tensor] = None, eps_in: Optional[torch.Tensor] = None,
+                                       eps_out: Optional[torch.Tensor] = None, d_head_out: Optional[torch.Tensor] = None,
+                                       metrics: Optional[torch.Tensor] = None, weight: float = 1.0, row0: int = 0,
+                                       scratch_key: str = "ppo_variant_head") -> Tuple[torch.Tensor, torch.Tensor]:
+    """The actor half of ff_ppo_penalty_continuous / ff_dpo_continuous (kind STX_PPO_KL_PENALTY / STX_PPO_DPO) on head outputs
+    (mb, 2A) computed elsewhere; entropy noise as ppo_tanh_normal_head_grads.  Returns (d_head_out, metrics[8])."""
+    dev = _need_cuda(head_out, idx, action, logp_old, adv, adv_stats, d_head_out, metrics)
+    mb, A2 = head_out.shape
+    if idx is not None and idx.dtype != torch.int32:
+        raise StxError("ppo_variant_tanh_normal_head_grads: idx must be int32")
+    if action.ndim != 2 or action.shape[1] != A2 // 2 or (behaviour is not None and (behaviour.ndim != 2 or behaviour.shape[1] != A2)):
+        raise StxError("ppo_variant_tanh_normal_head_grads: action must be (B, A) and behaviour (B, 2A) with 2A = head_out.shape[1]")
+    d_head_out = torch.empty(mb, A2, dtype=torch.float32, device=dev) if d_head_out is None else d_head_out
+    metrics = torch.zeros(8, dtype=torch.float32, device=dev) if metrics is None else metrics
+    if metrics.numel() < 7:
+        raise StxError("ppo_variant_tanh_normal_head_grads: metrics must hold at least 7 floats")
+    hd = _tanh_normal_ppo(action, minimum, maximum, min_scale, seed, offset, dev_counter, eps_in, eps_out)
+    v = _variant(kind, behaviour, kl_coef, dpo_alpha, dpo_beta)
+    lib = _lib.load()
+    scratch = _zeros_scratch((scratch_key,), lib.stx_ppo_head_scratch_bytes(mb), dev)
+    _lib.check(lib.stx_ppo_variant_tanh_normal_head_grads(_p(head_out), _p(idx), int(row0), C.byref(hd), C.byref(v), _p(logp_old), _p(adv),
+                                                          _p(adv_stats), mb, A2 // 2, float(ent_coef), _p(d_head_out), _p(metrics), float(weight),
+                                                          _p(scratch), _stream()), "stx_ppo_variant_tanh_normal_head_grads")
+    return d_head_out, metrics
+
+
+def _variant_batch_checks(who, actor, critic, param_arena, batch, grad_arena, metrics, workspace):
+    _need_cuda(param_arena, batch.obs, batch.action, batch.log_prob, batch.value, batch.advantages, batch.targets, batch.adv_stats, batch.perm,
+               grad_arena, metrics, workspace)
+    if batch.perm is not None and batch.perm.dtype != torch.int32:
+        raise StxError(f"{who}: perm must be int32")
+    if batch.obs.dtype != torch.float32:
+        raise StxError(f"{who}: obs must be float32 (the KL-penalty and DPO losses run on the fp32 path)")
+    _, coff, total = arena_offsets(actor, critic)
+    if param_arena.numel() < total or grad_arena.numel() < total or metrics.numel() < 7:
+        raise StxError(f"{who}: arena too small or metrics below 7 floats")
+    return coff
+
+
+def ppo_penalty_minibatch_grads(actor: MlpSpec, critic: MlpSpec, param_arena: torch.Tensor, batch: PpoBatch, mb_off: int, mb: int,
+                                behaviour: torch.Tensor, kl_coef: float, clip_eps: float, ent_coef: float, vf_coef: float, standardize: bool,
+                                grad_arena: torch.Tensor, metrics: torch.Tensor, workspace: torch.Tensor, precision: int = STX_PREC_F32,
+                                grad_weight: float = 1.0, overwrite: bool = False) -> None:
+    """ppo_minibatch_grads with ff_ppo_penalty's actor loss (ff_ppo_penalty.py:149-210): behaviour (B, A) holds the behaviour
+    policy's logits per batch row; clip_eps clips only the value loss."""
+    coff = _variant_batch_checks("ppo_penalty_minibatch_grads", actor, critic, param_arena, batch, grad_arena, metrics, workspace)
+    if batch.action.dtype != torch.int32:
+        raise StxError("ppo_penalty_minibatch_grads: action must be int32")
+    if behaviour.shape != (batch.action.numel(), actor.sizes[-1]):
+        raise StxError(f"ppo_penalty_minibatch_grads: behaviour must be ({batch.action.numel()}, {actor.sizes[-1]})")
+    v = _variant(STX_PPO_KL_PENALTY, behaviour, kl_coef, 0.0, 0.0)
+    lib = _lib.load()
+    a, c, b = actor.c_struct(param_arena), critic.c_struct(param_arena[coff:]), batch.c_struct()
+    h = _lib.StxPpoHyper(float(clip_eps), float(ent_coef), float(vf_coef), int(bool(standardize)), int(bool(overwrite)), 0, None)
+    _lib.check(lib.stx_ppo_penalty_minibatch_grads(C.byref(a), C.byref(c), C.byref(b), C.byref(v), int(mb_off), int(mb), C.byref(h),
+                                                   float(grad_weight), _p(grad_arena), _p(metrics), int(precision), _p(workspace),
+                                                   workspace.numel(), _stream()), "stx_ppo_penalty_minibatch_grads")
+
+
+def ppo_variant_continuous_minibatch_grads(actor: MlpSpec, critic: MlpSpec, param_arena: torch.Tensor, batch: PpoBatch, mb_off: int, mb: int,
+                                           kind: int, clip_eps: float, ent_coef: float, vf_coef: float, standardize: bool,
+                                           grad_arena: torch.Tensor, metrics: torch.Tensor, workspace: torch.Tensor, minimum: float,
+                                           maximum: float, min_scale: float = 1e-3, behaviour: Optional[torch.Tensor] = None,
+                                           kl_coef: float = 0.0, dpo_alpha: float = 2.0, dpo_beta: float = 0.6, seed: int = 0,
+                                           offset: int = 0, dev_counter: Optional[torch.Tensor] = None,
+                                           eps_in: Optional[torch.Tensor] = None, eps_out: Optional[torch.Tensor] = None,
+                                           precision: int = STX_PREC_F32, grad_weight: float = 1.0, overwrite: bool = False) -> None:
+    """ppo_continuous_minibatch_grads with the actor loss of ff_ppo_penalty_continuous (kind STX_PPO_KL_PENALTY, behaviour (B, 2A)
+    head outputs) or ff_dpo_continuous (kind STX_PPO_DPO); entropy noise as in ppo_continuous_minibatch_grads."""
+    who = "ppo_variant_continuous_minibatch_grads"
+    coff = _variant_batch_checks(who, actor, critic, param_arena, batch, grad_arena, metrics, workspace)
+    B = int(batch.log_prob.numel())
+    if batch.action.shape != (B, actor.sizes[-1] // 2):
+        raise StxError(f"{who}: action must be float32 ({B}, {actor.sizes[-1] // 2})")
+    if behaviour is not None and behaviour.shape != (B, actor.sizes[-1]):
+        raise StxError(f"{who}: behaviour must be ({B}, {actor.sizes[-1]})")
+    hd = _tanh_normal_ppo(batch.action, minimum, maximum, min_scale, seed, offset, dev_counter, eps_in, eps_out)
+    v = _variant(kind, behaviour, kl_coef, dpo_alpha, dpo_beta)
+    lib = _lib.load()
+    a, c, b = actor.c_struct(param_arena), critic.c_struct(param_arena[coff:]), batch.c_struct()
+    b.action, b.B = None, B
+    h = _lib.StxPpoHyper(float(clip_eps), float(ent_coef), float(vf_coef), int(bool(standardize)), int(bool(overwrite)), 0, None)
+    _lib.check(lib.stx_ppo_variant_continuous_minibatch_grads(C.byref(a), C.byref(c), C.byref(b), C.byref(hd), C.byref(v), int(mb_off), int(mb),
+                                                              C.byref(h), float(grad_weight), _p(grad_arena), _p(metrics), int(precision),
+                                                              _p(workspace), workspace.numel(), _stream()),
+               "stx_ppo_variant_continuous_minibatch_grads")
+
+
 def sac_actor_seed(q1, q2, log_prob, log_alpha, dq1, dq2, metrics=None, weight: float = 1.0) -> None:
     _need_cuda(q1, q2, log_prob, log_alpha, dq1, dq2, metrics)
     _lib.check(_lib.load().stx_sac_actor_seed(_p(q1), _p(q2), _p(log_prob), _p(log_alpha), q1.numel(), _p(dq1), _p(dq2), _p(metrics), float(weight),

@@ -59,6 +59,15 @@ from stoix_b200.utils.total_timestep_checker import check_total_timesteps
 from stoix_b200.utils.training import make_learning_rate
 
 _METRIC_NAMES = ("actor_loss", "entropy", "value_loss", "advantages", "pred_value", "target_value")
+# The actor loss of the update: ppo_clip_loss (ff_ppo*), ppo_penalty_loss (ff_ppo_penalty*) or dpo_loss (ff_dpo_continuous).  The
+# variants report the reference's loss_info keys (ff_ppo_penalty.py:172-176,195-197; ff_dpo_continuous.py:166-169,187-189) as
+# (name, metrics slot) pairs; slot 6 is the KL divergence the penalty kernels accumulate.
+LOSS_VARIANTS = ("clip", "kl_penalty", "dpo")
+_VARIANT_METRICS = {
+    "clip": tuple((name, j) for j, name in enumerate(_METRIC_NAMES)),
+    "kl_penalty": (("actor_loss", 0), ("entropy", 1), ("kl_divergence", ops.METRIC_SLOT_KL), ("value_loss", 2)),
+    "dpo": (("actor_loss", 0), ("entropy", 1), ("value_loss", 2)),
+}
 
 
 def _world() -> Tuple[int, int]:
@@ -70,7 +79,8 @@ def _world() -> Tuple[int, int]:
 class _Shard:
     """Trajectory buffers of one (device, update-batch) shard: PPOTransition fields, time-major."""
 
-    def __init__(self, T: int, E: int, D: int, A: int, obs_dtype, device, normalize: bool = False, act_dim: int = 0):
+    def __init__(self, T: int, E: int, D: int, A: int, obs_dtype, device, normalize: bool = False, act_dim: int = 0,
+                 behaviour: bool = False):
         z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=device)
         self.obs = z(T + 1, E, D, dt=obs_dtype)      # row t = last_timestep.observation of step t
         self.next_obs = z(T, E, D, dt=obs_dtype)     # timestep.extras["next_obs"]   (ff_ppo.py:113)
@@ -92,6 +102,9 @@ class _Shard:
         self.advantages = z(T, E)
         self.targets = z(T, E)
         self.logits = z(E, A)                        # actor head output of one step: logits, or loc | scale pre-activation
+        # KL penalty: the head output of every rollout step is kept as the behaviour policy of the update (the rollout actor is
+        # the actor at the start of the update, ff_ppo_penalty.py:137, evaluated on the same rows the minibatches read)
+        self.behaviour = z(T, E, A) if behaviour else None
         self.perms = None  # (epochs, T*E) int32 shuffles of this update, allocated by the learner
         self.adv_stats: Optional[torch.Tensor] = None
 
@@ -117,12 +130,15 @@ def get_learner_fn(
     apply_fns: Tuple[ActorApply, CriticApply],
     update_fns: Tuple[Callable, Callable],
     config: DictConfig,
+    loss: str = "clip",
 ) -> LearnerFn[OnPolicyLearnerState]:
     """Get the learner function (ff_ppo.py:49-372).
 
     apply_fns: (actor_network.apply, critic_network.apply) bound methods; update_fns:
     (actor_optim.update, critic_optim.update) handles from stoix_b200.optim -- both are used for the
     network shapes / optimiser hyper-parameters they carry; the arithmetic runs in the fused kernels.
+    loss: the actor loss, one of LOSS_VARIANTS -- "clip" (ff_ppo, ff_ppo_continuous), "kl_penalty" (ff_ppo_penalty,
+    ff_ppo_penalty_continuous) or "dpo" (ff_dpo_continuous, tanh-Normal actor only).
     """
     actor_apply_fn, critic_apply_fn = apply_fns
     # The arithmetic of apply / update runs inside the fused kernels; what the learner needs from the four callables is the
@@ -154,6 +170,17 @@ def get_learner_fn(
     if tanh_head is not None and precision == ops.STX_PREC_BF16:
         raise ValueError("arch.precision=bf16 is not available with a tanh-Normal actor (NormalAffineTanhDistributionHead): the bf16 "
                          "tensor-core PPO kernels implement the Categorical head only; use arch.precision=f32")
+    if loss not in LOSS_VARIANTS:
+        raise ValueError(f"get_learner_fn: loss={loss!r}; expected one of {LOSS_VARIANTS}")
+    if loss != "clip" and precision == ops.STX_PREC_BF16:
+        raise ValueError(f"arch.precision=bf16 is not available with the {loss} actor loss: the bf16 tensor-core PPO kernels implement the "
+                         "clipped surrogate only; use arch.precision=f32")
+    if loss == "dpo" and tanh_head is None:
+        raise ValueError("the dpo actor loss needs a tanh-Normal actor (NormalAffineTanhDistributionHead); the reference has no discrete DPO")
+    kl_coef = float(sysc.kl_penalty_coef) if loss == "kl_penalty" else 0.0
+    dpo_alpha, dpo_beta = (float(sysc.alpha), float(sysc.beta)) if loss == "dpo" else (0.0, 0.0)
+    # ff_dpo_continuous.py:123 uses the raw reward; the clip and penalty systems scale it (ff_ppo_penalty.py:123)
+    reward_scale = 1.0 if loss == "dpo" else float(sysc.reward_scale)
 
     built: Dict[str, Any] = {}
 
@@ -167,7 +194,8 @@ def get_learner_fn(
         obs_dtype = torch.bfloat16 if precision == ops.STX_PREC_BF16 else torch.float32
         rs = getattr(state, "running_statistics", None)
         act_dim = tanh_head.action_dim if tanh_head is not None else 0
-        shards = [_Shard(T, E, D, A, obs_dtype, dev, normalize=rs is not None, act_dim=act_dim) for _ in range(U)]
+        shards = [_Shard(T, E, D, A, obs_dtype, dev, normalize=rs is not None, act_dim=act_dim, behaviour=loss == "kl_penalty")
+                  for _ in range(U)]
         decay = bool(sysc.decay_learning_rates)
         plan = ops.AdamPlan(
             [(0, sa.param_count, actor_opt.init_lr, actor_opt.max_grad_norm),
@@ -209,15 +237,16 @@ def get_learner_fn(
         a_tree = state.params.actor_params
         if b["rs"] is not None:  # normalise the observation with the PRE-update statistics (ff_ppo.py:90-94)
             ops.obs_normalize(sh.obs_raw[t], b["rs"].mean, b["rs"].std, out=sh.obs[t])
-        # SELECT ACTION (ff_ppo.py:97-101): logits -> sample -> log_prob
-        ops.mlp_forward(b["sa"], a_tree.flat, sh.obs[t], precision=precision, params_bf16=a_tree.flat_bf16, out=sh.logits, ws_key="learner")
+        # SELECT ACTION (ff_ppo.py:97-101): logits -> sample -> log_prob; the KL penalty keeps the head output as behaviour[t]
+        head = sh.logits if sh.behaviour is None else sh.behaviour[t]
+        ops.mlp_forward(b["sa"], a_tree.flat, sh.obs[t], precision=precision, params_bf16=a_tree.flat_bf16, out=head, ws_key="learner")
         if tanh_head is None:
-            ops.categorical(sh.logits, None, seeds[0] + u, t, b["roll_ctr"], out=(sh.action[t], sh.log_prob[t]))
+            ops.categorical(head, None, seeds[0] + u, t, b["roll_ctr"], out=(sh.action[t], sh.log_prob[t]))
         else:  # sample, then score the stored action by the inverse path the loss uses (ff_ppo_continuous.py:98-101)
             lo, hi, ms = tanh_head.minimum, tanh_head.maximum, tanh_head.min_scale
-            ops.tanh_normal_sample(sh.logits, lo, hi, ms, seed=seeds[0] + u, offset=t, dev_counter=b["roll_ctr"], action_out=sh.action[t],
+            ops.tanh_normal_sample(head, lo, hi, ms, seed=seeds[0] + u, offset=t, dev_counter=b["roll_ctr"], action_out=sh.action[t],
                                    want_eps=False)
-            ops.tanh_normal_log_prob(sh.logits, sh.action[t], lo, hi, ms, out=sh.log_prob[t])
+            ops.tanh_normal_log_prob(head, sh.action[t], lo, hi, ms, out=sh.log_prob[t])
         # STEP ENVIRONMENT (ff_ppo.py:104-116)
         if has_step_into:
             env.step_into(state.env_state[u], sh.action[t], sh.step_out(t), t)
@@ -305,7 +334,7 @@ def get_learner_fn(
             sh: _Shard = built["shards"][u]
             _, _, sh.adv_stats = ops.gae_ppo(
                 sh.reward, sh.value, sh.bootstrap_value, sh.done, sh.truncated, float(sysc.gamma),
-                float(sysc.gae_lambda), float(sysc.reward_scale), 1 if sysc.standardize_advantages else 0,
+                float(sysc.gae_lambda), reward_scale, 1 if sysc.standardize_advantages else 0,
                 out=(sh.advantages, sh.targets),
             )
 
@@ -356,6 +385,22 @@ def get_learner_fn(
                                              b["plan"], a_tree.arena_mu, a_tree.arena_nu, b["arena_bf16"])
                     continue
                 for u in range(U):  # vmap over "batch" + pmean("batch") (ff_ppo.py:253-256); first shard overwrites
+                    sh = b["shards"][u]
+                    behaviour = sh.behaviour.view(B, -1) if sh.behaviour is not None else None
+                    if loss != "clip" and tanh_head is not None:
+                        # ff_ppo_penalty_continuous.py:149-179 / ff_dpo_continuous.py:148-170, entropy noise as below
+                        kind = ops.STX_PPO_KL_PENALTY if loss == "kl_penalty" else ops.STX_PPO_DPO
+                        ops.ppo_variant_continuous_minibatch_grads(
+                            sa, sc, b["arena"], batches[u], i * mb, mb, kind, float(sysc.clip_eps), float(sysc.ent_coef), float(sysc.vf_coef),
+                            bool(sysc.standardize_advantages), grads, metrics[ep, i], b["ws"], tanh_head.minimum, tanh_head.maximum,
+                            tanh_head.min_scale, behaviour=behaviour, kl_coef=kl_coef, dpo_alpha=dpo_alpha, dpo_beta=dpo_beta,
+                            seed=seeds[0] + u, offset=ep * nmb + i, dev_counter=b["ent_ctr"], grad_weight=1.0 / U, overwrite=(u == 0))
+                        continue
+                    if loss == "kl_penalty":  # ff_ppo_penalty.py:149-210
+                        ops.ppo_penalty_minibatch_grads(sa, sc, b["arena"], batches[u], i * mb, mb, behaviour, kl_coef, float(sysc.clip_eps),
+                                                        float(sysc.ent_coef), float(sysc.vf_coef), bool(sysc.standardize_advantages), grads,
+                                                        metrics[ep, i], b["ws"], grad_weight=1.0 / U, overwrite=(u == 0))
+                        continue
                     if tanh_head is not None:
                         # entropy noise of this minibatch: (shard seed, row, call = ep * nmb + i + *ent_ctr)
                         ops.ppo_continuous_minibatch_grads(sa, sc, b["arena"], batches[u], i * mb, mb, float(sysc.clip_eps), float(sysc.ent_coef),
@@ -458,7 +503,7 @@ def get_learner_fn(
         # the observation the next learn() call starts from
         new_ts = [learner_state.timestep[u]._replace(observation=b["shards"][u].env_obs[T]) for u in range(U)]
         learner_state = learner_state._replace(timestep=new_ts)
-        train_metrics = {name: train_out[..., j] for j, name in enumerate(_METRIC_NAMES)}
+        train_metrics = {name: train_out[..., j] for name, j in _VARIANT_METRICS[loss]}
         return AnakinExperimentOutput(learner_state=learner_state, episode_metrics=ep_out, train_metrics=train_metrics)
 
     learner_fn.built = built  # exposed for tests / bench (trajectory buffers, graph handle)
@@ -497,10 +542,11 @@ def build_learner(
     env: Environment, keys: Tuple[int, int, int], config: DictConfig,
     action_head_kwargs: Callable[[Environment, DictConfig], Dict[str, Any]],
     random_actions: Callable[[DictConfig, int, torch.Generator, Any], torch.Tensor],
+    loss: str = "clip",
 ) -> Tuple[LearnerFn[OnPolicyLearnerState], Actor, OnPolicyLearnerState]:
     """The body of learner_setup shared by the PPO variants.  `action_head_kwargs(env, config)` reads the action space, records
     it in config.system and returns the action head's constructor arguments; `random_actions(config, E, gen, device)` draws the
-    uniform actions of the observation-normalisation warm-up."""
+    uniform actions of the observation-normalisation warm-up; `loss` is get_learner_fn's actor-loss variant."""
     rank, world = _world()
     device = torch.device("cuda", torch.cuda.current_device())
     n_devices = world
@@ -553,7 +599,7 @@ def build_learner(
 
     apply_fns = (actor_network.apply, critic_network.apply)
     update_fns = (actor_optim.update, critic_optim.update)
-    learn = get_learner_fn(env, apply_fns, update_fns, config)
+    learn = get_learner_fn(env, apply_fns, update_fns, config, loss=loss)
 
     # Initialise environment states and timesteps across update-batch shards (ff_ppo.py:492-501).
     U, E = int(config.arch.update_batch_size), int(config.arch.num_envs)
@@ -586,7 +632,7 @@ def build_learner(
     )
     # If normalizing observations, initialize running statistics from warm-up rollouts (ff_ppo.py:539-549); this adds a
     # `running_statistics` field to the learner state.
-    if config.system.normalize_observations:
+    if config.system.get("normalize_observations", False):  # ff_dpo.yaml has no such key
         from stoix_b200.utils import running_statistics as rstat
 
         warmup_observations = _collect_obs_norm_rollouts(env, key, config, random_actions)
