@@ -50,11 +50,16 @@ constexpr int kWTile = 64;               // rows per warpgroup tile
 constexpr int kFbThreads = 256;          // two warpgroups
 
 // ---- K3a shared-memory map ------------------------------------------------------------------------
-constexpr uint32_t kOffX = kImgWBytes;               // 2 warpgroups x 8 KB
-constexpr uint32_t kOffBias = kOffX + 2 * 8192;      // b0[256] b1[256] b2[16]
+// Each warpgroup has two stages of its tile inputs: the tile being computed and the next one, gathered with cp.async meanwhile.
+constexpr uint32_t kOffX = kImgWBytes;               // [2 warpgroups][2 stages] X tile, 8 KB
+constexpr uint32_t kOffLoss = kOffX + 4 * 8192;      // [2 warpgroups][2 stages][3][64] per-row loss inputs (see gather_tile)
+constexpr uint32_t kLossStageBytes = 3 * 64 * 4;
+constexpr uint32_t kOffBias = kOffLoss + 4 * kLossStageBytes;  // b0[256] b1[256] b2[16]
 constexpr uint32_t kOffDb = kOffBias + 528 * 4;      // [8 warps][db0[256] db1[256] db2[16]] accumulators
 constexpr uint32_t kOffBar = kOffDb + 8 * 528 * 4;
 constexpr uint32_t kFbSmemBytes = kOffBar + 64 + 1024;
+// + the kernel's static s_mw[8][6]; 227 KB is the most a block may use on sm_90
+static_assert(kFbSmemBytes + 8 * 6 * 4 <= 227 * 1024, "K3a shared memory exceeds the per-block limit");
 
 struct FbNet {
   const __nv_bfloat16* w2;   // [256 x A] bf16
@@ -97,12 +102,23 @@ __device__ __forceinline__ __nv_bfloat16* tiled_ptr(__nv_bfloat16* base, int64_t
 __device__ __forceinline__ int mask_word(int h, int i) { return 2 * h + (i >> 4); }
 __device__ __forceinline__ uint32_t mask_bit(int i, int e) { return (uint32_t)(2 * (i & 15) + e); }
 
-// Stores half h of a packed 64 x 256 register operand (rows row0, row0 + 8 of the thread; see stx_tc_ptx.cuh) to the tiled layout.
-__device__ __forceinline__ void store_act(__nv_bfloat16* base, const uint32_t (&a)[64], int h, int64_t row0, int lane, uint64_t pol) {
+// Stores half h of a packed 64 x 256 register operand (a: its 32 words of half h; rows row0, row0 + 8 of the thread, see
+// stx_tc_ptx.cuh) to the tiled layout.
+__device__ __forceinline__ void store_act(__nv_bfloat16* base, const uint32_t* a, int h, int64_t row0, int lane, uint64_t pol) {
 #pragma unroll
-  for (int i = 32 * h; i < 32 * h + 32; ++i)
-    st_hint(reinterpret_cast<uint32_t*>(tiled_ptr(base, row0 + 8 * (i & 1), 8 * (i >> 1) + 2 * (lane & 3), 32)), a[i], pol);
+  for (int i = 0; i < 32; ++i)
+    st_hint(reinterpret_cast<uint32_t*>(tiled_ptr(base, row0 + 8 * (i & 1), 128 * h + 8 * (i >> 1) + 2 * (lane & 3), 32)), a[i], pol);
 }
+
+// cp.async global -> shared, L2 only (every gathered row is read once here); src_bytes = 0 zero-fills the 16 bytes
+__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src, uint32_t src_bytes) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async4(uint32_t dst, const void* src) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(dst), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
 // One reduce-scatter step of colsum_half at lane distance S, on entries k, k + 4, k + 8, ... of one class (v[j] = entry k + 4 j):
 // of the 2 S entries still held, lane l keeps half (l & S) and adds its partner's copy of it.  S is a template parameter so
@@ -221,6 +237,33 @@ __global__ void __launch_bounds__(kFbThreads, 1)
   const CUtensorMap* tmW0 = which == 0 ? &tmW0a : &tmW0c;
   const CUtensorMap* tmW1 = which == 0 ? &tmW1a : &tmW1c;
 
+  const uint32_t xs0 = sbase + kOffX + wg * 2 * 8192;  // this warpgroup's X stages
+  float* li0 = reinterpret_cast<float*>(smem + kOffLoss + wg * 2 * kLossStageBytes);  // and its loss-input stages
+  const int dchunks = p.D >> 3;  // 16-byte chunks per observation row
+  // Starts the gather of a tile into stage s as one cp.async group: two threads per row, 4 chunks of 16 bytes each (zeros past
+  // D), and the row's loss inputs, stage layout [3][64]: action | logp_old | adv (actor), - | v_old | tgt (critic).
+  auto gather_tile = [&](int tile, int s) {
+    const int r = t >> 1, hf = t & 1;
+    const int64_t mrow = (int64_t)tile * kWTile + r;
+    const int64_t src = p.idx ? (int64_t)p.idx[mrow] : p.row0 + mrow;
+    const __nv_bfloat16* row = p.obs + src * p.D;
+    const uint32_t xd = xs0 + s * 8192 + r * 128;
+#pragma unroll
+    for (int cc = 0; cc < 4; ++cc) {
+      const int c = hf * 4 + cc;
+      cp_async16(xd + ((c ^ (r & 7)) << 4), c < dchunks ? row + c * 8 : row, c < dchunks ? 16u : 0u);  // Swizzle<3,4,3>
+    }
+    const uint32_t ld = smem_u32(li0 + s * 192 + r);
+    if (net.is_actor) {
+      if (hf == 0) cp_async4(ld, p.action + src), cp_async4(ld + 256, p.logp_old + src);
+      else cp_async4(ld + 512, p.adv + src);
+    } else {
+      if (hf == 0) cp_async4(ld + 256, p.v_old + src);
+      else cp_async4(ld + 512, p.tgt + src);
+    }
+    cp_async_commit();
+  };
+
   if (threadIdx.x == 0) {
     mbar_init(w_full, 1);
     fence_barrier_init();
@@ -230,6 +273,7 @@ __global__ void __launch_bounds__(kFbThreads, 1)
   griddep_launch();  // K3b cannot co-reside with this CTA anyway; lets its launch be queued early
   for (int i = threadIdx.x; i < 8 * 528; i += kFbThreads) s_db[i] = 0.f;
   griddep_wait();  // everything above overlapped the previous optimiser kernel; the weights below are its output
+  if (my_tiles > 0) gather_tile(g, 0);  // the permutation and the rollout data are written earlier in the chain too
   if (threadIdx.x == 0) {
     mbar_arrive_expect_tx(w_full, 32768 + 131072);
     const uint64_t pol_keep = l2_evict_last();  // the bf16 weights (K4's output) stay L2-resident for all CTAs and the next step
@@ -242,61 +286,51 @@ __global__ void __launch_bounds__(kFbThreads, 1)
 
   float m_acc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};  // actor_loss, entropy, value_loss, adv, pred value, target
   float* dbw = s_db + warp * 528;
-  uint8_t* xs = smem + kOffX + wg * 8192;
   const float inv_m = p.inv_m;
   float adv_mean = 0.f, adv_rstd = 1.f;
   if (p.adv_stats) adv_mean = p.adv_stats[0], adv_rstd = p.adv_stats[1];
-  const int dchunks = p.D >> 3;  // 16-byte chunks per observation row
   mbar_wait(w_full, 0, 2);
 
   for (int it = 0; it < my_tiles; ++it) {
-    const int tile = g + it * n_wg;
-    // ---------------- gather: two threads per row, 4 chunks of 16 bytes each ----------------
-    {
-      const int r = t >> 1, hf = t & 1;
-      const int64_t mrow = (int64_t)tile * kWTile + r;
-      const int64_t src = p.idx ? (int64_t)p.idx[mrow] : p.row0 + mrow;
-      uint4 v[4];
-#pragma unroll
-      for (int cc = 0; cc < 4; ++cc) {
-        const int c = hf * 4 + cc;
-        v[cc] = c < dchunks ? *reinterpret_cast<const uint4*>(p.obs + src * p.D + c * 8) : make_uint4(0u, 0u, 0u, 0u);
-      }
-      wg_sync(1 + wg);  // every warp of this warpgroup has finished layer 0 of the previous tile (X stage free)
-#pragma unroll
-      for (int cc = 0; cc < 4; ++cc) {
-        const int c = hf * 4 + cc;
-        *reinterpret_cast<uint4*>(xs + r * 128 + ((c ^ (r & 7)) << 4)) = v[cc];  // Swizzle<3,4,3>
-        if (which == 0) st_hint(reinterpret_cast<uint4*>(tiled_ptr(p.xg, mrow, 8 * c, 8)), v[cc], pol_stream);
-      }
-      fence_async_proxy();
-      wg_sync(1 + wg);
-    }
-    // ---------------- per-row loss inputs of rows row0 and row0 + 8 (consumed in E2) ----------------
-    const int64_t row0 = (int64_t)tile * kWTile + wq * 16 + (lane >> 2);
-    int pf_a[2] = {0, 0};
-    float pf_0[2] = {0.f, 0.f}, pf_1[2] = {0.f, 0.f};
-#pragma unroll
-    for (int rr = 0; rr < 2; ++rr) {
-      const int64_t m = row0 + 8 * rr;
-      const int64_t src = p.idx ? (int64_t)p.idx[m] : p.row0 + m;
-      if (net.is_actor) pf_a[rr] = p.action[src], pf_0[rr] = p.logp_old[src], pf_1[rr] = p.adv[src];
-      else pf_0[rr] = p.v_old[src], pf_1[rr] = p.tgt[src];
-    }
-    float acc[64];
+    const int tile = g + it * n_wg, s = it & 1;
+    const uint32_t xs = xs0 + s * 8192;
+    const float* li = li0 + s * 192;
+    cp_async_wait_all();
+    fence_async_proxy();  // this thread's cp.async writes (generic proxy) -> the wgmma reads of X (async proxy)
+    wg_sync(1 + wg);      // the whole tile has landed, and every warp is done with the previous tile and so with stage s ^ 1
+    const int64_t row0 = (int64_t)tile * kWTile + wq * 16 + (lane >> 2);  // rows row0 and row0 + 8 of this thread
+    float acc[64], acc1[64];
     uint32_t a1[64], a2[64];
     wg_zero(acc);
+    wg_zero(acc1);
     // ---------------- G0 / E0, G1 / E1: hidden layers ----------------
+    // G0 issues both halves before it waits for the first, so that half 1's MMAs run during half 0's epilogue and the gather
+    // below.  (The later 256-wide GEMMs run one half at a time: a second accumulator does not fit next to h1 and h2 there.)
+    gemm_x_w0_issue(acc, xs, sbase, 0);
+    gemm_x_w0_issue(acc1, xs, sbase, 1);
+    if (which == 0) {  // the gathered rows for K3b's dW0, copied from the X stage
+      const int r = t >> 1, hf = t & 1;
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      gemm_x_w0(acc, smem_u32(xs), sbase, h);
-      epi_bias_relu(acc, s_b0, h, a1, lane);
+      for (int cc = 0; cc < 4; ++cc) {
+        const int c = hf * 4 + cc;
+        const uint4 v = *reinterpret_cast<const uint4*>(smem + (xs - sbase) + r * 128 + ((c ^ (r & 7)) << 4));
+        st_hint(reinterpret_cast<uint4*>(tiled_ptr(p.xg, (int64_t)tile * kWTile + r, 8 * c, 8)), v, pol_stream);
+      }
     }
+    if (it + 1 < my_tiles) gather_tile(tile + n_wg, s ^ 1);
+    wg_wait<1>();
+    wg_fence_acc(acc);
+    epi_bias_relu(acc, s_b0, 0, a1, lane);
+    wg_wait_all(acc1);
+    epi_bias_relu(acc1, s_b0, 1, a1, lane);
+    // G1's MMAs read acc although its first k-step does not accumulate: zeroing it here, not before G1, would keep half 0's
+    // values live next to acc1 and a1 through E0 (ptxas then serialises every wgmma of the kernel, C7512)
+    wg_zero(acc);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       gemm_a_w1(acc, a1, sbase, h);
       epi_bias_relu(acc, s_b1, h, a2, lane);
-      store_act(net.h2, a2, h, row0, lane, pol_stream);
+      store_act(net.h2, &a2[32 * h], h, row0, lane, pol_stream);
     }
     // ---------------- G2 / E2: head + loss + d(head) ----------------
     float z[8];
@@ -307,12 +341,13 @@ __global__ void __launch_bounds__(kFbThreads, 1)
     for (int rr = 0; rr < 2; ++rr) {
       const int ix[4] = {2 * rr, 2 * rr + 1, 4 + 2 * rr, 5 + 2 * rr};
       const int col[4] = {2 * q4, 2 * q4 + 1, 8 + 2 * q4, 9 + 2 * q4};
+      const int rl = wq * 16 + (lane >> 2) + 8 * rr;  // the row's index in the tile's loss-input stage
       if (net.is_actor) {
         float zz[4], d4[4], loss, ent;
 #pragma unroll
         for (int k = 0; k < 4; ++k) zz[k] = z[ix[k]] + s_b2[col[k]];
-        const float adv = (pf_1[rr] - adv_mean) * adv_rstd;
-        actor_head_quad(zz, col, net.A, pf_a[rr], pf_0[rr], adv, p.clip_eps, p.ent_coef, inv_m, d4, loss, ent);
+        const float adv = (li[128 + rl] - adv_mean) * adv_rstd;
+        actor_head_quad(zz, col, net.A, __float_as_int(li[rl]), li[64 + rl], adv, p.clip_eps, p.ent_coef, inv_m, d4, loss, ent);
 #pragma unroll
         for (int k = 0; k < 4; ++k) dz[ix[k]] = d4[k];
         if (q4 == 0) m_acc[0] += loss, m_acc[1] += ent, m_acc[3] += adv;
@@ -320,7 +355,7 @@ __global__ void __launch_bounds__(kFbThreads, 1)
 #pragma unroll
         for (int k = 0; k < 4; ++k) dz[ix[k]] = 0.f;
         if (q4 == 0) {  // the value is column 0
-          const float v = z[2 * rr] + s_b2[0], vo = pf_0[rr], tg = pf_1[rr];
+          const float v = z[2 * rr] + s_b2[0], vo = li[64 + rl], tg = li[128 + rl];
           const float diff = v - vo;
           const float vclip = vo + fminf(fmaxf(diff, -p.clip_eps), p.clip_eps);
           const float e1 = v - tg, e2 = vclip - tg, q1 = e1 * e1, q2 = e2 * e2;
@@ -379,7 +414,7 @@ __global__ void __launch_bounds__(kFbThreads, 1)
         const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(&pk);
         acc[2 * i] = __bfloat162float(v.x), acc[2 * i + 1] = __bfloat162float(v.y);  // db0 sums the bf16 dh1 that K3b's dW0 uses
       }
-      store_act(net.dh1, a1, h, row0, lane, pol_stream);
+      store_act(net.dh1, &a1[32 * h], h, row0, lane, pol_stream);
       colsum_half(acc, dbw, h, lane);  // db0
     }
   }
@@ -491,12 +526,14 @@ __device__ __forceinline__ void dw_consume(uint8_t* smem, uint64_t* full, uint64
       }
     }
     wg_commit();
-    wg_wait<0>();
-    wg_fence_acc(acc[0]);
-    wg_fence_acc(acc[1]);
+    // chunk k stays in flight while this warp waits for chunk k + 1: only chunk k - 1's stage is known to be read
+    wg_wait<1>();
     __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[s]);
+    if (k > 0 && lane == 0) mbar_arrive(&empty[(k - 1) % kDwStages]);
   }
+  wg_wait<0>();
+  wg_fence_acc(acc[0]);
+  wg_fence_acc(acc[1]);
   // partial layout [N/4][256 rows][4]: element (m, c) at ((c/4) * 256 + m) * 4 + c % 4
   const uint64_t pol_keep = l2_evict_last();  // the reduce kernel reads these next: keep them in L2 under the activation stream
   float* out = job.part + (int64_t)cta * 256 * N;
@@ -539,12 +576,15 @@ __device__ __forceinline__ void dw1_consume(uint8_t* smem, uint64_t* img_full, u
         wg_mma_ss_n128<1, 1>(acc[nh], da, wg_desc(dh2 + nh * 16384 + ks * 256, 128, 1024, WG_INTERLEAVE), (k > 0 || ks > 0) ? 1u : 0u);
     }
     wg_commit();
-    wg_wait<0>();
-    wg_fence_acc(acc[0]);
-    wg_fence_acc(acc[1]);
+    // as dw_consume: release chunk k - 1's image once its MMAs are done, with chunk k still in flight.  The rebuild of chunk
+    // k + 1 waits for exactly that release (the image it overwrites is chunk k - 1's).
+    wg_wait<1>();
     __syncwarp();
-    if (lane == 0) mbar_arrive(&img_empty[b]);
+    if (k > 0 && lane == 0) mbar_arrive(&img_empty[b ^ 1]);
   }
+  wg_wait<0>();
+  wg_fence_acc(acc[0]);
+  wg_fence_acc(acc[1]);
   const uint64_t pol_keep = l2_evict_last();
   const int r = job.m0 + wg * 64 + wq * 16 + (lane >> 2);
 #pragma unroll

@@ -260,21 +260,34 @@ __device__ __forceinline__ void wg_zero(float (&d)[R]) {
   for (int i = 0; i < R; ++i) d[i] = 0.f;
 }
 
+// waits for every committed MMA group of the warpgroup, the last of which writes acc
+__device__ __forceinline__ void wg_wait_all(float (&acc)[64]) {
+  wg_wait<0>();
+  wg_fence_acc(acc);
+}
+
 // acc = X * W0[:, 128 h .. 128 h + 127]   (K = 64).  dx: K-major descriptor of the 64 x 64 X tile, advanced by x_kstep bytes
-// per 16 columns; w0_img: W0 image (layout above).
-__device__ __forceinline__ void gemm_x_w0_at(float (&acc)[64], uint64_t dx, uint32_t x_kstep, uint32_t w0_img, int h) {
+// per 16 columns; w0_img: W0 image (layout above).  The _issue forms commit the MMAs as one group and return without waiting
+// for it (the caller waits, e.g. with wg_wait_all); the others wait.  Both run the same MMAs.
+__device__ __forceinline__ void gemm_x_w0_at_issue(float (&acc)[64], uint64_t dx, uint32_t x_kstep, uint32_t w0_img, int h) {
   const uint64_t db = wg_desc(w0_img + h * 16384, 8192, 1024, WG_SW128);
   wg_fence_acc(acc);
   wg_fence();
 #pragma unroll
   for (int k = 0; k < 4; ++k) wg_mma_ss_n128<0, 1>(acc, wg_adv(dx, k * x_kstep), wg_adv(db, k * 2048), k > 0);
   wg_commit();
-  wg_wait<0>();
-  wg_fence_acc(acc);
+}
+__device__ __forceinline__ void gemm_x_w0_at(float (&acc)[64], uint64_t dx, uint32_t x_kstep, uint32_t w0_img, int h) {
+  gemm_x_w0_at_issue(acc, dx, x_kstep, w0_img, h);
+  wg_wait_all(acc);
 }
 // X as the 128B-swizzled tile of the layout above
+__device__ __forceinline__ void gemm_x_w0_issue(float (&acc)[64], uint32_t s_x, uint32_t sbase, int h) {
+  gemm_x_w0_at_issue(acc, wg_desc(s_x, 16, 1024, WG_SW128), 32, sbase + kImgW0, h);
+}
 __device__ __forceinline__ void gemm_x_w0(float (&acc)[64], uint32_t s_x, uint32_t sbase, int h) {
-  gemm_x_w0_at(acc, wg_desc(s_x, 16, 1024, WG_SW128), 32, sbase + kImgW0, h);
+  gemm_x_w0_issue(acc, s_x, sbase, h);
+  wg_wait_all(acc);
 }
 // acc = A * W1[:, 128 h ..]   (A: 64 x 256 in registers, 16 K blocks of 4 bf16x2)
 __device__ __forceinline__ void gemm_a_w1(float (&acc)[64], const uint32_t (&a)[64], uint32_t sbase, int h) {
