@@ -1,8 +1,7 @@
-// K1 (fp32 path) MLP forward, categorical head ops, and K3 (fp32 path) PPO minibatch gradients.
-// The bf16 wgmma implementations live in stx_tc_mlp.cu and are dispatched from here by precision.
+// K1 (fp32 path) MLP forward / backward, the categorical sampler, and the networks of the fp32 PPO minibatch (whose losses live
+// in stx_ppo_fp32.cu).  The bf16 wgmma implementations live in stx_tc_mlp.cu and are dispatched from here by precision.
 #include "stx_common.cuh"
 #include "stx_ppo_halves.cuh"
-#include "stx_ppo_loss.cuh"
 #include "stx_simt_gemm.cuh"
 
 namespace stx {
@@ -12,10 +11,6 @@ size_t tc_mlp_forward_workspace_bytes(const StxMlp* mlp, int64_t M);
 int tc_mlp_forward(const StxMlp* mlp, const void* x, int64_t ldx, const int32_t* row_idx, int64_t M,
                    float* out, void* ws, size_t ws_bytes, cudaStream_t st);
 size_t tc_ppo_workspace_bytes(const StxMlp* actor, const StxMlp* critic, int64_t mb);
-int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxPpoBatch* batch,
-                           int64_t mb_off, int64_t mb, const StxPpoHyper* hyper, float grad_weight,
-                           float* grad_arena, float* metrics, void* ws, size_t ws_bytes,
-                           cudaStream_t st, const StxFusedAdam* opt);
 
 namespace {
 
@@ -272,8 +267,8 @@ int simt_backward(const StxMlp* m, const float* x, int64_t ldx, const int32_t* r
 
 }  // namespace
 
-// ---- halves of the fp32 PPO minibatch shared with other policy heads (stx_ppo_continuous.cu) ----
-// Both carve `workspace` exactly as stx_ppo_minibatch_grads does, so one stx_ppo_workspace_bytes() workspace serves either net.
+// ---- the networks of the fp32 PPO minibatch (stx_ppo_fp32.cu) ----
+// Both carve `workspace` the same way, so one stx_ppo_workspace_bytes() workspace serves either net.
 int simt_check_mlp(const StxMlp* m, const char* who) { return check_mlp(m, who); }
 
 int simt_net_forward(const StxMlp* m, const float* x, int64_t ldx, const int32_t* idx, int64_t mb, void* workspace, SimtHeadBufs* out,
@@ -287,26 +282,6 @@ int simt_net_backward(const StxMlp* m, const float* x, int64_t ldx, const int32_
                       float* net_grad, int overwrite, cudaStream_t st) {
   SimtPpoWs ws = carve(m, mb, reinterpret_cast<char*>(workspace));
   return simt_backward(m, x, ldx, idx, mb, ws, grad_weight, net_grad, overwrite, st);
-}
-
-// Critic half of _update_minibatch (ff_ppo.py:215-235, 244-247): forward, clipped value loss, backward into grad_arena + coff.
-int simt_ppo_critic_grads(const StxMlp* critic, const StxPpoBatch* b, int64_t mb_off, int64_t mb, const StxPpoHyper* h, float grad_weight,
-                          float* net_grad, float* metrics, void* workspace, cudaStream_t st) {
-  const int D = critic->sizes[0];
-  const float* obs = reinterpret_cast<const float*>(b->obs);
-  const int32_t* idx = b->perm ? b->perm + mb_off : nullptr;
-  const float* x = idx ? obs : obs + mb_off * (int64_t)D;  // without a permutation: the contiguous row range from mb_off
-  SimtPpoWs ws = carve(critic, mb, reinterpret_cast<char*>(workspace));
-  if (int rc = simt_forward(critic, x, D, idx, mb, ws.acts, ws.hacts, ws.stats, ws.head, st)) return rc;
-  LossArgs g{};
-  g.logits = nullptr, g.value = ws.head, g.value_ld = 1, g.idx = idx, g.row0 = mb_off;
-  g.action = b->action, g.logp_old = b->log_prob, g.v_old = b->value, g.adv = b->advantages, g.tgt = b->targets;
-  g.adv_stats = h->standardize_advantages ? b->adv_stats : nullptr, g.dlogits = nullptr, g.dvalue = ws.dhead, g.mb = mb, g.A = 0;
-  g.clip_eps = h->clip_eps, g.ent_coef = h->ent_coef, g.vf_coef = h->vf_coef;
-  g.partials = ws.loss_partials, g.counter = ws.counter, g.metrics = metrics, g.weight = grad_weight;
-  ppo_loss_grad_kernel<<<(unsigned)((mb + 255) / 256), 256, 0, st>>>(g);
-  STX_LAUNCH_OK();
-  return simt_backward(critic, x, D, idx, mb, ws, grad_weight, net_grad, h->overwrite_grads, st);
 }
 
 }  // namespace stx
@@ -380,34 +355,6 @@ extern "C" int stx_mlp_backward(const StxMlp* m, const float* x, int64_t ldx, co
   return simt_backward(m, x, ldx, row_idx, M, ws, grad_weight, net_grad, overwrite, st, d_input);
 }
 
-// ---- PPO loss heads on precomputed network outputs (the recurrent system runs its networks outside the fused PPO kernels) ----
-extern "C" size_t stx_ppo_head_scratch_bytes(int64_t mb) { return 256 + (size_t)((mb + 255) / 256) * 6 * sizeof(double); }
-
-extern "C" int stx_ppo_head_grads(const float* logits, const float* value, const int32_t* idx, int64_t row0, const int32_t* action,
-                                  const float* logp_old, const float* v_old, const float* adv, const float* targets, const float* adv_stats,
-                                  int64_t mb, int A, float clip_eps, float ent_coef, float vf_coef, float* d_logits, float* d_value, float* metrics,
-                                  float weight, void* scratch, void* stream) {
-  STX_REQUIRE((logits || value) && action && logp_old && v_old && adv && targets && metrics && scratch && mb > 0, STX_E_ARG,
-              "stx_ppo_head_grads: null pointer or mb=%lld", (long long)mb);
-  STX_REQUIRE(!logits || (d_logits && A > 0 && A <= kMaxActions), STX_E_SHAPE, "stx_ppo_head_grads: A=%d (max %d) / null d_logits", A, kMaxActions);
-  STX_REQUIRE(!value || d_value, STX_E_ARG, "stx_ppo_head_grads: null d_value");
-  cudaStream_t st = (cudaStream_t)stream;
-  for (int pass = 0; pass < 2; ++pass) {  // actor then critic: each is one launch of the kernel the fused fp32 path uses
-    if ((pass == 0 && !logits) || (pass == 1 && !value)) continue;
-    LossArgs g{};
-    g.logits = pass == 0 ? logits : nullptr, g.value = pass == 1 ? value : nullptr, g.value_ld = 1, g.idx = idx, g.row0 = row0;
-    g.action = action, g.logp_old = logp_old, g.v_old = v_old, g.adv = adv, g.tgt = targets, g.adv_stats = adv_stats;
-    g.dlogits = d_logits, g.dvalue = d_value, g.mb = mb, g.A = pass == 0 ? A : 0;
-    g.clip_eps = clip_eps, g.ent_coef = ent_coef, g.vf_coef = vf_coef;
-    g.counter = reinterpret_cast<unsigned int*>(scratch);
-    g.partials = reinterpret_cast<double*>(reinterpret_cast<char*>(scratch) + 256);
-    g.metrics = metrics, g.weight = weight;
-    ppo_loss_grad_kernel<<<(unsigned)((mb + 255) / 256), 256, 0, st>>>(g);
-    STX_LAUNCH_OK();
-  }
-  return STX_OK;
-}
-
 extern "C" int stx_categorical(const float* logits, int64_t E, int A, int sample, uint64_t seed,
                                uint64_t offset, const uint64_t* dev_counter, int32_t* action,
                                float* log_prob, float* entropy, void* stream) {
@@ -432,81 +379,4 @@ extern "C" size_t stx_ppo_workspace_bytes(const StxMlp* actor, const StxMlp* cri
   if (precision == STX_PREC_BF16) return tc_ppo_workspace_bytes(actor, critic, mb);
   const size_t a = carve(actor, mb, nullptr).bytes, c = carve(critic, mb, nullptr).bytes;
   return (a > c ? a : c);
-}
-
-extern "C" int stx_ppo_minibatch_update(const StxMlp* actor, const StxMlp* critic, const StxPpoBatch* b, int64_t mb_off, int64_t mb,
-                                        const StxPpoHyper* h, float grad_weight, float* grad_arena, float* metrics, void* workspace,
-                                        size_t workspace_bytes, const StxFusedAdam* opt, void* stream) {
-  if (int rc = check_mlp(actor, "stx_ppo_minibatch_update(actor)")) return rc;
-  if (int rc = check_mlp(critic, "stx_ppo_minibatch_update(critic)")) return rc;
-  STX_REQUIRE(b && h && grad_arena && metrics && workspace && opt, STX_E_ARG, "stx_ppo_minibatch_update: null pointer");
-  STX_REQUIRE(b->obs && b->action && b->log_prob && b->value && b->advantages && b->targets, STX_E_ARG,
-              "stx_ppo_minibatch_update: null batch field");
-  STX_REQUIRE(opt->param_arena && opt->mu && opt->nu && opt->counts && opt->segs && opt->scratch, STX_E_ARG,
-              "stx_ppo_minibatch_update: null optimiser field");
-  STX_REQUIRE(opt->nseg == 2, STX_E_SHAPE, "stx_ppo_minibatch_update: nseg=%d (segment 0 = actor arena, 1 = critic arena)", opt->nseg);
-  STX_REQUIRE(opt->hyper.steps_per_update > 0 && opt->hyper.num_updates > 0, STX_E_ARG,
-              "stx_ppo_minibatch_update: steps_per_update/num_updates must be positive");
-  STX_REQUIRE(mb > 0 && mb_off >= 0 && mb_off + mb <= b->B, STX_E_SHAPE, "stx_ppo_minibatch_update: minibatch [%lld,%lld) outside batch %lld",
-              (long long)mb_off, (long long)(mb_off + mb), (long long)b->B);
-  STX_REQUIRE(actor->sizes[0] == critic->sizes[0], STX_E_SHAPE, "actor/critic input dims differ");
-  STX_REQUIRE(critic->sizes[critic->n_layers] == 1, STX_E_SHAPE, "critic head must be scalar");
-  STX_REQUIRE(!h->standardize_advantages || b->adv_stats, STX_E_ARG, "standardize_advantages needs adv_stats");
-  STX_REQUIRE(workspace_bytes >= stx_ppo_workspace_bytes(actor, critic, mb, STX_PREC_BF16), STX_E_WORKSPACE,
-              "stx_ppo_minibatch_update: workspace %zu < %zu", workspace_bytes, stx_ppo_workspace_bytes(actor, critic, mb, STX_PREC_BF16));
-  return tc_ppo_minibatch_grads(actor, critic, b, mb_off, mb, h, grad_weight, grad_arena, metrics, workspace, workspace_bytes,
-                                (cudaStream_t)stream, opt);
-}
-
-extern "C" int stx_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic,
-                                       const StxPpoBatch* b, int64_t mb_off, int64_t mb,
-                                       const StxPpoHyper* h, float grad_weight, float* grad_arena,
-                                       float* metrics, int precision, void* workspace,
-                                       size_t workspace_bytes, void* stream) {
-  if (int rc = check_mlp(actor, "stx_ppo_minibatch_grads(actor)")) return rc;
-  if (int rc = check_mlp(critic, "stx_ppo_minibatch_grads(critic)")) return rc;
-  STX_REQUIRE(b && h && grad_arena && metrics && workspace, STX_E_ARG, "stx_ppo_minibatch_grads: null pointer");
-  STX_REQUIRE(b->obs && b->action && b->log_prob && b->value && b->advantages && b->targets, STX_E_ARG,
-              "stx_ppo_minibatch_grads: null batch field");
-  STX_REQUIRE(mb > 0 && mb_off >= 0 && mb_off + mb <= b->B, STX_E_SHAPE,
-              "stx_ppo_minibatch_grads: minibatch [%lld,%lld) outside batch %lld", (long long)mb_off,
-              (long long)(mb_off + mb), (long long)b->B);
-  STX_REQUIRE(actor->sizes[0] == critic->sizes[0], STX_E_SHAPE, "actor/critic input dims differ");
-  STX_REQUIRE(critic->sizes[critic->n_layers] == 1, STX_E_SHAPE, "critic head must be scalar");
-  STX_REQUIRE(actor->sizes[actor->n_layers] <= kMaxActions, STX_E_SHAPE, "action_dim %d > %d",
-              actor->sizes[actor->n_layers], kMaxActions);
-  STX_REQUIRE(!h->standardize_advantages || b->adv_stats, STX_E_ARG, "standardize_advantages needs adv_stats");
-  STX_REQUIRE(workspace_bytes >= stx_ppo_workspace_bytes(actor, critic, mb, precision), STX_E_WORKSPACE,
-              "stx_ppo_minibatch_grads: workspace %zu < %zu", workspace_bytes,
-              stx_ppo_workspace_bytes(actor, critic, mb, precision));
-  cudaStream_t st = (cudaStream_t)stream;
-  if (precision == STX_PREC_BF16)
-    return tc_ppo_minibatch_grads(actor, critic, b, mb_off, mb, h, grad_weight, grad_arena, metrics, workspace, workspace_bytes, st, nullptr);
-  STX_REQUIRE(precision == STX_PREC_F32, STX_E_UNSUPPORTED, "precision=%d", precision);
-
-  int64_t aoff, coff, total;
-  stx_ppo_arena_offsets(actor, critic, &aoff, &coff, &total);
-  const int D = actor->sizes[0];
-  const float* obs = reinterpret_cast<const float*>(b->obs);
-  const int32_t* idx = b->perm ? b->perm + mb_off : nullptr;
-  // Without a permutation the minibatch is the contiguous row range starting at mb_off.
-  const float* x = idx ? obs : obs + mb_off * (int64_t)D;
-  const float* stats = h->standardize_advantages ? b->adv_stats : nullptr;
-
-  // ---- actor: forward, loss, backward (ff_ppo.py:191-213, 238-241) ----
-  {
-    SimtPpoWs ws = carve(actor, mb, reinterpret_cast<char*>(workspace));
-    if (int rc = simt_forward(actor, x, D, idx, mb, ws.acts, ws.hacts, ws.stats, ws.head, st)) return rc;
-    LossArgs g{};
-    g.logits = ws.head, g.value = nullptr, g.idx = idx, g.row0 = mb_off;
-    g.action = b->action, g.logp_old = b->log_prob, g.v_old = b->value, g.adv = b->advantages, g.tgt = b->targets;
-    g.adv_stats = stats, g.dlogits = ws.dhead, g.dvalue = nullptr, g.mb = mb, g.A = actor->sizes[actor->n_layers];
-    g.clip_eps = h->clip_eps, g.ent_coef = h->ent_coef, g.vf_coef = h->vf_coef;
-    g.partials = ws.loss_partials, g.counter = ws.counter, g.metrics = metrics, g.weight = grad_weight;
-    ppo_loss_grad_kernel<<<(unsigned)((mb + 255) / 256), 256, 0, st>>>(g);
-    STX_LAUNCH_OK();
-    if (int rc = simt_backward(actor, x, D, idx, mb, ws, grad_weight, grad_arena + aoff, h->overwrite_grads, st)) return rc;
-  }
-  // ---- critic: forward, loss, backward (ff_ppo.py:215-235, 244-247) ----
-  return simt_ppo_critic_grads(critic, b, mb_off, mb, h, grad_weight, grad_arena + coff, metrics, workspace, st);
 }

@@ -1,5 +1,5 @@
-// The pieces of the fp32 PPO minibatch (stx_mlp.cu) that other policy heads reuse: one network's forward / backward on a
-// minibatch with the workspace carved as stx_ppo_workspace_bytes() sizes it, and the whole critic half.
+// The networks of the fp32 PPO minibatch (stx_mlp.cu), as the loss entries (stx_ppo_fp32.cu) use them: one network's forward /
+// backward on a minibatch with the workspace carved as stx_ppo_workspace_bytes() sizes it.
 #pragma once
 #include "stx_common.cuh"
 
@@ -17,7 +17,5 @@ int simt_net_forward(const StxMlp* m, const float* x, int64_t ldx, const int32_t
                      cudaStream_t st);
 int simt_net_backward(const StxMlp* m, const float* x, int64_t ldx, const int32_t* idx, int64_t mb, void* workspace, float grad_weight,
                       float* net_grad, int overwrite, cudaStream_t st);
-int simt_ppo_critic_grads(const StxMlp* critic, const StxPpoBatch* b, int64_t mb_off, int64_t mb, const StxPpoHyper* h, float grad_weight,
-                          float* net_grad, float* metrics, void* workspace, cudaStream_t st);
 
 }  // namespace stx

@@ -1,6 +1,6 @@
 // Device arithmetic of the tanh-Normal policy head (NormalAffineTanhDistributionHead, stoix/networks/heads.py:44-65, on
 // AffineTanhTransformedDistribution, stoix/networks/distributions.py:19-89), shared by the SAC kernels (stx_sac.cu) and the
-// continuous PPO kernels (stx_ppo_continuous.cu).  tfp pieces restated from their published definitions: Normal.log_prob,
+// fp32 PPO loss kernels (stx_ppo_loss.cuh, stx_ppo_fp32.cu).  tfp pieces restated from their published definitions: Normal.log_prob,
 // log_cdf / log_survival_function, bijectors.Tanh.forward_log_det_jacobian(x) = 2 (log 2 - x - softplus(-2x)).
 #pragma once
 #include "stx_common.cuh"
@@ -62,7 +62,7 @@ __device__ __forceinline__ TanhNormalDim tanh_normal_log_prob_given(float loc, f
   return r;
 }
 
-// ---- the seeded entropy estimate of the PPO losses (stx_ppo_continuous.cu, stx_ppo_variants.cu) ----
+// ---- the seeded entropy estimate of the PPO losses (stx_ppo_loss.cuh) ----
 constexpr uint32_t kTagPpoEntropy = 0x50504f45u;  // "PPOE"
 
 // Entropy noise eps' of row m, dims j0..j0+3 (layout in include/stx.h); eps_in (nullable, (rows, A)) replaces the draw.

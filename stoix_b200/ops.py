@@ -301,6 +301,36 @@ def ppo_workspace(actor: MlpSpec, critic: MlpSpec, mb: int, precision: int, devi
     return torch.zeros(int(nbytes), dtype=torch.uint8, device=device)
 
 
+def _minibatch_structs(who: str, actor: MlpSpec, critic: MlpSpec, param_arena: torch.Tensor, batch: PpoBatch, grad_arena: torch.Tensor,
+                       metrics: torch.Tensor, workspace: torch.Tensor, hyper: Tuple, *, obs_dtype: torch.dtype, fp32_only: str = "",
+                       n_metrics: int = 6, categorical: bool = True, param_arena_bf16: Optional[torch.Tensor] = None,
+                       arenas: Tuple[torch.Tensor, ...] = (), adam_scratch: Optional[torch.Tensor] = None):
+    """The checks every PPO minibatch wrapper shares, and its StxMlp (actor, critic), StxPpoBatch and StxPpoHyper.  hyper =
+    (clip_eps, ent_coef, vf_coef, standardize, overwrite); `arenas` must hold the whole arena too; a tanh-Normal batch
+    (categorical=False) holds float (B, A) actions that go to the C entry through StxTanhNormalPpo instead."""
+    _need_cuda(param_arena, batch.obs, batch.action, batch.log_prob, batch.value, batch.advantages, batch.targets, batch.adv_stats, batch.perm,
+               grad_arena, metrics, workspace, param_arena_bf16, *arenas)
+    if (categorical and batch.action.dtype != torch.int32) or (batch.perm is not None and batch.perm.dtype != torch.int32):
+        raise StxError(f"{who}: action / perm must be int32" if categorical else f"{who}: perm must be int32")
+    if batch.obs.dtype != obs_dtype:
+        raise StxError(f"{who}: obs must be {obs_dtype}" + (f" ({fp32_only} runs on the fp32 path)" if fp32_only else ""))
+    _, coff, total = arena_offsets(actor, critic)
+    if min(t.numel() for t in (param_arena, grad_arena) + arenas) < total or metrics.numel() < n_metrics:
+        raise StxError(f"{who}: arena too small or metrics below {n_metrics} floats")
+    a = actor.c_struct(param_arena, param_arena_bf16)
+    c = critic.c_struct(param_arena[coff:], param_arena_bf16[coff:] if param_arena_bf16 is not None else None)
+    b = batch.c_struct()
+    if not categorical:
+        B = int(batch.log_prob.numel())
+        if batch.action.shape != (B, actor.sizes[-1] // 2):
+            raise StxError(f"{who}: action must be float32 ({B}, {actor.sizes[-1] // 2})")
+        b.action, b.B = None, B
+    clip_eps, ent_coef, vf_coef, standardize, overwrite = hyper
+    h = _lib.StxPpoHyper(float(clip_eps), float(ent_coef), float(vf_coef), int(bool(standardize)), int(bool(overwrite)), 0,
+                         adam_scratch.data_ptr() if adam_scratch is not None else None)
+    return a, c, b, h
+
+
 def ppo_minibatch_grads(actor: MlpSpec, critic: MlpSpec, param_arena: torch.Tensor, batch: PpoBatch,
                         mb_off: int, mb: int, clip_eps: float, ent_coef: float, vf_coef: float,
                         standardize: bool, grad_arena: torch.Tensor, metrics: torch.Tensor,
@@ -309,26 +339,13 @@ def ppo_minibatch_grads(actor: MlpSpec, critic: MlpSpec, param_arena: torch.Tens
                         adam_scratch: Optional[torch.Tensor] = None) -> None:
     """Accumulate grad_weight * d(loss)/d(params) of minibatch [mb_off, mb_off+mb) into grad_arena and
     the six loss metrics into `metrics` (ff_ppo.py:184-247)."""
-    _need_cuda(param_arena, batch.obs, batch.action, batch.log_prob, batch.value, batch.advantages,
-               batch.targets, batch.adv_stats, batch.perm, grad_arena, metrics, workspace)
-    if batch.action.dtype != torch.int32 or (batch.perm is not None and batch.perm.dtype != torch.int32):
-        raise StxError("ppo_minibatch_grads: action / perm must be int32")
-    want = torch.float32 if precision == STX_PREC_F32 else torch.bfloat16
-    if batch.obs.dtype != want:
-        raise StxError(f"ppo_minibatch_grads: obs must be {want} for precision {precision}")
-    _, coff, total = arena_offsets(actor, critic)
-    if param_arena.numel() < total or grad_arena.numel() < total or metrics.numel() < 6:
-        raise StxError("ppo_minibatch_grads: arena or metrics too small")
-    lib = _lib.load()
-    a = actor.c_struct(param_arena, param_arena_bf16)
-    c = critic.c_struct(param_arena[coff:], param_arena_bf16[coff:] if param_arena_bf16 is not None else None)
-    b = batch.c_struct()
-    h = _lib.StxPpoHyper(float(clip_eps), float(ent_coef), float(vf_coef), int(bool(standardize)), int(bool(overwrite)), 0,
-                         adam_scratch.data_ptr() if adam_scratch is not None else None)
+    a, c, b, h = _minibatch_structs("ppo_minibatch_grads", actor, critic, param_arena, batch, grad_arena, metrics, workspace,
+                                    (clip_eps, ent_coef, vf_coef, standardize, overwrite),
+                                    obs_dtype=torch.float32 if precision == STX_PREC_F32 else torch.bfloat16,
+                                    param_arena_bf16=param_arena_bf16, adam_scratch=adam_scratch)
     _lib.check(
-        lib.stx_ppo_minibatch_grads(C.byref(a), C.byref(c), C.byref(b), int(mb_off), int(mb), C.byref(h),
-                                    float(grad_weight), _p(grad_arena), _p(metrics), precision,
-                                    _p(workspace), workspace.numel(), _stream()),
+        _lib.load().stx_ppo_minibatch_grads(C.byref(a), C.byref(c), C.byref(b), int(mb_off), int(mb), C.byref(h), float(grad_weight),
+                                            _p(grad_arena), _p(metrics), precision, _p(workspace), workspace.numel(), _stream()),
         "stx_ppo_minibatch_grads",
     )
 
@@ -342,29 +359,18 @@ def ppo_minibatch_update(actor: MlpSpec, critic: MlpSpec, param_arena: torch.Ten
     clip_by_global_norm + Adam on both networks, bf16 shadow refresh; the gradient reduction and the optimiser share
     one launch (stx_ppo_minibatch_update).  bf16 path, one shard, one device; `plan` must hold exactly the two
     segments (actor arena, critic arena).  Same results as ppo_minibatch_grads(overwrite=True) + clip_adam_step."""
-    _need_cuda(param_arena, batch.obs, batch.action, batch.log_prob, batch.value, batch.advantages,
-               batch.targets, batch.adv_stats, batch.perm, grad_arena, metrics, workspace, mu, nu, param_arena_bf16)
-    if batch.action.dtype != torch.int32 or (batch.perm is not None and batch.perm.dtype != torch.int32):
-        raise StxError("ppo_minibatch_update: action / perm must be int32")
-    if batch.obs.dtype != torch.bfloat16:
-        raise StxError("ppo_minibatch_update: obs must be bfloat16 (STX_PREC_BF16 path)")
-    _, coff, total = arena_offsets(actor, critic)
-    if min(param_arena.numel(), grad_arena.numel(), mu.numel(), nu.numel(), param_arena_bf16.numel()) < total or metrics.numel() < 6:
-        raise StxError("ppo_minibatch_update: arena or metrics too small")
+    a, c, b, h = _minibatch_structs("ppo_minibatch_update", actor, critic, param_arena, batch, grad_arena, metrics, workspace,
+                                    (clip_eps, ent_coef, vf_coef, standardize, True), obs_dtype=torch.bfloat16,
+                                    param_arena_bf16=param_arena_bf16, arenas=(mu, nu, param_arena_bf16))
     if plan.nseg != 2:
         raise StxError("ppo_minibatch_update: the optimiser plan must have the two segments (actor, critic)")
-    lib = _lib.load()
-    a = actor.c_struct(param_arena, param_arena_bf16)
-    c = critic.c_struct(param_arena[coff:], param_arena_bf16[coff:])
-    b = batch.c_struct()
-    h = _lib.StxPpoHyper(float(clip_eps), float(ent_coef), float(vf_coef), int(bool(standardize)), 1, 0, None)
     plan.hyper.grad_scale = float(grad_scale)
     plan.hyper.prenorm = 0
     opt = _lib.StxFusedAdam(_p(param_arena), _p(mu), _p(nu), _p(plan.counts), _p(plan.segs), plan.nseg, 0, plan.hyper,
                             _p(param_arena_bf16), _p(plan.gnorm), _p(plan.scratch))
     _lib.check(
-        lib.stx_ppo_minibatch_update(C.byref(a), C.byref(c), C.byref(b), int(mb_off), int(mb), C.byref(h), float(grad_weight),
-                                     _p(grad_arena), _p(metrics), _p(workspace), workspace.numel(), C.byref(opt), _stream()),
+        _lib.load().stx_ppo_minibatch_update(C.byref(a), C.byref(c), C.byref(b), int(mb_off), int(mb), C.byref(h), float(grad_weight),
+                                             _p(grad_arena), _p(metrics), _p(workspace), workspace.numel(), C.byref(opt), _stream()),
         "stx_ppo_minibatch_update",
     )
 
@@ -733,6 +739,20 @@ def _tanh_normal_ppo(action,minimum, maximum, min_scale, seed, offset, dev_count
                                  float(maximum), float(min_scale), 0)
 
 
+def _head_grads_io(who: str, head_out: torch.Tensor, idx: Optional[torch.Tensor], d_head_out: Optional[torch.Tensor],
+                   metrics: Optional[torch.Tensor], n_metrics: int, scratch_key: str, *tensors: Optional[torch.Tensor]):
+    """The checks and buffers the actor head-grad wrappers share: (d_head_out, metrics, scratch), allocating what is not given
+    (metrics zeroed, 6 or 8 floats)."""
+    dev = _need_cuda(head_out, idx, d_head_out, metrics, *tensors)
+    if idx is not None and idx.dtype != torch.int32:
+        raise StxError(f"{who}: idx must be int32")
+    d_head_out = torch.empty(head_out.shape, dtype=torch.float32, device=dev) if d_head_out is None else d_head_out
+    metrics = torch.zeros(6 if n_metrics <= 6 else 8, dtype=torch.float32, device=dev) if metrics is None else metrics
+    if metrics.numel() < n_metrics:
+        raise StxError(f"{who}: metrics must hold at least {n_metrics} floats")
+    return d_head_out, metrics, _zeros_scratch((scratch_key,), _lib.load().stx_ppo_head_scratch_bytes(head_out.shape[0]), dev)
+
+
 def ppo_tanh_normal_head_grads(head_out: torch.Tensor, idx: Optional[torch.Tensor], action: torch.Tensor, logp_old: torch.Tensor,
                                adv: torch.Tensor, adv_stats: Optional[torch.Tensor], clip_eps: float, ent_coef: float, minimum: float,
                                maximum: float, min_scale: float = 1e-3, seed: int = 0, offset: int = 0,
@@ -743,22 +763,15 @@ def ppo_tanh_normal_head_grads(head_out: torch.Tensor, idx: Optional[torch.Tenso
     """The actor half of continuous PPO's _update_minibatch on head outputs computed elsewhere (stx_ppo_tanh_normal_head_grads):
     row m of head_out (mb, 2A) pairs with batch row idx[m] (or row0 + m) of action (B, A) / logp_old / adv.
     Returns (d_head_out, metrics[6]); metrics slots 0, 1, 3 = actor_loss, entropy, mean advantage."""
-    dev = _need_cuda(head_out, idx, action, logp_old, adv, adv_stats, d_head_out, metrics)
+    who = "ppo_tanh_normal_head_grads"
+    d_head_out, metrics, scratch = _head_grads_io(who, head_out, idx, d_head_out, metrics, 6, scratch_key, action, logp_old, adv, adv_stats)
     mb, A2 = head_out.shape
-    if idx is not None and idx.dtype != torch.int32:
-        raise StxError("ppo_tanh_normal_head_grads: idx must be int32")
     if action.ndim != 2 or action.shape[1] != A2 // 2:
-        raise StxError("ppo_tanh_normal_head_grads: action must be (B, A) with 2A = head_out.shape[1]")
-    if d_head_out is None:
-        d_head_out = torch.empty(mb, A2, dtype=torch.float32, device=dev)
-    if metrics is None:
-        metrics = torch.zeros(6, dtype=torch.float32, device=dev)
+        raise StxError(f"{who}: action must be (B, A) with 2A = head_out.shape[1]")
     hd = _tanh_normal_ppo(action, minimum, maximum, min_scale, seed, offset, dev_counter, eps_in, eps_out)
-    lib = _lib.load()
-    scratch = _zeros_scratch((scratch_key,), lib.stx_ppo_head_scratch_bytes(mb), dev)
-    _lib.check(lib.stx_ppo_tanh_normal_head_grads(_p(head_out), _p(idx), int(row0), C.byref(hd), _p(logp_old), _p(adv), _p(adv_stats), mb, A2 // 2,
-                                                  float(clip_eps), float(ent_coef), _p(d_head_out), _p(metrics), float(weight), _p(scratch),
-                                                  _stream()), "stx_ppo_tanh_normal_head_grads")
+    _lib.check(_lib.load().stx_ppo_tanh_normal_head_grads(_p(head_out), _p(idx), int(row0), C.byref(hd), _p(logp_old), _p(adv), _p(adv_stats), mb,
+                                                          A2 // 2, float(clip_eps), float(ent_coef), _p(d_head_out), _p(metrics), float(weight),
+                                                          _p(scratch), _stream()), "stx_ppo_tanh_normal_head_grads")
     return d_head_out, metrics
 
 
@@ -770,29 +783,14 @@ def ppo_continuous_minibatch_grads(actor: MlpSpec, critic: MlpSpec, param_arena:
                                    precision: int = STX_PREC_F32, grad_weight: float = 1.0, overwrite: bool = False) -> None:
     """ppo_minibatch_grads for a tanh-Normal actor (ff_ppo_continuous.py:184-247): batch.action holds the float (B, A) actions.
     Entropy noise from Philox (seed, minibatch row, offset + *dev_counter) unless eps_in (mb, A) is given; eps_out records it."""
-    _need_cuda(param_arena, batch.obs, batch.action, batch.log_prob, batch.value, batch.advantages, batch.targets, batch.adv_stats, batch.perm,
-               grad_arena, metrics, workspace)
-    if batch.perm is not None and batch.perm.dtype != torch.int32:
-        raise StxError("ppo_continuous_minibatch_grads: perm must be int32")
-    if batch.obs.dtype != torch.float32:
-        raise StxError("ppo_continuous_minibatch_grads: obs must be float32 (the tanh-Normal head runs on the fp32 path)")
-    _, coff, total = arena_offsets(actor, critic)
-    if param_arena.numel() < total or grad_arena.numel() < total or metrics.numel() < 6:
-        raise StxError("ppo_continuous_minibatch_grads: arena or metrics too small")
-    B = int(batch.log_prob.numel())
-    if batch.action.shape != (B, actor.sizes[-1] // 2):
-        raise StxError(f"ppo_continuous_minibatch_grads: action must be float32 ({B}, {actor.sizes[-1] // 2})")
+    a, c, b, h = _minibatch_structs("ppo_continuous_minibatch_grads", actor, critic, param_arena, batch, grad_arena, metrics, workspace,
+                                    (clip_eps, ent_coef, vf_coef, standardize, overwrite), obs_dtype=torch.float32,
+                                    fp32_only="the tanh-Normal head", categorical=False)
     hd = _tanh_normal_ppo(batch.action, minimum, maximum, min_scale, seed, offset, dev_counter, eps_in, eps_out)
-    lib = _lib.load()
-    a = actor.c_struct(param_arena)
-    c = critic.c_struct(param_arena[coff:])
-    b = batch.c_struct()
-    b.action, b.B = None, B
-    h = _lib.StxPpoHyper(float(clip_eps), float(ent_coef), float(vf_coef), int(bool(standardize)), int(bool(overwrite)), 0, None)
     _lib.check(
-        lib.stx_ppo_continuous_minibatch_grads(C.byref(a), C.byref(c), C.byref(b), C.byref(hd), int(mb_off), int(mb), C.byref(h),
-                                               float(grad_weight), _p(grad_arena), _p(metrics), int(precision), _p(workspace),
-                                               workspace.numel(), _stream()),
+        _lib.load().stx_ppo_continuous_minibatch_grads(C.byref(a), C.byref(c), C.byref(b), C.byref(hd), int(mb_off), int(mb), C.byref(h),
+                                                       float(grad_weight), _p(grad_arena), _p(metrics), int(precision), _p(workspace),
+                                                       workspace.numel(), _stream()),
         "stx_ppo_continuous_minibatch_grads",
     )
 
@@ -871,21 +869,16 @@ def ppo_penalty_head_grads(logits: torch.Tensor, idx: Optional[torch.Tensor], be
     """The actor half of ff_ppo_penalty's _update_minibatch on logits (mb, A) computed elsewhere: row m pairs with batch row idx[m]
     (or row0 + m) of behaviour (B, A) / action / logp_old / adv.  Returns (d_logits, metrics[8]); slots 0, 1, 6 = actor_loss,
     entropy, kl_divergence."""
-    dev = _need_cuda(logits, idx, behaviour, action, logp_old, adv, adv_stats, d_logits, metrics)
+    who = "ppo_penalty_head_grads"
+    d_logits, metrics, scratch = _head_grads_io(who, logits, idx, d_logits, metrics, 7, scratch_key, behaviour, action, logp_old, adv, adv_stats)
     mb, A = logits.shape
-    if (idx is not None and idx.dtype != torch.int32) or action.dtype != torch.int32:
-        raise StxError("ppo_penalty_head_grads: idx / action must be int32")
+    if action.dtype != torch.int32:
+        raise StxError(f"{who}: action must be int32")
     if behaviour.ndim != 2 or behaviour.shape[1] != A:
-        raise StxError("ppo_penalty_head_grads: behaviour must be (B, A) with A = logits.shape[1]")
-    d_logits = torch.empty(mb, A, dtype=torch.float32, device=dev) if d_logits is None else d_logits
-    metrics = torch.zeros(8, dtype=torch.float32, device=dev) if metrics is None else metrics
-    if metrics.numel() < 7:
-        raise StxError("ppo_penalty_head_grads: metrics must hold at least 7 floats")
+        raise StxError(f"{who}: behaviour must be (B, A) with A = logits.shape[1]")
     v = _variant(STX_PPO_KL_PENALTY, behaviour, kl_coef, 0.0, 0.0)
-    lib = _lib.load()
-    scratch = _zeros_scratch((scratch_key,), lib.stx_ppo_head_scratch_bytes(mb), dev)
-    _lib.check(lib.stx_ppo_penalty_head_grads(_p(logits), _p(idx), int(row0), C.byref(v), _p(action), _p(logp_old), _p(adv), _p(adv_stats), mb, A,
-                                              float(ent_coef), _p(d_logits), _p(metrics), float(weight), _p(scratch), _stream()),
+    _lib.check(_lib.load().stx_ppo_penalty_head_grads(_p(logits), _p(idx), int(row0), C.byref(v), _p(action), _p(logp_old), _p(adv), _p(adv_stats),
+                                                      mb, A, float(ent_coef), _p(d_logits), _p(metrics), float(weight), _p(scratch), _stream()),
                "stx_ppo_penalty_head_grads")
     return d_logits, metrics
 
@@ -900,37 +893,17 @@ def ppo_variant_tanh_normal_head_grads(head_out: torch.Tensor, idx: Optional[tor
                                        scratch_key: str = "ppo_variant_head") -> Tuple[torch.Tensor, torch.Tensor]:
     """The actor half of ff_ppo_penalty_continuous / ff_dpo_continuous (kind STX_PPO_KL_PENALTY / STX_PPO_DPO) on head outputs
     (mb, 2A) computed elsewhere; entropy noise as ppo_tanh_normal_head_grads.  Returns (d_head_out, metrics[8])."""
-    dev = _need_cuda(head_out, idx, action, logp_old, adv, adv_stats, d_head_out, metrics)
+    who = "ppo_variant_tanh_normal_head_grads"
+    d_head_out, metrics, scratch = _head_grads_io(who, head_out, idx, d_head_out, metrics, 7, scratch_key, action, logp_old, adv, adv_stats)
     mb, A2 = head_out.shape
-    if idx is not None and idx.dtype != torch.int32:
-        raise StxError("ppo_variant_tanh_normal_head_grads: idx must be int32")
     if action.ndim != 2 or action.shape[1] != A2 // 2 or (behaviour is not None and (behaviour.ndim != 2 or behaviour.shape[1] != A2)):
-        raise StxError("ppo_variant_tanh_normal_head_grads: action must be (B, A) and behaviour (B, 2A) with 2A = head_out.shape[1]")
-    d_head_out = torch.empty(mb, A2, dtype=torch.float32, device=dev) if d_head_out is None else d_head_out
-    metrics = torch.zeros(8, dtype=torch.float32, device=dev) if metrics is None else metrics
-    if metrics.numel() < 7:
-        raise StxError("ppo_variant_tanh_normal_head_grads: metrics must hold at least 7 floats")
+        raise StxError(f"{who}: action must be (B, A) and behaviour (B, 2A) with 2A = head_out.shape[1]")
     hd = _tanh_normal_ppo(action, minimum, maximum, min_scale, seed, offset, dev_counter, eps_in, eps_out)
     v = _variant(kind, behaviour, kl_coef, dpo_alpha, dpo_beta)
-    lib = _lib.load()
-    scratch = _zeros_scratch((scratch_key,), lib.stx_ppo_head_scratch_bytes(mb), dev)
-    _lib.check(lib.stx_ppo_variant_tanh_normal_head_grads(_p(head_out), _p(idx), int(row0), C.byref(hd), C.byref(v), _p(logp_old), _p(adv),
-                                                          _p(adv_stats), mb, A2 // 2, float(ent_coef), _p(d_head_out), _p(metrics), float(weight),
-                                                          _p(scratch), _stream()), "stx_ppo_variant_tanh_normal_head_grads")
+    _lib.check(_lib.load().stx_ppo_variant_tanh_normal_head_grads(_p(head_out), _p(idx), int(row0), C.byref(hd), C.byref(v), _p(logp_old), _p(adv),
+                                                                  _p(adv_stats), mb, A2 // 2, float(ent_coef), _p(d_head_out), _p(metrics),
+                                                                  float(weight), _p(scratch), _stream()), "stx_ppo_variant_tanh_normal_head_grads")
     return d_head_out, metrics
-
-
-def _variant_batch_checks(who, actor, critic, param_arena, batch, grad_arena, metrics, workspace):
-    _need_cuda(param_arena, batch.obs, batch.action, batch.log_prob, batch.value, batch.advantages, batch.targets, batch.adv_stats, batch.perm,
-               grad_arena, metrics, workspace)
-    if batch.perm is not None and batch.perm.dtype != torch.int32:
-        raise StxError(f"{who}: perm must be int32")
-    if batch.obs.dtype != torch.float32:
-        raise StxError(f"{who}: obs must be float32 (the KL-penalty and DPO losses run on the fp32 path)")
-    _, coff, total = arena_offsets(actor, critic)
-    if param_arena.numel() < total or grad_arena.numel() < total or metrics.numel() < 7:
-        raise StxError(f"{who}: arena too small or metrics below 7 floats")
-    return coff
 
 
 def ppo_penalty_minibatch_grads(actor: MlpSpec, critic: MlpSpec, param_arena: torch.Tensor, batch: PpoBatch, mb_off: int, mb: int,
@@ -939,18 +912,16 @@ def ppo_penalty_minibatch_grads(actor: MlpSpec, critic: MlpSpec, param_arena: to
                                 grad_weight: float = 1.0, overwrite: bool = False) -> None:
     """ppo_minibatch_grads with ff_ppo_penalty's actor loss (ff_ppo_penalty.py:149-210): behaviour (B, A) holds the behaviour
     policy's logits per batch row; clip_eps clips only the value loss."""
-    coff = _variant_batch_checks("ppo_penalty_minibatch_grads", actor, critic, param_arena, batch, grad_arena, metrics, workspace)
-    if batch.action.dtype != torch.int32:
-        raise StxError("ppo_penalty_minibatch_grads: action must be int32")
+    who = "ppo_penalty_minibatch_grads"
+    a, c, b, h = _minibatch_structs(who, actor, critic, param_arena, batch, grad_arena, metrics, workspace,
+                                    (clip_eps, ent_coef, vf_coef, standardize, overwrite), obs_dtype=torch.float32,
+                                    fp32_only="the KL-penalty loss", n_metrics=7)
     if behaviour.shape != (batch.action.numel(), actor.sizes[-1]):
-        raise StxError(f"ppo_penalty_minibatch_grads: behaviour must be ({batch.action.numel()}, {actor.sizes[-1]})")
+        raise StxError(f"{who}: behaviour must be ({batch.action.numel()}, {actor.sizes[-1]})")
     v = _variant(STX_PPO_KL_PENALTY, behaviour, kl_coef, 0.0, 0.0)
-    lib = _lib.load()
-    a, c, b = actor.c_struct(param_arena), critic.c_struct(param_arena[coff:]), batch.c_struct()
-    h = _lib.StxPpoHyper(float(clip_eps), float(ent_coef), float(vf_coef), int(bool(standardize)), int(bool(overwrite)), 0, None)
-    _lib.check(lib.stx_ppo_penalty_minibatch_grads(C.byref(a), C.byref(c), C.byref(b), C.byref(v), int(mb_off), int(mb), C.byref(h),
-                                                   float(grad_weight), _p(grad_arena), _p(metrics), int(precision), _p(workspace),
-                                                   workspace.numel(), _stream()), "stx_ppo_penalty_minibatch_grads")
+    _lib.check(_lib.load().stx_ppo_penalty_minibatch_grads(C.byref(a), C.byref(c), C.byref(b), C.byref(v), int(mb_off), int(mb), C.byref(h),
+                                                           float(grad_weight), _p(grad_arena), _p(metrics), int(precision), _p(workspace),
+                                                           workspace.numel(), _stream()), "stx_ppo_penalty_minibatch_grads")
 
 
 def ppo_variant_continuous_minibatch_grads(actor: MlpSpec, critic: MlpSpec, param_arena: torch.Tensor, batch: PpoBatch, mb_off: int, mb: int,
@@ -964,21 +935,16 @@ def ppo_variant_continuous_minibatch_grads(actor: MlpSpec, critic: MlpSpec, para
     """ppo_continuous_minibatch_grads with the actor loss of ff_ppo_penalty_continuous (kind STX_PPO_KL_PENALTY, behaviour (B, 2A)
     head outputs) or ff_dpo_continuous (kind STX_PPO_DPO); entropy noise as in ppo_continuous_minibatch_grads."""
     who = "ppo_variant_continuous_minibatch_grads"
-    coff = _variant_batch_checks(who, actor, critic, param_arena, batch, grad_arena, metrics, workspace)
-    B = int(batch.log_prob.numel())
-    if batch.action.shape != (B, actor.sizes[-1] // 2):
-        raise StxError(f"{who}: action must be float32 ({B}, {actor.sizes[-1] // 2})")
-    if behaviour is not None and behaviour.shape != (B, actor.sizes[-1]):
-        raise StxError(f"{who}: behaviour must be ({B}, {actor.sizes[-1]})")
+    a, c, b, h = _minibatch_structs(who, actor, critic, param_arena, batch, grad_arena, metrics, workspace,
+                                    (clip_eps, ent_coef, vf_coef, standardize, overwrite), obs_dtype=torch.float32,
+                                    fp32_only="the KL-penalty and DPO losses", n_metrics=7, categorical=False)
+    if behaviour is not None and behaviour.shape != (b.B, actor.sizes[-1]):
+        raise StxError(f"{who}: behaviour must be ({b.B}, {actor.sizes[-1]})")
     hd = _tanh_normal_ppo(batch.action, minimum, maximum, min_scale, seed, offset, dev_counter, eps_in, eps_out)
     v = _variant(kind, behaviour, kl_coef, dpo_alpha, dpo_beta)
-    lib = _lib.load()
-    a, c, b = actor.c_struct(param_arena), critic.c_struct(param_arena[coff:]), batch.c_struct()
-    b.action, b.B = None, B
-    h = _lib.StxPpoHyper(float(clip_eps), float(ent_coef), float(vf_coef), int(bool(standardize)), int(bool(overwrite)), 0, None)
-    _lib.check(lib.stx_ppo_variant_continuous_minibatch_grads(C.byref(a), C.byref(c), C.byref(b), C.byref(hd), C.byref(v), int(mb_off), int(mb),
-                                                              C.byref(h), float(grad_weight), _p(grad_arena), _p(metrics), int(precision),
-                                                              _p(workspace), workspace.numel(), _stream()),
+    _lib.check(_lib.load().stx_ppo_variant_continuous_minibatch_grads(C.byref(a), C.byref(c), C.byref(b), C.byref(hd), C.byref(v), int(mb_off),
+                                                                      int(mb), C.byref(h), float(grad_weight), _p(grad_arena), _p(metrics),
+                                                                      int(precision), _p(workspace), workspace.numel(), _stream()),
                "stx_ppo_variant_continuous_minibatch_grads")
 
 
