@@ -242,8 +242,8 @@ int simt_backward(const StxMlp* m, const float* x, int64_t ldx, const int32_t* r
       STX_CUDA_OK(simt::launch_gemm<simt::DX>(d, 1, st));
       if (ln) {
         const float* gamma = m->params + boff[i - 1];
-        simt::ln_backward_kernel<<<ws.ln_blocks, 32 * simt::kLnWarps, sizeof(float) * simt::kLnWarps * 2 * nin, st>>>(
-            ws.dbuf[pp], ws.acts[i], ws.stats[i], gamma, gamma + nin, m->activation, mb, nin, ws.ln_rows, ws.ln_part);
+        STX_CUDA_OK(simt::launch_ln_backward(ws.dbuf[pp], ws.acts[i], ws.stats[i], gamma, gamma + nin, m->activation, mb, nin, ws.ln_rows,
+                                             ws.ln_blocks, ws.ln_part, st));
         STX_LAUNCH_OK();
         // d(scale | bias) of layer i-1: fixed-order sum over the blocks, straight into the gradient arena
         if (net_grad != nullptr)

@@ -549,5 +549,25 @@ static __global__ void __launch_bounds__(32 * kLnWarps) ln_backward_kernel(float
   }
 }
 
+// ln_backward_kernel takes kLnWarps * 2N floats of dynamic shared memory: 64 KiB at the widest width check_mlp accepts
+// (N = 32 * kLnMaxCols), more than the 48 KiB a launch may use without opting in (every width above 768).  The opt-in is made
+// once per device for the largest size, as launch_gemm does for the panel kernel; it is not a stream operation, so a launch
+// under stream capture may make it.
+constexpr uint32_t kLnMaxSmemBytes = sizeof(float) * kLnWarps * 2 * 32 * kLnMaxCols;
+static inline cudaError_t launch_ln_backward(float* D, const float* U, const float* stats, const float* gamma, const float* beta, int act, int64_t M,
+                                      int N, int rows_per_block, int blocks, float* part, cudaStream_t st) {
+  static unsigned long long opted = 0;  // bit d: dynamic shared memory opt-in done on device d
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev >= 64 || !((opted >> dev) & 1ull)) {
+    e = cudaFuncSetAttribute(ln_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLnMaxSmemBytes);
+    if (e != cudaSuccess) return e;
+    if (dev < 64) opted |= 1ull << dev;
+  }
+  ln_backward_kernel<<<blocks, 32 * kLnWarps, sizeof(float) * kLnWarps * 2 * N, st>>>(D, U, stats, gamma, beta, act, M, N, rows_per_block, part);
+  return cudaGetLastError();
+}
+
 }  // namespace simt
 }  // namespace stx
