@@ -10,7 +10,9 @@
 //   warps 0..3   one warpgroup: the layer chain of stx_tc_mlp.cu on wgmma (activations in registers), then
 //                Gumbel-max sampling + log-prob of the logits (same Philox counters as stx_categorical =>
 //                identical actions for identical logits).
-//   warps 4..5   environment producers (one thread per env row): SyntheticBoxEnv's dynamics do not depend on
+//   warps 4..7   environment producers (two threads per env row, each drawing half of its features: the Philox draws
+//                and normal transforms of a step cost more issue slots than the MMA chain of the step when one warp per
+//                32 rows has to produce them all): SyntheticBoxEnv's dynamics do not depend on
 //                the action (stx_env.cu), so the producers run one step AHEAD of the policy: while the
 //                tensor cores evaluate step t they draw step t's outcome and observation t+1 (same Philox
 //                streams as stx_synth_env_step => bit-identical trajectory), write the trajectory rows and
@@ -30,8 +32,8 @@ int make_map_2d_pub(CUtensorMap* m, const void* base, uint64_t rows, uint64_t co
 namespace ro {
 
 constexpr int kTileM = 64, kH = 256;
-constexpr int kProdWarps = 2;
-constexpr int kThreads = 128 + 32 * kProdWarps;  // 192
+constexpr int kProdWarps = 4;
+constexpr int kThreads = 128 + 32 * kProdWarps;  // 256
 
 constexpr uint32_t kOffX = kImgWBytes;  // 2 stages x 8 KB
 constexpr uint32_t kOffBias = kOffX + 2 * 8192;
@@ -97,8 +99,8 @@ __global__ void __launch_bounds__(kThreads, 1)
   __syncthreads();
 
   if (warp >= 4) {
-    // ===================== environment producers: one thread per env row =====================
-    const int r = threadIdx.x - 128;
+    // ===================== environment producers: two threads per env row =====================
+    const int r = (threadIdx.x - 128) & 63, hf = (threadIdx.x - 128) >> 6;  // row, half of its 16-byte chunks: c = 4 hf + cc
     const int64_t e = tile_row0 + r;
     const int dchunks = p.D >> 3;
     const uint64_t step0 = p.env_step + (p.env_counter ? *p.env_counter : 0ull);
@@ -109,7 +111,8 @@ __global__ void __launch_bounds__(kThreads, 1)
     {
       uint8_t* xs = smem + kOffX + r * 128;
 #pragma unroll
-      for (int c = 0; c < 8; ++c) {
+      for (int cc = 0; cc < 4; ++cc) {
+        const int c = 4 * hf + cc;
         uint4 v = make_uint4(0u, 0u, 0u, 0u);
         if (c < dchunks) v = *reinterpret_cast<const uint4*>(p.obs + e * p.D + c * 8);
         *reinterpret_cast<uint4*>(xs + ((c ^ (r & 7)) << 4)) = v;
@@ -133,7 +136,8 @@ __global__ void __launch_bounds__(kThreads, 1)
       if (fill && t >= 1) mbar_wait(&x_empty[s], (((t - 1) >> 1) & 1), 30);  // layer 0 of step t-1 has read this stage
       uint8_t* xs = smem + kOffX + s * 8192 + r * 128;
 #pragma unroll 1
-      for (int c = 0; c < 8; ++c) {
+      for (int cc = 0; cc < 4; ++cc) {
+        const int c = 4 * hf + cc;
         uint4 nx = make_uint4(0u, 0u, 0u, 0u), ob;
         if (c < dchunks) {
           uint32_t w[4];
@@ -166,7 +170,7 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
         if (fill) *reinterpret_cast<uint4*>(xs + ((c ^ (r & 7)) << 4)) = ob;
       }
-      {
+      if (hf == 0) {
         const float rwd = normal2(rs.x, rs.y).x;
         const int64_t o = (int64_t)t * p.E + e;
         const float ret = run_ret + rwd;
@@ -186,7 +190,7 @@ __global__ void __launch_bounds__(kThreads, 1)
         if (lane == 0) mbar_arrive(&x_full[s]);
       }
     }
-    p.run_return[e] = run_ret, p.run_length[e] = run_len;
+    if (hf == 0) p.run_return[e] = run_ret, p.run_length[e] = run_len;
   } else {
     // ===================== the MMA warpgroup =====================
     const int q4 = lane & 3;
