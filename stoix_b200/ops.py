@@ -399,13 +399,35 @@ def clipped_value_loss_value(pred_value_t, behavior_value_t, targets_t, epsilon)
 # ------------------------------------------------------------------------------------------------
 
 
+ADAM_MAX_SEGS = 8  # kAdamMaxSegs of stx_adam.cu
+
+
 class AdamPlan:
-    """Device-resident segment table + scratch for stx_clip_adam_step."""
+    """Device-resident segment table + scratch for stx_clip_adam_step.
+
+    segments: (offset, count, init_lr, max_grad_norm) per optimiser, 1..8 of them, disjoint.  The kernels read a segment as
+    float4 items from `offset` on, so an offset must be a multiple of 4 floats (include/stx.h); a table that breaks this is
+    refused here, before anything is allocated, instead of becoming a misaligned vector access on the device."""
 
     def __init__(self, segments: Sequence[Tuple[int, int, float, float]], device, b1=0.9, b2=0.999, eps=1e-5,
                  decay=True, steps_per_update=1, num_updates=1):
         import numpy as np
 
+        segments = [tuple(s) for s in segments]
+        if not 1 <= len(segments) <= ADAM_MAX_SEGS:
+            raise StxError(f"AdamPlan: {len(segments)} segments (1..{ADAM_MAX_SEGS} supported)")
+        for off, cnt, _, _ in segments:
+            if int(off) != off or int(cnt) != cnt:
+                raise StxError(f"AdamPlan: segment ({off}, {cnt}): offset and count must be integers")
+            if off < 0 or off % 4:
+                raise StxError(f"AdamPlan: segment offset {off} is not a non-negative multiple of 4 floats (float4 access)")
+            if cnt < 1:
+                raise StxError(f"AdamPlan: segment at offset {off} has count {cnt} (at least 1)")
+        spans = sorted((int(off), int(off) + int(cnt)) for off, cnt, _, _ in segments)
+        for (a0, a1), (b0, b1_) in zip(spans, spans[1:]):
+            if b0 < a1:
+                raise StxError(f"AdamPlan: segments [{a0}, {a1}) and [{b0}, {b1_}) overlap")
+        self.end = spans[-1][1]  # the arenas must hold at least this many floats
         self.nseg = len(segments)
         arr = (_lib.StxAdamSeg * self.nseg)()
         for i, (off, cnt, lr, mgn) in enumerate(segments):
@@ -419,8 +441,21 @@ class AdamPlan:
                                        int(steps_per_update), int(num_updates), 0)
 
 
+def _check_adam_arenas(who: str, plan: AdamPlan, params_bf16: Optional[torch.Tensor], **arenas: torch.Tensor) -> None:
+    """The fp32 arenas (and the bf16 shadow) must be contiguous, of the right dtype and hold every segment of the plan."""
+    named = list(arenas.items()) + ([("params_bf16", params_bf16)] if params_bf16 is not None else [])
+    for name, t in named:
+        want = torch.bfloat16 if name == "params_bf16" else torch.float32
+        if t.dtype != want or not t.is_contiguous():
+            raise StxError(f"{who}: {name} must be a contiguous {want} tensor (got {t.dtype}"
+                           f"{'' if t.is_contiguous() else ', not contiguous'})")
+        if t.numel() < plan.end:
+            raise StxError(f"{who}: {name} holds {t.numel()} elements, the last optimiser segment ends at {plan.end}")
+
+
 def clip_adam_step(plan: AdamPlan, params: torch.Tensor, grads: torch.Tensor, mu: torch.Tensor, nu: torch.Tensor,
                    grad_scale: float = 1.0, params_bf16: Optional[torch.Tensor] = None, prenorm: bool = False) -> None:
+    _check_adam_arenas("clip_adam_step", plan, params_bf16, params=params, grads=grads, mu=mu, nu=nu)
     _need_cuda(params, grads, mu, nu, params_bf16)
     plan.hyper.grad_scale = float(grad_scale)
     plan.hyper.prenorm = int(bool(prenorm))
@@ -478,6 +513,7 @@ class PeerGradBuffers:
 def allreduce_clip_adam_step(plan: AdamPlan, peers: PeerGradBuffers, which: int, params: torch.Tensor, mu: torch.Tensor,
                              nu: torch.Tensor, params_bf16: Optional[torch.Tensor] = None) -> None:
     """Fused mean all-reduce of gradient arena `which` (0/1, ping-pong) + clip + Adam on every rank."""
+    _check_adam_arenas("allreduce_clip_adam_step", plan, params_bf16, params=params, mu=mu, nu=nu)
     _need_cuda(params, mu, nu, params_bf16)
     plan.hyper.grad_scale = 1.0 / peers.world
     plan.hyper.prenorm = 0

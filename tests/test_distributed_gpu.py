@@ -166,6 +166,7 @@ def test_fused_allreduce_kernel_on_one_device(world, mode):
     Three calls, so that the generation counter, bias correction and LR schedule advance."""
     from oracle import ppo_oracle as O
     from stoix_b200 import _lib, ops
+    from tests import adam_reference as AR
 
     dev = torch.device("cuda", 0)
     rng = np.random.default_rng(world)
@@ -190,6 +191,12 @@ def test_fused_allreduce_kernel_on_one_device(world, mode):
     ref_p = [p0[:n_a].astype(np.float64), p0[coff:coff + n_c].astype(np.float64)]
     ref_st = [O.AdamState(np.zeros(n_a), np.zeros(n_a)), O.AdamState(np.zeros(n_c), np.zeros(n_c))]
     P = lambda t: C.c_void_p(t.data_ptr())
+    # per-step check against tests/adam_reference.py: the reduced gradient each rank applied is the fp32 sum in rank order; the
+    # two-shot form's threads square and sum ceil(slice / (8 blocks x 256 threads)) float4 items of the arena in fp32
+    h = AR.Hyper(grad_scale=1.0 / world, decay=True, steps_per_update=2, num_updates=4)
+    chunk = -(-(total // 4) // world)
+    items = [-(-chunk // (8 * 256))] * len(segs) if mode == 2 else None
+    host = lambda t: t.detach().cpu().numpy()
     for call in range(1, 4):
         g_np = [np.zeros(total, np.float32) for _ in range(world)]
         for r in range(world):
@@ -197,6 +204,7 @@ def test_fused_allreduce_kernel_on_one_device(world, mode):
             g_np[r][coff:coff + n_c] = rng.standard_normal(n_c) * (0.5 if r == 0 else 0.05)
             ranks[r]["grads"].copy_(torch.tensor(g_np[r]))
         torch.cuda.synchronize()
+        pre = [dict(p=host(rk["params"]), mu=host(rk["mu"]), nu=host(rk["nu"]), counts=host(rk["plan"].counts)) for rk in ranks]
         for r in range(world):
             rk = ranks[r]
             rk["plan"].hyper.grad_scale = 1.0 / world
@@ -218,6 +226,16 @@ def test_fused_allreduce_kernel_on_one_device(world, mode):
             assert int(ranks[r]["pad"][slot + r].item()) == call  # its own announcement arrived in its own pad too
             if mode == 2:
                 assert ranks[r]["pad"][slot + 8:slot + 8 + world].cpu().tolist() == [call] * world
+        gsum32 = np.zeros(total, np.float32)
+        for r in range(world):   # acc += v[r] in rank order, fp32
+            gsum32 = gsum32 + g_np[r]
+        for r, rk in enumerate(ranks):
+            got = dict(p=host(rk["params"]), mu=host(rk["mu"]), nu=host(rk["nu"]), counts=host(rk["plan"].counts), gnorm=host(rk["plan"].gnorm))
+            g_applied = host(rk["gsum"])[:total]
+            for off, cnt, _, _ in segs:
+                np.testing.assert_array_equal(g_applied[off:off + cnt], gsum32[off:off + cnt], err_msg=f"virtual rank {r}: reduced gradient")
+            want = AR.step(pre[r]["p"], pre[r]["mu"], pre[r]["nu"], pre[r]["counts"], g_applied, segs, h, items=items)
+            AR.check(got, want, pre[r], label=f"mode {mode} world {world} rank {r} call {call}")
         mean = np.mean(np.stack([g.astype(np.float64) for g in g_np]), axis=0)
         for s, (off, cnt, lr, mgn) in enumerate(segs):
             k = ref_st[s].sched_count // 2

@@ -157,3 +157,58 @@ def test_recurrent_and_sac_arena_layouts_match_the_oracle_flat_order():
     lay = sac_arena_layout(sa, sq)
     assert all(lay[k] % 8 == 0 for k in ("actor", "q1", "q2", "alpha", "total")) and lay["q1"] >= sa.param_count
     assert lay["q2"] - lay["q1"] >= sq.param_count == 204801 and lay["q_block"] == lay["alpha"] - lay["q1"] and lay["total"] == lay["alpha"] + 8
+
+
+def test_adam_plan_refuses_bad_segment_tables(monkeypatch):
+    """include/stx.h: a segment offset is a float4 index (multiple of 4), counts >= 1, segments disjoint, 1..8 of them.  The table
+    is refused before anything is allocated or the library is called (a misaligned plan would fault on the device instead)."""
+    from stoix_b200 import _lib, ops
+
+    def boom(*a, **k):
+        raise AssertionError("AdamPlan allocated or called the library before checking its segment table")
+
+    ok = ops.AdamPlan([(0, 10, 1e-3, 0.5), (12, 1, 1e-3, 0.5)], "cpu")   # adjacent after padding: accepted
+    assert ok.end == 13 and ok.nseg == 2
+    monkeypatch.setattr(_lib, "load", boom)
+    monkeypatch.setattr(torch, "zeros", boom)
+    monkeypatch.setattr(torch, "from_numpy", boom)
+    bad = {
+        "not a non-negative multiple of 4": [[(2, 10, 1e-3, 0.5)], [(0, 8, 1e-3, 0.5), (10, 4, 1e-3, 0.5)], [(-4, 8, 1e-3, 0.5)]],
+        "has count": [[(0, 0, 1e-3, 0.5)], [(0, 8, 1e-3, 0.5), (8, -3, 1e-3, 0.5)]],
+        "overlap": [[(0, 9, 1e-3, 0.5), (8, 4, 1e-3, 0.5)], [(16, 4, 1e-3, 0.5), (0, 20, 1e-3, 0.5)], [(0, 4, 1e-3, 0.5), (0, 4, 1e-3, 0.5)]],
+        "segments": [[], [(8 * i, 4, 1e-3, 0.5) for i in range(9)]],
+    }
+    for msg, tables in bad.items():
+        for segs in tables:
+            with pytest.raises(_lib.StxError, match=msg):
+                ops.AdamPlan(segs, "cpu")
+
+
+def test_clip_adam_step_refuses_arenas_that_do_not_fit_the_plan(monkeypatch):
+    """clip_adam_step checks dtype, contiguity and length of every arena against the plan before it calls the library."""
+    from stoix_b200 import _lib, ops
+
+    plan = ops.AdamPlan([(0, 10, 1e-3, 0.5), (16, 5, 1e-3, 0.5)], "cpu")   # last segment ends at 21
+
+    def boom(*a, **k):
+        raise AssertionError("clip_adam_step called the library before checking its arenas")
+
+    monkeypatch.setattr(_lib, "load", boom)
+    f = lambda n=24, dt=torch.float32: torch.zeros(n, dtype=dt)
+    good = dict(params=f(), grads=f(), mu=f(), nu=f())
+    cases = [
+        (dict(params=f(dt=torch.float64)), "params must be a contiguous torch.float32"),
+        (dict(grads=f(dt=torch.bfloat16)), "grads must be a contiguous torch.float32"),
+        (dict(mu=f(48)[::2]), "mu must be a contiguous"),
+        (dict(nu=f(20)), "nu holds 20 elements"),
+        (dict(grads=f(21 - 1)), "grads holds 20 elements"),
+        (dict(params_bf16=f()), "params_bf16 must be a contiguous torch.bfloat16"),
+        (dict(params_bf16=f(16, torch.bfloat16)), "params_bf16 holds 16 elements"),
+    ]
+    for override, msg in cases:
+        kw = dict(good, **override)
+        with pytest.raises(_lib.StxError, match=msg):
+            ops.clip_adam_step(plan, kw["params"], kw["grads"], kw["mu"], kw["nu"], params_bf16=kw.get("params_bf16"))
+    # arenas that fit reach the next check: CPU tensors have no kernel
+    with pytest.raises(_lib.StxError, match="only on CUDA"):
+        ops.clip_adam_step(plan, f(21), f(21), f(21), f(21), params_bf16=f(21, torch.bfloat16))
