@@ -552,6 +552,63 @@ int stx_ppo_variant_continuous_minibatch_grads(const StxMlp* actor, const StxMlp
                                                float* grad_arena, float* metrics, int precision, void* workspace, size_t workspace_bytes,
                                                void* stream);
 
+/* ------------------------------------------------------------------ PQN: parallel Q-networks (fp32) ------------
+ * The Q-learning system of stoix/systems/q_learning/ff_pqn.py: epsilon-greedy rollout, Q(lambda) targets, the l2 / Huber Q loss
+ * and optax.chain(clip_by_global_norm, radam).
+ *
+ * stx_epsilon_greedy: distrax.EpsilonGreedy(preferences=q, epsilon).sample / .mode (stoix/networks/heads.py:202-217, ff_pqn.py:54-95)
+ *   on q (E, A) rows.  epsilon is evaluated on the device from the optimiser count word `count` (nullable: count 0):
+ *     update_no = *count / sched->steps_per_update                                          (ff_pqn.py:72)
+ *     decay:    optax.linear_schedule(init_value, end_value, transition_steps) at update_no, in fp32:
+ *               c = min(max(update_no, 0), transition_steps); eps = (init - end) * (1 - c / transition_steps) + end
+ *               (transition_steps <= 0: eps = init_value)                                   (ff_pqn.py:286-297)
+ *     constant: eps = end_value
+ *   so a captured CUDA graph follows the schedule as the optimiser count advances.  Draw: two words (w0, w1) of Philox4x32-10
+ *   keyed by seed with counter (row, call = offset + *dev_counter, as stx_categorical): explore if (w0 >> 8) * 2^-24 < eps
+ *   (exact in fp32; always true at eps = 1), the action then being (w1 * A) >> 32 in 64-bit integers; otherwise the
+ *   ((w1 * n_ties) >> 32)-th of the n_ties maximal indices.  mode != 0: the first maximal index (distrax mode()), no draw.
+ *   epsilon_out / update_no_out (nullable, (E)) record the values for the episode metrics (ff_pqn.py:85-86).
+ * stx_q_lambda_f32: batch_q_lambda (stoix/utils/multistep.py:533-569) over batch_lambda_returns (:314-408), time-major, on the
+ *   rollout's stored flags: q_t (T, E, A) = Q of the successor rows, v_t = max_a q_t, d_t = gamma (1 - (done | truncated)),
+ *   G_t = r_t + d_t [(1 - lambda) v_t + lambda G_{t+1}], the scan starting from v_t[T-1].  Evaluated as K2's chunked affine
+ *   scan G_t = a_t + c_t G_{t+1} with a_t = r_t + d_t (1 - lambda) v_t, c_t = d_t lambda (last step: a = r + d v, c = 0).
+ *   Writes targets (T, E) only.
+ * stx_lambda_returns_f32: the generic face: float discount_t (T, E), v_t (T, E, A) reduced by max over A (A = 1:
+ *   batch_lambda_returns itself), optional per-element lambda_t (NULL -> scalar lambda_).
+ * stx_q_loss_grads: _q_loss_fn (ff_pqn.py:139-162) on Q rows computed elsewhere: row m of q (mb, A) pairs with batch row idx[m]
+ *   (or row0 + m) of action / targets; td = targets - q[m, a]; loss = rlax.l2_loss(td) = td^2 / 2, or rlax.huber_loss(td, delta)
+ *   when delta > 0; writes d q = d mean(loss) / d q: -clip(td, -delta, delta) / mb (l2: -td / mb) in column a, 0 elsewhere;
+ *   metrics[0] += weight * mean(loss) (q_loss).  scratch: stx_ppo_head_scratch_bytes(mb), zeroed once.
+ * stx_clip_radam_step: stx_clip_adam_step with optax.scale_by_radam (b1, b2, eps, eps_root, threshold; no nesterov) in place of
+ *   scale_by_adam (ff_pqn.py:263-267): rho_inf = 2 / (1 - b2) - 1, rho_t = rho_inf - 2 t b2^t / (1 - b2^t) with t = count + 1;
+ *   update = r_t mhat / (sqrt(vhat + eps_root) + eps), r_t = sqrt((rho_t - 4)(rho_t - 2) rho_inf / ((rho_inf - 4)(rho_inf - 2) rho_t))
+ *   if rho_t >= threshold, else mhat.  rho_t and r_t are evaluated in double precision (in fp32 rho_t cancels catastrophically);
+ *   everything else as stx_clip_adam_step.  hyper->adam.prenorm must be 0. */
+typedef struct StxEpsilonSchedule {
+  float init_value;          /* 1.0 in ff_pqn */
+  float end_value;           /* system.training_epsilon (the constant schedule's value) */
+  float transition_steps;    /* arch.num_updates * system.exploration_fraction */
+  int32_t steps_per_update;  /* epochs * num_minibatches: optimiser steps per update */
+  int32_t decay;             /* system.decay_epsilon */
+  int32_t reserved;
+} StxEpsilonSchedule;
+typedef struct StxRadamHyper {
+  StxAdamHyper adam;  /* b1, b2, eps, grad_scale and the learning-rate schedule, as for stx_clip_adam_step */
+  float eps_root;     /* optax.radam default 0 */
+  float threshold;    /* optax.radam default 5 */
+} StxRadamHyper;
+int stx_epsilon_greedy(const float* q, int64_t E, int A, int mode, uint64_t seed, uint64_t offset, const uint64_t* dev_counter,
+                       const int32_t* count, const StxEpsilonSchedule* sched, int32_t* action, float* epsilon_out, int32_t* update_no_out,
+                       void* stream);
+int stx_q_lambda_f32(const float* q_t, int A, const float* r_t, const uint8_t* done, const uint8_t* truncated, int T, int E, float gamma,
+                     float lambda_, float* targets, void* stream);
+int stx_lambda_returns_f32(const float* r_t, const float* discount_t, const float* v_t, int A, const float* lambda_t, float lambda_, int T,
+                           int E, float* targets, void* stream);
+int stx_q_loss_grads(const float* q, const int32_t* idx, int64_t row0, const int32_t* action, const float* targets, int64_t mb, int A,
+                     float huber_delta, float* d_q, float* metrics, float weight, void* scratch, void* stream);
+int stx_clip_radam_step(float* param_arena, const float* grad_arena, float* mu, float* nu, int32_t* counts, const StxAdamSeg* segs, int nseg,
+                        const StxRadamHyper* hyper, void* params_bf16, float* gnorm_out, void* scratch, void* stream);
+
 /* Utility casts used by the bf16 path (obs / weight shadows). */
 int stx_cast_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream);
 

@@ -81,6 +81,25 @@ class StxFusedAdam(C.Structure):
     ]
 
 
+class StxRadamHyper(C.Structure):
+    _fields_ = [
+        ("adam", StxAdamHyper),
+        ("eps_root", C.c_float),
+        ("threshold", C.c_float),
+    ]
+
+
+class StxEpsilonSchedule(C.Structure):
+    _fields_ = [
+        ("init_value", C.c_float),
+        ("end_value", C.c_float),
+        ("transition_steps", C.c_float),
+        ("steps_per_update", C.c_int32),
+        ("decay", C.c_int32),
+        ("reserved", C.c_int32),
+    ]
+
+
 class StxReplay(C.Structure):
     _fields_ = [
         ("obs", C.c_void_p),
@@ -224,6 +243,12 @@ _SIGNATURES = {
     "stx_ppo_variant_continuous_minibatch_grads": (C.c_int, [C.POINTER(StxMlp), C.POINTER(StxMlp), C.POINTER(StxPpoBatch),
                                                              C.POINTER(StxTanhNormalPpo), C.POINTER(StxPpoVariant), C.c_int64, C.c_int64,
                                                              C.POINTER(StxPpoHyper), C.c_float, _P, _P, C.c_int, _P, C.c_size_t, _P]),
+    "stx_epsilon_greedy": (C.c_int, [_P, C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_uint64, _P, _P, C.POINTER(StxEpsilonSchedule), _P, _P, _P,
+                                     _P]),
+    "stx_q_lambda_f32": (C.c_int, [_P, C.c_int, _P, _P, _P, C.c_int, C.c_int, C.c_float, C.c_float, _P, _P]),
+    "stx_lambda_returns_f32": (C.c_int, [_P, _P, _P, C.c_int, _P, C.c_float, C.c_int, C.c_int, _P, _P]),
+    "stx_q_loss_grads": (C.c_int, [_P, _P, C.c_int64, _P, _P, C.c_int64, C.c_int, C.c_float, _P, _P, C.c_float, _P, _P]),
+    "stx_clip_radam_step": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.POINTER(StxRadamHyper), _P, _P, _P, _P]),
 }
 
 _lib = None

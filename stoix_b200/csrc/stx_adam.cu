@@ -74,21 +74,30 @@ __device__ __forceinline__ void grid_barrier(unsigned long long* arrive) {
   __syncthreads();
 }
 
+// The update rule of phase 2: Adam (stx_clip_adam_step and the fused all-reduce forms) or, with RADAM, optax.scale_by_radam
+// (stx_clip_radam_step).  The rectifier of RAdam depends on the step count only; it is derived once per segment in double
+// precision next to the bias corrections: rho_t = rho_inf - 2 t b2^t / (1 - b2^t) subtracts two numbers of nearly the same size
+// (rho_inf = 1999 at b2 = 0.999), which in fp32 puts a relative error of 1.8e-3 on r_t at t = 6 (DESIGN.md section 2, tolerance scheme).
+struct RadamArgs {
+  float eps_root, threshold;
+};
+
 // PEER: 0 = local gradients; 1 = one-shot all-reduce (every rank loads all W arenas); 2 = two-shot (rank r reduces slice r from
 // the W arenas and stores the result into every rank's buffer: (W-1)/W of the arena in and out instead of W-1 arenas in; the
 // second cross-rank hand-shake doubles as the grid barrier of the norm, whose per-rank partial sums travel with the slices).
-template <bool PRENORM, int PEER>
+template <bool PRENORM, int PEER, bool RADAM = false>
 __global__ void __launch_bounds__(kAdamThreads)
     clip_adam_kernel(float* __restrict__ P, const float* G, float* __restrict__ MU,
                      float* __restrict__ NU, int32_t* __restrict__ counts,
                      const StxAdamSeg* __restrict__ segs, int nseg, StxAdamHyper h,
                      __nv_bfloat16* __restrict__ P16, float* __restrict__ gnorm_out,
-                     AdamScratch* scratch, const PeerSync ps) {
+                     AdamScratch* scratch, const PeerSync ps, const RadamArgs rx) {
   double* partials = reinterpret_cast<double*>(scratch + 1);
   unsigned long long* finish = reinterpret_cast<unsigned long long*>(partials + kAdamMaxSegs * kNumSMs) + 2;  // after the peer words
   __shared__ double sred[32];
   __shared__ StxAdamSeg s_seg[kAdamMaxSegs];
   __shared__ float s_gs[kAdamMaxSegs], s_bc1[kAdamMaxSegs], s_bc2[kAdamMaxSegs], s_lr[kAdamMaxSegs], s_gn[kAdamMaxSegs];
+  __shared__ float s_rect[kAdamMaxSegs];  // RADAM: r_t, or 0 on the un-rectified branch (rho_t < threshold)
   const int gtid = blockIdx.x * blockDim.x + threadIdx.x;
   const int gthreads = gridDim.x * blockDim.x;
   griddep_launch();
@@ -300,6 +309,15 @@ __global__ void __launch_bounds__(kAdamThreads)
       s_bc2[s] = 1.0f - powf(h.b2, (float)c);
       s_lr[s] = lr;
       s_gn[s] = g_norm;
+      if constexpr (RADAM) {  // optax.scale_by_radam, rectifier in double precision
+        const double b2 = (double)h.b2, t = (double)c;
+        const double rho_inf = 2.0 / (1.0 - b2) - 1.0;
+        const double b2t = pow(b2, t);
+        const double rho = rho_inf - 2.0 * t * b2t / (1.0 - b2t);
+        s_rect[s] = rho >= (double)rx.threshold
+                        ? (float)sqrt((rho - 4.0) * (rho - 2.0) * rho_inf / ((rho_inf - 4.0) * (rho_inf - 2.0) * rho))
+                        : 0.f;
+      }
     }
   }
   __syncthreads();
@@ -307,6 +325,16 @@ __global__ void __launch_bounds__(kAdamThreads)
   for (int s = 0; s < nseg; ++s) {
     const StxAdamSeg seg = s_seg[s];
     const float gs = s_gs[s], bc1 = s_bc1[s], bc2 = s_bc2[s], lr = s_lr[s];
+    const float rect = RADAM ? s_rect[s] : 0.f;
+    // the step direction of one element: Adam's, or RAdam's (r_t mhat / (sqrt(vhat + eps_root) + eps), else mhat)
+    auto direction = [&](float me, float ve) -> float {
+      if constexpr (RADAM) {
+        const float mh = me / bc1;
+        return rect > 0.f ? rect * mh / (sqrtf(ve / bc2 + rx.eps_root) + h.eps) : mh;
+      } else {
+        return (me / bc1) / (sqrtf(ve / bc2) + h.eps);
+      }
+    };
     float* p = P + seg.offset;
     float* mu = MU + seg.offset;
     float* nu = NU + seg.offset;
@@ -327,7 +355,7 @@ __global__ void __launch_bounds__(kAdamThreads)
       for (int k = 0; k < 4; ++k) {
         me[k] = h.b1 * me[k] + ob1 * ge[k];
         ve[k] = h.b2 * ve[k] + ob2 * ge[k] * ge[k];
-        const float u = (me[k] / bc1) / (sqrtf(ve[k] / bc2) + h.eps);
+        const float u = direction(me[k], ve[k]);
         pe[k] = pe[k] - lr * u;
       }
       st_hint(reinterpret_cast<float4*>(mu) + i, make_float4(me[0], me[1], me[2], me[3]), pol_keep);
@@ -345,7 +373,7 @@ __global__ void __launch_bounds__(kAdamThreads)
       const float ge = g[i] * gs;
       const float me = h.b1 * mu[i] + ob1 * ge;
       const float ve = h.b2 * nu[i] + ob2 * ge * ge;
-      const float u = (me / bc1) / (sqrtf(ve / bc2) + h.eps);
+      const float u = direction(me, ve);
       const float pn = p[i] - lr * u;
       mu[i] = me, nu[i] = ve, p[i] = pn;
       if (P16) P16[seg.offset + i] = __float2bfloat16_rn(pn);
@@ -409,13 +437,32 @@ extern "C" int stx_clip_adam_step(float* param_arena, const float* grad_arena, f
   if (hyper->prenorm)
     STX_CUDA_OK(launch_pdl(clip_adam_kernel<true, 0>, dim3(grid), dim3(kAdamThreads), 0, (cudaStream_t)stream, param_arena, grad_arena,
                            mu, nu, counts, segs, nseg, *hyper, reinterpret_cast<__nv_bfloat16*>(params_bf16), gnorm_out,
-                           reinterpret_cast<AdamScratch*>(scratch), none));
+                           reinterpret_cast<AdamScratch*>(scratch), none, RadamArgs{}));
   else
     STX_CUDA_OK(launch_pdl(clip_adam_kernel<false, 0>, dim3(grid), dim3(kAdamThreads), 0, (cudaStream_t)stream, param_arena, grad_arena,
                            mu, nu, counts, segs, nseg, *hyper, reinterpret_cast<__nv_bfloat16*>(params_bf16), gnorm_out,
-                           reinterpret_cast<AdamScratch*>(scratch), none));
+                           reinterpret_cast<AdamScratch*>(scratch), none, RadamArgs{}));
   STX_LAUNCH_OK();
   (void)adam_grid;
+  return STX_OK;
+}
+
+// clip + RAdam: the same launch as stx_clip_adam_step with the RAdam rule (PQN, ff_pqn.py:263-267).
+extern "C" int stx_clip_radam_step(float* param_arena, const float* grad_arena, float* mu, float* nu, int32_t* counts, const StxAdamSeg* segs,
+                                   int nseg, const StxRadamHyper* hyper, void* params_bf16, float* gnorm_out, void* scratch, void* stream) {
+  STX_REQUIRE(param_arena && grad_arena && mu && nu && counts && segs && hyper && scratch, STX_E_ARG, "stx_clip_radam_step: null pointer");
+  STX_REQUIRE(nseg >= 1 && nseg <= kAdamMaxSegs, STX_E_SHAPE, "stx_clip_radam_step: nseg=%d (max %d)", nseg, kAdamMaxSegs);
+  STX_REQUIRE(aligned16(param_arena) && aligned16(grad_arena) && aligned16(mu) && aligned16(nu), STX_E_ALIGN,
+              "stx_clip_radam_step: arenas must be 16-byte aligned");
+  STX_REQUIRE(hyper->adam.steps_per_update > 0 && hyper->adam.num_updates > 0, STX_E_ARG,
+              "stx_clip_radam_step: steps_per_update/num_updates must be positive");
+  STX_REQUIRE(!hyper->adam.prenorm, STX_E_ARG, "stx_clip_radam_step: prenorm is not available with RAdam");
+  STX_REQUIRE(hyper->eps_root >= 0.f, STX_E_ARG, "stx_clip_radam_step: eps_root=%g must be >= 0", (double)hyper->eps_root);
+  const PeerSync none{};
+  STX_CUDA_OK(launch_pdl(clip_adam_kernel<false, 0, true>, dim3(kNumSMs), dim3(kAdamThreads), 0, (cudaStream_t)stream, param_arena, grad_arena,
+                         mu, nu, counts, segs, nseg, hyper->adam, reinterpret_cast<__nv_bfloat16*>(params_bf16), gnorm_out,
+                         reinterpret_cast<AdamScratch*>(scratch), none, RadamArgs{hyper->eps_root, hyper->threshold}));
+  STX_LAUNCH_OK();
   return STX_OK;
 }
 
@@ -453,7 +500,7 @@ extern "C" int stx_allreduce_clip_adam_step(float* param_arena, const float* con
   ps.gsum = gsum, ps.world = world, ps.rank = rank;
   STX_CUDA_OK(launch_pdl(clip_adam_kernel<false, 1>, dim3(kNumSMs), dim3(kAdamThreads), 0, (cudaStream_t)stream, param_arena,
                          static_cast<const float*>(gsum), mu, nu, counts, segs, nseg, *hyper,
-                         reinterpret_cast<__nv_bfloat16*>(params_bf16), gnorm_out, reinterpret_cast<AdamScratch*>(scratch), ps));
+                         reinterpret_cast<__nv_bfloat16*>(params_bf16), gnorm_out, reinterpret_cast<AdamScratch*>(scratch), ps, RadamArgs{}));
   STX_LAUNCH_OK();
   return STX_OK;
 }
@@ -488,7 +535,7 @@ extern "C" int stx_allreduce2_clip_adam_step(float* param_arena, const float* co
   ps.gsum = peer_gsum[rank], ps.world = world, ps.rank = rank, ps.total4 = arena_len / 4;
   STX_CUDA_OK(launch_pdl(clip_adam_kernel<false, 2>, dim3(grid > 0 ? grid : kNumSMs), dim3(kAdamThreads), 0, (cudaStream_t)stream, param_arena,
                          static_cast<const float*>(ps.gsum), mu, nu, counts, segs, nseg, *hyper, reinterpret_cast<__nv_bfloat16*>(params_bf16),
-                         gnorm_out, reinterpret_cast<AdamScratch*>(scratch), ps));
+                         gnorm_out, reinterpret_cast<AdamScratch*>(scratch), ps, RadamArgs{}));
   STX_LAUNCH_OK();
   return STX_OK;
 }

@@ -20,7 +20,10 @@ namespace {
 
 constexpr int kChunks = 32;  // chunk lanes per block == warp width (suffix scan by shuffles)
 
+// An input form's load yields, per element, the affine map acc_t = d + c * acc_{t+1} and the value v the targets add to acc.
+// kTargetsOnly: the form's result is acc itself, stored as the targets (no advantages, no statistics).
 struct PpoIn {  // exactly what ff_ppo.py:164-169 feeds
+  static constexpr bool kTargetsOnly = false;
   const float *reward, *v_tm1, *v_t;
   const uint8_t *done, *trunc;
   float gamma, lambda, reward_scale;
@@ -61,6 +64,7 @@ struct PpoIn {  // exactly what ff_ppo.py:164-169 feeds
 };
 
 struct GenericIn {  // float discount / lambda / truncation arrays (multistep.py:97-105)
+  static constexpr bool kTargetsOnly = false;
   const float *r, *disc, *lam_t, *v_tm1, *v_t, *trunc;
   float lambda;
   template <int VEC>
@@ -73,6 +77,38 @@ struct GenericIn {  // float discount / lambda / truncation arrays (multistep.py
       v[k] = __ldg(v_tm1 + off + k);
       d[k] = __ldg(r + off + k) + dk * __ldg(v_t + off + k) - v[k];
       c[k] = dk * lk * (1.0f - tk);
+    }
+  }
+};
+
+// Lambda returns (batch_lambda_returns, multistep.py:384-408) with v_t = max over the A columns of q (batch_q_lambda,
+// :559-569; A = 1: v_t itself):  G_t = r_t + d_t [(1 - lambda) v_t + lambda G_{t+1}], the scan starting from G_T = v_t[T-1], i.e.
+// the affine map a_t = r_t + d_t (1 - lambda) v_t, c_t = d_t lambda, and on the last step a = r + d v, c = 0.  The discount is
+// either a float array or gamma (1 - (done | truncated)) from the rollout's flags (ff_pqn.py:107-109, done = timestep.last()).
+struct LambdaIn {
+  static constexpr bool kTargetsOnly = true;
+  const float *q, *r, *disc, *lam_t;  // q: (T, E, A); disc / lam_t nullable
+  const uint8_t *done, *trunc;         // used when disc is NULL
+  int A;
+  float gamma, lambda;
+  int64_t last;                        // flat offset of the first element of step T-1
+  template <int VEC>
+  __device__ __forceinline__ void load(int64_t off, float* d, float* c, float* v) const {
+#pragma unroll
+    for (int k = 0; k < VEC; ++k) {
+      const int64_t i = off + k;
+      const float* row = q + i * A;
+      float vmax = __ldg(row);
+      for (int j = 1; j < A; ++j) {  // NaN-propagating max, as jnp.max (fmaxf would drop a NaN)
+        const float x = __ldg(row + j);
+        vmax = (x > vmax || x != x) ? x : vmax;
+      }
+      const float dk = disc ? __ldg(disc + i) : ((__ldg(done + i) | __ldg(trunc + i)) ? 0.f : gamma);
+      const float lk = lam_t ? __ldg(lam_t + i) : lambda;
+      const bool is_last = i >= last;
+      d[k] = __ldg(r + i) + dk * ((is_last ? 1.0f : 1.0f - lk) * vmax);
+      c[k] = is_last ? 0.f : dk * lk;
+      v[k] = 0.f;
     }
   }
 };
@@ -159,7 +195,17 @@ __global__ void __launch_bounds__(QUADS* kChunks, MINB)
         av[k] = fmaf(a[j][k], sA[chunk][q * VEC + k], b[j][k]);
         tv[k] = v[j][k] + av[k];  // multistep.py:132: targets use the un-standardised advantage
       }
-      if (env_ok && t < T) {
+      if constexpr (In::kTargetsOnly) {
+        if (env_ok && t < T) {
+          const int64_t off = (int64_t)t * E + e0;
+          if constexpr (VEC == 4)
+            stg_stream4(tgt + off, make_float4(av[0], av[1], av[2], av[3]));
+          else if constexpr (VEC == 2)
+            stg_stream2(tgt + off, make_float2(av[0], av[1]));
+          else
+            tgt[off] = av[0];
+        }
+      } else if (env_ok && t < T) {
         const int64_t off = (int64_t)t * E + e0;
         if constexpr (VEC == 4) {
           stg_stream4(adv + off, make_float4(av[0], av[1], av[2], av[3]));
@@ -452,12 +498,14 @@ int launch_gae_tma(const PpoIn& in, int T, int E, int want, float* adv, float* t
               : launch_gae_tma_shape<32, 128>(in, T, E, want, adv, tgt, stats, partials, counter, st);
 }
 int launch_gae_tma(const GenericIn&, int, int, int, float*, float*, float*, double2*, unsigned int*, cudaStream_t) { return 1; }
+int launch_gae_tma(const LambdaIn&, int, int, int, float*, float*, float*, double2*, unsigned int*, cudaStream_t) { return 1; }
 
 template <class In>
 int launch_gae(const In& in, int T, int E, bool vec4, int standardize, float* adv, float* tgt,
                float* stats, void* scratch, cudaStream_t st) {
+  // (the statistics' scratch; the lambda-return forms take none)
   unsigned int* counter = reinterpret_cast<unsigned int*>(scratch);
-  double2* partials = reinterpret_cast<double2*>(reinterpret_cast<char*>(scratch) + 16);
+  double2* partials = scratch ? reinterpret_cast<double2*>(reinterpret_cast<char*>(scratch) + 16) : nullptr;
   const int want = standardize != 0;
   bool done_tma = false;
   // large shapes: the TMA-pipelined persistent kernel (codes 500 / 501 force its 32x128 / 64x64 tiles, any other non-zero code disables it)
@@ -571,4 +619,22 @@ extern "C" int stx_gae_generic_f32(const float* r_t, const float* discount_t, co
   const bool vec4 = (E % 4 == 0) && aligned16(adv) && aligned16(targets);
   GenericIn in{r_t, discount_t, lambda_t, v_tm1, v_t, truncation_t, lambda_};
   return launch_gae(in, T, E, vec4, standardize, adv, targets, stats, scratch, (cudaStream_t)stream);
+}
+
+extern "C" int stx_q_lambda_f32(const float* q_t, int A, const float* r_t, const uint8_t* done, const uint8_t* truncated, int T, int E,
+                                float gamma, float lambda_, float* targets, void* stream) {
+  STX_REQUIRE(q_t && r_t && done && truncated && targets, STX_E_ARG, "stx_q_lambda_f32: null pointer");
+  STX_REQUIRE(T > 0 && E > 0 && A > 0, STX_E_ARG, "stx_q_lambda_f32: T=%d E=%d A=%d must be positive", T, E, A);
+  LambdaIn in{q_t, r_t, nullptr, nullptr, done, truncated, A, gamma, lambda_, (int64_t)(T - 1) * E};
+  const bool vec4 = (E % 4 == 0) && aligned16(targets);
+  return launch_gae(in, T, E, vec4, 0, nullptr, targets, nullptr, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int stx_lambda_returns_f32(const float* r_t, const float* discount_t, const float* v_t, int A, const float* lambda_t, float lambda_,
+                                      int T, int E, float* targets, void* stream) {
+  STX_REQUIRE(r_t && discount_t && v_t && targets, STX_E_ARG, "stx_lambda_returns_f32: null pointer");
+  STX_REQUIRE(T > 0 && E > 0 && A > 0, STX_E_ARG, "stx_lambda_returns_f32: T=%d E=%d A=%d must be positive", T, E, A);
+  LambdaIn in{v_t, r_t, discount_t, lambda_t, nullptr, nullptr, A, 0.f, lambda_, (int64_t)(T - 1) * E};
+  const bool vec4 = (E % 4 == 0) && aligned16(targets);
+  return launch_gae(in, T, E, vec4, 0, nullptr, targets, nullptr, nullptr, (cudaStream_t)stream);
 }

@@ -131,6 +131,58 @@ __global__ void categorical_kernel(const float* __restrict__ logits, int64_t E, 
   }
 }
 
+// ---- epsilon-greedy head (PQN) -------------------------------------------------------------
+// distrax.EpsilonGreedy(preferences=q, epsilon): (1 - eps) uniform over the argmax set + eps / A.  Integer arithmetic on two
+// Philox words, so an oracle reproduces every action bit for bit (layout in include/stx.h).  The schedule is evaluated with
+// explicitly rounded fp32 operations (no contraction), so it equals a literal fp32 evaluation.
+__device__ __forceinline__ float epsilon_at(const StxEpsilonSchedule& s, int32_t update_no) {
+  if (!s.decay) return s.end_value;
+  if (!(s.transition_steps > 0.f)) return s.init_value;   // optax.polynomial_schedule with transition_steps <= 0
+  const float c = fminf(fmaxf((float)update_no, 0.f), s.transition_steps);
+  const float frac = __fsub_rn(1.0f, __fdiv_rn(c, s.transition_steps));
+  return __fadd_rn(__fmul_rn(__fsub_rn(s.init_value, s.end_value), frac), s.end_value);
+}
+
+__global__ void epsilon_greedy_kernel(const float* __restrict__ q, int64_t E, int A, int mode, uint64_t seed, uint64_t offset,
+                                      const uint64_t* __restrict__ dev_counter, const int32_t* __restrict__ count, StxEpsilonSchedule sched,
+                                      int32_t* __restrict__ action, float* __restrict__ eps_out, int32_t* __restrict__ upd_out) {
+  const int64_t e = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (e >= E) return;
+  const float* z = q + e * A;
+  float zmax = -INFINITY;
+  int first = 0, n_ties = 0;
+  for (int j = 0; j < A; ++j) {
+    const float v = z[j];
+    if (v > zmax) zmax = v, first = j, n_ties = 1;
+    else if (v == zmax) ++n_ties;
+  }
+  const int32_t upd = (count ? *count : 0) / sched.steps_per_update;   // ff_pqn.py:72: count // (epochs * num_minibatches)
+  const float eps = epsilon_at(sched, upd);
+  if (eps_out) eps_out[e] = eps;
+  if (upd_out) upd_out[e] = upd;
+  if (mode) {
+    action[e] = first;
+    return;
+  }
+  const uint64_t call = offset + (dev_counter ? *dev_counter : 0ull);
+  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+  const uint32_t c2 = (uint32_t)(call >> 32) ^ ((uint32_t)((uint64_t)e >> 32) << 16);
+  const uint4 r = Philox::rand4(make_uint4((uint32_t)e, (uint32_t)call, c2, 0x45475259u), key);
+  // (w0 >> 8) * 2^-24 is exact and below 1: eps = 1 always explores, eps = 0 never does
+  if ((float)(r.x >> 8) * (1.0f / 16777216.0f) < eps) {
+    action[e] = (int32_t)(((uint64_t)r.y * (uint64_t)A) >> 32);
+    return;
+  }
+  const int pick = (int)(((uint64_t)r.y * (uint64_t)n_ties) >> 32);   // the pick-th maximal index
+  int a = first;
+  for (int j = first, seen = 0; j < A; ++j)
+    if (z[j] == zmax && seen++ == pick) {
+      a = j;
+      break;
+    }
+  action[e] = a;
+}
+
 // ---- fp32 PPO minibatch: workspace carving -------------------------------------------------
 struct SimtPpoWs {
   float* acts[STX_MAX_LAYERS + 1];  // pre-activation Dense outputs U_i of the torso layers, index 1..n-1
@@ -353,6 +405,18 @@ extern "C" int stx_mlp_backward(const StxMlp* m, const float* x, int64_t ldx, co
   cudaStream_t st = (cudaStream_t)stream;
   STX_CUDA_OK(cudaMemcpyAsync(ws.dhead, d_out, sizeof(float) * (size_t)M * m->sizes[m->n_layers], cudaMemcpyDeviceToDevice, st));
   return simt_backward(m, x, ldx, row_idx, M, ws, grad_weight, net_grad, overwrite, st, d_input);
+}
+
+extern "C" int stx_epsilon_greedy(const float* q, int64_t E, int A, int mode, uint64_t seed, uint64_t offset, const uint64_t* dev_counter,
+                                  const int32_t* count, const StxEpsilonSchedule* sched, int32_t* action, float* epsilon_out,
+                                  int32_t* update_no_out, void* stream) {
+  STX_REQUIRE(q && sched && action, STX_E_ARG, "stx_epsilon_greedy: null pointer");
+  STX_REQUIRE(E > 0 && A > 0, STX_E_SHAPE, "stx_epsilon_greedy: E=%lld A=%d", (long long)E, A);
+  STX_REQUIRE(sched->steps_per_update > 0, STX_E_ARG, "stx_epsilon_greedy: steps_per_update=%d must be positive", sched->steps_per_update);
+  epsilon_greedy_kernel<<<(unsigned)((E + 255) / 256), 256, 0, (cudaStream_t)stream>>>(q, E, A, mode, seed, offset, dev_counter, count, *sched,
+                                                                                         action, epsilon_out, update_no_out);
+  STX_LAUNCH_OK();
+  return STX_OK;
 }
 
 extern "C" int stx_categorical(const float* logits, int64_t E, int A, int sample, uint64_t seed,

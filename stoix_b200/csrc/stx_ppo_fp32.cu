@@ -1,6 +1,7 @@
 // The PPO losses of the fp32 path: the minibatch entries (actor forward, actor loss, actor backward, then the critic half),
 // the loss heads on precomputed network outputs, the value-only and KL faces, and the tanh-Normal rollout faces.  The bf16
-// minibatch (stx_tc_ppo.cu) shares only the validation here.  Kernels: stx_ppo_loss.cuh; networks: stx_mlp.cu.
+// minibatch (stx_tc_ppo.cu) shares only the validation here.  Kernels: stx_ppo_loss.cuh; networks: stx_mlp.cu.  PQN's Q loss
+// (stx_q_loss_grads) lives here too: it reuses the rows and the metric reduction of these losses.
 //
 // Reference: the _update_minibatch of stoix/systems/ppo/anakin/ff_ppo.py:184-247, ff_ppo_continuous.py:184-247,
 // ff_ppo_penalty.py:149-210, ff_ppo_penalty_continuous.py:149-210 and ff_dpo_continuous.py:148-170: each changes only the
@@ -184,6 +185,38 @@ int fp32_minibatch(const StxMlp* actor, const StxMlp* critic, const StxPpoBatch*
   const LossRows r{idx, mb_off, mb, hb.loss_partials, hb.counter, metrics, grad_weight};
   if (int rc = launch_critic_loss(r, hb.head, b->value, b->targets, hb.dhead, h->clip_eps, h->vf_coef, st)) return rc;
   return simt_net_backward(critic, x, D, idx, mb, workspace, grad_weight, grad_arena + coff, h->overwrite_grads, st);
+}
+
+// ---- PQN Q loss + its gradient with respect to the Q rows (one thread per minibatch row).
+//
+// Reference: _q_loss_fn of stoix/systems/q_learning/ff_pqn.py:139-162 under jax.grad, with rlax.l2_loss and rlax.huber_loss:
+//   td = target - q[a];  l2:    loss = td^2 / 2,                                 d loss / d q[a] = -td
+//                        Huber: loss = q^2 / 2 + delta (|td| - q), q = min(|td|, delta),  d loss / d q[a] = -clip(td, -delta, delta)
+// averaged over the minibatch (d q = that / mb; every other column 0).  At |td| = delta both Huber branches give the same value
+// (delta^2 / 2) and the same derivative (-td = -clip(td)), so the tie needs no rule.  Rows are read through the permutation and
+// the metric is reduced with the PPO losses' LossRows / reduce_metrics (stx_ppo_loss.cuh).
+__global__ void __launch_bounds__(256) q_loss_kernel(LossRows r, const float* __restrict__ q, const int32_t* __restrict__ action,
+                                                     const float* __restrict__ targets, int A, float delta, float* __restrict__ dq) {
+  const int64_t m = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  double s_loss = 0.0;
+  const float inv_m = 1.0f / (float)r.mb;
+  if (m < r.mb) {
+    const int64_t src = r.src(m);
+    const int a = action[src];
+    const float td = targets[src] - q[m * A + a];
+    float loss, g;
+    if (delta > 0.f) {  // rlax.huber_loss
+      const float ax = fabsf(td), quad = fminf(ax, delta), lin = ax - quad;
+      loss = 0.5f * quad * quad + delta * lin;
+      g = fminf(fmaxf(td, -delta), delta);
+    } else {  // rlax.l2_loss
+      loss = 0.5f * td * td;
+      g = td;
+    }
+    s_loss = (double)loss;
+    for (int j = 0; j < A; ++j) dq[m * A + j] = j == a ? -g * inv_m : 0.f;
+  }
+  reduce_metrics<1>({s_loss}, {0}, r);
 }
 
 }  // namespace
@@ -397,4 +430,14 @@ extern "C" int stx_ppo_variant_continuous_minibatch_grads(const StxMlp* actor, c
   g.behaviour = v->behaviour, g.tn = *head, g.kl_coef = v->kl_coef, g.dpo_alpha = v->dpo_alpha, g.dpo_beta = v->dpo_beta;
   return fp32_minibatch(actor, critic, b, mb_off, mb, h, grad_weight, grad_arena, metrics, workspace, g, tanh_normal_variant(v->kind),
                         (cudaStream_t)stream);
+}
+
+extern "C" int stx_q_loss_grads(const float* q, const int32_t* idx, int64_t row0, const int32_t* action, const float* targets, int64_t mb, int A,
+                                float huber_delta, float* d_q, float* metrics, float weight, void* scratch, void* stream) {
+  STX_REQUIRE(q && action && targets && d_q && metrics && scratch, STX_E_ARG, "stx_q_loss_grads: null pointer");
+  STX_REQUIRE(mb > 0 && A > 0 && row0 >= 0, STX_E_SHAPE, "stx_q_loss_grads: mb=%lld A=%d row0=%lld", (long long)mb, A, (long long)row0);
+  const LossRows r = scratch_rows(idx, row0, mb, metrics, weight, scratch);
+  q_loss_kernel<<<(unsigned)((mb + 255) / 256), 256, 0, (cudaStream_t)stream>>>(r, q, action, targets, A, huber_delta, d_q);
+  STX_LAUNCH_OK();
+  return STX_OK;
 }

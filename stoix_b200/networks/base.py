@@ -113,8 +113,14 @@ class FeedForwardActor(_FeedForward):
         super().__init__(action_head, torso, input_layer)
         self.action_head = action_head
 
-    def apply(self, params: ParamTree, observation: torch.Tensor):
-        return self.action_head.distribution(self._forward(params, observation))
+    def apply(self, params: ParamTree, observation: torch.Tensor, input_kwargs: Optional[Dict[str, Any]] = None,
+              torso_kwargs: Optional[Dict[str, Any]] = None, head_kwargs: Optional[Dict[str, Any]] = None):
+        """base.py:26-36.  head_kwargs reach the head's distribution (e.g. {"epsilon": e} for DiscreteQNetworkHead); the input layer and
+        the MLP torso take no keyword arguments, so input_kwargs / torso_kwargs must be empty."""
+        if input_kwargs or torso_kwargs:
+            raise TypeError("FeedForwardActor.apply: the input layer and the MLP torso take no keyword arguments")
+        out = self._forward(params, observation)
+        return self.action_head.distribution(out, **head_kwargs) if head_kwargs else self.action_head.distribution(out)
 
     __call__ = apply
 

@@ -1,7 +1,7 @@
 """CategoricalHead / NormalAffineTanhDistributionHead / ScalarCriticHead -- constructor-compatible with
 stoix/networks/heads.py:30-41, 44-65, 129-134, and the distribution objects the actor returns (tfd.Categorical's sample /
 log_prob / entropy / mode as used at ff_ppo.py:100-101,199,205; the tanh-Normal's sample / log_prob / mode as used at
-ff_sac.py:119-122,165-167)."""
+ff_sac.py:119-122,165-167); DiscreteQNetworkHead (heads.py:202-217) and its EpsilonGreedy (ff_pqn.py:79-82)."""
 from __future__ import annotations
 
 from typing import Optional, Sequence, Union
@@ -124,6 +124,41 @@ class AffineTanhNormal:
         A = self.head_out.shape[-1] // 2
         s, sh = (self.maximum - self.minimum) / 2.0, (self.minimum + self.maximum) / 2.0
         return sh + s * torch.tanh(self.head_out[..., :A])
+
+
+class EpsilonGreedy:
+    """distrax.EpsilonGreedy(preferences=q, epsilon) backed by stx_epsilon_greedy: with probability 1 - epsilon a uniformly chosen
+    maximal action, else a uniform action.  `sample` draws from Philox (seed, row, offset + *dev_counter); `mode` is the first
+    argmax."""
+
+    def __init__(self, preferences: torch.Tensor, epsilon: float):
+        self.preferences = preferences
+        self.epsilon = float(epsilon)
+        self._lead = tuple(preferences.shape[:-1])
+        self._flat = preferences.reshape(-1, preferences.shape[-1]).contiguous()
+
+    def _sched(self):
+        return ops.epsilon_schedule_struct(self.epsilon, self.epsilon, 0.0, decay=False)
+
+    def sample(self, seed=None, offset: int = 0, dev_counter: Optional[torch.Tensor] = None) -> torch.Tensor:
+        return ops.epsilon_greedy(self._flat, self._sched(), _seed_to_int(seed), offset, dev_counter).view(self._lead)
+
+    def mode(self) -> torch.Tensor:
+        return ops.epsilon_greedy(self._flat, self._sched(), mode=True).view(self._lead)
+
+
+class DiscreteQNetworkHead:
+    """heads.py:202-217: Dense(action_dim), orthogonal(1.0) kernel, returning EpsilonGreedy(q, epsilon); `epsilon` passed at apply
+    time (head_kwargs) overrides the constructor's."""
+
+    def __init__(self, action_dim: int, epsilon: float = 0.1, kernel_init: Optional[float] = None):
+        self.action_dim = int(action_dim)
+        self.epsilon = float(epsilon)
+        self.out_dim = self.action_dim
+        self.kernel_init_scale = 1.0 if kernel_init is None else float(kernel_init)
+
+    def distribution(self, q_values: torch.Tensor, epsilon: Optional[float] = None) -> EpsilonGreedy:
+        return EpsilonGreedy(q_values, self.epsilon if epsilon is None else epsilon)
 
 
 class NormalAffineTanhDistributionHead:

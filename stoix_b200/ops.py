@@ -407,10 +407,13 @@ class AdamPlan:
 
     segments: (offset, count, init_lr, max_grad_norm) per optimiser, 1..8 of them, disjoint.  The kernels read a segment as
     float4 items from `offset` on, so an offset must be a multiple of 4 floats (include/stx.h); a table that breaks this is
-    refused here, before anything is allocated, instead of becoming a misaligned vector access on the device."""
+    refused here, before anything is allocated, instead of becoming a misaligned vector access on the device.
+
+    rule: "adam" (optax.scale_by_adam, stx_clip_adam_step) or "radam" (optax.scale_by_radam with eps_root and threshold,
+    stx_clip_radam_step); clip_adam_step runs whichever the plan holds."""
 
     def __init__(self, segments: Sequence[Tuple[int, int, float, float]], device, b1=0.9, b2=0.999, eps=1e-5,
-                 decay=True, steps_per_update=1, num_updates=1):
+                 decay=True, steps_per_update=1, num_updates=1, rule: str = "adam", eps_root: float = 0.0, threshold: float = 5.0):
         import numpy as np
 
         segments = [tuple(s) for s in segments]
@@ -439,6 +442,12 @@ class AdamPlan:
         self.scratch = torch.zeros(int(_lib.load().stx_adam_scratch_bytes(self.nseg)), dtype=torch.uint8, device=device)
         self.hyper = _lib.StxAdamHyper(float(b1), float(b2), float(eps), 1.0, int(bool(decay)),
                                        int(steps_per_update), int(num_updates), 0)
+        if rule not in ("adam", "radam"):
+            raise StxError(f"AdamPlan: rule={rule!r}; expected 'adam' or 'radam'")
+        if rule == "radam" and eps_root < 0:
+            raise StxError(f"AdamPlan: eps_root={eps_root} must be >= 0")
+        self.rule = rule
+        self.radam = _lib.StxRadamHyper(self.hyper, float(eps_root), float(threshold)) if rule == "radam" else None
 
 
 def _check_adam_arenas(who: str, plan: AdamPlan, params_bf16: Optional[torch.Tensor], **arenas: torch.Tensor) -> None:
@@ -460,6 +469,16 @@ def clip_adam_step(plan: AdamPlan, params: torch.Tensor, grads: torch.Tensor, mu
     plan.hyper.grad_scale = float(grad_scale)
     plan.hyper.prenorm = int(bool(prenorm))
     lib = _lib.load()
+    if plan.rule == "radam":
+        if prenorm:
+            raise StxError("clip_adam_step: prenorm is not available with the radam rule")
+        plan.radam.adam = plan.hyper
+        _lib.check(
+            lib.stx_clip_radam_step(_p(params), _p(grads), _p(mu), _p(nu), _p(plan.counts), _p(plan.segs), plan.nseg,
+                                    C.byref(plan.radam), _p(params_bf16), _p(plan.gnorm), _p(plan.scratch), _stream()),
+            "stx_clip_radam_step",
+        )
+        return
     _lib.check(
         lib.stx_clip_adam_step(_p(params), _p(grads), _p(mu), _p(nu), _p(plan.counts), _p(plan.segs), plan.nseg,
                                C.byref(plan.hyper), _p(params_bf16), _p(plan.gnorm), _p(plan.scratch), _stream()),
@@ -513,6 +532,9 @@ class PeerGradBuffers:
 def allreduce_clip_adam_step(plan: AdamPlan, peers: PeerGradBuffers, which: int, params: torch.Tensor, mu: torch.Tensor,
                              nu: torch.Tensor, params_bf16: Optional[torch.Tensor] = None) -> None:
     """Fused mean all-reduce of gradient arena `which` (0/1, ping-pong) + clip + Adam on every rank."""
+    if plan.rule != "adam":
+        raise StxError("allreduce_clip_adam_step: the fused all-reduce kernels implement the adam rule only; use an NCCL all-reduce "
+                       "followed by clip_adam_step")
     _check_adam_arenas("allreduce_clip_adam_step", plan, params_bf16, params=params, mu=mu, nu=nu)
     _need_cuda(params, mu, nu, params_bf16)
     plan.hyper.grad_scale = 1.0 / peers.world
@@ -1161,3 +1183,93 @@ def lstm_sequence_backward(d_h_seq: torch.Tensor, reset: torch.Tensor, w_h: torc
         raise StxError("lstm_sequence_backward: d_h_seq (T, E, H) / d_gi (T, E, 4H) must be contiguous float32")
     _lib.check(_lib.load().stx_lstm_sequence_backward(_p(d_h_seq), _p(r8), _p(w_h), T, E, H, _p(ws), ws.numel(), _p(d_gi), _p(d_w_h), float(grad_weight),
                                                       int(bool(overwrite)), _p(d_carry0), _stream()), "stx_lstm_sequence_backward")
+
+
+# ------------------------------------------------------------------------------------------------
+# PQN: epsilon-greedy head, Q(lambda) targets, Q loss (stoix/systems/q_learning/ff_pqn.py)
+# ------------------------------------------------------------------------------------------------
+
+
+def epsilon_schedule_struct(init_value: float, end_value: float, transition_steps: float, steps_per_update: int = 1,
+                            decay: bool = True) -> _lib.StxEpsilonSchedule:
+    """The device-evaluated epsilon schedule of stx_epsilon_greedy; decay=False is the constant schedule at end_value."""
+    return _lib.StxEpsilonSchedule(float(init_value), float(end_value), float(transition_steps), int(steps_per_update), int(bool(decay)), 0)
+
+
+def epsilon_greedy(q: torch.Tensor, sched: _lib.StxEpsilonSchedule, seed: int = 0, offset: int = 0, dev_counter: Optional[torch.Tensor] = None,
+                   count: Optional[torch.Tensor] = None, mode: bool = False, out: Optional[torch.Tensor] = None,
+                   epsilon_out: Optional[torch.Tensor] = None, update_no_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """distrax.EpsilonGreedy(q, epsilon).sample (mode=False) or .mode() on q (E, A) float32; epsilon from `sched` at the optimiser
+    count word `count` (int32, nullable: count 0).  Returns the int32 actions (E)."""
+    dev = _need_cuda(q, dev_counter, count, out, epsilon_out, update_no_out)
+    if q.dtype != torch.float32 or q.ndim != 2:
+        raise StxError("epsilon_greedy: q must be float32 (E, A)")
+    if count is not None and count.dtype != torch.int32:
+        raise StxError("epsilon_greedy: count must be an int32 device word")
+    E, A = q.shape
+    if out is None:
+        out = torch.empty(E, dtype=torch.int32, device=dev)
+    if out.dtype != torch.int32 or out.numel() != E:
+        raise StxError("epsilon_greedy: out must be int32 (E)")
+    for name, t, dt in (("epsilon_out", epsilon_out, torch.float32), ("update_no_out", update_no_out, torch.int32)):
+        if t is not None and (t.dtype != dt or t.numel() != E):
+            raise StxError(f"epsilon_greedy: {name} must be {dt} (E)")
+    _lib.check(_lib.load().stx_epsilon_greedy(_p(q), E, A, int(bool(mode)), int(seed) & (2**64 - 1), int(offset), _p(dev_counter), _p(count),
+                                              C.byref(sched), _p(out), _p(epsilon_out), _p(update_no_out), _stream()), "stx_epsilon_greedy")
+    return out
+
+
+def q_lambda(q_t: torch.Tensor, reward: torch.Tensor, done: torch.Tensor, truncated: torch.Tensor, gamma: float, q_lambda_: float,
+             out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Q(lambda) targets (T, E) of a time-major rollout: q_t (T, E, A) the successor rows' Q values, discount gamma (1 - (done | truncated))."""
+    dev = _need_cuda(q_t, reward, done, truncated, out)
+    T, E = reward.shape
+    if q_t.dtype != torch.float32 or q_t.ndim != 3 or tuple(q_t.shape[:2]) != (T, E) or reward.dtype != torch.float32:
+        raise StxError("q_lambda: q_t must be float32 (T, E, A) and reward float32 (T, E)")
+    done8 = done.view(torch.uint8) if done.dtype == torch.bool else done
+    trunc8 = truncated.view(torch.uint8) if truncated.dtype == torch.bool else truncated
+    if done8.dtype != torch.uint8 or trunc8.dtype != torch.uint8 or done8.shape != (T, E) or trunc8.shape != (T, E):
+        raise StxError("q_lambda: done / truncated must be bool or uint8 (T, E)")
+    if out is None:
+        out = torch.empty((T, E), dtype=torch.float32, device=dev)
+    _lib.check(_lib.load().stx_q_lambda_f32(_p(q_t), int(q_t.shape[2]), _p(reward), _p(done8), _p(trunc8), T, E, float(gamma), float(q_lambda_),
+                                            _p(out), _stream()), "stx_q_lambda_f32")
+    return out
+
+
+def lambda_returns(r_t: torch.Tensor, discount_t: torch.Tensor, v_t: torch.Tensor, lambda_) -> torch.Tensor:
+    """Time-major lambda returns (T, E) with float discounts; v_t (T, E) or (T, E, A) (then max over A: Q(lambda)); lambda_ a scalar or a
+    (T, E) tensor."""
+    dev = _need_cuda(r_t, discount_t, v_t)
+    T, E = r_t.shape
+    A = 1 if v_t.ndim == 2 else int(v_t.shape[2])
+    if tuple(v_t.shape[:2]) != (T, E) or discount_t.shape != (T, E) or any(x.dtype != torch.float32 for x in (r_t, discount_t, v_t)):
+        raise StxError("lambda_returns: r_t, discount_t float32 (T, E); v_t float32 (T, E) or (T, E, A)")
+    lam_t, lam = None, 0.0
+    if isinstance(lambda_, torch.Tensor) and lambda_.ndim > 0:
+        lam_t = lambda_.to(torch.float32).expand(T, E).contiguous()
+        _need_cuda(lam_t)
+    else:
+        lam = float(lambda_)
+    out = torch.empty((T, E), dtype=torch.float32, device=dev)
+    _lib.check(_lib.load().stx_lambda_returns_f32(_p(r_t), _p(discount_t), _p(v_t), A, _p(lam_t), lam, T, E, _p(out), _stream()),
+               "stx_lambda_returns_f32")
+    return out
+
+
+def q_loss_grads(q: torch.Tensor, idx: Optional[torch.Tensor], action: torch.Tensor, targets: torch.Tensor, huber_delta: float, d_q: torch.Tensor,
+                 metrics: torch.Tensor, weight: float = 1.0, row0: int = 0, scratch_key: str = "q_loss") -> None:
+    """_q_loss_fn (ff_pqn.py:139-162) on Q rows computed elsewhere: d mean(loss) / d q into d_q (mb, A), metrics[0] += weight * q_loss.
+    Row m pairs with batch row idx[m] (or row0 + m) of action / targets."""
+    dev = _need_cuda(q, idx, action, targets, d_q, metrics)
+    if q.dtype != torch.float32 or q.ndim != 2 or d_q.dtype != torch.float32 or d_q.shape != q.shape:
+        raise StxError("q_loss_grads: q and d_q must be float32 (mb, A)")
+    if action.dtype != torch.int32 or targets.dtype != torch.float32 or (idx is not None and idx.dtype != torch.int32):
+        raise StxError("q_loss_grads: action / idx int32, targets float32")
+    mb, A = q.shape
+    if idx is not None and idx.numel() != mb:
+        raise StxError("q_loss_grads: idx must hold one row index per q row")
+    lib = _lib.load()
+    scratch = _zeros_scratch((scratch_key,), lib.stx_ppo_head_scratch_bytes(mb), dev)
+    _lib.check(lib.stx_q_loss_grads(_p(q), _p(idx), int(row0), _p(action), _p(targets), mb, A, float(huber_delta), _p(d_q), _p(metrics),
+                                    float(weight), _p(scratch), _stream()), "stx_q_loss_grads")

@@ -1,8 +1,8 @@
-"""optax-shaped facade over the fused optimiser kernel (stx_clip_adam_step).
+"""optax-shaped facade over the fused optimiser kernels (stx_clip_adam_step, stx_clip_radam_step).
 
 `chain(clip_by_global_norm(m), adam(lr, eps=...))` mirrors the construction at
 stoix/systems/ppo/anakin/ff_ppo.py:456-463.  The returned object's `.update` is what the reference
-passes around as `update_fns`; the learner reads its hyper-parameters and runs BOTH optimisers
+passes around as `update_fns`; `chain(clip_by_global_norm(m), radam(lr))` (ff_pqn.py:263-267) runs the RAdam rule; the learner reads its hyper-parameters and runs BOTH optimisers
 (actor and critic) in a single fused launch over the flat arenas."""
 from __future__ import annotations
 
@@ -24,6 +24,11 @@ class _Adam:
     eps_root: float = 0.0
 
 
+@dataclass
+class _Radam(_Adam):
+    threshold: float = 5.0
+
+
 def clip_by_global_norm(max_norm: float) -> _Clip:
     return _Clip(float(max_norm))
 
@@ -32,6 +37,11 @@ def adam(learning_rate, b1: float = 0.9, b2: float = 0.999, eps: float = 1e-8, e
     if eps_root != 0.0:
         raise NotImplementedError("eps_root != 0 is not used by the reference PPO and is not built")
     return _Adam(learning_rate, b1, b2, eps, eps_root)
+
+
+def radam(learning_rate, b1: float = 0.9, b2: float = 0.999, eps: float = 1e-8, eps_root: float = 0.0, threshold: float = 5.0) -> _Radam:
+    """optax.radam (scale_by_radam without nesterov, then the learning rate), as ff_pqn.py:263-267 chains it after the clip."""
+    return _Radam(learning_rate, b1, b2, eps, eps_root, threshold)
 
 
 class OptState(NamedTuple):
@@ -53,6 +63,17 @@ class GradientTransformation:
 
     def __init__(self, clip: Optional[_Clip], adam_: _Adam):
         self.clip, self.adam = clip, adam_
+
+    @property
+    def rule(self) -> str:
+        """"radam" for an optax.radam stage, else "adam"."""
+        return "radam" if isinstance(self.adam, _Radam) else "adam"
+
+    def plan_kwargs(self) -> dict:
+        """The AdamPlan arguments of this stage's update rule."""
+        if self.rule == "radam":
+            return {"rule": "radam", "eps_root": self.adam.eps_root, "threshold": self.adam.threshold}
+        return {}
 
     @property
     def max_grad_norm(self) -> float:
@@ -94,7 +115,8 @@ class GradientTransformation:
         sched = self.schedule
         plan = ops.AdamPlan([(0, n, self.init_lr, self.max_grad_norm if self.clip is not None else 3.0e38)], g.device,
                             b1=self.adam.b1, b2=self.adam.b2, eps=self.adam.eps, decay=sched is not None,
-                            steps_per_update=getattr(sched, "steps_per_update", 1), num_updates=getattr(sched, "num_updates", 1))
+                            steps_per_update=getattr(sched, "steps_per_update", 1), num_updates=getattr(sched, "num_updates", 1),
+                            **self.plan_kwargs())
         plan.counts[0:1].copy_(state.count.reshape(-1)[:1])
         plan.counts[1:2].copy_(state.sched_count.reshape(-1)[:1])
         ops.clip_adam_step(plan, p, gg, mu, nu)
@@ -112,5 +134,5 @@ def chain(*parts) -> GradientTransformation:
     clip = next((p for p in parts if isinstance(p, _Clip)), None)
     adam_ = next((p for p in parts if isinstance(p, _Adam)), None)
     if adam_ is None:
-        raise ValueError("chain() needs an adam() stage")
+        raise ValueError("chain() needs an adam() or radam() stage")
     return GradientTransformation(clip, adam_)
