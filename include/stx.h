@@ -418,6 +418,29 @@ int stx_replay_sample(const StxReplay* rb, int64_t M, uint64_t seed, uint64_t of
                       float* xq_old, float* xq_new, float* xq_next, int64_t ld, float* reward, uint8_t* done, int32_t* idx_out,
                       void* stream);
 
+/* Discrete transition ring buffer -- the item buffer of the DQN family (stoix/systems/q_learning/ff_dqn.py:339-347), whose
+ * Transition holds one integer action per row (ff_dqn.py:317-324).  Same semantics as StxReplay (same add order and overwrite,
+ * device write position / fill count, the Philox indices of stx_uniform_indices, idx_in overriding them); the two rings share
+ * their kernels as one template over the action type.
+ *   sample: writes obs (M, obs_dim), next_obs (M, obs_dim), action (M), reward (M), done (M) and idx_out (M, nullable).  obs and
+ *           next_obs may be the two halves of one (2M, obs_dim) block, so that one forward covers both (ff_mdqn's target net). */
+typedef struct StxReplayDiscrete {
+  float* obs;        /* [capacity][obs_dim] */
+  int32_t* action;   /* [capacity] */
+  float* reward;     /* [capacity] */
+  uint8_t* done;     /* [capacity]: timestep.last() (ff_dqn.py:121) */
+  float* next_obs;   /* [capacity][obs_dim] */
+  int64_t* state;    /* device int64[2] = {write position, number of valid items} */
+  int64_t capacity;
+  int32_t obs_dim;
+  int32_t reserved;
+} StxReplayDiscrete;
+int stx_replay_add_discrete(const StxReplayDiscrete* rb, const float* obs, const int32_t* action, const float* reward, const uint8_t* done,
+                            const float* next_obs, int64_t n, void* stream);
+int stx_replay_sample_discrete(const StxReplayDiscrete* rb, int64_t M, uint64_t seed, uint64_t offset, const uint64_t* dev_counter,
+                               const int32_t* idx_in, float* obs, float* next_obs, int32_t* action, float* reward, uint8_t* done,
+                               int32_t* idx_out, void* stream);
+
 /* ------------------------------------------------------------------ recurrent PPO building blocks (fp32) ------
  * stx_gru_sequence_forward / _backward: ScannedRNN(cell_type="gru") (stoix/networks/base.py:124-159; flax.linen.GRUCell) over a
  *   (T, E) sequence with episode resets, as RecurrentActor / RecurrentCritic run it (base.py:162-222) one step at a time in the
@@ -608,6 +631,35 @@ int stx_q_loss_grads(const float* q, const int32_t* idx, int64_t row0, const int
                      float huber_delta, float* d_q, float* metrics, float weight, void* scratch, void* stream);
 int stx_clip_radam_step(float* param_arena, const float* grad_arena, float* mu, float* nu, int32_t* counts, const StxAdamSeg* segs, int nseg,
                         const StxRadamHyper* hyper, void* params_bf16, float* gnorm_out, void* scratch, void* stream);
+
+/* ------------------------------------------------------------------ DQN family: one-step Q-learning losses (fp32) ----
+ * stx_q_td_loss_grads: the _q_loss_fn of ff_dqn.py:147-178 / ff_ddqn.py / ff_mdqn.py / ff_dqn_reg.py:147-182 under jax.grad, on
+ * Q rows computed elsewhere; one thread per row m of the sampled batch (rows contiguous, (M, A) each):
+ *   r = clip(reward, -max_abs_reward, max_abs_reward);  d = (1 - done) gamma, done = timestep.last() (truncation cuts too)
+ *   STX_Q_DQN, STX_Q_DQN_REG: target = r + d max_a q_t                           (utils/loss.py:106-124 q_learning)
+ *   STX_Q_DOUBLE:             target = r + d q_t[argmax q_aux], q_aux = q_t_selector, first maximal index as jnp.argmax
+ *                                                                                  (utils/loss.py:127-146 double_q_learning)
+ *   STX_Q_MUNCHAUSEN:         target = r + alpha clip(tau log_softmax(q_aux / tau)[a], clip_value_min, 0) + d tau logsumexp(q_t / tau),
+ *                             q_aux = q_tm1_target (the target net on obs), both in max-subtracted form (utils/loss.py:190-223)
+ *   td = target - q_tm1[a];  loss = rlax.l2_loss(td), or rlax.huber_loss(td, huber_delta) when huber_delta > 0 (the element of
+ *   stx_q_loss_grads); d_q = d mean(loss) / d q_tm1 in column a, 0 elsewhere.  STX_Q_DQN_REG adds regularizer_coeff mean(q_tm1[a])
+ *   (ff_dqn_reg.py:174-176) to the loss: + regularizer_coeff / M in column a, and the q_loss metric includes the term.
+ *   discount (nullable): per-row d given directly (the value faces of utils/loss.py take d_t); then done and gamma are unused.
+ *   metrics[0] += weight * mean(loss) (q_loss).  scratch: stx_ppo_head_scratch_bytes(M), zeroed once. */
+enum { STX_Q_DQN = 0, STX_Q_DOUBLE = 1, STX_Q_MUNCHAUSEN = 2, STX_Q_DQN_REG = 3 };
+typedef struct StxQTdHyper {
+  float gamma;
+  float max_abs_reward;
+  float huber_delta;
+  float entropy_temperature;     /* Munchausen tau */
+  float munchausen_coefficient;  /* Munchausen alpha */
+  float clip_value_min;
+  float regularizer_coeff;       /* DQN-Reg */
+  int32_t reserved;
+} StxQTdHyper;
+int stx_q_td_loss_grads(int rule, const float* q_tm1, const float* q_t, const float* q_aux, const int32_t* action, const float* reward,
+                        const uint8_t* done, const float* discount, int64_t M, int A, const StxQTdHyper* hyper, float* d_q, float* metrics,
+                        float weight, void* scratch, void* stream);
 
 /* Utility casts used by the bf16 path (obs / weight shadows). */
 int stx_cast_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream);

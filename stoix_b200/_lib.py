@@ -114,6 +114,33 @@ class StxReplay(C.Structure):
     ]
 
 
+class StxReplayDiscrete(C.Structure):
+    _fields_ = [
+        ("obs", C.c_void_p),
+        ("action", C.c_void_p),
+        ("reward", C.c_void_p),
+        ("done", C.c_void_p),
+        ("next_obs", C.c_void_p),
+        ("state", C.c_void_p),
+        ("capacity", C.c_int64),
+        ("obs_dim", C.c_int32),
+        ("reserved", C.c_int32),
+    ]
+
+
+class StxQTdHyper(C.Structure):
+    _fields_ = [
+        ("gamma", C.c_float),
+        ("max_abs_reward", C.c_float),
+        ("huber_delta", C.c_float),
+        ("entropy_temperature", C.c_float),
+        ("munchausen_coefficient", C.c_float),
+        ("clip_value_min", C.c_float),
+        ("regularizer_coeff", C.c_float),
+        ("reserved", C.c_int32),
+    ]
+
+
 class StxPpoBatch(C.Structure):
     _fields_ = [
         ("obs", C.c_void_p),
@@ -249,6 +276,9 @@ _SIGNATURES = {
     "stx_lambda_returns_f32": (C.c_int, [_P, _P, _P, C.c_int, _P, C.c_float, C.c_int, C.c_int, _P, _P]),
     "stx_q_loss_grads": (C.c_int, [_P, _P, C.c_int64, _P, _P, C.c_int64, C.c_int, C.c_float, _P, _P, C.c_float, _P, _P]),
     "stx_clip_radam_step": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.POINTER(StxRadamHyper), _P, _P, _P, _P]),
+    "stx_replay_add_discrete": (C.c_int, [C.POINTER(StxReplayDiscrete), _P, _P, _P, _P, _P, C.c_int64, _P]),
+    "stx_replay_sample_discrete": (C.c_int, [C.POINTER(StxReplayDiscrete), C.c_int64, C.c_uint64, C.c_uint64, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "stx_q_td_loss_grads": (C.c_int, [C.c_int, _P, _P, _P, _P, _P, _P, _P, C.c_int64, C.c_int, C.POINTER(StxQTdHyper), _P, _P, C.c_float, _P, _P]),
 }
 
 _lib = None

@@ -1,7 +1,8 @@
 // The PPO losses of the fp32 path: the minibatch entries (actor forward, actor loss, actor backward, then the critic half),
 // the loss heads on precomputed network outputs, the value-only and KL faces, and the tanh-Normal rollout faces.  The bf16
 // minibatch (stx_tc_ppo.cu) shares only the validation here.  Kernels: stx_ppo_loss.cuh; networks: stx_mlp.cu.  PQN's Q loss
-// (stx_q_loss_grads) lives here too: it reuses the rows and the metric reduction of these losses.
+// (stx_q_loss_grads) and the DQN family's one-step Q losses (stx_q_td_loss_grads) live here too: they reuse the rows and the metric
+// reduction of these losses.
 //
 // Reference: the _update_minibatch of stoix/systems/ppo/anakin/ff_ppo.py:184-247, ff_ppo_continuous.py:184-247,
 // ff_ppo_penalty.py:149-210, ff_ppo_penalty_continuous.py:149-210 and ff_dpo_continuous.py:148-170: each changes only the
@@ -187,13 +188,26 @@ int fp32_minibatch(const StxMlp* actor, const StxMlp* critic, const StxPpoBatch*
   return simt_net_backward(critic, x, D, idx, mb, workspace, grad_weight, grad_arena + coff, h->overwrite_grads, st);
 }
 
+// ---- rlax.l2_loss / rlax.huber_loss of a TD error and d loss / d td, the element of every Q loss here:
+//   l2:    loss = td^2 / 2,                                       g = td
+//   Huber: loss = q^2 / 2 + delta (|td| - q), q = min(|td|, delta),  g = clip(td, -delta, delta)   (delta > 0)
+// so d loss / d q[a] = -g.  At |td| = delta both Huber branches give the same value (delta^2 / 2) and the same derivative
+// (td = clip(td)), so the tie needs no rule.
+__device__ __forceinline__ void td_loss(float td, float delta, float& loss, float& g) {
+  if (delta > 0.f) {  // rlax.huber_loss
+    const float ax = fabsf(td), quad = fminf(ax, delta), lin = ax - quad;
+    loss = 0.5f * quad * quad + delta * lin;
+    g = fminf(fmaxf(td, -delta), delta);
+  } else {  // rlax.l2_loss
+    loss = 0.5f * td * td;
+    g = td;
+  }
+}
+
 // ---- PQN Q loss + its gradient with respect to the Q rows (one thread per minibatch row).
 //
-// Reference: _q_loss_fn of stoix/systems/q_learning/ff_pqn.py:139-162 under jax.grad, with rlax.l2_loss and rlax.huber_loss:
-//   td = target - q[a];  l2:    loss = td^2 / 2,                                 d loss / d q[a] = -td
-//                        Huber: loss = q^2 / 2 + delta (|td| - q), q = min(|td|, delta),  d loss / d q[a] = -clip(td, -delta, delta)
-// averaged over the minibatch (d q = that / mb; every other column 0).  At |td| = delta both Huber branches give the same value
-// (delta^2 / 2) and the same derivative (-td = -clip(td)), so the tie needs no rule.  Rows are read through the permutation and
+// Reference: _q_loss_fn of stoix/systems/q_learning/ff_pqn.py:139-162 under jax.grad: td = target - q[a], td_loss above,
+// averaged over the minibatch (d q = -g / mb in column a; every other column 0).  Rows are read through the permutation and
 // the metric is reduced with the PPO losses' LossRows / reduce_metrics (stx_ppo_loss.cuh).
 __global__ void __launch_bounds__(256) q_loss_kernel(LossRows r, const float* __restrict__ q, const int32_t* __restrict__ action,
                                                      const float* __restrict__ targets, int A, float delta, float* __restrict__ dq) {
@@ -205,16 +219,81 @@ __global__ void __launch_bounds__(256) q_loss_kernel(LossRows r, const float* __
     const int a = action[src];
     const float td = targets[src] - q[m * A + a];
     float loss, g;
-    if (delta > 0.f) {  // rlax.huber_loss
-      const float ax = fabsf(td), quad = fminf(ax, delta), lin = ax - quad;
-      loss = 0.5f * quad * quad + delta * lin;
-      g = fminf(fmaxf(td, -delta), delta);
-    } else {  // rlax.l2_loss
-      loss = 0.5f * td * td;
-      g = td;
-    }
+    td_loss(td, delta, loss, g);
     s_loss = (double)loss;
     for (int j = 0; j < A; ++j) dq[m * A + j] = j == a ? -g * inv_m : 0.f;
+  }
+  reduce_metrics<1>({s_loss}, {0}, r);
+}
+
+// ---- one-step Q-learning losses of the DQN family (one thread per sampled row); see stx_q_td_loss_grads in stx.h.
+// The bootstrap value of the row's successor, one struct per rule.  q_t / q_aux point at the row.
+struct MaxTarget {  // q_learning: max_a q_t
+  __device__ __forceinline__ static float next_value(const float* q_t, const float*, int A, const StxQTdHyper&) {
+    float v = q_t[0];
+    for (int j = 1; j < A; ++j) v = fmaxf(v, q_t[j]);
+    return v;
+  }
+  __device__ __forceinline__ static float bonus(const float*, int, int, const StxQTdHyper&) { return 0.f; }
+};
+struct DoubleTarget {  // double_q_learning: q_t_value[argmax q_t_selector], the first maximal index (jnp.argmax)
+  __device__ __forceinline__ static float next_value(const float* q_t, const float* sel, int A, const StxQTdHyper&) {
+    int best = 0;
+    float bv = sel[0];
+    for (int j = 1; j < A; ++j)
+      if (sel[j] > bv) bv = sel[j], best = j;
+    return q_t[best];
+  }
+  __device__ __forceinline__ static float bonus(const float*, int, int, const StxQTdHyper&) { return 0.f; }
+};
+struct MunchausenTarget {  // munchausen_q_learning: soft-Bellman value tau logsumexp(q_t / tau) and the clipped log-policy bonus
+  // tau logsumexp(q / tau) = max q + tau log sum exp((q - max q) / tau): with tau = 0.03 the exponents of the plain form run to
+  // the hundreds, here they are <= 0.
+  __device__ __forceinline__ static float max_and_log_sum(const float* q, int A, float tau, float& mx) {
+    mx = q[0];
+    for (int j = 1; j < A; ++j) mx = fmaxf(mx, q[j]);
+    float s = 0.f;
+    for (int j = 0; j < A; ++j) s += expf((q[j] - mx) / tau);
+    return logf(s);
+  }
+  __device__ __forceinline__ static float next_value(const float* q_t, const float*, int A, const StxQTdHyper& h) {
+    float mx;
+    const float ls = max_and_log_sum(q_t, A, h.entropy_temperature, mx);
+    return mx + h.entropy_temperature * ls;
+  }
+  // alpha clip(tau log_softmax(q_tm1_target / tau)[a], clip_value_min, 0), tau log_softmax(q / tau)[a] = (q[a] - max q) - tau log s
+  __device__ __forceinline__ static float bonus(const float* q_tgt, int a, int A, const StxQTdHyper& h) {
+    float mx;
+    const float ls = max_and_log_sum(q_tgt, A, h.entropy_temperature, mx);
+    const float m = (q_tgt[a] - mx) - h.entropy_temperature * ls;
+    return h.munchausen_coefficient * fminf(fmaxf(m, h.clip_value_min), 0.f);
+  }
+};
+
+template <class Rule, bool REG>
+__global__ void __launch_bounds__(256) q_td_loss_kernel(LossRows r, const float* __restrict__ q_tm1, const float* __restrict__ q_t,
+                                                        const float* __restrict__ q_aux, const int32_t* __restrict__ action,
+                                                        const float* __restrict__ reward, const uint8_t* __restrict__ done,
+                                                        const float* __restrict__ discount, int A, StxQTdHyper h, float* __restrict__ dq) {
+  const int64_t m = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  double s_loss = 0.0;
+  const float inv_m = 1.0f / (float)r.mb;
+  if (m < r.mb) {
+    const int a = action[m];
+    const float rt = fminf(fmaxf(reward[m], -h.max_abs_reward), h.max_abs_reward);          // jnp.clip(reward, -max, max)
+    const float dt = discount ? discount[m] : (1.f - (float)done[m]) * h.gamma;               // (1 - done) gamma
+    const float* aux = q_aux ? q_aux + m * A : nullptr;
+    const float target = (rt + Rule::bonus(aux, a, A, h)) + dt * Rule::next_value(q_t + m * A, aux, A, h);
+    const float qa = q_tm1[m * A + a];
+    float loss, g;
+    td_loss(target - qa, h.huber_delta, loss, g);
+    float da = -g * inv_m;
+    if (REG) {  // + regularizer_coeff mean(q_tm1[a]) (ff_dqn_reg.py:174-176)
+      loss += h.regularizer_coeff * qa;
+      da += h.regularizer_coeff * inv_m;
+    }
+    s_loss = (double)loss;
+    for (int j = 0; j < A; ++j) dq[m * A + j] = j == a ? da : 0.f;
   }
   reduce_metrics<1>({s_loss}, {0}, r);
 }
@@ -438,6 +517,32 @@ extern "C" int stx_q_loss_grads(const float* q, const int32_t* idx, int64_t row0
   STX_REQUIRE(mb > 0 && A > 0 && row0 >= 0, STX_E_SHAPE, "stx_q_loss_grads: mb=%lld A=%d row0=%lld", (long long)mb, A, (long long)row0);
   const LossRows r = scratch_rows(idx, row0, mb, metrics, weight, scratch);
   q_loss_kernel<<<(unsigned)((mb + 255) / 256), 256, 0, (cudaStream_t)stream>>>(r, q, action, targets, A, huber_delta, d_q);
+  STX_LAUNCH_OK();
+  return STX_OK;
+}
+
+extern "C" int stx_q_td_loss_grads(int rule, const float* q_tm1, const float* q_t, const float* q_aux, const int32_t* action, const float* reward,
+                                   const uint8_t* done, const float* discount, int64_t M, int A, const StxQTdHyper* hyper, float* d_q, float* metrics,
+                                   float weight, void* scratch, void* stream) {
+  const char* who = "stx_q_td_loss_grads";
+  STX_REQUIRE(q_tm1 && q_t && action && reward && (done || discount) && hyper && d_q && metrics && scratch, STX_E_ARG, "%s: null pointer", who);
+  STX_REQUIRE(M > 0 && A > 0, STX_E_SHAPE, "%s: M=%lld A=%d", who, (long long)M, A);
+  STX_REQUIRE(rule >= STX_Q_DQN && rule <= STX_Q_DQN_REG, STX_E_UNSUPPORTED, "%s: rule %d", who, rule);
+  STX_REQUIRE((rule != STX_Q_DOUBLE && rule != STX_Q_MUNCHAUSEN) || q_aux, STX_E_ARG, "%s: rule %d needs q_aux (%s)", who, rule,
+              rule == STX_Q_DOUBLE ? "q_t_selector" : "q_tm1_target");
+  STX_REQUIRE(rule != STX_Q_MUNCHAUSEN || hyper->entropy_temperature > 0.f, STX_E_ARG, "%s: entropy_temperature must be > 0", who);
+  const LossRows r = scratch_rows(nullptr, 0, M, metrics, weight, scratch);
+  const unsigned grid = (unsigned)((M + 255) / 256);
+  cudaStream_t st = (cudaStream_t)stream;
+  const StxQTdHyper h = *hyper;
+  switch (rule) {
+    case STX_Q_DQN: q_td_loss_kernel<MaxTarget, false><<<grid, 256, 0, st>>>(r, q_tm1, q_t, nullptr, action, reward, done, discount, A, h, d_q); break;
+    case STX_Q_DOUBLE: q_td_loss_kernel<DoubleTarget, false><<<grid, 256, 0, st>>>(r, q_tm1, q_t, q_aux, action, reward, done, discount, A, h, d_q); break;
+    case STX_Q_MUNCHAUSEN:
+      q_td_loss_kernel<MunchausenTarget, false><<<grid, 256, 0, st>>>(r, q_tm1, q_t, q_aux, action, reward, done, discount, A, h, d_q);
+      break;
+    default: q_td_loss_kernel<MaxTarget, true><<<grid, 256, 0, st>>>(r, q_tm1, q_t, nullptr, action, reward, done, discount, A, h, d_q); break;
+  }
   STX_LAUNCH_OK();
   return STX_OK;
 }

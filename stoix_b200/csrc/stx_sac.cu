@@ -152,16 +152,22 @@ __global__ void polyak_kernel(float* __restrict__ target, const float* __restric
 }
 
 // ---- replay buffer: uniform indices + row gather (flashbax item buffer sample: uniform with replacement over the filled part) ----
+// Sample index r of a call: word r & 3 of Philox (seed; r / 4, call, tag), scaled to floor(u * n), u in [0, 1).  Every sampler
+// (stx_uniform_indices and both rings) draws through this function, so they agree index for index.
+__device__ __forceinline__ int64_t uniform_index(int64_t r, uint64_t seed, uint64_t call, uint64_t n) {
+  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
+  const uint4 w = Philox::rand4(make_uint4((uint32_t)(r >> 2), (uint32_t)call, (uint32_t)(call >> 32), 0x52504c59u), key);
+  const uint32_t v[4] = {w.x, w.y, w.z, w.w};
+  return (int64_t)(((uint64_t)v[r & 3] * n) >> 32);
+}
+
 __global__ void uniform_index_kernel(int32_t* __restrict__ idx, int64_t M, uint64_t seed, uint64_t offset, const uint64_t* __restrict__ counter,
                                      const int64_t* __restrict__ range) {
   const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (i * 4 >= M) return;
   const uint64_t call = offset + (counter ? *counter : 0ull);
-  const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
-  const uint4 w = Philox::rand4(make_uint4((uint32_t)i, (uint32_t)call, (uint32_t)(call >> 32), 0x52504c59u), key);
-  const uint32_t v[4] = {w.x, w.y, w.z, w.w};
   const uint64_t n = (uint64_t)*range;
-  for (int k = 0; k < 4 && i * 4 + k < M; ++k) idx[i * 4 + k] = (int32_t)(((uint64_t)v[k] * n) >> 32);  // floor(u * n), u in [0, 1)
+  for (int k = 0; k < 4 && i * 4 + k < M; ++k) idx[i * 4 + k] = (int32_t)uniform_index(i * 4 + k, seed, call, n);
 }
 
 // dst[r, 0:C] (leading dim ld_dst) = src[idx[r], 0:C]; one warp per row, coalesced
@@ -177,15 +183,21 @@ __global__ void gather_bytes_kernel(const uint8_t* __restrict__ src, const int32
   if (r < M) dst[r] = src[idx[r]];
 }
 
-// ---- transition ring buffer (obs, action, reward, done, next_obs): the flashbax item buffer of ff_sac.py:449-456 with its
-// write position / fill count in DEVICE memory, so add + sample are stream-ordered and CUDA-graph replayable.  One warp per row.
-__global__ void replay_add_kernel(StxReplay rb, const float* __restrict__ obs, const float* __restrict__ action, const float* __restrict__ reward,
+// ---- transition ring buffers (obs, action, reward, done, next_obs): the flashbax item buffer of ff_sac.py:449-456 /
+// ff_dqn.py:339-347 with its write position / fill count in DEVICE memory, so add + sample are stream-ordered and CUDA-graph
+// replayable.  One template over the ring (StxReplay: float action rows of act_dim; StxReplayDiscrete: one int32 action per
+// row); one warp per row.
+__device__ __forceinline__ int action_cols(const StxReplay& rb) { return rb.act_dim; }
+__device__ __forceinline__ int action_cols(const StxReplayDiscrete&) { return 1; }
+
+template <class Ring, class Act>
+__global__ void replay_add_kernel(Ring rb, const float* __restrict__ obs, const Act* __restrict__ action, const float* __restrict__ reward,
                                   const uint8_t* __restrict__ done, const float* __restrict__ next_obs, int64_t n, int64_t skip) {
   const int64_t r = skip + blockIdx.x * (int64_t)(blockDim.x >> 5) + (threadIdx.x >> 5);
   if (r >= n) return;
   const int lane = threadIdx.x & 31;
   const int64_t slot = (rb.state[0] + r) % rb.capacity;
-  const int D = rb.obs_dim, A = rb.act_dim;
+  const int D = rb.obs_dim, A = action_cols(rb);
   for (int c = lane; c < D; c += 32) {
     rb.obs[slot * D + c] = obs[r * D + c];
     rb.next_obs[slot * D + c] = next_obs[r * D + c];
@@ -196,43 +208,76 @@ __global__ void replay_add_kernel(StxReplay rb, const float* __restrict__ obs, c
     rb.done[slot] = done[r];
   }
 }
-__global__ void replay_advance_kernel(StxReplay rb, int64_t n) {
+template <class Ring>
+__global__ void replay_advance_kernel(Ring rb, int64_t n) {
   rb.state[0] = (rb.state[0] + n) % rb.capacity;
   rb.state[1] = min(rb.state[1] + n, rb.capacity);
 }
-// Sample M items uniformly with replacement (same Philox words as uniform_index_kernel => same indices) and lay them out as the
-// three network inputs of one SAC epoch: xq_old = (obs | stored action), xq_new = (obs | .), xq_next = (next_obs | .); the
-// action columns of xq_new / xq_next are filled later by the policy-head sampler.
-__global__ void replay_sample_kernel(StxReplay rb, int64_t M, uint64_t seed, uint64_t offset, const uint64_t* __restrict__ counter,
-                                     const int32_t* __restrict__ idx_in, float* __restrict__ xq_old, float* __restrict__ xq_new,
-                                     float* __restrict__ xq_next, int64_t ld, float* __restrict__ reward, uint8_t* __restrict__ done,
+
+// Where a sampled row goes.  SAC: the three network inputs of one epoch, xq_old = (obs | stored action), xq_new = (obs | .),
+// xq_next = (next_obs | .); the action columns of xq_new / xq_next are filled later by the policy-head sampler.
+struct SacInputs {
+  float *xq_old, *xq_new, *xq_next;
+  int64_t ld;
+  __device__ __forceinline__ void row(const StxReplay& rb, int64_t j, int64_t r, int lane) const {
+    const int D = rb.obs_dim, A = rb.act_dim;
+    for (int c = lane; c < D; c += 32) {
+      const float o = rb.obs[j * D + c];
+      xq_old[r * ld + c] = o;
+      if (xq_new) xq_new[r * ld + c] = o;
+      if (xq_next) xq_next[r * ld + c] = rb.next_obs[j * D + c];
+    }
+    for (int c = lane; c < A; c += 32) xq_old[r * ld + D + c] = rb.action[j * A + c];
+  }
+};
+// DQN: the Transition fields as they are, obs / next_obs (M, obs_dim) and action (M).
+struct DiscreteBatch {
+  float *obs, *next_obs;
+  int32_t* action;
+  __device__ __forceinline__ void row(const StxReplayDiscrete& rb, int64_t j, int64_t r, int lane) const {
+    const int D = rb.obs_dim;
+    for (int c = lane; c < D; c += 32) {
+      obs[r * D + c] = rb.obs[j * D + c];
+      next_obs[r * D + c] = rb.next_obs[j * D + c];
+    }
+    if (lane == 0) action[r] = rb.action[j];
+  }
+};
+
+// Sample M items uniformly with replacement (the indices of uniform_index_kernel) or take idx_in.
+template <class Ring, class Out>
+__global__ void replay_sample_kernel(Ring rb, int64_t M, uint64_t seed, uint64_t offset, const uint64_t* __restrict__ counter,
+                                     const int32_t* __restrict__ idx_in, Out out, float* __restrict__ reward, uint8_t* __restrict__ done,
                                      int32_t* __restrict__ idx_out) {
   const int64_t r = blockIdx.x * (int64_t)(blockDim.x >> 5) + (threadIdx.x >> 5);
   if (r >= M) return;
   const int lane = threadIdx.x & 31;
-  int64_t j;
-  if (idx_in) {
-    j = idx_in[r];
-  } else {
-    const uint64_t call = offset + (counter ? *counter : 0ull);
-    const uint2 key = make_uint2((uint32_t)seed, (uint32_t)(seed >> 32));
-    const uint4 w = Philox::rand4(make_uint4((uint32_t)(r >> 2), (uint32_t)call, (uint32_t)(call >> 32), 0x52504c59u), key);
-    const uint32_t v[4] = {w.x, w.y, w.z, w.w};
-    j = (int64_t)(((uint64_t)v[r & 3] * (uint64_t)rb.state[1]) >> 32);
-  }
-  const int D = rb.obs_dim, A = rb.act_dim;
-  for (int c = lane; c < D; c += 32) {
-    const float o = rb.obs[j * D + c];
-    xq_old[r * ld + c] = o;
-    if (xq_new) xq_new[r * ld + c] = o;
-    if (xq_next) xq_next[r * ld + c] = rb.next_obs[j * D + c];
-  }
-  for (int c = lane; c < A; c += 32) xq_old[r * ld + D + c] = rb.action[j * A + c];
+  const int64_t j = idx_in ? (int64_t)idx_in[r] : uniform_index(r, seed, offset + (counter ? *counter : 0ull), (uint64_t)rb.state[1]);
+  out.row(rb, j, r, lane);
   if (lane == 0) {
     reward[r] = rb.reward[j];
     done[r] = rb.done[j];
     if (idx_out) idx_out[r] = (int32_t)j;
   }
+}
+
+template <class Ring, class Act>
+int replay_add(const Ring& rb, const float* obs, const Act* action, const float* reward, const uint8_t* done, const float* next_obs, int64_t n,
+               cudaStream_t st) {
+  const int64_t skip = n > rb.capacity ? n - rb.capacity : 0;   // more rows than slots: only the newest `capacity` survive
+  replay_add_kernel<Ring, Act><<<(unsigned)((n - skip + 7) / 8), 256, 0, st>>>(rb, obs, action, reward, done, next_obs, n, skip);
+  STX_LAUNCH_OK();
+  replay_advance_kernel<Ring><<<1, 1, 0, st>>>(rb, n);
+  STX_LAUNCH_OK();
+  return STX_OK;
+}
+
+template <class Ring, class Out>
+int replay_sample(const Ring& rb, int64_t M, uint64_t seed, uint64_t offset, const uint64_t* counter, const int32_t* idx_in, const Out& out,
+                  float* reward, uint8_t* done, int32_t* idx_out, cudaStream_t st) {
+  replay_sample_kernel<Ring, Out><<<(unsigned)((M + 7) / 8), 256, 0, st>>>(rb, M, seed, offset, counter, idx_in, out, reward, done, idx_out);
+  STX_LAUNCH_OK();
+  return STX_OK;
 }
 
 }  // namespace
@@ -247,22 +292,33 @@ static bool replay_ok(const StxReplay* rb) {
 extern "C" int stx_replay_add(const StxReplay* rb, const float* obs, const float* action, const float* reward, const uint8_t* done,
                               const float* next_obs, int64_t n, void* stream) {
   STX_REQUIRE(replay_ok(rb) && obs && action && reward && done && next_obs && n > 0, STX_E_ARG, "stx_replay_add: bad arguments");
-  const int64_t skip = n > rb->capacity ? n - rb->capacity : 0;   // more rows than slots: only the newest `capacity` survive
-  replay_add_kernel<<<(unsigned)((n - skip + 7) / 8), 256, 0, (cudaStream_t)stream>>>(*rb, obs, action, reward, done, next_obs, n, skip);
-  STX_LAUNCH_OK();
-  replay_advance_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(*rb, n);
-  STX_LAUNCH_OK();
-  return STX_OK;
+  return replay_add(*rb, obs, action, reward, done, next_obs, n, (cudaStream_t)stream);
 }
 
 extern "C" int stx_replay_sample(const StxReplay* rb, int64_t M, uint64_t seed, uint64_t offset, const uint64_t* dev_counter, const int32_t* idx_in,
                                  float* xq_old, float* xq_new, float* xq_next, int64_t ld, float* reward, uint8_t* done, int32_t* idx_out,
                                  void* stream) {
   STX_REQUIRE(replay_ok(rb) && xq_old && reward && done && M > 0 && ld >= rb->obs_dim + rb->act_dim, STX_E_ARG, "stx_replay_sample: bad arguments");
-  replay_sample_kernel<<<(unsigned)((M + 7) / 8), 256, 0, (cudaStream_t)stream>>>(*rb, M, seed, offset, dev_counter, idx_in, xq_old, xq_new, xq_next, ld,
-                                                                                  reward, done, idx_out);
-  STX_LAUNCH_OK();
-  return STX_OK;
+  return replay_sample(*rb, M, seed, offset, dev_counter, idx_in, SacInputs{xq_old, xq_new, xq_next, ld}, reward, done, idx_out,
+                       (cudaStream_t)stream);
+}
+
+static bool replay_ok(const StxReplayDiscrete* rb) {
+  return rb && rb->obs && rb->action && rb->reward && rb->done && rb->next_obs && rb->state && rb->capacity > 0 && rb->obs_dim > 0;
+}
+
+extern "C" int stx_replay_add_discrete(const StxReplayDiscrete* rb, const float* obs, const int32_t* action, const float* reward,
+                                       const uint8_t* done, const float* next_obs, int64_t n, void* stream) {
+  STX_REQUIRE(replay_ok(rb) && obs && action && reward && done && next_obs && n > 0, STX_E_ARG, "stx_replay_add_discrete: bad arguments");
+  return replay_add(*rb, obs, action, reward, done, next_obs, n, (cudaStream_t)stream);
+}
+
+extern "C" int stx_replay_sample_discrete(const StxReplayDiscrete* rb, int64_t M, uint64_t seed, uint64_t offset, const uint64_t* dev_counter,
+                                          const int32_t* idx_in, float* obs, float* next_obs, int32_t* action, float* reward, uint8_t* done,
+                                          int32_t* idx_out, void* stream) {
+  STX_REQUIRE(replay_ok(rb) && obs && next_obs && action && reward && done && M > 0, STX_E_ARG, "stx_replay_sample_discrete: bad arguments");
+  return replay_sample(*rb, M, seed, offset, dev_counter, idx_in, DiscreteBatch{obs, next_obs, action}, reward, done, idx_out,
+                       (cudaStream_t)stream);
 }
 
 extern "C" int stx_tanh_normal_sample(const float* head_out, int64_t M, int A, const float* eps_in, uint64_t seed, uint64_t offset,

@@ -1096,6 +1096,55 @@ def replay_sample(rb: ReplayRing, M: int, seed: int, xq_old: torch.Tensor, rewar
                                              _p(xq_new), _p(xq_next), int(ld), _p(reward), _p(done), _p(idx_out), _stream()), "stx_replay_sample")
 
 
+class DiscreteReplayRing:
+    """Device storage + StxReplayDiscrete descriptor of the DQN family's transition ring (one int32 action per row;
+    stx_replay_add_discrete / stx_replay_sample_discrete)."""
+
+    def __init__(self, capacity: int, obs_dim: int, device):
+        self.capacity, self.obs_dim = int(capacity), int(obs_dim)
+        z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=device)
+        self.obs, self.next_obs = z(self.capacity, self.obs_dim), z(self.capacity, self.obs_dim)
+        self.action, self.reward, self.done = z(self.capacity, dt=torch.int32), z(self.capacity), z(self.capacity, dt=torch.uint8)
+        self.state = z(2, dt=torch.int64)   # {write position, valid items}
+        self.c = _lib.StxReplayDiscrete(_p(self.obs), _p(self.action), _p(self.reward), _p(self.done), _p(self.next_obs), _p(self.state),
+                                        self.capacity, self.obs_dim, 0)
+
+
+def _u8(t: torch.Tensor) -> torch.Tensor:
+    return t.view(torch.uint8) if t.dtype == torch.bool else t
+
+
+def replay_add_discrete(rb: DiscreteReplayRing, obs, action, reward, done, next_obs) -> None:
+    """Append the rows of a (T, E, ...) / (n, ...) batch of transitions (contiguous; obs / next_obs / reward fp32, action int32,
+    done uint8 / bool) in time-major order."""
+    _need_cuda(obs, action, reward, done, next_obs)
+    n = int(reward.numel())
+    for t, cols, dt, name in ((obs, rb.obs_dim, torch.float32, "obs"), (next_obs, rb.obs_dim, torch.float32, "next_obs"),
+                              (reward, 1, torch.float32, "reward"), (action, 1, torch.int32, "action"), (_u8(done), 1, torch.uint8, "done")):
+        if t.dtype != dt or not t.is_contiguous() or t.numel() != n * cols:
+            raise StxError(f"replay_add_discrete: {name} must be contiguous {dt} with {n} x {cols} elements")
+    _lib.check(_lib.load().stx_replay_add_discrete(C.byref(rb.c), _p(obs), _p(action), _p(reward), _p(_u8(done)), _p(next_obs), n, _stream()),
+               "stx_replay_add_discrete")
+
+
+def replay_sample_discrete(rb: DiscreteReplayRing, M: int, seed: int, obs: torch.Tensor, next_obs: torch.Tensor, action: torch.Tensor,
+                           reward: torch.Tensor, done: torch.Tensor, offset: int = 0, dev_counter: Optional[torch.Tensor] = None,
+                           idx_in: Optional[torch.Tensor] = None, idx_out: Optional[torch.Tensor] = None) -> None:
+    """One launch: draw M indices (or take idx_in) and write obs, next_obs (M, obs_dim), action, reward, done (M)."""
+    _need_cuda(obs, next_obs, action, reward, done, dev_counter, idx_in, idx_out)
+    M = int(M)
+    for t, cols, dt, name in ((obs, rb.obs_dim, torch.float32, "obs"), (next_obs, rb.obs_dim, torch.float32, "next_obs"),
+                              (reward, 1, torch.float32, "reward"), (action, 1, torch.int32, "action"), (_u8(done), 1, torch.uint8, "done")):
+        if t.dtype != dt or not t.is_contiguous() or t.numel() != M * cols:
+            raise StxError(f"replay_sample_discrete: {name} must be contiguous {dt} with {M} x {cols} elements")
+    for t, name in ((idx_in, "idx_in"), (idx_out, "idx_out")):
+        if t is not None and (t.dtype != torch.int32 or not t.is_contiguous() or t.numel() != M):
+            raise StxError(f"replay_sample_discrete: {name} must be contiguous int32 (M)")
+    _lib.check(_lib.load().stx_replay_sample_discrete(C.byref(rb.c), M, int(seed) & (2**64 - 1), int(offset), _p(dev_counter), _p(idx_in), _p(obs),
+                                                      _p(next_obs), _p(action), _p(reward), _p(_u8(done)), _p(idx_out), _stream()),
+               "stx_replay_sample_discrete")
+
+
 # ------------------------------------------------------------------------------------------------
 # recurrent PPO building blocks (stoix/networks/base.py:124-222, stoix/systems/ppo/anakin/rec_ppo.py)
 # ------------------------------------------------------------------------------------------------
@@ -1273,3 +1322,42 @@ def q_loss_grads(q: torch.Tensor, idx: Optional[torch.Tensor], action: torch.Ten
     scratch = _zeros_scratch((scratch_key,), lib.stx_ppo_head_scratch_bytes(mb), dev)
     _lib.check(lib.stx_q_loss_grads(_p(q), _p(idx), int(row0), _p(action), _p(targets), mb, A, float(huber_delta), _p(d_q), _p(metrics),
                                     float(weight), _p(scratch), _stream()), "stx_q_loss_grads")
+
+
+# ------------------------------------------------------------------------------------------------
+# DQN family: one-step Q-learning losses (stoix/utils/loss.py:106-146, 190-223; stoix/systems/q_learning/ff_dqn_reg.py:165-176)
+# ------------------------------------------------------------------------------------------------
+
+Q_RULES = {"q_learning": 0, "double_q_learning": 1, "munchausen_q_learning": 2, "q_learning_reg": 3}   # STX_Q_* of stx.h
+
+
+def q_td_hyper(gamma: float = 0.99, max_abs_reward: float = float("inf"), huber_delta: float = 0.0, entropy_temperature: float = 0.03,
+               munchausen_coefficient: float = 0.9, clip_value_min: float = -1e3, regularizer_coeff: float = 0.0) -> _lib.StxQTdHyper:
+    return _lib.StxQTdHyper(float(gamma), float(max_abs_reward), float(huber_delta), float(entropy_temperature), float(munchausen_coefficient),
+                            float(clip_value_min), float(regularizer_coeff), 0)
+
+
+def q_td_loss_grads(rule: str, q_tm1: torch.Tensor, q_t: torch.Tensor, action: torch.Tensor, reward: torch.Tensor, hyper: _lib.StxQTdHyper,
+                    d_q: torch.Tensor, metrics: torch.Tensor, done: Optional[torch.Tensor] = None, discount: Optional[torch.Tensor] = None,
+                    q_aux: Optional[torch.Tensor] = None, weight: float = 1.0, scratch_key: str = "q_td_loss") -> None:
+    """The loss of `rule` (a key of Q_RULES) on Q rows computed elsewhere, all (M, A) contiguous fp32: d mean(loss) / d q_tm1 into d_q,
+    metrics[0] += weight * loss.  q_aux: the DDQN selector Q(online, next_obs) / the MDQN Q(target, obs).  The discount is
+    (1 - done) gamma from `done` (uint8 / bool), or `discount` (M) fp32 given directly."""
+    dev = _need_cuda(q_tm1, q_t, q_aux, action, reward, done, discount, d_q, metrics)
+    if rule not in Q_RULES:
+        raise StxError(f"q_td_loss_grads: rule {rule!r} is not one of {sorted(Q_RULES)}")
+    if q_tm1.dtype != torch.float32 or q_tm1.ndim != 2 or not q_tm1.is_contiguous():
+        raise StxError("q_td_loss_grads: q_tm1 must be contiguous float32 (M, A)")
+    M, A = q_tm1.shape
+    for t, name in ((q_t, "q_t"), (q_aux, "q_aux"), (d_q, "d_q")):
+        if t is not None and (t.dtype != torch.float32 or tuple(t.shape) != (M, A) or not t.is_contiguous()):
+            raise StxError(f"q_td_loss_grads: {name} must be contiguous float32 ({M}, {A})")
+    for t, dt, name in ((action, torch.int32, "action"), (reward, torch.float32, "reward"), (discount, torch.float32, "discount"),
+                        (None if done is None else _u8(done), torch.uint8, "done")):
+        if t is not None and (t.dtype != dt or t.numel() != M or not t.is_contiguous()):
+            raise StxError(f"q_td_loss_grads: {name} must be contiguous {dt} (M)")
+    lib = _lib.load()
+    scratch = _zeros_scratch((scratch_key,), lib.stx_ppo_head_scratch_bytes(M), dev)
+    _lib.check(lib.stx_q_td_loss_grads(Q_RULES[rule], _p(q_tm1), _p(q_t), _p(q_aux), _p(action), _p(reward), _p(None if done is None else _u8(done)),
+                                       _p(discount), M, A, C.byref(hyper), _p(d_q), _p(metrics), float(weight), _p(scratch), _stream()),
+               "stx_q_td_loss_grads")
