@@ -12,6 +12,7 @@ from typing import List, Optional, Tuple
 
 from stoix_b200.config import DictConfig
 from stoix_b200.envs.base import Environment
+from stoix_b200.systems import anakin
 from stoix_b200.systems.ppo.anakin import ff_ppo as _ppo
 from stoix_b200.systems.ppo.anakin import ff_ppo_continuous as _cont
 
@@ -26,13 +27,13 @@ def learner_setup(env: Environment, keys: Tuple[int, int, int], config: DictConf
 
 def run_experiment(_config: DictConfig) -> float:
     """Runs experiment (ff_dpo_continuous.py:436-583)."""
-    return _ppo.run_with(_config, learner_setup)
+    return anakin.run_experiment(_config, learner_setup, net_keys=2)
 
 
 def hydra_entry_point(cfg: Optional[DictConfig] = None, overrides: Optional[List[str]] = None) -> float:
     """Experiment entry point with config default_ff_dpo_continuous:
     `python -m stoix_b200.systems.ppo.anakin.ff_dpo_continuous arch.total_num_envs=1024 ...`"""
-    return _ppo.entry_with(cfg, overrides, "default_ff_dpo_continuous", run_experiment)
+    return anakin.entry_point(cfg, overrides, "default_ff_dpo_continuous", run_experiment, "PPO")
 
 
 if __name__ == "__main__":

@@ -24,11 +24,7 @@ position lives in device memory so replays draw fresh numbers.
 """
 from __future__ import annotations
 
-import copy
-import gc
 import os
-import sys
-import time
 from typing import Any, Callable, Dict, List, Optional, Tuple
 
 import torch
@@ -46,16 +42,13 @@ from stoix_b200.base_types import (
     LearnerFn,
     OnPolicyLearnerState,
 )
-from stoix_b200.config import DictConfig, compose, instantiate, to_container
-from stoix_b200.envs.base import Environment, StepOut, TimeStep
+from stoix_b200.config import DictConfig, instantiate, to_container
+from stoix_b200.envs.base import Environment, StepOut
 from stoix_b200.networks.base import FeedForwardActor as Actor
 from stoix_b200.networks.base import FeedForwardCritic as Critic
-from stoix_b200.networks.base import build_param_tree
 from stoix_b200.networks.heads import NormalAffineTanhDistributionHead
+from stoix_b200.systems import anakin
 from stoix_b200.systems.ppo.ppo_types import PPOTransition
-from stoix_b200.utils import make_env as environments
-from stoix_b200.utils.logger import LogEvent, StoixLogger
-from stoix_b200.utils.total_timestep_checker import check_total_timesteps
 from stoix_b200.utils.training import make_learning_rate
 
 _METRIC_NAMES = ("actor_loss", "entropy", "value_loss", "advantages", "pred_value", "target_value")
@@ -68,12 +61,6 @@ _VARIANT_METRICS = {
     "kl_penalty": (("actor_loss", 0), ("entropy", 1), ("kl_divergence", ops.METRIC_SLOT_KL), ("value_loss", 2)),
     "dpo": (("actor_loss", 0), ("entropy", 1), ("value_loss", 2)),
 }
-
-
-def _world() -> Tuple[int, int]:
-    if dist.is_available() and dist.is_initialized():
-        return dist.get_rank(), dist.get_world_size()
-    return 0, 1
 
 
 class _Shard:
@@ -141,19 +128,10 @@ def get_learner_fn(
     ff_ppo_penalty_continuous) or "dpo" (ff_dpo_continuous, tanh-Normal actor only).
     """
     actor_apply_fn, critic_apply_fn = apply_fns
-    # The arithmetic of apply / update runs inside the fused kernels; what the learner needs from the four callables is the
-    # description they are bound to (layer sizes, optimiser hyper-parameters).  Anything else cannot be honoured silently.
-    def _owner(fn, kind, what):
-        obj = getattr(fn, "__self__", None)
-        if not isinstance(obj, kind):
-            raise TypeError(f"get_learner_fn: {what} must be the bound `{'apply' if kind is not optax.GradientTransformation else 'update'}` of a "
-                            f"stoix_b200 {kind.__name__} (got {fn!r}); arbitrary callables cannot be lowered onto the CUDA kernels")
-        return obj
-
-    actor_net, critic_net = _owner(actor_apply_fn, Actor, "apply_fns[0]"), _owner(critic_apply_fn, Critic, "apply_fns[1]")
-    actor_opt = _owner(update_fns[0], optax.GradientTransformation, "update_fns[0]")
-    critic_opt = _owner(update_fns[1], optax.GradientTransformation, "update_fns[1]")
-    rank, world = _world()
+    actor_net, critic_net = anakin.owner(actor_apply_fn, Actor, "apply_fns[0]"), anakin.owner(critic_apply_fn, Critic, "apply_fns[1]")
+    actor_opt = anakin.owner(update_fns[0], optax.GradientTransformation, "update_fns[0]")
+    critic_opt = anakin.owner(update_fns[1], optax.GradientTransformation, "update_fns[1]")
+    rank, world = anakin.world()
 
     sysc, arch = config.system, config.arch
     T, E, U = int(sysc.rollout_length), int(arch.num_envs), int(arch.update_batch_size)
@@ -163,7 +141,6 @@ def get_learner_fn(
     mb = B // nmb
     precision = ops.STX_PREC_BF16 if str(arch.get("precision", "f32")) == "bf16" else ops.STX_PREC_F32
     use_graph = bool(arch.get("cuda_graph", True))
-    has_step_into = hasattr(env, "step_into")
     # The actor head decides the action buffer, the rollout sampler, the gradient entry and the entropy RNG; everything else
     # (GAE, shuffles, shards, all-reduce, observation normalisation, graph capture) is shared.
     tanh_head = actor_net.action_head if isinstance(actor_net.action_head, NormalAffineTanhDistributionHead) else None
@@ -248,21 +225,7 @@ def get_learner_fn(
                                    want_eps=False)
             ops.tanh_normal_log_prob(head, sh.action[t], lo, hi, ms, out=sh.log_prob[t])
         # STEP ENVIRONMENT (ff_ppo.py:104-116)
-        if has_step_into:
-            env.step_into(state.env_state[u], sh.action[t], sh.step_out(t), t)
-        else:
-            new_state, ts = env.step(state.env_state[u], sh.action[t])
-            state.env_state[u] = new_state
-            out = sh.step_out(t)
-            out.obs.copy_(ts.observation)
-            out.next_obs.copy_(ts.extras["next_obs"])
-            out.reward.copy_(ts.reward)
-            out.done.copy_(ts.discount == 0.0)                           # ff_ppo.py:107
-            out.truncated.copy_(ts.last() & (ts.discount != 0.0))        # ff_ppo.py:108
-            em = ts.extras["episode_metrics"]
-            out.episode_return.copy_(em["episode_return"])
-            out.episode_length.copy_(em["episode_length"])
-            out.is_terminal_step.copy_(em["is_terminal_step"])
+        anakin.step_env(env, state.env_state, u, sh.action[t], sh.step_out(t), t)
 
     def _rollout_phase(state: OnPolicyLearnerState) -> None:
         """STEP ENVIRONMENT FOR ROLLOUT LENGTH (ff_ppo.py:138-140) + the batched critic evaluations."""
@@ -474,26 +437,7 @@ def get_learner_fn(
         }
         train_out = torch.empty(n_upd, epochs, nmb, 8, device=dev)
         for k in range(n_upd):
-            if use_graph and b["eager_done"] and b["graph"] is None:
-                g = torch.cuda.CUDAGraph()
-                torch.cuda.synchronize()
-                # No cyclic GC while the stream is capturing: collecting an older learner (its CUDAGraph is destroyed
-                # in the collector) is "not permitted when stream is capturing" and would invalidate this capture.
-                gc.collect()
-                gc_was_enabled = gc.isenabled()
-                gc.disable()
-                try:
-                    with torch.cuda.graph(g):
-                        _update_step(learner_state)
-                finally:
-                    if gc_was_enabled:
-                        gc.enable()
-                b["graph"] = g
-            if b["graph"] is not None:
-                b["graph"].replay()
-            else:
-                _update_step(learner_state)  # first update runs eagerly (module loading, NCCL warm-up)
-                b["eager_done"] = True
+            anakin.update_once(b, use_graph, _update_step, learner_state)
             for u in range(U):
                 sh = b["shards"][u]
                 ep_out["episode_return"][k, u].copy_(sh.episode_return)
@@ -547,9 +491,8 @@ def build_learner(
     """The body of learner_setup shared by the PPO variants.  `action_head_kwargs(env, config)` reads the action space, records
     it in config.system and returns the action head's constructor arguments; `random_actions(config, E, gen, device)` draws the
     uniform actions of the observation-normalisation warm-up; `loss` is get_learner_fn's actor-loss variant."""
-    rank, world = _world()
+    rank, world = anakin.world()
     device = torch.device("cuda", torch.cuda.current_device())
-    n_devices = world
 
     head_kwargs = action_head_kwargs(env, config)
 
@@ -602,16 +545,9 @@ def build_learner(
     learn = get_learner_fn(env, apply_fns, update_fns, config, loss=loss)
 
     # Initialise environment states and timesteps across update-batch shards (ff_ppo.py:492-501).
-    U, E = int(config.arch.update_batch_size), int(config.arch.num_envs)
-    env_states: List[Any] = []
-    timesteps: List[TimeStep] = []
+    U = int(config.arch.update_batch_size)
     shard_keys = srandom.split(key, U + 1)
-    for u in range(U):
-        if hasattr(env, "seed"):
-            env.seed = (int(config.arch.seed) + 7919 * rank + 15485863 * u) & ((1 << 63) - 1)
-        st, ts = env.reset(srandom.split(shard_keys[u], E))
-        env_states.append(st)
-        timesteps.append(ts)
+    env_states, timesteps = anakin.reset_shards(env, shard_keys, config, rank)
 
     # Load model from checkpoint if specified (ff_ppo.py:504-512) -- params only, as in the reference.
     if config.logger.checkpointing.load_model:
@@ -623,9 +559,7 @@ def build_learner(
             ops.cast_bf16(arena, out=arena_bf16)
 
     # step keys: (sampling seed, shuffle seed) -- per-rank streams like the per-device keys at :515-518
-    step_key = srandom.split(shard_keys[U], 2 * n_devices)
-    rollout_seed = step_key[2 * rank] & ((1 << 62) - 1)
-    shuffle_seed = step_key[2 * rank + 1] & ((1 << 62) - 1)
+    rollout_seed, shuffle_seed = anakin.rank_seeds(shard_keys[U], 2, rank, world)
 
     init_learner_state = OnPolicyLearnerState(
         params=params, opt_states=opt_states, key=(rollout_seed, shuffle_seed), env_state=env_states, timestep=timesteps,
@@ -646,12 +580,13 @@ def _collect_obs_norm_rollouts(env: Environment, key: int, config: DictConfig, r
     system.obs_norm_warmup_steps steps (ff_ppo.py:375-421); not counted in the timestep budget.
     Returns (warmup_steps + 1, num_envs, *obs_shape) raw observations of this rank's env shard."""
     steps, E = int(config.system.obs_norm_warmup_steps), int(config.arch.num_envs)
-    if _world()[0] == 0:
+    rank = anakin.world()[0]
+    if rank == 0:
         print(f"Initializing observation normalization with {steps * int(config.arch.total_num_envs)} observations... "
               "Be aware, we do not count this in the timestep budget.")
     keys = srandom.split(key, E + 1)
     if hasattr(env, "seed"):
-        env.seed = (int(config.arch.seed) + 104729 * (_world()[0] + 1)) & ((1 << 63) - 1)
+        env.seed = (int(config.arch.seed) + 104729 * (rank + 1)) & ((1 << 63) - 1)
     env_state, ts = env.reset(keys[:E])
     dev = ts.observation.device
     gen = torch.Generator(device=dev)
@@ -664,130 +599,15 @@ def _collect_obs_norm_rollouts(env: Environment, key: int, config: DictConfig, r
     return torch.stack(obs, 0)
 
 
-def get_final_step_metrics(metrics: Dict[str, torch.Tensor]) -> Tuple[Dict[str, torch.Tensor], bool]:
-    """stoa.get_final_step_metrics as used at ff_ppo.py:624: keep entries of finished episodes."""
-    mask = metrics["is_terminal_step"]
-    has_final = bool(mask.any().item())
-    out = {k: (v[mask] if has_final else v.reshape(-1)[:0]) for k, v in metrics.items() if k != "is_terminal_step"}
-    return out, has_final
-
-
 def run_experiment(_config: DictConfig) -> float:
     """Runs experiment (ff_ppo.py:554-706)."""
-    return run_with(_config, learner_setup)
-
-
-def run_with(_config: DictConfig, setup: Callable) -> float:
-    """The body of run_experiment shared by the PPO variants; `setup` is the variant's learner_setup."""
-    from stoix_b200.evaluator import evaluator_setup, get_distribution_act_fn
-
-    config = copy.deepcopy(_config)
-    rank, world = _world()
-    n_devices = world
-    config.num_devices = n_devices
-    config.rank = rank
-    config = check_total_timesteps(config, quiet=rank != 0)
-    assert config.arch.num_updates >= config.arch.num_evaluation, \
-        "Number of updates per evaluation must be less than total number of updates."
-
-    env, eval_env = environments.make(config=config)
-
-    key, key_e, actor_net_key, critic_net_key = srandom.split(srandom.PRNGKey(config.arch.seed), num=4)
-    learn, actor_network, learner_state = setup(env, (key, actor_net_key, critic_net_key), config)
-
-    evaluator, absolute_metric_evaluator = evaluator_setup(
-        eval_env=eval_env, key_e=key_e, eval_act_fn=get_distribution_act_fn(config, actor_network.apply), config=config,
-    )
-
-    steps_per_rollout = (n_devices * config.arch.num_updates_per_eval * config.system.rollout_length
-                         * config.arch.update_batch_size * config.arch.num_envs)
-
-    logger = StoixLogger(config)
-    logger.log_config(to_container(config, resolve=True))
-    save_checkpoint = config.logger.checkpointing.save_model
-    if save_checkpoint:
-        from stoix_b200.utils.checkpointing import Checkpointer
-
-        checkpointer = Checkpointer(metadata=to_container(config), model_name=config.system.system_name,
-                                    **to_container(config.logger.checkpointing.save_args))
-
-    max_episode_return = -float("inf")
-    best_params = learner_state.params.actor_params.flat.clone()
-    evaluator_output = None
-    eval_step = 0
-    for eval_step in range(config.arch.num_evaluation):
-        start_time = time.time()
-        learner_output = learn(learner_state)
-        torch.cuda.synchronize()  # jax.block_until_ready (ff_ppo.py:619)
-        elapsed_time = time.time() - start_time
-        t = int(steps_per_rollout * (eval_step + 1))
-        episode_metrics, ep_completed = get_final_step_metrics(learner_output.episode_metrics)
-        episode_metrics["steps_per_second"] = torch.tensor(steps_per_rollout / elapsed_time)
-
-        logger.log({"timestep": t}, t, eval_step, LogEvent.MISC)
-        if ep_completed:
-            logger.log(episode_metrics, t, eval_step, LogEvent.ACT)
-        train_metrics = dict(learner_output.train_metrics)
-        opt_steps_per_eval = config.arch.num_updates_per_eval * (config.system.epochs * config.system.num_minibatches)
-        train_metrics["steps_per_second"] = torch.tensor(opt_steps_per_eval / elapsed_time)
-        logger.log(train_metrics, t, eval_step, LogEvent.TRAIN)
-
-        start_time = time.time()
-        trained_params = learner_output.learner_state.params.actor_params
-        evaluator_output = evaluator(trained_params, srandom.split(key_e, eval_step + 2)[-1],
-                                     running_statistics=getattr(learner_state, "running_statistics", None))
-        torch.cuda.synchronize()
-        elapsed_time = time.time() - start_time
-        episode_return = float(evaluator_output["episode_return"].mean().item())
-        steps_per_eval = int(evaluator_output["episode_length"].sum().item())
-        evaluator_output["steps_per_second"] = torch.tensor(steps_per_eval / max(elapsed_time, 1e-9))
-        logger.log(evaluator_output, t, eval_step, LogEvent.EVAL)
-
-        if save_checkpoint and rank == 0:
-            checkpointer.save(timestep=t, unreplicated_learner_state=learner_output.learner_state, episode_return=episode_return)
-
-        if config.arch.absolute_metric and max_episode_return <= episode_return:
-            best_params = trained_params.flat.clone()
-            max_episode_return = episode_return
-
-        learner_state = learner_output.learner_state
-
-    if config.arch.absolute_metric:
-        start_time = time.time()
-        t = int(steps_per_rollout * (eval_step + 1))
-        best_tree = build_param_tree(learner_state.params.actor_params.spec, best_params, "action_head")
-        if learner_state.params.actor_params.flat_bf16 is not None:
-            best_tree.flat_bf16 = ops.cast_bf16(best_params)
-        evaluator_output = absolute_metric_evaluator(best_tree, srandom.split(key_e, 1)[0],
-                                                     running_statistics=getattr(learner_state, "running_statistics", None))
-        torch.cuda.synchronize()
-        elapsed_time = time.time() - start_time
-        steps_per_eval = int(evaluator_output["episode_length"].sum().item())
-        evaluator_output["steps_per_second"] = torch.tensor(steps_per_eval / max(elapsed_time, 1e-9))
-        logger.log(evaluator_output, t, eval_step, LogEvent.ABSOLUTE)
-
-    logger.stop()
-    return float(evaluator_output[config.env.eval_metric].float().mean().item())
+    return anakin.run_experiment(_config, learner_setup, net_keys=2)
 
 
 def hydra_entry_point(cfg: Optional[DictConfig] = None, overrides: Optional[List[str]] = None) -> float:
     """Experiment entry point (ff_ppo.py:709-727).  Without hydra-core the composition happens here:
     `python -m stoix_b200.systems.ppo.anakin.ff_ppo env=synthetic/box arch.total_num_envs=4096 ...`"""
-    return entry_with(cfg, overrides, "default_ff_ppo", run_experiment)
-
-
-def entry_with(cfg: Optional[DictConfig], overrides: Optional[List[str]], config_name: str, run: Callable[[DictConfig], float]) -> float:
-    """The body of hydra_entry_point shared by the PPO variants."""
-    if cfg is None:
-        cfg = compose(config_name, overrides if overrides is not None else sys.argv[1:], config_dir="default/anakin")
-    if "RANK" in os.environ and not dist.is_initialized():
-        torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", 0)))
-        dist.init_process_group("nccl")
-    t0 = time.time()
-    eval_performance = run(cfg)
-    if _world()[0] == 0:
-        print(f"PPO experiment completed in {time.time() - t0:.2f} seconds.")
-    return eval_performance
+    return anakin.entry_point(cfg, overrides, "default_ff_ppo", run_experiment, "PPO")
 
 
 if __name__ == "__main__":

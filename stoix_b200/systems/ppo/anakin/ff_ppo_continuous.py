@@ -14,6 +14,7 @@ import torch
 
 from stoix_b200.config import DictConfig
 from stoix_b200.envs.base import Environment
+from stoix_b200.systems import anakin
 from stoix_b200.systems.ppo.anakin import ff_ppo as _ppo
 from stoix_b200.systems.ppo.anakin.ff_ppo import get_learner_fn  # noqa: F401  (the shared learner, ff_ppo_continuous.py:49-370)
 
@@ -40,13 +41,13 @@ def learner_setup(env: Environment, keys: Tuple[int, int, int], config: DictConf
 
 def run_experiment(_config: DictConfig) -> float:
     """Runs experiment (ff_ppo_continuous.py:548-700)."""
-    return _ppo.run_with(_config, learner_setup)
+    return anakin.run_experiment(_config, learner_setup, net_keys=2)
 
 
 def hydra_entry_point(cfg: Optional[DictConfig] = None, overrides: Optional[List[str]] = None) -> float:
     """Experiment entry point with config default_ff_ppo_continuous:
     `python -m stoix_b200.systems.ppo.anakin.ff_ppo_continuous arch.total_num_envs=1024 system.rollout_length=32 ...`"""
-    return _ppo.entry_with(cfg, overrides, "default_ff_ppo_continuous", run_experiment)
+    return anakin.entry_point(cfg, overrides, "default_ff_ppo_continuous", run_experiment, "PPO")
 
 
 if __name__ == "__main__":

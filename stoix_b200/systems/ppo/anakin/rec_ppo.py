@@ -18,11 +18,6 @@ discount_t = (1 - last_done_t) * gamma; minibatches are column subsets of the ba
 """
 from __future__ import annotations
 
-import copy
-import gc
-import os
-import sys
-import time
 from typing import Any, Callable, Dict, List, Optional, Tuple
 
 import torch
@@ -32,23 +27,15 @@ from stoix_b200 import ops
 from stoix_b200 import optim as optax
 from stoix_b200 import random as srandom
 from stoix_b200.base_types import ActorCriticOptStates, ActorCriticParams, AnakinExperimentOutput
-from stoix_b200.config import DictConfig, compose, instantiate, to_container
-from stoix_b200.envs.base import Environment, StepOut, TimeStep
+from stoix_b200.config import DictConfig, instantiate, to_container
+from stoix_b200.envs.base import Environment, StepOut
 from stoix_b200.networks.recurrent import RecLayout, RecurrentActor, RecurrentCritic, ScannedRNN
+from stoix_b200.systems import anakin
 from stoix_b200.systems.ppo.ppo_types import ActorCriticHiddenStates, RNNLearnerState, RNNPPOTransition
-from stoix_b200.utils import make_env as environments
-from stoix_b200.utils.logger import LogEvent, StoixLogger
-from stoix_b200.utils.total_timestep_checker import check_total_timesteps
 from stoix_b200.utils.training import make_learning_rate
 
 _METRIC_NAMES = ("actor_loss", "entropy", "value_loss", "advantages", "pred_value", "target_value")
 _pad8 = lambda n: (int(n) + 7) // 8 * 8
-
-
-def _world() -> Tuple[int, int]:
-    if dist.is_available() and dist.is_initialized():
-        return dist.get_rank(), dist.get_world_size()
-    return 0, 1
 
 
 class _Shard:
@@ -89,20 +76,12 @@ class _NetWs:
         self.out, self.d_out = z(M, out_dim), z(M, out_dim)
 
 
-def _owner(fn, kind, what):
-    obj = getattr(fn, "__self__", None)
-    if not isinstance(obj, kind):
-        raise TypeError(f"get_learner_fn: {what} must be a bound method of a stoix_b200 {kind.__name__} (got {fn!r}); arbitrary callables "
-                        "cannot be lowered onto the CUDA kernels")
-    return obj
-
-
 def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], update_fns: Tuple[Callable, Callable], config: DictConfig):
     """Get the learner function (rec_ppo.py:38-428)."""
     actor_apply_fn, critic_apply_fn = apply_fns
-    actor_net, critic_net = _owner(actor_apply_fn, RecurrentActor, "apply_fns[0]"), _owner(critic_apply_fn, RecurrentCritic, "apply_fns[1]")
-    actor_opt, critic_opt = (_owner(f, optax.GradientTransformation, f"update_fns[{i}]") for i, f in enumerate(update_fns))
-    rank, world = _world()
+    actor_net, critic_net = anakin.owner(actor_apply_fn, RecurrentActor, "apply_fns[0]"), anakin.owner(critic_apply_fn, RecurrentCritic, "apply_fns[1]")
+    actor_opt, critic_opt = (anakin.owner(f, optax.GradientTransformation, f"update_fns[{i}]") for i, f in enumerate(update_fns))
+    rank, world = anakin.world()
     sysc, arch = config.system, config.arch
     T, E, U = int(sysc.rollout_length), int(arch.num_envs), int(arch.update_batch_size)
     epochs, nmb = int(sysc.epochs), int(sysc.num_minibatches)
@@ -162,20 +141,10 @@ def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], updat
                 h_a, logits = _net_step(actor_net, a_tree, sh.h_a_cur, sh.obs[t], sh.reset[t])
                 ops.categorical(logits.contiguous(), None, state.key[0] + u, t, b["roll_ctr"], out=(sh.action[t], sh.log_prob[t]))
                 sh.h_actor[t].copy_(h_a), sh.h_a_cur.copy_(h_a)
-                if has_step_into:   # zero-copy: the env kernel writes the transition rows in place (device-resident step counter)
-                    env.step_into(state.env_state[u], sh.action[t],
-                                  StepOut(sh.obs[t + 1], sh.next_obs_scratch, sh.reward[t], sh.done[t + 1], sh.trunc[t + 1], sh.episode_return[t],
-                                          sh.episode_length[t], sh.is_terminal_step[t].view(torch.uint8)), t)
-                else:
-                    new_state, ts = env.step(state.env_state[u], sh.action[t])
-                    state.env_state[u] = new_state
-                    sh.obs[t + 1].copy_(ts.observation)
-                    sh.reward[t].copy_(ts.reward)
-                    sh.done[t + 1].copy_(ts.discount == 0.0)                              # :105
-                    sh.trunc[t + 1].copy_(ts.last() & (ts.discount != 0.0))               # :106
-                    em = ts.extras["episode_metrics"]
-                    sh.episode_return[t].copy_(em["episode_return"]), sh.episode_length[t].copy_(em["episode_length"])
-                    sh.is_terminal_step[t].copy_(em["is_terminal_step"])
+                # the env writes the transition rows in place; flags land in row t + 1, the ones BEFORE that step (:105-106)
+                anakin.step_env(env, state.env_state, u, sh.action[t],
+                                StepOut(sh.obs[t + 1], sh.next_obs_scratch, sh.reward[t], sh.done[t + 1], sh.trunc[t + 1], sh.episode_return[t],
+                                        sh.episode_length[t], sh.is_terminal_step[t].view(torch.uint8)), t)
                 main.wait_stream(side)             # next step (and the bootstrap value) read h_c_cur / obs written on both streams
             torch.bitwise_or(sh.done[T], sh.trunc[T], out=sh.reset[T])
             _, last_val = _net_step(critic_net, c_tree, sh.h_c_cur, sh.obs[T], sh.reset[T])
@@ -276,24 +245,7 @@ def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], updat
                   "is_terminal_step": torch.empty(n_upd, U, T, E, dtype=torch.bool, device=dev)}
         train_out = torch.empty(n_upd, epochs, nmb, 8, device=dev)
         for k in range(n_upd):
-            if use_graph and b["eager_done"] and b["graph"] is None:   # one CUDA graph per update step, as ff_ppo: ~10k launches replayed
-                g = torch.cuda.CUDAGraph()
-                torch.cuda.synchronize()
-                gc.collect()
-                gc_was_enabled = gc.isenabled()
-                gc.disable()
-                try:
-                    with torch.cuda.graph(g):
-                        _update_step(learner_state)
-                finally:
-                    if gc_was_enabled:
-                        gc.enable()
-                b["graph"] = g
-            if b["graph"] is not None:
-                b["graph"].replay()
-            else:
-                _update_step(learner_state)
-                b["eager_done"] = True
+            anakin.update_once(b, use_graph, _update_step, learner_state)   # one CUDA graph per update step: ~10k launches replayed
             for u in range(U):
                 sh = b["shards"][u]
                 ep_out["episode_return"][k, u].copy_(sh.episode_return), ep_out["episode_length"][k, u].copy_(sh.episode_length)
@@ -326,7 +278,7 @@ def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], updat
 
 def learner_setup(env: Environment, keys: Tuple[int, int, int], config: DictConfig):
     """Initialise learner_fn, networks, optimisers, environment and states (rec_ppo.py:431-590)."""
-    rank, world = _world()
+    rank, world = anakin.world()
     device = torch.device("cuda", torch.cuda.current_device())
     num_actions = int(env.action_space().num_values)
     config.system.action_dim = num_actions
@@ -374,21 +326,12 @@ def learner_setup(env: Environment, keys: Tuple[int, int, int], config: DictConf
 
         Checkpointer(model_name=config.system.system_name, **to_container(config.logger.checkpointing.load_args)).restore_params(arena)
 
-    env_states: List[Any] = []
-    timesteps: List[TimeStep] = []
     shard_keys = srandom.split(key, U + 1)
-    for u in range(U):
-        if hasattr(env, "seed"):
-            env.seed = (int(config.arch.seed) + 7919 * rank + 15485863 * u) & ((1 << 63) - 1)
-        st, ts = env.reset(srandom.split(shard_keys[u], E))
-        env_states.append(st)
-        timesteps.append(ts)
-    step_key = srandom.split(shard_keys[U], 2 * world)
-    m62 = (1 << 62) - 1
+    env_states, timesteps = anakin.reset_shards(env, shard_keys, config, rank)
     dones = [torch.zeros(E, dtype=torch.bool, device=device) for _ in range(U)]
     truncs = [torch.zeros(E, dtype=torch.bool, device=device) for _ in range(U)]
     hstates = [ActorCriticHiddenStates(init_policy_hstate.clone(), init_critic_hstate.clone()) for _ in range(U)]
-    init_learner_state = RNNLearnerState(params, ActorCriticOptStates(a_state, c_state), (step_key[2 * rank] & m62, step_key[2 * rank + 1] & m62),
+    init_learner_state = RNNLearnerState(params, ActorCriticOptStates(a_state, c_state), anakin.rank_seeds(shard_keys[U], 2, rank, world),
                                          env_states, timesteps, dones, truncs, hstates)
     return learn, actor_network, init_learner_state
 
@@ -421,81 +364,18 @@ def get_rnn_evaluator_fn(env: Environment, actor_network: RecurrentActor, config
     return evaluator
 
 
-def get_final_step_metrics(metrics: Dict[str, torch.Tensor]) -> Tuple[Dict[str, torch.Tensor], bool]:
-    mask = metrics["is_terminal_step"]
-    has_final = bool(mask.any().item())
-    return {k: (v[mask] if has_final else v.reshape(-1)[:0]) for k, v in metrics.items() if k != "is_terminal_step"}, has_final
-
-
 def run_experiment(_config: DictConfig) -> float:
-    """Runs experiment (rec_ppo.py:593-750)."""
-    config = copy.deepcopy(_config)
-    rank, world = _world()
-    config.num_devices, config.rank = world, rank
-    config = check_total_timesteps(config, quiet=rank != 0)
-    assert config.arch.num_updates >= config.arch.num_evaluation, "Number of updates per evaluation must be less than total number of updates."
-    env, eval_env = environments.make(config=config)
-    key, key_e, actor_net_key, critic_net_key = srandom.split(srandom.PRNGKey(config.arch.seed), num=4)
-    learn, actor_network, learner_state = learner_setup(env, (key, actor_net_key, critic_net_key), config)
-    evaluator = get_rnn_evaluator_fn(eval_env, actor_network, config)
-    absolute_metric_evaluator = get_rnn_evaluator_fn(eval_env, actor_network, config, 10)
-
-    steps_per_rollout = world * config.arch.num_updates_per_eval * config.system.rollout_length * config.arch.update_batch_size * config.arch.num_envs
-    logger = StoixLogger(config)
-    logger.log_config(to_container(config, resolve=True))
-    max_episode_return = -float("inf")
-    best_params = learner_state.params.actor_params.flat.clone()
-    evaluator_output, eval_step = None, 0
-    for eval_step in range(config.arch.num_evaluation):
-        start_time = time.time()
-        learner_output = learn(learner_state)
-        torch.cuda.synchronize()
-        elapsed_time = time.time() - start_time
-        t = int(steps_per_rollout * (eval_step + 1))
-        episode_metrics, ep_completed = get_final_step_metrics(learner_output.episode_metrics)
-        episode_metrics["steps_per_second"] = torch.tensor(steps_per_rollout / elapsed_time)
-        logger.log({"timestep": t}, t, eval_step, LogEvent.MISC)
-        if ep_completed:
-            logger.log(episode_metrics, t, eval_step, LogEvent.ACT)
-        train_metrics = dict(learner_output.train_metrics)
-        train_metrics["steps_per_second"] = torch.tensor(config.arch.num_updates_per_eval * config.system.epochs * config.system.num_minibatches / elapsed_time)
-        logger.log(train_metrics, t, eval_step, LogEvent.TRAIN)
-        start_time = time.time()
-        trained_params = learner_output.learner_state.params.actor_params
-        evaluator_output = evaluator(trained_params, srandom.split(key_e, eval_step + 2)[-1])
-        torch.cuda.synchronize()
-        elapsed_time = time.time() - start_time
-        episode_return = float(evaluator_output["episode_return"].mean().item())
-        evaluator_output["steps_per_second"] = torch.tensor(int(evaluator_output["episode_length"].sum().item()) / max(elapsed_time, 1e-9))
-        logger.log(evaluator_output, t, eval_step, LogEvent.EVAL)
-        if config.arch.absolute_metric and max_episode_return <= episode_return:
-            best_params = trained_params.flat.clone()
-            max_episode_return = episode_return
-        learner_state = learner_output.learner_state
-    if config.arch.absolute_metric:
-        t = int(steps_per_rollout * (eval_step + 1))
-        best_tree = actor_network.build_tree(learner_state.params.actor_params.layout, best_params)
-        start_time = time.time()
-        evaluator_output = absolute_metric_evaluator(best_tree, srandom.split(key_e, 1)[0])
-        torch.cuda.synchronize()
-        evaluator_output["steps_per_second"] = torch.tensor(int(evaluator_output["episode_length"].sum().item()) / max(time.time() - start_time, 1e-9))
-        logger.log(evaluator_output, t, eval_step, LogEvent.ABSOLUTE)
-    logger.stop()
-    return float(evaluator_output[config.env.eval_metric].float().mean().item())
+    """Runs experiment (rec_ppo.py:593-750), evaluating with the hidden state carried (get_rnn_evaluator_fn)."""
+    return anakin.run_experiment(
+        _config, learner_setup, net_keys=2,
+        make_evaluators=lambda eval_env, key_e, net, config: (get_rnn_evaluator_fn(eval_env, net, config),
+                                                              get_rnn_evaluator_fn(eval_env, net, config, 10)),
+        best_tree=lambda net, tree, flat: net.build_tree(tree.layout, flat))
 
 
 def hydra_entry_point(cfg: Optional[DictConfig] = None, overrides: Optional[List[str]] = None) -> float:
     """`python -m stoix_b200.systems.ppo.anakin.rec_ppo env=gymnax/cartpole arch.total_num_envs=256 ...`"""
-    if cfg is None:
-        cfg = compose("default_rec_ppo", overrides if overrides is not None else sys.argv[1:], config_dir="default/anakin")
-    if "RANK" in os.environ and not dist.is_initialized():
-        torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", 0)))
-        dist.init_process_group("nccl")
-    t0 = time.time()
-    eval_performance = run_experiment(cfg)
-    if _world()[0] == 0:
-        print(f"Recurrent PPO experiment completed in {time.time() - t0:.2f} seconds.")
-    return eval_performance
+    return anakin.entry_point(cfg, overrides, "default_rec_ppo", run_experiment, "Recurrent PPO")
 
 
 if __name__ == "__main__":

@@ -29,11 +29,7 @@ fp32 only: arch.precision=bf16 raises.
 """
 from __future__ import annotations
 
-import copy
-import gc
-import os
-import sys
-import time
+from functools import partial
 from typing import Any, Callable, Dict, List, NamedTuple, Optional, Sequence, Tuple
 
 import torch
@@ -43,27 +39,19 @@ from stoix_b200 import ops
 from stoix_b200 import optim as optax
 from stoix_b200 import random as srandom
 from stoix_b200.base_types import AnakinExperimentOutput
-from stoix_b200.config import DictConfig, compose, instantiate, to_container
+from stoix_b200.config import DictConfig, instantiate, to_container
 from stoix_b200.envs.base import Environment, StepOut, TimeStep
 from stoix_b200.networks.base import FeedForwardActor as Actor
 from stoix_b200.networks.base import build_param_tree
 from stoix_b200.networks.heads import DiscreteQNetworkHead
+from stoix_b200.systems import anakin
 from stoix_b200.systems.q_learning.dqn_types import Transition
 from stoix_b200.systems.sac.sac_types import OffPolicyLearnerState, OnlineAndTarget
-from stoix_b200.utils import make_env as environments
-from stoix_b200.utils.logger import LogEvent, StoixLogger
 from stoix_b200.utils.replay import DiscreteTransitionBuffer
-from stoix_b200.utils.total_timestep_checker import check_total_timesteps
 from stoix_b200.utils.training import make_learning_rate
 
 LOSSES = tuple(ops.Q_RULES)
 _NAMES = {"q_learning": "DQN", "double_q_learning": "DDQN", "munchausen_q_learning": "MDQN", "q_learning_reg": "DQN-Reg"}
-
-
-def _world() -> Tuple[int, int]:
-    if dist.is_available() and dist.is_initialized():
-        return dist.get_rank(), dist.get_world_size()
-    return 0, 1
 
 
 def _refuse_unsupported(config: DictConfig) -> None:
@@ -167,14 +155,6 @@ def batch_grads(loss: str, spec: ops.MlpSpec, online: torch.Tensor, target: torc
         ops.mlp_backward(spec, online, obs, dq, work.ws, net_grad=grads, grad_weight=1.0 / U, overwrite=(u == 0))
 
 
-def _owner(fn, kind, what):
-    obj = getattr(fn, "__self__", None)
-    if not isinstance(obj, kind):
-        raise TypeError(f"{what} must be a bound method of a stoix_b200 {kind.__name__} (got {fn!r}); arbitrary callables cannot be "
-                        "lowered onto the CUDA kernels")
-    return obj
-
-
 def get_warmup_fn(env: Environment, q_params: OnlineAndTarget, q_apply_fn: Callable, buffer_add_fn: Callable, config: DictConfig) -> Callable:
     """ff_dqn.py:37-89: `warmup_steps` environment steps with the initial online parameters and the training epsilon, added to
     the buffer (one shard per call)."""
@@ -201,15 +181,15 @@ def get_learner_fn(env: Environment, q_apply_fn: Callable, q_update_fn: Callable
     """ff_dqn.py:92-258.  q_apply_fn: the bound `apply` of the Q network (a FeedForwardActor with a DiscreteQNetworkHead); q_update_fn:
     the bound `update` of chain(clip_by_global_norm, adam); buffer_fns = (DiscreteTransitionBuffer.add, .sample_into) unbound, applied
     to learner_state.buffer_state[u]; loss: one of LOSSES."""
-    q_net = _owner(q_apply_fn, Actor, "q_apply_fn")
+    q_net = anakin.owner(q_apply_fn, Actor, "q_apply_fn")
     if not isinstance(q_net.action_head, DiscreteQNetworkHead):
         raise TypeError("get_learner_fn: q_apply_fn must be the bound `apply` of a FeedForwardActor with a DiscreteQNetworkHead")
-    opt = _owner(q_update_fn, optax.GradientTransformation, "q_update_fn")
+    opt = anakin.owner(q_update_fn, optax.GradientTransformation, "q_update_fn")
     if loss not in LOSSES:
         raise ValueError(f"get_learner_fn: loss {loss!r} is not one of {LOSSES}")
     _refuse_unsupported(config)
     buffer_add_fn, buffer_sample_fn = buffer_fns
-    rank, world = _world()
+    rank, world = anakin.world()
     sysc, arch = config.system, config.arch
     T, E, U = int(sysc.rollout_length), int(arch.num_envs), int(arch.update_batch_size)
     epochs, M = int(sysc.epochs), int(sysc.batch_size)
@@ -217,7 +197,6 @@ def get_learner_fn(env: Environment, q_apply_fn: Callable, q_update_fn: Callable
     hyper = loss_hyper(loss, config)
     sched = ops.epsilon_schedule_struct(float(sysc.training_epsilon), float(sysc.training_epsilon), 0.0, 1, decay=False)
     use_graph = bool(arch.get("cuda_graph", True))
-    has_step_into = hasattr(env, "step_into")
     built: Dict[str, Any] = {}
 
     def _build(state: OffPolicyLearnerState) -> None:
@@ -246,21 +225,7 @@ def get_learner_fn(env: Environment, q_apply_fn: Callable, q_update_fn: Callable
             for t in range(T):
                 ops.mlp_forward(b["spec"], online, ro.obs[t], out=ro.q[t], ws_key="dqn_rollout")
                 ops.epsilon_greedy(ro.q[t], sched, seed=state.key[0] + u, offset=t, dev_counter=b["roll_ctr"], out=ro.action[t])
-                if has_step_into:
-                    env.step_into(state.env_state[u], ro.action[t], ro.step_out(t), t)
-                else:
-                    new_state, ts = env.step(state.env_state[u], ro.action[t])
-                    state.env_state[u] = new_state
-                    out = ro.step_out(t)
-                    out.obs.copy_(ts.observation)
-                    out.next_obs.copy_(ts.extras["next_obs"])
-                    out.reward.copy_(ts.reward)
-                    out.done.copy_(ts.discount == 0.0)
-                    out.truncated.copy_(ts.last() & (ts.discount != 0.0))
-                    em = ts.extras["episode_metrics"]
-                    out.episode_return.copy_(em["episode_return"])
-                    out.episode_length.copy_(em["episode_length"])
-                    out.is_terminal_step.copy_(em["is_terminal_step"])
+                anakin.step_env(env, state.env_state, u, ro.action[t], ro.step_out(t), t)
             torch.bitwise_or(ro.terminated, ro.truncated, out=ro.done)
             buffer_add_fn(state.buffer_state[u], ro.transition())
 
@@ -311,29 +276,7 @@ def get_learner_fn(env: Environment, q_apply_fn: Callable, q_update_fn: Callable
                   "is_terminal_step": torch.empty(n_upd, U, T, E, dtype=torch.bool, device=dev)}
         train_out = torch.empty(n_upd, epochs, device=dev)
         for k in range(n_upd):
-            if use_graph and b["eager_done"] and b["graph"] is None:
-                g = torch.cuda.CUDAGraph()
-                torch.cuda.synchronize()
-                gc.collect()   # no cyclic GC (which may destroy an older CUDAGraph) while the stream is capturing
-                gc_was_enabled = gc.isenabled()
-                gc.disable()
-                added = [buf.added for buf in learner_state.buffer_state]   # capturing launches nothing: keep the host mirrors
-                try:
-                    with torch.cuda.graph(g):
-                        _update_step(learner_state)
-                finally:
-                    if gc_was_enabled:
-                        gc.enable()
-                for buf, n in zip(learner_state.buffer_state, added):
-                    buf.added = n
-                b["graph"] = g
-            if b["graph"] is not None:
-                b["graph"].replay()
-                for buf in learner_state.buffer_state:
-                    buf.added += T * E   # host mirror of the item count under replay
-            else:
-                _update_step(learner_state)   # the first update runs eagerly (module loading, NCCL warm-up)
-                b["eager_done"] = True
+            anakin.update_once(b, use_graph, _update_step, learner_state, learner_state.buffer_state, T * E)
             for u in range(U):
                 ro = b["rollouts"][u]
                 ep_out["episode_return"][k, u].copy_(ro.episode_return)
@@ -363,8 +306,7 @@ def learner_setup(env: Environment, keys: Tuple[int, int], config: DictConfig, l
     """Initialise learner_fn, network, optimiser, buffer, environment and states (ff_dqn.py:261-414).  Returns the EVAL network
     (epsilon = system.evaluation_epsilon) as the second element, which is what the reference hands to the evaluator."""
     _refuse_unsupported(config)
-    rank, world = _world()
-    n_devices = world
+    rank, n_devices = anakin.world()
     device = torch.device("cuda", torch.cuda.current_device())
     action_dim = int(env.action_space().num_values)
     config.system.action_dim = action_dim
@@ -401,7 +343,7 @@ def learner_setup(env: Environment, keys: Tuple[int, int], config: DictConfig, l
     params = OnlineAndTarget(online, target)
 
     # Replay buffer (:316-347): one ring per (device, update-batch shard)
-    U, E = int(config.arch.update_batch_size), int(config.arch.num_envs)
+    U = int(config.arch.update_batch_size)
     assert int(config.system.total_buffer_size) % n_devices == 0, "The total buffer size should be divisible by the number of devices!"
     assert int(config.system.total_batch_size) % n_devices == 0, "The total batch size should be divisible by the number of devices!"
     config.system.buffer_size = int(config.system.total_buffer_size) // (n_devices * U)
@@ -414,19 +356,10 @@ def learner_setup(env: Environment, keys: Tuple[int, int], config: DictConfig, l
     learn = get_learner_fn(env, q_network.apply, q_optim.update, buffer_fns, config, loss=loss)
     warmup = get_warmup_fn(env, params, q_network.apply, DiscreteTransitionBuffer.add, config)
 
-    env_states: List[Any] = []
-    timesteps: List[TimeStep] = []
-    for u in range(U):
-        if hasattr(env, "seed"):
-            env.seed = (int(config.arch.seed) + 7919 * rank + 15485863 * u) & ((1 << 63) - 1)
-        st, ts = env.reset(srandom.split(shard_keys[u], E))
-        env_states.append(st)
-        timesteps.append(ts)
+    env_states, timesteps = anakin.reset_shards(env, shard_keys, config, rank)
 
     # per-rank streams: rollout epsilon-greedy draws; warm-up draws on their own key (:383-409)
-    step_key = srandom.split(shard_keys[U + 1], 2 * n_devices)
-    m62 = (1 << 62) - 1
-    act_seed, warm_seed = step_key[2 * rank] & m62, step_key[2 * rank + 1] & m62
+    act_seed, warm_seed = anakin.rank_seeds(shard_keys[U + 1], 2, rank, n_devices)
     for u in range(U):
         env_states[u], timesteps[u], _, _ = warmup(env_states[u], timesteps[u], buffer_states[u], warm_seed + 0xA5A5 * u)
 
@@ -435,97 +368,20 @@ def learner_setup(env: Environment, keys: Tuple[int, int], config: DictConfig, l
     return learn, eval_q_network, init_learner_state
 
 
-class _QParams(NamedTuple):
-    actor_params: Any   # the Checkpointer stores the arenas of params.actor_params: the online network
-
-
-class _CheckpointView(NamedTuple):
-    params: _QParams
+def online_params(learner_state: OffPolicyLearnerState):
+    """The policy of the DQN family: the online network, which is evaluated, tracked and checkpointed."""
+    return learner_state.params.online
 
 
 def run_experiment(_config: DictConfig, loss: str = "q_learning") -> float:
     """Runs experiment (ff_dqn.py:417-556)."""
-    from stoix_b200.evaluator import evaluator_setup, get_distribution_act_fn
-    from stoix_b200.systems.sac.ff_sac import get_final_step_metrics
-
-    config = copy.deepcopy(_config)
-    rank, world = _world()
-    config.num_devices, config.rank = world, rank
-    config = check_total_timesteps(config, quiet=rank != 0)
-    assert config.arch.num_updates >= config.arch.num_evaluation, "Number of updates per evaluation must be less than total number of updates."
-    env, eval_env = environments.make(config=config)
-    key, key_e, q_net_key = srandom.split(srandom.PRNGKey(config.arch.seed), num=3)
-    learn, eval_q_network, learner_state = learner_setup(env, (key, q_net_key), config, loss=loss)
-    evaluator, absolute_metric_evaluator = evaluator_setup(eval_env=eval_env, key_e=key_e,
-                                                           eval_act_fn=get_distribution_act_fn(config, eval_q_network.apply), config=config)
-    steps_per_rollout = world * config.arch.num_updates_per_eval * config.system.rollout_length * config.arch.update_batch_size * config.arch.num_envs
-    logger = StoixLogger(config)
-    logger.log_config(to_container(config, resolve=True))
-    save_checkpoint = config.logger.checkpointing.save_model
-    if save_checkpoint:
-        from stoix_b200.utils.checkpointing import Checkpointer
-
-        checkpointer = Checkpointer(metadata=to_container(config), model_name=config.system.system_name,
-                                    **to_container(config.logger.checkpointing.save_args))
-    max_episode_return = -float("inf")
-    best_params = learner_state.params.online.flat.clone()
-    evaluator_output = None
-    eval_step = 0
-    for eval_step in range(config.arch.num_evaluation):
-        start_time = time.time()
-        learner_output = learn(learner_state)
-        torch.cuda.synchronize()
-        elapsed_time = time.time() - start_time
-        t = int(steps_per_rollout * (eval_step + 1))
-        episode_metrics, ep_completed = get_final_step_metrics(learner_output.episode_metrics)
-        episode_metrics["steps_per_second"] = torch.tensor(steps_per_rollout / elapsed_time)
-        logger.log({"timestep": t}, t, eval_step, LogEvent.MISC)
-        if ep_completed:
-            logger.log(episode_metrics, t, eval_step, LogEvent.ACT)
-        train_metrics = dict(learner_output.train_metrics)
-        opt_steps_per_eval = config.arch.num_updates_per_eval * config.system.epochs   # (:495)
-        train_metrics["steps_per_second"] = torch.tensor(opt_steps_per_eval / elapsed_time)
-        logger.log(train_metrics, t, eval_step, LogEvent.TRAIN)
-        start_time = time.time()
-        trained_params = learner_output.learner_state.params.online
-        evaluator_output = evaluator(trained_params, srandom.split(key_e, eval_step + 2)[-1])
-        torch.cuda.synchronize()
-        elapsed_time = time.time() - start_time
-        episode_return = float(evaluator_output["episode_return"].mean().item())
-        evaluator_output["steps_per_second"] = torch.tensor(int(evaluator_output["episode_length"].sum().item()) / max(elapsed_time, 1e-9))
-        logger.log(evaluator_output, t, eval_step, LogEvent.EVAL)
-        if save_checkpoint and rank == 0:
-            checkpointer.save(timestep=t, unreplicated_learner_state=_CheckpointView(_QParams(trained_params)), episode_return=episode_return)
-        if config.arch.absolute_metric and max_episode_return <= episode_return:
-            best_params = trained_params.flat.clone()
-            max_episode_return = episode_return
-        learner_state = learner_output.learner_state
-    if config.arch.absolute_metric:
-        start_time = time.time()
-        t = int(steps_per_rollout * (eval_step + 1))
-        best_tree = build_param_tree(learner_state.params.online.spec, best_params, "action_head")
-        evaluator_output = absolute_metric_evaluator(best_tree, srandom.split(key_e, 1)[0])
-        torch.cuda.synchronize()
-        elapsed_time = time.time() - start_time
-        evaluator_output["steps_per_second"] = torch.tensor(int(evaluator_output["episode_length"].sum().item()) / max(elapsed_time, 1e-9))
-        logger.log(evaluator_output, t, eval_step, LogEvent.ABSOLUTE)
-    logger.stop()
-    return float(evaluator_output[config.env.eval_metric].float().mean().item())
+    return anakin.run_experiment(_config, partial(learner_setup, loss=loss), net_keys=1, policy=online_params)
 
 
 def hydra_entry_point(cfg: Optional[DictConfig] = None, overrides: Optional[List[str]] = None, loss: str = "q_learning",
                       config_name: str = "default_ff_dqn") -> float:
     """Experiment entry point: `python -m stoix_b200.systems.q_learning.ff_dqn arch.total_num_envs=1024 ...`"""
-    if cfg is None:
-        cfg = compose(config_name, overrides if overrides is not None else sys.argv[1:], config_dir="default/anakin")
-    if "RANK" in os.environ and not dist.is_initialized():
-        torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", 0)))
-        dist.init_process_group("nccl")
-    t0 = time.time()
-    eval_performance = run_experiment(cfg, loss=loss)
-    if _world()[0] == 0:
-        print(f"{_NAMES[loss]} experiment completed in {time.time() - t0:.2f} seconds.")
-    return eval_performance
+    return anakin.entry_point(cfg, overrides, config_name, partial(run_experiment, loss=loss), _NAMES[loss])
 
 
 if __name__ == "__main__":

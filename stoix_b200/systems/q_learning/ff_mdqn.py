@@ -5,6 +5,7 @@ from __future__ import annotations
 from typing import List, Optional, Tuple
 
 from stoix_b200.config import DictConfig
+from stoix_b200.systems import anakin
 from stoix_b200.systems.q_learning import ff_dqn as _dqn
 from stoix_b200.systems.q_learning.ff_dqn import get_warmup_fn  # noqa: F401  (same warm-up as ff_dqn)
 
@@ -20,11 +21,11 @@ def learner_setup(env, keys: Tuple[int, int], config: DictConfig):
 
 
 def run_experiment(_config: DictConfig) -> float:
-    return _dqn.run_experiment(_config, loss=LOSS)
+    return anakin.run_experiment(_config, learner_setup, net_keys=1, policy=_dqn.online_params)
 
 
 def hydra_entry_point(cfg: Optional[DictConfig] = None, overrides: Optional[List[str]] = None) -> float:
-    return _dqn.hydra_entry_point(cfg, overrides, loss=LOSS, config_name="default_ff_mdqn")
+    return anakin.entry_point(cfg, overrides, "default_ff_mdqn", run_experiment, "MDQN")
 
 
 if __name__ == "__main__":

@@ -29,11 +29,7 @@ fp32 only: arch.precision=bf16 raises (the tensor-core kernels implement relu / 
 """
 from __future__ import annotations
 
-import copy
-import gc
-import sys
-import time
-from typing import Any, Callable, Dict, List, NamedTuple, Optional, Tuple
+from typing import Any, Callable, Dict, List, Optional, Tuple
 
 import torch
 import torch.distributed as dist
@@ -42,20 +38,12 @@ from stoix_b200 import ops
 from stoix_b200 import optim as optax
 from stoix_b200 import random as srandom
 from stoix_b200.base_types import AnakinExperimentOutput, LearnerFn, OnPolicyLearnerState
-from stoix_b200.config import DictConfig, compose, instantiate, to_container
-from stoix_b200.envs.base import Environment, StepOut, TimeStep
+from stoix_b200.config import DictConfig, instantiate, to_container
+from stoix_b200.envs.base import Environment, StepOut
 from stoix_b200.networks.base import FeedForwardActor as Actor
 from stoix_b200.networks.heads import DiscreteQNetworkHead
-from stoix_b200.utils import make_env as environments
-from stoix_b200.utils.logger import LogEvent, StoixLogger
-from stoix_b200.utils.total_timestep_checker import check_total_timesteps
+from stoix_b200.systems import anakin
 from stoix_b200.utils.training import make_learning_rate
-
-
-def _world() -> Tuple[int, int]:
-    if dist.is_available() and dist.is_initialized():
-        return dist.get_rank(), dist.get_world_size()
-    return 0, 1
 
 
 def _refuse_bf16(config: DictConfig) -> None:
@@ -113,16 +101,16 @@ def get_learner_fn(
     q_apply_fn: the bound `apply` of the Q network (a FeedForwardActor with a DiscreteQNetworkHead); q_update_fn: the bound `update`
     of chain(clip_by_global_norm, radam); epsilon_schedule: linear_schedule / constant_schedule of this module (their constants are
     evaluated on the device).  The arithmetic runs in the kernels; these carry the shapes and hyper-parameters."""
-    q_net = getattr(q_apply_fn, "__self__", None)
-    if not isinstance(q_net, Actor) or not isinstance(q_net.action_head, DiscreteQNetworkHead):
+    q_net = anakin.owner(q_apply_fn, Actor, "q_apply_fn")
+    if not isinstance(q_net.action_head, DiscreteQNetworkHead):
         raise TypeError("get_learner_fn: q_apply_fn must be the bound `apply` of a FeedForwardActor with a DiscreteQNetworkHead")
-    opt = getattr(q_update_fn, "__self__", None)
-    if not isinstance(opt, optax.GradientTransformation) or opt.rule != "radam":
+    opt = anakin.owner(q_update_fn, optax.GradientTransformation, "q_update_fn")
+    if opt.rule != "radam":
         raise TypeError("get_learner_fn: q_update_fn must be the bound `update` of chain(clip_by_global_norm(..), radam(..))")
     if not hasattr(epsilon_schedule, "device_schedule"):
         raise TypeError("get_learner_fn: epsilon_schedule must come from ff_pqn.linear_schedule / constant_schedule")
     _refuse_bf16(config)
-    rank, world = _world()
+    rank, world = anakin.world()
     sysc, arch = config.system, config.arch
     T, E, U = int(sysc.rollout_length), int(arch.num_envs), int(arch.update_batch_size)
     epochs, nmb = int(sysc.epochs), int(sysc.num_minibatches)
@@ -130,7 +118,6 @@ def get_learner_fn(
     assert B % nmb == 0, "rollout_length * num_envs must be divisible by num_minibatches"
     mb = B // nmb
     use_graph = bool(arch.get("cuda_graph", True))
-    has_step_into = hasattr(env, "step_into")
     gamma, q_lambda, delta = float(sysc.gamma), float(sysc.q_lambda), float(sysc.huber_loss_parameter)
     sched = epsilon_schedule.device_schedule(epochs * nmb)
     built: Dict[str, Any] = {}
@@ -167,21 +154,7 @@ def get_learner_fn(
                 ops.mlp_forward(b["spec"], tree.flat, sh.obs[t], out=sh.q[t], ws_key="pqn")
                 ops.epsilon_greedy(sh.q[t], sched, seed=state.key[0] + u, offset=t, dev_counter=b["roll_ctr"], count=count, out=sh.action[t],
                                    epsilon_out=sh.epsilon[t], update_no_out=sh.update_no[t])
-                if has_step_into:
-                    env.step_into(state.env_state[u], sh.action[t], sh.step_out(t), t)
-                else:
-                    new_state, ts = env.step(state.env_state[u], sh.action[t])
-                    state.env_state[u] = new_state
-                    out = sh.step_out(t)
-                    out.obs.copy_(ts.observation)
-                    out.next_obs.copy_(ts.extras["next_obs"])
-                    out.reward.copy_(ts.reward)
-                    out.done.copy_(ts.discount == 0.0)
-                    out.truncated.copy_(ts.last() & (ts.discount != 0.0))
-                    em = ts.extras["episode_metrics"]
-                    out.episode_return.copy_(em["episode_return"])
-                    out.episode_length.copy_(em["episode_length"])
-                    out.is_terminal_step.copy_(em["is_terminal_step"])
+                anakin.step_env(env, state.env_state, u, sh.action[t], sh.step_out(t), t)
             ops.mlp_forward(b["spec"], tree.flat, sh.obs[T], out=sh.q[T], ws_key="pqn")
 
     def _targets_phase(state: OnPolicyLearnerState) -> None:
@@ -263,24 +236,7 @@ def get_learner_fn(
         }
         train_out = torch.empty(n_upd, epochs, nmb, device=dev)
         for k in range(n_upd):
-            if use_graph and b["eager_done"] and b["graph"] is None:
-                g = torch.cuda.CUDAGraph()
-                torch.cuda.synchronize()
-                gc.collect()  # no cyclic GC while capturing (see ff_ppo)
-                gc_was_enabled = gc.isenabled()
-                gc.disable()
-                try:
-                    with torch.cuda.graph(g):
-                        _update_step(learner_state)
-                finally:
-                    if gc_was_enabled:
-                        gc.enable()
-                b["graph"] = g
-            if b["graph"] is not None:
-                b["graph"].replay()
-            else:
-                _update_step(learner_state)  # the first update runs eagerly (module loading, NCCL warm-up)
-                b["eager_done"] = True
+            anakin.update_once(b, use_graph, _update_step, learner_state)
             for u in range(U):
                 sh = b["shards"][u]
                 for name in ("episode_return", "episode_length", "is_terminal_step", "epsilon", "update_no"):
@@ -335,7 +291,7 @@ def learner_setup(env: Environment, keys: Tuple[int, int], config: DictConfig) -
     """Initialise learner_fn, network, optimiser, environment and states (ff_pqn.py:223-330).  Returns the EVAL network (epsilon =
     system.evaluation_epsilon) as the second element, which is what the reference hands to the evaluator."""
     _refuse_bf16(config)
-    rank, world = _world()
+    rank, world = anakin.world()
     device = torch.device("cuda", torch.cuda.current_device())
     action_dim = int(env.action_space().num_values)
     config.system.action_dim = action_dim
@@ -367,16 +323,9 @@ def learner_setup(env: Environment, keys: Tuple[int, int], config: DictConfig) -
 
     learn = get_learner_fn(env, q_network.apply, q_optim.update, epsilon_schedule, config)
 
-    U, E = int(config.arch.update_batch_size), int(config.arch.num_envs)
-    env_states: List[Any] = []
-    timesteps: List[TimeStep] = []
+    U = int(config.arch.update_batch_size)
     shard_keys = srandom.split(key, U + 1)
-    for u in range(U):
-        if hasattr(env, "seed"):
-            env.seed = (int(config.arch.seed) + 7919 * rank + 15485863 * u) & ((1 << 63) - 1)
-        st, ts = env.reset(srandom.split(shard_keys[u], E))
-        env_states.append(st)
-        timesteps.append(ts)
+    env_states, timesteps = anakin.reset_shards(env, shard_keys, config, rank)
 
     if config.logger.checkpointing.load_model:
         from stoix_b200.utils.checkpointing import Checkpointer
@@ -384,108 +333,20 @@ def learner_setup(env: Environment, keys: Tuple[int, int], config: DictConfig) -
         loaded = Checkpointer(model_name=config.system.system_name, **to_container(config.logger.checkpointing.load_args))
         loaded.restore_params(arena)
 
-    step_key = srandom.split(shard_keys[U], 2 * world)
-    rollout_seed = step_key[2 * rank] & ((1 << 62) - 1)
-    shuffle_seed = step_key[2 * rank + 1] & ((1 << 62) - 1)
+    rollout_seed, shuffle_seed = anakin.rank_seeds(shard_keys[U], 2, rank, world)
     init_learner_state = OnPolicyLearnerState(params=params, opt_states=opt_states, key=(rollout_seed, shuffle_seed), env_state=env_states,
                                               timestep=timesteps)
     return learn, eval_q_network, init_learner_state
 
 
-class _QParams(NamedTuple):
-    actor_params: Any  # the Checkpointer stores the arenas of params.actor_params
-
-
-class _CheckpointView(NamedTuple):
-    params: _QParams
-
-
 def run_experiment(_config: DictConfig) -> float:
-    """Runs experiment (ff_pqn.py:333-485)."""
-    from stoix_b200.evaluator import evaluator_setup, get_distribution_act_fn
-    from stoix_b200.systems.ppo.anakin.ff_ppo import get_final_step_metrics
-
-    config = copy.deepcopy(_config)
-    rank, world = _world()
-    config.num_devices, config.rank = world, rank
-    config = check_total_timesteps(config, quiet=rank != 0)
-    assert config.arch.num_updates >= config.arch.num_evaluation, "Number of updates per evaluation must be less than total number of updates."
-    env, eval_env = environments.make(config=config)
-    key, key_e, q_net_key = srandom.split(srandom.PRNGKey(config.arch.seed), num=3)
-    learn, eval_q_network, learner_state = learner_setup(env, (key, q_net_key), config)
-    evaluator, absolute_metric_evaluator = evaluator_setup(eval_env=eval_env, key_e=key_e,
-                                                           eval_act_fn=get_distribution_act_fn(config, eval_q_network.apply), config=config)
-    steps_per_rollout = world * config.arch.num_updates_per_eval * config.system.rollout_length * config.arch.update_batch_size * config.arch.num_envs
-    logger = StoixLogger(config)
-    logger.log_config(to_container(config, resolve=True))
-    save_checkpoint = config.logger.checkpointing.save_model
-    if save_checkpoint:
-        from stoix_b200.utils.checkpointing import Checkpointer
-
-        checkpointer = Checkpointer(metadata=to_container(config), model_name=config.system.system_name,
-                                    **to_container(config.logger.checkpointing.save_args))
-    max_episode_return = -float("inf")
-    best_params = learner_state.params.flat.clone()
-    evaluator_output = None
-    eval_step = 0
-    for eval_step in range(config.arch.num_evaluation):
-        start_time = time.time()
-        learner_output = learn(learner_state)
-        torch.cuda.synchronize()
-        elapsed_time = time.time() - start_time
-        t = int(steps_per_rollout * (eval_step + 1))
-        episode_metrics, ep_completed = get_final_step_metrics(learner_output.episode_metrics)
-        episode_metrics["steps_per_second"] = torch.tensor(steps_per_rollout / elapsed_time)
-        logger.log({"timestep": t}, t, eval_step, LogEvent.MISC)
-        if ep_completed:
-            logger.log(episode_metrics, t, eval_step, LogEvent.ACT)
-        train_metrics = dict(learner_output.train_metrics)
-        opt_steps_per_eval = config.arch.num_updates_per_eval * config.system.epochs * config.system.num_minibatches
-        train_metrics["steps_per_second"] = torch.tensor(opt_steps_per_eval / elapsed_time)
-        logger.log(train_metrics, t, eval_step, LogEvent.TRAIN)
-        start_time = time.time()
-        trained_params = learner_output.learner_state.params
-        evaluator_output = evaluator(trained_params, srandom.split(key_e, eval_step + 2)[-1])
-        torch.cuda.synchronize()
-        elapsed_time = time.time() - start_time
-        episode_return = float(evaluator_output["episode_return"].mean().item())
-        evaluator_output["steps_per_second"] = torch.tensor(int(evaluator_output["episode_length"].sum().item()) / max(elapsed_time, 1e-9))
-        logger.log(evaluator_output, t, eval_step, LogEvent.EVAL)
-        if save_checkpoint and rank == 0:
-            checkpointer.save(timestep=t, unreplicated_learner_state=_CheckpointView(_QParams(trained_params)), episode_return=episode_return)
-        if config.arch.absolute_metric and max_episode_return <= episode_return:
-            best_params = trained_params.flat.clone()
-            max_episode_return = episode_return
-        learner_state = learner_output.learner_state
-    if config.arch.absolute_metric:
-        from stoix_b200.networks.base import build_param_tree
-
-        start_time = time.time()
-        t = int(steps_per_rollout * (eval_step + 1))
-        best_tree = build_param_tree(learner_state.params.spec, best_params, "action_head")
-        evaluator_output = absolute_metric_evaluator(best_tree, srandom.split(key_e, 1)[0])
-        torch.cuda.synchronize()
-        elapsed_time = time.time() - start_time
-        evaluator_output["steps_per_second"] = torch.tensor(int(evaluator_output["episode_length"].sum().item()) / max(elapsed_time, 1e-9))
-        logger.log(evaluator_output, t, eval_step, LogEvent.ABSOLUTE)
-    logger.stop()
-    return float(evaluator_output[config.env.eval_metric].float().mean().item())
+    """Runs experiment (ff_pqn.py:333-485): the Q network's parameters are evaluated, tracked and checkpointed."""
+    return anakin.run_experiment(_config, learner_setup, net_keys=1, policy=lambda s: s.params)
 
 
 def hydra_entry_point(cfg: Optional[DictConfig] = None, overrides: Optional[List[str]] = None) -> float:
     """Experiment entry point with config default_ff_pqn: `python -m stoix_b200.systems.q_learning.ff_pqn arch.total_num_envs=1024 ...`"""
-    import os
-
-    if cfg is None:
-        cfg = compose("default_ff_pqn", overrides if overrides is not None else sys.argv[1:], config_dir="default/anakin")
-    if "RANK" in os.environ and not dist.is_initialized():
-        torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", 0)))
-        dist.init_process_group("nccl")
-    t0 = time.time()
-    eval_performance = run_experiment(cfg)
-    if _world()[0] == 0:
-        print(f"PQN experiment completed in {time.time() - t0:.2f} seconds.")
-    return eval_performance
+    return anakin.entry_point(cfg, overrides, "default_ff_pqn", run_experiment, "PQN")
 
 
 if __name__ == "__main__":

@@ -19,11 +19,6 @@ Every random stream position (policy noise, replay indices) is a device counter,
 """
 from __future__ import annotations
 
-import copy
-import gc
-import os
-import sys
-import time
 from typing import Any, Callable, Dict, List, Optional, Tuple
 
 import torch
@@ -33,25 +28,17 @@ from stoix_b200 import ops
 from stoix_b200 import optim as optax
 from stoix_b200 import random as srandom
 from stoix_b200.base_types import AnakinExperimentOutput
-from stoix_b200.config import DictConfig, compose, instantiate, to_container
+from stoix_b200.config import DictConfig, instantiate, to_container
 from stoix_b200.envs.base import Environment, TimeStep
 from stoix_b200.networks.base import FeedForwardActor as Actor
 from stoix_b200.networks.base import FeedForwardQ, MultiNetwork, build_param_tree
+from stoix_b200.systems import anakin
 from stoix_b200.systems.sac.sac_types import OffPolicyLearnerState, OnlineAndTarget, SACOptStates, SACParams, Transition
-from stoix_b200.utils import make_env as environments
-from stoix_b200.utils.logger import LogEvent, StoixLogger
 from stoix_b200.utils.replay import TransitionBuffer
-from stoix_b200.utils.total_timestep_checker import check_total_timesteps
 from stoix_b200.utils.training import make_learning_rate
 
 _METRIC_NAMES = ("actor_loss", "entropy", "q_loss", "q_error", "q1_pred", "q2_pred", "alpha_loss", "alpha")
 _pad8 = lambda n: (int(n) + 7) // 8 * 8
-
-
-def _world() -> Tuple[int, int]:
-    if dist.is_available() and dist.is_initialized():
-        return dist.get_rank(), dist.get_world_size()
-    return 0, 1
 
 
 def sac_arena_layout(actor: ops.MlpSpec, q: ops.MlpSpec) -> Dict[str, int]:
@@ -91,14 +78,6 @@ class _Shard:
                           {"episode_return": self.episode_return, "episode_length": self.episode_length, "is_terminal_step": self.is_terminal_step})
 
 
-def _owner(fn, kind, what):
-    obj = getattr(fn, "__self__", None)
-    if not isinstance(obj, kind):
-        raise TypeError(f"{what} must be a bound method of a stoix_b200 {kind.__name__} (got {fn!r}); arbitrary callables cannot be "
-                        "lowered onto the CUDA kernels")
-    return obj
-
-
 def _policy_step(env: Environment, actor_apply_fn, actor_params, env_state, obs: torch.Tensor, seed: int, offset: int, counter):
     """SELECT ACTION + STEP ENVIRONMENT (ff_sac.py:56-75 / 121-140)."""
     action = actor_apply_fn(actor_params, obs).sample(seed=seed, offset=offset, dev_counter=counter)
@@ -131,11 +110,11 @@ def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], updat
     they are read for the shapes / hyper-parameters they are bound to, the arithmetic runs in the kernels named in the header.
     buffer_fns = (TransitionBuffer.add, TransitionBuffer.sample_into) unbound, applied to learner_state.buffer_state[u]."""
     actor_apply_fn, q_apply_fn = apply_fns
-    actor_net = _owner(actor_apply_fn, Actor, "apply_fns[0]")
-    _owner(q_apply_fn, MultiNetwork, "apply_fns[1]")
-    actor_opt, q_opt, alpha_opt = (_owner(f, optax.GradientTransformation, f"update_fns[{i}]") for i, f in enumerate(update_fns))
+    actor_net = anakin.owner(actor_apply_fn, Actor, "apply_fns[0]")
+    anakin.owner(q_apply_fn, MultiNetwork, "apply_fns[1]")
+    actor_opt, q_opt, alpha_opt = (anakin.owner(f, optax.GradientTransformation, f"update_fns[{i}]") for i, f in enumerate(update_fns))
     buffer_add_fn, buffer_sample_fn = buffer_fns
-    rank, world = _world()
+    rank, world = anakin.world()
     sysc, arch = config.system, config.arch
     T, E, U = int(sysc.rollout_length), int(arch.num_envs), int(arch.update_batch_size)
     epochs, B = int(sysc.epochs), int(sysc.batch_size)
@@ -269,30 +248,9 @@ def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], updat
                   "is_terminal_step": torch.empty(n_upd, U, T, E, dtype=torch.bool, device=dev)}
         train_out = torch.empty(n_upd, epochs, 8, device=dev)
         for k in range(n_upd):
-            if use_graph and b["eager_done"] and b["graph"] is None:
-                g = torch.cuda.CUDAGraph()
-                torch.cuda.synchronize()
-                gc.collect()   # no cyclic GC (which may destroy an older CUDAGraph) while the stream is capturing
-                gc_was_enabled = gc.isenabled()
-                gc.disable()
-                added = [sh.buffer.added for sh in b["shards"]]   # capturing launches nothing: keep the host mirrors where they are
-                try:
-                    with torch.cuda.graph(g):
-                        _update_step(learner_state)
-                finally:
-                    if gc_was_enabled:
-                        gc.enable()
-                for sh, n in zip(b["shards"], added):
-                    sh.buffer.added = n
-                b["graph"] = g
-            if b["graph"] is not None:
-                b["graph"].replay()
-            else:
-                _update_step(learner_state)
-                b["eager_done"] = True
+            anakin.update_once(b, use_graph, _update_step, learner_state, [sh.buffer for sh in b["shards"]], T * E)
             for u in range(U):
                 sh = b["shards"][u]
-                sh.buffer.added += T * E if b["graph"] is not None else 0   # host mirror of the item count under replay
                 ep_out["episode_return"][k, u].copy_(sh.episode_return)
                 ep_out["episode_length"][k, u].copy_(sh.episode_length)
                 ep_out["is_terminal_step"][k, u].copy_(sh.is_terminal_step)
@@ -318,9 +276,8 @@ def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], updat
 
 def learner_setup(env: Environment, keys: Tuple[int, int, int], config: DictConfig):
     """Initialise learner_fn, networks, optimisers, buffer, environment and states (ff_sac.py:347-513)."""
-    rank, world = _world()
+    rank, n_devices = anakin.world()
     device = torch.device("cuda", torch.cuda.current_device())
-    n_devices = world
 
     action_space = env.action_space()
     action_dim = int(action_space.shape[-1])
@@ -384,7 +341,7 @@ def learner_setup(env: Environment, keys: Tuple[int, int, int], config: DictConf
     update_fns = (actor_optim.update, q_optim.update, alpha_optim.update)
 
     # Replay buffer (:429-456): one ring per (device, update-batch shard)
-    U, E = int(config.arch.update_batch_size), int(config.arch.num_envs)
+    U = int(config.arch.update_batch_size)
     assert int(config.system.total_buffer_size) % n_devices == 0, "The total buffer size should be divisible by the number of devices!"
     assert int(config.system.total_batch_size) % n_devices == 0, "The total batch size should be divisible by the number of devices!"
     config.system.buffer_size = int(config.system.total_buffer_size) // (n_devices * U)
@@ -398,14 +355,7 @@ def learner_setup(env: Environment, keys: Tuple[int, int, int], config: DictConf
     warmup = get_warmup_fn(env, params, actor_network.apply, TransitionBuffer.add, config)
 
     # Initialise environment states and timesteps across update-batch shards (:463-474).
-    env_states: List[Any] = []
-    timesteps: List[TimeStep] = []
-    for u in range(U):
-        if hasattr(env, "seed"):
-            env.seed = (int(config.arch.seed) + 7919 * rank + 15485863 * u) & ((1 << 63) - 1)
-        st, ts = env.reset(srandom.split(shard_keys[u], E))
-        env_states.append(st)
-        timesteps.append(ts)
+    env_states, timesteps = anakin.reset_shards(env, shard_keys, config, rank)
 
     if config.logger.checkpointing.load_model:   # params only, as in the reference (:477-486)
         from stoix_b200.utils.checkpointing import Checkpointer
@@ -415,9 +365,7 @@ def learner_setup(env: Environment, keys: Tuple[int, int, int], config: DictConf
         target_arena.copy_(arena[lay["q1"]: lay["alpha"]])
 
     # per-rank streams: (rollout policy noise, loss noise); warm-up noise on its own key (:489-496)
-    step_key = srandom.split(shard_keys[U + 1], 3 * n_devices)
-    m62 = (1 << 62) - 1
-    act_seed, eps_seed, warm_seed = (step_key[3 * rank + i] & m62 for i in range(3))
+    act_seed, eps_seed, warm_seed = anakin.rank_seeds(shard_keys[U + 1], 3, rank, n_devices)
 
     # Warm up the buffer (:507-509).
     for u in range(U):
@@ -427,108 +375,14 @@ def learner_setup(env: Environment, keys: Tuple[int, int, int], config: DictConf
     return learn, actor_network, init_learner_state
 
 
-def get_final_step_metrics(metrics: Dict[str, torch.Tensor]) -> Tuple[Dict[str, torch.Tensor], bool]:
-    mask = metrics["is_terminal_step"]
-    has_final = bool(mask.any().item())
-    out = {k: (v[mask] if has_final else v.reshape(-1)[:0]) for k, v in metrics.items() if k != "is_terminal_step"}
-    return out, has_final
-
-
 def run_experiment(_config: DictConfig) -> float:
     """Runs experiment (ff_sac.py:516-675)."""
-    from stoix_b200.evaluator import evaluator_setup, get_distribution_act_fn
-
-    config = copy.deepcopy(_config)
-    rank, world = _world()
-    n_devices = world
-    config.num_devices = n_devices
-    config.rank = rank
-    config = check_total_timesteps(config, quiet=rank != 0)
-    assert config.arch.num_updates >= config.arch.num_evaluation, \
-        "Number of updates per evaluation must be less than total number of updates."
-
-    env, eval_env = environments.make(config=config)
-    key, key_e, actor_net_key, q_net_key = srandom.split(srandom.PRNGKey(config.arch.seed), num=4)
-    learn, actor_network, learner_state = learner_setup(env, (key, actor_net_key, q_net_key), config)
-
-    evaluator, absolute_metric_evaluator = evaluator_setup(
-        eval_env=eval_env, key_e=key_e, eval_act_fn=get_distribution_act_fn(config, actor_network.apply), config=config)
-
-    steps_per_rollout = (n_devices * config.arch.num_updates_per_eval * config.system.rollout_length
-                         * config.arch.update_batch_size * config.arch.num_envs)
-    logger = StoixLogger(config)
-    logger.log_config(to_container(config, resolve=True))
-    save_checkpoint = config.logger.checkpointing.save_model
-    if save_checkpoint:
-        from stoix_b200.utils.checkpointing import Checkpointer
-
-        checkpointer = Checkpointer(metadata=to_container(config), model_name=config.system.system_name,
-                                    **to_container(config.logger.checkpointing.save_args))
-
-    max_episode_return = -float("inf")
-    best_params = learner_state.params.actor_params.flat.clone()
-    evaluator_output = None
-    eval_step = 0
-    for eval_step in range(config.arch.num_evaluation):
-        start_time = time.time()
-        learner_output = learn(learner_state)
-        torch.cuda.synchronize()
-        elapsed_time = time.time() - start_time
-        t = int(steps_per_rollout * (eval_step + 1))
-        episode_metrics, ep_completed = get_final_step_metrics(learner_output.episode_metrics)
-        episode_metrics["steps_per_second"] = torch.tensor(steps_per_rollout / elapsed_time)
-        logger.log({"timestep": t}, t, eval_step, LogEvent.MISC)
-        if ep_completed:
-            logger.log(episode_metrics, t, eval_step, LogEvent.ACT)
-        train_metrics = dict(learner_output.train_metrics)
-        opt_steps_per_eval = config.arch.num_updates_per_eval * config.system.epochs
-        train_metrics["steps_per_second"] = torch.tensor(opt_steps_per_eval / elapsed_time)
-        logger.log(train_metrics, t, eval_step, LogEvent.TRAIN)
-
-        start_time = time.time()
-        trained_params = learner_output.learner_state.params.actor_params
-        evaluator_output = evaluator(trained_params, srandom.split(key_e, eval_step + 2)[-1])
-        torch.cuda.synchronize()
-        elapsed_time = time.time() - start_time
-        episode_return = float(evaluator_output["episode_return"].mean().item())
-        steps_per_eval = int(evaluator_output["episode_length"].sum().item())
-        evaluator_output["steps_per_second"] = torch.tensor(steps_per_eval / max(elapsed_time, 1e-9))
-        logger.log(evaluator_output, t, eval_step, LogEvent.EVAL)
-
-        if save_checkpoint and rank == 0:
-            checkpointer.save(timestep=t, unreplicated_learner_state=learner_output.learner_state, episode_return=episode_return)
-        if config.arch.absolute_metric and max_episode_return <= episode_return:
-            best_params = trained_params.flat.clone()
-            max_episode_return = episode_return
-        learner_state = learner_output.learner_state
-
-    if config.arch.absolute_metric:
-        start_time = time.time()
-        t = int(steps_per_rollout * (eval_step + 1))
-        best_tree = build_param_tree(learner_state.params.actor_params.spec, best_params, "action_head")
-        evaluator_output = absolute_metric_evaluator(best_tree, srandom.split(key_e, 1)[0])
-        torch.cuda.synchronize()
-        elapsed_time = time.time() - start_time
-        steps_per_eval = int(evaluator_output["episode_length"].sum().item())
-        evaluator_output["steps_per_second"] = torch.tensor(steps_per_eval / max(elapsed_time, 1e-9))
-        logger.log(evaluator_output, t, eval_step, LogEvent.ABSOLUTE)
-
-    logger.stop()
-    return float(evaluator_output[config.env.eval_metric].float().mean().item())
+    return anakin.run_experiment(_config, learner_setup, net_keys=2)
 
 
 def hydra_entry_point(cfg: Optional[DictConfig] = None, overrides: Optional[List[str]] = None) -> float:
     """Experiment entry point: `python -m stoix_b200.systems.sac.ff_sac arch.total_num_envs=1024 system.total_batch_size=256 ...`"""
-    if cfg is None:
-        cfg = compose("default_ff_sac", overrides if overrides is not None else sys.argv[1:], config_dir="default/anakin")
-    if "RANK" in os.environ and not dist.is_initialized():
-        torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", 0)))
-        dist.init_process_group("nccl")
-    t0 = time.time()
-    eval_performance = run_experiment(cfg)
-    if _world()[0] == 0:
-        print(f"SAC experiment completed in {time.time() - t0:.2f} seconds.")
-    return eval_performance
+    return anakin.entry_point(cfg, overrides, "default_ff_sac", run_experiment, "SAC")
 
 
 if __name__ == "__main__":
