@@ -7,7 +7,7 @@ passes around as `update_fns`; `chain(clip_by_global_norm(m), radam(lr))` (ff_pq
 from __future__ import annotations
 
 from dataclasses import dataclass, field
-from typing import Any, Callable, NamedTuple, Optional, Union
+from typing import Any, Callable, List, NamedTuple, Optional, Sequence, Tuple, Union
 
 
 @dataclass
@@ -69,12 +69,6 @@ class GradientTransformation:
         """"radam" for an optax.radam stage, else "adam"."""
         return "radam" if isinstance(self.adam, _Radam) else "adam"
 
-    def plan_kwargs(self) -> dict:
-        """The AdamPlan arguments of this stage's update rule."""
-        if self.rule == "radam":
-            return {"rule": "radam", "eps_root": self.adam.eps_root, "threshold": self.adam.threshold}
-        return {}
-
     @property
     def max_grad_norm(self) -> float:
         return self.clip.max_norm if self.clip is not None else float("inf")
@@ -112,13 +106,8 @@ class GradientTransformation:
         buf = lambda src: torch.cat([src.reshape(-1).float(), src.new_zeros(pad, dtype=torch.float32)]) if pad else src.reshape(-1).float().clone()
         p = torch.zeros(n + pad, dtype=torch.float32, device=g.device)
         mu, nu, gg = buf(state.mu), buf(state.nu), buf(g)
-        sched = self.schedule
-        plan = ops.AdamPlan([(0, n, self.init_lr, self.max_grad_norm if self.clip is not None else 3.0e38)], g.device,
-                            b1=self.adam.b1, b2=self.adam.b2, eps=self.adam.eps, decay=sched is not None,
-                            steps_per_update=getattr(sched, "steps_per_update", 1), num_updates=getattr(sched, "num_updates", 1),
-                            **self.plan_kwargs())
-        plan.counts[0:1].copy_(state.count.reshape(-1)[:1])
-        plan.counts[1:2].copy_(state.sched_count.reshape(-1)[:1])
+        counts = torch.cat([state.count.reshape(-1)[:1], state.sched_count.reshape(-1)[:1]]).to(device=g.device, dtype=torch.int32)
+        plan = adam_plan([(0, n, self)], g.device, counts)
         ops.clip_adam_step(plan, p, gg, mu, nu)
         new_state = OptState(plan.counts[0:1].clone(), mu[:n].view_as(state.mu), nu[:n].view_as(state.nu), plan.counts[1:2].clone())
         return p[:n].view_as(g), new_state   # parameters started at zero: what is left is the update -lr * u
@@ -128,6 +117,37 @@ def apply_updates(params, updates):
     """optax.apply_updates: params + updates (functional)."""
     p = GradientTransformation._flat(params)
     return p + GradientTransformation._flat(updates)
+
+
+def adam_plan(segments: Sequence[Tuple[int, int, GradientTransformation]], device, counts) -> "ops.AdamPlan":
+    """The ops.AdamPlan of one fused optimiser launch over `segments` = (offset, count, transformation): each segment takes its
+    learning rate and clip norm from its transformation; the update rule, b1 / b2 / eps and the learning-rate decay come from the
+    first one's stage and schedule (make_learning_rate attaches steps_per_update and num_updates to a decaying schedule; without
+    one the kernels read neither).  `counts` (int32, one {count, schedule count} pair per segment, usually a learner state's
+    arena_counts) becomes the plan's counters, so the kernel steps it in place."""
+    from . import ops
+
+    opt = segments[0][2]
+    sched = opt.schedule
+    rule = {"rule": "radam", "eps_root": opt.adam.eps_root, "threshold": opt.adam.threshold} if opt.rule == "radam" else {}
+    plan = ops.AdamPlan([(off, n, o.init_lr, o.max_grad_norm if o.clip is not None else 3.0e38) for off, n, o in segments], device,
+                        b1=opt.adam.b1, b2=opt.adam.b2, eps=opt.adam.eps, decay=sched is not None,
+                        steps_per_update=getattr(sched, "steps_per_update", 1), num_updates=getattr(sched, "num_updates", 1), **rule)
+    plan.counts = counts
+    return plan
+
+
+def arena_state(tree, arena, segments: Sequence[Tuple[int, int]]) -> List[OptState]:
+    """The optimiser state of a flat parameter arena: mu / nu arenas shaped like it and one int32 {count, schedule count} pair per
+    segment (offset, count).  Returns one OptState of views per segment, and attaches arena, arena_mu, arena_nu and arena_counts
+    to `tree`: the fused kernels work on the whole arenas, and a checkpoint of the tree carries them."""
+    import torch
+
+    mu, nu = torch.zeros_like(arena), torch.zeros_like(arena)
+    counts = torch.zeros(2 * len(segments), dtype=torch.int32, device=arena.device)
+    tree.arena, tree.arena_mu, tree.arena_nu, tree.arena_counts = arena, mu, nu, counts
+    return [OptState(counts[2 * i:2 * i + 1], mu[off:off + n], nu[off:off + n], counts[2 * i + 1:2 * i + 2])
+            for i, (off, n) in enumerate(segments)]
 
 
 def chain(*parts) -> GradientTransformation:

@@ -28,6 +28,7 @@ from stoix_b200.config import DictConfig, compose, to_container
 from stoix_b200.envs.base import Environment, StepOut, TimeStep
 from stoix_b200.evaluator import evaluator_setup, get_distribution_act_fn
 from stoix_b200.networks.base import build_param_tree
+from stoix_b200.systems.sac.sac_types import Transition
 from stoix_b200.utils import make_env as environments
 from stoix_b200.utils.checkpointing import Checkpointer
 from stoix_b200.utils.logger import LogEvent, StoixLogger
@@ -84,12 +85,145 @@ def step_env(env: Environment, env_states: List[Any], u: int, action: torch.Tens
     out.obs.copy_(ts.observation)
     out.next_obs.copy_(ts.extras["next_obs"])
     out.reward.copy_(ts.reward)
-    out.done.copy_(ts.discount == 0.0)
-    out.truncated.copy_(ts.last() & (ts.discount != 0.0))
+    torch.eq(ts.discount, 0.0, out=out.done)
+    torch.gt(ts.last(), out.done, out=out.truncated)   # last and not terminated
     em = ts.extras["episode_metrics"]
     out.episode_return.copy_(em["episode_return"])
     out.episode_length.copy_(em["episode_length"])
     out.is_terminal_step.copy_(em["is_terminal_step"])
+
+
+class Trajectory:
+    """What the environment writes in one (device, update-batch) shard's T-step rollout, time-major.  Row t of obs is the
+    observation step t acts on; row T is the carry, the first observation of the next rollout.  terminated / truncated are the
+    env's flags (StepOut.done / .truncated).  With raw_obs the environment writes fp32 observations into obs_raw / next_obs_raw
+    and obs / next_obs (obs_dtype) hold the normalised copies the networks read."""
+
+    perms: Optional[torch.Tensor] = None   # (epochs, T*E) int32 minibatch shuffles of the update, allocated by shuffle()
+
+    def __init__(self, T: int, E: int, D: int, device, obs_dtype=torch.float32, raw_obs: bool = False):
+        z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=device)
+        self.T = T
+        self.obs, self.next_obs = z(T + 1, E, D, dt=obs_dtype), z(T, E, D, dt=obs_dtype)
+        self.obs_raw, self.next_obs_raw = (z(T + 1, E, D), z(T, E, D)) if raw_obs else (None, None)
+        self.reward = z(T, E)
+        self.terminated, self.truncated = z(T, E, dt=torch.uint8), z(T, E, dt=torch.uint8)
+        self.episode_return, self.episode_length = z(T, E), z(T, E, dt=torch.int32)
+        self.is_terminal_step = z(T, E, dt=torch.uint8)
+
+    @property
+    def env_obs(self) -> torch.Tensor:
+        """(T+1, E, D) observations as the environment produced them (raw when normalising)."""
+        return self.obs if self.obs_raw is None else self.obs_raw
+
+    def step_out(self, t: int) -> StepOut:
+        nxt = self.next_obs if self.next_obs_raw is None else self.next_obs_raw
+        return StepOut(self.env_obs[t + 1], nxt[t], self.reward[t], self.terminated[t], self.truncated[t], self.episode_return[t],
+                       self.episode_length[t], self.is_terminal_step[t])
+
+    def carry_in(self) -> None:
+        """The latest observation (row T of the previous rollout) is the first of this rollout; the finished trajectory stays
+        readable until then."""
+        self.env_obs[0].copy_(self.env_obs[self.T])
+
+    def advance(self, env: Environment, env_state: Any) -> None:
+        """Move the env's device-resident step counter past this rollout (graph replays then step fresh numbers)."""
+        if hasattr(env, "advance"):
+            env.advance(env_state, self.T)
+
+
+def shuffle(shards: Sequence[Trajectory], epochs: int, seed: int, counter: torch.Tensor) -> None:
+    """SHUFFLE MINIBATCHES for all epochs of an update: one keyed permutation of the T*E flat rows per (shard, epoch), at stream
+    position `counter`, into shard.perms."""
+    for u, sh in enumerate(shards):
+        n = sh.reward.numel()
+        if sh.perms is None:
+            sh.perms = torch.zeros(epochs, n, dtype=torch.int32, device=counter.device)
+        for ep in range(epochs):
+            ops.make_permutation(n, seed + u, ep, dev_counter=counter, out=sh.perms[ep])
+
+
+def shuffle_beside(built: Dict[str, Any], epochs: int, seed: int, rollout: Callable[[], None]) -> None:
+    """shuffle() on built["side_stream"] while `rollout()` runs on the current stream: forked before it, joined after it.  The
+    permutations depend on the seed and built["perm_ctr"] only, not on the rollout, which leaves most SMs idle."""
+    main, side = torch.cuda.current_stream(), built["side_stream"]
+    side.wait_stream(main)  # fork (a graph branch when captured)
+    with torch.cuda.stream(side):
+        shuffle(built["shards"], epochs, seed, built["perm_ctr"])
+    rollout()
+    main.wait_stream(side)  # join
+
+
+def ensure_built(built: Dict[str, Any], build: Callable[[Any], None], state: Any) -> None:
+    """Build a learner once, from its first learner state: build(state) fills `built` (with its "shards"), and each shard's carry
+    row T starts from state.timestep[u].observation."""
+    if not built:
+        build(state)
+        for sh, ts in zip(built["shards"], state.timestep):
+            sh.env_obs[-1].copy_(ts.observation)
+
+
+_EPISODE_FIELDS = ("episode_return", "episode_length", "is_terminal_step")
+
+
+def learn(built: Dict[str, Any], build: Callable[[Any], None], step: Callable[[Any], None], state: Any, config: DictConfig,
+          extra_fields: Sequence[str] = (), buffers: Sequence[Any] = ()) -> Tuple[List[TimeStep], Dict[str, torch.Tensor], torch.Tensor]:
+    """The body of every Anakin learner_fn around its update step: ensure_built, then arch.num_updates_per_eval update_once calls
+    (buffers: the replay buffers each step adds its T*E transitions to).  Returns the timesteps the next learn() starts from,
+    the episode metrics (plus each shard's `extra_fields`) as (n_upd, U, T, E) tensors, and built["metrics"] after every update,
+    stacked as (n_upd, *metrics.shape)."""
+    ensure_built(built, build, state)
+    shards, metrics = built["shards"], built["metrics"]
+    n_upd = int(config.arch.num_updates_per_eval)
+    fields = _EPISODE_FIELDS + tuple(extra_fields)
+    dtype = lambda name: torch.bool if name == "is_terminal_step" else getattr(shards[0], name).dtype
+    ep_out = {name: torch.empty(n_upd, len(shards), *getattr(shards[0], name).shape, dtype=dtype(name), device=metrics.device)
+              for name in fields}
+    train_out = torch.empty(n_upd, *metrics.shape, dtype=metrics.dtype, device=metrics.device)
+    items = shards[0].reward.numel()
+    for k in range(n_upd):
+        update_once(built, bool(config.arch.get("cuda_graph", True)), step, state, buffers, items)
+        for u, sh in enumerate(shards):
+            for name in fields:
+                ep_out[name][k, u].copy_(getattr(sh, name))
+        train_out[k].copy_(metrics)
+    timestep = [ts._replace(observation=sh.env_obs[-1]) for ts, sh in zip(state.timestep, shards)]
+    return timestep, ep_out, train_out
+
+
+def replay_buffers(config: DictConfig, key: int, rank: int, n_devices: int, make: Callable[[int, int, int], Any]) -> List[Any]:
+    """This rank's replay buffers, one per update-batch shard: system.total_buffer_size / total_batch_size are split evenly over
+    (device, shard) into config.system.buffer_size / batch_size, and buffer u = make(buffer_size, batch_size, seed) with
+    seed = split(key, n_devices * U)[rank * U + u]."""
+    U = int(config.arch.update_batch_size)
+    assert int(config.system.total_buffer_size) % n_devices == 0, "The total buffer size should be divisible by the number of devices!"
+    assert int(config.system.total_batch_size) % n_devices == 0, "The total batch size should be divisible by the number of devices!"
+    config.system.buffer_size = int(config.system.total_buffer_size) // (n_devices * U)
+    config.system.batch_size = int(config.system.total_batch_size) // (n_devices * U)
+    seeds = srandom.split(key, n_devices * U)
+    return [make(config.system.buffer_size, config.system.batch_size, seeds[rank * U + u]) for u in range(U)]
+
+
+def warmup_fn(env: Environment, draw: Callable[[torch.Tensor, int, int], torch.Tensor], buffer_add_fn: Callable,
+              config: DictConfig) -> Callable:
+    """The warm-up of an off-policy system: system.warmup_steps environment steps of one shard, acting with
+    draw(obs, key, t), added to the buffer as one Transition (done = timestep.last())."""
+    W = int(config.system.warmup_steps)
+
+    def warmup(env_state, timestep: TimeStep, buffer_state, key: int):
+        obs_l, act_l, rew_l, done_l, nobs_l = [], [], [], [], []
+        for t in range(W):
+            obs = timestep.observation.float().clone()
+            action = draw(obs, key, t)
+            env_state, timestep = env.step(env_state, action)
+            obs_l.append(obs), act_l.append(action), rew_l.append(timestep.reward.float())
+            done_l.append(timestep.last().to(torch.uint8)), nobs_l.append(timestep.extras["next_obs"].float())
+        if W > 0:
+            st = lambda xs: torch.stack(xs).contiguous()
+            buffer_add_fn(buffer_state, Transition(st(obs_l), st(act_l), st(rew_l), st(done_l), st(nobs_l), {}))
+        return env_state, timestep, key, buffer_state
+
+    return warmup
 
 
 def update_once(built: Dict[str, Any], use_graph: bool, step: Callable, state: Any, buffers: Sequence[Any] = (),

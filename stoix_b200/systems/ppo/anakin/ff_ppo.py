@@ -42,13 +42,14 @@ from stoix_b200.base_types import (
     LearnerFn,
     OnPolicyLearnerState,
 )
-from stoix_b200.config import DictConfig, instantiate, to_container
-from stoix_b200.envs.base import Environment, StepOut
+from stoix_b200.config import DictConfig, instantiate
+from stoix_b200.envs.base import Environment
 from stoix_b200.networks.base import FeedForwardActor as Actor
 from stoix_b200.networks.base import FeedForwardCritic as Critic
 from stoix_b200.networks.heads import NormalAffineTanhDistributionHead
 from stoix_b200.systems import anakin
 from stoix_b200.systems.ppo.ppo_types import PPOTransition
+from stoix_b200.utils.checkpointing import warm_start
 from stoix_b200.utils.training import make_learning_rate
 
 _METRIC_NAMES = ("actor_loss", "entropy", "value_loss", "advantages", "pred_value", "target_value")
@@ -63,47 +64,28 @@ _VARIANT_METRICS = {
 }
 
 
-class _Shard:
-    """Trajectory buffers of one (device, update-batch) shard: PPOTransition fields, time-major."""
+class _Shard(anakin.Trajectory):
+    """Trajectory buffers of one (device, update-batch) shard: PPOTransition fields, time-major.  With normalize_observations the
+    environment writes raw fp32 observations (they feed the running statistics, ff_ppo.py:145-162) and obs / next_obs hold the
+    normalised copies every network kernel reads (:90-94,113-115)."""
 
     def __init__(self, T: int, E: int, D: int, A: int, obs_dtype, device, normalize: bool = False, act_dim: int = 0,
                  behaviour: bool = False):
+        super().__init__(T, E, D, device, obs_dtype=obs_dtype, raw_obs=normalize)
         z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=device)
-        self.obs = z(T + 1, E, D, dt=obs_dtype)      # row t = last_timestep.observation of step t
-        self.next_obs = z(T, E, D, dt=obs_dtype)     # timestep.extras["next_obs"]   (ff_ppo.py:113)
-        # normalize_observations: the environment writes RAW fp32 observations here (they feed the running statistics,
-        # ff_ppo.py:145-162) and obs / next_obs above hold the normalised copies every network kernel reads (:90-94,113-115)
-        self.obs_raw = z(T + 1, E, D) if normalize else None
-        self.next_obs_raw = z(T, E, D) if normalize else None
+        self.done = self.terminated   # the transition's done: terminated only, truncation bootstraps
         # Categorical: (T, E) int32 action indices; tanh-Normal (act_dim > 0): (T, E, act_dim) float32 actions
         self.action = z(T, E, act_dim) if act_dim > 0 else z(T, E, dt=torch.int32)
         self.log_prob = z(T, E)
         self.value = z(T, E)
         self.bootstrap_value = z(T, E)
-        self.reward = z(T, E)
-        self.done = z(T, E, dt=torch.uint8)
-        self.truncated = z(T, E, dt=torch.uint8)
-        self.episode_return = z(T, E)
-        self.episode_length = z(T, E, dt=torch.int32)
-        self.is_terminal_step = z(T, E, dt=torch.uint8)
         self.advantages = z(T, E)
         self.targets = z(T, E)
         self.logits = z(E, A)                        # actor head output of one step: logits, or loc | scale pre-activation
         # KL penalty: the head output of every rollout step is kept as the behaviour policy of the update (the rollout actor is
         # the actor at the start of the update, ff_ppo_penalty.py:137, evaluated on the same rows the minibatches read)
         self.behaviour = z(T, E, A) if behaviour else None
-        self.perms = None  # (epochs, T*E) int32 shuffles of this update, allocated by the learner
         self.adv_stats: Optional[torch.Tensor] = None
-
-    def step_out(self, t: int) -> StepOut:
-        obs, nxt = (self.obs, self.next_obs) if self.obs_raw is None else (self.obs_raw, self.next_obs_raw)
-        return StepOut(obs[t + 1], nxt[t], self.reward[t], self.done[t], self.truncated[t],
-                       self.episode_return[t], self.episode_length[t], self.is_terminal_step[t])
-
-    @property
-    def env_obs(self) -> torch.Tensor:
-        """(T+1, E, D) observations as the environment produced them (raw when normalising)."""
-        return self.obs if self.obs_raw is None else self.obs_raw
 
     def transition(self, T: int) -> PPOTransition:
         info = {"episode_return": self.episode_return, "episode_length": self.episode_length,
@@ -140,7 +122,6 @@ def get_learner_fn(
     assert B % nmb == 0, "rollout_length * num_envs must be divisible by num_minibatches"
     mb = B // nmb
     precision = ops.STX_PREC_BF16 if str(arch.get("precision", "f32")) == "bf16" else ops.STX_PREC_F32
-    use_graph = bool(arch.get("cuda_graph", True))
     # The actor head decides the action buffer, the rollout sampler, the gradient entry and the entropy RNG; everything else
     # (GAE, shuffles, shards, all-reduce, observation normalisation, graph capture) is shared.
     tanh_head = actor_net.action_head if isinstance(actor_net.action_head, NormalAffineTanhDistributionHead) else None
@@ -173,15 +154,7 @@ def get_learner_fn(
         act_dim = tanh_head.action_dim if tanh_head is not None else 0
         shards = [_Shard(T, E, D, A, obs_dtype, dev, normalize=rs is not None, act_dim=act_dim, behaviour=loss == "kl_penalty")
                   for _ in range(U)]
-        decay = bool(sysc.decay_learning_rates)
-        plan = ops.AdamPlan(
-            [(0, sa.param_count, actor_opt.init_lr, actor_opt.max_grad_norm),
-             (coff, sc.param_count, critic_opt.init_lr, critic_opt.max_grad_norm)],
-            dev, b1=actor_opt.adam.b1, b2=actor_opt.adam.b2, eps=actor_opt.adam.eps, decay=decay,
-            steps_per_update=epochs * nmb, num_updates=int(arch.num_updates),
-        )
-        # optimiser counters live in the learner state (so a checkpointed state carries them)
-        plan.counts = a_tree.arena_counts
+        plan = optax.adam_plan([(0, sa.param_count, actor_opt), (coff, sc.param_count, critic_opt)], dev, a_tree.arena_counts)
         peers = None
         if world > 1 and bool(arch.get("fused_allreduce", True)) and (epochs * nmb) % 2 == 0 and world <= 8:
             try:  # gradient arenas in NVLink peer memory: the all-reduce is fused into the optimiser kernel
@@ -301,23 +274,11 @@ def get_learner_fn(
                 out=(sh.advantages, sh.targets),
             )
 
-    def _shuffle_phase(state: OnPolicyLearnerState) -> None:
-        """SHUFFLE MINIBATCHES (ff_ppo.py:294-307) for ALL epochs of this update: one keyed permutation of the flat index per
-        (shard, epoch).  They depend on the key and the device-resident stream counter only, not on the rollout, so the
-        update step issues them on a side stream underneath the rollout (which occupies E/64 of the 132 SMs)."""
-        b = built
-        for u in range(U):
-            sh = b["shards"][u]
-            if sh.perms is None:
-                sh.perms = torch.zeros(epochs, T * E, dtype=torch.int32, device=b["dev"])
-            for ep in range(epochs):
-                ops.make_permutation(T * E, state.key[1] + u, ep, dev_counter=b["perm_ctr"], out=sh.perms[ep])
-
     def _update_phase(state: OnPolicyLearnerState, shuffled: bool = False) -> None:
-        """UPDATE EPOCHS (ff_ppo.py:181-338)."""
+        """UPDATE EPOCHS (ff_ppo.py:181-338), after SHUFFLE MINIBATCHES (:294-307) unless the update step ran it under the rollout."""
         b = built
         if not shuffled:
-            _shuffle_phase(state)
+            anakin.shuffle(b["shards"], epochs, state.key[1], b["perm_ctr"])
         sa, sc = b["sa"], b["sc"]
         a_tree = state.params.actor_params
         seeds = state.key
@@ -391,76 +352,38 @@ def get_learner_fn(
             dist.all_reduce(metrics, op=dist.ReduceOp.SUM)
             metrics.mul_(1.0 / world)
 
-    def _carry_in_phase(state: OnPolicyLearnerState) -> None:
-        """The latest observation (row T of the previous rollout) is the first of this rollout
-        (learner_state.timestep of ff_ppo.py:131-134); the finished trajectory stays readable until then."""
-        for u in range(U):
-            sh = built["shards"][u]
-            sh.env_obs[0].copy_(sh.env_obs[T])
+    def _rollout_stats_gae(state: OnPolicyLearnerState) -> None:
+        _rollout_phase(state)
+        _stats_phase(state)
+        _gae_phase(state)
 
-    def _advance_phase(state: OnPolicyLearnerState) -> None:
-        """Advance the device-resident RNG stream positions (graph replays then draw fresh numbers)."""
+    def _update_step(state: OnPolicyLearnerState) -> None:
+        """A single update of the network (ff_ppo.py:61-341), in place on the learner state."""
         b = built
-        for u in range(U):
-            if hasattr(env, "advance"):
-                env.advance(state.env_state[u], T)
+        for sh in b["shards"]:   # learner_state.timestep of ff_ppo.py:131-134
+            sh.carry_in()
+        # the shuffles run underneath the rollout, which occupies E/64 of the 132 SMs
+        anakin.shuffle_beside(b, epochs, state.key[1], lambda: _rollout_stats_gae(state))
+        _update_phase(state, shuffled=True)
+        # advance the device-resident RNG stream positions (graph replays then draw fresh numbers)
+        for sh, env_state in zip(b["shards"], state.env_state):
+            sh.advance(env, env_state)
         ops.counter_add(b["roll_ctr"], T)
         ops.counter_add(b["perm_ctr"], epochs)
         if tanh_head is not None:
             ops.counter_add(b["ent_ctr"], epochs * nmb)
 
-    def _update_step(state: OnPolicyLearnerState) -> None:
-        """A single update of the network (ff_ppo.py:61-341), in place on the learner state."""
-        _carry_in_phase(state)
-        main = torch.cuda.current_stream()
-        side = built["side_stream"]
-        side.wait_stream(main)  # fork (a graph branch when captured)
-        with torch.cuda.stream(side):
-            _shuffle_phase(state)
-        _rollout_phase(state)
-        _stats_phase(state)
-        _gae_phase(state)
-        main.wait_stream(side)  # join
-        _update_phase(state, shuffled=True)
-        _advance_phase(state)
-
     def learner_fn(learner_state: OnPolicyLearnerState) -> AnakinExperimentOutput[OnPolicyLearnerState]:
         """Run arch.num_updates_per_eval update steps (ff_ppo.py:343-370)."""
-        learner_fn.ensure_built(learner_state)  # buffers + rollout seeded with last_timestep.observation
-        b = built
-        n_upd = int(arch.num_updates_per_eval)
-        dev = b["dev"]
-        ep_out = {
-            "episode_return": torch.empty(n_upd, U, T, E, device=dev),
-            "episode_length": torch.empty(n_upd, U, T, E, dtype=torch.int32, device=dev),
-            "is_terminal_step": torch.empty(n_upd, U, T, E, dtype=torch.bool, device=dev),
-        }
-        train_out = torch.empty(n_upd, epochs, nmb, 8, device=dev)
-        for k in range(n_upd):
-            anakin.update_once(b, use_graph, _update_step, learner_state)
-            for u in range(U):
-                sh = b["shards"][u]
-                ep_out["episode_return"][k, u].copy_(sh.episode_return)
-                ep_out["episode_length"][k, u].copy_(sh.episode_length)
-                ep_out["is_terminal_step"][k, u].copy_(sh.is_terminal_step)
-            train_out[k].copy_(b["metrics"])
-        # the observation the next learn() call starts from
-        new_ts = [learner_state.timestep[u]._replace(observation=b["shards"][u].env_obs[T]) for u in range(U)]
-        learner_state = learner_state._replace(timestep=new_ts)
+        timestep, episode_metrics, train_out = anakin.learn(built, _build, _update_step, learner_state, config)
         train_metrics = {name: train_out[..., j] for name, j in _VARIANT_METRICS[loss]}
-        return AnakinExperimentOutput(learner_state=learner_state, episode_metrics=ep_out, train_metrics=train_metrics)
+        return AnakinExperimentOutput(learner_state=learner_state._replace(timestep=timestep), episode_metrics=episode_metrics,
+                                      train_metrics=train_metrics)
 
     learner_fn.built = built  # exposed for tests / bench (trajectory buffers, graph handle)
     learner_fn.update_step = _update_step
     learner_fn.phases = {"rollout": _rollout_phase, "stats": _stats_phase, "gae": _gae_phase, "update": _update_phase}
-
-    def _ensure_built(st: OnPolicyLearnerState) -> None:
-        if not built:
-            _build(st)
-            for u in range(U):  # last_timestep.observation seeds the carry slot (row T)
-                built["shards"][u].env_obs[T].copy_(st.timestep[u].observation)
-
-    learner_fn.ensure_built = _ensure_built
+    learner_fn.ensure_built = lambda st: anakin.ensure_built(built, _build, st)
     return learner_fn
 
 
@@ -527,18 +450,11 @@ def build_learner(
     if precision == ops.STX_PREC_BF16:
         arena_bf16 = ops.cast_bf16(arena)
         actor_params.flat_bf16, critic_params.flat_bf16 = arena_bf16[:coff], arena_bf16[coff:]
-    actor_params.arena, actor_params.arena_bf16 = arena, arena_bf16
+    actor_params.arena_bf16 = arena_bf16
 
-    # Optimiser state: flat mu / nu arenas + device-resident counters (ScaleByAdamState, ScaleByScheduleState).
-    mu, nu = torch.zeros_like(arena), torch.zeros_like(arena)
-    counts = torch.zeros(4, dtype=torch.int32, device=device)
-    a_state = optax.OptState(counts[0:1], mu[: sa.param_count], nu[: sa.param_count], counts[1:2])
-    c_state = optax.OptState(counts[2:3], mu[coff : coff + sc.param_count], nu[coff : coff + sc.param_count], counts[3:4])
-    # the flat arenas every fused kernel works on ride along on the actor tree
-    actor_params.arena_mu, actor_params.arena_nu, actor_params.arena_counts = mu, nu, counts
-
+    # Optimiser state (ScaleByAdamState, ScaleByScheduleState per network); the flat arenas ride along on the actor tree.
     params = ActorCriticParams(actor_params, critic_params)
-    opt_states = ActorCriticOptStates(a_state, c_state)
+    opt_states = ActorCriticOptStates(*optax.arena_state(actor_params, arena, [(0, sa.param_count), (coff, sc.param_count)]))
 
     apply_fns = (actor_network.apply, critic_network.apply)
     update_fns = (actor_optim.update, critic_optim.update)
@@ -550,13 +466,8 @@ def build_learner(
     env_states, timesteps = anakin.reset_shards(env, shard_keys, config, rank)
 
     # Load model from checkpoint if specified (ff_ppo.py:504-512) -- params only, as in the reference.
-    if config.logger.checkpointing.load_model:
-        from stoix_b200.utils.checkpointing import Checkpointer
-
-        loaded = Checkpointer(model_name=config.system.system_name, **to_container(config.logger.checkpointing.load_args))
-        loaded.restore_params(arena)
-        if arena_bf16 is not None:
-            ops.cast_bf16(arena, out=arena_bf16)
+    if warm_start(config, arena) and arena_bf16 is not None:
+        ops.cast_bf16(arena, out=arena_bf16)
 
     # step keys: (sampling seed, shuffle seed) -- per-rank streams like the per-device keys at :515-518
     rollout_seed, shuffle_seed = anakin.rank_seeds(shard_keys[U], 2, rank, world)

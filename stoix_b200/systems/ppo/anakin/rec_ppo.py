@@ -27,11 +27,12 @@ from stoix_b200 import ops
 from stoix_b200 import optim as optax
 from stoix_b200 import random as srandom
 from stoix_b200.base_types import ActorCriticOptStates, ActorCriticParams, AnakinExperimentOutput
-from stoix_b200.config import DictConfig, instantiate, to_container
+from stoix_b200.config import DictConfig, instantiate
 from stoix_b200.envs.base import Environment, StepOut
 from stoix_b200.networks.recurrent import RecLayout, RecurrentActor, RecurrentCritic, ScannedRNN
 from stoix_b200.systems import anakin
 from stoix_b200.systems.ppo.ppo_types import ActorCriticHiddenStates, RNNLearnerState, RNNPPOTransition
+from stoix_b200.utils.checkpointing import warm_start
 from stoix_b200.utils.training import make_learning_rate
 
 _METRIC_NAMES = ("actor_loss", "entropy", "value_loss", "advantages", "pred_value", "target_value")
@@ -44,6 +45,7 @@ class _Shard:
     def __init__(self, T: int, E: int, D: int, H: int, device):   # H = carry width (2 x hidden for lstm)
         z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=device)
         self.obs = z(T + 1, E, D)                       # row t = last_timestep.observation of step t, row T = the carry
+        self.env_obs = self.obs                         # the rows anakin.learn seeds and carries
         self.done, self.trunc = z(T + 1, E, dt=torch.uint8), z(T + 1, E, dt=torch.uint8)   # flags BEFORE step t
         self.reset = z(T + 1, E, dt=torch.uint8)        # done | truncated
         self.action = z(T, E, dt=torch.int32)
@@ -92,7 +94,6 @@ def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], updat
     assert cols_total % nmb == 0, "num_envs * num_recurrent_chunks must be divisible by num_minibatches"
     C = cols_total // nmb
     gamma, lam = float(sysc.gamma), float(sysc.gae_lambda)
-    use_graph = bool(arch.get("cuda_graph", True))
     has_step_into = hasattr(env, "step_into")
     built: Dict[str, Any] = {}
 
@@ -103,10 +104,7 @@ def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], updat
         D, A, H = la.spec_pre.sizes[0], la.spec_post.sizes[-1], la.S   # H: carry width
         coff = _pad8(la.param_count)
         total = coff + _pad8(lc.param_count)
-        plan = ops.AdamPlan([(0, la.param_count, actor_opt.init_lr, actor_opt.max_grad_norm), (coff, lc.param_count, critic_opt.init_lr, critic_opt.max_grad_norm)],
-                            dev, b1=actor_opt.adam.b1, b2=actor_opt.adam.b2, eps=actor_opt.adam.eps, decay=bool(sysc.decay_learning_rates),
-                            steps_per_update=epochs * nmb, num_updates=int(arch.num_updates))
-        plan.counts = a_tree.arena_counts
+        plan = optax.adam_plan([(0, la.param_count, actor_opt), (coff, lc.param_count, critic_opt)], dev, a_tree.arena_counts)
         built.update(la=la, lc=lc, dev=dev, D=D, A=A, H=H, coff=coff, total=total, plan=plan, arena=a_tree.arena,
                      shards=[_Shard(T, E, D, H, dev) for _ in range(U)],
                      ws_a=_NetWs(la, chunk, C, A, dev), ws_c=_NetWs(lc, chunk, C, 1, dev),
@@ -117,6 +115,9 @@ def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], updat
                      side_stream=torch.cuda.Stream(device=dev), metrics_c=torch.zeros(8, dtype=torch.float32, device=dev),
                      graph=None, eager_done=False,
                      t_rows=(torch.arange(chunk, device=dev, dtype=torch.int64) * cols_total)[:, None])
+        for sh, done, trunc, h in zip(built["shards"], state.done, state.truncated, state.hstates):   # the carried flags and hidden states
+            sh.done[T].copy_(done), sh.trunc[T].copy_(trunc)
+            sh.h_a_cur.copy_(h.policy_hidden_state), sh.h_c_cur.copy_(h.critic_hidden_state)
 
     def _net_step(net, tree, h_cur: torch.Tensor, obs_t: torch.Tensor, reset_t: torch.Tensor):
         """One step of a recurrent network (rec_ppo.py:90-101): T = 1 sequence."""
@@ -238,38 +239,17 @@ def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], updat
         _update_phase(state)
 
     def learner_fn(learner_state: RNNLearnerState) -> AnakinExperimentOutput:
-        learner_fn.ensure_built(learner_state)
-        b = built
-        n_upd, dev = int(arch.num_updates_per_eval), b["dev"]
-        ep_out = {"episode_return": torch.empty(n_upd, U, T, E, device=dev), "episode_length": torch.empty(n_upd, U, T, E, dtype=torch.int32, device=dev),
-                  "is_terminal_step": torch.empty(n_upd, U, T, E, dtype=torch.bool, device=dev)}
-        train_out = torch.empty(n_upd, epochs, nmb, 8, device=dev)
-        for k in range(n_upd):
-            anakin.update_once(b, use_graph, _update_step, learner_state)   # one CUDA graph per update step: ~10k launches replayed
-            for u in range(U):
-                sh = b["shards"][u]
-                ep_out["episode_return"][k, u].copy_(sh.episode_return), ep_out["episode_length"][k, u].copy_(sh.episode_length)
-                ep_out["is_terminal_step"][k, u].copy_(sh.is_terminal_step)
-            train_out[k].copy_(b["metrics"])
-        sh0 = b["shards"]
+        # one CUDA graph per update step: ~10k launches replayed
+        timestep, episode_metrics, train_out = anakin.learn(built, _build, _update_step, learner_state, config)
+        shards = built["shards"]
         learner_state = learner_state._replace(
-            timestep=[learner_state.timestep[u]._replace(observation=sh0[u].obs[T]) for u in range(U)],
-            done=[sh0[u].done[T].bool() for u in range(U)], truncated=[sh0[u].trunc[T].bool() for u in range(U)],
-            hstates=[ActorCriticHiddenStates(sh0[u].h_a_cur, sh0[u].h_c_cur) for u in range(U)])
+            timestep=timestep, done=[sh.done[T].bool() for sh in shards], truncated=[sh.trunc[T].bool() for sh in shards],
+            hstates=[ActorCriticHiddenStates(sh.h_a_cur, sh.h_c_cur) for sh in shards])
         train_metrics = {name: train_out[..., j] for j, name in enumerate(_METRIC_NAMES)}
-        return AnakinExperimentOutput(learner_state=learner_state, episode_metrics=ep_out, train_metrics=train_metrics)
-
-    def _ensure_built(st: RNNLearnerState) -> None:
-        if not built:
-            _build(st)
-            for u in range(U):
-                sh = built["shards"][u]
-                sh.obs[T].copy_(st.timestep[u].observation)
-                sh.done[T].copy_(st.done[u]), sh.trunc[T].copy_(st.truncated[u])
-                sh.h_a_cur.copy_(st.hstates[u].policy_hidden_state), sh.h_c_cur.copy_(st.hstates[u].critic_hidden_state)
+        return AnakinExperimentOutput(learner_state=learner_state, episode_metrics=episode_metrics, train_metrics=train_metrics)
 
     learner_fn.built = built
-    learner_fn.ensure_built = _ensure_built
+    learner_fn.ensure_built = lambda st: anakin.ensure_built(built, _build, st)
     learner_fn.phases = {"rollout": _rollout_phase, "gae": _gae_phase, "update": _update_phase}
     learner_fn.update_step = _update_step
     learner_fn.geometry = {"chunk": chunk, "num_chunks": nc, "cols_per_minibatch": C}
@@ -310,28 +290,21 @@ def learner_setup(env: Environment, keys: Tuple[int, int, int], config: DictConf
     arena = torch.zeros(coff + _pad8(lc.param_count), dtype=torch.float32, device=device)
     actor_params = actor_network.init(actor_net_key, init_policy_hstate, init_x, flat=arena[:coff])
     critic_params = critic_network.init(critic_net_key, init_critic_hstate, init_x, flat=arena[coff:])
-    mu, nu = torch.zeros_like(arena), torch.zeros_like(arena)
-    counts = torch.zeros(4, dtype=torch.int32, device=device)
-    a_state = optax.OptState(counts[0:1], mu[: la.param_count], nu[: la.param_count], counts[1:2])
-    c_state = optax.OptState(counts[2:3], mu[coff: coff + lc.param_count], nu[coff: coff + lc.param_count], counts[3:4])
-    actor_params.arena, actor_params.arena_mu, actor_params.arena_nu, actor_params.arena_counts = arena, mu, nu, counts
+    opt_states = ActorCriticOptStates(*optax.arena_state(actor_params, arena, [(0, la.param_count), (coff, lc.param_count)]))
 
     apply_fns = (actor_network.apply, critic_network.apply)
     update_fns = (actor_optim.update, critic_optim.update)
     learn = get_learner_fn(env, apply_fns, update_fns, config)
 
     params = ActorCriticParams(actor_params, critic_params)
-    if config.logger.checkpointing.load_model:
-        from stoix_b200.utils.checkpointing import Checkpointer
-
-        Checkpointer(model_name=config.system.system_name, **to_container(config.logger.checkpointing.load_args)).restore_params(arena)
+    warm_start(config, arena)
 
     shard_keys = srandom.split(key, U + 1)
     env_states, timesteps = anakin.reset_shards(env, shard_keys, config, rank)
     dones = [torch.zeros(E, dtype=torch.bool, device=device) for _ in range(U)]
     truncs = [torch.zeros(E, dtype=torch.bool, device=device) for _ in range(U)]
     hstates = [ActorCriticHiddenStates(init_policy_hstate.clone(), init_critic_hstate.clone()) for _ in range(U)]
-    init_learner_state = RNNLearnerState(params, ActorCriticOptStates(a_state, c_state), anakin.rank_seeds(shard_keys[U], 2, rank, world),
+    init_learner_state = RNNLearnerState(params, opt_states, anakin.rank_seeds(shard_keys[U], 2, rank, world),
                                          env_states, timesteps, dones, truncs, hstates)
     return learn, actor_network, init_learner_state
 

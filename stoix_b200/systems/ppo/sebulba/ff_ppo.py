@@ -53,6 +53,7 @@ from stoix_b200.utils.sebulba_utils import (
     TimingTracker,
 )
 from stoix_b200.utils.total_timestep_checker import check_total_timesteps
+from stoix_b200.utils.checkpointing import warm_start
 from stoix_b200.utils.training import make_learning_rate
 
 _METRIC_NAMES = ("actor_loss", "entropy", "value_loss", "advantages", "pred_value", "target_value")
@@ -325,11 +326,7 @@ def get_learner_step_fn(apply_fns: Tuple[ActorApply, CriticApply], update_fns: T
         D = sa.sizes[0]
         z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=dev)
         obs_dt = torch.bfloat16 if precision == ops.STX_PREC_BF16 else torch.float32
-        plan = ops.AdamPlan([(0, sa.param_count, actor_opt.init_lr, actor_opt.max_grad_norm),
-                             (coff, sc.param_count, critic_opt.init_lr, critic_opt.max_grad_norm)], dev, b1=actor_opt.adam.b1,
-                            b2=actor_opt.adam.b2, eps=actor_opt.adam.eps, decay=bool(sysc.decay_learning_rates),
-                            steps_per_update=epochs * nmb, num_updates=int(arch.num_updates))
-        plan.counts = a_tree.arena_counts
+        plan = optax.adam_plan([(0, sa.param_count, actor_opt), (coff, sc.param_count, critic_opt)], dev, a_tree.arena_counts)
         built.update(sa=sa, sc=sc, dev=dev, D=D, total=total, plan=plan, arena=a_tree.arena, arena_bf16=getattr(a_tree, "arena_bf16", None),
                      obs=z(T + 1, E, D, dt=obs_dt), action=z(T + 1, E, dt=torch.int32), value=z(T + 1, E), log_prob=z(T + 1, E),
                      reward=z(T + 1, E), done=z(T + 1, E, dt=torch.uint8), truncated=z(T + 1, E, dt=torch.uint8),
@@ -541,23 +538,15 @@ def learner_setup(env_factory: cpu_envs.EnvFactory, keys: Tuple[int, int, int], 
         if precision == ops.STX_PREC_BF16:
             arena_bf16 = ops.cast_bf16(arena)
             actor_params.flat_bf16, critic_params.flat_bf16 = arena_bf16[:coff], arena_bf16[coff:]
-        actor_params.arena, actor_params.arena_bf16 = arena, arena_bf16
-        mu, nu = torch.zeros_like(arena), torch.zeros_like(arena)
-        counts = torch.zeros(4, dtype=torch.int32, device=device)
-    a_state = optax.OptState(counts[0:1], mu[: sa.param_count], nu[: sa.param_count], counts[1:2])
-    c_state = optax.OptState(counts[2:3], mu[coff:coff + sc.param_count], nu[coff:coff + sc.param_count], counts[3:4])
-    actor_params.arena_mu, actor_params.arena_nu, actor_params.arena_counts = mu, nu, counts
+        actor_params.arena_bf16 = arena_bf16
+        opt_states = ActorCriticOptStates(*optax.arena_state(actor_params, arena, [(0, sa.param_count), (coff, sc.param_count)]))
     params = ActorCriticParams(actor_params, critic_params)
     apply_fns = (actor_network.apply, critic_network.apply)
     update_fns = (actor_optim.update, critic_optim.update)
     learn_step = get_learner_step_fn(apply_fns, update_fns, config)
-    if config.logger.checkpointing.load_model:
-        from stoix_b200.utils.checkpointing import Checkpointer
-
-        Checkpointer(model_name=config.system.system_name, **to_container(config.logger.checkpointing.load_args)).restore_params(arena)
-        if arena_bf16 is not None:
-            ops.cast_bf16(arena, out=arena_bf16)
-    learner_state = CoreLearnerState(params, ActorCriticOptStates(a_state, c_state), int(key) & ((1 << 62) - 1))
+    if warm_start(config, arena) and arena_bf16 is not None:
+        ops.cast_bf16(arena, out=arena_bf16)
+    learner_state = CoreLearnerState(params, opt_states, int(key) & ((1 << 62) - 1))
     return learn_step, apply_fns, learner_state
 
 

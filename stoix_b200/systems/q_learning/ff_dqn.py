@@ -39,14 +39,15 @@ from stoix_b200 import ops
 from stoix_b200 import optim as optax
 from stoix_b200 import random as srandom
 from stoix_b200.base_types import AnakinExperimentOutput
-from stoix_b200.config import DictConfig, instantiate, to_container
-from stoix_b200.envs.base import Environment, StepOut, TimeStep
+from stoix_b200.config import DictConfig, instantiate
+from stoix_b200.envs.base import Environment
 from stoix_b200.networks.base import FeedForwardActor as Actor
 from stoix_b200.networks.base import build_param_tree
 from stoix_b200.networks.heads import DiscreteQNetworkHead
 from stoix_b200.systems import anakin
 from stoix_b200.systems.q_learning.dqn_types import Transition
 from stoix_b200.systems.sac.sac_types import OffPolicyLearnerState, OnlineAndTarget
+from stoix_b200.utils.checkpointing import warm_start
 from stoix_b200.utils.replay import DiscreteTransitionBuffer
 from stoix_b200.utils.training import make_learning_rate
 
@@ -76,27 +77,15 @@ def loss_hyper(loss: str, config: DictConfig):
     return ops.q_td_hyper(**kw)
 
 
-class _Rollout:
+class _Shard(anakin.Trajectory):
     """Trajectory buffers of one (device, update-batch) shard, time-major: the Transition fields (dqn_types.py) plus the Q rows."""
 
     def __init__(self, T: int, E: int, D: int, A: int, device):
+        super().__init__(T, E, D, device)
         z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=device)
-        self.obs = z(T + 1, E, D)               # row t = last_timestep.observation of step t; row T = the next rollout's first
-        self.next_obs = z(T, E, D)              # timestep.extras["next_obs"]
         self.q = z(T, E, A)                     # Q(online, obs[t]), the rows the sampler acted on
         self.action = z(T, E, dt=torch.int32)
-        self.reward = z(T, E)
-        self.terminated = z(T, E, dt=torch.uint8)
-        self.truncated = z(T, E, dt=torch.uint8)
         self.done = z(T, E, dt=torch.uint8)     # timestep.last() = terminated | truncated (ff_dqn.py:121)
-        self.episode_return = z(T, E)
-        self.episode_length = z(T, E, dt=torch.int32)
-        self.is_terminal_step = z(T, E, dt=torch.uint8)
-        self.T = T
-
-    def step_out(self, t: int) -> StepOut:
-        return StepOut(self.obs[t + 1], self.next_obs[t], self.reward[t], self.terminated[t], self.truncated[t], self.episode_return[t],
-                       self.episode_length[t], self.is_terminal_step[t])
 
     def transition(self) -> Transition:
         return Transition(self.obs[: self.T], self.action, self.reward, self.done, self.next_obs,
@@ -158,22 +147,8 @@ def batch_grads(loss: str, spec: ops.MlpSpec, online: torch.Tensor, target: torc
 def get_warmup_fn(env: Environment, q_params: OnlineAndTarget, q_apply_fn: Callable, buffer_add_fn: Callable, config: DictConfig) -> Callable:
     """ff_dqn.py:37-89: `warmup_steps` environment steps with the initial online parameters and the training epsilon, added to
     the buffer (one shard per call)."""
-    W = int(config.system.warmup_steps)
-
-    def warmup(env_state, timestep: TimeStep, buffer_state, key: int):
-        obs_l, act_l, rew_l, done_l, nobs_l = [], [], [], [], []
-        for t in range(W):
-            obs = timestep.observation.float().clone()
-            action = q_apply_fn(q_params.online, obs).sample(seed=key, offset=t)
-            env_state, timestep = env.step(env_state, action)
-            obs_l.append(obs), act_l.append(action.to(torch.int32)), rew_l.append(timestep.reward.float())
-            done_l.append(timestep.last().to(torch.uint8)), nobs_l.append(timestep.extras["next_obs"].float())
-        if W > 0:
-            st = lambda xs: torch.stack(xs).contiguous()
-            buffer_add_fn(buffer_state, Transition(st(obs_l), st(act_l), st(rew_l), st(done_l), st(nobs_l), {}))
-        return env_state, timestep, key, buffer_state
-
-    return warmup
+    draw = lambda obs, key, t: q_apply_fn(q_params.online, obs).sample(seed=key, offset=t).to(torch.int32)
+    return anakin.warmup_fn(env, draw, buffer_add_fn, config)
 
 
 def get_learner_fn(env: Environment, q_apply_fn: Callable, q_update_fn: Callable, buffer_fns: Tuple[Callable, Callable], config: DictConfig,
@@ -196,7 +171,6 @@ def get_learner_fn(env: Environment, q_apply_fn: Callable, q_update_fn: Callable
     tau = float(sysc.tau)
     hyper = loss_hyper(loss, config)
     sched = ops.epsilon_schedule_struct(float(sysc.training_epsilon), float(sysc.training_epsilon), 0.0, 1, decay=False)
-    use_graph = bool(arch.get("cuda_graph", True))
     built: Dict[str, Any] = {}
 
     def _build(state: OffPolicyLearnerState) -> None:
@@ -204,12 +178,10 @@ def get_learner_fn(env: Environment, q_apply_fn: Callable, q_update_fn: Callable
         spec = tree.spec
         dev = tree.flat.device
         D, A = spec.sizes[0], spec.sizes[-1]
-        lr_sched = opt.schedule
-        plan = ops.AdamPlan([(0, spec.param_count, opt.init_lr, opt.max_grad_norm)], dev, b1=opt.adam.b1, b2=opt.adam.b2, eps=opt.adam.eps,
-                            decay=lr_sched is not None, steps_per_update=getattr(lr_sched, "steps_per_update", 1),
-                            num_updates=getattr(lr_sched, "num_updates", 1), **opt.plan_kwargs())
-        plan.counts = tree.arena_counts   # the optimiser counters live in the learner state (so a checkpoint carries them)
-        built.update(spec=spec, dev=dev, plan=plan, rollouts=[_Rollout(T, E, D, A, dev) for _ in range(U)],
+        shards = [_Shard(T, E, D, A, dev) for _ in range(U)]
+        # "rollouts": the name this list had before it was "shards" like every other learner's; callers that read it keep working
+        built.update(spec=spec, dev=dev, plan=optax.adam_plan([(0, spec.param_count, opt)], dev, tree.arena_counts),
+                     shards=shards, rollouts=shards,
                      batches=[make_batch(M, D, dev) for _ in range(U)], work=make_work(spec, M, dev),
                      grads=torch.zeros(tree.arena.numel(), dtype=torch.float32, device=dev),
                      metrics=torch.zeros(epochs, dtype=torch.float32, device=dev),
@@ -221,7 +193,7 @@ def get_learner_fn(env: Environment, q_apply_fn: Callable, q_update_fn: Callable
         b = built
         online = state.params.online.flat
         for u in range(U):
-            ro: _Rollout = b["rollouts"][u]
+            ro: _Shard = b["shards"][u]
             for t in range(T):
                 ops.mlp_forward(b["spec"], online, ro.obs[t], out=ro.q[t], ws_key="dqn_rollout")
                 ops.epsilon_greedy(ro.q[t], sched, seed=state.key[0] + u, offset=t, dev_counter=b["roll_ctr"], out=ro.action[t])
@@ -241,22 +213,13 @@ def get_learner_fn(env: Environment, q_apply_fn: Callable, q_update_fn: Callable
         batch_grads(loss, b["spec"], online.flat, target.flat, b["batches"], hyper, b["grads"], metric, b["work"])
         if world > 1:   # pmean over "device": summed by NCCL here, scaled in the optimiser step
             dist.all_reduce(b["grads"], op=dist.ReduceOp.SUM)
-        ops.clip_adam_step(b["plan"], online.arena, b["grads"], state.opt_states.mu, state.opt_states.nu, grad_scale=1.0 / world)
+        ops.clip_adam_step(b["plan"], online.arena, b["grads"], online.arena_mu, online.arena_nu, grad_scale=1.0 / world)
         ops.polyak_update(target.arena, online.arena, tau)   # optax.incremental_update (:207-209)
-
-    def _carry_in_phase(state: OffPolicyLearnerState) -> None:
-        for ro in built["rollouts"]:
-            ro.obs[0].copy_(ro.obs[T])
-
-    def _advance_phase(state: OffPolicyLearnerState) -> None:
-        for u in range(U):
-            if hasattr(env, "advance"):
-                env.advance(state.env_state[u], T)
-        ops.counter_add(built["roll_ctr"], T)
 
     def _update_step(state: OffPolicyLearnerState) -> None:
         """A single update (ff_dqn.py:103-234), in place on the learner state."""
-        _carry_in_phase(state)
+        for sh in built["shards"]:
+            sh.carry_in()
         _rollout_phase(state)
         built["metrics"].zero_()
         for ep in range(epochs):
@@ -264,37 +227,18 @@ def get_learner_fn(env: Environment, q_apply_fn: Callable, q_update_fn: Callable
         if world > 1:
             dist.all_reduce(built["metrics"], op=dist.ReduceOp.SUM)
             built["metrics"].mul_(1.0 / world)
-        _advance_phase(state)
+        for sh, env_state in zip(built["shards"], state.env_state):
+            sh.advance(env, env_state)
+        ops.counter_add(built["roll_ctr"], T)
 
     def learner_fn(learner_state: OffPolicyLearnerState) -> AnakinExperimentOutput:
         """arch.num_updates_per_eval update steps (ff_dqn.py:236-256)."""
-        learner_fn.ensure_built(learner_state)
-        b = built
-        n_upd, dev = int(arch.num_updates_per_eval), b["dev"]
-        ep_out = {"episode_return": torch.empty(n_upd, U, T, E, device=dev),
-                  "episode_length": torch.empty(n_upd, U, T, E, dtype=torch.int32, device=dev),
-                  "is_terminal_step": torch.empty(n_upd, U, T, E, dtype=torch.bool, device=dev)}
-        train_out = torch.empty(n_upd, epochs, device=dev)
-        for k in range(n_upd):
-            anakin.update_once(b, use_graph, _update_step, learner_state, learner_state.buffer_state, T * E)
-            for u in range(U):
-                ro = b["rollouts"][u]
-                ep_out["episode_return"][k, u].copy_(ro.episode_return)
-                ep_out["episode_length"][k, u].copy_(ro.episode_length)
-                ep_out["is_terminal_step"][k, u].copy_(ro.is_terminal_step)
-            train_out[k].copy_(b["metrics"])
-        new_ts = [learner_state.timestep[u]._replace(observation=b["rollouts"][u].obs[T]) for u in range(U)]
-        learner_state = learner_state._replace(timestep=new_ts)
-        return AnakinExperimentOutput(learner_state=learner_state, episode_metrics=ep_out, train_metrics={"q_loss": train_out})
-
-    def _ensure_built(st: OffPolicyLearnerState) -> None:
-        if not built:
-            _build(st)
-            for u in range(U):
-                built["rollouts"][u].obs[T].copy_(st.timestep[u].observation)
+        timestep, episode_metrics, train_out = anakin.learn(built, _build, _update_step, learner_state, config, buffers=learner_state.buffer_state)
+        return AnakinExperimentOutput(learner_state=learner_state._replace(timestep=timestep), episode_metrics=episode_metrics,
+                                      train_metrics={"q_loss": train_out})
 
     learner_fn.built = built
-    learner_fn.ensure_built = _ensure_built
+    learner_fn.ensure_built = lambda st: anakin.ensure_built(built, _build, st)
     learner_fn.update_step = _update_step
     learner_fn.update_epoch = _update_epoch
     learner_fn.rollout_phase = _rollout_phase
@@ -326,17 +270,8 @@ def learner_setup(env: Environment, keys: Tuple[int, int], config: DictConfig, l
     spec = q_network.spec_for(init_x.shape[-1])
     arena = torch.zeros((spec.param_count + 7) // 8 * 8, dtype=torch.float32, device=device)
     online = q_network.init(q_net_key, init_x, flat=arena)
-    online.arena = arena
-    mu, nu = torch.zeros_like(arena), torch.zeros_like(arena)
-    counts = torch.zeros(2, dtype=torch.int32, device=device)   # {adam count, schedule count}, stepped in place by the learner
-    opt_states = optax.OptState(counts[0:1], mu, nu, counts[1:2])
-    online.arena_mu, online.arena_nu, online.arena_counts = mu, nu, counts
-
-    if config.logger.checkpointing.load_model:   # params only, as in the reference (:372-380)
-        from stoix_b200.utils.checkpointing import Checkpointer
-
-        loaded = Checkpointer(model_name=config.system.system_name, **to_container(config.logger.checkpointing.load_args))
-        loaded.restore_params(arena)
+    (opt_states,) = optax.arena_state(online, arena, [(0, spec.param_count)])
+    warm_start(config, arena)   # (:372-380)
     target_arena = arena.clone()
     target = build_param_tree(spec, target_arena, "action_head")
     target.arena = target_arena
@@ -344,13 +279,9 @@ def learner_setup(env: Environment, keys: Tuple[int, int], config: DictConfig, l
 
     # Replay buffer (:316-347): one ring per (device, update-batch shard)
     U = int(config.arch.update_batch_size)
-    assert int(config.system.total_buffer_size) % n_devices == 0, "The total buffer size should be divisible by the number of devices!"
-    assert int(config.system.total_batch_size) % n_devices == 0, "The total batch size should be divisible by the number of devices!"
-    config.system.buffer_size = int(config.system.total_buffer_size) // (n_devices * U)
-    config.system.batch_size = int(config.system.total_batch_size) // (n_devices * U)
     shard_keys = srandom.split(key, U + 2)
-    buffer_states = [DiscreteTransitionBuffer(config.system.buffer_size, config.system.batch_size, config.system.batch_size, init_x.shape[-1],
-                                              device, seed=srandom.split(shard_keys[U], n_devices * U)[rank * U + u]) for u in range(U)]
+    buffer_states = anakin.replay_buffers(config, shard_keys[U], rank, n_devices,
+                                          lambda size, batch, seed: DiscreteTransitionBuffer(size, batch, batch, init_x.shape[-1], device, seed=seed))
     buffer_fns = (DiscreteTransitionBuffer.add, DiscreteTransitionBuffer.sample_into)
 
     learn = get_learner_fn(env, q_network.apply, q_optim.update, buffer_fns, config, loss=loss)

@@ -38,11 +38,12 @@ from stoix_b200 import ops
 from stoix_b200 import optim as optax
 from stoix_b200 import random as srandom
 from stoix_b200.base_types import AnakinExperimentOutput, LearnerFn, OnPolicyLearnerState
-from stoix_b200.config import DictConfig, instantiate, to_container
-from stoix_b200.envs.base import Environment, StepOut
+from stoix_b200.config import DictConfig, instantiate
+from stoix_b200.envs.base import Environment
 from stoix_b200.networks.base import FeedForwardActor as Actor
 from stoix_b200.networks.heads import DiscreteQNetworkHead
 from stoix_b200.systems import anakin
+from stoix_b200.utils.checkpointing import warm_start
 from stoix_b200.utils.training import make_learning_rate
 
 
@@ -52,29 +53,18 @@ def _refuse_bf16(config: DictConfig) -> None:
                          "Categorical actor-critic only, not a Q network with its activation, LayerNorm and Q loss; use arch.precision=f32")
 
 
-class _Shard:
+class _Shard(anakin.Trajectory):
     """Trajectory buffers of one (device, update-batch) shard, time-major: the Transition fields (dqn_types.py:9-15) plus the Q rows."""
 
     def __init__(self, T: int, E: int, D: int, A: int, device):
+        super().__init__(T, E, D, device)
         z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=device)
-        self.obs = z(T + 1, E, D)                     # row t = last_timestep.observation of step t; row T = the next rollout's first
-        self.next_obs = z(T, E, D)                    # timestep.extras["next_obs"]
+        self.done = self.terminated                   # the targets use done | truncated = timestep.last() (ff_pqn.py:84)
         self.q = z(T + 1, E, A)                       # q[t] = Q(obs[t]) with the rollout's parameters
         self.action = z(T, E, dt=torch.int32)
-        self.reward = z(T, E)
-        self.done = z(T, E, dt=torch.uint8)           # terminated; the targets use done | truncated = timestep.last() (ff_pqn.py:84)
-        self.truncated = z(T, E, dt=torch.uint8)
-        self.episode_return = z(T, E)
-        self.episode_length = z(T, E, dt=torch.int32)
-        self.is_terminal_step = z(T, E, dt=torch.uint8)
         self.epsilon = z(T, E)                        # info["epsilon"], info["update_no"] (ff_pqn.py:85-86)
         self.update_no = z(T, E, dt=torch.int32)
         self.targets = z(T, E)
-        self.perms = None
-
-    def step_out(self, t: int) -> StepOut:
-        return StepOut(self.obs[t + 1], self.next_obs[t], self.reward[t], self.done[t], self.truncated[t], self.episode_return[t],
-                       self.episode_length[t], self.is_terminal_step[t])
 
 
 def minibatch_grads(spec: ops.MlpSpec, params: torch.Tensor, rows: List[Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]],
@@ -117,7 +107,6 @@ def get_learner_fn(
     B = T * E
     assert B % nmb == 0, "rollout_length * num_envs must be divisible by num_minibatches"
     mb = B // nmb
-    use_graph = bool(arch.get("cuda_graph", True))
     gamma, q_lambda, delta = float(sysc.gamma), float(sysc.q_lambda), float(sysc.huber_loss_parameter)
     sched = epsilon_schedule.device_schedule(epochs * nmb)
     built: Dict[str, Any] = {}
@@ -127,13 +116,8 @@ def get_learner_fn(
         spec = tree.spec
         dev = tree.flat.device
         D, A = spec.sizes[0], spec.sizes[-1]
-        lr_sched = opt.schedule
-        plan = ops.AdamPlan([(0, spec.param_count, opt.init_lr, opt.max_grad_norm)], dev, b1=opt.adam.b1, b2=opt.adam.b2, eps=opt.adam.eps,
-                            decay=lr_sched is not None, steps_per_update=getattr(lr_sched, "steps_per_update", 1),
-                            num_updates=getattr(lr_sched, "num_updates", 1), **opt.plan_kwargs())
-        plan.counts = tree.arena_counts  # the optimiser counters live in the learner state (so a checkpoint carries them)
         built.update(
-            spec=spec, dev=dev, plan=plan, shards=[_Shard(T, E, D, A, dev) for _ in range(U)],
+            spec=spec, dev=dev, plan=optax.adam_plan([(0, spec.param_count, opt)], dev, tree.arena_counts), shards=[_Shard(T, E, D, A, dev) for _ in range(U)],
             grads=torch.zeros(tree.arena.numel(), dtype=torch.float32, device=dev),
             metrics=torch.zeros(epochs, nmb, dtype=torch.float32, device=dev),
             ws=ops.mlp_train_workspace(spec, mb, dev),
@@ -165,13 +149,7 @@ def get_learner_fn(
 
     def _shuffle_phase(state: OnPolicyLearnerState) -> None:
         """SHUFFLE MINIBATCHES (ff_pqn.py:184-197): one keyed permutation per (shard, epoch), independent of the rollout."""
-        b = built
-        for u in range(U):
-            sh = b["shards"][u]
-            if sh.perms is None:
-                sh.perms = torch.zeros(epochs, B, dtype=torch.int32, device=b["dev"])
-            for ep in range(epochs):
-                ops.make_permutation(B, state.key[1] + u, ep, dev_counter=b["perm_ctr"], out=sh.perms[ep])
+        anakin.shuffle(built["shards"], epochs, state.key[1], built["perm_ctr"])
 
     def _update_phase(state: OnPolicyLearnerState, shuffled: bool = False) -> None:
         """UPDATE EPOCHS (ff_pqn.py:122-207)."""
@@ -181,7 +159,6 @@ def get_learner_fn(
         spec, tree = b["spec"], state.params
         D = spec.sizes[0]
         metrics, grads, ws, q_mb, dq_mb = b["metrics"], b["grads"], b["ws"], b["q_mb"], b["dq_mb"]
-        opt_state = state.opt_states
         metrics.zero_()
         for ep in range(epochs):
             for i in range(nmb):  # _update_minibatch (ff_pqn.py:127-180)
@@ -189,74 +166,37 @@ def get_learner_fn(
                 minibatch_grads(spec, tree.flat, rows, delta, grads, metrics[ep, i:i + 1], ws, q_mb, dq_mb)
                 if world > 1:  # pmean over "device": summed by NCCL here, scaled in the optimiser step
                     dist.all_reduce(grads, op=dist.ReduceOp.SUM)
-                ops.clip_adam_step(b["plan"], tree.arena, grads, opt_state.mu, opt_state.nu, grad_scale=1.0 / world)
+                ops.clip_adam_step(b["plan"], tree.arena, grads, tree.arena_mu, tree.arena_nu, grad_scale=1.0 / world)
         if world > 1:
             dist.all_reduce(metrics, op=dist.ReduceOp.SUM)
             metrics.mul_(1.0 / world)
 
-    def _carry_in_phase(state: OnPolicyLearnerState) -> None:
-        for u in range(U):
-            sh = built["shards"][u]
-            sh.obs[0].copy_(sh.obs[T])
-
-    def _advance_phase(state: OnPolicyLearnerState) -> None:
-        b = built
-        for u in range(U):
-            if hasattr(env, "advance"):
-                env.advance(state.env_state[u], T)
-        ops.counter_add(b["roll_ctr"], T)
-        ops.counter_add(b["perm_ctr"], epochs)
+    def _rollout_targets(state: OnPolicyLearnerState) -> None:
+        _rollout_phase(state)
+        _targets_phase(state)
 
     def _update_step(state: OnPolicyLearnerState) -> None:
         """A single update (ff_pqn.py:50-210), in place on the learner state; the shuffles run on a side stream under the rollout."""
-        _carry_in_phase(state)
-        main = torch.cuda.current_stream()
-        side = built["side_stream"]
-        side.wait_stream(main)
-        with torch.cuda.stream(side):
-            _shuffle_phase(state)
-        _rollout_phase(state)
-        _targets_phase(state)
-        main.wait_stream(side)
+        b = built
+        for sh in b["shards"]:
+            sh.carry_in()
+        anakin.shuffle_beside(b, epochs, state.key[1], lambda: _rollout_targets(state))
         _update_phase(state, shuffled=True)
-        _advance_phase(state)
+        for sh, env_state in zip(b["shards"], state.env_state):
+            sh.advance(env, env_state)
+        ops.counter_add(b["roll_ctr"], T)
+        ops.counter_add(b["perm_ctr"], epochs)
 
     def learner_fn(learner_state: OnPolicyLearnerState) -> AnakinExperimentOutput[OnPolicyLearnerState]:
         """Run arch.num_updates_per_eval update steps (ff_pqn.py:212-226)."""
-        learner_fn.ensure_built(learner_state)
-        b = built
-        n_upd = int(arch.num_updates_per_eval)
-        dev = b["dev"]
-        ep_out = {
-            "episode_return": torch.empty(n_upd, U, T, E, device=dev),
-            "episode_length": torch.empty(n_upd, U, T, E, dtype=torch.int32, device=dev),
-            "is_terminal_step": torch.empty(n_upd, U, T, E, dtype=torch.bool, device=dev),
-            "epsilon": torch.empty(n_upd, U, T, E, device=dev),
-            "update_no": torch.empty(n_upd, U, T, E, dtype=torch.int32, device=dev),
-        }
-        train_out = torch.empty(n_upd, epochs, nmb, device=dev)
-        for k in range(n_upd):
-            anakin.update_once(b, use_graph, _update_step, learner_state)
-            for u in range(U):
-                sh = b["shards"][u]
-                for name in ("episode_return", "episode_length", "is_terminal_step", "epsilon", "update_no"):
-                    ep_out[name][k, u].copy_(getattr(sh, name))
-            train_out[k].copy_(b["metrics"])
-        new_ts = [learner_state.timestep[u]._replace(observation=b["shards"][u].obs[T]) for u in range(U)]
-        learner_state = learner_state._replace(timestep=new_ts)
-        return AnakinExperimentOutput(learner_state=learner_state, episode_metrics=ep_out, train_metrics={"q_loss": train_out})
+        timestep, episode_metrics, train_out = anakin.learn(built, _build, _update_step, learner_state, config, extra_fields=("epsilon", "update_no"))
+        return AnakinExperimentOutput(learner_state=learner_state._replace(timestep=timestep), episode_metrics=episode_metrics,
+                                      train_metrics={"q_loss": train_out})
 
     learner_fn.built = built
     learner_fn.update_step = _update_step
     learner_fn.phases = {"rollout": _rollout_phase, "targets": _targets_phase, "shuffle": _shuffle_phase, "update": _update_phase}
-
-    def _ensure_built(st: OnPolicyLearnerState) -> None:
-        if not built:
-            _build(st)
-            for u in range(U):
-                built["shards"][u].obs[T].copy_(st.timestep[u].observation)
-
-    learner_fn.ensure_built = _ensure_built
+    learner_fn.ensure_built = lambda st: anakin.ensure_built(built, _build, st)
     return learner_fn
 
 
@@ -310,11 +250,7 @@ def learner_setup(env: Environment, keys: Tuple[int, int], config: DictConfig) -
     spec = q_network.spec_for(init_x.shape[-1])
     arena = torch.zeros((spec.param_count + 7) // 8 * 8, dtype=torch.float32, device=device)
     params = q_network.init(q_net_key, init_x, flat=arena)
-    params.arena = arena
-    mu, nu = torch.zeros_like(arena), torch.zeros_like(arena)
-    counts = torch.zeros(2, dtype=torch.int32, device=device)   # {radam count, schedule count}, stepped in place by the learner
-    opt_states = optax.OptState(counts[0:1], mu, nu, counts[1:2])
-    params.arena_mu, params.arena_nu, params.arena_counts = mu, nu, counts
+    (opt_states,) = optax.arena_state(params, arena, [(0, spec.param_count)])
     if config.system.decay_epsilon:
         epsilon_schedule = linear_schedule(1.0, float(config.system.training_epsilon),
                                            float(config.arch.num_updates) * float(config.system.exploration_fraction))
@@ -327,11 +263,7 @@ def learner_setup(env: Environment, keys: Tuple[int, int], config: DictConfig) -
     shard_keys = srandom.split(key, U + 1)
     env_states, timesteps = anakin.reset_shards(env, shard_keys, config, rank)
 
-    if config.logger.checkpointing.load_model:
-        from stoix_b200.utils.checkpointing import Checkpointer
-
-        loaded = Checkpointer(model_name=config.system.system_name, **to_container(config.logger.checkpointing.load_args))
-        loaded.restore_params(arena)
+    warm_start(config, arena)
 
     rollout_seed, shuffle_seed = anakin.rank_seeds(shard_keys[U], 2, rank, world)
     init_learner_state = OnPolicyLearnerState(params=params, opt_states=opt_states, key=(rollout_seed, shuffle_seed), env_state=env_states,

@@ -28,12 +28,13 @@ from stoix_b200 import ops
 from stoix_b200 import optim as optax
 from stoix_b200 import random as srandom
 from stoix_b200.base_types import AnakinExperimentOutput
-from stoix_b200.config import DictConfig, instantiate, to_container
-from stoix_b200.envs.base import Environment, TimeStep
+from stoix_b200.config import DictConfig, instantiate
+from stoix_b200.envs.base import Environment
 from stoix_b200.networks.base import FeedForwardActor as Actor
 from stoix_b200.networks.base import FeedForwardQ, MultiNetwork, build_param_tree
 from stoix_b200.systems import anakin
 from stoix_b200.systems.sac.sac_types import OffPolicyLearnerState, OnlineAndTarget, SACOptStates, SACParams, Transition
+from stoix_b200.utils.checkpointing import warm_start
 from stoix_b200.utils.replay import TransitionBuffer
 from stoix_b200.utils.training import make_learning_rate
 
@@ -50,16 +51,14 @@ def sac_arena_layout(actor: ops.MlpSpec, q: ops.MlpSpec) -> Dict[str, int]:
     return {"actor": 0, "q1": off_q1, "q2": off_q2, "alpha": off_alpha, "total": off_alpha + 8, "q_block": off_alpha - off_q1}
 
 
-class _Shard:
+class _Shard(anakin.Trajectory):
     """Per (device, update-batch) shard: rollout trajectory (Transition fields, time-major), replay buffer, epoch workspaces."""
 
     def __init__(self, T: int, E: int, B: int, D: int, A: int, sa: ops.MlpSpec, sq: ops.MlpSpec, buffer: TransitionBuffer, device):
+        super().__init__(T, E, D, device)
         z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=device)
-        self.obs, self.next_obs, self.action = z(T, E, D), z(T, E, D), z(T, E, A)
-        self.reward, self.done = z(T, E), z(T, E, dt=torch.uint8)
-        self.episode_return, self.episode_length = z(T, E), z(T, E, dt=torch.int32)
-        self.is_terminal_step = z(T, E, dt=torch.bool)
-        self.cur_obs = z(E, D)                      # last_timestep.observation
+        self.action = z(T, E, A)
+        self.done = z(T, E, dt=torch.uint8)         # timestep.last() = terminated | truncated
         self.buffer = buffer
         # one sampled batch as the three network inputs (obs | action), leading dimension D + A
         self.xq_old, self.xq_new, self.xq_next = z(B, D + A), z(B, D + A), z(B, D + A)
@@ -74,34 +73,14 @@ class _Shard:
         self.d_in = [z(B, D + A) for _ in range(2)]
 
     def transition(self) -> Transition:
-        return Transition(self.obs, self.action, self.reward, self.done, self.next_obs,
+        return Transition(self.obs[: self.T], self.action, self.reward, self.done, self.next_obs,
                           {"episode_return": self.episode_return, "episode_length": self.episode_length, "is_terminal_step": self.is_terminal_step})
-
-
-def _policy_step(env: Environment, actor_apply_fn, actor_params, env_state, obs: torch.Tensor, seed: int, offset: int, counter):
-    """SELECT ACTION + STEP ENVIRONMENT (ff_sac.py:56-75 / 121-140)."""
-    action = actor_apply_fn(actor_params, obs).sample(seed=seed, offset=offset, dev_counter=counter)
-    env_state, timestep = env.step(env_state, action)
-    return env_state, timestep, action
 
 
 def get_warmup_fn(env: Environment, params: SACParams, actor_apply_fn: Callable, buffer_add_fn: Callable, config: DictConfig) -> Callable:
     """ff_sac.py:40-92: `warmup_steps` environment steps with the initial policy, added to the buffer (one shard per call)."""
-    W = int(config.system.warmup_steps)
-
-    def warmup(env_state, timestep: TimeStep, buffer_state, key: int):
-        obs_l, act_l, rew_l, done_l, nobs_l = [], [], [], [], []
-        for t in range(W):
-            obs = timestep.observation.float()
-            env_state, timestep, action = _policy_step(env, actor_apply_fn, params.actor_params, env_state, obs, key, t, None)
-            obs_l.append(obs.clone()), act_l.append(action), rew_l.append(timestep.reward.float())
-            done_l.append(timestep.last().to(torch.uint8)), nobs_l.append(timestep.extras["next_obs"].float())
-        if W > 0:
-            st = lambda xs: torch.stack(xs).contiguous()
-            buffer_add_fn(buffer_state, Transition(st(obs_l), st(act_l), st(rew_l), st(done_l), st(nobs_l), {}))
-        return env_state, timestep, key, buffer_state
-
-    return warmup
+    draw = lambda obs, key, t: actor_apply_fn(params.actor_params, obs).sample(seed=key, offset=t, dev_counter=None)
+    return anakin.warmup_fn(env, draw, buffer_add_fn, config)
 
 
 def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], update_fns: Tuple[Callable, Callable, Callable],
@@ -122,7 +101,6 @@ def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], updat
     target_entropy = float(sysc.target_entropy)
     lo, hi = float(sysc.action_minimum), float(sysc.action_maximum)
     min_scale = float(actor_net.action_head.min_scale)
-    use_graph = bool(arch.get("cuda_graph", True))
     built: Dict[str, Any] = {}
 
     def _build(state: OffPolicyLearnerState) -> None:
@@ -131,13 +109,8 @@ def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], updat
         dev = a_tree.flat.device
         lay = sac_arena_layout(sa, sq)
         D, A = sa.sizes[0], sa.sizes[-1] // 2
-        segs = [(lay["actor"], sa.param_count, actor_opt.init_lr, actor_opt.max_grad_norm),
-                (lay["q1"], lay["q_block"], q_opt.init_lr, q_opt.max_grad_norm)]
-        if autotune:
-            segs.append((lay["alpha"], 1, alpha_opt.init_lr, alpha_opt.max_grad_norm))
-        plan = ops.AdamPlan(segs, dev, b1=actor_opt.adam.b1, b2=actor_opt.adam.b2, eps=actor_opt.adam.eps,
-                            decay=bool(sysc.decay_learning_rates), steps_per_update=epochs, num_updates=int(arch.num_updates))
-        plan.counts = a_tree.arena_counts[: 2 * len(segs)]   # optimiser counters live in the learner state
+        segs = [(lay["actor"], sa.param_count, actor_opt), (lay["q1"], lay["q_block"], q_opt)] + ([(lay["alpha"], 1, alpha_opt)] if autotune else [])
+        plan = optax.adam_plan(segs, dev, a_tree.arena_counts[: 2 * len(segs)])
         shards = [_Shard(T, E, B, D, A, sa, sq, state.buffer_state[u], dev) for u in range(U)]
         built.update(sa=sa, sq=sq, dev=dev, lay=lay, D=D, A=A, plan=plan, shards=shards, arena=a_tree.arena, target=a_tree.target_arena,
                      grads=torch.zeros(lay["total"], dtype=torch.float32, device=dev),
@@ -152,20 +125,12 @@ def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], updat
         act_seed = state.key[0]
         for u in range(U):
             sh = b["shards"][u]
-            for t in range(T):
-                sh.obs[t].copy_(sh.cur_obs)
-                env_state, ts, action = _policy_step(env, actor_apply_fn, state.params.actor_params, state.env_state[u], sh.obs[t],
-                                                     act_seed + 0x9E37 * u, t, b["act_ctr"])
-                state.env_state[u] = env_state
-                sh.action[t].copy_(action)
-                sh.reward[t].copy_(ts.reward)
-                sh.done[t].copy_(ts.last())
-                sh.next_obs[t].copy_(ts.extras["next_obs"])
-                info = ts.extras["episode_metrics"]
-                sh.episode_return[t].copy_(info["episode_return"])
-                sh.episode_length[t].copy_(info["episode_length"])
-                sh.is_terminal_step[t].copy_(info["is_terminal_step"])
-                sh.cur_obs.copy_(ts.observation)
+            for t in range(T):   # SELECT ACTION (the policy's sample, written in place) + STEP ENVIRONMENT (:121-140)
+                pi = actor_apply_fn(state.params.actor_params, sh.obs[t])
+                ops.tanh_normal_sample(pi.head_out, pi.minimum, pi.maximum, pi.min_scale, seed=act_seed + 0x9E37 * u, offset=t,
+                                       dev_counter=b["act_ctr"], action_out=sh.action[t], want_eps=False)
+                anakin.step_env(env, state.env_state, u, sh.action[t], sh.step_out(t), t)
+            torch.bitwise_or(sh.terminated, sh.truncated, out=sh.done)
             buffer_add_fn(sh.buffer, sh.transition())
         ops.counter_add(b["act_ctr"], T)
 
@@ -234,40 +199,23 @@ def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], updat
         ops.polyak_update(b["target"], b["arena"][lay["q1"]: lay["alpha"]], tau)   # optax.incremental_update (:296-299)
 
     def _update_step(state: OffPolicyLearnerState) -> None:
+        for sh in built["shards"]:
+            sh.carry_in()
         _rollout_phase(state)
         for ep in range(epochs):
             _update_epoch(state, ep)
+        for sh, env_state in zip(built["shards"], state.env_state):
+            sh.advance(env, env_state)
 
     def learner_fn(learner_state: OffPolicyLearnerState) -> AnakinExperimentOutput:
         """arch.num_updates_per_eval update steps (ff_sac.py:330-344)."""
-        learner_fn.ensure_built(learner_state)
-        b = built
-        n_upd, dev = int(arch.num_updates_per_eval), b["dev"]
-        ep_out = {"episode_return": torch.empty(n_upd, U, T, E, device=dev),
-                  "episode_length": torch.empty(n_upd, U, T, E, dtype=torch.int32, device=dev),
-                  "is_terminal_step": torch.empty(n_upd, U, T, E, dtype=torch.bool, device=dev)}
-        train_out = torch.empty(n_upd, epochs, 8, device=dev)
-        for k in range(n_upd):
-            anakin.update_once(b, use_graph, _update_step, learner_state, [sh.buffer for sh in b["shards"]], T * E)
-            for u in range(U):
-                sh = b["shards"][u]
-                ep_out["episode_return"][k, u].copy_(sh.episode_return)
-                ep_out["episode_length"][k, u].copy_(sh.episode_length)
-                ep_out["is_terminal_step"][k, u].copy_(sh.is_terminal_step)
-            train_out[k].copy_(b["metrics"])
-        new_ts = [learner_state.timestep[u]._replace(observation=b["shards"][u].cur_obs) for u in range(U)]
-        learner_state = learner_state._replace(timestep=new_ts)
+        timestep, episode_metrics, train_out = anakin.learn(built, _build, _update_step, learner_state, config, buffers=learner_state.buffer_state)
         train_metrics = {name: train_out[..., j] for j, name in enumerate(_METRIC_NAMES)}
-        return AnakinExperimentOutput(learner_state=learner_state, episode_metrics=ep_out, train_metrics=train_metrics)
-
-    def _ensure_built(st: OffPolicyLearnerState) -> None:
-        if not built:
-            _build(st)
-            for u in range(U):
-                built["shards"][u].cur_obs.copy_(st.timestep[u].observation)
+        return AnakinExperimentOutput(learner_state=learner_state._replace(timestep=timestep), episode_metrics=episode_metrics,
+                                      train_metrics=train_metrics)
 
     learner_fn.built = built
-    learner_fn.ensure_built = _ensure_built
+    learner_fn.ensure_built = lambda st: anakin.ensure_built(built, _build, st)
     learner_fn.update_step = _update_step
     learner_fn.update_epoch = _update_epoch
     learner_fn.rollout_phase = _rollout_phase
@@ -329,11 +277,8 @@ def learner_setup(env: Environment, keys: Tuple[int, int, int], config: DictConf
         log_alpha.fill_(math.log(float(config.system.init_alpha)))
     config.system.target_entropy = target_entropy
 
-    mu, nu = torch.zeros_like(arena), torch.zeros_like(arena)
-    counts = torch.zeros(6, dtype=torch.int32, device=device)
-    seg = lambda off, n, i: optax.OptState(counts[2 * i: 2 * i + 1], mu[off: off + n], nu[off: off + n], counts[2 * i + 1: 2 * i + 2])
-    opt_states = SACOptStates(seg(lay["actor"], sa.param_count, 0), seg(lay["q1"], lay["q_block"], 1), seg(lay["alpha"], 1, 2))
-    actor_params.arena, actor_params.arena_mu, actor_params.arena_nu, actor_params.arena_counts = arena, mu, nu, counts
+    # three optimiser states, the alpha one stepped only with autotune
+    opt_states = SACOptStates(*optax.arena_state(actor_params, arena, [(lay["actor"], sa.param_count), (lay["q1"], lay["q_block"]), (lay["alpha"], 1)]))
     actor_params.target_arena = target_arena
     params = SACParams(actor_params, OnlineAndTarget(online_q_params, target_q_params), log_alpha)
 
@@ -342,13 +287,9 @@ def learner_setup(env: Environment, keys: Tuple[int, int, int], config: DictConf
 
     # Replay buffer (:429-456): one ring per (device, update-batch shard)
     U = int(config.arch.update_batch_size)
-    assert int(config.system.total_buffer_size) % n_devices == 0, "The total buffer size should be divisible by the number of devices!"
-    assert int(config.system.total_batch_size) % n_devices == 0, "The total batch size should be divisible by the number of devices!"
-    config.system.buffer_size = int(config.system.total_buffer_size) // (n_devices * U)
-    config.system.batch_size = int(config.system.total_batch_size) // (n_devices * U)
     shard_keys = srandom.split(key, U + 2)
-    buffer_states = [TransitionBuffer(config.system.buffer_size, config.system.batch_size, config.system.batch_size, init_x.shape[-1], action_dim,
-                                      device, seed=srandom.split(shard_keys[U], n_devices * U)[rank * U + u]) for u in range(U)]
+    buffer_states = anakin.replay_buffers(config, shard_keys[U], rank, n_devices,
+                                          lambda size, batch, seed: TransitionBuffer(size, batch, batch, init_x.shape[-1], action_dim, device, seed=seed))
     buffer_fns = (TransitionBuffer.add, TransitionBuffer.sample_into)
 
     learn = get_learner_fn(env, apply_fns, update_fns, buffer_fns, config)
@@ -357,11 +298,7 @@ def learner_setup(env: Environment, keys: Tuple[int, int, int], config: DictConf
     # Initialise environment states and timesteps across update-batch shards (:463-474).
     env_states, timesteps = anakin.reset_shards(env, shard_keys, config, rank)
 
-    if config.logger.checkpointing.load_model:   # params only, as in the reference (:477-486)
-        from stoix_b200.utils.checkpointing import Checkpointer
-
-        loaded = Checkpointer(model_name=config.system.system_name, **to_container(config.logger.checkpointing.load_args))
-        loaded.restore_params(arena)
+    if warm_start(config, arena):   # (:477-486)
         target_arena.copy_(arena[lay["q1"]: lay["alpha"]])
 
     # per-rank streams: (rollout policy noise, loss noise); warm-up noise on its own key (:489-496)

@@ -10,6 +10,8 @@ from typing import Any, Dict, Optional
 
 import torch
 
+from stoix_b200.config import to_container
+
 
 class Checkpointer:
     def __init__(self, model_name: str, metadata: Optional[Dict] = None, rel_dir: str = "checkpoints",
@@ -56,3 +58,13 @@ class Checkpointer:
         blob = torch.load(path, map_location="cpu")
         arena.copy_(blob["params"])
         return arena
+
+
+def warm_start(config, arena: torch.Tensor) -> bool:
+    """Warm start: with logger.checkpointing.load_model set, load the parameters of the checkpoint logger.checkpointing.load_args
+    names into `arena` (parameters only, as the reference restores them).  Returns whether it loaded; the caller then refreshes
+    whatever is derived from the arena (a bf16 shadow, target networks)."""
+    if not config.logger.checkpointing.load_model:
+        return False
+    Checkpointer(model_name=config.system.system_name, **to_container(config.logger.checkpointing.load_args)).restore_params(arena)
+    return True

@@ -205,3 +205,142 @@ def test_rank_seeds_split_per_rank_and_mask_62_bits(n, world_size):
         assert seeds == tuple(step_key[n * rank + i] & ((1 << 62) - 1) for i in range(n))
         assert all(0 <= s < (1 << 62) for s in seeds)
     assert len({s for r in range(world_size) for s in anakin.rank_seeds(key, n, r, world_size)}) == n * world_size
+
+
+def _compose(name, overrides=()):
+    from stoix_b200.config import compose
+
+    return compose(name, list(overrides), config_dir="default/anakin")
+
+
+def test_learn_builds_once_seeds_the_carry_and_collects_every_update():
+    from stoix_b200.envs.base import TimeStep
+
+    T, E, D, U, n_upd = 3, 2, 4, 2, 3
+    config = _compose("default_ff_pqn", ["arch.cuda_graph=False"])
+    config.arch.num_updates_per_eval = n_upd
+    built, rec = {}, {"builds": 0, "calls": 0, "first_rows": {}}
+
+    def build(state):
+        rec["builds"] += 1
+        shards = [anakin.Trajectory(T, E, D, "cpu") for _ in range(U)]
+        for sh in shards:
+            sh.epsilon = torch.zeros(T, E)
+        built.update(shards=shards, metrics=torch.zeros(2, 5), graph=None, eager_done=False)
+
+    def step(state):
+        k = rec["calls"]
+        rec["calls"] += 1
+        for u, sh in enumerate(built["shards"]):
+            sh.carry_in()
+            if k == 0:
+                rec["first_rows"][u] = sh.obs[0].clone()
+            v = 100 * k + 10 * u
+            sh.obs[1:].fill_(v)
+            sh.episode_return.fill_(v + 1)
+            sh.episode_length.fill_(v + 2)
+            sh.is_terminal_step.fill_((k + u) % 2)
+            sh.epsilon.fill_(v + 3)
+        built["metrics"].fill_(k)
+
+    state = SimpleNamespace(timestep=[TimeStep(None, None, None, torch.full((E, D), -1.0 - u), {}) for u in range(U)])
+    timestep, ep, train = anakin.learn(built, build, step, state, config, extra_fields=("epsilon",))
+    assert rec["builds"] == 1 and built["eager_done"] and built["graph"] is None
+    # the carry row T starts from the learner state's observation and is the first row of the first rollout
+    assert all(torch.equal(rec["first_rows"][u], torch.full((E, D), -1.0 - u)) for u in range(U))
+    assert set(ep) == {"episode_return", "episode_length", "is_terminal_step", "epsilon"}
+    assert {k: (tuple(v.shape), v.dtype) for k, v in ep.items()} == {
+        "episode_return": ((n_upd, U, T, E), torch.float32), "episode_length": ((n_upd, U, T, E), torch.int32),
+        "is_terminal_step": ((n_upd, U, T, E), torch.bool), "epsilon": ((n_upd, U, T, E), torch.float32)}
+    for k in range(n_upd):
+        for u in range(U):
+            v = 100 * k + 10 * u
+            assert (ep["episode_return"][k, u] == v + 1).all() and (ep["episode_length"][k, u] == v + 2).all()
+            assert (ep["is_terminal_step"][k, u] == bool((k + u) % 2)).all() and (ep["epsilon"][k, u] == v + 3).all()
+    assert train.shape == (n_upd, 2, 5) and [float(train[k].unique()) for k in range(n_upd)] == [0.0, 1.0, 2.0]
+    # the next learn() starts from row T of the last rollout
+    for u, ts in enumerate(timestep):
+        assert ts.observation.data_ptr() == built["shards"][u].obs[T].data_ptr() and (ts.observation == 100 * (n_upd - 1) + 10 * u).all()
+    # a second call reuses the buffers and carries on from that row
+    anakin.learn(built, build, step, SimpleNamespace(timestep=timestep), config)
+    assert rec["builds"] == 1 and rec["calls"] == 2 * n_upd
+
+
+@pytest.mark.parametrize("segments", [[(0, 5)], [(0, 5), (8, 7)], [(0, 5), (8, 16), (24, 1)]])
+def test_arena_state_views_and_counts_layout(segments):
+    from stoix_b200 import optim
+
+    arena = torch.arange(32, dtype=torch.float32)
+    tree = SimpleNamespace()
+    states = optim.arena_state(tree, arena, segments)
+    assert tree.arena is arena and len(states) == len(segments)
+    for name in ("arena_mu", "arena_nu"):
+        t = getattr(tree, name)
+        assert t.shape == arena.shape and t.dtype == torch.float32 and not t.any() and t.data_ptr() != arena.data_ptr()
+    counts = tree.arena_counts
+    assert counts.dtype == torch.int32 and counts.tolist() == [0] * (2 * len(segments))
+    for i, ((off, n), st) in enumerate(zip(segments, states)):
+        # {count, schedule count} of segment i are counts[2i], counts[2i + 1]; mu / nu are views of the arenas
+        assert st.count.data_ptr() == counts[2 * i:].data_ptr() and st.count.shape == (1,)
+        assert st.sched_count.data_ptr() == counts[2 * i + 1:].data_ptr() and st.sched_count.shape == (1,)
+        assert st.mu.data_ptr() == tree.arena_mu[off:].data_ptr() and st.mu.shape == (n,)
+        assert st.nu.data_ptr() == tree.arena_nu[off:].data_ptr() and st.nu.shape == (n,)
+
+
+def test_replay_buffers_split_the_totals_and_seed_each_shard():
+    key = srandom.PRNGKey(11)
+    config = _compose("default_ff_dqn", ["arch.update_batch_size=2", "system.total_buffer_size=1200", "system.total_batch_size=96"])
+    made = anakin.replay_buffers(config, key, 1, 3, lambda size, batch, seed: (size, batch, seed))
+    assert (config.system.buffer_size, config.system.batch_size) == (200, 16)
+    # seed of shard u on rank r: split(key, n_devices * U)[r * U + u]
+    assert made == [(200, 16, 7285328837743276888), (200, 16, 14567865290730263530)]
+    assert [m[2] for m in made] == srandom.split(key, 6)[2:4]
+    for bad in (["system.total_buffer_size=1201"], ["system.total_batch_size=97"]):
+        with pytest.raises(AssertionError):
+            anakin.replay_buffers(_compose("default_ff_dqn", bad), key, 0, 3, lambda *a: a)
+
+
+class _Plan:
+    def __init__(self, segments, device, **kwargs):
+        self.segments, self.device, self.kwargs, self.counts = segments, device, kwargs, None
+
+
+@pytest.mark.parametrize("decay", [True, False])
+@pytest.mark.parametrize("system", ["ff_ppo", "rec_ppo", "ff_sac"])
+def test_adam_plan_takes_decay_and_its_constants_from_the_schedule(monkeypatch, system, decay):
+    """The plan arguments PPO, rec_ppo and SAC passed before: decay = system.decay_learning_rates, steps_per_update = epochs *
+    num_minibatches (epochs for SAC), num_updates = arch.num_updates.  Without decay the kernel reads neither constant."""
+    from stoix_b200 import ops
+    from stoix_b200 import optim as optax
+    from stoix_b200.utils.training import make_learning_rate
+
+    monkeypatch.setattr(ops, "AdamPlan", _Plan)
+    config = _compose(f"default_{system}", [f"system.decay_learning_rates={decay}", "system.epochs=3"])
+    config.arch.num_updates = 70
+    nmb = int(config.system.get("num_minibatches", 1))
+    lrs = (config.system.actor_lr, config.system.q_lr, config.system.alpha_lr) if system == "ff_sac" else (config.system.actor_lr, config.system.critic_lr)
+    opts = [optax.chain(optax.clip_by_global_norm(config.system.max_grad_norm),
+                        optax.adam(make_learning_rate(lr, config, 3, None if system == "ff_sac" else nmb), eps=1e-5)) for lr in lrs]
+    counts = torch.zeros(2 * len(opts), dtype=torch.int32)
+    plan = optax.adam_plan([(8 * i, 5 + i, o) for i, o in enumerate(opts)], "cpu", counts)
+    assert plan.counts is counts and plan.device == "cpu"
+    assert plan.segments == [(8 * i, 5 + i, float(lr), float(config.system.max_grad_norm)) for i, lr in enumerate(lrs)]
+    kw = plan.kwargs
+    assert (kw["b1"], kw["b2"], kw["eps"], kw["decay"]) == (0.9, 0.999, 1e-5, decay)
+    assert "rule" not in kw
+    if decay:
+        assert (kw["steps_per_update"], kw["num_updates"]) == (3 * nmb, 70)
+    else:
+        assert kw["steps_per_update"] > 0 and kw["num_updates"] > 0
+
+
+def test_adam_plan_carries_the_radam_rule(monkeypatch):
+    from stoix_b200 import ops
+    from stoix_b200 import optim as optax
+
+    monkeypatch.setattr(ops, "AdamPlan", _Plan)
+    opt = optax.chain(optax.clip_by_global_norm(0.5), optax.radam(5e-4, eps_root=1e-9, threshold=4.0))
+    plan = optax.adam_plan([(0, 10, opt)], "cpu", None)
+    assert plan.segments == [(0, 10, 5e-4, 0.5)]
+    assert {k: plan.kwargs[k] for k in ("rule", "eps_root", "threshold", "decay")} == {"rule": "radam", "eps_root": 1e-9, "threshold": 4.0,
+                                                                                        "decay": False}
