@@ -661,6 +661,44 @@ int stx_q_td_loss_grads(int rule, const float* q_tm1, const float* q_t, const fl
                         const uint8_t* done, const float* discount, int64_t M, int A, const StxQTdHyper* hyper, float* d_q, float* metrics,
                         float weight, void* scratch, void* stream);
 
+/* ------------------------------------------------------------------ distributional Q-learning: C51 and QR-DQN (fp32) ----
+ * Head rows (M, A N) in the reference's layout: column a N + i is action a, atom / quantile i (reshape(-1, A, N), heads.py:251,288).
+ * stx_dist_q_values: the expected Q of each action, q (M, A), that EpsilonGreedy acts on; one thread per (row, action), i in order:
+ *   STX_DIST_CATEGORICAL: sum_i softmax(logits[a, :])_i atoms_i, the softmax in max-subtracted form (heads.py:252-253); atoms (N)
+ *   STX_DIST_QUANTILE:    (sum_i q[a, i]) / N, jnp.mean (heads.py:289); atoms unused
+ * stx_categorical_q_loss_grads: categorical_double_q_learning (utils/loss.py:81-103) under jax.grad, as ff_c51.py:159-188 calls it:
+ *   r = clip(reward, +-max_abs_reward), d = (1 - done) gamma (or discount[m]), a* = first argmax of q_sel (M, A);
+ *   p = softmax(logits_t[a*]); target_z = r + d atoms_t; t = rlax.categorical_l2_project(target_z, p, atoms_tm1);
+ *   loss = -sum_j t_j log_softmax(logits_tm1[a])_j; d_logits = (softmax(logits_tm1[a]) sum_j t_j - t) / M in action a's N columns,
+ *   0 in the others.  The projection is a gather: target atom i sums over the source atoms j = 0..N-1 in order (no atomics).
+ * stx_quantile_q_loss_grads: quantile_q_learning + quantile_regression_loss (utils/loss.py:226-314), as ff_qr_dqn.py:159-202 calls
+ *   it: a* = first argmax_a of (sum_i q_sel[a, i]) / N (q_sel nullable -> q_t, the reference's selector); target_j = r + d q_t[a*, j];
+ *   delta_ij = target_j - q_tm1[a, i]; w_ij = |tau_i - 1[delta_ij < 0]| (delta = 0 weighs tau_i); loss = sum_i mean_j w_ij rho(delta_ij)
+ *   with rho = rlax.huber_loss(., huber_delta) when huber_delta > 0, else |.|; d q_tm1[a, i] = -(sum_j w_ij rho'(delta_ij)) / (N M),
+ *   rho' = clip(delta, -huber_delta, huber_delta), or for |.| JAX's select(delta >= 0, 1, -1) (slope +1 at 0); 0 in other columns.
+ *   The row is spread over TPR threads (32 / 64 / 128 / 256 for N <= 32 / 64 / 128 / larger, 256 / TPR rows per CTA); thread i
+ *   accumulates over j in order and the row's loss is a fixed-order tree, so two launches give the same bits.
+ * Both losses: atoms_* / tau are read at row m as ptr + m ld_* (ld 0: one shared row); discount (nullable, per row) replaces
+ *   (1 - done) gamma; loss_rows (nullable, (M)) receives each row's loss; metrics[0] += weight mean(loss).
+ *   N <= STX_DIST_MAX_N (shared-memory bound), else STX_E_SHAPE.  scratch: stx_dist_q_scratch_bytes(M), zeroed once. */
+enum { STX_DIST_CATEGORICAL = 0, STX_DIST_QUANTILE = 1 };
+#define STX_DIST_MAX_N 2048
+typedef struct StxDistQHyper {
+  float gamma;
+  float max_abs_reward;
+  float huber_delta;  /* QR-DQN kappa; unused by C51 */
+  int32_t reserved;
+} StxDistQHyper;
+size_t stx_dist_q_scratch_bytes(int64_t M);
+int stx_dist_q_values(int kind, const float* head, int64_t M, int A, int N, const float* atoms, float* q, void* stream);
+int stx_categorical_q_loss_grads(const float* logits_tm1, const float* logits_t, const float* q_sel, const float* atoms_tm1, int64_t ld_atoms_tm1,
+                                 const float* atoms_t, int64_t ld_atoms_t, const int32_t* action, const float* reward, const uint8_t* done,
+                                 const float* discount, int64_t M, int A, int N, const StxDistQHyper* hyper, float* d_logits, float* loss_rows,
+                                 float* metrics, float weight, void* scratch, void* stream);
+int stx_quantile_q_loss_grads(const float* q_tm1, const float* q_t, const float* q_sel, const float* tau, int64_t ld_tau, const int32_t* action,
+                              const float* reward, const uint8_t* done, const float* discount, int64_t M, int A, int N, const StxDistQHyper* hyper,
+                              float* d_q, float* loss_rows, float* metrics, float weight, void* scratch, void* stream);
+
 /* Utility casts used by the bf16 path (obs / weight shadows). */
 int stx_cast_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream);
 

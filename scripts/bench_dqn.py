@@ -1,11 +1,12 @@
-"""DQN-family update-step timing: env steps/s and optimiser steps/s of the captured update step of ff_dqn, ff_ddqn, ff_mdqn and
-ff_dqn_reg at two shapes, the systems alternated within each of three rounds, min-max over the rounds; plus the kernels of one
+"""DQN-family update-step timing: env steps/s and optimiser steps/s of the captured update step of ff_dqn, ff_ddqn, ff_mdqn,
+ff_dqn_reg, ff_c51 and ff_qr_dqn at two shapes, the systems alternated within each of three rounds, min-max over the rounds; plus the kernels of one
 eager update: stx_launch_count (the project's launches that go through STX_LAUNCH_OK, which leaves out the SIMT GEMMs of the MLP
 forward and backward) and every kernel the profiler records, GEMMs counted apart.  The card name and power limit are read in the same call.
 
     python scripts/bench_dqn.py [--updates 50] [--rounds 3]
 
-Shapes (all four systems run the same schedule, so that they differ only in the loss):
+Shapes (every system runs the same schedule, so that they differ only in the head and the loss; ff_c51 and ff_qr_dqn keep their
+own heads, 51 atoms and 200 quantiles per action):
   "default" = the reference's ff_dqn default: CartPole, 1024 envs, T = 2, 16 epochs of batch 512, silu MLP 2 x 256;
   "wide"    = the synthetic Box, obs 64, A = 8, 1024 envs, T = 2, 16 epochs of batch 4096, same network.
 Prints one JSON line per (round, shape, system), then one summary line per (shape, system)."""
@@ -18,7 +19,7 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 
-SYSTEMS = ("ff_dqn", "ff_ddqn", "ff_mdqn", "ff_dqn_reg")
+SYSTEMS = ("ff_dqn", "ff_ddqn", "ff_mdqn", "ff_dqn_reg", "ff_c51", "ff_qr_dqn")
 COMMON = ["arch.total_num_envs=1024", "system.rollout_length=2", "system.epochs=16", "system.total_buffer_size=1000000", "system.warmup_steps=16",
           "logger.use_console=False", "arch.num_evaluation=1"]
 SHAPES = {

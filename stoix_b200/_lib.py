@@ -141,6 +141,15 @@ class StxQTdHyper(C.Structure):
     ]
 
 
+class StxDistQHyper(C.Structure):
+    _fields_ = [
+        ("gamma", C.c_float),
+        ("max_abs_reward", C.c_float),
+        ("huber_delta", C.c_float),
+        ("reserved", C.c_int32),
+    ]
+
+
 class StxPpoBatch(C.Structure):
     _fields_ = [
         ("obs", C.c_void_p),
@@ -279,6 +288,12 @@ _SIGNATURES = {
     "stx_replay_add_discrete": (C.c_int, [C.POINTER(StxReplayDiscrete), _P, _P, _P, _P, _P, C.c_int64, _P]),
     "stx_replay_sample_discrete": (C.c_int, [C.POINTER(StxReplayDiscrete), C.c_int64, C.c_uint64, C.c_uint64, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "stx_q_td_loss_grads": (C.c_int, [C.c_int, _P, _P, _P, _P, _P, _P, _P, C.c_int64, C.c_int, C.POINTER(StxQTdHyper), _P, _P, C.c_float, _P, _P]),
+    "stx_dist_q_scratch_bytes": (C.c_size_t, [C.c_int64]),
+    "stx_dist_q_values": (C.c_int, [C.c_int, _P, C.c_int64, C.c_int, C.c_int, _P, _P, _P]),
+    "stx_categorical_q_loss_grads": (C.c_int, [_P, _P, _P, _P, C.c_int64, _P, C.c_int64, _P, _P, _P, _P, C.c_int64, C.c_int, C.c_int,
+                                               C.POINTER(StxDistQHyper), _P, _P, _P, C.c_float, _P, _P]),
+    "stx_quantile_q_loss_grads": (C.c_int, [_P, _P, _P, _P, C.c_int64, _P, _P, _P, _P, C.c_int64, C.c_int, C.c_int, C.POINTER(StxDistQHyper), _P,
+                                            _P, _P, C.c_float, _P, _P]),
 }
 
 _lib = None

@@ -188,22 +188,6 @@ int fp32_minibatch(const StxMlp* actor, const StxMlp* critic, const StxPpoBatch*
   return simt_net_backward(critic, x, D, idx, mb, workspace, grad_weight, grad_arena + coff, h->overwrite_grads, st);
 }
 
-// ---- rlax.l2_loss / rlax.huber_loss of a TD error and d loss / d td, the element of every Q loss here:
-//   l2:    loss = td^2 / 2,                                       g = td
-//   Huber: loss = q^2 / 2 + delta (|td| - q), q = min(|td|, delta),  g = clip(td, -delta, delta)   (delta > 0)
-// so d loss / d q[a] = -g.  At |td| = delta both Huber branches give the same value (delta^2 / 2) and the same derivative
-// (td = clip(td)), so the tie needs no rule.
-__device__ __forceinline__ void td_loss(float td, float delta, float& loss, float& g) {
-  if (delta > 0.f) {  // rlax.huber_loss
-    const float ax = fabsf(td), quad = fminf(ax, delta), lin = ax - quad;
-    loss = 0.5f * quad * quad + delta * lin;
-    g = fminf(fmaxf(td, -delta), delta);
-  } else {  // rlax.l2_loss
-    loss = 0.5f * td * td;
-    g = td;
-  }
-}
-
 // ---- PQN Q loss + its gradient with respect to the Q rows (one thread per minibatch row).
 //
 // Reference: _q_loss_fn of stoix/systems/q_learning/ff_pqn.py:139-162 under jax.grad: td = target - q[a], td_loss above,

@@ -22,23 +22,13 @@
 // instantiation evaluates exactly the float expressions of its pair.
 #pragma once
 #include "stx_common.cuh"
+#include "stx_loss_rows.cuh"
 #include "stx_tanh_normal.cuh"
 
 namespace stx {
 
 constexpr int kMaxActions = 32;  // Categorical logits / tanh-Normal dims per thread
 constexpr int kSlotKl = 6;       // metrics slot of kl_divergence (0 actor_loss, 1 entropy, 2 value_loss, 3 advantages, 4 / 5 value, target)
-
-// The minibatch rows of a loss kernel and where it accumulates its metrics.
-struct LossRows {
-  const int32_t* idx;     // perm + mb_off (nullable -> row0 + m)
-  int64_t row0, mb;
-  double* partials;       // [grid][6] per-block metric partials
-  unsigned int* counter;  // last-block ticket, zero between calls
-  float* metrics;         // accumulated with weight
-  float weight;
-  __device__ __forceinline__ int64_t src(int64_t m) const { return idx ? (int64_t)idx[m] : row0 + m; }
-};
 
 struct ActorLossArgs {
   LossRows r;
@@ -53,27 +43,6 @@ struct ActorLossArgs {
   int A;
   float clip_eps, kl_coef, dpo_alpha, dpo_beta, ent_coef;
 };
-
-// Deterministic metric reduction of the loss kernels: per-block partials, then the last block sums them in block order.
-// Partial column k (of the 6 per block) feeds metrics[slot[k]].
-template <int N>
-__device__ __forceinline__ void reduce_metrics(const double (&v)[N], const int (&slot)[N], const LossRows& r) {
-  __shared__ double sm[32];
-#pragma unroll
-  for (int k = 0; k < N; ++k) {
-    const double s = block_sum<double>(v[k], sm);
-    if (threadIdx.x == 0) r.partials[(int64_t)blockIdx.x * 6 + k] = s;
-  }
-  if (last_block_ticket(r.counter, gridDim.x)) {
-#pragma unroll
-    for (int k = 0; k < N; ++k) {
-      double s = 0.0;
-      for (unsigned int i = threadIdx.x; i < gridDim.x; i += blockDim.x) s += r.partials[(int64_t)i * 6 + k];
-      s = block_sum<double>(s, sm);
-      if (threadIdx.x == 0) r.metrics[slot[k]] += r.weight * (float)(s / (double)r.mb);
-    }
-  }
-}
 
 // ---- heads: load a row, logp(stored action), entropy and (KL) KL(behaviour || pi); then write d head --------------------
 

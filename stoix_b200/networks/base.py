@@ -35,6 +35,21 @@ def _orthogonal(gen: torch.Generator, n_in: int, n_out: int, scale: float) -> to
     return (scale * q).to(torch.float32)
 
 
+def _lecun_normal(gen: torch.Generator, n_in: int, n_out: int, scale: float) -> torch.Tensor:
+    """flax.linen.initializers.lecun_normal() = variance_scaling(scale, "fan_in", "truncated_normal"): a normal truncated to
+    [-2, 2] standard deviations, scaled to variance scale / fan_in (std sqrt(scale / n_in) / 0.8796..., the std of the unit
+    normal truncated there).  Out-of-range draws are redrawn."""
+    a = torch.randn(n_in, n_out, generator=gen, dtype=torch.float64)
+    bad = a.abs() > 2.0
+    while bool(bad.any()):
+        a[bad] = torch.randn(int(bad.sum()), generator=gen, dtype=torch.float64)
+        bad = a.abs() > 2.0
+    return (a * (np.sqrt(scale / n_in) / 0.87962566103423978)).to(torch.float32)
+
+
+_KERNEL_INITS = {"orthogonal": _orthogonal, "lecun_normal": _lecun_normal}
+
+
 def build_param_tree(spec: ops.MlpSpec, flat: torch.Tensor, head_name: str, flat_bf16=None) -> ParamTree:
     sl = spec.layer_slices()
     n = spec.n_layers
@@ -82,8 +97,9 @@ class _FeedForward:
             blocks = getattr(self.head, "kernel_blocks", None) if i == spec.n_layers - 1 else None
             if blocks:  # several Dense heads side by side (NormalAffineTanhDistributionHead): independent orthogonal blocks
                 host[sl[i][0]] = torch.cat([_orthogonal(gen, spec.sizes[i], int(b), scale) for b in blocks], dim=1).reshape(-1)
-            else:
-                host[sl[i][0]] = _orthogonal(gen, spec.sizes[i], spec.sizes[i + 1], scale).reshape(-1)
+            else:   # the head's kernel_init_kind (orthogonal unless the head names another, as the distributional Q heads do)
+                kind = getattr(self.head, "kernel_init_kind", "orthogonal") if i == spec.n_layers - 1 else "orthogonal"
+                host[sl[i][0]] = _KERNEL_INITS[kind](gen, spec.sizes[i], spec.sizes[i + 1], scale).reshape(-1)
             if spec.has_ln(i):
                 host[sl[i][1]] = 1.0  # LayerNorm scale = ones, bias = zeros (flax defaults)
         if flat is None:

@@ -1,7 +1,8 @@
 """CategoricalHead / NormalAffineTanhDistributionHead / ScalarCriticHead -- constructor-compatible with
 stoix/networks/heads.py:30-41, 44-65, 129-134, and the distribution objects the actor returns (tfd.Categorical's sample /
 log_prob / entropy / mode as used at ff_ppo.py:100-101,199,205; the tanh-Normal's sample / log_prob / mode as used at
-ff_sac.py:119-122,165-167); DiscreteQNetworkHead (heads.py:202-217) and its EpsilonGreedy (ff_pqn.py:79-82)."""
+ff_sac.py:119-122,165-167); DiscreteQNetworkHead (heads.py:202-217) and its EpsilonGreedy (ff_pqn.py:79-82);
+DistributionalDiscreteQNetwork and QuantileDiscreteQNetwork (heads.py:236-292)."""
 from __future__ import annotations
 
 from typing import Optional, Sequence, Union
@@ -173,3 +174,63 @@ class NormalAffineTanhDistributionHead:
 
     def distribution(self, head_out: torch.Tensor) -> AffineTanhNormal:
         return AffineTanhNormal(head_out, self.minimum, self.maximum, self.min_scale)
+
+
+def linspace_f32(start: float, stop: float, num: int) -> np.ndarray:
+    """jnp.linspace(start, stop, num) in float32 by JAX's formula: start (1 - s_i) + stop s_i with s_i = i / (num - 1), the last
+    point exactly `stop`.  The C51 atoms: the kernels, the value faces and the oracle all read these values."""
+    start, stop = np.float32(start), np.float32(stop)
+    if num == 1:
+        return np.array([start], np.float32)
+    s = np.arange(num, dtype=np.float32) / np.float32(num - 1)
+    out = (start * (np.float32(1) - s) + stop * s).astype(np.float32)
+    out[-1] = stop
+    return out
+
+
+class DistributionalDiscreteQNetwork:
+    """heads.py:236-258: Dense(action_dim num_atoms) with a lecun_normal kernel; apply returns (EpsilonGreedy(q), logits (M, A, N),
+    atoms (M, N)), q = sum_i softmax(logits[a])_i atoms_i from stx_dist_q_values."""
+
+    kernel_init_kind = "lecun_normal"
+
+    def __init__(self, action_dim: int, epsilon: float = 0.1, num_atoms: int = 51, vmin: float = 0.0, vmax: float = 500.0):
+        self.action_dim, self.epsilon, self.num_atoms = int(action_dim), float(epsilon), int(num_atoms)
+        self.vmin, self.vmax = float(vmin), float(vmax)
+        self.out_dim = self.action_dim * self.num_atoms
+        self.kernel_init_scale = 1.0
+        self.atoms_host = linspace_f32(self.vmin, self.vmax, self.num_atoms)
+        self._atoms = {}
+
+    def atoms(self, device) -> torch.Tensor:
+        """The (N) atoms on `device`, built once per device."""
+        key = str(device)
+        if key not in self._atoms:
+            self._atoms[key] = torch.tensor(self.atoms_host, device=device)
+        return self._atoms[key]
+
+    def distribution(self, logits: torch.Tensor, epsilon: Optional[float] = None):
+        A, N = self.action_dim, self.num_atoms
+        flat = logits.reshape(-1, A * N).contiguous()
+        atoms = self.atoms(flat.device)
+        q = ops.dist_q_values("categorical", flat, A, N, atoms)
+        return (EpsilonGreedy(q, self.epsilon if epsilon is None else epsilon), flat.view(-1, A, N),
+                atoms.expand(flat.shape[0], N))
+
+
+class QuantileDiscreteQNetwork:
+    """heads.py:275-292: Dense(action_dim num_quantiles) with a lecun_normal kernel; apply returns (EpsilonGreedy(q), q_dist (M, A, N)),
+    q = mean_i q_dist[a, i] from stx_dist_q_values."""
+
+    kernel_init_kind = "lecun_normal"
+
+    def __init__(self, action_dim: int, epsilon: float = 0.1, num_quantiles: int = 200):
+        self.action_dim, self.epsilon, self.num_quantiles = int(action_dim), float(epsilon), int(num_quantiles)
+        self.out_dim = self.action_dim * self.num_quantiles
+        self.kernel_init_scale = 1.0
+
+    def distribution(self, out: torch.Tensor, epsilon: Optional[float] = None):
+        A, N = self.action_dim, self.num_quantiles
+        flat = out.reshape(-1, A * N).contiguous()
+        q = ops.dist_q_values("quantile", flat, A, N)
+        return EpsilonGreedy(q, self.epsilon if epsilon is None else epsilon), flat.view(-1, A, N)

@@ -1361,3 +1361,100 @@ def q_td_loss_grads(rule: str, q_tm1: torch.Tensor, q_t: torch.Tensor, action: t
     _lib.check(lib.stx_q_td_loss_grads(Q_RULES[rule], _p(q_tm1), _p(q_t), _p(q_aux), _p(action), _p(reward), _p(None if done is None else _u8(done)),
                                        _p(discount), M, A, C.byref(hyper), _p(d_q), _p(metrics), float(weight), _p(scratch), _stream()),
                "stx_q_td_loss_grads")
+
+
+# ------------------------------------------------------------------------------------------------
+# Distributional Q-learning: C51 and QR-DQN (stoix/utils/loss.py:81-103, 226-314; stoix/networks/heads.py:236-292)
+# ------------------------------------------------------------------------------------------------
+
+DIST_KINDS = {"categorical": 0, "quantile": 1}   # STX_DIST_* of stx.h
+DIST_MAX_N = 2048                                # STX_DIST_MAX_N
+
+
+def dist_q_hyper(gamma: float = 0.99, max_abs_reward: float = float("inf"), huber_delta: float = 0.0) -> _lib.StxDistQHyper:
+    return _lib.StxDistQHyper(float(gamma), float(max_abs_reward), float(huber_delta), 0)
+
+
+def dist_q_values(kind: str, head: torch.Tensor, A: int, N: int, atoms: Optional[torch.Tensor] = None,
+                  out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Expected Q (M, A) of head rows (M, A N), column a N + i = action a, atom / quantile i: sum_i softmax(logits[a])_i atoms_i
+    ("categorical", atoms (N) fp32) or mean_i q[a, i] ("quantile")."""
+    dev = _need_cuda(head, atoms, out)
+    if kind not in DIST_KINDS:
+        raise StxError(f"dist_q_values: kind {kind!r} is not one of {sorted(DIST_KINDS)}")
+    if head.dtype != torch.float32 or head.ndim != 2 or head.shape[1] != A * N or not head.is_contiguous():
+        raise StxError(f"dist_q_values: head must be contiguous float32 (M, {A * N})")
+    if kind == "categorical" and (atoms is None or atoms.dtype != torch.float32 or atoms.numel() != N or not atoms.is_contiguous()):
+        raise StxError(f"dist_q_values: atoms must be contiguous float32 ({N})")
+    M = head.shape[0]
+    if out is None:
+        out = torch.empty(M, A, dtype=torch.float32, device=dev)
+    elif out.dtype != torch.float32 or tuple(out.shape) != (M, A) or not out.is_contiguous():
+        raise StxError(f"dist_q_values: out must be contiguous float32 ({M}, {A})")
+    _lib.check(_lib.load().stx_dist_q_values(DIST_KINDS[kind], _p(head), M, int(A), int(N), _p(atoms if kind == "categorical" else None), _p(out),
+                                             _stream()), "stx_dist_q_values")
+    return out
+
+
+def _dist_rows(who: str, ref: torch.Tensor, M: int, W: int, mats, rows, per_row, N: int):
+    for t, name in mats:
+        if t is not None and (t.dtype != torch.float32 or tuple(t.shape) != (M, W) or not t.is_contiguous()):
+            raise StxError(f"{who}: {name} must be contiguous float32 ({M}, {W})")
+    for t, dt, name in rows:
+        if t is not None and (t.dtype != dt or t.numel() != M or not t.is_contiguous()):
+            raise StxError(f"{who}: {name} must be contiguous {dt} (M)")
+    lds = []
+    for t, name in per_row:   # (N): one row shared by every sample (row stride 0), or (M, N): the reference's per-row arrays
+        if t.dtype != torch.float32 or not t.is_contiguous() or not (tuple(t.shape) == (N,) or tuple(t.shape) == (M, N)):
+            raise StxError(f"{who}: {name} must be contiguous float32 ({N}) or ({M}, {N})")
+        lds.append(0 if t.ndim == 1 else N)
+    return lds
+
+
+def categorical_q_loss_grads(logits_tm1: torch.Tensor, logits_t: torch.Tensor, q_sel: torch.Tensor, atoms_tm1: torch.Tensor, atoms_t: torch.Tensor,
+                             action: torch.Tensor, reward: torch.Tensor, hyper: _lib.StxDistQHyper, d_logits: torch.Tensor, metrics: torch.Tensor,
+                             done: Optional[torch.Tensor] = None, discount: Optional[torch.Tensor] = None,
+                             loss_rows: Optional[torch.Tensor] = None, weight: float = 1.0, scratch_key: str = "c51_loss") -> None:
+    """categorical_double_q_learning under jax.grad (stx_categorical_q_loss_grads): logits (M, A N), q_sel (M, A) the selector's
+    expected Q, atoms (N) or (M, N).  d mean(loss) / d logits_tm1 into d_logits, metrics[0] += weight mean(loss), the per-row loss
+    into loss_rows (M) when given.  The discount is (1 - done) gamma, or `discount` (M) given directly."""
+    dev = _need_cuda(logits_tm1, logits_t, q_sel, atoms_tm1, atoms_t, action, reward, done, discount, d_logits, metrics, loss_rows)
+    if q_sel.ndim != 2 or logits_tm1.ndim != 2:
+        raise StxError("categorical_q_loss_grads: logits must be (M, A N) and q_sel (M, A)")
+    M, A = q_sel.shape
+    N = int(atoms_tm1.shape[-1])
+    if N <= 0 or logits_tm1.shape[1] != A * N:
+        raise StxError(f"categorical_q_loss_grads: logits_tm1 has {logits_tm1.shape[1]} columns, not A N = {A} x {N}")
+    ld = _dist_rows("categorical_q_loss_grads", logits_tm1, M, A * N, ((logits_tm1, "logits_tm1"), (logits_t, "logits_t"), (d_logits, "d_logits")),
+                    ((action, torch.int32, "action"), (reward, torch.float32, "reward"), (discount, torch.float32, "discount"),
+                     (None if done is None else _u8(done), torch.uint8, "done"), (loss_rows, torch.float32, "loss_rows")),
+                    ((atoms_tm1, "atoms_tm1"), (atoms_t, "atoms_t")), N)
+    _dist_rows("categorical_q_loss_grads", q_sel, M, A, ((q_sel, "q_sel"),), (), (), N)
+    lib = _lib.load()
+    scratch = _zeros_scratch((scratch_key,), lib.stx_dist_q_scratch_bytes(M), dev)
+    _lib.check(lib.stx_categorical_q_loss_grads(_p(logits_tm1), _p(logits_t), _p(q_sel), _p(atoms_tm1), ld[0], _p(atoms_t), ld[1], _p(action), _p(reward),
+                                                _p(None if done is None else _u8(done)), _p(discount), M, A, N, C.byref(hyper), _p(d_logits),
+                                                _p(loss_rows), _p(metrics), float(weight), _p(scratch), _stream()), "stx_categorical_q_loss_grads")
+
+
+def quantile_q_loss_grads(q_tm1: torch.Tensor, q_t: torch.Tensor, tau: torch.Tensor, action: torch.Tensor, reward: torch.Tensor,
+                          hyper: _lib.StxDistQHyper, d_q: torch.Tensor, metrics: torch.Tensor, A: int, q_sel: Optional[torch.Tensor] = None,
+                          done: Optional[torch.Tensor] = None, discount: Optional[torch.Tensor] = None,
+                          loss_rows: Optional[torch.Tensor] = None, weight: float = 1.0, scratch_key: str = "qr_loss") -> None:
+    """quantile_q_learning under jax.grad (stx_quantile_q_loss_grads): quantile rows (M, A N), tau (N) or (M, N), q_sel (M, A N)
+    the greedy selector's quantiles (None: q_t, as ff_qr_dqn).  Outputs as categorical_q_loss_grads."""
+    dev = _need_cuda(q_tm1, q_t, q_sel, tau, action, reward, done, discount, d_q, metrics, loss_rows)
+    if q_tm1.ndim != 2:
+        raise StxError("quantile_q_loss_grads: q_tm1 must be (M, A N)")
+    M, N = q_tm1.shape[0], int(tau.shape[-1])
+    if N <= 0 or q_tm1.shape[1] != A * N:
+        raise StxError(f"quantile_q_loss_grads: q_tm1 has {q_tm1.shape[1]} columns, not A N = {A} x {N}")
+    (ld,) = _dist_rows("quantile_q_loss_grads", q_tm1, M, A * N, ((q_tm1, "q_tm1"), (q_t, "q_t"), (q_sel, "q_sel"), (d_q, "d_q")),
+                       ((action, torch.int32, "action"), (reward, torch.float32, "reward"), (discount, torch.float32, "discount"),
+                        (None if done is None else _u8(done), torch.uint8, "done"), (loss_rows, torch.float32, "loss_rows")),
+                       ((tau, "tau"),), N)
+    lib = _lib.load()
+    scratch = _zeros_scratch((scratch_key,), lib.stx_dist_q_scratch_bytes(M), dev)
+    _lib.check(lib.stx_quantile_q_loss_grads(_p(q_tm1), _p(q_t), _p(q_sel), _p(tau), ld, _p(action), _p(reward), _p(None if done is None else _u8(done)),
+                                             _p(discount), M, int(A), N, C.byref(hyper), _p(d_q), _p(loss_rows), _p(metrics), float(weight),
+                                             _p(scratch), _stream()), "stx_quantile_q_loss_grads")

@@ -12,6 +12,15 @@ hydra_entry_point).  The four reference systems differ only in `_q_loss_fn`; her
                                                                                    stacked (obs | next_obs) rows (ff_mdqn.py:154)
   q_learning_reg           q_learning + regularizer_coeff mean(q_tm1[a])           - (ff_dqn_reg.py:165-176)
 
+The distributional systems ff_c51 and ff_qr_dqn run the same body with a head of A N outputs per row (column a N + i = action
+a, atom / quantile i) and a loss kernel of their own; the rollout and the warm-up put stx_dist_q_values (the expected Q) between
+the forward and epsilon-greedy, so the shard's q (T, E, A) holds expected values:
+
+  loss                            kernel                          extra forward per shard and epoch
+  ------------------------------  ------------------------------  -------------------------------------------------------------
+  categorical_double_q_learning   stx_categorical_q_loss_grads    online on next_obs + stx_dist_q_values (ff_c51.py:165-168)
+  quantile_q_learning             stx_quantile_q_loss_grads       - (the selector is the target distribution, ff_qr_dqn.py:193-194)
+
   reference (JAX)                                      here (H100)
   ---------------------------------------------------  ------------------------------------------------------------------
   flashbax item buffer, int action (dqn_types.py)      discrete device ring (stx_replay_add_discrete / _sample_discrete):
@@ -43,7 +52,7 @@ from stoix_b200.config import DictConfig, instantiate
 from stoix_b200.envs.base import Environment
 from stoix_b200.networks.base import FeedForwardActor as Actor
 from stoix_b200.networks.base import build_param_tree
-from stoix_b200.networks.heads import DiscreteQNetworkHead
+from stoix_b200.networks.heads import DiscreteQNetworkHead, DistributionalDiscreteQNetwork, QuantileDiscreteQNetwork
 from stoix_b200.systems import anakin
 from stoix_b200.systems.q_learning.dqn_types import Transition
 from stoix_b200.systems.sac.sac_types import OffPolicyLearnerState, OnlineAndTarget
@@ -51,23 +60,55 @@ from stoix_b200.utils.checkpointing import warm_start
 from stoix_b200.utils.replay import DiscreteTransitionBuffer
 from stoix_b200.utils.training import make_learning_rate
 
-LOSSES = tuple(ops.Q_RULES)
-_NAMES = {"q_learning": "DQN", "double_q_learning": "DDQN", "munchausen_q_learning": "MDQN", "q_learning_reg": "DQN-Reg"}
+# the distributional losses: loss -> (head class, stx_dist_q_values kind, system, network config)
+DIST_LOSSES = {"categorical_double_q_learning": (DistributionalDiscreteQNetwork, "categorical", "ff_c51", "mlp_c51"),
+               "quantile_q_learning": (QuantileDiscreteQNetwork, "quantile", "ff_qr_dqn", "mlp_qr_dqn")}
+LOSSES = tuple(ops.Q_RULES) + tuple(DIST_LOSSES)
+_NAMES = {"q_learning": "DQN", "double_q_learning": "DDQN", "munchausen_q_learning": "MDQN", "q_learning_reg": "DQN-Reg",
+          "categorical_double_q_learning": "C51", "quantile_q_learning": "QR-DQN"}
 
 
-def _refuse_unsupported(config: DictConfig) -> None:
+def _refuse_unsupported(config: DictConfig, loss: str = "q_learning") -> None:
     if str(config.arch.get("precision", "f32")) == "bf16":
         raise ValueError("arch.precision=bf16 is not available for the DQN family: the bf16 tensor-core kernels implement the relu 2 x 256 "
                          "Categorical actor-critic only, not a Q network with its activation, LayerNorm and Q loss; use arch.precision=f32")
     target = str(config.network.actor_network.action_head.get("_target_", ""))
-    if not target.endswith("DiscreteQNetworkHead"):
+    name = target.rsplit(".", 1)[-1]
+    dist = {v[0].__name__: (k, v[2], v[3]) for k, v in DIST_LOSSES.items()}
+    if loss in DIST_LOSSES:
+        _, _, system, network = DIST_LOSSES[loss]
+        if name != DIST_LOSSES[loss][0].__name__:
+            raise ValueError(f"{system} runs the {DIST_LOSSES[loss][0].__name__} head (network={network}); action head {target!r} is not "
+                             "implemented for it")
+    elif name in dist:
+        raise ValueError(f"action head {target!r} is a distributional head: it runs with {dist[name][1]} (network={dist[name][2]}), not "
+                         f"with the {loss} loss")
+    elif not target.endswith("DiscreteQNetworkHead"):
         raise ValueError(f"the DQN family here runs the plain Q head (network=mlp_dqn); action head {target!r} (dueling, noisy, "
                          "distributional) is not implemented")
 
 
-def loss_hyper(loss: str, config: DictConfig):
-    """The StxQTdHyper of `loss` from config.system (the keys of system/q_learning/ff_{dqn,mdqn,dqn_reg}.yaml)."""
+class DistLoss(NamedTuple):
+    """The hyper-parameters of a distributional loss: the kernel's StxDistQHyper, the action count A, the atom / quantile count N
+    and the support row (N) every sample shares: the C51 atoms, or QR-DQN's quantile midpoints tau_i = (i + 0.5) / N."""
+    hyper: Any
+    A: int
+    N: int
+    support: torch.Tensor
+
+
+def loss_hyper(loss: str, config: DictConfig, head: Any = None, device=None):
+    """The StxQTdHyper of `loss` from config.system (the keys of system/q_learning/ff_{dqn,mdqn,dqn_reg}.yaml); for a distributional
+    loss the DistLoss of `head` on `device`."""
     s = config.system
+    if loss in DIST_LOSSES:
+        huber = float(s.huber_loss_parameter) if loss == "quantile_q_learning" else 0.0
+        hyper = ops.dist_q_hyper(gamma=float(s.gamma), max_abs_reward=float(s.max_abs_reward), huber_delta=huber)
+        if loss == "categorical_double_q_learning":
+            return DistLoss(hyper, head.action_dim, head.num_atoms, head.atoms(device))
+        N = head.num_quantiles
+        tau = (torch.arange(N, dtype=torch.float32) + 0.5) / N   # ff_qr_dqn.py:180-182, in float32
+        return DistLoss(hyper, head.action_dim, N, tau.to(device))
     kw = dict(gamma=float(s.gamma), max_abs_reward=float(s.max_abs_reward), huber_delta=float(s.huber_loss_parameter))
     if loss == "munchausen_q_learning":
         kw.update(entropy_temperature=float(s.entropy_temperature), munchausen_coefficient=float(s.munchausen_coefficient),
@@ -101,18 +142,20 @@ class Batch(NamedTuple):
 
 
 class Work(NamedTuple):
-    """Workspaces of batch_grads for M rows: ws (train-mode forward), q_tm1 (M, A), q_tgt (2M, A), q_sel (M, A), dq (M, A)."""
+    """Workspaces of batch_grads for M rows of head width A: ws (train-mode forward), q_tm1 (M, A), q_tgt (2M, A), q_sel (M, A),
+    dq (M, A); for C51 q_val (M, n_actions), the selector's expected Q."""
     ws: torch.Tensor
     q_tm1: torch.Tensor
     q_tgt: torch.Tensor
     q_sel: torch.Tensor
     dq: torch.Tensor
+    q_val: Optional[torch.Tensor] = None
 
 
-def make_work(spec: ops.MlpSpec, M: int, device) -> Work:
+def make_work(spec: ops.MlpSpec, M: int, device, n_actions: Optional[int] = None) -> Work:
     A = spec.sizes[-1]
     z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=device)
-    return Work(ops.mlp_train_workspace(spec, M, device), z(M, A), z(2 * M, A), z(M, A), z(M, A))
+    return Work(ops.mlp_train_workspace(spec, M, device), z(M, A), z(2 * M, A), z(M, A), z(M, A), None if n_actions is None else z(M, n_actions))
 
 
 def make_batch(M: int, D: int, device) -> Batch:
@@ -125,7 +168,8 @@ def batch_grads(loss: str, spec: ops.MlpSpec, online: torch.Tensor, target: torc
     """jax.grad(_q_loss_fn) + pmean over "batch" of one epoch (ff_dqn.py:147-200): per shard the online train-mode forward on obs,
     the target forward on next_obs (MDQN: on obs and next_obs in one launch; DDQN adds the online forward on next_obs), the loss
     kernel and the backward.  `grads` receives the mean over the U shards (the first overwrites, weight 1/U each) and
-    metric[0] += mean q_loss."""
+    metric[0] += mean q_loss.  The distributional losses take a DistLoss as `hyper`: C51 adds the online forward on next_obs and
+    its expected Q as the selector (ff_c51.py:165-168); QR-DQN selects on the target distribution inside its kernel."""
     U = len(batches)
     q_tm1, q_tgt, q_sel, dq = work.q_tm1, work.q_tgt, work.q_sel, work.dq
     for u, b in enumerate(batches):
@@ -133,21 +177,36 @@ def batch_grads(loss: str, spec: ops.MlpSpec, online: torch.Tensor, target: torc
         obs, nxt = b.xs[:M], b.xs[M:]
         ops.mlp_forward_train(spec, online, obs, work.ws, out=q_tm1)
         q_aux = None
-        if loss == "munchausen_q_learning":
+        if loss in DIST_LOSSES:
+            ops.mlp_forward(spec, target, nxt, out=q_tgt[M:], ws_key="dqn_target")
+            if loss == "categorical_double_q_learning":
+                ops.mlp_forward(spec, online, nxt, out=q_sel, ws_key="dqn_selector")
+                ops.dist_q_values("categorical", q_sel, hyper.A, hyper.N, hyper.support, out=work.q_val)
+                ops.categorical_q_loss_grads(q_tm1, q_tgt[M:], work.q_val, hyper.support, hyper.support, b.action, b.reward, hyper.hyper, dq,
+                                             metric, done=b.done, weight=1.0 / U)
+            else:
+                ops.quantile_q_loss_grads(q_tm1, q_tgt[M:], hyper.support, b.action, b.reward, hyper.hyper, dq, metric, hyper.A, done=b.done,
+                                          weight=1.0 / U)
+        elif loss == "munchausen_q_learning":
             ops.mlp_forward(spec, target, b.xs, out=q_tgt, ws_key="dqn_target")
             q_aux = q_tgt[:M]
         else:
             ops.mlp_forward(spec, target, nxt, out=q_tgt[M:], ws_key="dqn_target")
             if loss == "double_q_learning":
                 q_aux = ops.mlp_forward(spec, online, nxt, out=q_sel, ws_key="dqn_selector")
-        ops.q_td_loss_grads(loss, q_tm1, q_tgt[M:], b.action, b.reward, hyper, dq, metric, done=b.done, q_aux=q_aux, weight=1.0 / U)
+        if loss not in DIST_LOSSES:
+            ops.q_td_loss_grads(loss, q_tm1, q_tgt[M:], b.action, b.reward, hyper, dq, metric, done=b.done, q_aux=q_aux, weight=1.0 / U)
         ops.mlp_backward(spec, online, obs, dq, work.ws, net_grad=grads, grad_weight=1.0 / U, overwrite=(u == 0))
 
 
 def get_warmup_fn(env: Environment, q_params: OnlineAndTarget, q_apply_fn: Callable, buffer_add_fn: Callable, config: DictConfig) -> Callable:
     """ff_dqn.py:37-89: `warmup_steps` environment steps with the initial online parameters and the training epsilon, added to
     the buffer (one shard per call)."""
-    draw = lambda obs, key, t: q_apply_fn(q_params.online, obs).sample(seed=key, offset=t).to(torch.int32)
+    def draw(obs, key, t):
+        pi = q_apply_fn(q_params.online, obs)
+        pi = pi[0] if isinstance(pi, tuple) else pi   # the distributional heads return (EpsilonGreedy(expected q), ...)
+        return pi.sample(seed=key, offset=t).to(torch.int32)
+
     return anakin.warmup_fn(env, draw, buffer_add_fn, config)
 
 
@@ -155,21 +214,22 @@ def get_learner_fn(env: Environment, q_apply_fn: Callable, q_update_fn: Callable
                    loss: str = "q_learning"):
     """ff_dqn.py:92-258.  q_apply_fn: the bound `apply` of the Q network (a FeedForwardActor with a DiscreteQNetworkHead); q_update_fn:
     the bound `update` of chain(clip_by_global_norm, adam); buffer_fns = (DiscreteTransitionBuffer.add, .sample_into) unbound, applied
-    to learner_state.buffer_state[u]; loss: one of LOSSES."""
+    to learner_state.buffer_state[u]; loss: one of LOSSES (a distributional loss needs its head, DIST_LOSSES)."""
     q_net = anakin.owner(q_apply_fn, Actor, "q_apply_fn")
-    if not isinstance(q_net.action_head, DiscreteQNetworkHead):
-        raise TypeError("get_learner_fn: q_apply_fn must be the bound `apply` of a FeedForwardActor with a DiscreteQNetworkHead")
-    opt = anakin.owner(q_update_fn, optax.GradientTransformation, "q_update_fn")
     if loss not in LOSSES:
         raise ValueError(f"get_learner_fn: loss {loss!r} is not one of {LOSSES}")
-    _refuse_unsupported(config)
+    head_cls = DIST_LOSSES[loss][0] if loss in DIST_LOSSES else DiscreteQNetworkHead
+    if not isinstance(q_net.action_head, head_cls):
+        raise TypeError(f"get_learner_fn: q_apply_fn must be the bound `apply` of a FeedForwardActor with a {head_cls.__name__}")
+    opt = anakin.owner(q_update_fn, optax.GradientTransformation, "q_update_fn")
+    _refuse_unsupported(config, loss)
+    dist_kind = DIST_LOSSES[loss][1] if loss in DIST_LOSSES else None
     buffer_add_fn, buffer_sample_fn = buffer_fns
     rank, world = anakin.world()
     sysc, arch = config.system, config.arch
     T, E, U = int(sysc.rollout_length), int(arch.num_envs), int(arch.update_batch_size)
     epochs, M = int(sysc.epochs), int(sysc.batch_size)
     tau = float(sysc.tau)
-    hyper = loss_hyper(loss, config)
     sched = ops.epsilon_schedule_struct(float(sysc.training_epsilon), float(sysc.training_epsilon), 0.0, 1, decay=False)
     built: Dict[str, Any] = {}
 
@@ -177,12 +237,14 @@ def get_learner_fn(env: Environment, q_apply_fn: Callable, q_update_fn: Callable
         tree = state.params.online
         spec = tree.spec
         dev = tree.flat.device
-        D, A = spec.sizes[0], spec.sizes[-1]
+        D, A = spec.sizes[0], (q_net.action_head.action_dim if dist_kind else spec.sizes[-1])
         shards = [_Shard(T, E, D, A, dev) for _ in range(U)]
         # "rollouts": the name this list had before it was "shards" like every other learner's; callers that read it keep working
         built.update(spec=spec, dev=dev, plan=optax.adam_plan([(0, spec.param_count, opt)], dev, tree.arena_counts),
-                     shards=shards, rollouts=shards,
-                     batches=[make_batch(M, D, dev) for _ in range(U)], work=make_work(spec, M, dev),
+                     shards=shards, rollouts=shards, hyper=loss_hyper(loss, config, q_net.action_head, dev),
+                     head_out=torch.zeros(E, spec.sizes[-1], device=dev) if dist_kind else None,   # the rollout's A N head row
+                     batches=[make_batch(M, D, dev) for _ in range(U)],
+                     work=make_work(spec, M, dev, A if loss == "categorical_double_q_learning" else None),
                      grads=torch.zeros(tree.arena.numel(), dtype=torch.float32, device=dev),
                      metrics=torch.zeros(epochs, dtype=torch.float32, device=dev),
                      roll_ctr=torch.zeros(1, dtype=torch.int64, device=dev),   # epsilon-greedy call index
@@ -195,7 +257,12 @@ def get_learner_fn(env: Environment, q_apply_fn: Callable, q_update_fn: Callable
         for u in range(U):
             ro: _Shard = b["shards"][u]
             for t in range(T):
-                ops.mlp_forward(b["spec"], online, ro.obs[t], out=ro.q[t], ws_key="dqn_rollout")
+                if dist_kind:
+                    ops.mlp_forward(b["spec"], online, ro.obs[t], out=b["head_out"], ws_key="dqn_rollout")
+                    h = b["hyper"]
+                    ops.dist_q_values(dist_kind, b["head_out"], h.A, h.N, h.support, out=ro.q[t])
+                else:
+                    ops.mlp_forward(b["spec"], online, ro.obs[t], out=ro.q[t], ws_key="dqn_rollout")
                 ops.epsilon_greedy(ro.q[t], sched, seed=state.key[0] + u, offset=t, dev_counter=b["roll_ctr"], out=ro.action[t])
                 anakin.step_env(env, state.env_state, u, ro.action[t], ro.step_out(t), t)
             torch.bitwise_or(ro.terminated, ro.truncated, out=ro.done)
@@ -210,7 +277,7 @@ def get_learner_fn(env: Environment, q_apply_fn: Callable, q_update_fn: Callable
                 bt = b["batches"][u]
                 buffer_sample_fn(state.buffer_state[u], bt.xs[:M], bt.xs[M:], bt.action, bt.reward, bt.done, idx_in=idx_in)
         metric = b["metrics"][ep: ep + 1]
-        batch_grads(loss, b["spec"], online.flat, target.flat, b["batches"], hyper, b["grads"], metric, b["work"])
+        batch_grads(loss, b["spec"], online.flat, target.flat, b["batches"], b["hyper"], b["grads"], metric, b["work"])
         if world > 1:   # pmean over "device": summed by NCCL here, scaled in the optimiser step
             dist.all_reduce(b["grads"], op=dist.ReduceOp.SUM)
         ops.clip_adam_step(b["plan"], online.arena, b["grads"], online.arena_mu, online.arena_nu, grad_scale=1.0 / world)
@@ -249,7 +316,7 @@ def get_learner_fn(env: Environment, q_apply_fn: Callable, q_update_fn: Callable
 def learner_setup(env: Environment, keys: Tuple[int, int], config: DictConfig, loss: str = "q_learning"):
     """Initialise learner_fn, network, optimiser, buffer, environment and states (ff_dqn.py:261-414).  Returns the EVAL network
     (epsilon = system.evaluation_epsilon) as the second element, which is what the reference hands to the evaluator."""
-    _refuse_unsupported(config)
+    _refuse_unsupported(config, loss)
     rank, n_devices = anakin.world()
     device = torch.device("cuda", torch.cuda.current_device())
     action_dim = int(env.action_space().num_values)

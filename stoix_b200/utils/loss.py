@@ -75,3 +75,40 @@ def munchausen_q_learning(q_tm1: torch.Tensor, q_tm1_target: torch.Tensor, a_tm1
     h = ops.q_td_hyper(huber_delta=huber_loss_parameter, entropy_temperature=entropy_temperature, munchausen_coefficient=munchausen_coefficient,
                        clip_value_min=clip_value_min)
     return _q_face("munchausen_q_learning", q_tm1, a_tm1, r_t, d_t, q_t_target, q_tm1_target, h)
+
+
+def _check_actions(who: str, a_tm1: torch.Tensor, A: int) -> torch.Tensor:
+    if a_tm1.numel() and (int(a_tm1.min()) < 0 or int(a_tm1.max()) >= A):   # the kernels index row m at action a unchecked
+        raise ops.StxError(f"{who}: a_tm1 must lie in [0, {A}), got [{int(a_tm1.min())}, {int(a_tm1.max())}]")
+    return a_tm1.to(torch.int32).reshape(-1).contiguous()
+
+
+def categorical_double_q_learning(q_logits_tm1: torch.Tensor, q_atoms_tm1: torch.Tensor, a_tm1: torch.Tensor, r_t: torch.Tensor, d_t: torch.Tensor,
+                                  q_logits_t: torch.Tensor, q_atoms_t: torch.Tensor, q_t_selector: torch.Tensor) -> torch.Tensor:
+    """stoix/utils/loss.py:81-103: per row, the cross-entropy of log_softmax(q_logits_tm1[a_tm1]) against
+    rlax.categorical_l2_project(r_t + d_t q_atoms_t, softmax(q_logits_t[argmax q_t_selector]), q_atoms_tm1).  Logits (M, A, N),
+    atoms (M, N), q_t_selector (M, A); returns the (M) vector."""
+    M, A, N = q_logits_tm1.shape
+    rows = lambda x: x.to(torch.float32).reshape(M, A * N).contiguous()
+    a = _check_actions("categorical_double_q_learning", a_tm1, A)
+    out = torch.empty(M, dtype=torch.float32, device=q_logits_tm1.device)
+    metrics = torch.zeros(1, dtype=torch.float32, device=q_logits_tm1.device)
+    ops.categorical_q_loss_grads(rows(q_logits_tm1), rows(q_logits_t), _q_rows(q_t_selector), _q_rows(q_atoms_tm1), _q_rows(q_atoms_t), a, _flat(r_t),
+                                 ops.dist_q_hyper(), torch.empty(M, A * N, dtype=torch.float32, device=out.device), metrics, discount=_flat(d_t),
+                                 loss_rows=out, scratch_key="c51_face")
+    return out
+
+
+def quantile_q_learning(dist_q_tm1: torch.Tensor, tau_q_tm1: torch.Tensor, a_tm1: torch.Tensor, r_t: torch.Tensor, d_t: torch.Tensor,
+                        dist_q_t_selector: torch.Tensor, dist_q_t: torch.Tensor, huber_param: float = 0.0) -> torch.Tensor:
+    """stoix/utils/loss.py:271-314: mean over rows of quantile_regression_loss(dist_q_tm1[:, :, a_tm1], tau_q_tm1, r_t + d_t
+    dist_q_t[:, :, a*], huber_param), a* = argmax_a mean_i dist_q_t_selector[:, i, a].  Distributions (M, N, A) as the reference
+    takes them (after its swapaxes), tau_q_tm1 (M, N); returns the scalar mean."""
+    M, N, A = dist_q_tm1.shape
+    rows = lambda x: x.to(torch.float32).transpose(1, 2).reshape(M, A * N).contiguous()   # to the head layout (M, A N)
+    a = _check_actions("quantile_q_learning", a_tm1, A)
+    metrics = torch.zeros(1, dtype=torch.float32, device=dist_q_tm1.device)
+    ops.quantile_q_loss_grads(rows(dist_q_tm1), rows(dist_q_t), _q_rows(tau_q_tm1), a, _flat(r_t), ops.dist_q_hyper(huber_delta=huber_param),
+                              torch.empty(M, A * N, dtype=torch.float32, device=metrics.device), metrics, A, q_sel=rows(dist_q_t_selector),
+                              discount=_flat(d_t), scratch_key="qr_face")
+    return metrics[0]
