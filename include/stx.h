@@ -699,6 +699,103 @@ int stx_quantile_q_loss_grads(const float* q_tm1, const float* q_t, const float*
                               const float* reward, const uint8_t* done, const float* discount, int64_t M, int A, int N, const StxDistQHyper* hyper,
                               float* d_q, float* loss_rows, float* metrics, float weight, void* scratch, void* stream);
 
+/* stx_categorical_q_loss_grads with a per-row importance weight w (M) (ff_rainbow.py:196-204): d_logits of row m is scaled by w[m]
+ * and metrics[0] += weight mean(w loss); loss_rows stays the unweighted loss (the new priorities).  w NULL is the unweighted
+ * kernel itself, the same bits as stx_categorical_q_loss_grads. */
+int stx_categorical_q_loss_grads_weighted(const float* logits_tm1, const float* logits_t, const float* q_sel, const float* atoms_tm1,
+                                          int64_t ld_atoms_tm1, const float* atoms_t, int64_t ld_atoms_t, const int32_t* action, const float* reward,
+                                          const uint8_t* done, const float* discount, const float* w, int64_t M, int A, int N,
+                                          const StxDistQHyper* hyper, float* d_logits, float* loss_rows, float* metrics, float weight, void* scratch,
+                                          void* stream);
+
+/* ------------------------------------------------------------------ Rainbow: noisy layers, dueling head, prioritised ring (fp32) ----
+ * Noisy layers (NoisyLinear, stoix/networks/layers.py:71-169): y = x (mu_w + sigma_w o eps_w) + mu_b + sigma_b o eps_b with factorised
+ * noise eps_w = f(eps_in) f(eps_out)^T, eps_b = f(eps_out), f(z) = sign(z) sqrt|z| of standard normals, one draw per layer per call.
+ *   The parameter arena holds every layer as kernel mu_w (in x out), bias mu_b (out), sigma_w (in x out), sigma_b (out), at
+ *   StxNoisyLayer.param.  stx_noisy_weights writes the effective weights mu + sigma o eps of every layer into a dense StxMlp arena
+ *   `eff` (at eff_w with row stride ld, the bias at eff_b), so stx_mlp_forward(_train) / stx_mlp_backward run unchanged on it; entries
+ *   of `eff` no layer covers (the zero blocks of a block-diagonal layer) are never written.  Products in order, each rounded:
+ *   eff_w = mu_w + sigma_w (f_in f_out), eff_b = mu_b + sigma_b f_out.
+ *   noise: the f values, layer after layer f_in (in) then f_out (out) at StxNoisyLayer.noise.  draw != 0: noise element j is
+ *   f(z), z = the first normal of normal2 over words (x, y) of Philox4x32-10 keyed by seed with counter (j, call, call >> 32,
+ *   0x4E4F4953), call = offset + *dev_counter (nullable), and `noise` receives them; draw = 0: `noise` is an input.
+ * stx_noisy_fold: the gradient of the parameters from the gradient of the effective arena under the same noise:
+ *   d mu_w = g_w, d sigma_w = g_w (f_in f_out), d mu_b = g_b, d sigma_b = g_b f_out, written (overwrite) or added into `grad`
+ *   (parameter layout).
+ * stx_dueling_combine: head rows (M, N + A N) = (v | adv), column N + a N + i = adv[a, i]  ->  q_logits (M, A N),
+ *   q[a, i] = (v[i] + adv[a, i]) - (sum_a adv[a, i]) / A, a in order (dueling.py:117).
+ * stx_dueling_backward: d_head (M, N + A N) from d q_logits: dv[i] = sum_a dq[a, i], dadv[a, i] = dq[a, i] - (sum_a dq[a, i]) / A. */
+#define STX_NOISY_MAX_LAYERS 8
+typedef struct StxNoisyLayer {
+  int64_t param;  /* first float of the layer (mu_w) in the parameter arena */
+  int64_t eff_w;  /* first weight of the layer's block in the effective arena */
+  int64_t eff_b;  /* first bias of the layer's block in the effective arena */
+  int64_t noise;  /* first f_in of the layer in the noise buffer */
+  int32_t in, out;
+  int32_t ld;     /* row stride of the effective weight block (the width of its StxMlp layer) */
+  int32_t reserved;
+} StxNoisyLayer;
+typedef struct StxNoisyNet {
+  StxNoisyLayer layers[STX_NOISY_MAX_LAYERS];
+  int32_t n_layers;
+  int32_t reserved;
+} StxNoisyNet;
+int stx_noisy_weights(const StxNoisyNet* net, const float* params, float* eff, float* noise, int draw, uint64_t seed, uint64_t offset,
+                      const uint64_t* dev_counter, void* stream);
+int stx_noisy_fold(const StxNoisyNet* net, const float* eff_grad, const float* noise, float* grad, int overwrite, void* stream);
+int stx_dueling_combine(const float* head, int64_t M, int A, int N, float* q_logits, void* stream);
+int stx_dueling_backward(const float* d_q_logits, int64_t M, int A, int N, float* d_head, void* stream);
+
+/* Prioritised trajectory ring -- fbx.make_prioritised_trajectory_buffer as ff_rainbow.py:433-442 builds it (add_batch_size = E,
+ * sample_sequence_length = min_length_time_axis = n_step, period = 1, max_length_time_axis = L), with the n-step target of
+ * ff_rainbow.py:222-246 computed while sampling.
+ *   Storage is time-major: row (t, e) at t E + e, one write index for all envs.  Item i = e L + p is the sequence of env e
+ *   starting at ring row p.  With write index w and c = min(rows written, L), the age of row p is (w - 1 - p) mod L and item
+ *   (e, p) is valid iff n - 1 <= age(p) < c: its n rows are written and do not straddle the write head.  Invalid items have
+ *   priority 0.  Priorities live in a sum tree of fan-out STX_PRIO_FANOUT over the E L leaves (leaf i = item i; level after
+ *   level, stx_prio_tree_floats floats); a parent is the sum of its children in index order, rebuilt from them after every
+ *   change (no atomics: two launches on the same state give the same bits).
+ *   add:    T time rows of (T, E) batches at rows w .. w + T - 1 (mod L; only the last L if T > L), then the items starting
+ *           at rows w - n + 1 .. w + T - 1 (at most L per env) are re-evaluated: valid ones get *max_priority, the others 0.
+ *   sample: stratified: sample r takes v = ((r + u_r) total) / M (u_r = u_in[r], or u01 of word r & 3 of Philox (seed; r / 4,
+ *           call, call >> 32, 0x5052494F), call = offset + *dev_counter) and descends from the root: at each node the children
+ *           in order, entering the first with v < s (s its sum), else v -= s; if none, the last child with s > 0.  It writes
+ *           the item's step-0 obs and action, step n-1 next_obs, the n-step reward G_0 (G = r_{n-1}; G_k = r_k + d_k G_{k+1},
+ *           d_k = (1 - done_k) gamma, batch_discounted_returns with v = 0), done = any(done_0 .. done_{n-1}), idx_out (the item),
+ *           prob_out = leaf / total and weight_out w = (1/p)^beta / max_batch (1/p)^beta, beta = linear schedule from beta0 to 1
+ *           over beta_steps at *count (optax.linear_schedule: c = clip(count, 0, steps), beta = (beta0 - 1)(1 - c / steps) + 1;
+ *           beta0 when steps <= 0; count nullable = 0).  obs / next_obs may be the two halves of one (2M, obs_dim) block.
+ *   set_priorities: leaf idx[m] = priorities[m]^priority_exponent; for an index given twice the last occurrence in batch order
+ *           wins (resolved in O(M) through `owner`); *max_priority = max(*max_priority, max_m priorities[m]^priority_exponent).
+ *           Precondition, not checked on the device: every idx[m] is in [0, E L), as the sampler's idx_out is.
+ *   scratch: stx_prio_scratch_bytes(), zeroed once. */
+#define STX_PRIO_FANOUT 32
+typedef struct StxReplayPrioritised {
+  float* obs;            /* [L][E][obs_dim] */
+  int32_t* action;       /* [L][E] */
+  float* reward;         /* [L][E] */
+  uint8_t* done;         /* [L][E]: timestep.last() */
+  float* next_obs;       /* [L][E][obs_dim] */
+  float* tree;           /* stx_prio_tree_floats(E L) floats, zero-initialised */
+  int64_t* state;        /* device int64[2] = {write index, min(rows written, L)}, zero-initialised */
+  float* max_priority;   /* device float[1]: max_recorded_priority, 1.0 initially */
+  int64_t length;        /* L = max_length_time_axis */
+  int32_t envs;          /* E = add_batch_size */
+  int32_t obs_dim;
+  int32_t n_step;        /* sample_sequence_length */
+  float priority_exponent;
+  int32_t* owner;        /* [E L] int32, -1 between calls: set_priorities' claim of each leaf */
+} StxReplayPrioritised;
+int64_t stx_prio_tree_floats(int64_t items);
+size_t stx_prio_scratch_bytes(void);
+int stx_replay_add_prioritised(const StxReplayPrioritised* rb, const float* obs, const int32_t* action, const float* reward, const uint8_t* done,
+                               const float* next_obs, int T, void* stream);
+int stx_replay_sample_prioritised(const StxReplayPrioritised* rb, int64_t M, uint64_t seed, uint64_t offset, const uint64_t* dev_counter,
+                                  const float* u_in, const int32_t* count, float beta0, float beta_steps, float gamma, float* obs, float* next_obs,
+                                  int32_t* action, float* reward, uint8_t* done, int32_t* idx_out, float* prob_out, float* weight_out, void* scratch,
+                                  void* stream);
+int stx_replay_set_priorities(const StxReplayPrioritised* rb, const int32_t* idx, const float* priorities, int64_t M, void* stream);
+
 /* Utility casts used by the bf16 path (obs / weight shadows). */
 int stx_cast_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream);
 

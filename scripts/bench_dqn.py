@@ -1,12 +1,13 @@
 """DQN-family update-step timing: env steps/s and optimiser steps/s of the captured update step of ff_dqn, ff_ddqn, ff_mdqn,
-ff_dqn_reg, ff_c51 and ff_qr_dqn at two shapes, the systems alternated within each of three rounds, min-max over the rounds; plus the kernels of one
+ff_dqn_reg, ff_c51, ff_qr_dqn and ff_rainbow at two shapes, the systems alternated within each of three rounds, min-max over the rounds; plus the kernels of one
 eager update: stx_launch_count (the project's launches that go through STX_LAUNCH_OK, which leaves out the SIMT GEMMs of the MLP
 forward and backward) and every kernel the profiler records, GEMMs counted apart.  The card name and power limit are read in the same call.
 
-    python scripts/bench_dqn.py [--updates 50] [--rounds 3]
+    python scripts/bench_dqn.py [--updates 50] [--rounds 3] [--systems ff_c51,ff_rainbow]
 
-Shapes (every system runs the same schedule, so that they differ only in the head and the loss; ff_c51 and ff_qr_dqn keep their
-own heads, 51 atoms and 200 quantiles per action):
+Shapes (every system runs the same schedule, so that they differ only in the network, the head, the loss and the buffer; ff_c51 and
+ff_qr_dqn keep their own heads, 51 atoms and 200 quantiles per action; ff_rainbow its noisy dueling C51 network, 256 -> 2 x 512 branches,
+and its prioritised 5-step ring):
   "default" = the reference's ff_dqn default: CartPole, 1024 envs, T = 2, 16 epochs of batch 512, silu MLP 2 x 256;
   "wide"    = the synthetic Box, obs 64, A = 8, 1024 envs, T = 2, 16 epochs of batch 4096, same network.
 Prints one JSON line per (round, shape, system), then one summary line per (shape, system)."""
@@ -19,7 +20,8 @@ import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 
-SYSTEMS = ("ff_dqn", "ff_ddqn", "ff_mdqn", "ff_dqn_reg", "ff_c51", "ff_qr_dqn")
+SYSTEMS = ("ff_dqn", "ff_ddqn", "ff_mdqn", "ff_dqn_reg", "ff_c51", "ff_qr_dqn", "ff_rainbow")
+NET_KEYS = {"ff_rainbow": 3}   # (key, network key, noise key); the others take (key, network key)
 COMMON = ["arch.total_num_envs=1024", "system.rollout_length=2", "system.epochs=16", "system.total_buffer_size=1000000", "system.warmup_steps=16",
           "logger.use_console=False", "arch.num_evaluation=1"]
 SHAPES = {
@@ -51,7 +53,7 @@ def _setup(system: str, shape: str, updates: int):
     cfg.num_devices, cfg.rank = 1, 0
     cfg = check_total_timesteps(cfg, quiet=True)
     env, _ = environments.make(cfg)
-    learn, _, state = mod.learner_setup(env, tuple(srandom.split(srandom.PRNGKey(0), 2)), cfg)
+    learn, _, state = mod.learner_setup(env, tuple(srandom.split(srandom.PRNGKey(0), NET_KEYS.get(system, 2))), cfg)
     return cfg, learn, state
 
 
@@ -107,13 +109,14 @@ def main():
     ap.add_argument("--updates", type=int, default=50)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--shapes", default="default,wide")
+    ap.add_argument("--systems", default=",".join(SYSTEMS))
     a = ap.parse_args()
     torch.cuda.set_device(0)
     card = _card()
     seen = {}
     for r in range(a.rounds):
         for shape in a.shapes.split(","):
-            for system in SYSTEMS:          # alternate the systems within each round
+            for system in a.systems.split(","):   # alternate the systems within each round
                 res = run(system, shape, a.updates)
                 seen.setdefault((shape, system), []).append(res)
                 print(json.dumps({"round": r, **res, **card}), flush=True)

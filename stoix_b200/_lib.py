@@ -150,6 +150,50 @@ class StxDistQHyper(C.Structure):
     ]
 
 
+STX_NOISY_MAX_LAYERS = 8
+STX_PRIO_FANOUT = 32
+
+
+class StxNoisyLayer(C.Structure):
+    _fields_ = [
+        ("param", C.c_int64),
+        ("eff_w", C.c_int64),
+        ("eff_b", C.c_int64),
+        ("noise", C.c_int64),
+        ("in_", C.c_int32),
+        ("out", C.c_int32),
+        ("ld", C.c_int32),
+        ("reserved", C.c_int32),
+    ]
+
+
+class StxNoisyNet(C.Structure):
+    _fields_ = [
+        ("layers", StxNoisyLayer * STX_NOISY_MAX_LAYERS),
+        ("n_layers", C.c_int32),
+        ("reserved", C.c_int32),
+    ]
+
+
+class StxReplayPrioritised(C.Structure):
+    _fields_ = [
+        ("obs", C.c_void_p),
+        ("action", C.c_void_p),
+        ("reward", C.c_void_p),
+        ("done", C.c_void_p),
+        ("next_obs", C.c_void_p),
+        ("tree", C.c_void_p),
+        ("state", C.c_void_p),
+        ("max_priority", C.c_void_p),
+        ("length", C.c_int64),
+        ("envs", C.c_int32),
+        ("obs_dim", C.c_int32),
+        ("n_step", C.c_int32),
+        ("priority_exponent", C.c_float),
+        ("owner", C.c_void_p),
+    ]
+
+
 class StxPpoBatch(C.Structure):
     _fields_ = [
         ("obs", C.c_void_p),
@@ -294,6 +338,18 @@ _SIGNATURES = {
                                                C.POINTER(StxDistQHyper), _P, _P, _P, C.c_float, _P, _P]),
     "stx_quantile_q_loss_grads": (C.c_int, [_P, _P, _P, _P, C.c_int64, _P, _P, _P, _P, C.c_int64, C.c_int, C.c_int, C.POINTER(StxDistQHyper), _P,
                                             _P, _P, C.c_float, _P, _P]),
+    "stx_categorical_q_loss_grads_weighted": (C.c_int, [_P, _P, _P, _P, C.c_int64, _P, C.c_int64, _P, _P, _P, _P, _P, C.c_int64, C.c_int, C.c_int,
+                                                        C.POINTER(StxDistQHyper), _P, _P, _P, C.c_float, _P, _P]),
+    "stx_noisy_weights": (C.c_int, [C.POINTER(StxNoisyNet), _P, _P, _P, C.c_int, C.c_uint64, C.c_uint64, _P, _P]),
+    "stx_noisy_fold": (C.c_int, [C.POINTER(StxNoisyNet), _P, _P, _P, C.c_int, _P]),
+    "stx_dueling_combine": (C.c_int, [_P, C.c_int64, C.c_int, C.c_int, _P, _P]),
+    "stx_dueling_backward": (C.c_int, [_P, C.c_int64, C.c_int, C.c_int, _P, _P]),
+    "stx_prio_tree_floats": (C.c_int64, [C.c_int64]),
+    "stx_prio_scratch_bytes": (C.c_size_t, []),
+    "stx_replay_add_prioritised": (C.c_int, [C.POINTER(StxReplayPrioritised), _P, _P, _P, _P, _P, C.c_int, _P]),
+    "stx_replay_sample_prioritised": (C.c_int, [C.POINTER(StxReplayPrioritised), C.c_int64, C.c_uint64, C.c_uint64, _P, _P, _P, C.c_float, C.c_float,
+                                                C.c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "stx_replay_set_priorities": (C.c_int, [C.POINTER(StxReplayPrioritised), _P, _P, C.c_int64, _P]),
 }
 
 _lib = None

@@ -87,13 +87,14 @@ __device__ __forceinline__ void zero_other_actions(float* __restrict__ row, int 
 }
 
 // ---- C51: categorical_double_q_learning.  Shared memory per row: clipped target atoms zp (N), target probabilities p (N), the
-// projected target t (N, each entry touched by its owner only).
-template <int TPR>
+// projected target t (N, each entry touched by its owner only).  WEIGHTED (Rainbow): row m's gradient is scaled by w[m] and its
+// metric term is w[m] loss; the unweighted instantiation is the kernel ff_c51 runs.
+template <int TPR, bool WEIGHTED>
 __global__ void __launch_bounds__(kDistThreads) categorical_q_loss_kernel(
     LossRows rows, const float* __restrict__ logits_tm1, const float* __restrict__ logits_t, const float* __restrict__ q_sel,
     const float* __restrict__ atoms_tm1, int64_t ld_tm1, const float* __restrict__ atoms_t, int64_t ld_t, const int32_t* __restrict__ action,
-    const float* __restrict__ reward, const uint8_t* __restrict__ done, const float* __restrict__ discount, int A, int N, StxDistQHyper h,
-    float* __restrict__ d_logits, float* __restrict__ loss_rows) {
+    const float* __restrict__ reward, const uint8_t* __restrict__ done, const float* __restrict__ discount, const float* __restrict__ row_w, int A,
+    int N, StxDistQHyper h, float* __restrict__ d_logits, float* __restrict__ loss_rows) {
   extern __shared__ float smem[];
   __shared__ float red[kDistThreads / 32];
   const int lane = threadIdx.x % TPR;
@@ -166,14 +167,18 @@ __global__ void __launch_bounds__(kDistThreads) categorical_q_loss_kernel(
   for (int k = lane; k < N; k += TPR) {
     const float sh = la[k] - lm;
     ce += t[k] * (sh - lse);
-    if (w.live) d_logits[w.m * W + (int64_t)a * N + k] = ((expf(sh) / sa) * st - t[k]) * inv_m;
+    if (w.live) {
+      const float g = ((expf(sh) / sa) * st - t[k]) * inv_m;
+      d_logits[w.m * W + (int64_t)a * N + k] = WEIGHTED ? __fmul_rn(g, row_w[w.mm]) : g;
+    }
   }
   const float loss = -row_reduce<TPR, false>(ce, red);
   if (w.live) {
     zero_other_actions(d_logits + w.m * W, a, A, N, lane, TPR);
     if (loss_rows && lane == 0) loss_rows[w.m] = loss;
   }
-  reduce_metrics<1>({(w.live && lane == 0) ? (double)loss : 0.0}, {0}, rows);
+  const float term = WEIGHTED ? __fmul_rn(row_w[w.mm], loss) : loss;
+  reduce_metrics<1>({(w.live && lane == 0) ? (double)term : 0.0}, {0}, rows);
 }
 
 // ---- QR-DQN: quantile_q_learning.  Shared memory per row: the target quantiles (N) and the selector means (A).
@@ -266,12 +271,12 @@ extern "C" int stx_dist_q_values(int kind, const float* head, int64_t M, int A, 
   return STX_OK;
 }
 
-extern "C" int stx_categorical_q_loss_grads(const float* logits_tm1, const float* logits_t, const float* q_sel, const float* atoms_tm1,
-                                            int64_t ld_atoms_tm1, const float* atoms_t, int64_t ld_atoms_t, const int32_t* action,
-                                            const float* reward, const uint8_t* done, const float* discount, int64_t M, int A, int N,
-                                            const StxDistQHyper* hyper, float* d_logits, float* loss_rows, float* metrics, float weight,
-                                            void* scratch, void* stream) {
-  const char* who = "stx_categorical_q_loss_grads";
+namespace stx {
+namespace {
+int categorical_loss(const float* logits_tm1, const float* logits_t, const float* q_sel, const float* atoms_tm1, int64_t ld_atoms_tm1,
+                     const float* atoms_t, int64_t ld_atoms_t, const int32_t* action, const float* reward, const uint8_t* done, const float* discount,
+                     const float* row_w, int64_t M, int A, int N, const StxDistQHyper* hyper, float* d_logits, float* loss_rows, float* metrics,
+                     float weight, void* scratch, void* stream, const char* who) {
   const int tpr = dist_tpr(N);
   const size_t smem = (size_t)(kDistThreads / tpr) * 3 * (size_t)N * sizeof(float);
   if (int rc = check_loss_args(logits_tm1, logits_t, q_sel, action, reward, done, discount, M, A, N, hyper, d_logits, metrics, scratch, smem, who))
@@ -281,18 +286,45 @@ extern "C" int stx_categorical_q_loss_grads(const float* logits_tm1, const float
   const unsigned grid = (unsigned)((M + kDistThreads / tpr - 1) / (kDistThreads / tpr));
   cudaStream_t st = (cudaStream_t)stream;
   const StxDistQHyper h = *hyper;
-#define STX_C51(T)                                                                                                                         \
-  categorical_q_loss_kernel<T><<<grid, kDistThreads, smem, st>>>(r, logits_tm1, logits_t, q_sel, atoms_tm1, ld_atoms_tm1, atoms_t, ld_atoms_t, \
-                                                                 action, reward, done, discount, A, N, h, d_logits, loss_rows)
-  switch (tpr) {
-    case 32: STX_C51(32); break;
-    case 64: STX_C51(64); break;
-    case 128: STX_C51(128); break;
-    default: STX_C51(256); break;
+#define STX_C51(T, WT)                                                                                                                       \
+  categorical_q_loss_kernel<T, WT><<<grid, kDistThreads, smem, st>>>(r, logits_tm1, logits_t, q_sel, atoms_tm1, ld_atoms_tm1, atoms_t, ld_atoms_t, \
+                                                                     action, reward, done, discount, row_w, A, N, h, d_logits, loss_rows)
+#define STX_C51_TPR(WT)            \
+  switch (tpr) {                   \
+    case 32: STX_C51(32, WT); break;   \
+    case 64: STX_C51(64, WT); break;   \
+    case 128: STX_C51(128, WT); break; \
+    default: STX_C51(256, WT); break;  \
   }
+  if (row_w) {
+    STX_C51_TPR(true)
+  } else {
+    STX_C51_TPR(false)
+  }
+#undef STX_C51_TPR
 #undef STX_C51
   STX_LAUNCH_OK();
   return STX_OK;
+}
+}  // namespace
+}  // namespace stx
+
+extern "C" int stx_categorical_q_loss_grads(const float* logits_tm1, const float* logits_t, const float* q_sel, const float* atoms_tm1,
+                                            int64_t ld_atoms_tm1, const float* atoms_t, int64_t ld_atoms_t, const int32_t* action,
+                                            const float* reward, const uint8_t* done, const float* discount, int64_t M, int A, int N,
+                                            const StxDistQHyper* hyper, float* d_logits, float* loss_rows, float* metrics, float weight,
+                                            void* scratch, void* stream) {
+  return categorical_loss(logits_tm1, logits_t, q_sel, atoms_tm1, ld_atoms_tm1, atoms_t, ld_atoms_t, action, reward, done, discount, nullptr, M, A, N,
+                          hyper, d_logits, loss_rows, metrics, weight, scratch, stream, "stx_categorical_q_loss_grads");
+}
+
+extern "C" int stx_categorical_q_loss_grads_weighted(const float* logits_tm1, const float* logits_t, const float* q_sel, const float* atoms_tm1,
+                                                     int64_t ld_atoms_tm1, const float* atoms_t, int64_t ld_atoms_t, const int32_t* action,
+                                                     const float* reward, const uint8_t* done, const float* discount, const float* w, int64_t M, int A,
+                                                     int N, const StxDistQHyper* hyper, float* d_logits, float* loss_rows, float* metrics, float weight,
+                                                     void* scratch, void* stream) {
+  return categorical_loss(logits_tm1, logits_t, q_sel, atoms_tm1, ld_atoms_tm1, atoms_t, ld_atoms_t, action, reward, done, discount, w, M, A, N, hyper,
+                          d_logits, loss_rows, metrics, weight, scratch, stream, "stx_categorical_q_loss_grads_weighted");
 }
 
 extern "C" int stx_quantile_q_loss_grads(const float* q_tm1, const float* q_t, const float* q_sel, const float* tau, int64_t ld_tau,

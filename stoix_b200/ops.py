@@ -1414,11 +1414,13 @@ def _dist_rows(who: str, ref: torch.Tensor, M: int, W: int, mats, rows, per_row,
 def categorical_q_loss_grads(logits_tm1: torch.Tensor, logits_t: torch.Tensor, q_sel: torch.Tensor, atoms_tm1: torch.Tensor, atoms_t: torch.Tensor,
                              action: torch.Tensor, reward: torch.Tensor, hyper: _lib.StxDistQHyper, d_logits: torch.Tensor, metrics: torch.Tensor,
                              done: Optional[torch.Tensor] = None, discount: Optional[torch.Tensor] = None,
-                             loss_rows: Optional[torch.Tensor] = None, weight: float = 1.0, scratch_key: str = "c51_loss") -> None:
+                             loss_rows: Optional[torch.Tensor] = None, weight: float = 1.0, scratch_key: str = "c51_loss",
+                             row_weight: Optional[torch.Tensor] = None) -> None:
     """categorical_double_q_learning under jax.grad (stx_categorical_q_loss_grads): logits (M, A N), q_sel (M, A) the selector's
     expected Q, atoms (N) or (M, N).  d mean(loss) / d logits_tm1 into d_logits, metrics[0] += weight mean(loss), the per-row loss
-    into loss_rows (M) when given.  The discount is (1 - done) gamma, or `discount` (M) given directly."""
-    dev = _need_cuda(logits_tm1, logits_t, q_sel, atoms_tm1, atoms_t, action, reward, done, discount, d_logits, metrics, loss_rows)
+    into loss_rows (M) when given.  The discount is (1 - done) gamma, or `discount` (M) given directly.  row_weight (M): Rainbow's
+    importance weights (stx_categorical_q_loss_grads_weighted): the loss is mean(w loss); loss_rows stays unweighted."""
+    dev = _need_cuda(logits_tm1, logits_t, q_sel, atoms_tm1, atoms_t, action, reward, done, discount, d_logits, metrics, loss_rows, row_weight)
     if q_sel.ndim != 2 or logits_tm1.ndim != 2:
         raise StxError("categorical_q_loss_grads: logits must be (M, A N) and q_sel (M, A)")
     M, A = q_sel.shape
@@ -1427,14 +1429,22 @@ def categorical_q_loss_grads(logits_tm1: torch.Tensor, logits_t: torch.Tensor, q
         raise StxError(f"categorical_q_loss_grads: logits_tm1 has {logits_tm1.shape[1]} columns, not A N = {A} x {N}")
     ld = _dist_rows("categorical_q_loss_grads", logits_tm1, M, A * N, ((logits_tm1, "logits_tm1"), (logits_t, "logits_t"), (d_logits, "d_logits")),
                     ((action, torch.int32, "action"), (reward, torch.float32, "reward"), (discount, torch.float32, "discount"),
-                     (None if done is None else _u8(done), torch.uint8, "done"), (loss_rows, torch.float32, "loss_rows")),
+                     (None if done is None else _u8(done), torch.uint8, "done"), (loss_rows, torch.float32, "loss_rows"),
+                     (row_weight, torch.float32, "row_weight")),
                     ((atoms_tm1, "atoms_tm1"), (atoms_t, "atoms_t")), N)
     _dist_rows("categorical_q_loss_grads", q_sel, M, A, ((q_sel, "q_sel"),), (), (), N)
     lib = _lib.load()
     scratch = _zeros_scratch((scratch_key,), lib.stx_dist_q_scratch_bytes(M), dev)
-    _lib.check(lib.stx_categorical_q_loss_grads(_p(logits_tm1), _p(logits_t), _p(q_sel), _p(atoms_tm1), ld[0], _p(atoms_t), ld[1], _p(action), _p(reward),
-                                                _p(None if done is None else _u8(done)), _p(discount), M, A, N, C.byref(hyper), _p(d_logits),
-                                                _p(loss_rows), _p(metrics), float(weight), _p(scratch), _stream()), "stx_categorical_q_loss_grads")
+    d8 = None if done is None else _u8(done)
+    if row_weight is None:
+        _lib.check(lib.stx_categorical_q_loss_grads(_p(logits_tm1), _p(logits_t), _p(q_sel), _p(atoms_tm1), ld[0], _p(atoms_t), ld[1], _p(action),
+                                                    _p(reward), _p(d8), _p(discount), M, A, N, C.byref(hyper), _p(d_logits), _p(loss_rows),
+                                                    _p(metrics), float(weight), _p(scratch), _stream()), "stx_categorical_q_loss_grads")
+    else:
+        _lib.check(lib.stx_categorical_q_loss_grads_weighted(_p(logits_tm1), _p(logits_t), _p(q_sel), _p(atoms_tm1), ld[0], _p(atoms_t), ld[1],
+                                                             _p(action), _p(reward), _p(d8), _p(discount), _p(row_weight), M, A, N, C.byref(hyper),
+                                                             _p(d_logits), _p(loss_rows), _p(metrics), float(weight), _p(scratch), _stream()),
+                   "stx_categorical_q_loss_grads_weighted")
 
 
 def quantile_q_loss_grads(q_tm1: torch.Tensor, q_t: torch.Tensor, tau: torch.Tensor, action: torch.Tensor, reward: torch.Tensor,
@@ -1458,3 +1468,146 @@ def quantile_q_loss_grads(q_tm1: torch.Tensor, q_t: torch.Tensor, tau: torch.Ten
     _lib.check(lib.stx_quantile_q_loss_grads(_p(q_tm1), _p(q_t), _p(q_sel), _p(tau), ld, _p(action), _p(reward), _p(None if done is None else _u8(done)),
                                              _p(discount), M, int(A), N, C.byref(hyper), _p(d_q), _p(loss_rows), _p(metrics), float(weight),
                                              _p(scratch), _stream()), "stx_quantile_q_loss_grads")
+
+
+# ------------------------------------------------------------------------------------------------
+# Rainbow: noisy layers, dueling combine, prioritised n-step ring (stoix/networks/layers.py:71-169, dueling.py:90-124,
+# stoix/systems/q_learning/ff_rainbow.py)
+# ------------------------------------------------------------------------------------------------
+
+
+def noisy_net_struct(layers: Sequence[Tuple[int, int, int, int, int, int, int]]) -> _lib.StxNoisyNet:
+    """StxNoisyNet of (param, eff_w, eff_b, noise, in, out, ld) per noisy layer."""
+    if not 1 <= len(layers) <= _lib.STX_NOISY_MAX_LAYERS:
+        raise StxError(f"noisy network with {len(layers)} layers unsupported (1 .. {_lib.STX_NOISY_MAX_LAYERS})")
+    net = _lib.StxNoisyNet()
+    net.n_layers = len(layers)
+    for i, (param, eff_w, eff_b, noise, n_in, n_out, ld) in enumerate(layers):
+        net.layers[i] = _lib.StxNoisyLayer(int(param), int(eff_w), int(eff_b), int(noise), int(n_in), int(n_out), int(ld), 0)
+    return net
+
+
+def _f32(t: torch.Tensor, n: int, name: str, who: str) -> None:
+    if t.dtype != torch.float32 or not t.is_contiguous() or t.numel() < n:
+        raise StxError(f"{who}: {name} must be contiguous float32 with at least {n} elements")
+
+
+def noisy_weights(net: _lib.StxNoisyNet, params: torch.Tensor, eff: torch.Tensor, noise: torch.Tensor, seed: int = 0, offset: int = 0,
+                  dev_counter: Optional[torch.Tensor] = None, draw: bool = True, sizes: Tuple[int, int, int] = (0, 0, 0)) -> None:
+    """Effective weights mu + sigma o eps of every noisy layer into the dense arena `eff` (stx_noisy_weights).  draw: fresh noise from
+    Philox (seed, call = offset + *dev_counter) written into `noise`; else `noise` is the input.  sizes = the floats the parameter
+    arena, the effective arena and the noise buffer must hold."""
+    _need_cuda(params, eff, noise, dev_counter)
+    for t, n, name in ((params, sizes[0], "params"), (eff, sizes[1], "eff"), (noise, sizes[2], "noise")):
+        _f32(t, n, name, "noisy_weights")
+    _lib.check(_lib.load().stx_noisy_weights(C.byref(net), _p(params), _p(eff), _p(noise), int(bool(draw)), int(seed) & (2**64 - 1), int(offset),
+                                             _p(dev_counter), _stream()), "stx_noisy_weights")
+
+
+def noisy_fold(net: _lib.StxNoisyNet, eff_grad: torch.Tensor, noise: torch.Tensor, grad: torch.Tensor, overwrite: bool = True,
+               sizes: Tuple[int, int, int] = (0, 0, 0)) -> None:
+    """d mu = g_eff, d sigma = g_eff o eps into the parameter-layout `grad` (stx_noisy_fold); overwrite or add."""
+    _need_cuda(eff_grad, noise, grad)
+    for t, n, name in ((grad, sizes[0], "grad"), (eff_grad, sizes[1], "eff_grad"), (noise, sizes[2], "noise")):
+        _f32(t, n, name, "noisy_fold")
+    _lib.check(_lib.load().stx_noisy_fold(C.byref(net), _p(eff_grad), _p(noise), _p(grad), int(bool(overwrite)), _stream()), "stx_noisy_fold")
+
+
+def _dueling_io(who: str, x: torch.Tensor, cols_in: int, out: Optional[torch.Tensor], cols_out: int) -> torch.Tensor:
+    _need_cuda(x, out)
+    if x.dtype != torch.float32 or x.ndim != 2 or x.shape[1] != cols_in or not x.is_contiguous():
+        raise StxError(f"{who}: input must be contiguous float32 (M, {cols_in})")
+    if out is None:
+        return torch.empty(x.shape[0], cols_out, dtype=torch.float32, device=x.device)
+    if out.dtype != torch.float32 or tuple(out.shape) != (x.shape[0], cols_out) or not out.is_contiguous():
+        raise StxError(f"{who}: out must be contiguous float32 ({x.shape[0]}, {cols_out})")
+    return out
+
+
+def dueling_combine(head: torch.Tensor, A: int, N: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """(v | adv) head rows (M, N + A N) -> q_logits (M, A N): v + adv - mean_a adv (stx_dueling_combine)."""
+    out = _dueling_io("dueling_combine", head, N + A * N, out, A * N)
+    _lib.check(_lib.load().stx_dueling_combine(_p(head), head.shape[0], int(A), int(N), _p(out), _stream()), "stx_dueling_combine")
+    return out
+
+
+def dueling_backward(d_q_logits: torch.Tensor, A: int, N: int, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """d q_logits (M, A N) -> d (v | adv) (M, N + A N) (stx_dueling_backward)."""
+    out = _dueling_io("dueling_backward", d_q_logits, A * N, out, N + A * N)
+    _lib.check(_lib.load().stx_dueling_backward(_p(d_q_logits), d_q_logits.shape[0], int(A), int(N), _p(out), _stream()), "stx_dueling_backward")
+    return out
+
+
+class PrioritisedRing:
+    """Device storage + StxReplayPrioritised descriptor of the prioritised n-step trajectory ring: L time rows of E envs, the sum
+    tree over its E L items, {write index, rows written}, max_recorded_priority (1.0 initially) and set_priorities' leaf claims."""
+
+    def __init__(self, length: int, envs: int, obs_dim: int, n_step: int, priority_exponent: float, device):
+        self.length, self.envs, self.obs_dim, self.n_step = int(length), int(envs), int(obs_dim), int(n_step)
+        self.priority_exponent = float(priority_exponent)
+        if not 1 <= self.n_step <= self.length or self.envs * self.length >= 2**31:
+            raise StxError(f"PrioritisedRing: n_step {n_step} must be in [1, length {length}] and envs x length < 2^31")
+        z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=device)
+        L, E = self.length, self.envs
+        self.obs, self.next_obs = z(L, E, self.obs_dim), z(L, E, self.obs_dim)
+        self.action, self.reward, self.done = z(L, E, dt=torch.int32), z(L, E), z(L, E, dt=torch.uint8)
+        self.tree = z(int(_lib.load().stx_prio_tree_floats(E * L)))
+        self.state = z(2, dt=torch.int64)
+        self.max_priority = torch.ones(1, dtype=torch.float32, device=device)
+        self.scratch = z(int(_lib.load().stx_prio_scratch_bytes()), dt=torch.uint8)
+        self.owner = torch.full((E * L,), -1, dtype=torch.int32, device=device)
+        self.c = _lib.StxReplayPrioritised(_p(self.obs), _p(self.action), _p(self.reward), _p(self.done), _p(self.next_obs), _p(self.tree),
+                                           _p(self.state), _p(self.max_priority), L, E, self.obs_dim, self.n_step, self.priority_exponent,
+                                           _p(self.owner))
+
+    @property
+    def priorities(self) -> torch.Tensor:
+        """The (E L) leaf priorities, item i = e L + p."""
+        return self.tree[: self.envs * self.length]
+
+
+def replay_add_prioritised(rb: PrioritisedRing, obs, action, reward, done, next_obs) -> None:
+    """Append T time rows of a (T, E, ...) batch (obs / next_obs / reward fp32, action int32, done uint8 / bool)."""
+    _need_cuda(obs, action, reward, done, next_obs)
+    if reward.ndim != 2 or reward.shape[1] != rb.envs:
+        raise StxError(f"replay_add_prioritised: reward must be (T, {rb.envs})")
+    T = int(reward.shape[0])
+    n = T * rb.envs
+    for t, cols, dt, name in ((obs, rb.obs_dim, torch.float32, "obs"), (next_obs, rb.obs_dim, torch.float32, "next_obs"),
+                              (reward, 1, torch.float32, "reward"), (action, 1, torch.int32, "action"), (_u8(done), 1, torch.uint8, "done")):
+        if t.dtype != dt or not t.is_contiguous() or t.numel() != n * cols:
+            raise StxError(f"replay_add_prioritised: {name} must be contiguous {dt} with {n} x {cols} elements")
+    _lib.check(_lib.load().stx_replay_add_prioritised(C.byref(rb.c), _p(obs), _p(action), _p(reward), _p(_u8(done)), _p(next_obs), T, _stream()),
+               "stx_replay_add_prioritised")
+
+
+def replay_sample_prioritised(rb: PrioritisedRing, M: int, seed: int, obs: torch.Tensor, next_obs: torch.Tensor, action: torch.Tensor,
+                              reward: torch.Tensor, done: torch.Tensor, idx: torch.Tensor, prob: torch.Tensor, weight: torch.Tensor, gamma: float,
+                              beta0: float, beta_steps: float, count: Optional[torch.Tensor] = None, offset: int = 0,
+                              dev_counter: Optional[torch.Tensor] = None, u_in: Optional[torch.Tensor] = None) -> None:
+    """One launch: M stratified proportional draws (or u_in (M) as the uniforms), the n-step rows of each into obs, next_obs (M, D),
+    action, reward, done, the item indices, p_i and the normalised importance weights (beta from the int32 Adam count word)."""
+    _need_cuda(obs, next_obs, action, reward, done, idx, prob, weight, count, dev_counter, u_in)
+    M = int(M)
+    for t, cols, dt, name in ((obs, rb.obs_dim, torch.float32, "obs"), (next_obs, rb.obs_dim, torch.float32, "next_obs"),
+                              (reward, 1, torch.float32, "reward"), (action, 1, torch.int32, "action"), (_u8(done), 1, torch.uint8, "done"),
+                              (idx, 1, torch.int32, "idx"), (prob, 1, torch.float32, "prob"), (weight, 1, torch.float32, "weight"),
+                              (u_in, 1, torch.float32, "u_in")):
+        if t is not None and (t.dtype != dt or not t.is_contiguous() or t.numel() != M * cols):
+            raise StxError(f"replay_sample_prioritised: {name} must be contiguous {dt} with {M} x {cols} elements")
+    if count is not None and count.dtype != torch.int32:
+        raise StxError("replay_sample_prioritised: count must be the int32 Adam count word")
+    _lib.check(_lib.load().stx_replay_sample_prioritised(C.byref(rb.c), M, int(seed) & (2**64 - 1), int(offset), _p(dev_counter), _p(u_in), _p(count),
+                                                         float(beta0), float(beta_steps), float(gamma), _p(obs), _p(next_obs), _p(action),
+                                                         _p(reward), _p(_u8(done)), _p(idx), _p(prob), _p(weight), _p(rb.scratch), _stream()),
+               "stx_replay_sample_prioritised")
+
+
+def replay_set_priorities(rb: PrioritisedRing, idx: torch.Tensor, priorities: torch.Tensor) -> None:
+    """leaf[idx[m]] = priorities[m] ** priority_exponent (the last of duplicate indices wins), ancestors rebuilt, max raised.  The
+    indices must lie in [0, E L) (the sampler's); they are not checked on the device."""
+    _need_cuda(idx, priorities)
+    M = int(idx.numel())
+    if idx.dtype != torch.int32 or priorities.dtype != torch.float32 or priorities.numel() != M or not idx.is_contiguous() or not priorities.is_contiguous():
+        raise StxError("replay_set_priorities: idx (M) int32 and priorities (M) float32, contiguous")
+    _lib.check(_lib.load().stx_replay_set_priorities(C.byref(rb.c), _p(idx), _p(priorities), M, _stream()), "stx_replay_set_priorities")

@@ -63,3 +63,39 @@ class DiscreteTransitionBuffer:
         ops.replay_sample_discrete(self.ring, self.sample_batch_size, self.seed, obs, next_obs, action, reward, done,
                                    dev_counter=self.counter.view(torch.int64), idx_in=idx_in, idx_out=idx_out)
         ops.counter_add(self.counter, 1)
+
+
+class PrioritisedTrajectoryBuffer:
+    """fbx.make_prioritised_trajectory_buffer as ff_rainbow.py:433-442 builds it, on the prioritised n-step ring
+    (stx_replay_add_prioritised / _sample_prioritised / stx_replay_set_priorities): add_batch_size = E envs, max_length_time_axis =
+    max_size // E time rows, sequences of n_step rows with period 1.  `sample_into` draws sample_batch_size items in proportion to
+    their priorities and writes each as its n-step transition (ff_rainbow.py:222-246) with p_i and the importance weight."""
+
+    def __init__(self, max_size: int, n_step: int, sample_batch_size: int, add_batch_size: int, priority_exponent: float, obs_dim: int, device,
+                 seed: int = 0):
+        self.max_length_time_axis = int(max_size) // int(add_batch_size)
+        self.n_step, self.sample_batch_size, self.add_batch_size = int(n_step), int(sample_batch_size), int(add_batch_size)
+        self.ring = ops.PrioritisedRing(self.max_length_time_axis, self.add_batch_size, obs_dim, self.n_step, priority_exponent, device)
+        self.seed = int(seed) & ((1 << 62) - 1)
+        self.counter = torch.zeros(1, dtype=torch.int64, device=device)   # sample calls so far (device-resident RNG stream position)
+        self.added = 0                                                    # host mirror of the items added (T E per add)
+
+    def add(self, transition) -> None:
+        """transition: .obs (T, E, D), .action (T, E) int32, .reward, .done (T, E), .next_obs, time-major."""
+        ops.replay_add_prioritised(self.ring, transition.obs, transition.action, transition.reward, transition.done, transition.next_obs)
+        self.added += int(transition.reward.numel())
+
+    def can_sample(self) -> bool:
+        """min_length_time_axis = n_step time rows written."""
+        return self.added // self.add_batch_size >= self.n_step
+
+    def sample_into(self, obs, next_obs, action, reward, done, idx, prob, weight, gamma: float, beta0: float, beta_steps: float,
+                    count: Optional[torch.Tensor] = None, u_in: Optional[torch.Tensor] = None) -> None:
+        """Draw one batch into the given (M, ...) buffers; advances the stream position.  obs and next_obs may be the two halves of
+        one (2M, D) block."""
+        ops.replay_sample_prioritised(self.ring, self.sample_batch_size, self.seed, obs, next_obs, action, reward, done, idx, prob, weight, gamma,
+                                      beta0, beta_steps, count=count, dev_counter=self.counter.view(torch.int64), u_in=u_in)
+        ops.counter_add(self.counter, 1)
+
+    def set_priorities(self, idx: torch.Tensor, priorities: torch.Tensor) -> None:
+        ops.replay_set_priorities(self.ring, idx, priorities)
