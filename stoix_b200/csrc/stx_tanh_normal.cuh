@@ -18,8 +18,16 @@ __device__ __forceinline__ float log_ndtrf(float z) {
   if (t < 3.f) return logf(0.5f * erfcf(t));
   return logf(0.5f * erfcxf(t)) - t * t;
 }
-// phi(z) / Phi(z)
-__device__ __forceinline__ float mills(float z) { return expf(-0.5f * z * z - kLogSqrt2Pi - log_ndtrf(z)); }
+// phi(z) / Phi(z).  Far in the left tail it is sqrt(2/pi) / erfcx(t), t = -z / sqrt 2, exactly.  The exp form below cancels
+// -z^2/2 against the -t^2 of log_ndtrf, so the rounding of t leaves a relative error that grows as 2^-24 z^2 (about 5e-5 at
+// z = -50, 5e-4 at z = -200, 6e-2 at z = -1500).  The switch sits at t = 64 (z = -90.5); below it the exp form is kept, so
+// every gradient whose z stays above -90.5 is unchanged bit for bit.
+constexpr float kMillsErfcxFrom = 64.f;
+__device__ __forceinline__ float mills(float z) {
+  const float t = -z * 0.70710678118654752f;
+  if (t < kMillsErfcxFrom) return expf(-0.5f * z * z - kLogSqrt2Pi - log_ndtrf(z));
+  return 0.7978845608028654f / erfcxf(t);
+}
 // forward log-det-Jacobian of tanh at x
 __device__ __forceinline__ float tanh_fldj(float x) { return 2.f * (0.6931471805599453f - x - softplusf(-2.f * x)); }
 
