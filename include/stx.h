@@ -170,7 +170,9 @@ void stx_tc_set_forward_ctas(int n);
  * buffer is left untouched.  Synchronous (not for capture). */
 int stx_tc_debug_set_clock_buffer(long long* buf);
 /* Profiling hook of the K3 launches: device buffer of [gridDim][8] int64 filled per CTA of K3a / K3b with
- * {role, total cycles, -, tiles (K3a) / -, -, chunks (K3b)} (see stx_tc_ppo.cu g_prof_buf); NULL disables. */
+ * K3a {1, total cycles, -, tiles, -, -, -, -} and, overwriting it, K3b {2 + job, total cycles, cycles before the end of
+ * griddepcontrol.wait, globaltimer (ns) after it, globaltimer at exit, chunks, -, -} (see stx_tc_ppo.cu g_prof_buf,
+ * scripts/k3b_jobs.py); NULL disables. */
 int stx_tc_debug_set_prof_buffer(long long* buf);
 
 /* Categorical head ops on logits (E, A) -- tfd.Categorical (stoix/networks/heads.py:41) as used at

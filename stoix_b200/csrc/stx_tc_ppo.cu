@@ -45,6 +45,12 @@ int make_map_tiled(CUtensorMap* m, const void* base, uint64_t tiles, uint32_t co
 __device__ long long* g_clock_buf = nullptr;
 __device__ long long* g_prof_buf = nullptr;
 
+__device__ __forceinline__ long long globaltimer_ns() {
+  long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
+
 constexpr int kH = 256;
 constexpr int kWTile = 64;               // rows per warpgroup tile
 constexpr int kFbThreads = 256;          // two warpgroups
@@ -603,7 +609,9 @@ __device__ __forceinline__ void dw1_consume(uint8_t* smem, uint64_t* img_full, u
 
 // dW1 operand rebuild (warpgroup 2): thread t plays K3a's thread t of the warpgroup that ran the chunk's 64-row tile.  Chunk k's
 // operands go to image buffer k % 2 while the consumers multiply chunk k - 1 out of the other buffer.  Thread 0 also keeps the
-// input ring full.
+// input ring full.  The MMAs of the rebuild and of the consumers share the SM's tensor cores in issue order: a rebuild GEMM issued
+// after the consumers have queued chunk k's 16 MMAs waits for all of them.  So chunk k + 1's first GEMM (x W0, the largest) is
+// issued before chunk k's image is signalled, and its epilogue runs while the consumers' MMAs do.
 __device__ __forceinline__ void dw1_rebuild(uint8_t* smem, uint64_t* full, uint64_t* img_full, uint64_t* img_empty, uint64_t* w_full,
                                             const CUtensorMap* map_x, const CUtensorMap* map_dz, const DwJob& job, int cta,
                                             int my_chunks, uint64_t pol_stream) {
@@ -625,7 +633,6 @@ __device__ __forceinline__ void dw1_rebuild(uint8_t* smem, uint64_t* full, uint6
   mbar_wait(w_full, 0, 24);
   for (int it = 0; it < my_chunks; ++it) {
     const int s = it % kDwStages, b = it & 1;
-    mbar_wait(&full[s], (it / kDwStages) & 1, 25);
     uint8_t* st = smem + s * kW1StageBytes;
     uint8_t* h1img = smem + kW1OffImg + b * kW1ImgBytes;
     uint8_t* dh2img = h1img + 16384;
@@ -633,7 +640,15 @@ __device__ __forceinline__ void dw1_rebuild(uint8_t* smem, uint64_t* full, uint6
     float acc[64];
     uint32_t a[64];
     // h1[:, m0 ..] = relu(x W0[:, m0 ..] + b0[m0 ..]): K3a's G0 / E0 with x K-major from the tiled layout ([colgroup][row][8])
-    gemm_x_w0_at(acc, wg_desc(smem_u32(st), 1024, 128, WG_INTERLEAVE), 2048, sbase + kW1OffW0, 0);
+    mbar_wait(&full[s], (it / kDwStages) & 1, 25);
+    wg_zero(acc);  // the first k-step does not accumulate, but the MMA still reads acc
+    gemm_x_w0_at_issue(acc, wg_desc(smem_u32(st), 1024, 128, WG_INTERLEAVE), 2048, sbase + kW1OffW0, 0);
+    if (it > 0) {  // chunk it - 1's image, signalled behind chunk it's first GEMM
+      mbar_arrive(&img_full[b ^ 1]);
+      wg_sync(3);  // every thread of this warpgroup is done with ring stage s - 1
+      if (t == 0 && it - 1 + kDwStages < my_chunks) load_chunk(it - 1 + kDwStages);
+    }
+    wg_wait_all(acc);
     epi_bias_relu(acc, s_b0, 0, a, lane);
     if (it >= 2) mbar_wait(&img_empty[b], ((it >> 1) - 1) & 1, 26);
 #pragma unroll
@@ -657,10 +672,8 @@ __device__ __forceinline__ void dw1_rebuild(uint8_t* smem, uint64_t* full, uint6
       }
     }
     fence_async_proxy();  // generic-proxy image stores -> visible to the consumers' wgmma
-    mbar_arrive(&img_full[b]);
-    wg_sync(3);  // every thread of this warpgroup is done with ring stage s
-    if (t == 0 && it + kDwStages < my_chunks) load_chunk(it + kDwStages);
   }
+  if (my_chunks > 0) mbar_arrive(&img_full[(my_chunks - 1) & 1]);
 }
 
 __global__ void __launch_bounds__(kDwThreads, 1) tc_dw_kernel(const __grid_constant__ DwMaps maps, const DwParams p) {
@@ -698,6 +711,11 @@ __global__ void __launch_bounds__(kDwThreads, 1) tc_dw_kernel(const __grid_const
   griddep_launch();
   __syncthreads();
   griddep_wait();  // the activations are K3a's output; the partials written below were read by the previous reduce
+  // (the profile record is K3a's until K3a has finished: only written from here on)
+  if (threadIdx.x == 0 && g_prof_buf != nullptr) {
+    long long* prof = g_prof_buf + (int64_t)blockIdx.x * 8;
+    prof[2] = clock64() - prof_t0, prof[3] = globaltimer_ns();
+  }
 
   const uint64_t pol_stream = l2_policy(p.act_policy);  // default evict_first: every activation tile is read exactly once
   if (job.rebuild) {
@@ -741,7 +759,7 @@ __global__ void __launch_bounds__(kDwThreads, 1) tc_dw_kernel(const __grid_const
   __syncthreads();
   if (g_prof_buf != nullptr && threadIdx.x == 0) {
     long long* prof = g_prof_buf + (int64_t)blockIdx.x * 8;
-    prof[0] = 2 + j, prof[1] = clock64() - prof_t0, prof[5] = my_chunks;
+    prof[0] = 2 + j, prof[1] = clock64() - prof_t0, prof[4] = globaltimer_ns(), prof[5] = my_chunks;
   }
 }
 
