@@ -798,6 +798,74 @@ int stx_replay_sample_prioritised(const StxReplayPrioritised* rb, int64_t M, uin
                                   void* stream);
 int stx_replay_set_priorities(const StxReplayPrioritised* rb, const int32_t* idx, const float* priorities, int64_t M, void* stream);
 
+/* ------------------------------------------------------------------ V-MPO (fp32): stoix/systems/mpo/ff_vmpo.py, ff_vmpo_continuous.py ----
+ * rlax.vmpo_loss (called at ff_vmpo.py:145-151, ff_vmpo_continuous.py:202-207) over the N = E (T-1) rows of one (device, update-batch)
+ * shard, restated from rlax's published mpo_ops.py (tests/vmpo_oracle.py):
+ * stx_vmpo_topk: tau = the k-th largest of adv[0..N) (k = int(0.5 N), rlax's top_k_fraction), by three radix passes over
+ *   order-preserving uint32 keys (integer histograms: exact and deterministic).  With `mask` (nullable) a fourth launch writes
+ *   mask[i] = (adv[i] >= tau) compared as floats (ties at tau are all selected, -0 == +0) and *count = K = |mask|.  N < 2 is
+ *   refused with STX_E_SHAPE.  scratch: stx_vmpo_topk_scratch_bytes(), zeroed once.
+ * stx_vmpo_loss_grads: two launches.  eta = softplus(duals[0]) + 1e-8, alpha_c = softplus(duals[1 + c]) + 1e-8; on the selected rows
+ *   m = max A_i / eta, Z = sum exp(A_i / eta - m), w_i = exp(A_i / eta - m) / Z (0 elsewhere; stop-gradient), K = *count.
+ *     L_pi = -sum_i w_i log pi(a_i | s_i)                                  (a sum, no 1/N)
+ *     L_eta = eta (epsilon + log Z + m - log K)
+ *     per KL column c: mean_kl_c = (1/N) sum_i kl_ic; L_kl = sum_c sg(alpha_c) mean_kl_c; L_alpha = sum_c alpha_c (eps_c - sg(mean_kl_c))
+ *   KL columns: STX_VMPO_CATEGORICAL: one, KL(target || online) of the logits (eps_c = epsilon_alpha).  STX_VMPO_TANH_NORMAL on the
+ *   pre-tanh Normals (loc | softplus(raw) + min_scale): kl_mean = KL(target || N(mu_online, sigma_target)) (eps_c = epsilon_alpha)
+ *   and kl_stddev = KL(target || N(mu_target, sigma_online)) (eps_c = epsilon_stddev); per_dim: A columns of each (mean columns
+ *   0..A-1, stddev columns A..2A-1), else one of each, summed over the dims.  The dual segment is [log_temperature, log_alpha_c
+ *   for each column c].  Writes d_head = d (L_pi + L_kl) / d head (the tanh-Normal scale chained through sigmoid(raw)); d_value
+ *   (value_rows rows, nullable when 0) = -(targets - value) / N on rows < N and 0 beyond (rlax.l2_loss(targets - v).mean());
+ *   dual_grad[d] = weight g_d (overwrite) or += weight g_d with g_0 = (epsilon + log Z + m - log K - sum_i w_i A_i / eta)
+ *   sigmoid(duals[0]), g_{1+c} = (eps_c - mean_kl_c) sigmoid(duals[1+c]); metrics[0..STX_VMPO_METRICS) += weight (L_pi, L_kl,
+ *   L_alpha, L_eta, eta, mean alpha of the mean (or Categorical) columns, mean alpha of the stddev columns (0 for Categorical),
+ *   mean advantage, value loss).  The whole-shard sums are fp64 in a fixed order.  scratch: stx_vmpo_loss_scratch_bytes(), zeroed once.
+ * stx_vmpo_after_step: after the optimiser step: duals[0..n_dual) = max(-18, duals) (clip_categorical_mpo_params, discrete_loss.py:
+ *   150-154; clip_dual_params, continuous_loss.py:142-147), and target[0..P) = online[0..P) when *count % period == 0
+ *   (optax.periodic_update, ff_vmpo.py:266-274; *count = the actor segment's Adam count = learner_step_count).
+ * stx_n_step_returns_f32: batch_n_step_bootstrapped_returns (stoix/utils/multistep.py:148-210) time-major, scalar lambda: targets
+ *   start from v_t shifted by n and padded with v_t[T-1], then for i = n-1 .. 0: G_t = r + d ((1 - l) v + l G_t) at step t + i,
+ *   with r = 0, d = 1, l = 1, v = v_t[T-1] past the end.  adv (nullable) = targets - v_tm1. */
+#define STX_VMPO_CATEGORICAL 0
+#define STX_VMPO_TANH_NORMAL 1
+#define STX_VMPO_MAX_A 32
+#define STX_VMPO_METRICS 9
+typedef struct StxVmpoLoss {
+  int32_t kind;               /* STX_VMPO_* */
+  int32_t A;                  /* actions (Categorical) or action dims (tanh-Normal), 1..STX_VMPO_MAX_A */
+  int32_t per_dim;            /* tanh-Normal: per_dim_constraining */
+  int32_t overwrite;          /* 1: dual_grad = weight g; 0: += */
+  int64_t N;                  /* rows of the shard, >= 2 */
+  int64_t value_rows;         /* rows of d_value (the critic's T E rows) */
+  const float* head;          /* (N, A) logits or (N, 2A) loc | raw scale of the online actor */
+  const float* head_target;   /* same, target actor */
+  const int32_t* action;      /* Categorical (N) */
+  const float* action_cont;   /* tanh-Normal (N, A) */
+  const float* adv;           /* (N) */
+  const uint8_t* mask;        /* (N) selection of stx_vmpo_topk */
+  const int32_t* count;       /* K */
+  const float* value;         /* (N) v_tm1 of the current critic */
+  const float* targets;       /* (N) value targets */
+  const float* duals;         /* dual segment of the parameter arena */
+  float* d_head;
+  float* d_value;
+  float* dual_grad;           /* dual segment of the gradient arena */
+  float* metrics;
+  float epsilon;              /* temperature constraint */
+  float epsilon_alpha;        /* epsilon_policy (Categorical) / epsilon_mean */
+  float epsilon_stddev;
+  float weight;
+  float minimum, maximum, min_scale;
+  int32_t reserved;
+} StxVmpoLoss;
+size_t stx_vmpo_topk_scratch_bytes(void);
+int stx_vmpo_topk(const float* adv, int64_t N, int64_t k, float* tau, uint8_t* mask, int32_t* count, void* scratch, void* stream);
+size_t stx_vmpo_loss_scratch_bytes(void);
+int stx_vmpo_loss_grads(const StxVmpoLoss* loss, void* scratch, void* stream);
+int stx_vmpo_after_step(float* duals, int n_dual, const float* online, float* target, int64_t P, const int32_t* count, int period, void* stream);
+int stx_n_step_returns_f32(const float* r_t, const float* discount_t, const float* v_t, const float* v_tm1, int T, int E, int n, float lambda_,
+                           float* targets, float* adv, void* stream);
+
 /* Utility casts used by the bf16 path (obs / weight shadows). */
 int stx_cast_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream);
 

@@ -237,6 +237,46 @@ class StxPpoVariant(C.Structure):
     ]
 
 
+
+STX_VMPO_CATEGORICAL = 0
+STX_VMPO_TANH_NORMAL = 1
+STX_VMPO_MAX_A = 32
+STX_VMPO_METRICS = 9
+
+
+class StxVmpoLoss(C.Structure):
+    _fields_ = [
+        ("kind", C.c_int32),
+        ("A", C.c_int32),
+        ("per_dim", C.c_int32),
+        ("overwrite", C.c_int32),
+        ("N", C.c_int64),
+        ("value_rows", C.c_int64),
+        ("head", C.c_void_p),
+        ("head_target", C.c_void_p),
+        ("action", C.c_void_p),
+        ("action_cont", C.c_void_p),
+        ("adv", C.c_void_p),
+        ("mask", C.c_void_p),
+        ("count", C.c_void_p),
+        ("value", C.c_void_p),
+        ("targets", C.c_void_p),
+        ("duals", C.c_void_p),
+        ("d_head", C.c_void_p),
+        ("d_value", C.c_void_p),
+        ("dual_grad", C.c_void_p),
+        ("metrics", C.c_void_p),
+        ("epsilon", C.c_float),
+        ("epsilon_alpha", C.c_float),
+        ("epsilon_stddev", C.c_float),
+        ("weight", C.c_float),
+        ("minimum", C.c_float),
+        ("maximum", C.c_float),
+        ("min_scale", C.c_float),
+        ("reserved", C.c_int32),
+    ]
+
+
 _P = C.c_void_p
 _SIGNATURES = {
     # name: (restype, argtypes)
@@ -350,6 +390,12 @@ _SIGNATURES = {
     "stx_replay_sample_prioritised": (C.c_int, [C.POINTER(StxReplayPrioritised), C.c_int64, C.c_uint64, C.c_uint64, _P, _P, _P, C.c_float, C.c_float,
                                                 C.c_float, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
     "stx_replay_set_priorities": (C.c_int, [C.POINTER(StxReplayPrioritised), _P, _P, C.c_int64, _P]),
+    "stx_vmpo_topk_scratch_bytes": (C.c_size_t, []),
+    "stx_vmpo_topk": (C.c_int, [_P, C.c_int64, C.c_int64, _P, _P, _P, _P, _P]),
+    "stx_vmpo_loss_scratch_bytes": (C.c_size_t, []),
+    "stx_vmpo_loss_grads": (C.c_int, [C.POINTER(StxVmpoLoss), _P, _P]),
+    "stx_vmpo_after_step": (C.c_int, [_P, C.c_int, _P, _P, C.c_int64, _P, C.c_int, _P]),
+    "stx_n_step_returns_f32": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float, _P, _P, _P]),
 }
 
 _lib = None

@@ -103,21 +103,6 @@ struct CategoricalRow {
   }
 };
 
-// KL(N(mb, sb) || N(mu, s)) of one dimension and its derivatives with respect to the second distribution's mu and s.  The value
-// is tfp's arrangement, 0.5 (dm / s)^2 + 0.5 expm1(2 d) - d with d = log sb - log s: no cancellation near KL = 0, where the
-// penalty starts every update, and exactly 0 for equal distributions.
-struct NormalKl {
-  float kl, d_mu, d_sigma;
-};
-__device__ __forceinline__ NormalKl normal_kl(float mu_b, float sigma_b, float mu, float sigma) {
-  const float dm = mu_b - mu, q = sigma_b * sigma_b + dm * dm, inv = 1.f / sigma, dls = logf(sigma_b) - logf(sigma), z = dm * inv;
-  NormalKl r;
-  r.kl = 0.5f * z * z + 0.5f * expm1f(2.f * dls) - dls;
-  r.d_mu = -dm * inv * inv;
-  r.d_sigma = inv - q * inv * inv * inv;
-  return r;
-}
-
 // Two passes over the dims, four at a time: the second regenerates the entropy noise of the first (layout in include/stx.h),
 // so the entropy draws of every loss on this head match.
 template <bool KL>

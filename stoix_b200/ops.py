@@ -1611,3 +1611,103 @@ def replay_set_priorities(rb: PrioritisedRing, idx: torch.Tensor, priorities: to
     if idx.dtype != torch.int32 or priorities.dtype != torch.float32 or priorities.numel() != M or not idx.is_contiguous() or not priorities.is_contiguous():
         raise StxError("replay_set_priorities: idx (M) int32 and priorities (M) float32, contiguous")
     _lib.check(_lib.load().stx_replay_set_priorities(C.byref(rb.c), _p(idx), _p(priorities), M, _stream()), "stx_replay_set_priorities")
+
+
+# ------------------------------------------------------------------------------------------------
+# V-MPO: exact top-k selection, fused loss + gradients, after-step, n-step returns (stoix/systems/mpo/ff_vmpo*.py)
+# ------------------------------------------------------------------------------------------------
+
+VMPO_KINDS = {"categorical": _lib.STX_VMPO_CATEGORICAL, "tanh_normal": _lib.STX_VMPO_TANH_NORMAL}
+VMPO_METRICS = ("loss_policy", "loss_kl", "loss_alpha", "loss_temperature", "temperature", "alpha", "alpha_stddev", "advantages", "v_loss")
+
+
+def vmpo_topk(adv: torch.Tensor, tau: Optional[torch.Tensor] = None, mask: Optional[torch.Tensor] = None, count: Optional[torch.Tensor] = None,
+              scratch_key: str = "vmpo_topk") -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """rlax.vmpo_loss's top-k selection over the N flat rows of `adv` (float32): tau = the k-th largest, k = int(0.5 N); mask (uint8, N)
+    = adv >= tau as floats; count (int32, 1) = K.  Returns (tau, mask, count)."""
+    dev = _need_cuda(adv, tau, mask, count)
+    if adv.dtype != torch.float32:
+        raise StxError("vmpo_topk: adv must be float32")
+    N = int(adv.numel())
+    tau = torch.empty(1, dtype=torch.float32, device=dev) if tau is None else tau
+    mask = torch.empty(N, dtype=torch.uint8, device=dev) if mask is None else mask
+    count = torch.empty(1, dtype=torch.int32, device=dev) if count is None else count
+    if mask.dtype != torch.uint8 or mask.numel() != N or count.dtype != torch.int32 or tau.dtype != torch.float32:
+        raise StxError("vmpo_topk: mask uint8 (N), count int32 (1), tau float32 (1)")
+    lib = _lib.load()
+    scratch = _zeros_scratch((scratch_key,), lib.stx_vmpo_topk_scratch_bytes(), dev)
+    _lib.check(lib.stx_vmpo_topk(_p(adv), N, int(0.5 * N), _p(tau), _p(mask), _p(count), _p(scratch), _stream()), "stx_vmpo_topk")
+    return tau, mask, count
+
+
+def vmpo_loss_grads(kind: str, head: torch.Tensor, head_target: torch.Tensor, action: torch.Tensor, adv: torch.Tensor, mask: torch.Tensor,
+                    count: torch.Tensor, value: torch.Tensor, targets: torch.Tensor, duals: torch.Tensor, d_head: torch.Tensor,
+                    dual_grad: torch.Tensor, metrics: torch.Tensor, epsilon: float, epsilon_alpha: float, epsilon_stddev: float = 0.0,
+                    per_dim: bool = True, d_value: Optional[torch.Tensor] = None, minimum: float = -1.0, maximum: float = 1.0,
+                    min_scale: float = 1e-3, weight: float = 1.0, overwrite: bool = True, scratch_key: str = "vmpo_loss") -> None:
+    """rlax.vmpo_loss of one shard and its gradients (include/stx.h, stx_vmpo_loss_grads): head / head_target (N, A) logits or (N, 2A)
+    loc | raw scale; action int32 (N) or float32 (N, A); adv, value (the critic's first N rows), targets float32 (N); mask / count from
+    vmpo_topk; duals the dual segment [log_temperature, log_alpha...]; d_value (value_rows) gets -(targets - value) / N on its first
+    N rows and 0 on the rest."""
+    if kind not in VMPO_KINDS:
+        raise StxError(f"vmpo_loss_grads: kind {kind!r} is not one of {sorted(VMPO_KINDS)}")
+    dev = _need_cuda(head, head_target, action, adv, mask, count, value, targets, duals, d_head, dual_grad, metrics, d_value)
+    tanh = kind == "tanh_normal"
+    N = int(adv.numel())
+    W = int(head.shape[-1])
+    A = W // 2 if tanh else W
+    for t, name in ((head, "head"), (head_target, "head_target"), (d_head, "d_head")):
+        if t.dtype != torch.float32 or tuple(t.shape) != (N, W):
+            raise StxError(f"vmpo_loss_grads: {name} must be float32 ({N}, {W})")
+    for t, name in ((adv, "adv"), (targets, "targets"), (duals, "duals"), (dual_grad, "dual_grad"), (metrics, "metrics"), (value, "value")):
+        if t.dtype != torch.float32:
+            raise StxError(f"vmpo_loss_grads: {name} must be float32")
+    if value.numel() < N or targets.numel() != N or mask.numel() != N or mask.dtype != torch.uint8 or count.dtype != torch.int32:
+        raise StxError("vmpo_loss_grads: value (>= N), targets (N) float32, mask uint8 (N), count int32")
+    ncol = (2 * A if per_dim else 2) if tanh else 1
+    if duals.numel() < 1 + ncol or dual_grad.numel() < 1 + ncol or metrics.numel() < _lib.STX_VMPO_METRICS:
+        raise StxError(f"vmpo_loss_grads: duals / dual_grad need {1 + ncol} floats, metrics {_lib.STX_VMPO_METRICS}")
+    if tanh and (action.dtype != torch.float32 or tuple(action.shape) != (N, A)):
+        raise StxError(f"vmpo_loss_grads: tanh-Normal actions must be float32 ({N}, {A})")
+    if not tanh and (action.dtype != torch.int32 or action.numel() != N):
+        raise StxError("vmpo_loss_grads: Categorical actions must be int32 (N)")
+    if d_value is not None and (d_value.dtype != torch.float32 or d_value.numel() < N):
+        raise StxError("vmpo_loss_grads: d_value must be float32 with at least N rows")
+    lib = _lib.load()
+    scratch = _zeros_scratch((scratch_key,), lib.stx_vmpo_loss_scratch_bytes(), dev)
+    s = _lib.StxVmpoLoss()
+    s.kind, s.A, s.per_dim, s.overwrite = VMPO_KINDS[kind], A, int(bool(per_dim)), int(bool(overwrite))
+    s.N, s.value_rows = N, 0 if d_value is None else int(d_value.numel())
+    s.head, s.head_target, s.adv, s.mask, s.count = head.data_ptr(), head_target.data_ptr(), adv.data_ptr(), mask.data_ptr(), count.data_ptr()
+    s.action, s.action_cont = (None, action.data_ptr()) if tanh else (action.data_ptr(), None)
+    s.value, s.targets, s.duals = value.data_ptr(), targets.data_ptr(), duals.data_ptr()
+    s.d_head, s.d_value, s.dual_grad, s.metrics = d_head.data_ptr(), None if d_value is None else d_value.data_ptr(), dual_grad.data_ptr(), metrics.data_ptr()
+    s.epsilon, s.epsilon_alpha, s.epsilon_stddev, s.weight = float(epsilon), float(epsilon_alpha), float(epsilon_stddev), float(weight)
+    s.minimum, s.maximum, s.min_scale = float(minimum), float(maximum), float(min_scale)
+    _lib.check(lib.stx_vmpo_loss_grads(C.byref(s), _p(scratch), _stream()), "stx_vmpo_loss_grads")
+
+
+def vmpo_after_step(duals: torch.Tensor, online: torch.Tensor, target: torch.Tensor, count: torch.Tensor, period: int) -> None:
+    """After the optimiser step: duals = max(-18, duals); target = online when *count % period == 0 (count: int32 on the device)."""
+    _need_cuda(duals, online, target, count)
+    if any(t.dtype != torch.float32 for t in (duals, online, target)) or count.dtype != torch.int32 or target.numel() < online.numel():
+        raise StxError("vmpo_after_step: duals / online / target float32 (target >= online), count int32")
+    _lib.check(_lib.load().stx_vmpo_after_step(_p(duals), int(duals.numel()), _p(online), _p(target), int(online.numel()), _p(count), int(period),
+                                               _stream()), "stx_vmpo_after_step")
+
+
+def n_step_returns(r_t: torch.Tensor, discount_t: torch.Tensor, v_t: torch.Tensor, n: int, lambda_: float = 1.0, v_tm1: Optional[torch.Tensor] = None,
+                   out: Optional[torch.Tensor] = None, adv_out: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """Time-major batch_n_step_bootstrapped_returns (multistep.py:148-210) with a scalar lambda: (targets, advantages = targets - v_tm1
+    when v_tm1 is given), all (T, E) float32."""
+    dev = _need_cuda(r_t, discount_t, v_t, v_tm1, out, adv_out)
+    T, E = r_t.shape
+    for t in (r_t, discount_t, v_t, v_tm1, out, adv_out):
+        if t is not None and (t.dtype != torch.float32 or tuple(t.shape) != (T, E)):
+            raise StxError("n_step_returns: every array must be float32 (T, E)")
+    out = torch.empty((T, E), dtype=torch.float32, device=dev) if out is None else out
+    if v_tm1 is not None and adv_out is None:
+        adv_out = torch.empty((T, E), dtype=torch.float32, device=dev)
+    _lib.check(_lib.load().stx_n_step_returns_f32(_p(r_t), _p(discount_t), _p(v_t), _p(v_tm1), T, E, int(n), float(lambda_), _p(out),
+                                                  _p(adv_out if v_tm1 is not None else None), _stream()), "stx_n_step_returns_f32")
+    return out, (adv_out if v_tm1 is not None else None)

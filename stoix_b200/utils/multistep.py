@@ -113,3 +113,26 @@ def _lambda_returns(r_t, discount_t, v_t, lambda_, time_major: bool, q_values: b
         lam = prep(lambda_.expand_as(discount_t))
     out = ops.lambda_returns(prep(r_t), prep(discount_t), prep(v_t), lam)
     return out if time_major else out.t().contiguous()
+
+
+def batch_n_step_bootstrapped_returns(
+    r_t: Array,
+    discount_t: Array,
+    v_t: Array,
+    n: int,
+    lambda_t: float = 1.0,
+    stop_target_gradients: bool = True,
+) -> Array:
+    """Strided n-step bootstrapped returns of batch-major [B, T] sequences (multistep.py:148-210), one CUDA launch
+    (stx_n_step_returns_f32) in the reference's operation order: the bootstrap values shifted by n and padded with v_t[:, -1], then
+    G = r + d ((1 - lambda) v + lambda G) from step t + n - 1 down to t, the padded steps reading r = 0, d = 1, lambda = 1.
+
+    Only a scalar lambda_t is implemented; an array raises.  `stop_target_gradients` is accepted for signature compatibility (the
+    outputs never carry gradients)."""
+    if getattr(lambda_t, "ndim", 0) > 0 or isinstance(lambda_t, (list, tuple)):
+        raise ValueError("batch_n_step_bootstrapped_returns: only a scalar lambda_t is implemented (the V-MPO systems pass none); "
+                         f"got an array of shape {tuple(getattr(lambda_t, 'shape', (len(lambda_t),)))}")
+    lam = float(lambda_t)
+    tm = lambda x: x.to(torch.float32).transpose(0, 1).contiguous()
+    targets, _ = ops.n_step_returns(tm(r_t), tm(discount_t), tm(v_t), int(n), lam)
+    return targets.transpose(0, 1).contiguous()
