@@ -866,6 +866,112 @@ int stx_vmpo_after_step(float* duals, int n_dual, const float* online, float* ta
 int stx_n_step_returns_f32(const float* r_t, const float* discount_t, const float* v_t, const float* v_tm1, int T, int E, int n, float lambda_,
                            float* targets, float* adv, void* stream);
 
+/* ------------------------------------------------------------------ MPO (fp32): stoix/systems/mpo/ff_mpo.py, ff_mpo_continuous.py ----
+ * stx_replay_add_sequence / stx_replay_sample_sequence: fbx.make_trajectory_buffer as ff_mpo.py:539-546 builds it, with
+ *   add_batch_size = E, max_length_time_axis = L, period = 1 (tests/mpo_oracle.py restates the rules).  Time-major ring of L x E
+ *   rows, one write index for all envs: add writes batch row t to ring row (w + t) mod L (only the newest L rows of a longer batch),
+ *   then w = (w + T) mod L and c = min(c + T, L) (state[0], state[1]; two launches).  sample draws, per sequence b, an env e uniform
+ *   in [0, E) and k uniform in [0, c - S + 1): the S rows from start = (w - c + k) mod L, which never straddle the write head.  The
+ *   draws are Philox(seed) at call offset + *dev_counter (nullable), or idx_in (B, 2) = (e, k) when given; idx_out (B, 2) = (e, start).
+ *   Outputs are time-major (S, B): obs (S, B, D), action (S, B, act_words), reward, done, log_prob.  period != 1 -> STX_E_UNSUPPORTED.
+ * stx_mpo_sample_actions: the target-Q input rows of M states in one launch, xq ((A + N + 1) M, D + A): block j < A holds
+ *   [obs_i | one_hot(j)] (the actor loss evaluates every action, ff_mpo.py:189-197), block A + n holds [obs_i | one_hot(a_ni)] with a_ni
+ *   drawn by inverse CDF from Categorical(logits_b[i]) (the bootstrap policy; its mode when stochastic = 0, with N = 1), or act_in (N, M)
+ *   when given, written to act_out (N, M, nullable); block A + N holds [obs_i | one_hot(action_i)].  Per state it also writes
+ *   log_rho = log_softmax(logits_t)[action] - log_prob, r = clip(reward, +-max_abs_reward) and d = (1 - done) gamma.
+ * stx_mpo_loss_grads: categorical_mpo_loss (discrete_loss.py:20-147) over M states, q (A, M): eta = softplus(duals[0]) + 1e-8,
+ *   alpha = softplus(duals[1]) + 1e-8, u = q / eta + log_softmax(target), w = softmax(u), loss = mean CE(w, online) + alpha mean KL(target
+ *   || online) + alpha (eps_policy - mean KL) + eta (eps + mean logsumexp u), with alpha held constant in the KL penalty and the KL held
+ *   constant in the alpha loss.  d_head (M, A) = [(p_o - w) + alpha (p_o - p_t)] / M; dual_grad = weight * (dL/deta sigmoid(duals[0]),
+ *   (eps_policy - mean KL) sigmoid(duals[1])), where dL/deta = eps + mean lse - mean(sum w q) / eta + mean(sum w (q - sum w q) log p_o) /
+ *   eta^2 (the E-step weights carry eta's gradient into the cross-entropy, as jax.grad of the reference does).  metrics[0..13) += weight
+ *   * (temperature, alpha, loss_temperature, loss_alpha, loss_policy, loss_kl, kl_nonparametric, entropy_online, entropy_target,
+ *   kl_mean_rel, kl_q_rel, q_min, q_max); q_min / q_max are the reference's mean over actions of the min / max over states.  With
+ *   q_boot (N, M): v = sum_n q_boot / N.  One launch; the whole-batch sums are fp64 in block order.
+ * STX_MPO_TANH_NORMAL (ff_mpo_continuous.py, continuous_loss.py:26-303): the rows are NL draws a = shift + s tanh(loc + sigma eps) of
+ *   the target policy ([obs | clip(a, minimum, maximum)], a itself kept in act_cont_out), N draws of the bootstrap policy (its mode
+ *   shift + s tanh(loc) when stochastic = 0) and the clipped stored action; eps is Philox(seed, row, dim) at call *dev_counter, or
+ *   eps_in.  log_rho sums tanh_normal_log_prob_given over the dims.  The loss: w = softmax_n(q / eta) held constant, loss_temperature
+ *   = eta (eps + mean lse - log NL), the decoupled cross-entropies of N(loc_o, sigma_t) (gradient to loc) and N(loc_t, sigma_o)
+ *   (gradient to the raw scale), and KL(target || fixed-stddev) / KL(target || fixed-mean) per dimension (C = A columns) or summed
+ *   (C = 1), each with its alpha = softplus + 1e-8 held constant in the penalty.  dual_grad = weight * ((eps + mean lse - log NL -
+ *   mean sum w q / eta) sigmoid(lt), (eps_c - mean KL_c) sigmoid(la_c)...); metrics[0..13) += weight * (temperature, alpha_mean,
+ *   alpha_stddev, loss_temperature, loss_alpha_mean, loss_alpha_stddev, loss_policy_mean, loss_policy_stddev, loss_kl_mean,
+ *   loss_kl_stddev, kl_mean, kl_stddev, kl_nonparametric) with the alphas and KLs averaged over their columns.
+ * stx_retrace_f32: batch_general_off_policy_returns_from_q_and_v (multistep.py:210-311), time-major: q_t (K-1, E), v_t, r_t,
+ *   discount_t, targets (K, E); the weights are c = lambda min(1, exp(log_rho)) (Retrace, log_rho (K-1, E)), or c_t (K-1, E) itself
+ *   when c_t is given (log_rho and lambda are then not read).
+ * stx_mpo_q_grad: dq (S, B) = (q - target) / (B (S-1)) on rows < S-1 and 0 on row S-1 (d of mean l2_loss); *metric += weight * that loss. */
+#define STX_MPO_CATEGORICAL 0
+#define STX_MPO_TANH_NORMAL 1
+#define STX_MPO_MAX_A 32
+#define STX_MPO_METRICS 14
+typedef struct StxSeqRing {
+  float* obs;                 /* (L, E, D) */
+  void* action;               /* (L, E, act_words) 32-bit words: one int32 (Categorical) or A float32 (tanh-Normal) */
+  float* reward;
+  uint8_t* done;
+  uint8_t* truncated;         /* stored, not read by the MPO targets */
+  float* log_prob;            /* behaviour log-probability */
+  int64_t* state;             /* [write row w, rows written c] */
+  int64_t length;             /* L */
+  int32_t envs, obs_dim, act_words, reserved;
+} StxSeqRing;
+typedef struct StxMpoRows {
+  int32_t kind, A, N, D;      /* STX_MPO_*; actions (Categorical) or action dims (tanh-Normal); bootstrap rows per state; obs width */
+  int64_t M;                  /* states */
+  int32_t NL;                 /* actor-loss rows per state: A (Categorical) or num_samples (tanh-Normal) */
+  int32_t stochastic;         /* 0: the mode of the bootstrap policy, N = 1 */
+  uint64_t seed;
+  const float* obs;           /* (M, D) */
+  const float* logits_t;      /* (M, A) logits or (M, 2A) loc | raw scale of the target actor */
+  const float* logits_b;      /* same, of the policy the bootstrap evaluates */
+  const void* action;         /* (M) int32 or (M, A) float32 stored actions */
+  const float* log_prob;      /* (M) behaviour log-probabilities */
+  const float* reward;        /* (M) */
+  const uint8_t* done;        /* (M) */
+  const int32_t* act_in;      /* Categorical: (N, M) injected bootstrap actions, nullable */
+  int32_t* act_out;           /* Categorical: (N, M), nullable */
+  const float* eps_in;        /* tanh-Normal: (NL + N, M, A) injected standard normals, nullable */
+  float* act_cont_out;        /* tanh-Normal: (NL, M, A) the unclipped actor-loss draws */
+  float* xq;                  /* ((NL + N + 1) M, D + A) */
+  float* log_rho;             /* (M) */
+  float* r;                   /* (M) */
+  float* d;                   /* (M) */
+  float gamma, max_abs_reward;
+  float minimum, maximum, min_scale;
+  int32_t reserved;
+} StxMpoRows;
+typedef struct StxMpoLoss {
+  int32_t kind, A, N, overwrite;
+  int64_t M;
+  int32_t NL, per_dim;        /* actor-loss rows per state (A for Categorical); tanh-Normal: per_dim_constraining */
+  const float* head;          /* (M, A) online logits or (M, 2A) loc | raw scale */
+  const float* head_target;   /* same, target actor */
+  const float* q;             /* (NL, M) target Q of the actor-loss rows */
+  const float* actions;       /* tanh-Normal: (NL, M, A) unclipped draws of the target policy */
+  const float* q_boot;        /* (N, M) bootstrap target Q, nullable */
+  const float* duals;         /* [log_temperature, log_alpha] or [log_temperature, log_alpha_mean (C), log_alpha_stddev (C)] */
+  float* v;                   /* (M) mean of q_boot */
+  float* d_head;
+  float* dual_grad;
+  float* metrics;
+  float epsilon, epsilon_policy, epsilon_stddev, weight;   /* epsilon_policy is epsilon_mean for the tanh-Normal kind */
+  float minimum, maximum, min_scale;
+  int32_t reserved;
+} StxMpoLoss;
+int stx_replay_add_sequence(const StxSeqRing* rb, const float* obs, const void* action, const float* reward, const uint8_t* done,
+                            const uint8_t* truncated, const float* log_prob, int T, void* stream);
+int stx_replay_sample_sequence(const StxSeqRing* rb, int B, int S, int period, uint64_t seed, uint64_t offset, const uint64_t* dev_counter,
+                               const int32_t* idx_in, int32_t* idx_out, float* obs, void* action, float* reward, uint8_t* done, float* log_prob,
+                               void* stream);
+int stx_mpo_sample_actions(const StxMpoRows* rows, uint64_t offset, const uint64_t* dev_counter, void* stream);
+size_t stx_mpo_loss_scratch_bytes(void);
+int stx_mpo_loss_grads(const StxMpoLoss* loss, void* scratch, void* stream);
+int stx_retrace_f32(const float* q_t, const float* v_t, const float* r_t, const float* discount_t, const float* log_rho, const float* c_t, float lambda_,
+                    int K, int E, float* targets, void* stream);
+int stx_mpo_q_grad(const float* q, const float* targets, int S, int B, float* dq, float* metric, float weight, void* stream);
+
 /* Utility casts used by the bf16 path (obs / weight shadows). */
 int stx_cast_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream);
 

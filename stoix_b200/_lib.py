@@ -277,6 +277,35 @@ class StxVmpoLoss(C.Structure):
     ]
 
 
+STX_MPO_CATEGORICAL = 0
+STX_MPO_TANH_NORMAL = 1
+STX_MPO_MAX_A = 32
+STX_MPO_METRICS = 14
+
+
+class StxSeqRing(C.Structure):
+    _fields_ = [("obs", C.c_void_p), ("action", C.c_void_p), ("reward", C.c_void_p), ("done", C.c_void_p), ("truncated", C.c_void_p),
+                ("log_prob", C.c_void_p), ("state", C.c_void_p), ("length", C.c_int64), ("envs", C.c_int32), ("obs_dim", C.c_int32),
+                ("act_words", C.c_int32), ("reserved", C.c_int32)]
+
+
+class StxMpoRows(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("A", C.c_int32), ("N", C.c_int32), ("D", C.c_int32), ("M", C.c_int64), ("NL", C.c_int32),
+                ("stochastic", C.c_int32), ("seed", C.c_uint64), ("obs", C.c_void_p), ("logits_t", C.c_void_p), ("logits_b", C.c_void_p),
+                ("action", C.c_void_p), ("log_prob", C.c_void_p), ("reward", C.c_void_p), ("done", C.c_void_p), ("act_in", C.c_void_p),
+                ("act_out", C.c_void_p), ("eps_in", C.c_void_p), ("act_cont_out", C.c_void_p), ("xq", C.c_void_p), ("log_rho", C.c_void_p),
+                ("r", C.c_void_p), ("d", C.c_void_p), ("gamma", C.c_float), ("max_abs_reward", C.c_float), ("minimum", C.c_float),
+                ("maximum", C.c_float), ("min_scale", C.c_float), ("reserved", C.c_int32)]
+
+
+class StxMpoLoss(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("A", C.c_int32), ("N", C.c_int32), ("overwrite", C.c_int32), ("M", C.c_int64), ("NL", C.c_int32),
+                ("per_dim", C.c_int32), ("head", C.c_void_p), ("head_target", C.c_void_p), ("q", C.c_void_p), ("actions", C.c_void_p),
+                ("q_boot", C.c_void_p), ("duals", C.c_void_p), ("v", C.c_void_p), ("d_head", C.c_void_p), ("dual_grad", C.c_void_p),
+                ("metrics", C.c_void_p), ("epsilon", C.c_float), ("epsilon_policy", C.c_float), ("epsilon_stddev", C.c_float),
+                ("weight", C.c_float), ("minimum", C.c_float), ("maximum", C.c_float), ("min_scale", C.c_float), ("reserved", C.c_int32)]
+
+
 _P = C.c_void_p
 _SIGNATURES = {
     # name: (restype, argtypes)
@@ -396,6 +425,14 @@ _SIGNATURES = {
     "stx_vmpo_loss_grads": (C.c_int, [C.POINTER(StxVmpoLoss), _P, _P]),
     "stx_vmpo_after_step": (C.c_int, [_P, C.c_int, _P, _P, C.c_int64, _P, C.c_int, _P]),
     "stx_n_step_returns_f32": (C.c_int, [_P, _P, _P, _P, C.c_int, C.c_int, C.c_int, C.c_float, _P, _P, _P]),
+    "stx_replay_add_sequence": (C.c_int, [C.POINTER(StxSeqRing), _P, _P, _P, _P, _P, _P, C.c_int, _P]),
+    "stx_replay_sample_sequence": (C.c_int, [C.POINTER(StxSeqRing), C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_uint64, _P, _P, _P, _P, _P, _P, _P,
+                                             _P, _P]),
+    "stx_mpo_sample_actions": (C.c_int, [C.POINTER(StxMpoRows), C.c_uint64, _P, _P]),
+    "stx_mpo_loss_scratch_bytes": (C.c_size_t, []),
+    "stx_mpo_loss_grads": (C.c_int, [C.POINTER(StxMpoLoss), _P, _P]),
+    "stx_retrace_f32": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_float, C.c_int, C.c_int, _P, _P]),
+    "stx_mpo_q_grad": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P, C.c_float, _P]),
 }
 
 _lib = None

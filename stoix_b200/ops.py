@@ -1711,3 +1711,179 @@ def n_step_returns(r_t: torch.Tensor, discount_t: torch.Tensor, v_t: torch.Tenso
     _lib.check(_lib.load().stx_n_step_returns_f32(_p(r_t), _p(discount_t), _p(v_t), _p(v_tm1), T, E, int(n), float(lambda_), _p(out),
                                                   _p(adv_out if v_tm1 is not None else None), _stream()), "stx_n_step_returns_f32")
     return out, (adv_out if v_tm1 is not None else None)
+
+
+# ------------------------------------------------------------------------------------------------
+# MPO: sequence replay ring, target-Q input rows, fused categorical loss, Retrace, Q-loss gradient (stoix/systems/mpo/ff_mpo.py)
+# ------------------------------------------------------------------------------------------------
+
+MPO_CONTINUOUS_METRICS = ("temperature", "alpha_mean", "alpha_stddev", "loss_temperature", "loss_alpha_mean", "loss_alpha_stddev",
+                          "loss_policy_mean", "loss_policy_stddev", "loss_kl_mean", "loss_kl_stddev", "kl_mean", "kl_stddev", "kl_nonparametric",
+                          "q_loss")
+MPO_METRICS = ("temperature", "alpha", "loss_temperature", "loss_alpha", "loss_policy", "loss_kl", "kl_nonparametric", "entropy_online",
+               "entropy_target", "kl_mean_rel", "kl_q_rel", "q_min", "q_max", "q_loss")
+
+
+class SequenceRing:
+    """Device storage of the time-major sequence ring (include/stx.h, StxSeqRing): L x E rows of obs, action (int32 with act_dim = 0,
+    else float32 (act_dim)), reward, done, truncated and behaviour log_prob, and the device state [write row, rows written]."""
+
+    def __init__(self, length: int, envs: int, obs_dim: int, device, act_dim: int = 0):
+        z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=device)
+        self.length, self.envs, self.obs_dim, self.act_dim = int(length), int(envs), int(obs_dim), int(act_dim)
+        self.obs = z(self.length, self.envs, self.obs_dim)
+        self.action = z(self.length, self.envs, self.act_dim) if self.act_dim else z(self.length, self.envs, dt=torch.int32)
+        self.reward, self.log_prob = z(self.length, self.envs), z(self.length, self.envs)
+        self.done, self.truncated = z(self.length, self.envs, dt=torch.uint8), z(self.length, self.envs, dt=torch.uint8)
+        self.state = z(2, dt=torch.int64)
+        s = _lib.StxSeqRing()
+        s.obs, s.action, s.reward, s.done = self.obs.data_ptr(), self.action.data_ptr(), self.reward.data_ptr(), self.done.data_ptr()
+        s.truncated, s.log_prob, s.state = self.truncated.data_ptr(), self.log_prob.data_ptr(), self.state.data_ptr()
+        s.length, s.envs, s.obs_dim, s.act_words = self.length, self.envs, self.obs_dim, max(self.act_dim, 1)
+        self.c = s
+
+    def action_ok(self, action: torch.Tensor, lead: Tuple[int, int]) -> bool:
+        if self.act_dim:
+            return action.dtype == torch.float32 and tuple(action.shape) == (*lead, self.act_dim)
+        return action.dtype == torch.int32 and tuple(action.shape) == tuple(lead)
+
+
+def replay_add_sequence(ring: SequenceRing, obs, action, reward, done, truncated, log_prob) -> None:
+    """Append a time-major (T, E, ...) batch: obs float32 (T, E, D), action int32 (T, E) or float32 (T, E, act_dim), reward / log_prob
+    float32, done / truncated uint8."""
+    _need_cuda(obs, action, reward, done, truncated, log_prob)
+    T, E = reward.shape
+    if E != ring.envs or tuple(obs.shape) != (T, E, ring.obs_dim) or obs.dtype != torch.float32 or not ring.action_ok(action, (T, E)) \
+            or done.dtype != torch.uint8 or truncated.dtype != torch.uint8 or log_prob.dtype != torch.float32 or reward.dtype != torch.float32:
+        raise StxError(f"replay_add_sequence: expected obs float32 (T, {ring.envs}, {ring.obs_dim}), the ring's action, float32 reward / log_prob, "
+                       "uint8 done / truncated")
+    _lib.check(_lib.load().stx_replay_add_sequence(C.byref(ring.c), _p(obs), _p(action), _p(reward), _p(done), _p(truncated), _p(log_prob), int(T),
+                                                   _stream()), "stx_replay_add_sequence")
+
+
+def replay_sample_sequence(ring: SequenceRing, S: int, seed: int, obs, action, reward, done, log_prob, period: int = 1,
+                           dev_counter: Optional[torch.Tensor] = None, idx_in: Optional[torch.Tensor] = None,
+                           idx_out: Optional[torch.Tensor] = None) -> None:
+    """Draw B = reward.shape[1] sequences of S rows into the time-major (S, B, ...) buffers.  idx_in (B, 2) int32 = (env, k-th valid start)
+    replaces the draws; idx_out (B, 2) int32 receives (env, start row)."""
+    _need_cuda(obs, action, reward, done, log_prob, dev_counter, idx_in, idx_out)
+    S_, B = reward.shape
+    if S_ != S or tuple(obs.shape) != (S, B, ring.obs_dim) or not ring.action_ok(action, (S, B)) or done.shape != (S, B) or log_prob.shape != (S, B):
+        raise StxError(f"replay_sample_sequence: outputs must be time-major ({S}, B, ...)")
+    for t in (idx_in, idx_out):
+        if t is not None and (t.dtype != torch.int32 or tuple(t.shape) != (B, 2)):
+            raise StxError("replay_sample_sequence: idx_in / idx_out must be int32 (B, 2)")
+    _lib.check(_lib.load().stx_replay_sample_sequence(C.byref(ring.c), int(B), int(S), int(period), int(seed) & ((1 << 64) - 1), 0, _p(dev_counter),
+                                                      _p(idx_in), _p(idx_out), _p(obs), _p(action), _p(reward), _p(done), _p(log_prob), _stream()),
+               "stx_replay_sample_sequence")
+
+
+def mpo_sample_actions(obs, logits_t, logits_b, action, log_prob, reward, done, N: int, xq, log_rho, r, d, gamma: float, max_abs_reward: float,
+                       stochastic: bool = True, seed: int = 0, dev_counter: Optional[torch.Tensor] = None, act_in: Optional[torch.Tensor] = None,
+                       act_out: Optional[torch.Tensor] = None, kind: str = "categorical", NL: int = 0, act_cont_out: Optional[torch.Tensor] = None,
+                       eps_in: Optional[torch.Tensor] = None, minimum: float = -1.0, maximum: float = 1.0, min_scale: float = 1e-3) -> None:
+    """The target-Q input rows of M states (include/stx.h, stx_mpo_sample_actions): xq ((NL + N + 1) M, D + A) = the NL actor-loss rows
+    (every action of a Categorical, NL = A; NL draws of the target tanh-Normal, kept unclipped in act_cont_out (NL, M, A)), N bootstrap
+    draws of logits_b (its mode with stochastic=False, N = 1), the stored action; plus log_rho, r, d (M)."""
+    _need_cuda(obs, logits_t, logits_b, action, log_prob, reward, done, xq, log_rho, r, d, dev_counter, act_in, act_out, act_cont_out, eps_in)
+    if kind not in ("categorical", "tanh_normal"):
+        raise StxError(f"mpo_sample_actions: kind {kind!r} is not categorical or tanh_normal")
+    tanh = kind == "tanh_normal"
+    M, D = obs.shape
+    W = int(logits_t.shape[-1])
+    A = W // 2 if tanh else W
+    NL = int(NL) if tanh else A
+    if not stochastic and N != 1:
+        raise StxError("mpo_sample_actions: the mode is one row per state (N = 1)")
+    if NL < 1 or tuple(logits_t.shape) != (M, W) or tuple(logits_b.shape) != (M, W) or tuple(xq.shape) != ((NL + N + 1) * M, D + A):
+        raise StxError(f"mpo_sample_actions: logits ({M}, {W}) and xq ((NL + N + 1) M, D + A) = ({(NL + N + 1) * M}, {D + A})")
+    if done.dtype != torch.uint8 or any(t.numel() != M for t in (log_prob, reward, done, log_rho, r, d)):
+        raise StxError("mpo_sample_actions: done uint8 (M), log_prob / reward / log_rho / r / d float32 (M)")
+    if tanh:
+        if action.dtype != torch.float32 or tuple(action.shape) != (M, A) or act_cont_out is None or act_cont_out.numel() != NL * M * A:
+            raise StxError(f"mpo_sample_actions: tanh-Normal actions float32 ({M}, {A}) and act_cont_out (NL, M, A)")
+        if eps_in is not None and (eps_in.dtype != torch.float32 or eps_in.numel() != (NL + N) * M * A):
+            raise StxError("mpo_sample_actions: eps_in must be float32 (NL + N, M, A)")
+    elif action.dtype != torch.int32 or action.numel() != M:
+        raise StxError("mpo_sample_actions: Categorical actions int32 (M)")
+    for t in (act_in, act_out):
+        if t is not None and (t.dtype != torch.int32 or t.numel() != N * M):
+            raise StxError("mpo_sample_actions: act_in / act_out must be int32 (N, M)")
+    s = _lib.StxMpoRows()
+    s.kind = _lib.STX_MPO_TANH_NORMAL if tanh else _lib.STX_MPO_CATEGORICAL
+    s.A, s.N, s.D, s.M, s.NL, s.stochastic, s.seed = A, int(N), int(D), int(M), NL, int(bool(stochastic)), int(seed) & ((1 << 64) - 1)
+    s.obs, s.logits_t, s.logits_b, s.action, s.log_prob = obs.data_ptr(), logits_t.data_ptr(), logits_b.data_ptr(), action.data_ptr(), log_prob.data_ptr()
+    s.reward, s.done, s.act_in, s.act_out = reward.data_ptr(), done.data_ptr(), _ptr_or_none(act_in), _ptr_or_none(act_out)
+    s.eps_in, s.act_cont_out = _ptr_or_none(eps_in), _ptr_or_none(act_cont_out)
+    s.xq, s.log_rho, s.r, s.d, s.gamma, s.max_abs_reward = xq.data_ptr(), log_rho.data_ptr(), r.data_ptr(), d.data_ptr(), float(gamma), float(max_abs_reward)
+    s.minimum, s.maximum, s.min_scale = float(minimum), float(maximum), float(min_scale)
+    _lib.check(_lib.load().stx_mpo_sample_actions(C.byref(s), 0, _p(dev_counter), _stream()), "stx_mpo_sample_actions")
+
+
+def _ptr_or_none(t: Optional[torch.Tensor]):
+    return None if t is None else t.data_ptr()
+
+
+def mpo_loss_grads(head, head_target, q, duals, d_head, dual_grad, metrics, epsilon: float, epsilon_policy: float, q_boot=None, v=None,
+                   weight: float = 1.0, overwrite: bool = True, scratch_key: str = "mpo_loss", kind: str = "categorical", actions=None,
+                   epsilon_stddev: float = 0.0, per_dim: bool = True, minimum: float = -1.0, maximum: float = 1.0, min_scale: float = 1e-3) -> None:
+    """The MPO loss of M states and its gradients (include/stx.h, stx_mpo_loss_grads).  Categorical: head / head_target / d_head (M, A),
+    q (A, M) target Q of every action, duals [log_temperature, log_alpha].  tanh-Normal: head / head_target / d_head (M, 2A), q (NL, M)
+    target Q of the NL draws `actions` (NL, M, A), duals [log_temperature, log_alpha_mean (C), log_alpha_stddev (C)] with C = A when
+    per_dim else 1; epsilon_policy is epsilon_mean.  With q_boot (N, M), v (M) = its mean over N."""
+    if kind not in ("categorical", "tanh_normal"):
+        raise StxError(f"mpo_loss_grads: kind {kind!r} is not categorical or tanh_normal")
+    tanh = kind == "tanh_normal"
+    dev = _need_cuda(head, head_target, q, duals, d_head, dual_grad, metrics, q_boot, v, actions)
+    M, W = head.shape
+    A = W // 2 if tanh else W
+    NL = q.numel() // M if tanh else A
+    if any(t.dtype != torch.float32 for t in (head, head_target, q, duals, d_head, dual_grad, metrics)):
+        raise StxError("mpo_loss_grads: every array must be float32")
+    if tuple(head_target.shape) != (M, W) or tuple(d_head.shape) != (M, W) or q.numel() != NL * M or NL < 1:
+        raise StxError(f"mpo_loss_grads: head_target / d_head ({M}, {W}), q (NL, {M})")
+    n_dual = 1 + (2 * (A if per_dim else 1) if tanh else 1)
+    if duals.numel() < n_dual or dual_grad.numel() < n_dual or metrics.numel() < _lib.STX_MPO_METRICS - 1:
+        raise StxError(f"mpo_loss_grads: duals / dual_grad need {n_dual} floats, metrics {_lib.STX_MPO_METRICS - 1}")
+    if tanh and (actions is None or actions.dtype != torch.float32 or actions.numel() != NL * M * A):
+        raise StxError(f"mpo_loss_grads: tanh-Normal actions float32 ({NL}, {M}, {A})")
+    N = 0
+    if q_boot is not None:
+        N = q_boot.numel() // M
+        if q_boot.dtype != torch.float32 or q_boot.numel() != N * M or N < 1 or v is None or v.numel() != M or v.dtype != torch.float32:
+            raise StxError("mpo_loss_grads: q_boot float32 (N, M) needs v float32 (M)")
+    lib = _lib.load()
+    scratch = _zeros_scratch((scratch_key,), lib.stx_mpo_loss_scratch_bytes(), dev)
+    s = _lib.StxMpoLoss()
+    s.kind = _lib.STX_MPO_TANH_NORMAL if tanh else _lib.STX_MPO_CATEGORICAL
+    s.A, s.N, s.overwrite, s.M, s.NL, s.per_dim = int(A), int(N), int(bool(overwrite)), int(M), int(NL), int(bool(per_dim))
+    s.head, s.head_target, s.q, s.q_boot, s.duals = head.data_ptr(), head_target.data_ptr(), q.data_ptr(), _ptr_or_none(q_boot), duals.data_ptr()
+    s.actions, s.v, s.d_head, s.dual_grad, s.metrics = _ptr_or_none(actions), _ptr_or_none(v), d_head.data_ptr(), dual_grad.data_ptr(), metrics.data_ptr()
+    s.epsilon, s.epsilon_policy, s.epsilon_stddev, s.weight = float(epsilon), float(epsilon_policy), float(epsilon_stddev), float(weight)
+    s.minimum, s.maximum, s.min_scale = float(minimum), float(maximum), float(min_scale)
+    _lib.check(lib.stx_mpo_loss_grads(C.byref(s), _p(scratch), _stream()), "stx_mpo_loss_grads")
+
+
+def retrace(q_t, v_t, r_t, discount_t, log_rho, lambda_: float, out: Optional[torch.Tensor] = None, c_t: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Time-major batch_general_off_policy_returns_from_q_and_v: v_t, r_t, discount_t (K, E), q_t (K-1, E); the weights are Retrace's
+    c = lambda min(1, exp(log_rho)) (log_rho (K-1, E)), or c_t (K-1, E) when given.  Returns the (K, E) targets."""
+    dev = _need_cuda(q_t, v_t, r_t, discount_t, log_rho, out, c_t)
+    K, E = v_t.shape
+    if (log_rho is None) == (c_t is None):
+        raise StxError("retrace: give exactly one of log_rho and c_t")
+    for t, shp in ((r_t, (K, E)), (discount_t, (K, E)), (q_t, (K - 1, E)), (log_rho, (K - 1, E)), (c_t, (K - 1, E)), (out, (K, E))):
+        if t is not None and (t.dtype != torch.float32 or tuple(t.shape) != shp):
+            raise StxError(f"retrace: v_t / r_t / discount_t float32 ({K}, {E}), q_t / log_rho ({K - 1}, {E})")
+    out = torch.empty((K, E), dtype=torch.float32, device=dev) if out is None else out
+    _lib.check(_lib.load().stx_retrace_f32(_p(q_t), _p(v_t), _p(r_t), _p(discount_t), _p(log_rho), _p(c_t), float(lambda_), int(K), int(E), _p(out), _stream()),
+               "stx_retrace_f32")
+    return out
+
+
+def mpo_q_grad(q, targets, dq, metric: Optional[torch.Tensor] = None, weight: float = 1.0) -> None:
+    """d of mean 0.5 (q - target)^2 over the first S-1 rows: q, dq (S, B), targets (S-1, B); metric (1) += weight * that loss."""
+    _need_cuda(q, targets, dq, metric)
+    S, B = q.shape
+    if tuple(targets.shape) != (S - 1, B) or tuple(dq.shape) != (S, B) or any(t.dtype != torch.float32 for t in (q, targets, dq)):
+        raise StxError(f"mpo_q_grad: q / dq float32 ({S}, {B}), targets ({S - 1}, {B})")
+    _lib.check(_lib.load().stx_mpo_q_grad(_p(q), _p(targets), int(S), int(B), _p(dq), _p(metric), float(weight), _stream()), "stx_mpo_q_grad")

@@ -1,5 +1,5 @@
-"""V-MPO state and parameter containers -- same fields and order as stoix/systems/mpo/mpo_types.py:13-73 (the MPO-only ones are not
-needed here); OnlineAndTarget as stoix/base_types.py."""
+"""MPO and V-MPO state and parameter containers -- same fields and order as stoix/systems/mpo/mpo_types.py:13-73; OnlineAndTarget as
+stoix/base_types.py."""
 from typing import Any, Dict, NamedTuple
 
 import torch
@@ -47,3 +47,24 @@ class VMPOLearnerState(NamedTuple):
     env_state: Any
     timestep: Any
     learner_step_count: torch.Tensor   # int32 (1) on the device: the actor segment's Adam count
+
+
+class MPOParams(NamedTuple):
+    actor_params: OnlineAndTarget
+    q_params: OnlineAndTarget
+    dual_params: Any
+
+
+class MPOOptStates(NamedTuple):
+    actor_opt_state: Any
+    q_opt_state: Any
+    dual_opt_state: Any
+
+
+class MPOLearnerState(NamedTuple):
+    params: MPOParams
+    opt_states: MPOOptStates
+    buffer_state: Any   # one SequenceBuffer per update-batch shard
+    key: Any
+    env_state: Any
+    timestep: Any

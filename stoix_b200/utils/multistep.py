@@ -136,3 +136,37 @@ def batch_n_step_bootstrapped_returns(
     tm = lambda x: x.to(torch.float32).transpose(0, 1).contiguous()
     targets, _ = ops.n_step_returns(tm(r_t), tm(discount_t), tm(v_t), int(n), lam)
     return targets.transpose(0, 1).contiguous()
+
+
+def batch_general_off_policy_returns_from_q_and_v(
+    q_t: Array,
+    v_t: Array,
+    r_t: Array,
+    discount_t: Array,
+    c_t: Array,
+    stop_target_gradients: bool = False,
+) -> Array:
+    """G_t = r_t + d_t (v_t - c_t q_t + c_t G_{t+1}) from G_{K-1} = r + d v (multistep.py:210-267), [B, K] inputs (q_t, c_t [B, K-1]),
+    in one launch of stx_retrace_f32 with the weights c_t as given.  The outputs carry no gradients."""
+    del stop_target_gradients
+    tm = lambda x: x.to(torch.float32).transpose(0, 1).contiguous()
+    out = ops.retrace(tm(q_t), tm(v_t), tm(r_t), tm(discount_t), None, 1.0, c_t=tm(c_t))
+    return out.transpose(0, 1).contiguous()
+
+
+def batch_retrace_continuous(
+    q_tm1: Array,
+    q_t: Array,
+    v_t: Array,
+    r_t: Array,
+    discount_t: Array,
+    log_rhos: Array,
+    lambda_: float,
+    stop_target_gradients: bool = True,
+) -> Array:
+    """Retrace error target - q_tm1 (multistep.py:270-311), [B, K] inputs (q_t, log_rhos [B, K-1]); one launch of stx_retrace_f32
+    computes the targets.  Only a scalar lambda_ is implemented."""
+    del stop_target_gradients
+    tm = lambda x: x.to(torch.float32).transpose(0, 1).contiguous()
+    target = ops.retrace(tm(q_t), tm(v_t), tm(r_t), tm(discount_t), tm(log_rhos), float(lambda_))
+    return target.transpose(0, 1) - q_tm1

@@ -99,3 +99,41 @@ class PrioritisedTrajectoryBuffer:
 
     def set_priorities(self, idx: torch.Tensor, priorities: torch.Tensor) -> None:
         ops.replay_set_priorities(self.ring, idx, priorities)
+
+
+class SequenceBuffer:
+    """fbx.make_trajectory_buffer as ff_mpo.py:539-546 builds it, on the sequence ring (stx_replay_add_sequence / _sample_sequence):
+    add_batch_size = E envs, max_length_time_axis = max_size // E time rows with one write index, sequences of sample_sequence_length
+    rows with period 1 that never straddle the write head.  `sample_into` writes the batch time-major (S, B, ...) into the epoch's
+    buffers."""
+
+    def __init__(self, max_size: int, sample_batch_size: int, sample_sequence_length: int, add_batch_size: int, obs_dim: int, device,
+                 period: int = 1, seed: int = 0, act_dim: int = 0):
+        if int(period) != 1:
+            raise ValueError(f"SequenceBuffer: period={period}; only period 1 is implemented (both MPO configs use 1)")
+        self.max_length_time_axis = int(max_size) // int(add_batch_size)
+        self.sample_batch_size, self.sample_sequence_length = int(sample_batch_size), int(sample_sequence_length)
+        if self.max_length_time_axis < self.sample_sequence_length:
+            raise ValueError(f"SequenceBuffer: max_size={max_size} over {add_batch_size} envs holds {self.max_length_time_axis} time rows, fewer "
+                             f"than one sequence of sample_sequence_length={self.sample_sequence_length}")
+        self.add_batch_size = int(add_batch_size)
+        self.ring = ops.SequenceRing(self.max_length_time_axis, self.add_batch_size, obs_dim, device, act_dim=act_dim)   # act_dim 0: int32
+        self.seed = int(seed) & ((1 << 62) - 1)
+        self.counter = torch.zeros(1, dtype=torch.int64, device=device)   # sample calls so far (device-resident RNG stream position)
+        self.added = 0                                                    # host mirror of the items added (T E per add)
+
+    def add(self, step) -> None:
+        """step: a time-major SequenceStep: .obs (T, E, D), .action (T, E) int32 or (T, E, act_dim) float32, .reward, .log_prob float32,
+        .done, .truncated uint8."""
+        ops.replay_add_sequence(self.ring, step.obs, step.action, step.reward, step.done, step.truncated, step.log_prob)
+        self.added += int(step.reward.numel())
+
+    def can_sample(self) -> bool:
+        """min_length_time_axis = sample_sequence_length time rows written."""
+        return min(self.added // self.add_batch_size, self.max_length_time_axis) >= self.sample_sequence_length
+
+    def sample_into(self, obs, action, reward, done, log_prob, idx_in: Optional[torch.Tensor] = None, idx_out: Optional[torch.Tensor] = None) -> None:
+        """Draw sample_batch_size sequences into the (S, B, ...) buffers; advances the stream position."""
+        ops.replay_sample_sequence(self.ring, self.sample_sequence_length, self.seed, obs, action, reward, done, log_prob,
+                                   dev_counter=self.counter.view(torch.int64), idx_in=idx_in, idx_out=idx_out)
+        ops.counter_add(self.counter, 1)
