@@ -66,8 +66,14 @@ typedef struct StxMlp {
   const float* params;                /* fp32 arena, stx_mlp_param_count() floats */
   const void* params_bf16;            /* bf16 shadow arena (same layout), STX_PREC_BF16 only; may be NULL for F32 */
   int32_t activation;                 /* STX_ACT_* of the torso layers (0 = relu) */
-  int32_t use_layer_norm;             /* 1: torso layers are Dense(no bias) + LayerNorm(eps 1e-6) */
+  int32_t use_layer_norm;             /* bit STX_LN_TORSO: torso layers are Dense(no bias) + LayerNorm(eps 1e-6);
+                                         bit STX_LN_FINAL: the last layer too, without activation (fp32 only) */
 } StxMlp;
+/* use_layer_norm bits.  STX_LN_FINAL is MLPTorso(use_layer_norm=True, activate_final=False) as DuelingQNetwork's branches use it
+ * (stoix/networks/torso.py, dueling.py): the last Dense has no bias and is followed by a LayerNorm (scale, bias) and no activation;
+ * its arena block is W, LayerNorm scale, LayerNorm bias like a torso layer's. */
+#define STX_LN_TORSO 1
+#define STX_LN_FINAL 2
 
 /* Hyper-parameters of _actor_loss_fn / _critic_loss_fn
  * (stoix/systems/ppo/anakin/ff_ppo.py:191-235; configs/system/ppo/ff_ppo.yaml:6-22). */
@@ -971,6 +977,86 @@ int stx_mpo_loss_grads(const StxMpoLoss* loss, void* scratch, void* stream);
 int stx_retrace_f32(const float* q_t, const float* v_t, const float* r_t, const float* discount_t, const float* log_rho, const float* c_t, float lambda_,
                     int K, int E, float* targets, void* stream);
 int stx_mpo_q_grad(const float* q, const float* targets, int S, int B, float* dq, float* metric, float weight, void* stream);
+
+/* ------------------------------------------------------------------ R2D2 (fp32): stoix/systems/q_learning/rec_r2d2.py ----
+ * Prioritised sequence ring with a period: fbx.make_prioritised_trajectory_buffer(max_size, min_length_time_axis = sample_sequence_length
+ *   = S, add_batch_size = E, period = p, priority_exponent) as rec_r2d2.py:644-653 builds it (tests/r2d2_oracle.py restates the rule).
+ *   Time-major storage, row (t, e) at t E + e, L = max_size // E time rows, one write index w for all envs, c = min(rows written, L).
+ *   Item i = e K + k (K = L // p, k < K) is the sequence of env e starting at ring row k p; rows past K p start no item.  With
+ *   age(row) = (w - 1 - row) mod L, the item is valid iff S - 1 <= age(k p) < c: its S rows are written and do not straddle the write
+ *   head (Rainbow's rule with n replaced by S).  Rows hold obs, action (int32), reward, done, truncated and reset_hidden_state; the
+ *   carry entering the step (RNNTransition.hstate; 2H for LSTM) is stored only at item-start rows, slot k E + e, since the loss reads
+ *   only hstate[0] of a sequence.  Priorities live in the sum tree of Rainbow's ring (fan-out STX_PRIO_FANOUT over the E K leaves).
+ *   add:    T rows at w .. w + T - 1 (mod L; only the newest L if T > L); then every item whose start row lies in w - S + 1 .. w + T - 1
+ *           (mod L, at most L rows) is re-evaluated: valid ones get *max_priority, the others 0; every parent is rebuilt.
+ *   sample: stratified as Rainbow's sampler, B strata: sequence b draws v = ((b + u_b) total) / B (u_b = u_in[b], or u01 of word b & 3
+ *           of Philox(seed; b / 4, call, call >> 32, 0x5052494F), call = offset + *dev_counter) and descends the tree.  Outputs are
+ *           time-major (S, B): obs (S, B, obs_dim), action, reward, done, reset; carry0 (B, carry_dim) = the stored carry of the item,
+ *           idx_out (B) the item, prob_out (B) = leaf / total.  With no valid item (total 0: at the reference default, L = 97, S = 80,
+ *           p = 40, the head often sits where no start row has S rows behind it) every draw is item 0 with prob 0; the loss's
+ *           1e-6 keeps its importance weights finite, and set_priorities then gives that item a priority.  That flashbax does the
+ *           same from an all-zero tree is inferred from its published rule, not checked against it.
+ *   set_priorities: Rainbow's: leaf idx[m] = priorities[m]^priority_exponent, the last of duplicate indices wins, ancestors rebuilt,
+ *           *max_priority raised.  Precondition, not checked on the device: every idx[m] is in [0, E K).
+ * stx_r2d2_loss_grads: rlax.transformed_n_step_q_learning with SIGNED_HYPERBOLIC_PAIR (rec_r2d2.py:331-384) over a learn window of T
+ *   rows of B sequences, q / q_target (T, B, A): a*_t = argmax_a q[t] (first maximum) and v_t = q_target[t, a*_t] for t = 1 .. T-1;
+ *   r_t = clip(reward, +-max_abs_reward), d_t = gamma (1 - done) (truncation does not cut the return, as in the reference), for
+ *   t < T-1.  Over seq = T - 1: targets_t = v[min(t + n - 1, seq - 1)], then for i = n-1 .. 0: targets_t = h(r_{t+i} + d_{t+i}
+ *   h^-1(targets_t)) with r = 0 and d = 1 past the window; td_t = targets_t - q[t, action_t].  h(x) = sign(x)(sqrt(|x|+1) - 1) + eps x,
+ *   h^-1(x) = sign(x)(z^2 - 1), z = (sqrt(1 + 4 eps (eps + 1 + |x|)) - 1) / (2 eps), both evaluated without cancellation near 0
+ *   (stx_r2d2_value_transform exposes them).  loss_b = 0.5 sum_t td^2; w_b = (1 / (prob_b + 1e-6))^beta / max_b', beta =
+ *   optax.linear_schedule(beta0 -> 1 over beta_steps) at *count.  d_q (T, B, A) = -w_b td_t / B at (t, action_t) for t < T-1, 0
+ *   elsewhere; priorities_b = eta max_t |td| + (1 - eta) mean_t |td|; metrics[0..6) += weight (mean_b w_b loss_b, mean q, max_b
+ *   priority, mean_b priority, mean_b max_t |td|, mean_b mean_t |td|); td (seq, B, nullable) receives the TD errors.  One launch;
+ *   the batch sums are fp64 in sequence order.  scratch: stx_r2d2_loss_scratch_bytes(B), zeroed once.
+ * stx_dueling_q: q = v + (adv - mean_a adv) (rec_r2d2's DuelingQNetwork order) with v = *value, the value branch's final LayerNorm
+ *   bias: that LayerNorm normalises a single element, so its output is exactly its bias.  stx_dueling_q_backward: d_adv = dq - mean_a dq;
+ *   *d_value = weight sum dq (overwrite) or += (rows then threads in a fixed order). */
+#define STX_R2D2_METRICS 6
+typedef struct StxR2d2Ring {
+  float* obs;                 /* (L, E, obs_dim) */
+  int32_t* action;            /* (L, E) */
+  float* reward;
+  uint8_t* done;
+  uint8_t* truncated;
+  uint8_t* reset;             /* reset_hidden_state */
+  float* carry;               /* (L // period, E, carry_dim) */
+  float* tree;                /* stx_r2d2_tree_floats() floats, zero-initialised */
+  int64_t* state;             /* {write index, min(rows written, L)} */
+  float* max_priority;        /* 1.0 initially */
+  int32_t* owner;             /* (E (L // period)) int32, -1 between calls */
+  int64_t length;             /* L */
+  int32_t envs, obs_dim, carry_dim, seq_len, period;
+  float priority_exponent;
+} StxR2d2Ring;
+typedef struct StxR2d2Loss {
+  int32_t T, B, A, n;         /* learn rows, sequences, actions, n-step */
+  const float* q;             /* (T, B, A) online Q */
+  const float* q_target;      /* (T, B, A) target Q */
+  const int32_t* action;      /* (T, B) */
+  const float* reward;        /* (T, B) */
+  const uint8_t* done;        /* (T, B) */
+  const float* prob;          /* (B) */
+  const int32_t* count;       /* Adam count word, nullable = 0 */
+  float* d_q;                 /* (T, B, A) */
+  float* priorities;          /* (B) */
+  float* metrics;             /* STX_R2D2_METRICS */
+  float* td;                  /* (T - 1, B), nullable */
+  float gamma, max_abs_reward, eta, tx_eps;
+  float beta0, beta_steps, weight;
+  int32_t reserved;
+} StxR2d2Loss;
+int64_t stx_r2d2_tree_floats(const StxR2d2Ring* rb);
+int stx_r2d2_ring_add(const StxR2d2Ring* rb, const float* obs, const int32_t* action, const float* reward, const uint8_t* done,
+                      const uint8_t* truncated, const uint8_t* reset, const float* carry, int T, void* stream);
+int stx_r2d2_ring_sample(const StxR2d2Ring* rb, int B, uint64_t seed, uint64_t offset, const uint64_t* dev_counter, const float* u_in, float* obs,
+                         int32_t* action, float* reward, uint8_t* done, uint8_t* reset, float* carry0, int32_t* idx_out, float* prob_out, void* stream);
+int stx_r2d2_ring_set_priorities(const StxR2d2Ring* rb, const int32_t* idx, const float* priorities, int64_t M, void* stream);
+int stx_r2d2_value_transform(const float* x, int64_t n, int inverse, float eps, float* out, void* stream);
+size_t stx_r2d2_loss_scratch_bytes(int B);
+int stx_r2d2_loss_grads(const StxR2d2Loss* loss, void* scratch, void* stream);
+int stx_dueling_q(const float* adv, const float* value, int64_t M, int A, float* q, void* stream);
+int stx_dueling_q_backward(const float* d_q, int64_t M, int A, float* d_adv, float* d_value, float weight, int overwrite, void* stream);
 
 /* Utility casts used by the bf16 path (obs / weight shadows). */
 int stx_cast_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream);

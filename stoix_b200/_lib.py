@@ -306,6 +306,26 @@ class StxMpoLoss(C.Structure):
                 ("weight", C.c_float), ("minimum", C.c_float), ("maximum", C.c_float), ("min_scale", C.c_float), ("reserved", C.c_int32)]
 
 
+STX_LN_TORSO = 1
+STX_LN_FINAL = 2
+STX_R2D2_METRICS = 6
+
+
+class StxR2d2Ring(C.Structure):
+    _fields_ = [("obs", C.c_void_p), ("action", C.c_void_p), ("reward", C.c_void_p), ("done", C.c_void_p), ("truncated", C.c_void_p),
+                ("reset", C.c_void_p), ("carry", C.c_void_p), ("tree", C.c_void_p), ("state", C.c_void_p), ("max_priority", C.c_void_p),
+                ("owner", C.c_void_p), ("length", C.c_int64), ("envs", C.c_int32), ("obs_dim", C.c_int32), ("carry_dim", C.c_int32),
+                ("seq_len", C.c_int32), ("period", C.c_int32), ("priority_exponent", C.c_float)]
+
+
+class StxR2d2Loss(C.Structure):
+    _fields_ = [("T", C.c_int32), ("B", C.c_int32), ("A", C.c_int32), ("n", C.c_int32), ("q", C.c_void_p), ("q_target", C.c_void_p),
+                ("action", C.c_void_p), ("reward", C.c_void_p), ("done", C.c_void_p), ("prob", C.c_void_p), ("count", C.c_void_p),
+                ("d_q", C.c_void_p), ("priorities", C.c_void_p), ("metrics", C.c_void_p), ("td", C.c_void_p), ("gamma", C.c_float),
+                ("max_abs_reward", C.c_float), ("eta", C.c_float), ("tx_eps", C.c_float), ("beta0", C.c_float), ("beta_steps", C.c_float),
+                ("weight", C.c_float), ("reserved", C.c_int32)]
+
+
 _P = C.c_void_p
 _SIGNATURES = {
     # name: (restype, argtypes)
@@ -433,6 +453,15 @@ _SIGNATURES = {
     "stx_mpo_loss_grads": (C.c_int, [C.POINTER(StxMpoLoss), _P, _P]),
     "stx_retrace_f32": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_float, C.c_int, C.c_int, _P, _P]),
     "stx_mpo_q_grad": (C.c_int, [_P, _P, C.c_int, C.c_int, _P, _P, C.c_float, _P]),
+    "stx_r2d2_tree_floats": (C.c_int64, [C.POINTER(StxR2d2Ring)]),
+    "stx_r2d2_ring_add": (C.c_int, [C.POINTER(StxR2d2Ring), _P, _P, _P, _P, _P, _P, _P, C.c_int, _P]),
+    "stx_r2d2_ring_sample": (C.c_int, [C.POINTER(StxR2d2Ring), C.c_int, C.c_uint64, C.c_uint64, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "stx_r2d2_ring_set_priorities": (C.c_int, [C.POINTER(StxR2d2Ring), _P, _P, C.c_int64, _P]),
+    "stx_r2d2_value_transform": (C.c_int, [_P, C.c_int64, C.c_int, C.c_float, _P, _P]),
+    "stx_r2d2_loss_scratch_bytes": (C.c_size_t, [C.c_int]),
+    "stx_r2d2_loss_grads": (C.c_int, [C.POINTER(StxR2d2Loss), _P, _P]),
+    "stx_dueling_q": (C.c_int, [_P, _P, C.c_int64, C.c_int, _P, _P]),
+    "stx_dueling_q_backward": (C.c_int, [_P, C.c_int64, C.c_int, _P, _P, C.c_float, C.c_int, _P]),
 }
 
 _lib = None

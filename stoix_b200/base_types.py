@@ -44,6 +44,20 @@ class OnPolicyLearnerState(NamedTuple):
     timestep: Any
 
 
+class RNNOffPolicyLearnerState(NamedTuple):
+    """stoix.base_types.RNNOffPolicyLearnerState (rec_r2d2): per update-batch shard lists of buffers, env states, timesteps, the
+    done / truncated flags of the last step and the carried hidden states."""
+    params: Any
+    opt_states: Any
+    buffer_state: Any
+    key: Any
+    env_state: Any
+    timestep: Any
+    done: Any
+    truncated: Any
+    hstates: Any
+
+
 class AnakinExperimentOutput(NamedTuple, Generic[StoixState]):
     """stoix/base_types.py:172-177."""
 

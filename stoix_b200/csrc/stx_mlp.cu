@@ -23,13 +23,18 @@ int check_mlp(const StxMlp* m, const char* who) {
     STX_REQUIRE(m->sizes[i] > 0, STX_E_SHAPE, "%s: sizes[%d]=%d", who, i, m->sizes[i]);
   STX_REQUIRE(m->params != nullptr, STX_E_ARG, "%s: null params", who);
   STX_REQUIRE(m->activation >= STX_ACT_RELU && m->activation <= STX_ACT_IDENTITY, STX_E_ARG, "%s: activation=%d", who, m->activation);
+  STX_REQUIRE(m->use_layer_norm >= 0 && m->use_layer_norm <= (STX_LN_TORSO | STX_LN_FINAL), STX_E_ARG, "%s: use_layer_norm=%d", who, m->use_layer_norm);
   if (m->use_layer_norm)
-    for (int i = 1; i < m->n_layers; ++i)
-      STX_REQUIRE(m->sizes[i] <= 32 * simt::kLnMaxCols, STX_E_SHAPE, "%s: LayerNorm width %d > %d", who, m->sizes[i], 32 * simt::kLnMaxCols);
+    for (int i = 1; i <= m->n_layers; ++i)
+      STX_REQUIRE(m->sizes[i] <= 32 * simt::kLnMaxCols || (i == m->n_layers && !(m->use_layer_norm & STX_LN_FINAL)), STX_E_SHAPE,
+                  "%s: LayerNorm width %d > %d", who, m->sizes[i], 32 * simt::kLnMaxCols);
   return STX_OK;
 }
 
-inline bool layer_has_ln(const StxMlp* m, int i) { return m->use_layer_norm && i < m->n_layers - 1; }
+inline bool final_ln(const StxMlp* m) { return (m->use_layer_norm & STX_LN_FINAL) != 0; }
+inline bool layer_has_ln(const StxMlp* m, int i) {
+  return i < m->n_layers - 1 ? (m->use_layer_norm & STX_LN_TORSO) != 0 : final_ln(m);
+}
 
 int max_width(const StxMlp* m) {
   int w = 0;
@@ -66,7 +71,9 @@ int simt_forward(const StxMlp* m, const float* x, int64_t ldx, const int32_t* ro
     g.B = m->params + woff[i];
     g.bias = ln ? nullptr : m->params + boff[i];  // torso.py:26: use_bias = not use_layer_norm
     g.M = M, g.N = m->sizes[i + 1], g.K = m->sizes[i];
-    if (last) {
+    if (last && ln) {  // STX_LN_FINAL: U, then out = LN(U) without activation
+      g.C = acts[i + 1] ? acts[i + 1] : out;
+    } else if (last) {
       g.C = out;
     } else if (ln) {   // U now; H = f(LN(U)) by ln_apply_kernel (inference: in place on the H buffer)
       g.C = acts[i + 1] ? acts[i + 1] : hacts[i + 1];
@@ -77,8 +84,8 @@ int simt_forward(const StxMlp* m, const float* x, int64_t ldx, const int32_t* ro
     STX_CUDA_OK(simt::launch_gemm<simt::FWD>(g, 1, st));
     if (ln) {
       const float* gamma = m->params + boff[i];
-      simt::ln_apply_kernel<<<(unsigned)((M + 7) / 8), 256, 0, st>>>(g.C, M, g.N, gamma, gamma + g.N, m->activation, stats ? stats[i + 1] : nullptr,
-                                                                     hacts[i + 1]);
+      simt::ln_apply_kernel<<<(unsigned)((M + 7) / 8), 256, 0, st>>>(g.C, M, g.N, gamma, gamma + g.N, last ? STX_ACT_IDENTITY : m->activation,
+                                                                     stats ? stats[i + 1] : nullptr, last ? out : hacts[i + 1]);
       STX_LAUNCH_OK();
     }
     in = last ? out : hacts[i + 1], ld = g.N, ridx = nullptr;
@@ -244,6 +251,10 @@ SimtPpoWs carve(const StxMlp* m, int64_t mb, char* base) {
   w.splits = pick_splits(m, mb);
   w.partials = reinterpret_cast<float*>(take((size_t)w.splits * stx_mlp_param_count(m) * 4));
   w.loss_partials = reinterpret_cast<double*>(take(((size_t)(mb + 255) / 256) * 6 * 8));
+  if (final_ln(m)) {   // the last layer's U and LayerNorm statistics
+    w.acts[m->n_layers] = reinterpret_cast<float*>(take((size_t)mb * m->sizes[m->n_layers] * 4));
+    w.stats[m->n_layers] = reinterpret_cast<float*>(take((size_t)mb * 2 * 4));
+  }
   w.bytes = o;
   return w;
 }
@@ -258,6 +269,16 @@ int simt_backward(const StxMlp* m, const float* x, int64_t ldx, const int32_t* r
   const int64_t rows_per_split = (mb + ws.splits - 1) / ws.splits;
   const float* dY = ws.dhead;
   int pp = 0;
+  if (final_ln(m)) {   // d out -> d U of the last layer in place, and d(scale | bias) of its LayerNorm
+    const int n = m->n_layers, w = m->sizes[n];
+    const float* gamma = m->params + boff[n - 1];
+    STX_CUDA_OK(simt::launch_ln_backward(ws.dhead, ws.acts[n], ws.stats[n], gamma, gamma + w, STX_ACT_IDENTITY, mb, w, ws.ln_rows, ws.ln_blocks,
+                                         ws.ln_part, st));
+    if (net_grad != nullptr)
+      simt::reduce_partials_kernel<<<(unsigned)((2 * w + 255) / 256), 256, 0, st>>>(ws.ln_part, ws.ln_blocks, 2 * (int64_t)w, 2 * (int64_t)w, grad_weight,
+                                                                                  net_grad + boff[n - 1], overwrite);
+    STX_LAUNCH_OK();
+  }
   for (int i = m->n_layers - 1; i >= 0; --i) {
     const int nin = m->sizes[i], nout = m->sizes[i + 1];
     // dW_i, db_i partials: input of layer i is x (gathered) for i == 0, else the stored layer output H_i
@@ -344,7 +365,7 @@ extern "C" int64_t stx_mlp_param_count(const StxMlp* m) {
   if (!m) return 0;
   int64_t o = 0;
   for (int i = 0; i < m->n_layers; ++i)
-    o += (int64_t)m->sizes[i] * m->sizes[i + 1] + ((m->use_layer_norm && i < m->n_layers - 1) ? 2 : 1) * (int64_t)m->sizes[i + 1];
+    o += (int64_t)m->sizes[i] * m->sizes[i + 1] + (layer_has_ln(m, i) ? 2 : 1) * (int64_t)m->sizes[i + 1];
   return o;
 }
 
@@ -364,8 +385,10 @@ extern "C" int stx_mlp_forward(const StxMlp* m, const void* x, int64_t ldx, cons
   STX_REQUIRE(ldx >= m->sizes[0], STX_E_SHAPE, "stx_mlp_forward: ldx=%lld < in dim %d", (long long)ldx, m->sizes[0]);
   STX_REQUIRE(workspace_bytes >= stx_mlp_forward_workspace_bytes(m, M, precision) && workspace, STX_E_WORKSPACE,
               "stx_mlp_forward: workspace %zu < %zu", workspace_bytes, stx_mlp_forward_workspace_bytes(m, M, precision));
-  if (precision == STX_PREC_BF16)
+  if (precision == STX_PREC_BF16) {
+    STX_REQUIRE(!final_ln(m), STX_E_UNSUPPORTED, "stx_mlp_forward: a final LayerNorm has no bf16 kernel");
     return tc_mlp_forward(m, x, ldx, row_idx, M, out, workspace, workspace_bytes, (cudaStream_t)stream);
+  }
   STX_REQUIRE(precision == STX_PREC_F32, STX_E_UNSUPPORTED, "stx_mlp_forward: precision=%d", precision);
   float* acts[STX_MAX_LAYERS + 1] = {nullptr};   // inference: pre-activations are not kept
   float* hacts[STX_MAX_LAYERS + 1] = {nullptr};

@@ -4,13 +4,15 @@
 // Reference: NoisyLinear (stoix/networks/layers.py:71-169), NoisyDistributionalDuelingQNetwork (stoix/networks/dueling.py:90-124), and
 // fbx.make_prioritised_trajectory_buffer with the n-step target of stoix/systems/q_learning/ff_rainbow.py:222-246.
 #include "stx_common.cuh"
+#include "stx_prio_tree.cuh"
 
 namespace stx {
 namespace {
 
+using prio::kTreeThreads;
+using prio::tree_rebuild;
+
 constexpr uint32_t kNoiseTag = 0x4E4F4953u;  // "NOIS"
-constexpr uint32_t kPrioTag = 0x5052494Fu;   // "PRIO"
-constexpr int kTreeThreads = 1024;           // the one CTA that rewrites leaves and rebuilds their ancestors
 
 // ---- noisy layers ----------------------------------------------------------------------------------------------------------------
 
@@ -115,45 +117,6 @@ __global__ void dueling_backward_kernel(const float* __restrict__ dq, int64_t M,
   for (int a = 0; a < A; ++a) row[N + (int64_t)a * N + i] = __fsub_rn(g[(int64_t)a * N], mean);
 }
 
-// ---- prioritised ring: sum tree ---------------------------------------------------------------------------------------------------
-
-struct TreeLevels {
-  int n;               // levels, leaves first, the root last
-  int64_t off[16], cnt[16];
-};
-
-__host__ __device__ inline TreeLevels tree_levels(int64_t items) {
-  TreeLevels t;
-  int64_t o = 0, c = items;
-  t.n = 0;
-  for (;;) {
-    t.off[t.n] = o, t.cnt[t.n] = c, ++t.n;
-    o += c;
-    if (c <= 1) break;
-    c = (c + STX_PRIO_FANOUT - 1) / STX_PRIO_FANOUT;
-  }
-  return t;
-}
-
-// Rebuild the ancestors of the dirty leaves leaf(0 .. nd-1), level by level, each parent as the sum of its children in index order.
-// Several dirty leaves share a parent: each of their threads writes the same sum.  Whole CTA.
-template <class Leaf>
-__device__ void tree_rebuild(float* __restrict__ tree, const TreeLevels& t, int64_t nd, Leaf leaf) {
-  for (int l = 1; l < t.n; ++l) {
-    __syncthreads();
-    int64_t span = 1;
-    for (int k = 0; k < l; ++k) span *= STX_PRIO_FANOUT;
-    for (int64_t j = threadIdx.x; j < nd; j += blockDim.x) {
-      const int64_t node = leaf(j) / span, c0 = node * STX_PRIO_FANOUT;
-      const int64_t c1 = min(c0 + STX_PRIO_FANOUT, t.cnt[l - 1]);
-      const float* ch = tree + t.off[l - 1];
-      float s = 0.f;
-      for (int64_t c = c0; c < c1; ++c) s = __fadd_rn(s, ch[c]);
-      tree[t.off[l] + node] = s;
-    }
-  }
-}
-
 // ---- prioritised ring: add --------------------------------------------------------------------------------------------------------
 
 // Rows (t, e) of the (T, E) batch, t >= skip, into ring row (w + t) mod L; one warp per row.
@@ -188,7 +151,7 @@ __global__ void __launch_bounds__(kTreeThreads) prio_add_kernel(StxReplayPriorit
     const int64_t p = (start + j % W) % L, age = ((w1 - 1 - p) % L + L) % L;
     rb.tree[leaf(j)] = (age >= n - 1 && age < c1) ? maxp : 0.f;
   }
-  tree_rebuild(rb.tree, tree_levels(E * L), E * W, leaf);
+  tree_rebuild(rb.tree, E * L, E * W, leaf);
   __syncthreads();
   if (threadIdx.x == 0) {
     rb.state[0] = w1;
@@ -210,35 +173,11 @@ __global__ void __launch_bounds__(256) prio_sample_kernel(StxReplayPrioritised r
                                                           unsigned int* __restrict__ ticket) {
   const int64_t r = blockIdx.x * (int64_t)(blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
-  const TreeLevels t = tree_levels((int64_t)rb.envs * rb.length);
+  const int64_t items = (int64_t)rb.envs * rb.length;
   if (r < M) {
-    float u;
-    if (u_in) {
-      u = u_in[r];
-    } else {
-      const uint64_t call = offset + (counter ? *counter : 0ull);
-      const uint4 wd = Philox::rand4(make_uint4((uint32_t)(r >> 2), (uint32_t)call, (uint32_t)(call >> 32), kPrioTag),
-                                     make_uint2((uint32_t)seed, (uint32_t)(seed >> 32)));
-      const uint32_t v4[4] = {wd.x, wd.y, wd.z, wd.w};
-      u = u01(v4[r & 3]);
-    }
-    const float total = rb.tree[t.off[t.n - 1]];
-    float v = __fdiv_rn(__fmul_rn(__fadd_rn((float)r, u), total), (float)M);
-    int64_t node = 0;  // index within level l
-    for (int l = t.n - 1; l > 0; --l) {
-      const int64_t c0 = node * STX_PRIO_FANOUT, nc = min((int64_t)STX_PRIO_FANOUT, t.cnt[l - 1] - c0);
-      const float s_lane = lane < nc ? rb.tree[t.off[l - 1] + c0 + lane] : 0.f;
-      int pick = -1, last_pos = 0;
-      for (int c = 0; c < nc; ++c) {  // every lane runs the same sequence on the same values
-        const float s = __shfl_sync(0xffffffffu, s_lane, c);
-        if (s > 0.f) last_pos = c;
-        if (pick < 0) {
-          if (v < s) pick = c;
-          else v = __fsub_rn(v, s);
-        }
-      }
-      node = c0 + (pick < 0 ? last_pos : pick);
-    }
+    const uint64_t call = offset + (counter ? *counter : 0ull);
+    const float total = rb.tree[prio::root_offset(items)];
+    const int64_t node = prio::tree_descend(rb.tree, items, r, prio::stratum_uniform(r, seed, call, u_in), M);
     const int64_t i = node, L = rb.length, E = rb.envs, e = i / L, p = i % L;
     const int n = rb.n_step, D = rb.obs_dim;
     const int64_t s0 = p * E + e, sn = ((p + n - 1) % L) * E + e;
@@ -287,32 +226,9 @@ __global__ void __launch_bounds__(256) prio_sample_kernel(StxReplayPrioritised r
 
 // ---- prioritised ring: set_priorities ---------------------------------------------------------------------------------------------
 
-// Duplicates in O(M): every row claims its leaf with an integer atomicMax of its batch position in rb.owner (-1 between calls), so
-// the last occurrence in batch order owns the leaf whatever the scheduling; the owner writes the value and resets the claim after
-// the rebuild.
 __global__ void __launch_bounds__(kTreeThreads) prio_set_kernel(StxReplayPrioritised rb, const int32_t* __restrict__ idx, const float* __restrict__ pr,
                                                                 int64_t M) {
-  __shared__ float red[kTreeThreads / 32];
-  for (int64_t m = threadIdx.x; m < M; m += blockDim.x) atomicMax(rb.owner + idx[m], (int)m);
-  __syncthreads();
-  float mx = -INFINITY;
-  for (int64_t m = threadIdx.x; m < M; m += blockDim.x) {
-    const float v = powf(pr[m], rb.priority_exponent);
-    mx = fmaxf(mx, v);
-    if (rb.owner[idx[m]] == (int)m) rb.tree[idx[m]] = v;
-  }
-#pragma unroll
-  for (int k = 16; k > 0; k >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, k));
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
-  __syncthreads();
-  tree_rebuild(rb.tree, tree_levels((int64_t)rb.envs * rb.length), M, [&](int64_t j) { return (int64_t)idx[j]; });
-  __syncthreads();  // every owner test above is done before the claims are cleared
-  for (int64_t m = threadIdx.x; m < M; m += blockDim.x) rb.owner[idx[m]] = -1;
-  if (threadIdx.x == 0) {
-    float m = red[0];
-    for (int k = 1; k < (int)(blockDim.x >> 5); ++k) m = fmaxf(m, red[k]);
-    *rb.max_priority = fmaxf(*rb.max_priority, m);
-  }
+  prio::set_priorities(rb.tree, rb.owner, rb.max_priority, rb.priority_exponent, (int64_t)rb.envs * rb.length, idx, pr, M);
 }
 
 bool noisy_ok(const StxNoisyNet* net, int64_t* blocks) {
@@ -371,8 +287,7 @@ extern "C" int stx_dueling_backward(const float* d_q_logits, int64_t M, int A, i
 
 extern "C" int64_t stx_prio_tree_floats(int64_t items) {
   if (items <= 0) return 0;
-  const TreeLevels t = tree_levels(items);
-  return t.off[t.n - 1] + 1;
+  return prio::root_offset(items) + 1;
 }
 
 extern "C" size_t stx_prio_scratch_bytes(void) { return 256; }

@@ -23,6 +23,24 @@ from .. import ops
 from .base import ParamTree, _lecun_normal
 from .heads import DistributionalDiscreteQNetwork, EpsilonGreedy, _seed_to_int
 from .torso import NoisyMLPTorso
+from .utils import parse_activation_fn
+
+
+class DuelingQNetwork:
+    """dueling.py:15-49: value MLPTorso((*layer_sizes, 1)) and advantage MLPTorso((*layer_sizes, A)) branches with activate_final=False,
+    q = v + (adv - mean_a adv), returning EpsilonGreedy(q, epsilon).  A description: the recurrent Q network (networks/recurrent.py)
+    runs it; only its use_layer_norm=True form is built, where the value branch's output is its final LayerNorm bias."""
+
+    def __init__(self, action_dim: int, epsilon: float, layer_sizes: Sequence[int], activation: str = "relu", use_layer_norm: bool = False,
+                 kernel_init: Optional[float] = None):
+        self.action_dim, self.epsilon = int(action_dim), float(epsilon)
+        self.branch_sizes = tuple(int(s) for s in layer_sizes)
+        self.activation, self.use_layer_norm = parse_activation_fn(activation), bool(use_layer_norm)
+        self.out_dim = self.action_dim
+        self.kernel_init_scale = float(np.sqrt(2.0)) if kernel_init is None else float(kernel_init)   # dueling.py:23
+
+    def distribution(self, q_values: torch.Tensor, epsilon: Optional[float] = None) -> EpsilonGreedy:
+        return EpsilonGreedy(q_values, self.epsilon if epsilon is None else epsilon)
 
 
 class NoisyDistributionalDuelingQNetwork(DistributionalDiscreteQNetwork):

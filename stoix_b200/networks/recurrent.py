@@ -3,7 +3,13 @@
 One flat fp32 arena per network: [pre-torso Dense layers | W_i (P x 3H, columns r|z|n) | b_i (3H) | W_h (H x 3H) | b_hn (H) |
 post-torso Dense layers | head].  `spec_pre` = MLP(D, *pre_sizes, 3H) -- the input projections of the cell are its "head"
 (Dense with bias, no activation) -- and `spec_post` = MLP(H, *post_sizes, out).  The parameter tree exposes flax's names
-(params / pre_torso / ScannedRNN_0 / GRUCell_0 / {ir, iz, in, hr, hz, hn} / post_torso / head) as views into the arena."""
+(params / pre_torso / ScannedRNN_0 / GRUCell_0 / {ir, iz, in, hr, hz, hn} / post_torso / head) as views into the arena.
+
+With a DuelingQNetwork head (R2D2), `spec_post` = MLP(H, *post_sizes, *branch_sizes, A) runs the post-torso and the advantage
+branch (MLPTorso_1, activate_final=False: its last Dense has no bias and is followed by a LayerNorm, MlpSpec.ln_final) as one chain,
+and the value branch (MLPTorso_0) follows in the arena as `spec_value` = MLP(post_out, *branch_sizes, 1), in the same form.  That
+branch ends in a LayerNorm over one element, whose output is exactly its bias: the network computes Q = v + (adv - mean adv) with
+v = that bias (stx_dueling_q) and never runs the rest of the branch, whose gradient is exactly zero."""
 from __future__ import annotations
 
 from typing import Any, Dict, Optional, Tuple
@@ -37,17 +43,31 @@ class RecLayout:
     """Offsets of the blocks of one recurrent network inside its flat arena."""
 
     def __init__(self, obs_dim: int, pre_sizes, H: int, post_sizes, out_dim: int, activation_pre: str, ln_pre: bool, activation_post: str, ln_post: bool,
-                 cell_type: str = "gru"):
+                 cell_type: str = "gru", branch_sizes=None):
         self.H, self.cell_type = int(H), cell_type
         self.G = 3 if cell_type == "gru" else 4                   # gate blocks of W_i / W_h
         self.S = self.H if cell_type == "gru" else 2 * self.H     # carry width
         self.spec_pre = ops.MlpSpec((int(obs_dim), *[int(s) for s in pre_sizes], self.G * self.H), activation=activation_pre, use_layer_norm=ln_pre)
-        self.spec_post = ops.MlpSpec((self.H, *[int(s) for s in post_sizes], int(out_dim)), activation=activation_post, use_layer_norm=ln_post)
+        self.dueling = branch_sizes is not None
+        self.n_post_torso = len(post_sizes)
+        branch = [int(s) for s in branch_sizes] if self.dueling else []
+        self.spec_post = ops.MlpSpec((self.H, *[int(s) for s in post_sizes], *branch, int(out_dim)), activation=activation_post, use_layer_norm=ln_post,
+                                     ln_final=self.dueling)
         self.off_pre = 0
         self.off_wh = self.spec_pre.param_count
         self.off_bhn = self.off_wh + self.H * self.G * self.H
         self.off_post = self.off_bhn + (self.H if cell_type == "gru" else 0)   # lstm: the hidden biases are the bias of W_i
-        self.param_count = self.off_post + self.spec_post.param_count
+        self.off_value = self.off_post + self.spec_post.param_count
+        self.spec_value = None
+        if self.dueling:
+            post_out = int(post_sizes[-1]) if len(post_sizes) else self.H
+            self.spec_value = ops.MlpSpec((post_out, *branch, 1), activation=activation_post, use_layer_norm=True, ln_final=True)
+        self.param_count = self.off_value + (self.spec_value.param_count if self.dueling else 0)
+
+    def value_bias(self, flat: torch.Tensor) -> torch.Tensor:
+        """The (1,) view of the value branch's final LayerNorm bias: the value of every state."""
+        sl = self.spec_value.ln_bias_slices()[-1]
+        return flat[self.off_value + sl.start: self.off_value + sl.stop]
 
     def blocks(self, flat: torch.Tensor):
         """(pre arena, W_h (H, G*H), b_hn (H; empty for lstm), post arena) views."""
@@ -80,7 +100,7 @@ class _Recurrent:
     def layout_for(self, obs_dim: int) -> RecLayout:
         return RecLayout(obs_dim, self.pre_torso.layer_sizes, self.hidden_state_dim, self.post_torso.layer_sizes, self.head.out_dim,
                          self.pre_torso.activation, self.pre_torso.use_layer_norm, self.post_torso.activation, self.post_torso.use_layer_norm,
-                         self.cell_type)
+                         self.cell_type, getattr(self.head, "branch_sizes", None))
 
     def build_tree(self, lay: RecLayout, flat: torch.Tensor) -> ParamTree:
         H = lay.H
@@ -101,9 +121,14 @@ class _Recurrent:
             for g, nm in enumerate("ifgo"):
                 cell["i" + nm] = {"kernel": blk(w_i, g)}
                 cell["h" + nm] = {"kernel": blk(w_h, g), "bias": blk(b_i, g)}
+        if lay.dueling:   # DuelingQNetwork: MLPTorso_0 = value branch, MLPTorso_1 = advantage branch
+            n_t, sv = lay.n_post_torso, lay.spec_value
+            head = {"MLPTorso_0": _dense_tree(sv, flat[lay.off_value: lay.param_count], 0, sv.n_layers),
+                    "MLPTorso_1": _dense_tree(lay.spec_post, post, n_t, n_post)}
+        else:
+            n_t, head = n_post - 1, _dense_tree(lay.spec_post, post, n_post - 1, n_post)
         tree = ParamTree({"params": {"pre_torso": _dense_tree(lay.spec_pre, pre, 0, n_pre - 1), "ScannedRNN_0": {cell_name: cell},
-                                     "post_torso": _dense_tree(lay.spec_post, post, 0, n_post - 1),
-                                     self.head_name: _dense_tree(lay.spec_post, post, n_post - 1, n_post)}})
+                                     "post_torso": _dense_tree(lay.spec_post, post, 0, n_t), self.head_name: head}})
         tree.flat, tree.layout, tree.spec, tree.flat_bf16 = flat[: lay.param_count], lay, lay.spec_post, None
         return tree
 
@@ -130,6 +155,11 @@ class _Recurrent:
                 if spec.has_ln(i):
                     host[off:][sl[i][1]] = 1.0
         host[lay.off_wh: lay.off_bhn].copy_(torch.cat([_orthogonal(gen, H, H, 1.0) for _ in range(lay.G)], dim=1).reshape(-1))
+        if lay.dueling:   # the value branch: orthogonal(kernel_init) kernels, LayerNorm scales 1, biases 0
+            sv, sl = lay.spec_value, lay.spec_value.layer_slices()
+            for i in range(sv.n_layers):
+                host[lay.off_value:][sl[i][0]] = _orthogonal(gen, sv.sizes[i], sv.sizes[i + 1], self.head.kernel_init_scale).reshape(-1)
+                host[lay.off_value:][sl[i][1]] = 1.0
         if flat is None:
             flat = torch.zeros(lay.param_count, dtype=torch.float32, device=obs.device)
         flat[: lay.param_count].copy_(host)
@@ -155,6 +185,8 @@ class _Recurrent:
             h_seq = ops.gru_sequence_forward(gi.view(T, E, 3 * lay.H), d8.contiguous(), hstate.contiguous(), w_h, b_hn, ws)
             last = h_seq[-1]
         out = ops.mlp_forward(lay.spec_post, post, h_seq.view(T * E, lay.H), ws_key=("rec_post", id(self)))
+        if lay.dueling:
+            out = ops.dueling_q(out, lay.value_bias(params.flat))
         return last, out.view(T, E, -1)
 
 

@@ -67,13 +67,14 @@ class MlpSpec:
     sizes: Tuple[int, ...]
     activation: str = "relu"
     use_layer_norm: bool = False
+    ln_final: bool = False   # MLPTorso(use_layer_norm=True, activate_final=False): last Dense without bias, LayerNorm, no activation
 
     @property
     def n_layers(self) -> int:
         return len(self.sizes) - 1
 
     def has_ln(self, i: int) -> bool:
-        return self.use_layer_norm and i < self.n_layers - 1
+        return (self.use_layer_norm and i < self.n_layers - 1) or (self.ln_final and i == self.n_layers - 1)
 
     @property
     def param_count(self) -> int:
@@ -111,7 +112,7 @@ class MlpSpec:
         for i, s in enumerate(self.sizes):
             m.sizes[i] = int(s)
         m.activation = _lib.STX_ACTIVATIONS[self.activation]
-        m.use_layer_norm = int(bool(self.use_layer_norm))
+        m.use_layer_norm = (_lib.STX_LN_TORSO if self.use_layer_norm else 0) | (_lib.STX_LN_FINAL if self.ln_final else 0)
         return m
 
 
@@ -1887,3 +1888,152 @@ def mpo_q_grad(q, targets, dq, metric: Optional[torch.Tensor] = None, weight: fl
     if tuple(targets.shape) != (S - 1, B) or tuple(dq.shape) != (S, B) or any(t.dtype != torch.float32 for t in (q, targets, dq)):
         raise StxError(f"mpo_q_grad: q / dq float32 ({S}, {B}), targets ({S - 1}, {B})")
     _lib.check(_lib.load().stx_mpo_q_grad(_p(q), _p(targets), int(S), int(B), _p(dq), _p(metric), float(weight), _stream()), "stx_mpo_q_grad")
+
+
+# ------------------------------------------------------------------------------------------------
+# R2D2: prioritised sequence ring with a period, dueling Q combine, fused transformed n-step double-Q loss
+# (stoix/systems/q_learning/rec_r2d2.py)
+# ------------------------------------------------------------------------------------------------
+
+R2D2_METRICS = ("q_loss", "mean_q", "max_priority", "mean_priority", "max_seq_td_error", "mean_seq_td_error")
+
+
+class R2d2Ring:
+    """Device storage + StxR2d2Ring descriptor of the prioritised sequence ring (include/stx.h): L time rows of E envs (obs, action,
+    reward, done, truncated, reset_hidden_state), the carry of every item-start row (L // period, E, carry_dim), the sum tree over the
+    E (L // period) items, {write index, rows written}, max_recorded_priority (1.0 initially) and set_priorities' leaf claims."""
+
+    def __init__(self, length: int, envs: int, obs_dim: int, carry_dim: int, seq_len: int, period: int, priority_exponent: float, device):
+        self.length, self.envs, self.obs_dim, self.carry_dim = int(length), int(envs), int(obs_dim), int(carry_dim)
+        self.seq_len, self.period, self.priority_exponent = int(seq_len), int(period), float(priority_exponent)
+        if not (1 <= self.seq_len <= self.length and 1 <= self.period <= self.length) or self.envs * self.length >= 2**31:
+            raise StxError(f"R2d2Ring: seq_len {seq_len} and period {period} must lie in [1, length {length}], envs x length < 2^31")
+        z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=device)
+        L, E = self.length, self.envs
+        self.items_per_env = L // self.period
+        self.obs, self.action, self.reward = z(L, E, self.obs_dim), z(L, E, dt=torch.int32), z(L, E)
+        self.done, self.truncated, self.reset = (z(L, E, dt=torch.uint8) for _ in range(3))
+        self.carry = z(self.items_per_env, E, self.carry_dim)
+        self.state = z(2, dt=torch.int64)
+        self.max_priority = torch.ones(1, dtype=torch.float32, device=device)
+        self.owner = torch.full((E * self.items_per_env,), -1, dtype=torch.int32, device=device)
+        c = _lib.StxR2d2Ring()
+        c.length, c.envs, c.obs_dim, c.carry_dim, c.seq_len, c.period = L, E, self.obs_dim, self.carry_dim, self.seq_len, self.period
+        c.priority_exponent = self.priority_exponent
+        self.tree = z(int(_lib.load().stx_r2d2_tree_floats(C.byref(c))))
+        for name in ("obs", "action", "reward", "done", "truncated", "reset", "carry", "tree", "state", "max_priority", "owner"):
+            setattr(c, name, getattr(self, name).data_ptr())
+        self.c = c
+
+    @property
+    def priorities(self) -> torch.Tensor:
+        """The E (L // period) leaf priorities, item i = e (L // period) + k."""
+        return self.tree[: self.envs * self.items_per_env]
+
+
+def r2d2_ring_add(rb: R2d2Ring, obs, action, reward, done, truncated, reset, carry) -> None:
+    """Append a time-major (T, E, ...) batch: obs float32 (T, E, D), action int32, reward float32, done / truncated / reset uint8 or bool
+    (T, E), carry float32 (T, E, carry_dim) = the carry entering each step (stored at item-start rows only)."""
+    _need_cuda(obs, action, reward, done, truncated, reset, carry)
+    if reward.ndim != 2 or reward.shape[1] != rb.envs:
+        raise StxError(f"r2d2_ring_add: reward must be (T, {rb.envs})")
+    T = int(reward.shape[0])
+    n = T * rb.envs
+    flags = [_u8(done), _u8(truncated), _u8(reset)]
+    for t, cols, dt, name in ((obs, rb.obs_dim, torch.float32, "obs"), (carry, rb.carry_dim, torch.float32, "carry"), (reward, 1, torch.float32, "reward"),
+                              (action, 1, torch.int32, "action"), (flags[0], 1, torch.uint8, "done"), (flags[1], 1, torch.uint8, "truncated"),
+                              (flags[2], 1, torch.uint8, "reset")):
+        if t.dtype != dt or not t.is_contiguous() or t.numel() != n * cols:
+            raise StxError(f"r2d2_ring_add: {name} must be contiguous {dt} with {n} x {cols} elements")
+    _lib.check(_lib.load().stx_r2d2_ring_add(C.byref(rb.c), _p(obs), _p(action), _p(reward), _p(flags[0]), _p(flags[1]), _p(flags[2]), _p(carry), T,
+                                             _stream()), "stx_r2d2_ring_add")
+
+
+def r2d2_ring_sample(rb: R2d2Ring, seed: int, obs, action, reward, done, reset, carry0, idx, prob, offset: int = 0,
+                     dev_counter: Optional[torch.Tensor] = None, u_in: Optional[torch.Tensor] = None) -> None:
+    """One launch: B = prob.numel() stratified proportional draws (or u_in (B) as the uniforms), written time-major: obs (S, B, D),
+    action / reward / done / reset (S, B), carry0 (B, carry_dim), idx (B) int32 items, prob (B) = leaf / total."""
+    _need_cuda(obs, action, reward, done, reset, carry0, idx, prob, dev_counter, u_in)
+    B, S = int(prob.numel()), rb.seq_len
+    for t, shp, dt, name in ((obs, (S, B, rb.obs_dim), torch.float32, "obs"), (action, (S, B), torch.int32, "action"),
+                             (reward, (S, B), torch.float32, "reward"), (done, (S, B), torch.uint8, "done"), (reset, (S, B), torch.uint8, "reset"),
+                             (carry0, (B, rb.carry_dim), torch.float32, "carry0"), (idx, (B,), torch.int32, "idx"), (prob, (B,), torch.float32, "prob"),
+                             (u_in, (B,), torch.float32, "u_in")):
+        if t is not None and (t.dtype != dt or tuple(t.shape) != shp or not t.is_contiguous()):
+            raise StxError(f"r2d2_ring_sample: {name} must be contiguous {dt} {shp}")
+    _lib.check(_lib.load().stx_r2d2_ring_sample(C.byref(rb.c), B, int(seed) & (2**64 - 1), int(offset), _p(dev_counter), _p(u_in), _p(obs), _p(action),
+                                                _p(reward), _p(done), _p(reset), _p(carry0), _p(idx), _p(prob), _stream()), "stx_r2d2_ring_sample")
+
+
+def r2d2_ring_set_priorities(rb: R2d2Ring, idx: torch.Tensor, priorities: torch.Tensor) -> None:
+    """leaf[idx[m]] = priorities[m] ** priority_exponent (the last of duplicate indices wins), ancestors rebuilt, max raised.  The
+    indices must lie in [0, E (L // period)) (the sampler's); they are not checked on the device."""
+    _need_cuda(idx, priorities)
+    M = int(idx.numel())
+    if idx.dtype != torch.int32 or priorities.dtype != torch.float32 or priorities.numel() != M or not idx.is_contiguous() or not priorities.is_contiguous():
+        raise StxError("r2d2_ring_set_priorities: idx (M) int32 and priorities (M) float32, contiguous")
+    _lib.check(_lib.load().stx_r2d2_ring_set_priorities(C.byref(rb.c), _p(idx), _p(priorities), M, _stream()), "stx_r2d2_ring_set_priorities")
+
+
+def r2d2_value_transform(x: torch.Tensor, inverse: bool = False, eps: float = 1e-3) -> torch.Tensor:
+    """rlax's signed_hyperbolic (h) or, with inverse, signed_parabolic (h^-1) of a float32 tensor, as the loss kernel evaluates them."""
+    _need_cuda(x)
+    if x.dtype != torch.float32 or not x.is_contiguous():
+        raise StxError("r2d2_value_transform: x must be contiguous float32")
+    out = torch.empty_like(x)
+    _lib.check(_lib.load().stx_r2d2_value_transform(_p(x), int(x.numel()), int(bool(inverse)), float(eps), _p(out), _stream()), "stx_r2d2_value_transform")
+    return out
+
+
+def r2d2_loss_grads(q: torch.Tensor, q_target: torch.Tensor, action: torch.Tensor, reward: torch.Tensor, done: torch.Tensor, prob: torch.Tensor,
+                    d_q: torch.Tensor, priorities: torch.Tensor, metrics: torch.Tensor, n: int, gamma: float, max_abs_reward: float, eta: float,
+                    beta0: float, beta_steps: float = 0.0, count: Optional[torch.Tensor] = None, weight: float = 1.0, tx_eps: float = 1e-3,
+                    td: Optional[torch.Tensor] = None, scratch_key: str = "r2d2_loss") -> None:
+    """The R2D2 loss of one learn window and its gradient (include/stx.h, stx_r2d2_loss_grads): q / q_target / d_q float32 (T, B, A),
+    action int32, reward float32, done uint8 (T, B), prob / priorities float32 (B), metrics (6) += weight * R2D2_METRICS; count is the
+    int32 Adam count word of the importance-sampling schedule; td (T - 1, B) optionally receives the TD errors."""
+    dev = _need_cuda(q, q_target, action, reward, done, prob, d_q, priorities, metrics, count, td)
+    if q.ndim != 3:
+        raise StxError("r2d2_loss_grads: q must be (T, B, A)")
+    T, B, A = q.shape
+    for t, shp, dt, name in ((q, (T, B, A), torch.float32, "q"), (q_target, (T, B, A), torch.float32, "q_target"), (d_q, (T, B, A), torch.float32, "d_q"),
+                             (action, (T, B), torch.int32, "action"), (reward, (T, B), torch.float32, "reward"), (done, (T, B), torch.uint8, "done"),
+                             (prob, (B,), torch.float32, "prob"), (priorities, (B,), torch.float32, "priorities"),
+                             (td, (T - 1, B), torch.float32, "td")):
+        if t is not None and (t.dtype != dt or tuple(t.shape) != shp or not t.is_contiguous()):
+            raise StxError(f"r2d2_loss_grads: {name} must be contiguous {dt} {shp}")
+    if metrics.dtype != torch.float32 or metrics.numel() < _lib.STX_R2D2_METRICS:
+        raise StxError(f"r2d2_loss_grads: metrics must be float32 with {_lib.STX_R2D2_METRICS} floats")
+    if count is not None and count.dtype != torch.int32:
+        raise StxError("r2d2_loss_grads: count must be the int32 Adam count word")
+    lib = _lib.load()
+    scratch = _zeros_scratch((scratch_key, int(B)), lib.stx_r2d2_loss_scratch_bytes(int(B)), dev)
+    s = _lib.StxR2d2Loss()
+    s.T, s.B, s.A, s.n = int(T), int(B), int(A), int(n)
+    s.q, s.q_target, s.action, s.reward, s.done, s.prob = q.data_ptr(), q_target.data_ptr(), action.data_ptr(), reward.data_ptr(), done.data_ptr(), prob.data_ptr()
+    s.count, s.d_q, s.priorities, s.metrics, s.td = _ptr_or_none(count), d_q.data_ptr(), priorities.data_ptr(), metrics.data_ptr(), _ptr_or_none(td)
+    s.gamma, s.max_abs_reward, s.eta, s.tx_eps = float(gamma), float(max_abs_reward), float(eta), float(tx_eps)
+    s.beta0, s.beta_steps, s.weight = float(beta0), float(beta_steps), float(weight)
+    _lib.check(lib.stx_r2d2_loss_grads(C.byref(s), _p(scratch), _stream()), "stx_r2d2_loss_grads")
+
+
+def dueling_q(adv: torch.Tensor, value: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Q (M, A) = v + (adv - mean_a adv) with v = value[0] (the value branch's final LayerNorm bias) (stx_dueling_q)."""
+    A = int(adv.shape[-1])
+    out = _dueling_io("dueling_q", adv, A, out, A)
+    if value.dtype != torch.float32 or value.numel() != 1:
+        raise StxError("dueling_q: value must be one float32")
+    _need_cuda(value)
+    _lib.check(_lib.load().stx_dueling_q(_p(adv), _p(value), adv.shape[0], A, _p(out), _stream()), "stx_dueling_q")
+    return out
+
+
+def dueling_q_backward(d_q: torch.Tensor, d_adv: torch.Tensor, d_value: torch.Tensor, weight: float = 1.0, overwrite: bool = True) -> None:
+    """d adv = d_q - mean_a d_q into d_adv (M, A); d_value (1) = weight * sum d_q (overwrite) or += (stx_dueling_q_backward)."""
+    A = int(d_q.shape[-1])
+    _dueling_io("dueling_q_backward", d_q, A, d_adv, A)
+    if d_value.dtype != torch.float32 or d_value.numel() != 1:
+        raise StxError("dueling_q_backward: d_value must be one float32")
+    _need_cuda(d_value)
+    _lib.check(_lib.load().stx_dueling_q_backward(_p(d_q), d_q.shape[0], A, _p(d_adv), _p(d_value), float(weight), int(bool(overwrite)), _stream()),
+               "stx_dueling_q_backward")

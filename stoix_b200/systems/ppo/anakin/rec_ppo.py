@@ -29,6 +29,7 @@ from stoix_b200 import random as srandom
 from stoix_b200.base_types import ActorCriticOptStates, ActorCriticParams, AnakinExperimentOutput
 from stoix_b200.config import DictConfig, instantiate
 from stoix_b200.envs.base import Environment, StepOut
+from stoix_b200.evaluator import get_rnn_evaluator_fn
 from stoix_b200.networks.recurrent import RecLayout, RecurrentActor, RecurrentCritic, ScannedRNN
 from stoix_b200.systems import anakin
 from stoix_b200.systems.ppo.ppo_types import ActorCriticHiddenStates, RNNLearnerState, RNNPPOTransition
@@ -307,34 +308,6 @@ def learner_setup(env: Environment, keys: Tuple[int, int, int], config: DictConf
     init_learner_state = RNNLearnerState(params, opt_states, anakin.rank_seeds(shard_keys[U], 2, rank, world),
                                          env_states, timesteps, dones, truncs, hstates)
     return learn, actor_network, init_learner_state
-
-
-def get_rnn_evaluator_fn(env: Environment, actor_network: RecurrentActor, config: DictConfig, eval_multiplier: int = 1) -> Callable:
-    """stoix/evaluator.py get_rnn_evaluator_fn: episodes in parallel with the hidden state carried and reset at episode starts."""
-    n_episodes = int(config.arch.num_eval_episodes) * eval_multiplier
-    max_steps = int(config.arch.get("max_eval_steps", 2000))
-
-    def evaluator(params, key) -> Dict[str, torch.Tensor]:
-        keys = srandom.split(key, n_episodes + 1)
-        state, ts = env.reset(keys[:n_episodes])
-        dev = ts.observation.device
-        h = actor_network.rnn.initialize_carry(n_episodes, dev)
-        reset = torch.zeros(n_episodes, dtype=torch.bool, device=dev)
-        alive = torch.ones(n_episodes, dtype=torch.bool, device=dev)
-        ret, length = torch.zeros(n_episodes, device=dev), torch.zeros(n_episodes, dtype=torch.int32, device=dev)
-        for step in range(max_steps):
-            h, pi = actor_network.apply(params, h, (ts.observation.float()[None], reset[None]))
-            action = (pi.mode() if config.arch.evaluation_greedy else pi.sample(seed=keys[-1] + step))[0]
-            state, ts = env.step(state, action)
-            reset = ts.last()
-            ret += ts.reward * alive
-            length += alive.to(torch.int32)
-            alive &= ~ts.last()
-            if step % 50 == 49 and not bool(alive.any().item()):
-                break
-        return {"episode_return": ret, "episode_length": length}
-
-    return evaluator
 
 
 def run_experiment(_config: DictConfig) -> float:

@@ -137,3 +137,45 @@ class SequenceBuffer:
         ops.replay_sample_sequence(self.ring, self.sample_sequence_length, self.seed, obs, action, reward, done, log_prob,
                                    dev_counter=self.counter.view(torch.int64), idx_in=idx_in, idx_out=idx_out)
         ops.counter_add(self.counter, 1)
+
+
+class PrioritisedSequenceBuffer:
+    """fbx.make_prioritised_trajectory_buffer as rec_r2d2.py:644-653 builds it, on the prioritised sequence ring (stx_r2d2_ring_add /
+    _sample / _set_priorities): add_batch_size = E envs, max_length_time_axis = max_size // E time rows, min_length_time_axis =
+    sample_sequence_length = S, items every `period` rows.  `sample_into` draws sample_batch_size sequences in proportion to their
+    priorities and writes them time-major (S, B, ...) with the carry at each sequence's start, the items and p_i."""
+
+    def __init__(self, max_size: int, sample_batch_size: int, sample_sequence_length: int, add_batch_size: int, period: int, priority_exponent: float,
+                 obs_dim: int, carry_dim: int, device, seed: int = 0):
+        self.max_length_time_axis = int(max_size) // int(add_batch_size)
+        self.sample_batch_size, self.sample_sequence_length = int(sample_batch_size), int(sample_sequence_length)
+        self.add_batch_size, self.period = int(add_batch_size), int(period)
+        if self.max_length_time_axis < self.sample_sequence_length:
+            raise ValueError(f"PrioritisedSequenceBuffer: max_size={max_size} over {add_batch_size} envs holds {self.max_length_time_axis} time "
+                             f"rows, fewer than one sequence of sample_sequence_length={self.sample_sequence_length}")
+        if not 1 <= self.period <= self.max_length_time_axis:
+            raise ValueError(f"PrioritisedSequenceBuffer: period={period} must lie in [1, {self.max_length_time_axis}] (the time rows per env)")
+        self.ring = ops.R2d2Ring(self.max_length_time_axis, self.add_batch_size, obs_dim, carry_dim, self.sample_sequence_length, self.period,
+                                 priority_exponent, device)
+        self.seed = int(seed) & ((1 << 62) - 1)
+        self.counter = torch.zeros(1, dtype=torch.int64, device=device)   # sample calls so far (device-resident RNG stream position)
+        self.added = 0                                                    # host mirror of the items added (T E per add)
+
+    def add(self, tr) -> None:
+        """tr: a time-major RNNTransition: .obs (T, E, D), .action int32, .reward, .reset_hidden_state, .done, .truncated (T, E) and
+        .hstate (T, E, carry_dim), the carry entering each step."""
+        ops.r2d2_ring_add(self.ring, tr.obs, tr.action, tr.reward, tr.done, tr.truncated, tr.reset_hidden_state, tr.hstate)
+        self.added += int(tr.reward.numel())
+
+    def can_sample(self) -> bool:
+        """min_length_time_axis = sample_sequence_length time rows written."""
+        return min(self.added // self.add_batch_size, self.max_length_time_axis) >= self.sample_sequence_length
+
+    def sample_into(self, obs, action, reward, done, reset, carry0, idx, prob, u_in: Optional[torch.Tensor] = None) -> None:
+        """Draw one batch into the (S, B, ...) buffers, carry0 (B, carry_dim), idx and prob (B); advances the stream position."""
+        ops.r2d2_ring_sample(self.ring, self.seed, obs, action, reward, done, reset, carry0, idx, prob, dev_counter=self.counter.view(torch.int64),
+                             u_in=u_in)
+        ops.counter_add(self.counter, 1)
+
+    def set_priorities(self, idx: torch.Tensor, priorities: torch.Tensor) -> None:
+        ops.r2d2_ring_set_priorities(self.ring, idx, priorities)
