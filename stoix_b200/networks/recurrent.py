@@ -23,7 +23,8 @@ from .inputs import ArrayInput
 
 
 class ScannedRNN:
-    """networks/base.py:124-159: description of the recurrent layer (the arithmetic is stx_gru_sequence_forward / _backward)."""
+    """networks/base.py:124-159: description of the recurrent layer (the arithmetic is stx_{gru,lstm}_sequence_forward / _backward,
+    run through RecLayout.sequence_forward / sequence_backward)."""
 
     def __init__(self, hidden_state_dim: int, cell_type: str = "gru"):
         cell_type = {"optimised_lstm": "lstm"}.get(str(cell_type), str(cell_type))   # OptimizedLSTMCell: same function as LSTMCell
@@ -74,6 +75,33 @@ class RecLayout:
         H = self.H
         return (flat[self.off_pre: self.off_wh], flat[self.off_wh: self.off_bhn].view(H, self.G * H), flat[self.off_bhn: self.off_post],
                 flat[self.off_post: self.param_count])
+
+    def sequence_workspace(self, T: int, E: int, device) -> torch.Tensor:
+        """Workspace of one (T, E) sequence of this cell: what its forward saves for the backward."""
+        return (ops.lstm_workspace if self.cell_type == "lstm" else ops.gru_workspace)(T, E, self.H, device)
+
+    def sequence_forward(self, p_flat: torch.Tensor, gi: torch.Tensor, reset: torch.Tensor, carry0: torch.Tensor, ws: torch.Tensor,
+                         out: Optional[torch.Tensor] = None, carry_last: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """The recurrence over gi (T, E, G*H) from carry0 (E, S) with the W_h (and b_hn) of the arena p_flat -> h_seq (T, E, H), into
+        `out` when given.  carry_last (E, S), when given, gets the carry after the last step."""
+        _, w_h, b_hn, _ = self.blocks(p_flat)
+        if self.cell_type == "lstm":
+            return ops.lstm_sequence_forward(gi, reset, carry0, w_h, ws, out=out, carry_last=carry_last)
+        h_seq = ops.gru_sequence_forward(gi, reset, carry0, w_h, b_hn, ws, out=out)
+        if carry_last is not None:   # the GRU's carry is its last output
+            carry_last.copy_(h_seq[-1])
+        return h_seq
+
+    def sequence_backward(self, p_flat: torch.Tensor, g_flat: torch.Tensor, d_h: torch.Tensor, reset: torch.Tensor, ws: torch.Tensor, d_gi: torch.Tensor,
+                          weight: float, overwrite: bool, d_carry0: Optional[torch.Tensor] = None) -> None:
+        """Backward through time of the last sequence_forward on `ws`: d_h (T, E, H) -> d_gi (T, E, G*H), and weight * d(W_h) (and
+        d(b_hn)) into the gradient arena g_flat (overwritten or added); d_carry0 (E, S) when given."""
+        _, w_h, _, _ = self.blocks(p_flat)
+        _, g_wh, g_bhn, _ = self.blocks(g_flat)
+        if self.cell_type == "lstm":
+            ops.lstm_sequence_backward(d_h, reset, w_h, ws, d_gi, d_w_h=g_wh, grad_weight=weight, overwrite=overwrite, d_carry0=d_carry0)
+        else:
+            ops.gru_sequence_backward(d_h, reset, w_h, ws, d_gi, d_w_h=g_wh, d_b_hn=g_bhn, grad_weight=weight, overwrite=overwrite, d_h0=d_carry0)
 
 
 def _dense_tree(spec: ops.MlpSpec, flat: torch.Tensor, first: int, last: int) -> Dict[str, Any]:
@@ -166,24 +194,19 @@ class _Recurrent:
         return self.build_tree(lay, flat)
 
     def _forward(self, params: ParamTree, hstate: torch.Tensor, observation_done):
-        """Inference form (rollout step, evaluator): pre-torso + input projections for all steps, the GRU sequence, post-torso + head."""
+        """Inference form (rollout step, evaluator): pre-torso + input projections for all steps, the recurrence, post-torso + head."""
         observation, done = observation_done
         obs = self.input_layer(observation).float()
         T, E, D = obs.shape
         lay: RecLayout = params.layout
-        pre, w_h, b_hn, post = lay.blocks(params.flat)
+        pre, _, _, post = lay.blocks(params.flat)
         gi = ops.mlp_forward(lay.spec_pre, pre, obs.reshape(T * E, D).contiguous(), ws_key=("rec_pre", id(self)))
         ws = self._ws.get((T, E))
-        lstm = lay.cell_type == "lstm"
         if ws is None:
-            ws = self._ws[(T, E)] = (ops.lstm_workspace if lstm else ops.gru_workspace)(T, E, lay.H, obs.device)
+            ws = self._ws[(T, E)] = lay.sequence_workspace(T, E, obs.device)
         d8 = done.to(torch.uint8) if done.dtype not in (torch.uint8, torch.bool) else done
-        if lstm:
-            last = torch.empty(E, 2 * lay.H, dtype=torch.float32, device=obs.device)
-            h_seq = ops.lstm_sequence_forward(gi.view(T, E, 4 * lay.H), d8.contiguous(), hstate.contiguous(), w_h, ws, carry_last=last)
-        else:
-            h_seq = ops.gru_sequence_forward(gi.view(T, E, 3 * lay.H), d8.contiguous(), hstate.contiguous(), w_h, b_hn, ws)
-            last = h_seq[-1]
+        last = torch.empty(E, lay.S, dtype=torch.float32, device=obs.device)
+        h_seq = lay.sequence_forward(params.flat, gi.view(T, E, lay.G * lay.H), d8.contiguous(), hstate.contiguous(), ws, carry_last=last)
         out = ops.mlp_forward(lay.spec_post, post, h_seq.view(T * E, lay.H), ws_key=("rec_post", id(self)))
         if lay.dueling:
             out = ops.dueling_q(out, lay.value_bias(params.flat))

@@ -9,7 +9,7 @@ discount_t = (1 - last_done_t) * gamma; minibatches are column subsets of the ba
   reference (JAX)                                   here (H100)
   ------------------------------------------------  -----------------------------------------------------------------------
   nn.scan of GRUCell over T inside jax.grad         pre-torso + input projections of ALL steps as one MLP launch chain,
-                                                    stx_gru_sequence_forward / _backward for the recurrence (BPTT with the saved
+                                                    RecLayout.sequence_forward / _backward for the recurrence (BPTT with the saved
                                                     gates, d W_h as one GEMM over the stored sequences), post-torso + head as
                                                     one MLP chain; the losses' output gradients from stx_ppo_head_grads
   permutation + take of the whole batch per epoch   keyed bijection over the columns; kernels gather rows through an index
@@ -72,7 +72,7 @@ class _NetWs:
         z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=device)
         M, H = chunk * C, lay.H
         self.ws_pre, self.ws_post = ops.mlp_train_workspace(lay.spec_pre, M, device), ops.mlp_train_workspace(lay.spec_post, M, device)
-        self.ws_gru = (ops.lstm_workspace if lay.cell_type == "lstm" else ops.gru_workspace)(chunk, C, H, device)
+        self.ws_seq = lay.sequence_workspace(chunk, C, device)
         self.gi, self.d_gi = z(chunk, C, lay.G * H), z(chunk, C, lay.G * H)
         self.h_seq, self.d_h = z(chunk, C, H), z(chunk, C, H)
         self.h0 = z(C, lay.S)
@@ -170,16 +170,12 @@ def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], updat
         """Forward over the chunk, loss head, backward through time for one network on the rows `idx` (rec_ppo.py:207-262)."""
         b = built
         D, H = b["D"], lay.H
-        pre, w_h, b_hn, post = lay.blocks(p_flat)
-        g_pre, g_wh, g_bhn, g_post = lay.blocks(g_flat)
+        pre, _, _, post = lay.blocks(p_flat)
+        g_pre, _, _, g_post = lay.blocks(g_flat)
         obs_flat = sh.obs[:T].reshape(T * E, D)
-        lstm = lay.cell_type == "lstm"
         ops.mlp_forward_train(lay.spec_pre, pre, obs_flat, w.ws_pre, out=w.gi.view(chunk * C, lay.G * H), row_idx=idx)
         ops.gather_rows(h_store.reshape(T * E, lay.S), idx[:C], w.h0)                    # hstates[0] of the chunk (:216-218)
-        if lstm:
-            ops.lstm_sequence_forward(w.gi, b["reset_mb"], w.h0, w_h, w.ws_gru, out=w.h_seq)
-        else:
-            ops.gru_sequence_forward(w.gi, b["reset_mb"], w.h0, w_h, b_hn, w.ws_gru, out=w.h_seq)
+        lay.sequence_forward(p_flat, w.gi, b["reset_mb"], w.h0, w.ws_seq, out=w.h_seq)
         ops.mlp_forward_train(lay.spec_post, post, w.h_seq.view(chunk * C, H), w.ws_post, out=w.out)
         stats = sh.adv_stats if sysc.standardize_advantages else None
         ops.ppo_head_grads(w.out if is_actor else None, None if is_actor else w.out, idx, sh.action.reshape(-1), sh.log_prob.reshape(-1),
@@ -188,10 +184,7 @@ def get_learner_fn(env: Environment, apply_fns: Tuple[Callable, Callable], updat
                            scratch_key="ppo_head_actor" if is_actor else "ppo_head_critic")
         ops.mlp_backward(lay.spec_post, post, w.h_seq.view(chunk * C, H), w.d_out, w.ws_post, net_grad=g_post, grad_weight=weight, overwrite=overwrite,
                          d_input=w.d_h.view(chunk * C, H))
-        if lstm:
-            ops.lstm_sequence_backward(w.d_h, b["reset_mb"], w_h, w.ws_gru, w.d_gi, d_w_h=g_wh, grad_weight=weight, overwrite=overwrite)
-        else:
-            ops.gru_sequence_backward(w.d_h, b["reset_mb"], w_h, w.ws_gru, w.d_gi, d_w_h=g_wh, d_b_hn=g_bhn, grad_weight=weight, overwrite=overwrite)
+        lay.sequence_backward(p_flat, g_flat, w.d_h, b["reset_mb"], w.ws_seq, w.d_gi, weight, overwrite)
         ops.mlp_backward(lay.spec_pre, pre, obs_flat, w.d_gi.view(chunk * C, lay.G * H), w.ws_pre, net_grad=g_pre, grad_weight=weight, overwrite=overwrite,
                          row_idx=idx)
 

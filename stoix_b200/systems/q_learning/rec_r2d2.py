@@ -128,13 +128,13 @@ class Work:
     def __init__(self, lay: RecLayout, S: int, burn_in: int, B: int, A: int, device):
         z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=device)
         H, G, Tl = lay.H, lay.G, S - burn_in
-        seq_ws = ops.lstm_workspace if lay.cell_type == "lstm" else ops.gru_workspace
         self.Tl = Tl
-        self.gi_all, self.h_all, self.ws_all = z(S, B, G * H), z(S, B, H), seq_ws(S, B, H, device)          # target, S rows
-        self.gi_burn, self.h_burn, self.ws_burn = z(max(burn_in, 1), B, G * H), z(max(burn_in, 1), B, H), seq_ws(max(burn_in, 1), B, H, device)
+        self.gi_all, self.h_all, self.ws_all = z(S, B, G * H), z(S, B, H), lay.sequence_workspace(S, B, device)   # target, S rows
+        self.gi_burn, self.h_burn = z(max(burn_in, 1), B, G * H), z(max(burn_in, 1), B, H)
+        self.ws_burn = lay.sequence_workspace(max(burn_in, 1), B, device)
         self.carry_on, self.carry_tg = z(B, lay.S), z(B, lay.S)                                              # burned-in carries
         self.ws_pre, self.ws_post = ops.mlp_train_workspace(lay.spec_pre, Tl * B, device), ops.mlp_train_workspace(lay.spec_post, Tl * B, device)
-        self.gi, self.d_gi, self.h_seq, self.d_h, self.ws_seq = z(Tl, B, G * H), z(Tl, B, G * H), z(Tl, B, H), z(Tl, B, H), seq_ws(Tl, B, H, device)
+        self.gi, self.d_gi, self.h_seq, self.d_h, self.ws_seq = z(Tl, B, G * H), z(Tl, B, G * H), z(Tl, B, H), z(Tl, B, H), lay.sequence_workspace(Tl, B, device)
         self.out, self.d_out = z(Tl * B, A), z(Tl * B, A)
         self.q, self.q_tg, self.d_q = z(Tl, B, A), z(Tl, B, A), z(Tl, B, A)
         self.priorities = z(B)
@@ -144,14 +144,8 @@ def _sequence(lay: RecLayout, p_flat: torch.Tensor, obs: torch.Tensor, reset: to
               ws: torch.Tensor, carry_last: Optional[torch.Tensor], key: str) -> None:
     """Pre-torso + input projections of every row (inference) and the recurrence from carry0; carry_last (nullable) gets the last carry."""
     T, B, D = obs.shape
-    pre, w_h, b_hn, _ = lay.blocks(p_flat)
-    ops.mlp_forward(lay.spec_pre, pre, obs.reshape(T * B, D), out=gi.view(T * B, -1), ws_key=key)
-    if lay.cell_type == "lstm":
-        ops.lstm_sequence_forward(gi, reset, carry0, w_h, ws, out=h_seq, carry_last=carry_last)
-    else:
-        ops.gru_sequence_forward(gi, reset, carry0, w_h, b_hn, ws, out=h_seq)
-        if carry_last is not None:
-            carry_last.copy_(h_seq[-1])
+    ops.mlp_forward(lay.spec_pre, lay.blocks(p_flat)[0], obs.reshape(T * B, D), out=gi.view(T * B, -1), ws_key=key)
+    lay.sequence_forward(p_flat, gi, reset, carry0, ws, out=h_seq, carry_last=carry_last)
 
 
 def _head(lay: RecLayout, p_flat: torch.Tensor, out: torch.Tensor, q: torch.Tensor) -> None:
@@ -178,15 +172,11 @@ def batch_grads(lay: RecLayout, online: torch.Tensor, target: torch.Tensor, bt: 
     if burn_in > 0:
         _sequence(lay, online, bt.obs[:burn_in], bt.reset[:burn_in], bt.carry0, w.gi_burn, w.h_burn, w.ws_burn, w.carry_on, "r2d2_burn_pre")
         carry = w.carry_on
-    pre, w_h, b_hn, post = lay.blocks(online)
-    g_pre, g_wh, g_bhn, g_post = lay.blocks(grads)
+    pre, _, _, post = lay.blocks(online)
+    g_pre, _, _, g_post = lay.blocks(grads)
     obs_l, reset_l = bt.obs[burn_in:].reshape(Tl * B, D), bt.reset[burn_in:]
-    lstm = lay.cell_type == "lstm"
     ops.mlp_forward_train(lay.spec_pre, pre, obs_l, w.ws_pre, out=w.gi.view(Tl * B, -1))
-    if lstm:
-        ops.lstm_sequence_forward(w.gi, reset_l, carry, w_h, w.ws_seq, out=w.h_seq)
-    else:
-        ops.gru_sequence_forward(w.gi, reset_l, carry, w_h, b_hn, w.ws_seq, out=w.h_seq)
+    lay.sequence_forward(online, w.gi, reset_l, carry, w.ws_seq, out=w.h_seq)
     ops.mlp_forward_train(lay.spec_post, post, w.h_seq.view(Tl * B, lay.H), w.ws_post, out=w.out)
     _head(lay, online, w.out, w.q)
     ops.r2d2_loss_grads(w.q, w.q_tg, bt.action[burn_in:], bt.reward[burn_in:], bt.done[burn_in:], bt.prob, w.d_q, w.priorities, metric,
@@ -197,10 +187,7 @@ def batch_grads(lay: RecLayout, online: torch.Tensor, target: torch.Tensor, bt: 
         w.d_out.copy_(w.d_q.view(Tl * B, -1))
     ops.mlp_backward(lay.spec_post, post, w.h_seq.view(Tl * B, lay.H), w.d_out, w.ws_post, net_grad=g_post, grad_weight=weight, overwrite=overwrite,
                      d_input=w.d_h.view(Tl * B, lay.H))
-    if lstm:
-        ops.lstm_sequence_backward(w.d_h, reset_l, w_h, w.ws_seq, w.d_gi, d_w_h=g_wh, grad_weight=weight, overwrite=overwrite)
-    else:
-        ops.gru_sequence_backward(w.d_h, reset_l, w_h, w.ws_seq, w.d_gi, d_w_h=g_wh, d_b_hn=g_bhn, grad_weight=weight, overwrite=overwrite)
+    lay.sequence_backward(online, grads, w.d_h, reset_l, w.ws_seq, w.d_gi, weight, overwrite)
     ops.mlp_backward(lay.spec_pre, pre, obs_l, w.d_gi.view(Tl * B, -1), w.ws_pre, net_grad=g_pre, grad_weight=weight, overwrite=overwrite)
 
 
