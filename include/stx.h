@@ -1058,6 +1058,53 @@ int stx_r2d2_loss_grads(const StxR2d2Loss* loss, void* scratch, void* stream);
 int stx_dueling_q(const float* adv, const float* value, int64_t M, int A, float* q, void* stream);
 int stx_dueling_q_backward(const float* d_q, int64_t M, int A, float* d_adv, float* d_value, float weight, int overwrite, void* stream);
 
+/* ------------------------------------------------------------------ IMPALA: V-trace (fp32) ----------------------------
+ * The learner step of stoix/systems/impala/sebulba/ff_impala.py:358-566 on one learner batch of T + 1 time rows and E env columns.
+ *
+ * stx_reward_stats: mean and population std (jnp.mean / jnp.std) of the rewards r[t * ld + e], t < T, e < E, in fp64 in a fixed
+ *   order, written as float32 stats[0] = mean, stats[1] = std (ff_impala.py:389-395).  One launch.
+ * stx_clip_rmsprop_step: stx_clip_adam_step with optax.rmsprop(lr) at its defaults (ff_impala.py:754-766): no centring, no momentum,
+ *   no bias correction, initial_scale 0, eps inside the square root:
+ *     nu = (1 - decay) g^2 + decay nu ;  p = p - lr g / sqrt(nu + eps)
+ *   with decay = hyper->b2 (hyper->b1 is not read) and the clip, learning-rate schedule and per-segment counts of stx_clip_adam_step.
+ *   Reads and writes nu only.  hyper->prenorm must be 0.
+ * stx_vtrace_loss_grads: one minibatch = one column block of Em envs, in one launch.  Per column, time-major (row t * Em + j):
+ *     logp = log_softmax(logits);  rho = exp(logp[a] - log_prob_b);  H = -sum p logp
+ *     r = reward (or reward_scale (reward - mean) / (std + reward_eps) with reward_stats);  d = gamma (1 - done)  (truncation ends the
+ *     trace like termination, as the reference does)
+ *   rlax.vtrace_td_error_and_advantage with v_tm1 = values[t], v_t = values[t + 1]:
+ *     c = lambda min(1, rho);  delta = min(clip_rho, rho) (r + d v_t - v_tm1);  acc_t = delta_t + d_t c_t acc_{t+1} (acc_T = 0)
+ *     vs = acc + v_tm1;  errors = vs - v_tm1
+ *     q_t = r_t + d_t (lambda vs_{t+1} + (1 - lambda) v_tm1_{t+1})  (t < T - 1),  q_{T-1} = r + d v_t
+ *     pg_adv = min(clip_pg_rho, rho) (q - v_tm1)
+ *   losses (sums, not means): value_loss = 0.5 sum errors^2 (the critic loss is vf_coef value_loss, gradient only through v_tm1),
+ *   actor_loss = -sum pg_adv logp[a] (pg_adv constant), entropy = sum H (the actor loss subtracts ent_coef entropy):
+ *     d_logits_k = -pg_adv (1[k = a] - p_k) + ent_coef p_k (logp_k + H);  d_value[t] = -vf_coef errors_t, d_value[T] = 0
+ *   metrics (STX_VTRACE_METRICS, overwritten): actor_loss, entropy, value_loss, mean q_estimate, mean pg_advantage.
+ *   Any T >= 1, Em >= 1, A >= 1.  action / log_prob_b / reward / done: element (t, j) at [t * ld + j] (a column block of the learner
+ *   batch).  scratch: stx_vtrace_loss_scratch_bytes(), zeroed once. */
+#define STX_VTRACE_METRICS 5
+typedef struct StxVtraceLoss {
+  const float* logits;        /* (T * Em, A) */
+  const float* values;        /* ((T + 1) * Em) */
+  const int32_t* action;      /* [t * ld + j], t < T */
+  const float* log_prob_b;    /* behaviour log-probabilities, [t * ld + j] */
+  const float* reward;        /* [t * ld + j] */
+  const uint8_t* done;        /* [t * ld + j] */
+  const float* reward_stats;  /* nullable: {mean, std} of stx_reward_stats, applied to the rewards as they are loaded */
+  float* d_logits;            /* (T * Em, A) */
+  float* d_value;             /* ((T + 1) * Em) */
+  float* metrics;             /* STX_VTRACE_METRICS */
+  int64_t ld;                 /* row stride of action / log_prob_b / reward / done, >= Em */
+  int32_t T, Em, A;
+  float gamma, lambda_, clip_rho, clip_pg_rho, ent_coef, vf_coef, reward_scale, reward_eps;
+} StxVtraceLoss;
+int stx_reward_stats(const float* reward, int T, int E, int64_t ld, float* stats, void* stream);
+int stx_clip_rmsprop_step(float* param_arena, const float* grad_arena, float* nu, int32_t* counts, const StxAdamSeg* segs, int nseg,
+                          const StxAdamHyper* hyper, void* params_bf16, float* gnorm_out, void* scratch, void* stream);
+size_t stx_vtrace_loss_scratch_bytes(void);
+int stx_vtrace_loss_grads(const StxVtraceLoss* loss, void* scratch, void* stream);
+
 /* Utility casts used by the bf16 path (obs / weight shadows). */
 int stx_cast_f32_to_bf16(const float* src, void* dst, int64_t n, void* stream);
 

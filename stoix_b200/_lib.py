@@ -89,6 +89,33 @@ class StxRadamHyper(C.Structure):
     ]
 
 
+class StxVtraceLoss(C.Structure):
+    _fields_ = [
+        ("logits", C.c_void_p),
+        ("values", C.c_void_p),
+        ("action", C.c_void_p),
+        ("log_prob_b", C.c_void_p),
+        ("reward", C.c_void_p),
+        ("done", C.c_void_p),
+        ("reward_stats", C.c_void_p),
+        ("d_logits", C.c_void_p),
+        ("d_value", C.c_void_p),
+        ("metrics", C.c_void_p),
+        ("ld", C.c_int64),
+        ("T", C.c_int32),
+        ("Em", C.c_int32),
+        ("A", C.c_int32),
+        ("gamma", C.c_float),
+        ("lambda_", C.c_float),
+        ("clip_rho", C.c_float),
+        ("clip_pg_rho", C.c_float),
+        ("ent_coef", C.c_float),
+        ("vf_coef", C.c_float),
+        ("reward_scale", C.c_float),
+        ("reward_eps", C.c_float),
+    ]
+
+
 class StxEpsilonSchedule(C.Structure):
     _fields_ = [
         ("init_value", C.c_float),
@@ -309,6 +336,7 @@ class StxMpoLoss(C.Structure):
 STX_LN_TORSO = 1
 STX_LN_FINAL = 2
 STX_R2D2_METRICS = 6
+STX_VTRACE_METRICS = 5
 
 
 class StxR2d2Ring(C.Structure):
@@ -462,6 +490,10 @@ _SIGNATURES = {
     "stx_r2d2_loss_grads": (C.c_int, [C.POINTER(StxR2d2Loss), _P, _P]),
     "stx_dueling_q": (C.c_int, [_P, _P, C.c_int64, C.c_int, _P, _P]),
     "stx_dueling_q_backward": (C.c_int, [_P, C.c_int64, C.c_int, _P, _P, C.c_float, C.c_int, _P]),
+    "stx_reward_stats": (C.c_int, [_P, C.c_int, C.c_int, C.c_int64, _P, _P]),
+    "stx_clip_rmsprop_step": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.POINTER(StxAdamHyper), _P, _P, _P, _P]),
+    "stx_vtrace_loss_scratch_bytes": (C.c_size_t, []),
+    "stx_vtrace_loss_grads": (C.c_int, [C.POINTER(StxVtraceLoss), _P, _P]),
 }
 
 _lib = None

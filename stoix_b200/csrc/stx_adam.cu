@@ -74,18 +74,19 @@ __device__ __forceinline__ void grid_barrier(unsigned long long* arrive) {
   __syncthreads();
 }
 
-// The update rule of phase 2: Adam (stx_clip_adam_step and the fused all-reduce forms) or, with RADAM, optax.scale_by_radam
-// (stx_clip_radam_step).  The rectifier of RAdam depends on the step count only; it is derived once per segment in double
+// The update rule of phase 2, a compile-time choice: Adam (stx_clip_adam_step and the fused all-reduce forms), optax.scale_by_radam
+// (stx_clip_radam_step) or optax.scale_by_rms at optax.rmsprop's defaults (stx_clip_rmsprop_step, which reads and writes nu only).  The rectifier of RAdam depends on the step count only; it is derived once per segment in double
 // precision next to the bias corrections: rho_t = rho_inf - 2 t b2^t / (1 - b2^t) subtracts two numbers of nearly the same size
 // (rho_inf = 1999 at b2 = 0.999), which in fp32 puts a relative error of 1.8e-3 on r_t at t = 6 (DESIGN.md section 2, tolerance scheme).
 struct RadamArgs {
   float eps_root, threshold;
 };
+enum UpdateRule : int { kRuleAdam = 0, kRuleRadam = 1, kRuleRmsprop = 2 };
 
 // PEER: 0 = local gradients; 1 = one-shot all-reduce (every rank loads all W arenas); 2 = two-shot (rank r reduces slice r from
 // the W arenas and stores the result into every rank's buffer: (W-1)/W of the arena in and out instead of W-1 arenas in; the
 // second cross-rank hand-shake doubles as the grid barrier of the norm, whose per-rank partial sums travel with the slices).
-template <bool PRENORM, int PEER, bool RADAM = false>
+template <bool PRENORM, int PEER, int RULE = kRuleAdam>
 __global__ void __launch_bounds__(kAdamThreads)
     clip_adam_kernel(float* __restrict__ P, const float* G, float* __restrict__ MU,
                      float* __restrict__ NU, int32_t* __restrict__ counts,
@@ -97,7 +98,7 @@ __global__ void __launch_bounds__(kAdamThreads)
   __shared__ double sred[32];
   __shared__ StxAdamSeg s_seg[kAdamMaxSegs];
   __shared__ float s_gs[kAdamMaxSegs], s_bc1[kAdamMaxSegs], s_bc2[kAdamMaxSegs], s_lr[kAdamMaxSegs], s_gn[kAdamMaxSegs];
-  __shared__ float s_rect[kAdamMaxSegs];  // RADAM: r_t, or 0 on the un-rectified branch (rho_t < threshold)
+  __shared__ float s_rect[kAdamMaxSegs];  // kRuleRadam: r_t, or 0 on the un-rectified branch (rho_t < threshold)
   const int gtid = blockIdx.x * blockDim.x + threadIdx.x;
   const int gthreads = gridDim.x * blockDim.x;
   griddep_launch();
@@ -309,7 +310,7 @@ __global__ void __launch_bounds__(kAdamThreads)
       s_bc2[s] = 1.0f - powf(h.b2, (float)c);
       s_lr[s] = lr;
       s_gn[s] = g_norm;
-      if constexpr (RADAM) {  // optax.scale_by_radam, rectifier in double precision
+      if constexpr (RULE == kRuleRadam) {  // optax.scale_by_radam, rectifier in double precision
         const double b2 = (double)h.b2, t = (double)c;
         const double rho_inf = 2.0 / (1.0 - b2) - 1.0;
         const double b2t = pow(b2, t);
@@ -325,10 +326,10 @@ __global__ void __launch_bounds__(kAdamThreads)
   for (int s = 0; s < nseg; ++s) {
     const StxAdamSeg seg = s_seg[s];
     const float gs = s_gs[s], bc1 = s_bc1[s], bc2 = s_bc2[s], lr = s_lr[s];
-    const float rect = RADAM ? s_rect[s] : 0.f;
+    const float rect = RULE == kRuleRadam ? s_rect[s] : 0.f;
     // the step direction of one element: Adam's, or RAdam's (r_t mhat / (sqrt(vhat + eps_root) + eps), else mhat)
     auto direction = [&](float me, float ve) -> float {
-      if constexpr (RADAM) {
+      if constexpr (RULE == kRuleRadam) {
         const float mh = me / bc1;
         return rect > 0.f ? rect * mh / (sqrtf(ve / bc2 + rx.eps_root) + h.eps) : mh;
       } else {
@@ -346,19 +347,26 @@ __global__ void __launch_bounds__(kAdamThreads)
         gv = pf_g[s < kPf ? s : 0], m = pf_m[s < kPf ? s : 0], v = pf_v[s < kPf ? s : 0], pv = pf_p[s < kPf ? s : 0];
       } else {
         gv = ld_hint(reinterpret_cast<const float4*>(g) + i, pol_keep);
-        m = ld_hint(reinterpret_cast<const float4*>(mu) + i, pol_keep), v = ld_hint(reinterpret_cast<const float4*>(nu) + i, pol_keep);
+        if constexpr (RULE == kRuleRmsprop) m = make_float4(0.f, 0.f, 0.f, 0.f);
+        else m = ld_hint(reinterpret_cast<const float4*>(mu) + i, pol_keep);
+        v = ld_hint(reinterpret_cast<const float4*>(nu) + i, pol_keep);
         pv = ld_hint(reinterpret_cast<const float4*>(p) + i, pol_keep);
       }
       float ge[4] = {gv.x * gs, gv.y * gs, gv.z * gs, gv.w * gs};
       float me[4] = {m.x, m.y, m.z, m.w}, ve[4] = {v.x, v.y, v.z, v.w}, pe[4] = {pv.x, pv.y, pv.z, pv.w};
 #pragma unroll
       for (int k = 0; k < 4; ++k) {
-        me[k] = h.b1 * me[k] + ob1 * ge[k];
-        ve[k] = h.b2 * ve[k] + ob2 * ge[k] * ge[k];
-        const float u = direction(me[k], ve[k]);
-        pe[k] = pe[k] - lr * u;
+        if constexpr (RULE == kRuleRmsprop) {  // optax.scale_by_rms, eps inside the square root
+          ve[k] = ob2 * ge[k] * ge[k] + h.b2 * ve[k];
+          pe[k] = pe[k] - lr * (ge[k] / sqrtf(ve[k] + h.eps));
+        } else {
+          me[k] = h.b1 * me[k] + ob1 * ge[k];
+          ve[k] = h.b2 * ve[k] + ob2 * ge[k] * ge[k];
+          const float u = direction(me[k], ve[k]);
+          pe[k] = pe[k] - lr * u;
+        }
       }
-      st_hint(reinterpret_cast<float4*>(mu) + i, make_float4(me[0], me[1], me[2], me[3]), pol_keep);
+      if constexpr (RULE != kRuleRmsprop) st_hint(reinterpret_cast<float4*>(mu) + i, make_float4(me[0], me[1], me[2], me[3]), pol_keep);
       st_hint(reinterpret_cast<float4*>(nu) + i, make_float4(ve[0], ve[1], ve[2], ve[3]), pol_keep);
       st_hint(reinterpret_cast<float4*>(p) + i, make_float4(pe[0], pe[1], pe[2], pe[3]), pol_keep);
       if (P16) {
@@ -371,11 +379,18 @@ __global__ void __launch_bounds__(kAdamThreads)
     }
     for (int64_t i = n4 * 4 + gtid; i < seg.count; i += gthreads) {
       const float ge = g[i] * gs;
-      const float me = h.b1 * mu[i] + ob1 * ge;
-      const float ve = h.b2 * nu[i] + ob2 * ge * ge;
-      const float u = direction(me, ve);
-      const float pn = p[i] - lr * u;
-      mu[i] = me, nu[i] = ve, p[i] = pn;
+      float pn;
+      if constexpr (RULE == kRuleRmsprop) {
+        const float ve = ob2 * ge * ge + h.b2 * nu[i];
+        pn = p[i] - lr * (ge / sqrtf(ve + h.eps));
+        nu[i] = ve, p[i] = pn;
+      } else {
+        const float me = h.b1 * mu[i] + ob1 * ge;
+        const float ve = h.b2 * nu[i] + ob2 * ge * ge;
+        const float u = direction(me, ve);
+        pn = p[i] - lr * u;
+        mu[i] = me, nu[i] = ve, p[i] = pn;
+      }
       if (P16) P16[seg.offset + i] = __float2bfloat16_rn(pn);
     }
   }
@@ -459,9 +474,26 @@ extern "C" int stx_clip_radam_step(float* param_arena, const float* grad_arena, 
   STX_REQUIRE(!hyper->adam.prenorm, STX_E_ARG, "stx_clip_radam_step: prenorm is not available with RAdam");
   STX_REQUIRE(hyper->eps_root >= 0.f, STX_E_ARG, "stx_clip_radam_step: eps_root=%g must be >= 0", (double)hyper->eps_root);
   const PeerSync none{};
-  STX_CUDA_OK(launch_pdl(clip_adam_kernel<false, 0, true>, dim3(kNumSMs), dim3(kAdamThreads), 0, (cudaStream_t)stream, param_arena, grad_arena,
+  STX_CUDA_OK(launch_pdl(clip_adam_kernel<false, 0, kRuleRadam>, dim3(kNumSMs), dim3(kAdamThreads), 0, (cudaStream_t)stream, param_arena, grad_arena,
                          mu, nu, counts, segs, nseg, hyper->adam, reinterpret_cast<__nv_bfloat16*>(params_bf16), gnorm_out,
                          reinterpret_cast<AdamScratch*>(scratch), none, RadamArgs{hyper->eps_root, hyper->threshold}));
+  STX_LAUNCH_OK();
+  return STX_OK;
+}
+
+// clip + RMSProp: the same launch with optax.rmsprop at its defaults (IMPALA, ff_impala.py:754-766); the mu arena is not touched.
+extern "C" int stx_clip_rmsprop_step(float* param_arena, const float* grad_arena, float* nu, int32_t* counts, const StxAdamSeg* segs, int nseg,
+                                     const StxAdamHyper* hyper, void* params_bf16, float* gnorm_out, void* scratch, void* stream) {
+  STX_REQUIRE(param_arena && grad_arena && nu && counts && segs && hyper && scratch, STX_E_ARG, "stx_clip_rmsprop_step: null pointer");
+  STX_REQUIRE(nseg >= 1 && nseg <= kAdamMaxSegs, STX_E_SHAPE, "stx_clip_rmsprop_step: nseg=%d (max %d)", nseg, kAdamMaxSegs);
+  STX_REQUIRE(aligned16(param_arena) && aligned16(grad_arena) && aligned16(nu), STX_E_ALIGN, "stx_clip_rmsprop_step: arenas must be 16-byte aligned");
+  STX_REQUIRE(hyper->steps_per_update > 0 && hyper->num_updates > 0, STX_E_ARG,
+              "stx_clip_rmsprop_step: steps_per_update/num_updates must be positive");
+  STX_REQUIRE(!hyper->prenorm, STX_E_ARG, "stx_clip_rmsprop_step: prenorm is not available with RMSProp");
+  const PeerSync none{};
+  STX_CUDA_OK(launch_pdl(clip_adam_kernel<false, 0, kRuleRmsprop>, dim3(kNumSMs), dim3(kAdamThreads), 0, (cudaStream_t)stream, param_arena,
+                         grad_arena, static_cast<float*>(nullptr), nu, counts, segs, nseg, *hyper, reinterpret_cast<__nv_bfloat16*>(params_bf16),
+                         gnorm_out, reinterpret_cast<AdamScratch*>(scratch), none, RadamArgs{}));
   STX_LAUNCH_OK();
   return STX_OK;
 }

@@ -410,8 +410,9 @@ class AdamPlan:
     float4 items from `offset` on, so an offset must be a multiple of 4 floats (include/stx.h); a table that breaks this is
     refused here, before anything is allocated, instead of becoming a misaligned vector access on the device.
 
-    rule: "adam" (optax.scale_by_adam, stx_clip_adam_step) or "radam" (optax.scale_by_radam with eps_root and threshold,
-    stx_clip_radam_step); clip_adam_step runs whichever the plan holds."""
+    rule: "adam" (optax.scale_by_adam, stx_clip_adam_step), "radam" (optax.scale_by_radam with eps_root and threshold,
+    stx_clip_radam_step) or "rmsprop" (optax.rmsprop at its defaults with decay = b2, stx_clip_rmsprop_step: b1 is not read and the mu
+    arena is not touched); clip_adam_step runs whichever the plan holds."""
 
     def __init__(self, segments: Sequence[Tuple[int, int, float, float]], device, b1=0.9, b2=0.999, eps=1e-5,
                  decay=True, steps_per_update=1, num_updates=1, rule: str = "adam", eps_root: float = 0.0, threshold: float = 5.0):
@@ -443,8 +444,8 @@ class AdamPlan:
         self.scratch = torch.zeros(int(_lib.load().stx_adam_scratch_bytes(self.nseg)), dtype=torch.uint8, device=device)
         self.hyper = _lib.StxAdamHyper(float(b1), float(b2), float(eps), 1.0, int(bool(decay)),
                                        int(steps_per_update), int(num_updates), 0)
-        if rule not in ("adam", "radam"):
-            raise StxError(f"AdamPlan: rule={rule!r}; expected 'adam' or 'radam'")
+        if rule not in ("adam", "radam", "rmsprop"):
+            raise StxError(f"AdamPlan: rule={rule!r}; expected 'adam', 'radam' or 'rmsprop'")
         if rule == "radam" and eps_root < 0:
             raise StxError(f"AdamPlan: eps_root={eps_root} must be >= 0")
         self.rule = rule
@@ -470,6 +471,15 @@ def clip_adam_step(plan: AdamPlan, params: torch.Tensor, grads: torch.Tensor, mu
     plan.hyper.grad_scale = float(grad_scale)
     plan.hyper.prenorm = int(bool(prenorm))
     lib = _lib.load()
+    if plan.rule == "rmsprop":
+        if prenorm:
+            raise StxError("clip_adam_step: prenorm is not available with the rmsprop rule")
+        _lib.check(
+            lib.stx_clip_rmsprop_step(_p(params), _p(grads), _p(nu), _p(plan.counts), _p(plan.segs), plan.nseg, C.byref(plan.hyper),
+                                      _p(params_bf16), _p(plan.gnorm), _p(plan.scratch), _stream()),
+            "stx_clip_rmsprop_step",
+        )
+        return
     if plan.rule == "radam":
         if prenorm:
             raise StxError("clip_adam_step: prenorm is not available with the radam rule")
@@ -2037,3 +2047,74 @@ def dueling_q_backward(d_q: torch.Tensor, d_adv: torch.Tensor, d_value: torch.Te
     _need_cuda(d_value)
     _lib.check(_lib.load().stx_dueling_q_backward(_p(d_q), d_q.shape[0], A, _p(d_adv), _p(d_value), float(weight), int(bool(overwrite)), _stream()),
                "stx_dueling_q_backward")
+
+
+# ------------------------------------------------------------------------------------------------
+# IMPALA: reward statistics and the fused V-trace loss (stoix/systems/impala/sebulba/ff_impala.py:358-566)
+# ------------------------------------------------------------------------------------------------
+
+
+VTRACE_METRICS = ("actor_loss", "entropy", "value_loss", "q_estimate", "pg_advantage")
+
+
+def reward_stats(reward: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """{mean, population std} (float32[2], on the device) of a (T, E) float32 reward matrix whose rows may be strided (e.g. the first T
+    rows of a (T + 1, E) buffer, or a column block of one)."""
+    dev = _need_cuda(out)
+    if not reward.is_cuda or reward.dtype != torch.float32 or reward.ndim != 2 or reward.stride(1) != 1:
+        raise StxError("reward_stats: reward must be a CUDA float32 (T, E) matrix with unit column stride")
+    T, E = reward.shape
+    if out is None:
+        out = torch.empty(2, dtype=torch.float32, device=reward.device)
+    if out.dtype != torch.float32 or out.numel() < 2 or (dev is not None and dev != reward.device):
+        raise StxError("reward_stats: out must be float32[2] on the reward's device")
+    _lib.check(_lib.load().stx_reward_stats(_p(reward), T, E, reward.stride(0), _p(out), _stream()), "stx_reward_stats")
+    return out
+
+
+def _block(name: str, t: torch.Tensor, T: int, Em: int, dtype) -> int:
+    if not t.is_cuda or t.dtype != dtype or t.ndim != 2 or t.shape[0] < T or t.shape[1] != Em or t.stride(1) != 1:
+        raise StxError(f"vtrace_loss_grads: {name} must be a CUDA {dtype} (>= {T}, {Em}) matrix with unit column stride, got "
+                       f"{t.dtype} {tuple(t.shape)}")
+    return t.stride(0)
+
+
+def vtrace_loss_grads(logits: torch.Tensor, values: torch.Tensor, action: torch.Tensor, log_prob_b: torch.Tensor, reward: torch.Tensor,
+                      done: torch.Tensor, d_logits: torch.Tensor, d_value: torch.Tensor, metrics: torch.Tensor, gamma: float, lambda_: float,
+                      clip_rho: float, clip_pg_rho: float, ent_coef: float, vf_coef: float, reward_stats: Optional[torch.Tensor] = None,
+                      reward_scale: float = 1.0, reward_eps: float = 1e-8) -> None:
+    """One IMPALA minibatch in one launch (stx_vtrace_loss_grads, rules in include/stx.h): logits (T * Em, A) and values ((T + 1) * Em) of
+    the column block, time-major; action (int32), log_prob_b, reward (float32) and done (uint8 / bool) as (>= T, Em) matrices, typically a
+    column block of the learner's (T + 1, E) buffers.  Writes d_logits (T * Em, A), d_value ((T + 1) * Em, zero on the bootstrap row) and
+    metrics[:5] = VTRACE_METRICS.  reward_stats (float32[2] from reward_stats()) normalises the rewards as they are loaded."""
+    _need_cuda(logits, values, d_logits, d_value, metrics, reward_stats)
+    if logits.dtype != torch.float32 or logits.ndim != 2:
+        raise StxError("vtrace_loss_grads: logits must be float32 (T * Em, A)")
+    Em = int(action.shape[1]) if action.ndim == 2 else -1
+    if Em < 1 or logits.shape[0] % Em:
+        raise StxError(f"vtrace_loss_grads: action must be (T, Em) with Em dividing the {logits.shape[0]} logit rows")
+    T, A = logits.shape[0] // Em, int(logits.shape[1])
+    done8 = done.view(torch.uint8) if done.dtype == torch.bool else done
+    ld = _block("action", action, T, Em, torch.int32)
+    for name, t, dt in (("log_prob_b", log_prob_b, torch.float32), ("reward", reward, torch.float32), ("done", done8, torch.uint8)):
+        if _block(name, t, T, Em, dt) != ld:
+            raise StxError("vtrace_loss_grads: action, log_prob_b, reward and done must share one row stride")
+    if values.dtype != torch.float32 or values.numel() != (T + 1) * Em:
+        raise StxError(f"vtrace_loss_grads: values must be float32 with (T + 1) * Em = {(T + 1) * Em} entries")
+    if d_logits.dtype != torch.float32 or d_logits.numel() != T * Em * A or d_value.dtype != torch.float32 or d_value.numel() != (T + 1) * Em:
+        raise StxError("vtrace_loss_grads: d_logits must be float32 (T * Em, A) and d_value float32 ((T + 1) * Em)")
+    if metrics.dtype != torch.float32 or metrics.numel() < _lib.STX_VTRACE_METRICS:
+        raise StxError(f"vtrace_loss_grads: metrics must be float32 with {_lib.STX_VTRACE_METRICS} entries")
+    if reward_stats is not None and (reward_stats.dtype != torch.float32 or reward_stats.numel() < 2):
+        raise StxError("vtrace_loss_grads: reward_stats must be float32[2]")
+    lib = _lib.load()
+    a = _lib.StxVtraceLoss()
+    a.logits, a.values, a.action, a.log_prob_b = logits.data_ptr(), values.data_ptr(), action.data_ptr(), log_prob_b.data_ptr()
+    a.reward, a.done = reward.data_ptr(), done8.data_ptr()
+    a.reward_stats = reward_stats.data_ptr() if reward_stats is not None else None
+    a.d_logits, a.d_value, a.metrics = d_logits.data_ptr(), d_value.data_ptr(), metrics.data_ptr()
+    a.ld, a.T, a.Em, a.A = ld, T, Em, A
+    a.gamma, a.lambda_, a.clip_rho, a.clip_pg_rho = float(gamma), float(lambda_), float(clip_rho), float(clip_pg_rho)
+    a.ent_coef, a.vf_coef, a.reward_scale, a.reward_eps = float(ent_coef), float(vf_coef), float(reward_scale), float(reward_eps)
+    scratch = _zeros_scratch(("vtrace",), lib.stx_vtrace_loss_scratch_bytes(), logits.device)
+    _lib.check(lib.stx_vtrace_loss_grads(C.byref(a), _p(scratch), _stream()), "stx_vtrace_loss_grads")

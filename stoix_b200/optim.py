@@ -1,8 +1,9 @@
-"""optax-shaped facade over the fused optimiser kernels (stx_clip_adam_step, stx_clip_radam_step).
+"""optax-shaped facade over the fused optimiser kernels (stx_clip_adam_step, stx_clip_radam_step, stx_clip_rmsprop_step).
 
 `chain(clip_by_global_norm(m), adam(lr, eps=...))` mirrors the construction at
 stoix/systems/ppo/anakin/ff_ppo.py:456-463.  The returned object's `.update` is what the reference
-passes around as `update_fns`; `chain(clip_by_global_norm(m), radam(lr))` (ff_pqn.py:263-267) runs the RAdam rule; the learner reads its hyper-parameters and runs BOTH optimisers
+passes around as `update_fns`; `chain(clip_by_global_norm(m), radam(lr))` (ff_pqn.py:263-267) runs the RAdam rule and
+`chain(clip_by_global_norm(m), rmsprop(lr))` (ff_impala.py:754-766) the RMSProp rule; the learner reads its hyper-parameters and runs BOTH optimisers
 (actor and critic) in a single fused launch over the flat arenas."""
 from __future__ import annotations
 
@@ -29,6 +30,13 @@ class _Radam(_Adam):
     threshold: float = 5.0
 
 
+@dataclass
+class _Rmsprop:
+    learning_rate: Union[float, Callable]
+    decay: float = 0.9
+    eps: float = 1e-8
+
+
 def clip_by_global_norm(max_norm: float) -> _Clip:
     return _Clip(float(max_norm))
 
@@ -42,6 +50,18 @@ def adam(learning_rate, b1: float = 0.9, b2: float = 0.999, eps: float = 1e-8, e
 def radam(learning_rate, b1: float = 0.9, b2: float = 0.999, eps: float = 1e-8, eps_root: float = 0.0, threshold: float = 5.0) -> _Radam:
     """optax.radam (scale_by_radam without nesterov, then the learning rate), as ff_pqn.py:263-267 chains it after the clip."""
     return _Radam(learning_rate, b1, b2, eps, eps_root, threshold)
+
+
+def rmsprop(learning_rate, decay: float = 0.9, eps: float = 1e-8, initial_scale: float = 0.0, eps_in_sqrt: bool = True, centered: bool = False,
+            momentum: Optional[float] = None, nesterov: bool = False, bias_correction: bool = False) -> _Rmsprop:
+    """optax.rmsprop: scale_by_rms (nu = (1 - decay) g^2 + decay nu, u = g / sqrt(nu + eps)), then the learning rate.  Only the defaults
+    IMPALA uses (ff_impala.py:754-766) are built; the state is the nu arena alone."""
+    if centered or momentum is not None or nesterov or bias_correction:
+        raise NotImplementedError("rmsprop: centered, momentum, nesterov and bias_correction are not used by the reference IMPALA and are "
+                                  "not built")
+    if initial_scale != 0.0 or not eps_in_sqrt:
+        raise NotImplementedError("rmsprop: only initial_scale=0 and eps_in_sqrt=True (optax's defaults) are built")
+    return _Rmsprop(learning_rate, float(decay), float(eps))
 
 
 class OptState(NamedTuple):
@@ -61,13 +81,13 @@ class GradientTransformation:
     `apply_updates(params, updates)` reproduces optax's two-step form.  The learner itself does not go through this
     face: it steps both optimisers in place in one launch over the shared arena and only reads the hyper-parameters."""
 
-    def __init__(self, clip: Optional[_Clip], adam_: _Adam):
+    def __init__(self, clip: Optional[_Clip], adam_: Union[_Adam, _Rmsprop]):
         self.clip, self.adam = clip, adam_
 
     @property
     def rule(self) -> str:
-        """"radam" for an optax.radam stage, else "adam"."""
-        return "radam" if isinstance(self.adam, _Radam) else "adam"
+        """"radam" for an optax.radam stage, "rmsprop" for an optax.rmsprop stage, else "adam"."""
+        return "radam" if isinstance(self.adam, _Radam) else "rmsprop" if isinstance(self.adam, _Rmsprop) else "adam"
 
     @property
     def max_grad_norm(self) -> float:
@@ -129,9 +149,13 @@ def adam_plan(segments: Sequence[Tuple[int, int, GradientTransformation]], devic
 
     opt = segments[0][2]
     sched = opt.schedule
-    rule = {"rule": "radam", "eps_root": opt.adam.eps_root, "threshold": opt.adam.threshold} if opt.rule == "radam" else {}
+    if opt.rule == "rmsprop":  # the kernel reads the RMSProp decay from b2
+        rule = {"rule": "rmsprop", "b1": 0.0, "b2": opt.adam.decay}
+    else:
+        rule = {"rule": "radam", "eps_root": opt.adam.eps_root, "threshold": opt.adam.threshold} if opt.rule == "radam" else {}
+        rule.update(b1=opt.adam.b1, b2=opt.adam.b2)
     plan = ops.AdamPlan([(off, n, o.init_lr, o.max_grad_norm if o.clip is not None else 3.0e38) for off, n, o in segments], device,
-                        b1=opt.adam.b1, b2=opt.adam.b2, eps=opt.adam.eps, decay=sched is not None,
+                        eps=opt.adam.eps, decay=sched is not None,
                         steps_per_update=getattr(sched, "steps_per_update", 1), num_updates=getattr(sched, "num_updates", 1), **rule)
     plan.counts = counts
     return plan
@@ -152,7 +176,7 @@ def arena_state(tree, arena, segments: Sequence[Tuple[int, int]]) -> List[OptSta
 
 def chain(*parts) -> GradientTransformation:
     clip = next((p for p in parts if isinstance(p, _Clip)), None)
-    adam_ = next((p for p in parts if isinstance(p, _Adam)), None)
+    adam_ = next((p for p in parts if isinstance(p, (_Adam, _Rmsprop))), None)
     if adam_ is None:
-        raise ValueError("chain() needs an adam() or radam() stage")
+        raise ValueError("chain() needs an adam(), radam() or rmsprop() stage")
     return GradientTransformation(clip, adam_)

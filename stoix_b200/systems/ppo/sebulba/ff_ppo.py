@@ -95,10 +95,15 @@ def _precision(config) -> int:
 
 class InferenceServer:
     """The batched policy / value evaluation of ONE actor thread (sebulba/ff_ppo.py:123-143 `get_act_fn`, jitted onto the
-    actor device at :160-161).  Owns a CUDA stream, pinned host buffers and the thread's (T+1)-step device storage."""
+    actor device at :160-161).  Owns a CUDA stream, pinned host buffers and the thread's (T+1)-step device storage.
+
+    `transition` is the NamedTuple the storage is delivered as; one without a `value` field (IMPALA's actors sample from the actor
+    alone) skips the critic forward."""
 
     def __init__(self, specs: Tuple[ops.MlpSpec, ops.MlpSpec], device: torch.device, num_envs: int, rollout_length: int,
-                 precision: int, seed: int, thread_id: int):
+                 precision: int, seed: int, thread_id: int, transition: type = PPOTransition):
+        self.transition = transition
+        self.critic = "value" in self.transition._fields
         self.sa, self.sc = specs
         self.device, self.E, self.T, self.precision, self.seed, self.tid = device, int(num_envs), int(rollout_length), precision, int(seed), thread_id
         _, self.coff, _ = ops.arena_offsets(self.sa, self.sc)
@@ -135,8 +140,9 @@ class InferenceServer:
                 self.obs[slot].copy_(self.h_obs, non_blocking=True)
             ops.mlp_forward(self.sa, a_flat, self.obs[slot], precision=self.precision, params_bf16=a16, out=self.logits, ws_key=key)
             ops.categorical(self.logits, None, self.seed, self.calls, out=(self.action[slot], self.log_prob[slot]))
-            ops.mlp_forward(self.sc, c_flat, self.obs[slot], precision=self.precision, params_bf16=c16,
-                            out=self.value[slot].view(self.E, 1), ws_key=key)
+            if self.critic:
+                ops.mlp_forward(self.sc, c_flat, self.obs[slot], precision=self.precision, params_bf16=c16,
+                                out=self.value[slot].view(self.E, 1), ws_key=key)
             self.h_action.copy_(self.action[slot], non_blocking=True)
             self.step_event.record(self.stream)
         self.step_event.synchronize()                                      # the host needs the actions to step the envs
@@ -160,8 +166,8 @@ class InferenceServer:
             self.truncated[lo:].copy_(self.h_trunc[lo:], non_blocking=True)
         self.h2d_bytes += (self.T + 1 - lo) * self.E * 6
 
-    def storage(self) -> PPOTransition:
-        return PPOTransition(self.done, self.truncated, self.action, self.value, self.reward, self.log_prob, self.obs)
+    def storage(self):
+        return self.transition(*[getattr(self, name) for name in self.transition._fields])
 
     def carry_last(self) -> None:
         """Keep the last transition as row 0 of the next rollout (sebulba/ff_ppo.py:279)."""
@@ -191,8 +197,9 @@ def get_act_fn(apply_fns: Tuple[ActorApply, CriticApply]) -> Callable:
 def get_rollout_fn(env_factory: cpu_envs.EnvFactory, actor_device: torch.device, parameter_server: ParameterServer,
                    rollout_pipeline: OnPolicyPipeline, apply_fns: Tuple[ActorApply, CriticApply], config: DictConfig,
                    logger: StoixLogger, learner_devices: Sequence[torch.device], seeds: List[int],
-                   thread_lifetime: ThreadLifetime) -> Callable[[int], None]:
-    """Create rollout function for actor threads (sebulba/ff_ppo.py:145-333)."""
+                   thread_lifetime: ThreadLifetime, transition: type = PPOTransition) -> Callable[[int], None]:
+    """Create rollout function for actor threads (sebulba/ff_ppo.py:145-333).  `transition`: the type of the delivered shards (see
+    InferenceServer)."""
     num_envs_per_actor = int(config.arch.actor.num_envs_per_actor)
     rollout_length = int(config.system.rollout_length)
     num_actor_threads = int(config.arch.actor.actor_per_device)
@@ -213,7 +220,7 @@ def get_rollout_fn(env_factory: cpu_envs.EnvFactory, actor_device: torch.device,
         local_step_count, actor_policy_version, num_rollouts = 0, -1, 0
         timer = TimingTracker(maxlen=10)
         server = InferenceServer(specs, actor_device, num_envs_per_actor, rollout_length, _precision(config), int(rng_key) & ((1 << 62) - 1),
-                                 thread_lifetime.id)
+                                 thread_lifetime.id, transition)
         rollout_fn.server = server  # exposed for tests / bench
         episode_metrics_storage: List[Dict[str, np.ndarray]] = []
         timestep = envs.reset(seed=seeds)
@@ -253,8 +260,8 @@ def get_rollout_fn(env_factory: cpu_envs.EnvFactory, actor_device: torch.device,
                     shards = []
                     for li, ld in enumerate(learner_devices):
                         sl = slice(li * per, (li + 1) * per)
-                        shards.append(PPOTransition(*[t[:, sl].to(ld, non_blocking=True) if ld != actor_device or n_learn > 1 else t.clone()
-                                                      for t in server.storage()]))
+                        shards.append(transition(*[t[:, sl].to(ld, non_blocking=True) if ld != actor_device or n_learn > 1 else t.clone()
+                                                   for t in server.storage()]))
                     ready.record(server.stream)
                 payload = (local_step_count, actor_policy_version, (shards, ready))
             with timer.time("rollout_queue_put_time"):
@@ -286,11 +293,11 @@ def get_rollout_fn(env_factory: cpu_envs.EnvFactory, actor_device: torch.device,
 
 
 def get_actor_thread(env_factory, actor_device, parameter_server, rollout_pipeline, apply_fns, rng_key, config, seeds, logger,
-                     learner_devices, thread_lifetime) -> threading.Thread:
+                     learner_devices, thread_lifetime, transition: type = PPOTransition) -> threading.Thread:
     """Create actor thread for environment data collection (sebulba/ff_ppo.py:336-375)."""
     rollout_fn = get_rollout_fn(env_factory=env_factory, actor_device=actor_device, parameter_server=parameter_server,
                                 rollout_pipeline=rollout_pipeline, apply_fns=apply_fns, config=config, logger=logger,
-                                learner_devices=learner_devices, seeds=seeds, thread_lifetime=thread_lifetime)
+                                learner_devices=learner_devices, seeds=seeds, thread_lifetime=thread_lifetime, transition=transition)
     th = threading.Thread(target=rollout_fn, args=(rng_key,), name=thread_lifetime.name)
     th.rollout_fn = rollout_fn
     return th
@@ -299,6 +306,13 @@ def get_actor_thread(env_factory, actor_device, parameter_server, rollout_pipeli
 # ---------------------------------------------------------------------------------------------------------------
 # learner side
 # ---------------------------------------------------------------------------------------------------------------
+
+
+def learner_envs(config: DictConfig) -> int:
+    """Environments per learner batch (total_num_envs over the learner devices); refuses more than one learner device."""
+    n_learn = len(config.arch.learner.device_ids)
+    assert n_learn == 1, "this build drives ONE learner device per process (see the module docstring)"
+    return int(config.arch.total_num_envs) // n_learn
 
 
 def get_learner_step_fn(apply_fns: Tuple[ActorApply, CriticApply], update_fns: Tuple[Callable, Callable],
@@ -310,9 +324,7 @@ def get_learner_step_fn(apply_fns: Tuple[ActorApply, CriticApply], update_fns: T
     actor_opt, critic_opt = update_fns[0].__self__, update_fns[1].__self__
     sysc, arch = config.system, config.arch
     T, epochs, nmb = int(sysc.rollout_length), int(sysc.epochs), int(sysc.num_minibatches)
-    n_learn = len(arch.learner.device_ids)
-    assert n_learn == 1, "this build drives ONE learner device per process (see the module docstring)"
-    E = int(arch.total_num_envs) // n_learn   # envs_per_batch (:522)
+    E = learner_envs(config)   # envs_per_batch (:522)
     B = T * E
     assert B % nmb == 0, "rollout_length * envs_per_batch must be divisible by num_minibatches"
     mb = B // nmb
@@ -501,8 +513,10 @@ def get_sebulba_eval_fn(env_factory: cpu_envs.EnvFactory, act_fn: Callable, conf
 
 
 def learner_setup(env_factory: cpu_envs.EnvFactory, keys: Tuple[int, int, int], learner_devices: Sequence[torch.device],
-                  config: DictConfig) -> Tuple[Callable, Tuple[ActorApply, CriticApply], CoreLearnerState]:
-    """Setup learner networks and initial state (sebulba/ff_ppo.py:703-798)."""
+                  config: DictConfig, optimisers: Optional[Tuple[Any, Any]] = None,
+                  step_fn_factory: Optional[Callable] = None) -> Tuple[Callable, Tuple[ActorApply, CriticApply], CoreLearnerState]:
+    """Setup learner networks and initial state (sebulba/ff_ppo.py:703-798).  Another actor-critic Sebulba system passes its
+    (actor, critic) optimisers and its get_learner_step_fn; the defaults are PPO's."""
     env = env_factory(num_envs=1)
     num_actions = int(env.action_space().num_values)
     obs_shape = tuple(env.observation_space().shape)
@@ -521,10 +535,12 @@ def learner_setup(env_factory: cpu_envs.EnvFactory, keys: Tuple[int, int, int], 
     precision = _precision(config)
     actor_network.precision = critic_network.precision = precision
 
-    actor_lr = make_learning_rate(config.system.actor_lr, config, config.system.epochs, config.system.num_minibatches)
-    critic_lr = make_learning_rate(config.system.critic_lr, config, config.system.epochs, config.system.num_minibatches)
-    actor_optim = optax.chain(optax.clip_by_global_norm(config.system.max_grad_norm), optax.adam(actor_lr, eps=1e-5))
-    critic_optim = optax.chain(optax.clip_by_global_norm(config.system.max_grad_norm), optax.adam(critic_lr, eps=1e-5))
+    if optimisers is None:
+        actor_lr = make_learning_rate(config.system.actor_lr, config, config.system.epochs, config.system.num_minibatches)
+        critic_lr = make_learning_rate(config.system.critic_lr, config, config.system.epochs, config.system.num_minibatches)
+        optimisers = (optax.chain(optax.clip_by_global_norm(config.system.max_grad_norm), optax.adam(actor_lr, eps=1e-5)),
+                      optax.chain(optax.clip_by_global_norm(config.system.max_grad_norm), optax.adam(critic_lr, eps=1e-5)))
+    actor_optim, critic_optim = optimisers
 
     obs_dim = int(np.prod(obs_shape))
     with torch.cuda.device(device):
@@ -543,15 +559,16 @@ def learner_setup(env_factory: cpu_envs.EnvFactory, keys: Tuple[int, int, int], 
     params = ActorCriticParams(actor_params, critic_params)
     apply_fns = (actor_network.apply, critic_network.apply)
     update_fns = (actor_optim.update, critic_optim.update)
-    learn_step = get_learner_step_fn(apply_fns, update_fns, config)
+    learn_step = (step_fn_factory or get_learner_step_fn)(apply_fns, update_fns, config)
     if warm_start(config, arena) and arena_bf16 is not None:
         ops.cast_bf16(arena, out=arena_bf16)
     learner_state = CoreLearnerState(params, opt_states, int(key) & ((1 << 62) - 1))
     return learn_step, apply_fns, learner_state
 
 
-def run_experiment(_config: DictConfig) -> float:
-    """Run PPO experiment (sebulba/ff_ppo.py:801-1023)."""
+def run_experiment(_config: DictConfig, setup: Optional[Callable] = None, transition: type = PPOTransition) -> float:
+    """Run PPO experiment (sebulba/ff_ppo.py:801-1023).  Another Sebulba system runs through the same threads by passing its own
+    `setup` (the signature of learner_setup) and the transition type its actors deliver."""
     from stoix_b200.evaluator import get_distribution_act_fn
 
     config = copy.deepcopy(_config)
@@ -570,7 +587,7 @@ def run_experiment(_config: DictConfig) -> float:
     key, key_e, actor_net_key, critic_net_key = srandom.split(srandom.PRNGKey(config.arch.seed), 4)
     np_rng = np.random.default_rng(int(config.arch.seed))
     torch.cuda.set_device(learner_devices[0])
-    learn_step, apply_fns, learner_state = learner_setup(env_factory, (key, actor_net_key, critic_net_key), learner_devices, config)
+    learn_step, apply_fns, learner_state = (setup or learner_setup)(env_factory, (key, actor_net_key, critic_net_key), learner_devices, config)
 
     eval_act_fn = get_distribution_act_fn(config, apply_fns[0])
     evaluator, evaluator_envs = get_sebulba_eval_fn(env_factory, eval_act_fn, config, np_rng, evaluator_device)
@@ -599,7 +616,7 @@ def run_experiment(_config: DictConfig) -> float:
             seeds = np_rng.integers(np.iinfo(np.int32).max, size=int(config.arch.actor.num_envs_per_actor)).tolist()
             lt = ThreadLifetime(thread_name=f"Actor-{dev.index}-{thread_id}-idx-{idx}", thread_id=idx)
             th = get_actor_thread(env_factory, dev, parameter_server, rollout_pipeline, apply_fns, thread_keys[idx], config, seeds, logger,
-                                  learner_devices, lt)
+                                  learner_devices, lt, transition)
             th.start()
             actor_threads.append(th)
             lifetimes.append(lt)
