@@ -182,8 +182,11 @@ int stx_tc_debug_set_clock_buffer(long long* buf);
 int stx_tc_debug_set_prof_buffer(long long* buf);
 
 /* Categorical head ops on logits (E, A) -- tfd.Categorical (stoix/networks/heads.py:41) as used at
- * ff_ppo.py:100-101.  If sample != 0: action = argmax_j(logits_j + Gumbel_j) with Philox4x32-10
- * keyed by seed with counter (row, call = offset + *dev_counter); else `action` is an input.
+ * ff_ppo.py:100-101.  If sample != 0: action = argmax_j(logits_j + Gumbel_j) (the first index on exact
+ * ties), Gumbel_j = -log(-log u01(w)) of word j & 3 of Philox4x32-10 keyed by (seed lo, seed hi) with
+ * counter (row lo, call lo, (call >> 32) ^ ((row >> 32) << 16) ^ (g << 24), "CATG" = 0x43415447),
+ * call = offset + *dev_counter and group g = j / 4; else `action` is an input.  The group field has
+ * 8 bits, so A <= 1024 (STX_E_SHAPE otherwise): beyond it the noise of group 256 would be group 0's.
  * dev_counter (nullable device uint64) lets a captured CUDA graph draw fresh numbers on every
  * replay: the caller bumps it with stx_counter_add at the end of the graph.  Always writes
  * log_prob = log_softmax(logits)[action]; entropy (nullable) = -sum p log p. */
@@ -324,11 +327,12 @@ int stx_synth_env_step(int64_t E, int D, uint64_t seed, uint64_t step, const uin
                        uint8_t* is_terminal, void* stream);
 
 /* Fused persistent rollout of the synthetic env on the bf16 tensor-core path: the T-step scan of _env_step
- * (ff_ppo.py:81-140) for the actor side in ONE launch (grid = E/128 CTAs, each owning 128 envs for all T
+ * (ff_ppo.py:81-140) for the actor side in ONE launch (grid = E/64 CTAs, each owning 64 envs for all T
  * steps): logits -> Gumbel-max action + log_prob (same Philox counters as stx_categorical with seed
  * cat_seed, call = cat_offset + t + *cat_counter) and the env step of stx_synth_env_step (step = env_step + t +
  * *env_counter), trajectory written time-major: obs (T+1,E,D) bf16 [row 0 is the input], next_obs (T,E,D)
- * bf16, the rest (T,E).  Bit-identical to the per-step path.  E % 128 == 0; actor as for STX_PREC_BF16. */
+ * bf16, the rest (T,E).  Bit-identical to the per-step path.  E % 64 == 0; actor MLP [D <= 64 (multiple
+ * of 8), 256, 256, A <= 16], relu, no LayerNorm, as for STX_PREC_BF16. */
 int stx_tc_rollout_synth(const StxMlp* actor, void* obs, void* next_obs, int32_t* action, float* log_prob,
                          float* reward, uint8_t* done, uint8_t* truncated, float* ep_return, int32_t* ep_length,
                          uint8_t* is_terminal, float* run_return, int32_t* run_length, int T, int64_t E,
@@ -882,8 +886,11 @@ int stx_n_step_returns_f32(const float* r_t, const float* discount_t, const floa
  *   Outputs are time-major (S, B): obs (S, B, D), action (S, B, act_words), reward, done, log_prob.  period != 1 -> STX_E_UNSUPPORTED.
  * stx_mpo_sample_actions: the target-Q input rows of M states in one launch, xq ((A + N + 1) M, D + A): block j < A holds
  *   [obs_i | one_hot(j)] (the actor loss evaluates every action, ff_mpo.py:189-197), block A + n holds [obs_i | one_hot(a_ni)] with a_ni
- *   drawn by inverse CDF from Categorical(logits_b[i]) (the bootstrap policy; its mode when stochastic = 0, with N = 1), or act_in (N, M)
- *   when given, written to act_out (N, M, nullable); block A + N holds [obs_i | one_hot(action_i)].  Per state it also writes
+ *   drawn by inverse CDF from Categorical(logits_b[i]) (the bootstrap policy; its mode, the first maximum, when stochastic = 0, with
+ *   N = 1), or act_in (N, M) when given, written to act_out (N, M, nullable); block A + N holds [obs_i | one_hot(action_i)].  The draw
+ *   is the first j with u < the fp32 running sum of softmax_j, u = u01(word 0 of Philox(seed lo, seed hi; n M + i lo, n M + i hi,
+ *   call lo, "MPOA" = 0x4D504F41 ^ call hi)), call = offset + *dev_counter; a u at or above the whole sum (fp32 rounding) takes the
+ *   last action with positive fp32 probability.  Per state it also writes
  *   log_rho = log_softmax(logits_t)[action] - log_prob, r = clip(reward, +-max_abs_reward) and d = (1 - done) gamma.
  * stx_mpo_loss_grads: categorical_mpo_loss (discrete_loss.py:20-147) over M states, q (A, M): eta = softplus(duals[0]) + 1e-8,
  *   alpha = softplus(duals[1]) + 1e-8, u = q / eta + log_softmax(target), w = softmax(u), loss = mean CE(w, online) + alpha mean KL(target

@@ -446,7 +446,8 @@ extern "C" int stx_categorical(const float* logits, int64_t E, int A, int sample
                                uint64_t offset, const uint64_t* dev_counter, int32_t* action,
                                float* log_prob, float* entropy, void* stream) {
   STX_REQUIRE(logits && action && log_prob, STX_E_ARG, "stx_categorical: null pointer");
-  STX_REQUIRE(E > 0 && A > 0, STX_E_SHAPE, "stx_categorical: E=%lld A=%d", (long long)E, A);
+  // the noise of actions 4g..4g+3 is keyed by g in an 8-bit counter field: past 256 groups the noise would repeat
+  STX_REQUIRE(E > 0 && A > 0 && A <= 1024, STX_E_SHAPE, "stx_categorical: E=%lld A=%d (1..1024)", (long long)E, A);
   categorical_kernel<<<(unsigned)((E + 255) / 256), 256, 0, (cudaStream_t)stream>>>(logits, E, A, sample, seed, offset, dev_counter, action, log_prob, entropy);
   STX_LAUNCH_OK();
   return STX_OK;

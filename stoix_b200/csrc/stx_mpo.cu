@@ -130,15 +130,21 @@ __global__ void __launch_bounds__(256) mpo_rows_kernel(StxMpoRows a, uint64_t ca
                                      make_uint2((uint32_t)a.seed, (uint32_t)(a.seed >> 32)));
       const float u = u01(wd.x);
       const float lse = row_lse(z, A);
+      // inverse CDF.  The fp32 sum can end below u (u01 reaches 1 - 2^-24): that remainder goes to the last action with positive
+      // fp32 probability, never to an action whose probability has underflowed to 0
       float cum = 0.f;
-      act = A - 1;  // inverse CDF; rounding leaves the last action the remainder
+      int last = 0;
+      act = -1;
       for (int j = 0; j < A; ++j) {
-        cum += expf(z[j] - lse);
+        const float p = expf(z[j] - lse);
+        if (p > 0.f) last = j;
+        cum += p;
         if (u < cum) {
           act = j;
           break;
         }
       }
+      if (act < 0) act = last;
     }
     if (lane == 0 && a.act_out) a.act_out[(int64_t)n * M + i] = act;
   } else {

@@ -62,7 +62,7 @@ def _rel(a, b):
     return np.linalg.norm(a - b) / max(np.linalg.norm(b), 1e-30)
 
 
-@pytest.mark.parametrize("B,mb_off,mb,D,A,use_perm", [
+_MINIBATCH_CASES = [
     (2048, 512, 1024, 64, 8, True),
     (512, 128, 256, 32, 5, False),
     (16384, 0, 16384, 64, 8, True),   # > 1 tile per CTA, every split-K CTA busy
@@ -70,14 +70,23 @@ def _rel(a, b):
     # BASELINE config 2 (the shape bench.py runs): B = T*E = 524 288 rows, minibatch 32 768 = 256 tiles per
     # network (3.46 tiles per K3a CTA, every split-K CTA with >= 7 chunks), shuffle indices up to 2^19
     (524288, 5 * 32768, 32768, 64, 8, True),
-])
-def test_tc_ppo_minibatch_grads_vs_bf16_oracle(B, mb_off, mb, D, A, use_perm):
+]
+
+
+@pytest.mark.parametrize("B,mb_off,mb,D,A,use_perm,saturated",
+                         [pytest.param(*c, False, id="-".join(map(str, c))) for c in _MINIBATCH_CASES]
+                         # K3a's actor head (__expf / __logf) at saturation: the final bias puts the other actions 30 to 110 below
+                         # action 0, so the taken action's log-probability reaches ~ -110 and most probabilities underflow
+                         + [pytest.param(2048, 512, 1024, 64, 8, True, True, id="saturated-2048-512-1024-64-8-True")])
+def test_tc_ppo_minibatch_grads_vs_bf16_oracle(B, mb_off, mb, D, A, use_perm, saturated):
     """K3 on tensor cores vs the oracle with the same bf16 operand rounding (weights, activations, dY);
     what is left is fp32 summation order and rare relu/rounding flips -> norm-wise 5e-3 per tensor."""
     from stoix_b200 import ops
 
     rng = np.random.default_rng(B + mb + A)
     actor, critic = _net(rng, D, A, 0.3), _net(rng, D, 1, 1.0)
+    if saturated:
+        actor.b[-1] = -np.concatenate([[0.0], np.linspace(30.0, 110.0, A - 1)])
     sa, sc = ops.MlpSpec((D, 256, 256, A)), ops.MlpSpec((D, 256, 256, 1))
     _, coff, total = ops.arena_offsets(sa, sc)
     flat = np.zeros(total, np.float32)
