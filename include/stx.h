@@ -326,13 +326,35 @@ int stx_synth_env_step(int64_t E, int D, uint64_t seed, uint64_t step, const uin
                        int32_t* run_length, float* ep_return, int32_t* ep_length,
                        uint8_t* is_terminal, void* stream);
 
-/* Fused persistent rollout of the synthetic env on the bf16 tensor-core path: the T-step scan of _env_step
- * (ff_ppo.py:81-140) for the actor side in ONE launch (grid = E/64 CTAs, each owning 64 envs for all T
- * steps): logits -> Gumbel-max action + log_prob (same Philox counters as stx_categorical with seed
- * cat_seed, call = cat_offset + t + *cat_counter) and the env step of stx_synth_env_step (step = env_step + t +
- * *env_counter), trajectory written time-major: obs (T+1,E,D) bf16 [row 0 is the input], next_obs (T,E,D)
- * bf16, the rest (T,E).  Bit-identical to the per-step path.  E % 64 == 0; actor MLP [D <= 64 (multiple
- * of 8), 256, 256, A <= 16], relu, no LayerNorm, as for STX_PREC_BF16. */
+/* Steps [0, T) of the synthetic env for all E envs in one launch over the whole GPU (its dynamics ignore the action):
+ * exactly T calls of stx_synth_env_step with step = step + t + *dev_counter, written time-major: obs (T+1,E,D) bf16
+ * [row 0 is the input, rows 1..T are written], next_obs (T,E,D) bf16, the rest (T,E); run_return / run_length carried.
+ * D % 4 == 0, D <= 128. */
+int stx_synth_env_trajectory(int64_t E, int D, int T, uint64_t seed, uint64_t step, const uint64_t* dev_counter, float p_term,
+                             float p_trunc, void* obs, void* next_obs, float* reward, uint8_t* done, uint8_t* truncated,
+                             float* ep_return, int32_t* ep_length, uint8_t* is_terminal, float* run_return, int32_t* run_length,
+                             void* stream);
+
+/* The actor side of the T-step scan of _env_step (ff_ppo.py:81-140) over observations that already exist (obs (T,E,D)
+ * bf16, time-major, e.g. from stx_synth_env_trajectory; valid when the dynamics ignore the action, so no step waits for
+ * the one before) in ONE persistent launch of min(T E / 64, max_ctas or one per SM) CTAs walking the 64-row tiles:
+ * logits -> Gumbel-max action + log_prob (same Philox counters as stx_categorical with seed cat_seed, call = cat_offset +
+ * t + *cat_counter), written (T,E).  E % 64 == 0; actor MLP [D <= 64 (multiple of 8), 256, 256, A <= 16], relu, no
+ * LayerNorm, as for STX_PREC_BF16. */
+int stx_tc_rollout_policy(const StxMlp* actor, const void* obs, int32_t* action, float* log_prob, int T, int64_t E,
+                          uint64_t cat_seed, uint64_t cat_offset, const uint64_t* cat_counter, int max_ctas, void* stream);
+
+/* The rollout's critic values on the bf16 tensor-core path: value[t] = critic(obs[t]), bootstrap_value[t] =
+ * critic(next_obs[t]) for (T,E) rows, from one forward over obs[0..T] (next_obs[t] == obs[t+1] unless is_terminal[t])
+ * and one over the next_obs rows where an episode ended.  Bit-identical to two full forward passes.  Obeys
+ * stx_tc_set_forward_ctas.  ws: stx_tc_rollout_values_workspace_bytes(T, E, D) bytes. */
+size_t stx_tc_rollout_values_workspace_bytes(int T, int64_t E, int D);
+int stx_tc_rollout_values(const StxMlp* critic, const void* obs, const void* next_obs, const uint8_t* is_terminal, int T, int64_t E,
+                          float* value, float* bootstrap_value, void* ws, size_t ws_bytes, void* stream);
+
+/* Fused rollout of the synthetic env on the bf16 tensor-core path: stx_synth_env_trajectory followed by
+ * stx_tc_rollout_policy on the same stream (env step = env_step + t + *env_counter).  Bit-identical to the per-step
+ * path.  E % 64 == 0; actor as for stx_tc_rollout_policy. */
 int stx_tc_rollout_synth(const StxMlp* actor, void* obs, void* next_obs, int32_t* action, float* log_prob,
                          float* reward, uint8_t* done, uint8_t* truncated, float* ep_return, int32_t* ep_length,
                          uint8_t* is_terminal, float* run_return, int32_t* run_length, int T, int64_t E,

@@ -390,6 +390,10 @@ _SIGNATURES = {
     "stx_make_permutation": (C.c_int, [_P, C.c_int64, C.c_uint64, C.c_uint64, _P, _P]),
     "stx_counter_add": (C.c_int, [_P, C.c_uint64, _P]),
     "stx_synth_env_step": (C.c_int, [C.c_int64, C.c_int, C.c_uint64, C.c_uint64, _P, C.c_float, C.c_float, _P, _P, _P, C.c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "stx_synth_env_trajectory": (C.c_int, [C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_uint64, _P, C.c_float, C.c_float] + [_P] * 11),
+    "stx_tc_rollout_policy": (C.c_int, [C.POINTER(StxMlp), _P, _P, _P, C.c_int, C.c_int64, C.c_uint64, C.c_uint64, _P, C.c_int, _P]),
+    "stx_tc_rollout_values_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int]),
+    "stx_tc_rollout_values": (C.c_int, [C.POINTER(StxMlp), _P, _P, _P, C.c_int, C.c_int64, _P, _P, _P, C.c_size_t, _P]),
     "stx_tc_rollout_synth": (C.c_int, [C.POINTER(StxMlp)] + [_P] * 12 + [C.c_int, C.c_int64, C.c_uint64, C.c_uint64, _P, C.c_float, C.c_float,
                                         C.c_uint64, C.c_uint64, _P, _P]),
     "stx_cast_f32_to_bf16": (C.c_int, [_P, _P, C.c_int64, _P]),

@@ -42,6 +42,7 @@ struct FwdParams {
   int64_t M;
   int A;
   int num_tiles;
+  const int32_t* dev_rows;  // optional: the row count is read from the device (M is then the capacity of x)
 };
 
 __device__ __forceinline__ void store_dbg(float* dbg, const uint32_t (&a)[64], int64_t row, int64_t M, int lane) {
@@ -70,6 +71,14 @@ __global__ void __launch_bounds__(kThreads, 1)
   const int wg = threadIdx.x >> 7, t = threadIdx.x & 127, warp = t >> 5, lane = threadIdx.x & 31;
   uint64_t* x_full = bars + 1 + 2 * wg;  // [2] per warpgroup
 
+  int64_t M = p.M;
+  int num_tiles = p.num_tiles;
+  if (p.dev_rows != nullptr) {  // a row count known only on the device: CTAs without a tile leave before loading weights
+    M = *p.dev_rows;
+    num_tiles = (int)((M + kTileM - 1) / kTileM);
+    if ((int)blockIdx.x * kWG >= num_tiles) return;
+  }
+
   if (threadIdx.x == 0) {
     mbar_init(w_full, 1);
     for (int i = 0; i < 2 * kWG; ++i) mbar_init(&bars[1 + i], 1);
@@ -84,7 +93,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   __syncthreads();
 
   const int n_wg = (int)gridDim.x * kWG, g = (int)blockIdx.x * kWG + wg;
-  const int my_tiles = g < p.num_tiles ? (p.num_tiles - g + n_wg - 1) / n_wg : 0;
+  const int my_tiles = g < num_tiles ? (num_tiles - g + n_wg - 1) / n_wg : 0;
   uint8_t* xs = smem + kOffX + wg * 16384;
   if (t == 0 && my_tiles > 0) {
     mbar_arrive_expect_tx(&x_full[0], 8192);
@@ -108,13 +117,13 @@ __global__ void __launch_bounds__(kThreads, 1)
       gemm_x_w0(acc, smem_u32(xs + s * 8192), sbase, h);
       epi_bias_relu(acc, s_b0, h, a1, lane);
     }
-    if (p.dbg_h1 != nullptr) store_dbg(p.dbg_h1, a1, row, p.M, lane);
+    if (p.dbg_h1 != nullptr) store_dbg(p.dbg_h1, a1, row, M, lane);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       gemm_a_w1(acc, a1, sbase, h);
       epi_bias_relu(acc, s_b1, h, a2, lane);
     }
-    if (p.dbg_h2 != nullptr) store_dbg(p.dbg_h2, a2, row, p.M, lane);
+    if (p.dbg_h2 != nullptr) store_dbg(p.dbg_h2, a2, row, M, lane);
     float z[8];
     wg_zero(z);
     gemm_a_w2(z, a2, sbase);
@@ -122,7 +131,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     for (int i = 0; i < 8; ++i) {  // z[i]: row + 8 ((i >> 1) & 1), column 8 (i >> 2) + 2 (lane % 4) + (i & 1)
       const int64_t rr = row + 8 * ((i >> 1) & 1);
       const int col = 8 * (i >> 2) + 2 * (lane & 3) + (i & 1);
-      if (rr < p.M && col < p.A) p.out[rr * p.A + col] = z[i] + s_b2[col];
+      if (rr < M && col < p.A) p.out[rr * p.A + col] = z[i] + s_b2[col];
     }
   }
 }
@@ -192,7 +201,7 @@ static bool tc_shape_ok(const StxMlp* m) {
 }
 
 int tc_forward_impl(const StxMlp* m, const void* x, int64_t ldx, int64_t M, float* out, float* dbg_h1, float* dbg_h2,
-                    cudaStream_t st) {
+                    cudaStream_t st, const int32_t* dev_rows = nullptr, int max_ctas = 0) {
   STX_REQUIRE(tc_shape_ok(m), STX_E_SHAPE,
               "STX_PREC_BF16 MLP kernels need a relu torso without LayerNorm and sizes [D<=64 (mult of 8), 256, 256, head<=16]; got %d layers [%d,%d,%d,%d]",
               m->n_layers, m->sizes[0], m->sizes[1], m->sizes[2], m->sizes[3]);
@@ -211,18 +220,54 @@ int tc_forward_impl(const StxMlp* m, const void* x, int64_t ldx, int64_t M, floa
   p.b2 = m->params + off_w2 + (int64_t)kH * A;
   p.out = out, p.dbg_h1 = dbg_h1, p.dbg_h2 = dbg_h2, p.M = M, p.A = A;
   p.num_tiles = (int)((M + kTileM - 1) / kTileM);
+  p.dev_rows = dev_rows;
   static bool attr_set = false;
   if (!attr_set) {
     STX_CUDA_OK(cudaFuncSetAttribute(tc_mlp_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
     attr_set = true;
   }
   if (int rc = use_trap_record(st)) return rc;
-  const int cap = (g_forward_ctas > 0 && g_forward_ctas < kNumSMs) ? g_forward_ctas : kNumSMs;
+  int cap = (g_forward_ctas > 0 && g_forward_ctas < kNumSMs) ? g_forward_ctas : kNumSMs;
+  if (max_ctas > 0 && max_ctas < cap) cap = max_ctas;
   const int want = (p.num_tiles + kWG - 1) / kWG;
   const int grid = want < cap ? want : cap;
   tc_mlp_fwd_kernel<<<grid, kThreads, kSmemBytes, st>>>(tmX, tmW0, tmW1, p);
   STX_LAUNCH_OK();
   return STX_OK;
+}
+
+// ---- the rollout's critic values, one forward per observation -----------------------------------------------------
+// value[t] = critic(obs[t]) and bootstrap_value[t] = critic(next_obs[t]) (ff_ppo.py:99, 113-116).  next_obs[t] equals
+// obs[t + 1] wherever the episode did not end at step t, so one forward over obs[0..T] serves both, and only the rows
+// where an episode ended (is_terminal: obs[t + 1] is then the reset observation) are evaluated again on next_obs.  The
+// forward is row-independent (each output row depends on its own input row and the weights only, summed in a fixed
+// order), so every value has the bits of the two full passes.
+
+// Rows with is_terminal set: slot[r] = their position in the compacted list, their next_obs rows copied to xe[slot].
+// The slot order depends on the block schedule; the values do not.
+__global__ void ended_rows_kernel(const uint8_t* __restrict__ is_terminal, const uint4* __restrict__ next_obs, int64_t n, int row_chunks,
+                                  int32_t* __restrict__ slot, uint4* __restrict__ xe, int32_t* __restrict__ count) {
+  const int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const bool ended = r < n && is_terminal[r] != 0;
+  const uint32_t ballot = __ballot_sync(0xffffffffu, ended);
+  if (ballot == 0u) return;
+  const int lane = threadIdx.x & 31;
+  int base = 0;
+  if (lane == 0) base = atomicAdd(count, __popc(ballot));
+  base = __shfl_sync(0xffffffffu, base, 0);
+  if (!ended) return;
+  const int k = base + __popc(ballot & ((1u << lane) - 1u));
+  slot[r] = k;
+  for (int c = 0; c < row_chunks; ++c) xe[(int64_t)k * row_chunks + c] = next_obs[r * row_chunks + c];
+}
+
+__global__ void rollout_values_kernel(const float* __restrict__ vals, const uint8_t* __restrict__ is_terminal, const int32_t* __restrict__ slot,
+                                      const float* __restrict__ ended_vals, int64_t n, int64_t E, float* __restrict__ value,
+                                      float* __restrict__ bootstrap) {
+  const int64_t r = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  value[r] = vals[r];
+  bootstrap[r] = is_terminal[r] != 0 ? ended_vals[slot[r]] : vals[r + E];
 }
 
 }  // namespace tc
@@ -243,4 +288,46 @@ extern "C" void stx_tc_set_forward_ctas(int n) { stx::tc::g_forward_ctas = n; }
 extern "C" int stx_tc_debug_forward(const StxMlp* mlp, const void* x, int64_t ldx, int64_t M, float* out, float* h1, float* h2,
                                     void* stream) {
   return stx::tc::tc_forward_impl(mlp, x, ldx, M, out, h1, h2, (cudaStream_t)stream);
+}
+
+// Workspace of stx_tc_rollout_values: vals ((T+1) E f32), ended values (T E f32), slots (T E i32), the count, then the
+// compacted next_obs rows (T E x D bf16), each part 256-byte aligned.
+static size_t rv_align(size_t b) { return (b + 255) & ~(size_t)255; }
+extern "C" size_t stx_tc_rollout_values_workspace_bytes(int T, int64_t E, int D) {
+  const size_t n = (size_t)T * (size_t)E;
+  return rv_align((n + E) * 4) + rv_align(n * 4) + rv_align(n * 4) + 256 + rv_align(n * (size_t)D * 2);
+}
+
+extern "C" int stx_tc_rollout_values(const StxMlp* critic, const void* obs, const void* next_obs, const uint8_t* is_terminal, int T,
+                                     int64_t E, float* value, float* bootstrap_value, void* ws, size_t ws_bytes, void* stream) {
+  using namespace stx;
+  STX_REQUIRE(critic && obs && next_obs && is_terminal && value && bootstrap_value && ws, STX_E_ARG, "stx_tc_rollout_values: null pointer");
+  STX_REQUIRE(T > 0 && E > 0 && (int64_t)(T + 1) * E < (1ll << 31), STX_E_SHAPE, "stx_tc_rollout_values: T=%d E=%lld", T, (long long)E);
+  STX_REQUIRE(critic->sizes[critic->n_layers] == 1, STX_E_SHAPE, "stx_tc_rollout_values: the critic must have one output");
+  const int D = critic->sizes[0];
+  STX_REQUIRE(D % 8 == 0, STX_E_SHAPE, "stx_tc_rollout_values: D=%d must be a multiple of 8", D);
+  STX_REQUIRE(ws_bytes >= stx_tc_rollout_values_workspace_bytes(T, E, D), STX_E_ARG, "stx_tc_rollout_values: workspace too small");
+  const cudaStream_t st = (cudaStream_t)stream;
+  const int64_t n = (int64_t)T * E;
+  uint8_t* w = reinterpret_cast<uint8_t*>(ws);
+  float* vals = reinterpret_cast<float*>(w);
+  w += rv_align((size_t)(n + E) * 4);
+  float* ended_vals = reinterpret_cast<float*>(w);
+  w += rv_align((size_t)n * 4);
+  int32_t* slot = reinterpret_cast<int32_t*>(w);
+  w += rv_align((size_t)n * 4);
+  int32_t* count = reinterpret_cast<int32_t*>(w);
+  w += 256;
+  void* xe = w;
+  STX_CUDA_OK(cudaMemsetAsync(count, 0, sizeof(int32_t), st));
+  const unsigned grid = (unsigned)((n + 255) / 256);
+  tc::ended_rows_kernel<<<grid, 256, 0, st>>>(is_terminal, reinterpret_cast<const uint4*>(next_obs), n, D / 8, slot,
+                                              reinterpret_cast<uint4*>(xe), count);
+  STX_LAUNCH_OK();
+  if (int rc = tc::tc_forward_impl(critic, obs, D, n + E, vals, nullptr, nullptr, st)) return rc;
+  // ~0.7 % of the rows at the benchmark's termination rates: a few dozen tiles, one per warpgroup
+  if (int rc = tc::tc_forward_impl(critic, xe, D, n, ended_vals, nullptr, nullptr, st, count, 48)) return rc;
+  tc::rollout_values_kernel<<<grid, 256, 0, st>>>(vals, is_terminal, slot, ended_vals, n, E, value, bootstrap_value);
+  STX_LAUNCH_OK();
+  return STX_OK;
 }

@@ -84,18 +84,20 @@ class SyntheticBoxEnv(Environment):
     # -- whole-rollout face (bf16 tensor-core path) ---------------------------------------------------
     fused_rollout_supported = True
 
-    def fused_rollout(self, state, actor_spec, actor_params, actor_params_bf16, shard, T: int, cat_seed: int, cat_counter,
-                      t0: int = 0, steps: int = None) -> None:
-        """Steps [t0, t0 + steps) of policy + env in one persistent kernel (stx_tc_rollout_synth); default: all T.  Valid
-        because this env's dynamics ignore the action, so the kernel generates step t+1's observation while the tensor
-        cores evaluate step t; the trajectory is bit-identical to T calls of step_into (and to any chunking: the RNG
-        counters are (env, absolute step))."""
-        n = T - t0 if steps is None else int(steps)
-        a, b = t0, t0 + n
-        ops.tc_rollout_synth(actor_spec, actor_params, actor_params_bf16, shard.obs[a:b + 1], shard.next_obs[a:b], shard.action[a:b],
-                             shard.log_prob[a:b], shard.reward[a:b], shard.done[a:b], shard.truncated[a:b], shard.episode_return[a:b],
-                             shard.episode_length[a:b], shard.is_terminal_step[a:b], state["run_return"], state["run_length"],
-                             state["seed"], a, state["counter"], self.p_term, self.p_trunc, cat_seed, a, cat_counter)
+    def fused_trajectory(self, state, shard, T: int) -> None:
+        """Steps [0, T) of every env of the shard in one launch over the whole GPU (stx_synth_env_trajectory).  Valid because
+        this env's dynamics ignore the action: obs[1..T], next_obs and the per-step scalars are bit-identical to T calls of
+        step_into (the RNG counters are (env, absolute step)), and the policy then only reads the observations."""
+        E = state["run_return"].shape[0]
+        ops.synth_env_trajectory(E, self.obs_dim, T, state["seed"], 0, self.p_term, self.p_trunc, shard.obs[:T + 1], shard.next_obs[:T],
+                                 shard.reward[:T], shard.terminated[:T], shard.truncated[:T], shard.episode_return[:T], shard.episode_length[:T],
+                                 shard.is_terminal_step[:T], state["run_return"], state["run_length"], dev_counter=state["counter"])
+
+    def fused_rollout(self, state, actor_spec, actor_params, actor_params_bf16, shard, T: int, cat_seed: int, cat_counter) -> None:
+        """All T steps of env + policy: fused_trajectory, then the policy over its observations (stx_tc_rollout_policy)."""
+        self.fused_trajectory(state, shard, T)
+        ops.tc_rollout_policy(actor_spec, actor_params, actor_params_bf16, shard.obs[:T], shard.action[:T], shard.log_prob[:T], cat_seed, 0,
+                              cat_counter)
 
     def advance(self, state, steps: int) -> None:
         """Move the device-resident step counter (end of a rollout; graph-capturable)."""

@@ -606,10 +606,59 @@ def synth_env_step(E, D, seed, step, p_term, p_trunc, action, obs_out, next_obs,
     )
 
 
+def synth_env_trajectory(E, D, T, seed, step, p_term, p_trunc, obs, next_obs, reward, done, truncated, ep_return, ep_length,
+                         is_terminal, run_return, run_length, dev_counter=None) -> None:
+    """Steps [0, T) of the synthetic env in one launch (stx_synth_env_trajectory): obs (T+1, E, D) bf16 with row 0 the input,
+    next_obs (T, E, D) bf16, the rest (T, E); the same values as T calls of synth_env_step."""
+    _need_cuda(obs, next_obs, reward, done, truncated, ep_return, ep_length, is_terminal, run_return, run_length, dev_counter)
+    if obs.dtype != torch.bfloat16 or next_obs.dtype != torch.bfloat16:
+        raise StxError("synth_env_trajectory: observation buffers must be bfloat16")
+    _lib.check(
+        _lib.load().stx_synth_env_trajectory(int(E), int(D), int(T), int(seed) & (2**64 - 1), int(step), _p(dev_counter), float(p_term),
+                                             float(p_trunc), _p(obs), _p(next_obs), _p(reward), _p(done), _p(truncated), _p(ep_return),
+                                             _p(ep_length), _p(is_terminal), _p(run_return), _p(run_length), _stream()),
+        "stx_synth_env_trajectory",
+    )
+
+
+def tc_rollout_policy(spec: MlpSpec, params, params_bf16, obs, action, log_prob, cat_seed, cat_offset, cat_counter,
+                      max_ctas: int = 0) -> None:
+    """The policy of a rollout over existing observations obs (T, E, D) bf16 (stx_tc_rollout_policy): Gumbel-max action and
+    log-prob of every (step, env), written to action / log_prob (T, E); one persistent CTA per SM, or max_ctas."""
+    _need_cuda(params, params_bf16, obs, action, log_prob, cat_counter)
+    if obs.dtype != torch.bfloat16 or not obs.is_contiguous():
+        raise StxError("tc_rollout_policy: obs must be contiguous bfloat16")
+    T, E = int(action.shape[0]), int(action.shape[1])
+    m = spec.c_struct(params, params_bf16)
+    _lib.check(
+        _lib.load().stx_tc_rollout_policy(C.byref(m), _p(obs), _p(action), _p(log_prob), T, E, int(cat_seed) & (2**64 - 1), int(cat_offset),
+                                          _p(cat_counter), int(max_ctas), _stream()),
+        "stx_tc_rollout_policy",
+    )
+
+
+def tc_rollout_values(spec: MlpSpec, params, params_bf16, obs, next_obs, is_terminal, value, bootstrap_value,
+                      ws_key: str = "rollout-values") -> None:
+    """value = critic(obs[:T]) and bootstrap_value = critic(next_obs) over (T, E) rows (stx_tc_rollout_values): one forward over
+    obs (T+1, E, D) plus one over the next_obs rows where is_terminal is set; bit-identical to two full forward passes."""
+    dev = _need_cuda(params, params_bf16, obs, next_obs, is_terminal, value, bootstrap_value)
+    T, E = int(value.shape[0]), int(value.shape[1])
+    D = int(spec.sizes[0])
+    if tuple(obs.shape) != (T + 1, E, D) or obs.dtype != torch.bfloat16 or next_obs.dtype != torch.bfloat16:
+        raise StxError(f"tc_rollout_values: obs must be bfloat16 ({T + 1}, {E}, {D}), got {obs.dtype} {tuple(obs.shape)}")
+    lib = _lib.load()
+    ws = _zeros_scratch((ws_key,), lib.stx_tc_rollout_values_workspace_bytes(T, E, D), dev)
+    m = spec.c_struct(params, params_bf16)
+    _lib.check(lib.stx_tc_rollout_values(C.byref(m), _p(obs), _p(next_obs), _p(is_terminal), T, E, _p(value), _p(bootstrap_value),
+                                         _p(ws), ws.numel(), _stream()),
+               "stx_tc_rollout_values")
+
+
 def tc_rollout_synth(spec: MlpSpec, params, params_bf16, obs, next_obs, action, log_prob, reward, done, truncated, ep_return,
                      ep_length, is_terminal, run_return, run_length, env_seed, env_step, env_counter, p_term, p_trunc, cat_seed,
                      cat_offset, cat_counter) -> None:
-    """Fused T-step rollout of the synthetic env (stx_tc_rollout_synth); buffers are the time-major trajectory."""
+    """Fused T-step rollout of the synthetic env (stx_tc_rollout_synth: the trajectory, then the policy over it); buffers
+    are the time-major trajectory."""
     _need_cuda(params, params_bf16, obs, next_obs, action, log_prob, reward, done, truncated, ep_return, ep_length, is_terminal,
                run_return, run_length, env_counter, cat_counter)
     if obs.dtype != torch.bfloat16 or next_obs.dtype != torch.bfloat16:

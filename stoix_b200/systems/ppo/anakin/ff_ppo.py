@@ -52,6 +52,8 @@ from stoix_b200.systems.ppo.ppo_types import PPOTransition
 from stoix_b200.utils.checkpointing import warm_start
 from stoix_b200.utils.training import make_learning_rate
 
+# The bf16 fused rollout's SM split: persistent policy CTAs; the critic's forward runs beside them on the other SMs.
+POLICY_CTAS = 82
 _METRIC_NAMES = ("actor_loss", "entropy", "value_loss", "advantages", "pred_value", "target_value")
 # The actor loss of the update: ppo_clip_loss (ff_ppo*), ppo_penalty_loss (ff_ppo_penalty*) or dpo_loss (ff_dpo_continuous).  The
 # variants report the reference's loss_info keys (ff_ppo_penalty.py:172-176,195-197; ff_dpo_continuous.py:166-169,187-189) as
@@ -175,7 +177,7 @@ def get_learner_fn(
             perm_ctr=torch.zeros(1, dtype=torch.int64, device=dev),   # shuffle stream index
             ent_ctr=torch.zeros(1, dtype=torch.int64, device=dev),    # tanh-Normal entropy noise: minibatch call index
             side_stream=torch.cuda.Stream(device=dev),                # the shuffles run here, underneath the rollout
-            critic_stream=torch.cuda.Stream(device=dev),              # chunked critic evaluation underneath the fused rollout
+            critic_stream=torch.cuda.Stream(device=dev),              # critic evaluation beside the fused rollout's policy
             rs=rs, rs_sums=torch.zeros(2 * D + 1, dtype=torch.float64, device=dev) if rs is not None else None,
             graph=None, eager_done=False,
         )
@@ -210,15 +212,8 @@ def get_learner_fn(
         fused = (precision == ops.STX_PREC_BF16 and bool(arch.get("fused_rollout", True)) and E % 128 == 0
                  and getattr(env, "fused_rollout_supported", False) and b["rs"] is None)
         # The two critic evaluations of _env_step (value = critic(obs_t), bootstrap_value = critic(next_obs_t), ff_ppo.py:99,
-        # 113-116) depend only on the observations, so they are batched over (steps x envs) rows.  With the fused rollout
-        # (E/64 of the 132 SMs busy: one CTA per 64 envs) the scan is cut into chunks and the critic of chunk c runs on a second stream on the
-        # idle SMs while the rollout kernel produces chunk c+1; only the last chunk's critic is left after the scan.
-        chunks = max(int(arch.get("rollout_chunks", 8)), 1) if fused else 1
-        while T % chunks != 0:  # largest divisor of T not above the request
-            chunks -= 1
-        Tc = T // chunks
+        # 113-116) depend only on the observations, so they are batched over (steps x envs) rows.
         main = torch.cuda.current_stream()
-        side = b["critic_stream"] if chunks > 1 else None
 
         def critic_rows(sh: _Shard, t_lo: int, t_hi: int) -> None:
             n = (t_hi - t_lo) * E
@@ -229,22 +224,23 @@ def get_learner_fn(
 
         for u in range(U):
             sh: _Shard = b["shards"][u]
-            if fused:  # persistent launches (envs whose dynamics ignore the action), `chunks` of Tc steps each
-                for c in range(chunks):
-                    env.fused_rollout(state.env_state[u], sa, a_tree.flat, a_tree.flat_bf16, sh, T, state.key[0] + u, b["roll_ctr"],
-                                      t0=c * Tc, steps=Tc)
-                    if side is not None:
-                        side.wait_stream(main)
-                        with torch.cuda.stream(side):
-                            # leave the rollout's SMs alone: a persistent forward CTA that has to wait for one of them
-                            # would hold its share of the tiles back until the rollout chunk ends
-                            ops.set_forward_cta_budget(ops.NUM_SMS - E // 64 if c + 1 < chunks else 0)
-                            critic_rows(sh, c * Tc, (c + 1) * Tc)
-                            ops.set_forward_cta_budget(0)
-                if side is not None:
-                    main.wait_stream(side)
-                else:
-                    critic_rows(sh, 0, T)
+            if fused:
+                # Envs whose dynamics ignore the action: the whole trajectory first, in one launch over the whole GPU.  The
+                # policy of step t then needs only obs[t], so the actor and the critic (once per observation) are both
+                # batched over all T x E rows: persistent launches over the SMs, POLICY_CTAS of them for the actor and the
+                # rest for the critic on a second stream beside it (both are bound by their tensor-core chains, so the split
+                # only balances their lengths).  arch.rollout_chunks is accepted and no longer read.
+                env.fused_trajectory(state.env_state[u], sh, T)
+                side = b["critic_stream"]
+                side.wait_stream(main)
+                with torch.cuda.stream(side):
+                    ops.set_forward_cta_budget(ops.NUM_SMS - POLICY_CTAS)
+                    ops.tc_rollout_values(sc, c_tree.flat, c_tree.flat_bf16, sh.obs, sh.next_obs, sh.is_terminal_step, sh.value,
+                                          sh.bootstrap_value, ws_key="learner-rollout-values")
+                    ops.set_forward_cta_budget(0)
+                ops.tc_rollout_policy(sa, a_tree.flat, a_tree.flat_bf16, sh.obs[:T], sh.action, sh.log_prob, state.key[0] + u, 0,
+                                      b["roll_ctr"], max_ctas=POLICY_CTAS)
+                main.wait_stream(side)
             else:
                 for t in range(T):
                     _env_step(state, u, t, state.key)
