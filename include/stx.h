@@ -793,7 +793,11 @@ int stx_dueling_backward(const float* d_q_logits, int64_t M, int A, int N, float
  *           at rows w - n + 1 .. w + T - 1 (at most L per env) are re-evaluated: valid ones get *max_priority, the others 0.
  *   sample: stratified: sample r takes v = ((r + u_r) total) / M (u_r = u_in[r], or u01 of word r & 3 of Philox (seed; r / 4,
  *           call, call >> 32, 0x5052494F), call = offset + *dev_counter) and descends from the root: at each node the children
- *           in order, entering the first with v < s (s its sum), else v -= s; if none, the last child with s > 0.  It writes
+ *           in order, entering the first with v < s (s its sum), else v -= s; if none (fp32 rounding left v at or past the node's
+ *           sum), the last child with s > 0, and the last positive child at every level below, so the draw ends on the last
+ *           positive item of that subtree.  The item is then within 64 h 2^-24 total of the fp64 inverse CDF (h the tree's
+ *           levels; tests/prio_reference.py derives the bound).  With no valid item (total 0) every draw is item 0 with
+ *           prob_out 0 and weight_out 1.  It writes
  *           the item's step-0 obs and action, step n-1 next_obs, the n-step reward G_0 (G = r_{n-1}; G_k = r_k + d_k G_{k+1},
  *           d_k = (1 - done_k) gamma, batch_discounted_returns with v = 0), done = any(done_0 .. done_{n-1}), idx_out (the item),
  *           prob_out = leaf / total and weight_out w = (1/p)^beta / max_batch (1/p)^beta, beta = linear schedule from beta0 to 1
@@ -1019,7 +1023,8 @@ int stx_mpo_q_grad(const float* q, const float* targets, int S, int B, float* dq
  *   add:    T rows at w .. w + T - 1 (mod L; only the newest L if T > L); then every item whose start row lies in w - S + 1 .. w + T - 1
  *           (mod L, at most L rows) is re-evaluated: valid ones get *max_priority, the others 0; every parent is rebuilt.
  *   sample: stratified as Rainbow's sampler, B strata: sequence b draws v = ((b + u_b) total) / B (u_b = u_in[b], or u01 of word b & 3
- *           of Philox(seed; b / 4, call, call >> 32, 0x5052494F), call = offset + *dev_counter) and descends the tree.  Outputs are
+ *           of Philox(seed; b / 4, call, call >> 32, 0x5052494F), call = offset + *dev_counter) and descends the tree by Rainbow's
+ *           rule (a level where no child takes v takes its last positive child, and so does every level below).  Outputs are
  *           time-major (S, B): obs (S, B, obs_dim), action, reward, done, reset; carry0 (B, carry_dim) = the stored carry of the item,
  *           idx_out (B) the item, prob_out (B) = leaf / total.  With no valid item (total 0: at the reference default, L = 97, S = 80,
  *           p = 40, the head often sits where no start row has S rows behind it) every draw is item 0 with prob 0; the loss's

@@ -63,7 +63,9 @@ __device__ __forceinline__ float stratum_uniform(int64_t r, uint64_t seed, uint6
 }
 
 // Stratified descent of one warp (every lane gets the leaf): v = ((r + u) total) / M from the root; at each node the children in
-// order, entering the first with v < s, else v -= s; if none, the last child with s > 0.
+// order, entering the first with v < s, else v -= s.  If none takes v (fp32 rounding left v at or past the node's sum), the last child
+// with s > 0, and at every level below the last positive child too (v = +inf): the draw ends on the subtree's last positive leaf,
+// next to v, not on its first.
 __device__ __forceinline__ int64_t tree_descend(const float* __restrict__ tree, int64_t items, int64_t r, float u, int64_t M) {
   const int lane = threadIdx.x & 31;
   const int n = tree_height(items);
@@ -82,6 +84,7 @@ __device__ __forceinline__ int64_t tree_descend(const float* __restrict__ tree, 
         else v = __fsub_rn(v, s);
       }
     }
+    if (pick < 0) v = INFINITY;
     node = c0 + (pick < 0 ? last_pos : pick);
   }
   return node;

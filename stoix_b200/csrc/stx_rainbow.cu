@@ -198,11 +198,15 @@ __global__ void __launch_bounds__(256) prio_sample_kernel(StxReplayPrioritised r
       o.done[r] = any ? 1 : 0;
       o.action[r] = rb.action[s0];
       o.idx[r] = (int32_t)i;
-      o.prob[r] = __fdiv_rn(rb.tree[i], total);
+      o.prob[r] = total > 0.f ? __fdiv_rn(rb.tree[i], total) : 0.f;   // no valid item: every draw is item 0 with p 0
     }
   }
   // the importance weights need the whole batch: the last block to finish computes them
   if (!last_block_ticket(ticket, gridDim.x)) return;
+  if (!(rb.tree[prio::root_offset(items)] > 0.f)) {   // p 0 everywhere: weights of 1, not (1/0)^beta / max = inf / inf
+    for (int64_t m = threadIdx.x; m < M; m += blockDim.x) o.weight[m] = 1.f;
+    return;
+  }
   float beta = beta0;
   if (beta_steps > 0.f) {
     const float c = fminf(fmaxf((float)(count ? *count : 0), 0.f), beta_steps);

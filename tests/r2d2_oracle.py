@@ -155,7 +155,8 @@ class Ring:
         return levels
 
     def sample_items(self, u: np.ndarray) -> np.ndarray:
-        """Stratified descent with the uniforms u (B) in fp32, as the device: v = ((b + u_b) total) / B."""
+        """Stratified descent with the uniforms u (B) in fp32, as the device: v = ((b + u_b) total) / B.  A level where no child takes
+        v (fp32 rounding left v at or past the node's sum) takes its last positive child, and so does every level below it (v = +inf)."""
         levels = self.tree()
         B = len(u)
         total = levels[-1][0]
@@ -174,6 +175,8 @@ class Ring:
                             pick = c
                         else:
                             v = np.float32(v - s)
+                if pick < 0:
+                    v = np.float32(np.inf)
                 node = node * FANOUT + (last_pos if pick < 0 else pick)
             out[b] = node
         return out

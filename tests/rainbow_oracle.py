@@ -189,10 +189,15 @@ class PrioRing:
                     self.prio[i] = self.maxp
 
     def sample(self, u: np.ndarray) -> np.ndarray:
+        """The first item whose cumulative priority exceeds v = (r + u_r) total / M; at or past the total, the last positive item
+        (with no positive item, item 0)."""
         M = len(u)
-        total = self.prio.sum()
-        v = (np.arange(M) + np.asarray(u, np.float64)) * total / M
-        return np.searchsorted(np.cumsum(self.prio), v, side="right")
+        cum = np.cumsum(self.prio)
+        pos = np.flatnonzero(self.prio > 0)
+        if len(pos) == 0:
+            return np.zeros(M, np.int64)
+        v = (np.arange(M) + np.asarray(u, np.float64)) * cum[-1] / M
+        return np.minimum(np.searchsorted(cum, v, side="right"), pos[-1])
 
     def transition(self, i: int, gamma: float):
         e, p = divmod(int(i), self.L)
