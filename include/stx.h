@@ -225,31 +225,6 @@ int stx_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const Stx
                             float* grad_arena, float* metrics, int precision, void* workspace,
                             size_t workspace_bytes, void* stream);
 
-/* One whole optimiser step on a minibatch = stx_ppo_minibatch_grads + stx_clip_adam_step (the body of
- * _update_minibatch, ff_ppo.py:184-284) with the gradient reduction and the optimiser fused into one launch:
- * the thread that reduces a gradient entry keeps it in a register, the blocks meet once at a grid barrier
- * for the two global norms, and the same thread applies clip + Adam to that entry.  STX_PREC_BF16 only,
- * single shard / single device (the gradients are overwritten, hyper->overwrite_grads is ignored);
- * opt->nseg must be 2 with segment 0 = actor arena and segment 1 = critic arena.  Same results as the
- * two separate calls (same reduction orders). */
-typedef struct StxFusedAdam {
-  float* param_arena;
-  float* mu;
-  float* nu;
-  int32_t* counts;          /* int32[2*nseg] device */
-  const StxAdamSeg* segs;   /* DEVICE pointer */
-  int32_t nseg;
-  int32_t reserved;
-  StxAdamHyper hyper;       /* prenorm is ignored */
-  void* params_bf16;        /* nullable */
-  float* gnorm_out;         /* nullable, float[nseg] */
-  void* scratch;            /* >= stx_adam_scratch_bytes(), zeroed once */
-} StxFusedAdam;
-int stx_ppo_minibatch_update(const StxMlp* actor, const StxMlp* critic, const StxPpoBatch* batch,
-                             int64_t mb_off, int64_t mb, const StxPpoHyper* hyper, float grad_weight,
-                             float* grad_arena, float* metrics, void* workspace, size_t workspace_bytes,
-                             const StxFusedAdam* opt, void* stream);
-
 /* Forward values of the two reference loss utilities (stoix/utils/loss.py:17-32 ppo_clip_loss,
  * :68-78 clipped_value_loss) over n elements; out[0] = mean.  scratch >= stx_loss_scratch_bytes(),
  * zeroed once.  (The training path uses the fused stx_ppo_minibatch_grads instead.) */
@@ -288,18 +263,6 @@ int stx_allreduce_clip_adam_step(float* param_arena, const float* const* peer_gr
                                  int world, int rank, int pad_slot_offset, float* gsum, float* mu, float* nu,
                                  int32_t* counts, const StxAdamSeg* segs, int nseg, const StxAdamHyper* hyper,
                                  void* params_bf16, float* gnorm_out, void* scratch, void* stream);
-/* Two-shot form (the default of the learner): rank r sums slice r of the W gradient arenas (peer LOADS, rank order) and stores
- * the result into every rank's reduced-gradient buffer (peer STORES), so (W-1)/W of the arena crosses NVLink in each direction
- * instead of W-1 arenas inbound; the per-rank sum-of-squares partials of the clipping norm travel with the slices and the second
- * hand-shake replaces the grid barrier of the norm.  Every element is reduced once, by one rank => identical on all ranks.
- *   peer_gsum[r]   HOST array of `world` DEVICE pointers: rank r's reduced-gradient buffer, peer-mapped, arena_len + 128 floats
- *                  (tail: double[world][8] norm partials).  arena_len % 4 == 0; the padding between segments must hold zeros.
- *   signal pads    slots [pad_slot_offset, +8) "gradients ready", [pad_slot_offset + 8, +16) "slice stored".
- *   grid           0 = one block per SM; tests that run several virtual ranks on one device pass a small co-resident grid. */
-int stx_allreduce2_clip_adam_step(float* param_arena, const float* const* peer_grads, float* const* peer_gsum, int64_t arena_len,
-                                  void* const* peer_signal_pads, int world, int rank, int pad_slot_offset, float* mu, float* nu,
-                                  int32_t* counts, const StxAdamSeg* segs, int nseg, const StxAdamHyper* hyper, void* params_bf16,
-                                  float* gnorm_out, void* scratch, int grid, void* stream);
 
 /* ------------------------------------------------------------------ shuffle -------------------
  * perm[i] = keyed bijection of [0, n) (cycle-walking Feistel over Philox rounds) replacing

@@ -65,22 +65,6 @@ class StxAdamHyper(C.Structure):
     ]
 
 
-class StxFusedAdam(C.Structure):
-    _fields_ = [
-        ("param_arena", C.c_void_p),
-        ("mu", C.c_void_p),
-        ("nu", C.c_void_p),
-        ("counts", C.c_void_p),
-        ("segs", C.c_void_p),
-        ("nseg", C.c_int32),
-        ("reserved", C.c_int32),
-        ("hyper", StxAdamHyper),
-        ("params_bf16", C.c_void_p),
-        ("gnorm_out", C.c_void_p),
-        ("scratch", C.c_void_p),
-    ]
-
-
 class StxRadamHyper(C.Structure):
     _fields_ = [
         ("adam", StxAdamHyper),
@@ -377,14 +361,11 @@ _SIGNATURES = {
     "stx_ppo_arena_offsets": (None, [C.POINTER(StxMlp), C.POINTER(StxMlp), C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "stx_ppo_workspace_bytes": (C.c_size_t, [C.POINTER(StxMlp), C.POINTER(StxMlp), C.c_int64, C.c_int]),
     "stx_ppo_minibatch_grads": (C.c_int, [C.POINTER(StxMlp), C.POINTER(StxMlp), C.POINTER(StxPpoBatch), C.c_int64, C.c_int64, C.POINTER(StxPpoHyper), C.c_float, _P, _P, C.c_int, _P, C.c_size_t, _P]),
-    "stx_ppo_minibatch_update": (C.c_int, [C.POINTER(StxMlp), C.POINTER(StxMlp), C.POINTER(StxPpoBatch), C.c_int64, C.c_int64, C.POINTER(StxPpoHyper), C.c_float, _P, _P, _P, C.c_size_t, C.POINTER(StxFusedAdam), _P]),
     "stx_loss_scratch_bytes": (C.c_size_t, []),
     "stx_ppo_clip_loss": (C.c_int, [_P, _P, _P, C.c_int64, C.c_float, _P, _P, _P]),
     "stx_clipped_value_loss": (C.c_int, [_P, _P, _P, C.c_int64, C.c_float, _P, _P, _P]),
     "stx_adam_scratch_bytes": (C.c_size_t, [C.c_int]),
     "stx_clip_adam_step": (C.c_int, [_P, _P, _P, _P, _P, _P, C.c_int, C.POINTER(StxAdamHyper), _P, _P, _P, _P]),
-    "stx_allreduce2_clip_adam_step": (C.c_int, [_P, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int64, C.POINTER(C.c_void_p), C.c_int, C.c_int,
-                                                C.c_int, _P, _P, _P, _P, C.c_int, _P, _P, _P, _P, C.c_int, _P]),
     "stx_allreduce_clip_adam_step": (C.c_int, [_P, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P,
                                                 C.c_int, C.POINTER(StxAdamHyper), _P, _P, _P, _P]),
     "stx_make_permutation": (C.c_int, [_P, C.c_int64, C.c_uint64, C.c_uint64, _P, _P]),

@@ -21,13 +21,6 @@ namespace stx {
 namespace {
 
 constexpr int kAdamThreads = 256;
-constexpr int kAdamMaxSegs = 8;
-
-struct AdamScratch {
-  unsigned long long arrive;  // monotonically increasing barrier ticket
-  unsigned long long n_partials;  // PRENORM: block partials per segment, published by the gradient producer
-  // followed by double partials[kAdamMaxSegs][grid]  (PRENORM: [nseg][n_partials])
-};
 
 // ---- C1 fused into K4: one-shot all-reduce over NVLink peer memory ------------------------------------
 // Every rank's gradient arena lives in symmetric (peer-mapped) memory.  Rank r announces "my gradients of
@@ -43,12 +36,6 @@ struct PeerSync {
   unsigned int* local_gen;      // device counter: number of completed calls
   float* gsum;                  // local arena receiving the summed gradient
   int world, rank;
-  // two-shot form (PEER == 2): reduce-scatter by peer loads, all-gather by peer stores
-  float* peer_gsum[8];          // every rank's reduced-gradient buffer (peer-mapped); tail: double norm[world][kAdamMaxSegs]
-  unsigned int* peer_pads2[8];  // second signal row: "my slice (and its sum of squares) is in your buffer"
-  unsigned int* my_pad2;
-  unsigned long long* done;     // local arrival ticket of the blocks of this rank (monotonic)
-  int64_t total4;               // arena length in float4
 };
 
 __device__ __forceinline__ void st_release_sys(unsigned int* p, unsigned int v) {
@@ -74,7 +61,7 @@ __device__ __forceinline__ void grid_barrier(unsigned long long* arrive) {
   __syncthreads();
 }
 
-// The update rule of phase 2, a compile-time choice: Adam (stx_clip_adam_step and the fused all-reduce forms), optax.scale_by_radam
+// The update rule of phase 2, a compile-time choice: Adam (stx_clip_adam_step and the fused all-reduce), optax.scale_by_radam
 // (stx_clip_radam_step) or optax.scale_by_rms at optax.rmsprop's defaults (stx_clip_rmsprop_step, which reads and writes nu only).  The rectifier of RAdam depends on the step count only; it is derived once per segment in double
 // precision next to the bias corrections: rho_t = rho_inf - 2 t b2^t / (1 - b2^t) subtracts two numbers of nearly the same size
 // (rho_inf = 1999 at b2 = 0.999), which in fp32 puts a relative error of 1.8e-3 on r_t at t = 6 (DESIGN.md section 2, tolerance scheme).
@@ -83,9 +70,7 @@ struct RadamArgs {
 };
 enum UpdateRule : int { kRuleAdam = 0, kRuleRadam = 1, kRuleRmsprop = 2 };
 
-// PEER: 0 = local gradients; 1 = one-shot all-reduce (every rank loads all W arenas); 2 = two-shot (rank r reduces slice r from
-// the W arenas and stores the result into every rank's buffer: (W-1)/W of the arena in and out instead of W-1 arenas in; the
-// second cross-rank hand-shake doubles as the grid barrier of the norm, whose per-rank partial sums travel with the slices).
+// PEER: 0 = local gradients; 1 = one-shot all-reduce (every rank loads all W arenas).
 template <bool PRENORM, int PEER, int RULE = kRuleAdam>
 __global__ void __launch_bounds__(kAdamThreads)
     clip_adam_kernel(float* __restrict__ P, const float* G, float* __restrict__ MU,
@@ -93,8 +78,7 @@ __global__ void __launch_bounds__(kAdamThreads)
                      const StxAdamSeg* __restrict__ segs, int nseg, StxAdamHyper h,
                      __nv_bfloat16* __restrict__ P16, float* __restrict__ gnorm_out,
                      AdamScratch* scratch, const PeerSync ps, const RadamArgs rx) {
-  double* partials = reinterpret_cast<double*>(scratch + 1);
-  unsigned long long* finish = reinterpret_cast<unsigned long long*>(partials + kAdamMaxSegs * kNumSMs) + 2;  // after the peer words
+  double* partials = scratch->partials;
   __shared__ double sred[32];
   __shared__ StxAdamSeg s_seg[kAdamMaxSegs];
   __shared__ float s_gs[kAdamMaxSegs], s_bc1[kAdamMaxSegs], s_bc2[kAdamMaxSegs], s_lr[kAdamMaxSegs], s_gn[kAdamMaxSegs];
@@ -106,89 +90,6 @@ __global__ void __launch_bounds__(kAdamThreads)
   if ((int)threadIdx.x < nseg) s_seg[threadIdx.x] = segs[threadIdx.x];
   __syncthreads();
 
-  __shared__ int s_last;
-  if (PEER == 2) {
-    // ---- phase 0: cross-rank hand-shake "gradients of call #gen complete" ----
-    const unsigned int gen = *reinterpret_cast<volatile unsigned int*>(ps.local_gen) + 1u;
-    if ((int)threadIdx.x < ps.world) {
-      const int peer = threadIdx.x;
-      if (blockIdx.x == 0) {
-        __threadfence_system();
-        st_release_sys(ps.peer_pads[peer] + ps.rank, gen);
-      }
-      unsigned int spins = 0;
-      unsigned long long t0 = 0ull;
-      while (ld_acquire_sys(ps.my_pad + peer) < gen) spin_guard(spins, t0, "peer gradient hand-shake");
-    }
-    __syncthreads();
-    // ---- phase A: reduce my slice of the arena over the W ranks (rank order), push it to every rank ----
-    const int W = ps.world;
-    const int64_t chunk = (ps.total4 + W - 1) / W;
-    const int64_t i_begin = (int64_t)ps.rank * chunk;
-    const int64_t i_end = (i_begin + chunk < ps.total4) ? i_begin + chunk : ps.total4;
-    float ssl[kAdamMaxSegs];
-#pragma unroll
-    for (int s = 0; s < kAdamMaxSegs; ++s) ssl[s] = 0.f;
-    for (int64_t i = i_begin + gtid; i < i_end; i += gthreads) {
-      float4 v[8];
-#pragma unroll
-      for (int r = 0; r < 8; ++r)   // all W loads in flight before the first add (one NVLink round trip, not W)
-        if (r < W) v[r] = __ldcg(reinterpret_cast<const float4*>(ps.peer_grads[r]) + i);
-      float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-      for (int r = 0; r < 8; ++r)
-        if (r < W) acc.x += v[r].x, acc.y += v[r].y, acc.z += v[r].z, acc.w += v[r].w;
-#pragma unroll
-      for (int q = 0; q < 8; ++q)
-        if (q < W) __stcg(reinterpret_cast<float4*>(ps.peer_gsum[q]) + i, acc);
-      // sum of squares of the scaled sum, per optimiser segment (padding between segments holds zeros)
-      const float gx = acc.x * h.grad_scale, gy = acc.y * h.grad_scale, gz = acc.z * h.grad_scale, gw = acc.w * h.grad_scale;
-      const float q2 = gx * gx + gy * gy + gz * gz + gw * gw;
-      const int64_t e0 = 4 * i;
-#pragma unroll
-      for (int s = 0; s < kAdamMaxSegs; ++s)
-        if (s < nseg && e0 >= s_seg[s].offset && e0 < s_seg[s].offset + s_seg[s].count) ssl[s] += q2;
-    }
-#pragma unroll
-    for (int s = 0; s < kAdamMaxSegs; ++s) {
-      if (s < nseg) {
-        const double bs = block_sum<double>((double)ssl[s], sred);
-        if (threadIdx.x == 0) partials[(int64_t)s * gridDim.x + blockIdx.x] = bs;
-      }
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      __threadfence_system();  // this block's slice stores and partials before its arrival
-      const unsigned long long t = atomicAdd(ps.done, 1ull);
-      s_last = (t % gridDim.x == gridDim.x - 1) ? 1 : 0;
-      __threadfence();
-    }
-    __syncthreads();
-    if (s_last) {
-      // the last block of this rank: rank partial per segment (fixed order), to every rank's norm table, then the signal
-      const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-      if (warp < nseg) {
-        double part = 0.0;
-        for (unsigned int b = lane; b < gridDim.x; b += 32) part += __ldcg(partials + (int64_t)warp * gridDim.x + b);
-        part = warp_sum(part);
-        if (lane < W)
-          reinterpret_cast<double*>(ps.peer_gsum[lane] + 4 * ps.total4)[ps.rank * kAdamMaxSegs + warp] = part;
-      }
-      __syncthreads();
-      if ((int)threadIdx.x < W) {
-        __threadfence_system();
-        st_release_sys(ps.peer_pads2[threadIdx.x] + ps.rank, gen);
-      }
-    }
-    // ---- phase B: wait until every rank's slice (and norm partial) has landed here ----
-    if ((int)threadIdx.x < W) {
-      unsigned int spins = 0;
-      unsigned long long t0 = 0ull;
-      while (ld_acquire_sys(ps.my_pad2 + threadIdx.x) < gen) spin_guard(spins, t0, "peer slice hand-shake");
-    }
-    __syncthreads();
-    G = ps.gsum;
-  }
   if (PEER == 1) {
     // ---- phase 0: cross-rank handshake, then all-reduce by direct peer loads into ps.gsum ----
     const unsigned int gen = *reinterpret_cast<volatile unsigned int*>(ps.local_gen) + 1u;
@@ -255,7 +156,7 @@ __global__ void __launch_bounds__(kAdamThreads)
     const double bs = block_sum<double>((double)acc, sred);
     if (threadIdx.x == 0) partials[(int64_t)s * gridDim.x + blockIdx.x] = bs;
   }
-  if (!PRENORM && PEER != 2) grid_barrier(&scratch->arrive);
+  if (!PRENORM) grid_barrier(&scratch->arrive);
   if (PEER == 1 && gtid == 0) *ps.local_gen = *ps.local_gen + 1u;  // every block read local_gen before this barrier
 
   // ---- phase 2 ----
@@ -287,13 +188,8 @@ __global__ void __launch_bounds__(kAdamThreads)
     int32_t cnt_adam = 0, cnt_sched = 0;  // requested together with the partials (one round trip, not two)
     if (lane == 0) cnt_adam = counts[2 * s], cnt_sched = counts[2 * s + 1];
     double part = 0.0;
-    if (PEER == 2) {  // per-rank partials of the segment, summed in rank order: the same number on every rank
-      const double* nt = reinterpret_cast<const double*>(ps.gsum + 4 * ps.total4);
-      for (int r = 0; r < ps.world; ++r) part += __ldcg(nt + r * kAdamMaxSegs + s);
-    } else {
-      for (unsigned int b = lane; b < nparts; b += 32) part += __ldcg(vp + b);
-      part = warp_sum(part);
-    }
+    for (unsigned int b = lane; b < nparts; b += 32) part += __ldcg(vp + b);
+    part = warp_sum(part);
     if (lane == 0) {
       const double ss = PRENORM ? part * (double)h.grad_scale * (double)h.grad_scale : part;
       const float g_norm = (float)sqrt(ss);
@@ -399,14 +295,13 @@ __global__ void __launch_bounds__(kAdamThreads)
   __syncthreads();
   if (threadIdx.x == 0) {
     __threadfence();
-    const unsigned long long t = atomicAdd(finish, 1ull);
+    const unsigned long long t = atomicAdd(&scratch->finish, 1ull);
     if (t % gridDim.x == gridDim.x - 1) {
       for (int s = 0; s < nseg; ++s) {
         counts[2 * s] += 1;
         counts[2 * s + 1] += 1;
         if (gnorm_out) gnorm_out[s] = s_gn[s];
       }
-      if (PEER == 2) *ps.local_gen = *ps.local_gen + 1u;  // every block of this call has read it
     }
   }
 }
@@ -417,13 +312,6 @@ __global__ void cast_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* _
     dst[i] = __float2bfloat16_rn(src[i]);
 }
 
-int adam_grid(int64_t total) {
-  int64_t blocks = (total / 4 + kAdamThreads - 1) / kAdamThreads;
-  if (blocks < 1) blocks = 1;
-  if (blocks > kNumSMs) blocks = kNumSMs;  // one wave, all blocks co-resident: the grid barrier is safe
-  return (int)blocks;
-}
-
 }  // namespace
 }  // namespace stx
 
@@ -431,7 +319,7 @@ using namespace stx;
 
 extern "C" size_t stx_adam_scratch_bytes(int nseg) {
   (void)nseg;
-  return sizeof(AdamScratch) + sizeof(double) * kAdamMaxSegs * kNumSMs + 64;  // + peer-sync generation words
+  return sizeof(AdamScratch);
 }
 
 // Host-side mirror of the segment table is needed to size the grid: callers pass the total span.
@@ -458,7 +346,6 @@ extern "C" int stx_clip_adam_step(float* param_arena, const float* grad_arena, f
                            mu, nu, counts, segs, nseg, *hyper, reinterpret_cast<__nv_bfloat16*>(params_bf16), gnorm_out,
                            reinterpret_cast<AdamScratch*>(scratch), none, RadamArgs{}));
   STX_LAUNCH_OK();
-  (void)adam_grid;
   return STX_OK;
 }
 
@@ -525,49 +412,11 @@ extern "C" int stx_allreduce_clip_adam_step(float* param_arena, const float* con
     ps.peer_pads[r] = reinterpret_cast<unsigned int*>(peer_signal_pads[r]) + pad_slot_offset;
   }
   ps.my_pad = ps.peer_pads[rank];
-  // local generation / release words live behind the barrier ticket of the optimiser scratch
-  char* sc = reinterpret_cast<char*>(scratch);
-  const size_t base = sizeof(AdamScratch) + sizeof(double) * kAdamMaxSegs * kNumSMs;
-  ps.local_gen = reinterpret_cast<unsigned int*>(sc + base);
+  ps.local_gen = &reinterpret_cast<AdamScratch*>(scratch)->gen;
   ps.gsum = gsum, ps.world = world, ps.rank = rank;
   STX_CUDA_OK(launch_pdl(clip_adam_kernel<false, 1>, dim3(kNumSMs), dim3(kAdamThreads), 0, (cudaStream_t)stream, param_arena,
                          static_cast<const float*>(gsum), mu, nu, counts, segs, nseg, *hyper,
                          reinterpret_cast<__nv_bfloat16*>(params_bf16), gnorm_out, reinterpret_cast<AdamScratch*>(scratch), ps, RadamArgs{}));
-  STX_LAUNCH_OK();
-  return STX_OK;
-}
-
-// Two-shot form of the above: peer_gsum[r] = rank r's reduced-gradient buffer (peer-mapped, arena_len + 128 floats: the tail is a
-// double[world][8] table of per-rank sum-of-squares partials), two signal rows [pad_slot_offset, +8) and [+8, +16).
-extern "C" int stx_allreduce2_clip_adam_step(float* param_arena, const float* const* peer_grads, float* const* peer_gsum, int64_t arena_len,
-                                             void* const* peer_signal_pads, int world, int rank, int pad_slot_offset, float* mu, float* nu,
-                                             int32_t* counts, const StxAdamSeg* segs, int nseg, const StxAdamHyper* hyper, void* params_bf16,
-                                             float* gnorm_out, void* scratch, int grid, void* stream) {
-  STX_REQUIRE(param_arena && peer_grads && peer_gsum && peer_signal_pads && mu && nu && counts && segs && hyper && scratch, STX_E_ARG,
-              "stx_allreduce2_clip_adam_step: null pointer");
-  STX_REQUIRE(world >= 2 && world <= 8 && rank >= 0 && rank < world, STX_E_SHAPE, "stx_allreduce2_clip_adam_step: world=%d rank=%d (2..8 ranks)", world, rank);
-  STX_REQUIRE(nseg >= 1 && nseg <= kAdamMaxSegs, STX_E_SHAPE, "stx_allreduce2_clip_adam_step: nseg=%d", nseg);
-  STX_REQUIRE(arena_len > 0 && arena_len % 4 == 0, STX_E_SHAPE, "stx_allreduce2_clip_adam_step: arena_len=%lld must be a multiple of 4", (long long)arena_len);
-  STX_REQUIRE(grid >= 0 && grid <= kNumSMs, STX_E_ARG, "stx_allreduce2_clip_adam_step: grid=%d", grid);
-  STX_REQUIRE(!hyper->prenorm, STX_E_ARG, "stx_allreduce2_clip_adam_step: prenorm is a single-device shortcut");
-  PeerSync ps{};
-  for (int r = 0; r < world; ++r) {
-    STX_REQUIRE(peer_grads[r] && peer_gsum[r] && peer_signal_pads[r], STX_E_ARG, "stx_allreduce2_clip_adam_step: null peer pointer %d", r);
-    STX_REQUIRE(aligned16(peer_grads[r]) && aligned16(peer_gsum[r]), STX_E_ALIGN, "stx_allreduce2_clip_adam_step: peer buffer %d not 16-byte aligned", r);
-    ps.peer_grads[r] = peer_grads[r];
-    ps.peer_gsum[r] = peer_gsum[r];
-    ps.peer_pads[r] = reinterpret_cast<unsigned int*>(peer_signal_pads[r]) + pad_slot_offset;
-    ps.peer_pads2[r] = ps.peer_pads[r] + 8;
-  }
-  ps.my_pad = ps.peer_pads[rank], ps.my_pad2 = ps.peer_pads2[rank];
-  char* sc = reinterpret_cast<char*>(scratch);
-  const size_t base = sizeof(AdamScratch) + sizeof(double) * kAdamMaxSegs * kNumSMs;
-  ps.local_gen = reinterpret_cast<unsigned int*>(sc + base);
-  ps.done = reinterpret_cast<unsigned long long*>(sc + base + 32);
-  ps.gsum = peer_gsum[rank], ps.world = world, ps.rank = rank, ps.total4 = arena_len / 4;
-  STX_CUDA_OK(launch_pdl(clip_adam_kernel<false, 2>, dim3(grid > 0 ? grid : kNumSMs), dim3(kAdamThreads), 0, (cudaStream_t)stream, param_arena,
-                         static_cast<const float*>(ps.gsum), mu, nu, counts, segs, nseg, *hyper, reinterpret_cast<__nv_bfloat16*>(params_bf16),
-                         gnorm_out, reinterpret_cast<AdamScratch*>(scratch), ps, RadamArgs{}));
   STX_LAUNCH_OK();
   return STX_OK;
 }

@@ -17,7 +17,7 @@ namespace stx {
 // implemented in stx_tc_mlp.cu
 int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxPpoBatch* batch, int64_t mb_off, int64_t mb,
                            const StxPpoHyper* hyper, float grad_weight, float* grad_arena, float* metrics, void* ws, size_t ws_bytes,
-                           cudaStream_t st, const StxFusedAdam* opt);
+                           cudaStream_t st);
 
 namespace {
 
@@ -425,26 +425,11 @@ extern "C" int stx_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic
   if (int rc = head_dims(actor, 1, &g.A, who)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   if (precision == STX_PREC_BF16)
-    return tc_ppo_minibatch_grads(actor, critic, b, mb_off, mb, h, grad_weight, grad_arena, metrics, workspace, workspace_bytes, st, nullptr);
+    return tc_ppo_minibatch_grads(actor, critic, b, mb_off, mb, h, grad_weight, grad_arena, metrics, workspace, workspace_bytes, st);
   STX_REQUIRE(precision == STX_PREC_F32, STX_E_UNSUPPORTED, "%s: precision=%d", who, precision);
   g.action = b->action;
   return fp32_minibatch(actor, critic, b, mb_off, mb, h, grad_weight, grad_arena, metrics, workspace, g, launch_actor_loss<CategoricalRow, ClipLoss>,
                         st);
-}
-
-extern "C" int stx_ppo_minibatch_update(const StxMlp* actor, const StxMlp* critic, const StxPpoBatch* b, int64_t mb_off, int64_t mb,
-                                        const StxPpoHyper* h, float grad_weight, float* grad_arena, float* metrics, void* workspace,
-                                        size_t workspace_bytes, const StxFusedAdam* opt, void* stream) {
-  const char* who = "stx_ppo_minibatch_update";
-  if (int rc = check_minibatch(actor, critic, b, mb_off, mb, h, grad_arena, metrics, STX_PREC_BF16, nullptr, workspace, workspace_bytes, who))
-    return rc;
-  STX_REQUIRE(b->action, STX_E_ARG, "%s: null batch action", who);
-  STX_REQUIRE(opt && opt->param_arena && opt->mu && opt->nu && opt->counts && opt->segs && opt->scratch, STX_E_ARG, "%s: null optimiser field", who);
-  STX_REQUIRE(opt->nseg == 2, STX_E_SHAPE, "%s: nseg=%d (segment 0 = actor arena, 1 = critic arena)", who, opt->nseg);
-  STX_REQUIRE(opt->hyper.steps_per_update > 0 && opt->hyper.num_updates > 0, STX_E_ARG, "%s: steps_per_update/num_updates must be positive",
-              who);
-  return tc_ppo_minibatch_grads(actor, critic, b, mb_off, mb, h, grad_weight, grad_arena, metrics, workspace, workspace_bytes,
-                                (cudaStream_t)stream, opt);
 }
 
 extern "C" int stx_ppo_continuous_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxPpoBatch* b, const StxTanhNormalPpo* head,

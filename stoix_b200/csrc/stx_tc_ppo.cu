@@ -22,8 +22,8 @@
 //      The activations travel K3a -> K3b in a tiled layout [tile of 128 rows][8-column group][row][8]:
 //      one TMA box of K3b lands 64 rows of every column group as un-swizzled core matrices (8 rows x 16 B).
 //  tc_reduce_kernel     fixed-order reduction of the per-CTA partials into the flat fp32 gradient arena
-//      (deterministic; also the bias gradients and the six loss metrics); optionally fused with clip + Adam
-//      (stx_ppo_minibatch_update).
+//      (deterministic; also the bias gradients and the six loss metrics); optionally leaves the sum(g^2)
+//      partials of both networks for clip + Adam (PRENORM).
 // The three kernels (and K4 behind them) are chained with programmatic dependent launch; activations carry
 // evict_first, partials / gradients evict_last L2 policies (see stx_common.cuh).
 #include <cuda.h>
@@ -792,42 +792,18 @@ struct RedParams {
 };
 
 constexpr int kRedThreads = 352;  // x 528 blocks >= the ~173k gradient entries of the benchmark networks: one element per thread
-constexpr int kRedMaxBlocks = 4 * kNumSMs;  // the optimiser scratch holds 8 x 132 doubles = 2 segments x 528 block partials
-
-// Optimiser context of the fused variant (stx_ppo_minibatch_update): clip_by_global_norm + Adam of stx_adam.cu applied
-// by the thread that reduced the gradient entry.  scratch layout = stx_adam.cu's AdamScratch.
-struct FusedOpt {
-  float* P;
-  float* MU;
-  float* NU;
-  int32_t* counts;
-  const StxAdamSeg* segs;
-  StxAdamHyper h;
-  __nv_bfloat16* P16;
-  float* gnorm_out;
-  unsigned long long* arrive;   // grid-barrier ticket (monotonic)
-  unsigned long long* finish;   // last-block ticket (monotonic)
-};
+constexpr int kRedMaxBlocks = 4 * kNumSMs;
+static_assert(2 * kRedMaxBlocks <= kAdamMaxSegs * kNumSMs, "AdamScratch::partials must hold 2 segments x kRedMaxBlocks block partials");
 
 // Fixed-order reduction of the per-CTA partials into the gradient arena.  One launch, every segment
 // concurrently; 4 independent accumulators per element for load-level parallelism; the association order
 // is fixed => run-to-run deterministic gradients.  Optionally leaves the per-block sum of squares of the
-// reduced gradient for the fused optimiser (which can then skip its own norm pass and grid barrier).
-//
-// FUSED: every thread owns at most ONE gradient entry (host-checked) and keeps it in a register; after the per-block
-// sum-of-squares partials are published the blocks meet at a software grid barrier (all blocks are co-resident: the
-// host checks the occupancy), every block re-reduces the partials in the fixed order of clip_adam_kernel<PRENORM>
-// and the thread applies clip + Adam + the bf16 shadow update to its entry: K4 without its launch, its gradient
-// re-read and its own ramp-up.
-template <bool FUSED>
-__global__ void __launch_bounds__(kRedThreads, 4) tc_reduce_kernel(const RedParams p, float* __restrict__ grad, const FusedOpt f) {
+// reduced gradient for clip + Adam (PRENORM: it then skips its own norm pass and grid barrier).
+__global__ void __launch_bounds__(kRedThreads, 4) tc_reduce_kernel(const RedParams p, float* __restrict__ grad) {
   griddep_launch();
   griddep_wait();
   const uint64_t pol_keep = l2_evict_last();  // partials and gradients: small, reused every step, latency-critical
   double sq0 = 0.0, sq1 = 0.0;
-  int64_t my_dst = -1;  // FUSED: arena index, value and optimiser segment of this thread's entry
-  float my_g = 0.f;
-  int my_net = 0;
   for (int gi = blockIdx.x * blockDim.x + threadIdx.x; gi < p.total_items; gi += gridDim.x * blockDim.x) {
     int s = 0, i = gi;
     while (i >= p.seg[s].items) i -= p.seg[s].items, ++s;
@@ -871,7 +847,6 @@ __global__ void __launch_bounds__(kRedThreads, 4) tc_reduce_kernel(const RedPara
       st_hint(dst, o, pol_keep);
       if (g.net) sq1 += (double)o * o;
       else sq0 += (double)o * o;
-      if (FUSED) my_dst = dst - grad, my_g = o, my_net = g.net;
     }
   }
   if (p.sumsq != nullptr) {  // only meaningful with overwrite (then o is the whole gradient)
@@ -887,72 +862,6 @@ __global__ void __launch_bounds__(kRedThreads, 4) tc_reduce_kernel(const RedPara
     float acc = 0.f;
     for (int k = 0; k < p.n_cta_total; ++k) acc += p.metric_part[(int64_t)k * 8 + threadIdx.x];
     p.metrics[threadIdx.x] += p.weight * acc * p.inv_mb;
-  }
-  if (FUSED) {
-    __shared__ StxAdamSeg s_seg[2];
-    __shared__ float s_gs[2], s_bc1[2], s_bc2[2], s_lr[2], s_gn[2];
-    if (threadIdx.x < 2) s_seg[threadIdx.x] = f.segs[threadIdx.x];
-    // ---- grid barrier (partials of every block are published above) ----
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      __threadfence();
-      const unsigned long long t = atomicAdd(f.arrive, 1ull);
-      const unsigned long long target = (t / gridDim.x + 1ull) * gridDim.x;
-      unsigned int spins = 0;
-      unsigned long long t0 = 0ull;
-      while (*reinterpret_cast<volatile unsigned long long*>(f.arrive) < target) spin_guard(spins, t0, "reduce+optimiser grid barrier");
-      __threadfence();
-    }
-    __syncthreads();
-    // ---- norms: warp s <-> segment s, same summation order as clip_adam_kernel<PRENORM> ----
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (warp < 2) {
-      const int s = warp;
-      const double* vp = p.sumsq + (int64_t)s * gridDim.x;
-      double part = 0.0;
-      for (unsigned int b = lane; b < gridDim.x; b += 32) part += __ldcg(vp + b);
-      part = warp_sum(part);
-      if (lane == 0) {
-        const double ss = part * (double)f.h.grad_scale * (double)f.h.grad_scale;
-        const float g_norm = (float)sqrt(ss);
-        const float clip = (g_norm < s_seg[s].max_grad_norm) ? 1.0f : s_seg[s].max_grad_norm / g_norm;
-        const int32_t c = f.counts[2 * s] + 1;
-        float lr = s_seg[s].init_lr;
-        if (f.h.decay) {
-          const int32_t k = f.counts[2 * s + 1] / f.h.steps_per_update;  // floor division, utils/training.py:25
-          lr = s_seg[s].init_lr * (1.0f - (float)k / (float)f.h.num_updates);
-        }
-        s_gs[s] = f.h.grad_scale * clip;
-        s_bc1[s] = 1.0f - powf(f.h.b1, (float)c);
-        s_bc2[s] = 1.0f - powf(f.h.b2, (float)c);
-        s_lr[s] = lr;
-        s_gn[s] = g_norm;
-      }
-    }
-    __syncthreads();
-    if (my_dst >= 0) {
-      const int s = my_net;
-      const float ge = my_g * s_gs[s];
-      const float me = f.h.b1 * f.MU[my_dst] + (1.0f - f.h.b1) * ge;
-      const float ve = f.h.b2 * f.NU[my_dst] + (1.0f - f.h.b2) * ge * ge;
-      const float u = (me / s_bc1[s]) / (sqrtf(ve / s_bc2[s]) + f.h.eps);
-      const float pn = f.P[my_dst] - s_lr[s] * u;
-      f.MU[my_dst] = me, f.NU[my_dst] = ve, f.P[my_dst] = pn;
-      if (f.P16) f.P16[my_dst] = __float2bfloat16_rn(pn);
-    }
-    // the step counters are advanced by whichever block finishes last (every block has read them by then)
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      __threadfence();
-      const unsigned long long t = atomicAdd(f.finish, 1ull);
-      if (t % gridDim.x == gridDim.x - 1) {
-        for (int s = 0; s < 2; ++s) {
-          f.counts[2 * s] += 1;
-          f.counts[2 * s + 1] += 1;
-          if (f.gnorm_out) f.gnorm_out[s] = s_gn[s];
-        }
-      }
-    }
   }
 }
 
@@ -1036,7 +945,7 @@ size_t tc_ppo_workspace_bytes(const StxMlp* a, const StxMlp* c, int64_t mb) {
 
 int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxPpoBatch* b, int64_t mb_off, int64_t mb,
                            const StxPpoHyper* h, float grad_weight, float* grad_arena, float* metrics, void* ws_raw, size_t,
-                           cudaStream_t st, const StxFusedAdam* opt) {
+                           cudaStream_t st) {
   using namespace tc;
   STX_REQUIRE(tc_ppo_shape_ok(actor) && tc_ppo_shape_ok(critic), STX_E_SHAPE,
               "STX_PREC_BF16 PPO kernels need a relu MLP without LayerNorm, sizes [D<=64 (mult of 8), 256, 256, head<=16]");
@@ -1145,33 +1054,13 @@ int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxP
   rp.n_seg = sidx;
   rp.metric_part = ws.metric_part, rp.n_cta_total = 2 * n_fb, rp.metrics = metrics;
   rp.weight = grad_weight, rp.inv_mb = 1.0f / (float)mb;
-  rp.overwrite = opt ? 1 : h->overwrite_grads;
-  // side output for the fused optimiser: partials[seg][block] right after the 16-byte header of its scratch
-  void* adam_scratch = opt ? opt->scratch : h->adam_scratch;
-  rp.sumsq = (rp.overwrite && adam_scratch) ? reinterpret_cast<double*>(reinterpret_cast<char*>(adam_scratch) + 16) : nullptr;
-  rp.sumsq_count = reinterpret_cast<unsigned long long*>(reinterpret_cast<char*>(adam_scratch) + 8);
+  rp.overwrite = h->overwrite_grads;
+  // side output for clip + Adam (PRENORM): the block partials and their count in its scratch
+  AdamScratch* adam_scratch = static_cast<AdamScratch*>(h->adam_scratch);
+  if (rp.overwrite && adam_scratch) rp.sumsq = adam_scratch->partials, rp.sumsq_count = &adam_scratch->n_partials;
   int red_blocks = (rp.total_items + kRedThreads - 1) / kRedThreads;  // one item per thread, blocks spread over all SMs
   if (red_blocks > kRedMaxBlocks) red_blocks = kRedMaxBlocks;
-  FusedOpt fo{};
-  if (opt) {
-    // one entry per thread and all blocks co-resident (grid barrier), else the caller must use the two-call path
-    static int blocks_per_sm = -1;
-    if (blocks_per_sm < 0) STX_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, tc_reduce_kernel<true>, kRedThreads, 0));
-    STX_REQUIRE(rp.total_items <= red_blocks * kRedThreads && red_blocks <= blocks_per_sm * kNumSMs, STX_E_SHAPE,
-                "stx_ppo_minibatch_update: %d gradient entries do not fit one co-resident wave (%d blocks x %d threads, %d blocks/SM)",
-                rp.total_items, red_blocks, kRedThreads, blocks_per_sm);
-    fo.P = opt->param_arena, fo.MU = opt->mu, fo.NU = opt->nu, fo.counts = opt->counts, fo.segs = opt->segs, fo.h = opt->hyper;
-    fo.P16 = reinterpret_cast<__nv_bfloat16*>(opt->params_bf16), fo.gnorm_out = opt->gnorm_out;
-    char* sc = reinterpret_cast<char*>(opt->scratch);
-    // own ticket words (stx_adam.cu keeps its barrier / last-block tickets for a kNumSMs-block grid in the same scratch: the
-    // modulo arithmetic of a ticket is only valid for one grid size)
-    char* tail = sc + 16 + sizeof(double) * 8 * kNumSMs;  // = sizeof(AdamScratch) + partials; 64 spare bytes follow
-    fo.arrive = reinterpret_cast<unsigned long long*>(tail + 24);
-    fo.finish = reinterpret_cast<unsigned long long*>(tail + 32);
-    STX_CUDA_OK(launch_pdl(tc_reduce_kernel<true>, dim3(red_blocks), dim3(kRedThreads), 0, st, rp, grad_arena, fo));
-  } else {
-    STX_CUDA_OK(launch_pdl(tc_reduce_kernel<false>, dim3(red_blocks), dim3(kRedThreads), 0, st, rp, grad_arena, fo));
-  }
+  STX_CUDA_OK(launch_pdl(tc_reduce_kernel, dim3(red_blocks), dim3(kRedThreads), 0, st, rp, grad_arena));
   STX_LAUNCH_OK();
   return STX_OK;
 }

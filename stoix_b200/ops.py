@@ -7,7 +7,6 @@ eager-PyTorch fallback -- a non-CUDA tensor raises StxError.
 from __future__ import annotations
 
 import ctypes as C
-import os
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -305,18 +304,18 @@ def ppo_workspace(actor: MlpSpec, critic: MlpSpec, mb: int, precision: int, devi
 def _minibatch_structs(who: str, actor: MlpSpec, critic: MlpSpec, param_arena: torch.Tensor, batch: PpoBatch, grad_arena: torch.Tensor,
                        metrics: torch.Tensor, workspace: torch.Tensor, hyper: Tuple, *, obs_dtype: torch.dtype, fp32_only: str = "",
                        n_metrics: int = 6, categorical: bool = True, param_arena_bf16: Optional[torch.Tensor] = None,
-                       arenas: Tuple[torch.Tensor, ...] = (), adam_scratch: Optional[torch.Tensor] = None):
+                       adam_scratch: Optional[torch.Tensor] = None):
     """The checks every PPO minibatch wrapper shares, and its StxMlp (actor, critic), StxPpoBatch and StxPpoHyper.  hyper =
-    (clip_eps, ent_coef, vf_coef, standardize, overwrite); `arenas` must hold the whole arena too; a tanh-Normal batch
+    (clip_eps, ent_coef, vf_coef, standardize, overwrite); a tanh-Normal batch
     (categorical=False) holds float (B, A) actions that go to the C entry through StxTanhNormalPpo instead."""
     _need_cuda(param_arena, batch.obs, batch.action, batch.log_prob, batch.value, batch.advantages, batch.targets, batch.adv_stats, batch.perm,
-               grad_arena, metrics, workspace, param_arena_bf16, *arenas)
+               grad_arena, metrics, workspace, param_arena_bf16)
     if (categorical and batch.action.dtype != torch.int32) or (batch.perm is not None and batch.perm.dtype != torch.int32):
         raise StxError(f"{who}: action / perm must be int32" if categorical else f"{who}: perm must be int32")
     if batch.obs.dtype != obs_dtype:
         raise StxError(f"{who}: obs must be {obs_dtype}" + (f" ({fp32_only} runs on the fp32 path)" if fp32_only else ""))
     _, coff, total = arena_offsets(actor, critic)
-    if min(t.numel() for t in (param_arena, grad_arena) + arenas) < total or metrics.numel() < n_metrics:
+    if min(t.numel() for t in (param_arena, grad_arena)) < total or metrics.numel() < n_metrics:
         raise StxError(f"{who}: arena too small or metrics below {n_metrics} floats")
     a = actor.c_struct(param_arena, param_arena_bf16)
     c = critic.c_struct(param_arena[coff:], param_arena_bf16[coff:] if param_arena_bf16 is not None else None)
@@ -351,31 +350,6 @@ def ppo_minibatch_grads(actor: MlpSpec, critic: MlpSpec, param_arena: torch.Tens
     )
 
 
-def ppo_minibatch_update(actor: MlpSpec, critic: MlpSpec, param_arena: torch.Tensor, batch: PpoBatch,
-                         mb_off: int, mb: int, clip_eps: float, ent_coef: float, vf_coef: float,
-                         standardize: bool, grad_arena: torch.Tensor, metrics: torch.Tensor,
-                         workspace: torch.Tensor, plan: "AdamPlan", mu: torch.Tensor, nu: torch.Tensor,
-                         param_arena_bf16: torch.Tensor, grad_weight: float = 1.0, grad_scale: float = 1.0) -> None:
-    """One whole optimiser step on minibatch [mb_off, mb_off+mb) (ff_ppo.py:184-284): gradients of both losses,
-    clip_by_global_norm + Adam on both networks, bf16 shadow refresh; the gradient reduction and the optimiser share
-    one launch (stx_ppo_minibatch_update).  bf16 path, one shard, one device; `plan` must hold exactly the two
-    segments (actor arena, critic arena).  Same results as ppo_minibatch_grads(overwrite=True) + clip_adam_step."""
-    a, c, b, h = _minibatch_structs("ppo_minibatch_update", actor, critic, param_arena, batch, grad_arena, metrics, workspace,
-                                    (clip_eps, ent_coef, vf_coef, standardize, True), obs_dtype=torch.bfloat16,
-                                    param_arena_bf16=param_arena_bf16, arenas=(mu, nu, param_arena_bf16))
-    if plan.nseg != 2:
-        raise StxError("ppo_minibatch_update: the optimiser plan must have the two segments (actor, critic)")
-    plan.hyper.grad_scale = float(grad_scale)
-    plan.hyper.prenorm = 0
-    opt = _lib.StxFusedAdam(_p(param_arena), _p(mu), _p(nu), _p(plan.counts), _p(plan.segs), plan.nseg, 0, plan.hyper,
-                            _p(param_arena_bf16), _p(plan.gnorm), _p(plan.scratch))
-    _lib.check(
-        _lib.load().stx_ppo_minibatch_update(C.byref(a), C.byref(c), C.byref(b), int(mb_off), int(mb), C.byref(h), float(grad_weight),
-                                             _p(grad_arena), _p(metrics), _p(workspace), workspace.numel(), C.byref(opt), _stream()),
-        "stx_ppo_minibatch_update",
-    )
-
-
 def _loss_value(fn_name: str, a, b, c, eps: float) -> torch.Tensor:
     dev = _need_cuda(a, b, c)
     if not (a.dtype == b.dtype == c.dtype == torch.float32) or not (a.numel() == b.numel() == c.numel()):
@@ -400,7 +374,7 @@ def clipped_value_loss_value(pred_value_t, behavior_value_t, targets_t, epsilon)
 # ------------------------------------------------------------------------------------------------
 
 
-ADAM_MAX_SEGS = 8  # kAdamMaxSegs of stx_adam.cu
+ADAM_MAX_SEGS = 8  # kAdamMaxSegs of stx_common.cuh
 
 
 class AdamPlan:
@@ -521,21 +495,10 @@ class PeerGradBuffers:
         self.slot = pad_words - 64  # far from the channels torch's own barriers use at the start of the pad
         pad = h0.get_signal_pad(self.rank, (pad_words,), torch.uint32) if hasattr(h0, "get_signal_pad") else None
         if pad is not None:
-            pad[self.slot:self.slot + 16] = 0
+            pad[self.slot:self.slot + 8] = 0
         self.grad_ptrs = [(C.c_void_p * self.world)(*[int(p) for p in h.buffer_ptrs]) for h in self.handles]
         self.pad_ptrs = (C.c_void_p * self.world)(*[int(p) for p in h0.signal_pad_ptrs])
         self.gsum = torch.zeros(int(total), dtype=torch.float32, device=device)
-        # two-shot form: the reduced gradient of every rank is written by its peers -> symmetric too (+ the norm table)
-        self.total = int(total)
-        self.gsum2 = symm_mem.empty(self.total + 128, dtype=torch.float32, device=device)
-        self.gsum2.zero_()
-        self.gsum2_handle = symm_mem.rendezvous(self.gsum2, group)
-        self.gsum2_ptrs = (C.c_void_p * self.world)(*[int(p) for p in self.gsum2_handle.buffer_ptrs])
-        # 1 = one-shot (default), 2 = two-shot: the second cross-GPU hand-shake of two-shot (fence.sys after the peer stores,
-        # last-block norm, signal flight) can cost more than the (W-1) extra arenas of 0.67 MB it saves.
-        self.mode = int(os.environ.get("STX_ALLREDUCE_MODE", "1"))
-        if self.total % 4 != 0:
-            self.mode = 1
         torch.cuda.synchronize()
         dist.barrier(group)
 
@@ -550,14 +513,6 @@ def allreduce_clip_adam_step(plan: AdamPlan, peers: PeerGradBuffers, which: int,
     _need_cuda(params, mu, nu, params_bf16)
     plan.hyper.grad_scale = 1.0 / peers.world
     plan.hyper.prenorm = 0
-    if peers.mode == 2:
-        _lib.check(
-            _lib.load().stx_allreduce2_clip_adam_step(_p(params), peers.grad_ptrs[which], peers.gsum2_ptrs, peers.total, peers.pad_ptrs, peers.world,
-                                                      peers.rank, peers.slot, _p(mu), _p(nu), _p(plan.counts), _p(plan.segs), plan.nseg,
-                                                      C.byref(plan.hyper), _p(params_bf16), _p(plan.gnorm), _p(plan.scratch), 0, _stream()),
-            "stx_allreduce2_clip_adam_step",
-        )
-        return
     _lib.check(
         _lib.load().stx_allreduce_clip_adam_step(_p(params), peers.grad_ptrs[which], peers.pad_ptrs, peers.world, peers.rank, peers.slot,
                                                  _p(peers.gsum), _p(mu), _p(nu), _p(plan.counts), _p(plan.segs), plan.nseg,

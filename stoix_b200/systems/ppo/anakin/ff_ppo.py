@@ -24,7 +24,6 @@ position lives in device memory so replays draw fresh numbers.
 """
 from __future__ import annotations
 
-import os
 from typing import Any, Callable, Dict, List, Optional, Tuple
 
 import torch
@@ -292,18 +291,11 @@ def get_learner_fn(
             # single shard on a single device: the gradient reduction can hand sum(g^2) straight to the fused
             # optimiser (no separate norm pass / grid barrier); otherwise the all-reduce sits in between.
             prenorm = precision == ops.STX_PREC_BF16 and U == 1 and world == 1
-            fused_update = bool(arch.get("fused_update", False)) or os.environ.get("STX_FUSED_UPDATE", "0") == "1"
             peers = b["peers_obj"]
             for i in range(nmb):  # _update_minibatch (ff_ppo.py:184-284)
                 which = (ep * nmb + i) & 1
                 if peers is not None:
                     grads = peers.bufs[which]  # ping-pong arenas in peer-mapped memory
-                if prenorm and fused_update:
-                    # gradients + both optimiser updates (ff_ppo.py:184-273) with the reduction and clip+Adam in one launch
-                    ops.ppo_minibatch_update(sa, sc, b["arena"], batches[0], i * mb, mb, float(sysc.clip_eps), float(sysc.ent_coef),
-                                             float(sysc.vf_coef), bool(sysc.standardize_advantages), grads, metrics[ep, i], b["ws"],
-                                             b["plan"], a_tree.arena_mu, a_tree.arena_nu, b["arena_bf16"])
-                    continue
                 for u in range(U):  # vmap over "batch" + pmean("batch") (ff_ppo.py:253-256); first shard overwrites
                     sh = b["shards"][u]
                     behaviour = sh.behaviour.view(B, -1) if sh.behaviour is not None else None

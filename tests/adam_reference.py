@@ -1,5 +1,5 @@
-"""One optimiser step of the clip + Adam kernel (K4, stoix_b200/csrc/stx_adam.cu, and its fused copy in tc_reduce_kernel) in
-float64, with a per-element error bound derived from the kernel's fp32 arithmetic.
+"""One optimiser step of the clip + Adam kernel (K4, stoix_b200/csrc/stx_adam.cu) in float64, with a per-element error
+bound derived from the kernel's fp32 arithmetic.
 
 `step(p, mu, nu, counts, g, segs, hyper)` takes the state BEFORE the step (what the kernel read) and returns what the step
 must produce and how far the kernel may be from it.  Nothing is chained: every GPU test feeds it the kernel's own pre-step
@@ -20,7 +20,7 @@ from __future__ import annotations
 
 import math
 from dataclasses import dataclass
-from typing import List, Optional, Sequence, Tuple
+from typing import List, Sequence, Tuple
 
 import numpy as np
 
@@ -30,8 +30,8 @@ TINY = 2.0 ** -149        # >= the absolute rounding error of one fp32 operation
 POWF_ULP = 4              # CUDA Math API / CUDA C++ Programming Guide, "Mathematical Functions", single-precision table:
 #                           powf(x, y) has a maximum error of 4 ulp over the full range (no -use_fast_math in this build)
 KERNEL_THREADS = 132 * 256   # clip_adam_kernel: one block of 256 threads per SM, always 132 blocks
-NORM_LOCAL = "local"      # fp32 sum of squares per thread, then double (local, one-shot and two-shot forms)
-NORM_DOUBLE = "double"    # squares of the fp32 gradient summed in double (prenorm and fused forms: tc_reduce_kernel)
+NORM_LOCAL = "local"      # fp32 sum of squares per thread, then double (local and one-shot forms)
+NORM_DOUBLE = "double"    # squares of the fp32 gradient summed in double (prenorm form: tc_reduce_kernel)
 
 f32 = np.float32
 
@@ -87,7 +87,7 @@ def norm_items(count: int, threads: int = KERNEL_THREADS) -> int:
     return max(1, -(-(count // 4) // threads))
 
 
-def _segment(p, m, v, g, count_adam, count_sched, seg: Seg, h: Hyper, norm: str, items: Optional[int]):
+def _segment(p, m, v, g, count_adam, count_sched, seg: Seg, h: Hyper, norm: str):
     """Expected values and bounds of one segment.  All inputs are the fp32 values the kernel read, as float64."""
     off, cnt, init_lr, max_norm = seg
     b1, b2, eps, gsc = (float(f32(x)) for x in (h.b1, h.b2, h.eps, h.grad_scale))
@@ -100,11 +100,11 @@ def _segment(p, m, v, g, count_adam, count_sched, seg: Seg, h: Hyper, norm: str,
     gn = math.sqrt(ss)
     if norm == NORM_LOCAL:
         # A thread squares and sums in fp32: ge = g * gs (1 rounding, squared: 2), ge * ge (1), the 3 adds inside a float4
-        # item, then one add per item into its accumulator (`items` float4 items + the scalar tail) -- at most items + 7
+        # item, then one add per item into its accumulator (norm_items float4 items + the scalar tail) -- at most items + 7
         # roundings on any term.  All terms are >= 0, so the per-thread sums, and hence ss, carry at most
         # (1 + U32)^(items + 7) - 1 relatively.  The block / partial sums in double add <= cnt * U64, sqrt in double 1 U64,
         # the cast to float 1 U32.
-        m_r = (items if items is not None else norm_items(cnt)) + 7
+        m_r = norm_items(cnt) + 7
         eps_n = math.sqrt(1.0 + _gam(m_r)) * (1.0 + (cnt + 2) * U64) * (1.0 + U32) - 1.0
     elif norm == NORM_DOUBLE:
         # (double) o * o is exact, the sums and the two multiplications by grad_scale round in double: (cnt + 4) U64,
@@ -180,10 +180,8 @@ def _segment(p, m, v, g, count_adam, count_sched, seg: Seg, h: Hyper, norm: str,
     return dict(p=Pn, mu=M, nu=V, gnorm=gn, p_b=E_p, mu_b=E_m, nu_b=E_v, gn_b=gn_bound, clipped=clipped)
 
 
-def step(p, mu, nu, counts, g, segs: Sequence[Seg], hyper: Hyper, norm: str = NORM_LOCAL,
-         items: Optional[Sequence[Optional[int]]] = None) -> Step:
-    """Expected result of one clip + Adam step from the pre-step state (fp32 arrays of the whole arena, int counts[2 nseg]).
-    `items[s]` overrides the float4 items a thread sums in fp32 for segment s (the two-shot form strides over the arena)."""
+def step(p, mu, nu, counts, g, segs: Sequence[Seg], hyper: Hyper, norm: str = NORM_LOCAL) -> Step:
+    """Expected result of one clip + Adam step from the pre-step state (fp32 arrays of the whole arena, int counts[2 nseg])."""
     p, mu, nu, g = (np.asarray(a, dtype=np.float32).astype(np.float64) for a in (p, mu, nu, g))
     counts = np.asarray(counts, dtype=np.int64)
     out = {k: a.copy() for k, a in (("p", p), ("mu", mu), ("nu", nu))}
@@ -193,8 +191,7 @@ def step(p, mu, nu, counts, g, segs: Sequence[Seg], hyper: Hyper, norm: str = NO
     for s, seg in enumerate(segs):
         off, cnt = int(seg[0]), int(seg[1])
         sl = slice(off, off + cnt)
-        r = _segment(p[sl], mu[sl], nu[sl], g[sl], counts[2 * s], counts[2 * s + 1], seg, hyper, norm,
-                     None if items is None else items[s])
+        r = _segment(p[sl], mu[sl], nu[sl], g[sl], counts[2 * s], counts[2 * s + 1], seg, hyper, norm)
         for k in ("p", "mu", "nu"):
             out[k][sl], bnd[k][sl] = r[k], r[k + "_b"]
         inside[sl] = True

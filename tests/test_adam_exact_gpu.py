@@ -7,9 +7,9 @@ gradient arena (K4 must not write it) and every float outside the optimiser segm
 shadow.  Within the bounds: parameters, moments and the reported pre-clip global norm.
 
 Forms: the local form (norm pass + grid barrier) on three segment layouts through a whole schedule; the prenorm form as the
-bf16 learner chains it (the sum-of-squares partials come from K3's gradient reduction); the reduction with the optimiser
-fused into it; all three through the learner (the CUDA graph on, as shipped).  The all-reduce forms are checked the same way
-in tests/test_distributed_gpu.py::test_fused_allreduce_kernel_on_one_device."""
+bf16 learner chains it (the sum-of-squares partials come from K3's gradient reduction); both through the learner (the CUDA
+graph on, as shipped).  The one-shot all-reduce form is checked the same way in
+tests/test_distributed_gpu.py::test_fused_allreduce_kernel_on_one_device."""
 import numpy as np
 import pytest
 import torch
@@ -62,7 +62,7 @@ def test_local_form_steps_through_the_schedule(name, decay, grad_scale):
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
-# prenorm (the benchmark's path) and the fused reduction + optimiser
+# prenorm (the benchmark's path)
 # ---------------------------------------------------------------------------------------------------------------------------
 
 
@@ -95,11 +95,11 @@ def _bf16_problem(D, A, mb, seed):
 SHAPES = [(D, A, mb) for D in (8, 64) for A in (1, 8, 16) for mb in (128, 4096, 32768)]   # mb 32768: the benchmark's minibatch
 
 
-@pytest.mark.parametrize("form", ["prenorm", "fused"])
+@pytest.mark.parametrize("form", ["prenorm"])
 @pytest.mark.parametrize("D,A,mb", SHAPES)
 def test_bf16_update_forms(D, A, mb, form):
     """prenorm: ppo_minibatch_grads(bf16, overwrite, adam_scratch) then clip_adam_step(prenorm) with nothing enqueued between
-    them, so the programmatic-dependent-launch pairing is the one the learner ships.  fused: ppo_minibatch_update.  The pre-state
+    them, so the programmatic-dependent-launch pairing is the one the learner ships.  The pre-state
     is copied before K3 (neither K3 nor the reduction writes it), the gradient and the post-state after the step; the reported
     norm must be the fp64 norm of the gradient arena K3 wrote.  Two steps: the adam count and the schedule (spu 2) advance."""
     from stoix_b200 import ops
@@ -113,12 +113,9 @@ def test_bf16_update_forms(D, A, mb, form):
     h = R.Hyper(decay=True, steps_per_update=2, num_updates=4)
     for st in range(2):
         pre = _snap(P, MU, NU, plan.counts, SH)
-        if form == "fused":
-            ops.ppo_minibatch_update(sa, sc, P, batch, st * mb, mb, 0.2, 0.01, 0.5, True, G, metrics, ws, plan, MU, NU, SH)
-        else:
-            ops.ppo_minibatch_grads(sa, sc, P, batch, st * mb, mb, 0.2, 0.01, 0.5, True, G, metrics, ws, precision=ops.STX_PREC_BF16,
-                                    param_arena_bf16=SH, overwrite=True, adam_scratch=plan.scratch)
-            ops.clip_adam_step(plan, P, G, MU, NU, params_bf16=SH, prenorm=True)
+        ops.ppo_minibatch_grads(sa, sc, P, batch, st * mb, mb, 0.2, 0.01, 0.5, True, G, metrics, ws, precision=ops.STX_PREC_BF16,
+                                param_arena_bf16=SH, overwrite=True, adam_scratch=plan.scratch)
+        ops.clip_adam_step(plan, P, G, MU, NU, params_bf16=SH, prenorm=True)
         got = _snap(P, MU, NU, plan.counts, SH, None, plan.gnorm)
         g = G.cpu().numpy()
         want = R.step(pre["p"], pre["mu"], pre["nu"], pre["counts"], g, segs, h, norm=R.NORM_DOUBLE)
@@ -132,7 +129,7 @@ def test_bf16_update_forms(D, A, mb, form):
 # ---------------------------------------------------------------------------------------------------------------------------
 
 
-@pytest.mark.parametrize("precision,fused", [("bf16", False), ("bf16", True), ("f32", False)])
+@pytest.mark.parametrize("precision,fused", [("bf16", False), ("f32", False)])
 def test_learner_optimiser_steps(precision, fused):
     """ff_ppo with one epoch of one minibatch: one optimiser step per update, two updates (the first eager, the second from the
     captured CUDA graph).  The reference takes b1, b2, eps, the learning rates, max_grad_norm and the schedule from the config's
@@ -147,7 +144,7 @@ def test_learner_optimiser_steps(precision, fused):
     E, T = 256, 16
     cfg = compose("default_ff_ppo", ["env=synthetic/box", f"arch.total_num_envs={E}", f"system.rollout_length={T}", "system.epochs=1",
                                      "system.num_minibatches=1", f"arch.total_timesteps={E * T * 2}", "arch.num_evaluation=1",
-                                     f"arch.precision={precision}", f"arch.fused_update={fused}", "logger.use_console=False"])
+                                     f"arch.precision={precision}", "logger.use_console=False"])
     cfg.num_devices, cfg.rank = 1, 0
     cfg = check_total_timesteps(cfg, quiet=True)
     env, _ = make_env.make(cfg)

@@ -378,56 +378,3 @@ def _fused_vs_per_step_rollout(E, T, D, A, nmb):
         for k in a[upd]:
             assert torch.equal(a[upd][k], b[upd][k]), f"update {upd}: trajectory field {k} differs between fused and per-step rollout"
     assert torch.equal(pa, pb)
-
-
-@pytest.mark.parametrize("mb,A,decay", [(1024, 8, True), (4096, 5, False)])
-def test_fused_minibatch_update_matches_two_call_path(mb, A, decay):
-    """stx_ppo_minibatch_update (gradient reduction + clip + Adam in one launch) against
-    stx_ppo_minibatch_grads(overwrite) + stx_clip_adam_step(prenorm): same reduction orders, so parameters,
-    moments, counters and norms agree to fp32 rounding (FMA contraction may differ between the two kernels);
-    three consecutive steps so that the bias correction and the schedule counters advance."""
-    from stoix_b200 import ops
-
-    D, B = 64, 2 * mb
-    rng = np.random.default_rng(mb + A)
-    actor, critic = _net(rng, D, A, 0.3), _net(rng, D, 1, 1.0)
-    sa, sc = ops.MlpSpec((D, 256, 256, A)), ops.MlpSpec((D, 256, 256, 1))
-    _, coff, total = ops.arena_offsets(sa, sc)
-    flat = np.zeros(total, np.float32)
-    flat[: sa.param_count] = actor.flat()
-    flat[coff : coff + sc.param_count] = critic.flat()
-    obs_b = _t(rng.standard_normal((B, D)).astype(np.float32)).to(torch.bfloat16)
-    act = rng.integers(0, A, B).astype(np.int32)
-    batch = ops.PpoBatch(obs_b, _t(act, torch.int32), _t(-rng.random(B).astype(np.float32) - 1.0), _t(rng.standard_normal(B).astype(np.float32)),
-                         _t((rng.standard_normal(B) * 2).astype(np.float32)), _t(rng.standard_normal(B).astype(np.float32)),
-                         adv_stats=_t(np.array([0.1, 0.7])), perm=_t(rng.permutation(B).astype(np.int32), torch.int32))
-    ws = ops.ppo_workspace(sa, sc, mb, ops.STX_PREC_BF16, "cuda:0")
-    segs = [(0, sa.param_count, 3e-3, 0.5), (coff, sc.param_count, 1e-3, 0.05)]  # the critic segment gets clipped
-
-    def run(fused):
-        arena = _t(flat.copy())
-        shadow = ops.cast_bf16(arena)
-        mu, nu = torch.zeros_like(arena), torch.zeros_like(arena)
-        grads, metrics = torch.zeros(total, device="cuda:0"), torch.zeros(8, device="cuda:0")
-        plan = ops.AdamPlan(segs, "cuda:0", decay=decay, steps_per_update=2, num_updates=5)
-        for step in range(3):
-            off = (step % 2) * mb
-            if fused:
-                ops.ppo_minibatch_update(sa, sc, arena, batch, off, mb, 0.2, 0.01, 0.5, True, grads, metrics, ws, plan, mu, nu, shadow)
-            else:
-                ops.ppo_minibatch_grads(sa, sc, arena, batch, off, mb, 0.2, 0.01, 0.5, True, grads, metrics, ws,
-                                        precision=ops.STX_PREC_BF16, param_arena_bf16=shadow, overwrite=True, adam_scratch=plan.scratch)
-                ops.clip_adam_step(plan, arena, grads, mu, nu, params_bf16=shadow, prenorm=True)
-        torch.cuda.synchronize()
-        return [x.float().cpu().numpy() for x in (arena, mu, nu, shadow, grads, metrics, plan.gnorm)] + [plan.counts.cpu().numpy()]
-
-    ref, got = run(False), run(True)
-    np.testing.assert_array_equal(got[7], ref[7])              # counters
-    np.testing.assert_array_equal(got[4], ref[4])              # gradients of the last step: identical reduction
-    np.testing.assert_allclose(got[6], ref[6], rtol=1e-6)      # global norms
-    np.testing.assert_allclose(got[5], ref[5], rtol=1e-5, atol=1e-6)
-    assert ref[6][1] > 0.05, "the test wants the critic segment clipped"
-    for name, g, r in zip(("params", "mu", "nu"), got[:3], ref[:3]):
-        np.testing.assert_allclose(g, r, rtol=2e-5, atol=1e-8, err_msg=name)
-    assert (got[3] != ref[3]).mean() < 1e-3                    # bf16 shadow: at most rare 1-ulp rounding flips
-    assert np.abs(got[0] - flat).max() > 1e-4                  # and the parameters did move
