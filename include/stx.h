@@ -142,8 +142,13 @@ int stx_gae_ppo_f32(const float* reward, const float* v_tm1, const float* v_t, c
                     const uint8_t* truncated, int T, int E, float gamma, float lambda_,
                     float reward_scale, int standardize, float* adv, float* targets, float* stats,
                     void* scratch, void* stream);
-/* Tuning hook for experiments: force the env-quads per block (2, 4 or 8); 0 restores the heuristic. */
-void stx_gae_set_tuning(int quads);
+/* Tuning hook for experiments, process-wide, for stx_gae_ppo_f32, stx_gae_generic_f32, stx_q_lambda_f32 and
+ * stx_lambda_returns_f32.  code: 0 = the default selection; 2, 4, 8 = the scan kernel with that many env-quads
+ * (4 envs each) per block; 416 = the scan kernel with 16 quads per block and two resident blocks per SM;
+ * 500 / 501 = the TMA-pipelined kernel with 32 x 128 / 64 x 64 (envs x steps) tiles, PPO form only: where it
+ * declines (E % 16, alignment) and for the other forms, the default selection runs.  Any non-zero code but
+ * 500 / 501 keeps the TMA kernel off.  Returns STX_E_ARG for any other code, leaving the selection unchanged. */
+int stx_gae_set_tuning(int code);
 /* Generic face of the same function: float discount_t (T,E), optional per-element lambda (NULL ->
  * scalar lambda_), optional float truncation_t (NULL -> zeros).  Same outputs. */
 int stx_gae_generic_f32(const float* r_t, const float* discount_t, const float* lambda_t,

@@ -20,7 +20,7 @@ def bench(T, E, quads=0, iters=20, flush=True):
     tr = (~d) & (torch.rand(T, E, device=dev, generator=g) < 0.002)
     adv, tgt = torch.empty_like(r), torch.empty_like(r)
     flush_buf = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)
-    _lib.load().stx_gae_set_tuning(quads)
+    _lib.check(_lib.load().stx_gae_set_tuning(quads), f"stx_gae_set_tuning({quads})")
     for _ in range(3):
         ops.gae_ppo(r, v, b, d, tr, 0.99, 0.95, 1.0, 1, out=(adv, tgt))
     times = []
@@ -47,7 +47,7 @@ def bench(T, E, quads=0, iters=20, flush=True):
 if __name__ == "__main__":
     out = []
     for (T, E) in [(128, 4096), (128, 32768), (128, 65536), (128, 262144), (128, 1048576), (256, 524288), (128, 4194304)]:
-        for q in (0, 500, 501, 502, 416):   # 0 = the shipped heuristic, 500 / 501 = TMA-pipelined 32x128 / 64x64 tiles, 416 = 2 x 512 threads
+        for q in (0, 500, 501, 416):   # 0 = the shipped heuristic, 500 / 501 = TMA-pipelined 32x128 / 64x64 tiles, 416 = 2 x 512 threads
             for fl in (True,):
                 out.append(bench(T, E, q, flush=fl))
                 print(json.dumps(out[-1]), flush=True)

@@ -12,7 +12,7 @@ r, v, b = (torch.randn(T, E, device=dev) for _ in range(3))
 d = torch.rand(T, E, device=dev) < 0.005
 tr = (~d) & (torch.rand(T, E, device=dev) < 0.002)
 adv, tgt = torch.empty_like(r), torch.empty_like(r)
-_lib.load().stx_gae_set_tuning(quads)
+_lib.check(_lib.load().stx_gae_set_tuning(quads), f"stx_gae_set_tuning({quads})")
 for _ in range(3):
     ops.gae_ppo(r, v, b, d, tr, 0.99, 0.95, 1.0, 1, out=(adv, tgt))
 torch.cuda.synchronize()

@@ -348,7 +348,7 @@ _SIGNATURES = {
     "stx_debug_callfree_math": (C.c_int, [C.c_int, C.c_uint32, C.c_uint32, _P, _P]),
     "stx_mlp_param_count": (C.c_int64, [C.POINTER(StxMlp)]),
     "stx_gae_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int]),
-    "stx_gae_set_tuning": (None, [C.c_int]),
+    "stx_gae_set_tuning": (C.c_int, [C.c_int]),
     "stx_gae_ppo_f32": (C.c_int, [_P, _P, _P, _P, _P, C.c_int, C.c_int, C.c_float, C.c_float, C.c_float, C.c_int, _P, _P, _P, _P, _P]),
     "stx_gae_generic_f32": (C.c_int, [_P, _P, _P, C.c_float, _P, _P, _P, C.c_int, C.c_int, C.c_int, _P, _P, _P, _P, _P]),
     "stx_mlp_forward_workspace_bytes": (C.c_size_t, [C.POINTER(StxMlp), C.c_int64, C.c_int]),

@@ -15,6 +15,8 @@
 #include "stx_common.cuh"
 #include "stx_tc_ptx.cuh"
 
+#include <type_traits>
+
 namespace stx {
 namespace {
 
@@ -27,38 +29,27 @@ struct PpoIn {  // exactly what ff_ppo.py:164-169 feeds
   const float *reward, *v_tm1, *v_t;
   const uint8_t *done, *trunc;
   float gamma, lambda, reward_scale;
+  // one element's map from its inputs; done / trunc are the flag bytes (nonzero: set)
+  __device__ __forceinline__ void map(float r, float vt, float vtm1, uint32_t done_b, uint32_t trunc_b, float& d, float& c) const {
+    const float disc = (1.0f - (done_b ? 1.f : 0.f)) * gamma;      // ff_ppo.py:167-168
+    d = r * reward_scale + disc * vt - vtm1;                       // multistep.py:116
+    c = disc * lambda * (1.0f - (trunc_b ? 1.f : 0.f));            // multistep.py:123
+  }
+  // four adjacent envs: one flag byte per env in fd / ft
+  __device__ __forceinline__ void map4(float4 r, float4 vtm1, float4 vt, uint32_t fd, uint32_t ft, float* d, float* c, float* v) const {
+    const float r4[4] = {r.x, r.y, r.z, r.w}, e4[4] = {vt.x, vt.y, vt.z, vt.w};
+    v[0] = vtm1.x, v[1] = vtm1.y, v[2] = vtm1.z, v[3] = vtm1.w;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) map(r4[k], e4[k], v[k], (fd >> (8 * k)) & 0xffu, (ft >> (8 * k)) & 0xffu, d[k], c[k]);
+  }
   template <int VEC>
   __device__ __forceinline__ void load(int64_t off, float* d, float* c, float* v) const {
-    float r[VEC], vt[VEC], dn[VEC], tr[VEC];
     if constexpr (VEC == 4) {
-      float4 a = ldg_stream4(reward + off), b = ldg_stream4(v_tm1 + off), e = ldg_stream4(v_t + off);
-      uint32_t fd = ldg_stream_u32(done + off), ft = ldg_stream_u32(trunc + off);
-      r[0] = a.x, r[1] = a.y, r[2] = a.z, r[3] = a.w;
-      v[0] = b.x, v[1] = b.y, v[2] = b.z, v[3] = b.w;
-      vt[0] = e.x, vt[1] = e.y, vt[2] = e.z, vt[3] = e.w;
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        dn[k] = ((fd >> (8 * k)) & 0xffu) ? 1.f : 0.f;
-        tr[k] = ((ft >> (8 * k)) & 0xffu) ? 1.f : 0.f;
-      }
-    } else if constexpr (VEC == 2) {
-      float2 a = ldg_stream2(reward + off), b = ldg_stream2(v_tm1 + off), e = ldg_stream2(v_t + off);
-      uint32_t fd = ldg_stream_u16(done + off), ft = ldg_stream_u16(trunc + off);
-      r[0] = a.x, r[1] = a.y, v[0] = b.x, v[1] = b.y, vt[0] = e.x, vt[1] = e.y;
-#pragma unroll
-      for (int k = 0; k < 2; ++k) {
-        dn[k] = ((fd >> (8 * k)) & 0xffu) ? 1.f : 0.f;
-        tr[k] = ((ft >> (8 * k)) & 0xffu) ? 1.f : 0.f;
-      }
+      map4(ldg_stream4(reward + off), ldg_stream4(v_tm1 + off), ldg_stream4(v_t + off), ldg_stream_u32(done + off),
+           ldg_stream_u32(trunc + off), d, c, v);
     } else {
-      r[0] = __ldg(reward + off), v[0] = __ldg(v_tm1 + off), vt[0] = __ldg(v_t + off);
-      dn[0] = __ldg(done + off) ? 1.f : 0.f, tr[0] = __ldg(trunc + off) ? 1.f : 0.f;
-    }
-#pragma unroll
-    for (int k = 0; k < VEC; ++k) {
-      const float disc = (1.0f - dn[k]) * gamma;                      // ff_ppo.py:167-168
-      d[k] = r[k] * reward_scale + disc * vt[k] - v[k];               // multistep.py:116
-      c[k] = disc * lambda * (1.0f - tr[k]);                          // multistep.py:123
+      v[0] = __ldg(v_tm1 + off);
+      map(__ldg(reward + off), __ldg(v_t + off), v[0], __ldg(done + off), __ldg(trunc + off), d[0], c[0]);
     }
   }
 };
@@ -113,6 +104,117 @@ struct LambdaIn {
   }
 };
 
+// ---- the scan steps both kernels run -----------------------------------------------------------------------------------
+// A block covers W - 1 envs x 32 chunks of kL timesteps; the thread of chunk `chunk` owns VEC envs from column `col`.  sA / sB
+// are padded to W = envs + 1 columns.
+
+// Local reverse scan of the thread's kL x VEC maps: step j's acc is b[j] + a[j] * (acc entering the chunk); the chunk's whole
+// map (a[0], b[0]) goes to sA / sB.
+template <int kL, int VEC, int W>
+__device__ __forceinline__ void scan_chunk(const float (&d)[kL][VEC], const float (&c)[kL][VEC], float (&a)[kL][VEC], float (&b)[kL][VEC],
+                                           float (&sA)[kChunks][W], float (&sB)[kChunks][W], int chunk, int col) {
+#pragma unroll
+  for (int k = 0; k < VEC; ++k) {
+    float rb = 0.f, ra = 1.f;
+#pragma unroll
+    for (int j = kL - 1; j >= 0; --j) {
+      rb = fmaf(c[j][k], rb, d[j][k]);
+      ra = c[j][k] * ra;
+      b[j][k] = rb;
+      a[j][k] = ra;
+    }
+    sA[chunk][col + k] = ra;
+    sB[chunk][col + k] = rb;
+  }
+}
+
+// Suffix composition over the 32 chunks of each env: warp w owns envs w*VEC .. w*VEC+VEC-1, lane = chunk index.  Leaves the acc
+// entering each chunk in sA and the acc entering the previous (earlier) segment in sCarry.
+template <int VEC, int W>
+__device__ __forceinline__ void compose_chunks(float (&sA)[kChunks][W], const float (&sB)[kChunks][W], float* sCarry, int lane, int warp) {
+#pragma unroll
+  for (int k = 0; k < VEC; ++k) {
+    const int env = warp * VEC + k;
+    float A = sA[lane][env], B = sB[lane][env];
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      const float A2 = __shfl_down_sync(0xffffffffu, A, off);
+      const float B2 = __shfl_down_sync(0xffffffffu, B, off);
+      if (lane + off < 32) {
+        B = fmaf(A, B2, B);
+        A = A * A2;
+      }
+    }
+    const float carry = sCarry[env];
+    const float Ae = __shfl_down_sync(0xffffffffu, A, 1), Be = __shfl_down_sync(0xffffffffu, B, 1);
+    sA[lane][env] = (lane == 31) ? carry : fmaf(Ae, carry, Be);  // acc entering this chunk
+    __syncwarp();
+    if (lane == 0) sCarry[env] = fmaf(A, carry, B);  // acc entering the previous (earlier) segment
+  }
+}
+
+template <int VEC>
+__device__ __forceinline__ void store_row(float* p, const float* x) {
+  if constexpr (VEC == 4)
+    stg_stream4(p, make_float4(x[0], x[1], x[2], x[3]));
+  else
+    p[0] = x[0];
+}
+
+// The chunk's results from the acc entering it (sA): the advantages, the targets and their statistics' per-thread sums, or the
+// targets alone (kTargetsOnly).
+template <bool kTargetsOnly, int kL, int VEC, int W>
+__device__ __forceinline__ void store_chunk(const float (&a)[kL][VEC], const float (&b)[kL][VEC], const float (&v)[kL][VEC],
+                                            const float (&sA)[kChunks][W], int chunk, int col, int tbase, int T, int E, int e0,
+                                            bool env_ok, float* __restrict__ adv, float* __restrict__ tgt, float& lsum, float& lsq) {
+#pragma unroll
+  for (int j = 0; j < kL; ++j) {
+    const int t = tbase + j;
+    float av[VEC], tv[VEC];
+#pragma unroll
+    for (int k = 0; k < VEC; ++k) {
+      av[k] = fmaf(a[j][k], sA[chunk][col + k], b[j][k]);
+      tv[k] = v[j][k] + av[k];  // multistep.py:132: targets use the un-standardised advantage
+    }
+    if (env_ok && t < T) {
+      const int64_t off = (int64_t)t * E + e0;
+      if constexpr (kTargetsOnly) {
+        store_row<VEC>(tgt + off, av);
+      } else {
+        store_row<VEC>(adv + off, av);
+        store_row<VEC>(tgt + off, tv);
+#pragma unroll
+        for (int k = 0; k < VEC; ++k) lsum += av[k], lsq = fmaf(av[k], av[k], lsq);
+      }
+    }
+  }
+}
+
+// Advantage statistics: each block's fp64 sums to partials; the last block to arrive adds them up in block order and writes
+// stats = [mean, rstd].
+__device__ __forceinline__ void finish_stats(float lsum, float lsq, double* sRed, double2* __restrict__ partials, unsigned int* counter,
+                                             float* __restrict__ stats, int T, int E) {
+  const double bs = block_sum<double>((double)lsum, sRed);
+  const double bq = block_sum<double>((double)lsq, sRed);
+  if (threadIdx.x == 0) partials[blockIdx.x] = make_double2(bs, bq);
+  if (last_block_ticket(counter, gridDim.x)) {
+    double s = 0.0, q2 = 0.0;
+    for (unsigned int i = threadIdx.x; i < gridDim.x; i += blockDim.x) {
+      const double2 p = partials[i];
+      s += p.x, q2 += p.y;
+    }
+    s = block_sum<double>(s, sRed);
+    q2 = block_sum<double>(q2, sRed);
+    if (threadIdx.x == 0) {
+      const double n = (double)T * (double)E;
+      const double mean = s / n;
+      const double var = q2 / n - mean * mean;  // jax.nn.standardize: E[x^2] - E[x]^2
+      stats[0] = (float)mean;
+      stats[1] = (float)(1.0 / sqrt(var + 1e-5));
+    }
+  }
+}
+
 // MINB: resident blocks per SM the register allocation must allow.  A block runs load -> barrier -> scan -> barrier ->
 // store with nothing overlapped inside it, so HBM only stays busy if ANOTHER block of the same SM is in its load phase
 // meanwhile: the saturating shapes use 2 x 512 threads (<= 64 registers) instead of 1 x 1024.
@@ -148,100 +250,14 @@ __global__ void __launch_bounds__(QUADS* kChunks, MINB)
         for (int k = 0; k < VEC; ++k) d[j][k] = 0.f, c[j][k] = 1.f, v[j][k] = 0.f;  // identity map
       }
     }
-    // local reverse scan: adv[j] = b[j] + a[j] * acc_in
     float a[kL][VEC], b[kL][VEC];
-#pragma unroll
-    for (int k = 0; k < VEC; ++k) {
-      float rb = 0.f, ra = 1.f;
-#pragma unroll
-      for (int j = kL - 1; j >= 0; --j) {
-        rb = fmaf(c[j][k], rb, d[j][k]);
-        ra = c[j][k] * ra;
-        b[j][k] = rb;
-        a[j][k] = ra;
-      }
-      sA[chunk][q * VEC + k] = ra;
-      sB[chunk][q * VEC + k] = rb;
-    }
+    scan_chunk(d, c, a, b, sA, sB, chunk, q * VEC);
     __syncthreads();
-    // suffix composition over the 32 chunks of each env: warp w owns envs w*VEC .. w*VEC+VEC-1
-    // (QUADS warps per block, ENVS = QUADS*VEC), lane = chunk index.
-#pragma unroll
-    for (int k = 0; k < VEC; ++k) {
-      const int env = warp * VEC + k;
-      float A = sA[lane][env], B = sB[lane][env];
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const float A2 = __shfl_down_sync(0xffffffffu, A, off);
-        const float B2 = __shfl_down_sync(0xffffffffu, B, off);
-        if (lane + off < 32) {
-          B = fmaf(A, B2, B);
-          A = A * A2;
-        }
-      }
-      const float carry = sCarry[env];
-      const float Ae = __shfl_down_sync(0xffffffffu, A, 1), Be = __shfl_down_sync(0xffffffffu, B, 1);
-      sA[lane][env] = (lane == 31) ? carry : fmaf(Ae, carry, Be);  // acc entering this chunk
-      __syncwarp();
-      if (lane == 0) sCarry[env] = fmaf(A, carry, B);  // acc entering the previous (earlier) segment
-    }
+    compose_chunks<VEC>(sA, sB, sCarry, lane, warp);
     __syncthreads();
-#pragma unroll
-    for (int j = 0; j < kL; ++j) {
-      const int t = tbase + j;
-      float av[VEC], tv[VEC];
-#pragma unroll
-      for (int k = 0; k < VEC; ++k) {
-        av[k] = fmaf(a[j][k], sA[chunk][q * VEC + k], b[j][k]);
-        tv[k] = v[j][k] + av[k];  // multistep.py:132: targets use the un-standardised advantage
-      }
-      if constexpr (In::kTargetsOnly) {
-        if (env_ok && t < T) {
-          const int64_t off = (int64_t)t * E + e0;
-          if constexpr (VEC == 4)
-            stg_stream4(tgt + off, make_float4(av[0], av[1], av[2], av[3]));
-          else if constexpr (VEC == 2)
-            stg_stream2(tgt + off, make_float2(av[0], av[1]));
-          else
-            tgt[off] = av[0];
-        }
-      } else if (env_ok && t < T) {
-        const int64_t off = (int64_t)t * E + e0;
-        if constexpr (VEC == 4) {
-          stg_stream4(adv + off, make_float4(av[0], av[1], av[2], av[3]));
-          stg_stream4(tgt + off, make_float4(tv[0], tv[1], tv[2], tv[3]));
-        } else if constexpr (VEC == 2) {
-          stg_stream2(adv + off, make_float2(av[0], av[1]));
-          stg_stream2(tgt + off, make_float2(tv[0], tv[1]));
-        } else {
-          adv[off] = av[0];
-          tgt[off] = tv[0];
-        }
-#pragma unroll
-        for (int k = 0; k < VEC; ++k) lsum += av[k], lsq = fmaf(av[k], av[k], lsq);
-      }
-    }
+    store_chunk<In::kTargetsOnly>(a, b, v, sA, chunk, q * VEC, tbase, T, E, e0, env_ok, adv, tgt, lsum, lsq);
   }
-  if (!want_stats) return;
-  const double bs = block_sum<double>((double)lsum, sRed);
-  const double bq = block_sum<double>((double)lsq, sRed);
-  if (threadIdx.x == 0) partials[blockIdx.x] = make_double2(bs, bq);
-  if (last_block_ticket(counter, gridDim.x)) {
-    double s = 0.0, q2 = 0.0;
-    for (unsigned int i = threadIdx.x; i < gridDim.x; i += blockDim.x) {
-      const double2 p = partials[i];
-      s += p.x, q2 += p.y;
-    }
-    s = block_sum<double>(s, sRed);
-    q2 = block_sum<double>(q2, sRed);
-    if (threadIdx.x == 0) {
-      const double n = (double)T * (double)E;
-      const double mean = s / n;
-      const double var = q2 / n - mean * mean;  // jax.nn.standardize: E[x^2] - E[x]^2
-      stats[0] = (float)mean;
-      stats[1] = (float)(1.0 / sqrt(var + 1e-5));
-    }
-  }
+  if (want_stats) finish_stats(lsum, lsq, sRed, partials, counter, stats, T, E);
 }
 
 __global__ void standardize_inplace_kernel(float* __restrict__ adv, int64_t n,
@@ -254,10 +270,10 @@ __global__ void standardize_inplace_kernel(float* __restrict__ adv, int64_t n,
 
 // ---- TMA-pipelined form for the saturating shapes (PPO inputs) -------------------------------------------------------
 // gae_scan_kernel runs load -> barrier -> scan -> barrier -> store per block with nothing overlapped inside it; two resident
-// blocks per SM hide part of that (0.69 of the copy peak).  Here ONE persistent 256-thread block per SM walks its env tiles
-// (32 envs x 128 timesteps, 5 arrays = 56 KB) through a 3-stage shared-memory ring filled by TMA (one 2-D box per array and
+// blocks per SM hide part of that (0.69 of the copy peak).  Here ONE persistent block per SM walks its env tiles
+// (kGE envs x kGT timesteps, 5 arrays = 56 KB) through a 3-stage shared-memory ring filled by TMA (one 2-D box per array and
 // stage, one mbarrier per stage): the loads of the next two tiles are in flight while the current one is scanned and stored,
-// so the HBM read stream never stops.  The arithmetic is the code above, reading its inputs from shared memory.
+// so the HBM read stream never stops.  The arithmetic is the scan steps above, reading the inputs from shared memory.
 // Tile shapes: 32 envs x 128 timesteps (4 timesteps per thread, the association order of gae_scan_kernel) or 64 x 64 (2 per
 // thread, two segments per 128-step rollout): half as many distinct rows -- hence 2 MB pages -- in flight per tile, which is what
 // matters once the row pitch E * 4 B exceeds the page size .
@@ -272,9 +288,9 @@ constexpr uint32_t kGaeSmemBytes = kGStages * (3 * 128 * 32 * 4 + 2 * 128 * 32) 
 template <int kGE, int kGT>
 __global__ void __launch_bounds__(kGE / 4 * kChunks, 1)
     gae_tma_kernel(const __grid_constant__ CUtensorMap m_r, const __grid_constant__ CUtensorMap m_v, const __grid_constant__ CUtensorMap m_vt,
-                   const __grid_constant__ CUtensorMap m_dn, const __grid_constant__ CUtensorMap m_tr, float gamma, float lambda,
-                   float reward_scale, int T, int E, float* __restrict__ adv, float* __restrict__ tgt, int want_stats,
-                   double2* __restrict__ partials, unsigned int* counter, float* __restrict__ stats) {
+                   const __grid_constant__ CUtensorMap m_dn, const __grid_constant__ CUtensorMap m_tr, PpoIn in, int T, int E,
+                   float* __restrict__ adv, float* __restrict__ tgt, int want_stats, double2* __restrict__ partials, unsigned int* counter,
+                   float* __restrict__ stats) {
   using namespace tc;
   using GaeStage = GaeStageT<kGE, kGT>;
   static_assert(sizeof(GaeStage) * kGStages + 1024 == kGaeSmemBytes, "stage layout");
@@ -315,106 +331,34 @@ __global__ void __launch_bounds__(kGE / 4 * kChunks, 1)
     const int seg = nseg - 1 - (int)(k % nseg);
     const int e0 = ((int)blockIdx.x + (int)(k / nseg) * (int)gridDim.x) * kGE + q * VEC;
     const bool env_ok = e0 < E;
-    const int tbase = seg * kGT + chunk * kL, rbase = chunk * kL;
+    const int tbase = seg * kGT + chunk * kL, rbase = chunk * kL, col = q * VEC;
     if (seg == nseg - 1 && threadIdx.x < kGE) sCarry[threadIdx.x] = 0.f;  // multistep.py:127: acc starts at zero (read after the barrier below)
     const GaeStage& st = stages[k % kGStages];
     mbar_wait(&full[k % kGStages], (uint32_t)((k / kGStages) & 1), 900);
     float d[kL][VEC], c[kL][VEC], v[kL][VEC];
 #pragma unroll
     for (int j = 0; j < kL; ++j) {
-      const float4 rr = *reinterpret_cast<const float4*>(&st.r[rbase + j][q * VEC]);
-      const float4 vv = *reinterpret_cast<const float4*>(&st.v[rbase + j][q * VEC]);
-      const float4 ee = *reinterpret_cast<const float4*>(&st.vt[rbase + j][q * VEC]);
-      const uint32_t fd = *reinterpret_cast<const uint32_t*>(&st.dn[rbase + j][q * VEC]);
-      const uint32_t ft = *reinterpret_cast<const uint32_t*>(&st.tr[rbase + j][q * VEC]);
-      const float r4[4] = {rr.x, rr.y, rr.z, rr.w}, v4[4] = {vv.x, vv.y, vv.z, vv.w}, e4[4] = {ee.x, ee.y, ee.z, ee.w};
-      const bool ok = env_ok && (tbase + j) < T;
+      const int row = rbase + j;
+      in.map4(*reinterpret_cast<const float4*>(&st.r[row][col]), *reinterpret_cast<const float4*>(&st.v[row][col]),
+              *reinterpret_cast<const float4*>(&st.vt[row][col]), *reinterpret_cast<const uint32_t*>(&st.dn[row][col]),
+              *reinterpret_cast<const uint32_t*>(&st.tr[row][col]), d[j], c[j], v[j]);
+      if (!env_ok || tbase + j >= T) {
 #pragma unroll
-      for (int kk = 0; kk < VEC; ++kk) {
-        const float dn = ((fd >> (8 * kk)) & 0xffu) ? 1.f : 0.f, tr = ((ft >> (8 * kk)) & 0xffu) ? 1.f : 0.f;
-        const float disc = (1.0f - dn) * gamma;                                   // ff_ppo.py:167-168
-        d[j][kk] = ok ? r4[kk] * reward_scale + disc * e4[kk] - v4[kk] : 0.f;     // multistep.py:116
-        c[j][kk] = ok ? disc * lambda * (1.0f - tr) : 1.f;                        // multistep.py:123 (identity map outside the array)
-        v[j][kk] = v4[kk];
+        for (int kk = 0; kk < VEC; ++kk) d[j][kk] = 0.f, c[j][kk] = 1.f;  // identity map outside the array
       }
     }
     float a[kL][VEC], b[kL][VEC];
-#pragma unroll
-    for (int kk = 0; kk < VEC; ++kk) {
-      float rb = 0.f, ra = 1.f;
-#pragma unroll
-      for (int j = kL - 1; j >= 0; --j) {
-        rb = fmaf(c[j][kk], rb, d[j][kk]);
-        ra = c[j][kk] * ra;
-        b[j][kk] = rb;
-        a[j][kk] = ra;
-      }
-      sA[chunk][q * VEC + kk] = ra;
-      sB[chunk][q * VEC + kk] = rb;
-    }
+    scan_chunk(d, c, a, b, sA, sB, chunk, col);
     __syncthreads();  // every thread has consumed this stage: refill it with the tile three items ahead
     if (threadIdx.x == 0 && k + kGStages < my_items) issue(k + kGStages);
-#pragma unroll
-    for (int kk = 0; kk < VEC; ++kk) {  // suffix composition over the 32 chunks of each env: warp w owns envs w*VEC .. +VEC-1, lane = chunk
-      const int env = warp * VEC + kk;
-      float A = sA[lane][env], B = sB[lane][env];
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const float A2 = __shfl_down_sync(0xffffffffu, A, off);
-        const float B2 = __shfl_down_sync(0xffffffffu, B, off);
-        if (lane + off < 32) {
-          B = fmaf(A, B2, B);
-          A = A * A2;
-        }
-      }
-      const float carry = sCarry[env];
-      const float Ae = __shfl_down_sync(0xffffffffu, A, 1), Be = __shfl_down_sync(0xffffffffu, B, 1);
-      sA[lane][env] = (lane == 31) ? carry : fmaf(Ae, carry, Be);  // acc entering this chunk
-      __syncwarp();
-      if (lane == 0) sCarry[env] = fmaf(A, carry, B);              // acc entering the previous (earlier) segment
-    }
+    compose_chunks<VEC>(sA, sB, sCarry, lane, warp);
     __syncthreads();
-#pragma unroll
-    for (int j = 0; j < kL; ++j) {
-      const int t = tbase + j;
-      float av[VEC], tv[VEC];
-#pragma unroll
-      for (int kk = 0; kk < VEC; ++kk) {
-        av[kk] = fmaf(a[j][kk], sA[chunk][q * VEC + kk], b[j][kk]);
-        tv[kk] = v[j][kk] + av[kk];  // multistep.py:132: targets use the un-standardised advantage
-      }
-      if (env_ok && t < T) {
-        const int64_t off = (int64_t)t * E + e0;
-        stg_stream4(adv + off, make_float4(av[0], av[1], av[2], av[3]));
-        stg_stream4(tgt + off, make_float4(tv[0], tv[1], tv[2], tv[3]));
-#pragma unroll
-        for (int kk = 0; kk < VEC; ++kk) lsum += av[kk], lsq = fmaf(av[kk], av[kk], lsq);
-      }
-    }
+    store_chunk<false>(a, b, v, sA, chunk, col, tbase, T, E, e0, env_ok, adv, tgt, lsum, lsq);
   }
-  if (!want_stats) return;
-  const double bs = block_sum<double>((double)lsum, sRed);
-  const double bq = block_sum<double>((double)lsq, sRed);
-  if (threadIdx.x == 0) partials[blockIdx.x] = make_double2(bs, bq);
-  if (last_block_ticket(counter, gridDim.x)) {
-    double s = 0.0, q2 = 0.0;
-    for (unsigned int i = threadIdx.x; i < gridDim.x; i += blockDim.x) {
-      const double2 pp = partials[i];
-      s += pp.x, q2 += pp.y;
-    }
-    s = block_sum<double>(s, sRed);
-    q2 = block_sum<double>(q2, sRed);
-    if (threadIdx.x == 0) {
-      const double n = (double)T * (double)E;
-      const double mean = s / n;
-      const double var = q2 / n - mean * mean;  // jax.nn.standardize: E[x^2] - E[x]^2
-      stats[0] = (float)mean;
-      stats[1] = (float)(1.0 / sqrt(var + 1e-5));
-    }
-  }
+  if (want_stats) finish_stats(lsum, lsq, sRed, partials, counter, stats, T, E);
 }
 
-int g_quads_override = 0;
+int g_tuning = 0;  // stx_gae_set_tuning's code
 
 typedef CUresult (*GaeEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
                                 const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -482,8 +426,8 @@ int launch_gae_tma_shape(const PpoIn& in, int T, int E, int want, float* adv, fl
   if (int rc = tc::use_trap_record(st)) return rc;
   const int n_tiles = (E + kGE - 1) / kGE;
   const int grid = n_tiles < kNumSMs ? n_tiles : kNumSMs;
-  gae_tma_kernel<kGE, kGT><<<grid, kGE / 4 * kChunks, kGaeSmemBytes, st>>>(mr, mv, mvt, mdn, mtr, in.gamma, in.lambda, in.reward_scale, T, E, adv, tgt,
-                                                                           want, partials, counter, stats);
+  gae_tma_kernel<kGE, kGT><<<grid, kGE / 4 * kChunks, kGaeSmemBytes, st>>>(mr, mv, mvt, mdn, mtr, in, T, E, adv, tgt, want, partials, counter,
+                                                                           stats);
   STX_LAUNCH_OK();
   return STX_OK;
 }
@@ -491,14 +435,11 @@ int launch_gae_tma(const PpoIn& in, int T, int E, int want, float* adv, float* t
                    cudaStream_t st) {
   if (E % 16 != 0 || !aligned16(in.done) || !aligned16(in.trunc)) return 1;  // TMA: 16-byte aligned rows of the byte arrays
   // 32 x 128 tiles up to E = 32768, 64 x 64 from E = 65536: once the row pitch exceeds the page size, 64 x 64 tiles halve the
-  // rows (pages) in flight per tile; code 502 = 128 x 32 tiles
-  if (g_quads_override == 502) return launch_gae_tma_shape<128, 32>(in, T, E, want, adv, tgt, stats, partials, counter, st);
-  const bool wide = g_quads_override == 501 || (g_quads_override != 500 && E >= 65536);
+  // rows (pages) in flight per tile
+  const bool wide = g_tuning == 501 || (g_tuning != 500 && E >= 65536);
   return wide ? launch_gae_tma_shape<64, 64>(in, T, E, want, adv, tgt, stats, partials, counter, st)
               : launch_gae_tma_shape<32, 128>(in, T, E, want, adv, tgt, stats, partials, counter, st);
 }
-int launch_gae_tma(const GenericIn&, int, int, int, float*, float*, float*, double2*, unsigned int*, cudaStream_t) { return 1; }
-int launch_gae_tma(const LambdaIn&, int, int, int, float*, float*, float*, double2*, unsigned int*, cudaStream_t) { return 1; }
 
 template <class In>
 int launch_gae(const In& in, int T, int E, bool vec4, int standardize, float* adv, float* tgt,
@@ -507,52 +448,26 @@ int launch_gae(const In& in, int T, int E, bool vec4, int standardize, float* ad
   unsigned int* counter = reinterpret_cast<unsigned int*>(scratch);
   double2* partials = scratch ? reinterpret_cast<double2*>(reinterpret_cast<char*>(scratch) + 16) : nullptr;
   const int want = standardize != 0;
-  bool done_tma = false;
-  // large shapes: the TMA-pipelined persistent kernel (codes 500 / 501 force its 32x128 / 64x64 tiles, any other non-zero code disables it)
-  if (vec4 && (g_quads_override == 500 || g_quads_override == 501 || g_quads_override == 502 || (g_quads_override == 0 && E >= 32768))) {
-    const int rc = launch_gae_tma(in, T, E, want, adv, tgt, stats, partials, counter, st);
-    if (rc < 0) return rc;
-    done_tma = rc == STX_OK;
+  int rc = 1;  // STX_OK once the TMA kernel has run; 1 while it has not
+  // large PPO shapes: the TMA-pipelined persistent kernel (codes 500 / 501 force its 32x128 / 64x64 tiles, any other non-zero
+  // code disables it; where it declines, the 5xx codes take the default selection below)
+  if constexpr (std::is_same_v<In, PpoIn>) {
+    if (vec4 && (g_tuning == 500 || g_tuning == 501 || (g_tuning == 0 && E >= 32768)))
+      rc = launch_gae_tma(in, T, E, want, adv, tgt, stats, partials, counter, st);
   }
-  if (done_tma) {
-  } else if (vec4 && (g_quads_override / 100 == 4 || (g_quads_override == 0 && E / 4 >= 65536))) {
-    // several resident blocks per SM (code 4xx; the default for saturating shapes): 416 = 2 x 512 threads, 408 = 4 x 256
-    const int quads = g_quads_override == 0 ? 16 : g_quads_override % 100, total = E / 4;
-    const int grid = (total + quads - 1) / quads;
-    if (quads == 16)
-      gae_scan_kernel<In, 4, 16, 4, 2><<<grid, 16 * kChunks, 0, st>>>(in, T, E, adv, tgt, want, partials, counter, stats);
-    else
-      gae_scan_kernel<In, 4, 8, 4, 4><<<grid, 8 * kChunks, 0, st>>>(in, T, E, adv, tgt, want, partials, counter, stats);
-  } else if (vec4 && g_quads_override / 100 == 3) {  // L = 2 timesteps per thread (fewer registers, more resident blocks): code 3xx
-    const int quads = g_quads_override % 100, total = E / 4;
-    const int grid = (total + quads - 1) / quads;
-    if (quads == 32)
-      gae_scan_kernel<In, 4, 32, 2><<<grid, 32 * kChunks, 0, st>>>(in, T, E, adv, tgt, want, partials, counter, stats);
-    else if (quads == 16)
-      gae_scan_kernel<In, 4, 16, 2><<<grid, 16 * kChunks, 0, st>>>(in, T, E, adv, tgt, want, partials, counter, stats);
-    else
-      gae_scan_kernel<In, 4, 8, 2><<<grid, 8 * kChunks, 0, st>>>(in, T, E, adv, tgt, want, partials, counter, stats);
-  } else if (vec4 && g_quads_override / 100 == 2) {  // experimental float2 variants: tuning code 2xx
-    const int groups = g_quads_override % 100, total = E / 2;
-    const int grid = (total + groups - 1) / groups;
-    if (groups == 32)
-      gae_scan_kernel<In, 2, 32><<<grid, 32 * kChunks, 0, st>>>(in, T, E, adv, tgt, want, partials, counter, stats);
-    else
-      gae_scan_kernel<In, 2, 16><<<grid, 16 * kChunks, 0, st>>>(in, T, E, adv, tgt, want, partials, counter, stats);
+  if (rc < 0) return rc;
+  const bool forced_quads = g_tuning == 2 || g_tuning == 4 || g_tuning == 8;
+  if (rc == STX_OK) {
+  } else if (vec4 && (g_tuning == 416 || (!forced_quads && E / 4 >= 65536))) {
+    // saturating shapes: two resident 512-thread blocks per SM (code 416)
+    const int grid = (E / 4 + 15) / 16;
+    gae_scan_kernel<In, 4, 16, 4, 2><<<grid, 16 * kChunks, 0, st>>>(in, T, E, adv, tgt, want, partials, counter, stats);
   } else if (vec4) {
+    // Small E is latency-bound: more, smaller blocks; wider rows per block once the grid is large.  Codes 2, 4, 8 force the quads.
     const int quads_total = E / 4;
-    // Small E is latency-bound: more, smaller blocks.  Large E: 128-byte rows per warp access.
-    // wider rows per block once the grid is large
-    int quads = quads_total >= 65536 ? 32 : (quads_total >= 8 * kNumSMs * 2 ? 8 : (quads_total >= 4 * kNumSMs ? 4 : 2));
-    if (g_quads_override == 2 || g_quads_override == 4 || g_quads_override == 8 || g_quads_override == 16 ||
-        g_quads_override == 32)
-      quads = g_quads_override;
+    const int quads = forced_quads ? g_tuning : (quads_total >= 8 * kNumSMs * 2 ? 8 : (quads_total >= 4 * kNumSMs ? 4 : 2));
     const int grid = (quads_total + quads - 1) / quads;
-    if (quads == 32)
-      gae_scan_kernel<In, 4, 32><<<grid, 32 * kChunks, 0, st>>>(in, T, E, adv, tgt, want, partials, counter, stats);
-    else if (quads == 16)
-      gae_scan_kernel<In, 4, 16><<<grid, 16 * kChunks, 0, st>>>(in, T, E, adv, tgt, want, partials, counter, stats);
-    else if (quads == 8)
+    if (quads == 8)
       gae_scan_kernel<In, 4, 8><<<grid, 8 * kChunks, 0, st>>>(in, T, E, adv, tgt, want, partials, counter, stats);
     else if (quads == 4)
       gae_scan_kernel<In, 4, 4><<<grid, 4 * kChunks, 0, st>>>(in, T, E, adv, tgt, want, partials, counter, stats);
@@ -583,7 +498,12 @@ extern "C" size_t stx_gae_scratch_bytes(int T, int E) {
   return 16 + blocks * sizeof(double2);
 }
 
-extern "C" void stx_gae_set_tuning(int quads) { g_quads_override = quads; }
+extern "C" int stx_gae_set_tuning(int code) {
+  STX_REQUIRE(code == 0 || code == 2 || code == 4 || code == 8 || code == 416 || code == 500 || code == 501, STX_E_ARG,
+              "stx_gae_set_tuning: unknown code %d", code);
+  g_tuning = code;
+  return STX_OK;
+}
 
 static int check_common(int T, int E, int standardize, const void* adv, const void* tgt,
                         const void* stats, const void* scratch) {

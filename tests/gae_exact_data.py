@@ -35,9 +35,9 @@ UNIT_LIMIT = 2 ** 24     # fp32 holds every integer below this exactly
 NUM_SMS = 132            # kNumSMs
 CHUNKS = 32              # kChunks
 
-# every value stx_gae_set_tuning is documented to take: 0 = the default selection; 2..32 = gae_scan_kernel<In, 4, quads>;
-# 2xx = float2 loads; 3xx = 2 steps per thread; 4xx = several resident blocks per SM; 5xx = the TMA kernel (PPO form only)
-CODES = (0, 2, 4, 8, 16, 32, 216, 232, 308, 316, 332, 408, 416, 500, 501, 502)
+# every code stx_gae_set_tuning accepts: 0 = the default selection; 2, 4, 8 = gae_scan_kernel<In, 4, quads>; 416 = two resident
+# 512-thread blocks per SM; 500 / 501 = the TMA kernel's 32x128 / 64x64 tiles (PPO form only)
+CODES = (0, 2, 4, 8, 416, 500, 501)
 
 # input form of each face: which In struct of stx_gae.cu the call runs
 FACES = {
@@ -98,34 +98,21 @@ def launch_form(face: str, code: int, E: int, vec4: Optional[bool] = None, tma_a
     """The kernel launch_gae runs.  vec4: E % 4 == 0 and the pointers the entry point checks are 16-byte aligned (default:
     E % 4 == 0); tma_aligned: done / truncated 16-byte aligned (the PPO form's TMA condition besides E % 16)."""
     vec4 = (E % 4 == 0) if vec4 is None else vec4
-    if vec4 and (code in (500, 501, 502) or (code == 0 and E >= 32768)):
-        if FACES[face] == "PpoIn" and E % 16 == 0 and tma_aligned:
-            if code == 502:
-                return Form("tma", 128, 32)
-            wide = code == 501 or (code != 500 and E >= 65536)
-            return Form("tma", 64, 64) if wide else Form("tma", 32, 128)
-    if vec4 and (code // 100 == 4 or (code == 0 and E // 4 >= 65536)):
-        quads = 16 if code == 0 else code % 100
-        return Form("scan", 4, 16, 4, 2) if quads == 16 else Form("scan", 4, 8, 4, 4)
-    if vec4 and code // 100 == 3:
-        quads = code % 100
-        return Form("scan", 4, quads if quads in (32, 16) else 8, 2, 1)
-    if vec4 and code // 100 == 2:
-        return Form("scan", 2, 32 if code % 100 == 32 else 16)
+    if vec4 and FACES[face] == "PpoIn" and (code in (500, 501) or (code == 0 and E >= 32768)) and E % 16 == 0 and tma_aligned:
+        wide = code == 501 or (code != 500 and E >= 65536)
+        return Form("tma", 64, 64) if wide else Form("tma", 32, 128)
+    forced = code in (2, 4, 8)
+    if vec4 and (code == 416 or (not forced and E // 4 >= 65536)):
+        return Form("scan", 4, 16, 4, 2)
     if vec4:
         qt = E // 4
-        quads = 32 if qt >= 65536 else (8 if qt >= 8 * NUM_SMS * 2 else (4 if qt >= 4 * NUM_SMS else 2))
-        if code in (2, 4, 8, 16, 32):
-            quads = code
-        return Form("scan", 4, quads)
+        return Form("scan", 4, code if forced else (8 if qt >= 8 * NUM_SMS * 2 else (4 if qt >= 4 * NUM_SMS else 2)))
     return Form("scan", 1, 16)
 
 
-# the 13 gae_scan_kernel instantiations launch_gae has per input form, and the 3 gae_tma_kernel shapes
-SCAN_FORMS = tuple(Form("scan", *f) for f in ((4, 32, 4, 1), (4, 16, 4, 1), (4, 8, 4, 1), (4, 4, 4, 1), (4, 2, 4, 1), (2, 32, 4, 1),
-                                               (2, 16, 4, 1), (4, 32, 2, 1), (4, 16, 2, 1), (4, 8, 2, 1), (4, 16, 4, 2), (4, 8, 4, 4),
-                                               (1, 16, 4, 1)))
-TMA_FORMS = (Form("tma", 32, 128), Form("tma", 64, 64), Form("tma", 128, 32))
+# the 5 gae_scan_kernel instantiations launch_gae has per input form, and the 2 gae_tma_kernel shapes
+SCAN_FORMS = tuple(Form("scan", *f) for f in ((4, 16, 4, 2), (4, 8, 4, 1), (4, 4, 4, 1), (4, 2, 4, 1), (1, 16, 4, 1)))
+TMA_FORMS = (Form("tma", 32, 128), Form("tma", 64, 64))
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -60,12 +60,13 @@ def test_host_mirror_matches_launch_gae():
     assert [f("gae_generic", 0, E) for E in (32768, 262140, 262144)] == ["scan<4,8,4,1>", "scan<4,8,4,1>", "scan<4,16,4,2>"]
     assert f("gae_ppo", 0, 37) == f("gae_ppo", 416, 48, vec4=False) == f("q_lambda", 500, 64, vec4=False) == "scan<1,16,4,1>"
     # forced codes; the 5xx codes fall back to the default selection where TMA declines
-    assert [f("gae_ppo", c, 1024) for c in (216, 232, 308, 316, 332, 408, 416, 500, 501, 502)] == [
-        "scan<2,16,4,1>", "scan<2,32,4,1>", "scan<4,8,2,1>", "scan<4,16,2,1>", "scan<4,32,2,1>", "scan<4,8,4,4>", "scan<4,16,4,2>",
-        "tma<32,128>", "tma<64,64>", "tma<128,32>"]
-    assert [f("gae_ppo", c, 1028) for c in (500, 501, 502)] == ["scan<4,2,4,1>"] * 3
+    assert [f("gae_ppo", c, 1024) for c in (2, 4, 8, 416, 500, 501)] == [
+        "scan<4,2,4,1>", "scan<4,4,4,1>", "scan<4,8,4,1>", "scan<4,16,4,2>", "tma<32,128>", "tma<64,64>"]
+    assert [f("gae_ppo", c, 1028) for c in (500, 501)] == ["scan<4,2,4,1>"] * 2
     assert f("gae_ppo", 500, 1024, tma_aligned=False) == "scan<4,2,4,1>"
-    assert [f(face, 502, 1024) for face in ("gae_generic", "q_lambda", "lambda_returns")] == ["scan<4,2,4,1>"] * 3
+    assert [f(face, 501, 1024) for face in ("gae_generic", "q_lambda", "lambda_returns")] == ["scan<4,2,4,1>"] * 3
+    assert f("gae_ppo", 500, 262148) == f("gae_generic", 501, 262144) == "scan<4,16,4,2>"
+    assert [f("gae_generic", c, 262144) for c in (2, 4, 8)] == ["scan<4,2,4,1>", "scan<4,4,4,1>", "scan<4,8,4,1>"]
 
 
 def test_cases_reach_every_form():
@@ -94,6 +95,6 @@ def test_cases_reach_every_form():
         assert any(E % fm.a and T > fm.b and T % fm.b for _, T, E in runs), f"{fm.name}: never ragged in both E and T"
         assert any(-(-E // fm.a) > X.NUM_SMS for _, _, E in runs), f"{fm.name}: never several tiles per block"
     # the fallback: a 5xx code (or the default at E >= 32768) whose TMA declines because E % 16 != 0
-    assert any(X.launch_form("gae_ppo", c, E).kind == "scan" and E % 4 == 0 and E % 16 for c in (500, 501, 502)
+    assert any(X.launch_form("gae_ppo", c, E).kind == "scan" and E % 4 == 0 and E % 16 for c in (500, 501)
                for _, E in X.SHAPES)
     assert X.launch_form("gae_ppo", 0, 32772).name == "scan<4,8,4,1>" and X.launch_form("gae_ppo", 0, 262148).name == "scan<4,16,4,2>"

@@ -8,7 +8,7 @@ B. Statistics: standardize 1 and 2 on the PPO and generic forms, every code: `st
 C. Real-valued data (gamma 0.99, lambda 0.95, random flags, a random lambda array) at the multi-segment and ragged shapes:
    rtol / atol 1e-5 (BASELINE.md section 4); NaN and -inf entries in q_t follow jnp.max; two identical calls are equal.
 D. The default selection at the sizes where it picks its other paths, unaligned views, and the tuning-code -> kernel mapping
-   seen by the profiler.
+   seen by the profiler, codes outside the accepted set refused.
 """
 import ctypes
 import re
@@ -272,21 +272,26 @@ def _kernel_form(name):
     return None
 
 
+STX_E_ARG = -1              # include/stx.h
+REJECTED = (16, 308, 502)   # codes of launch forms K2 does not have: 16 quads, 2 steps per thread, 128 x 32 TMA tiles
+
+
 @pytest.mark.parametrize("face", ["gae_ppo", "gae_generic", "q_lambda", "lambda_returns"])
 def test_codes_launch_the_mirrored_kernels(face, tuning):
     """The kernel each tuning code launches, as the profiler names it, is the one launch_form (the mapping the tests above
-    rely on) says: every code at E = 48 (TMA-eligible for the PPO form), code 0 at E = 37 (VEC = 1)."""
+    rely on) says: every code at E = 48 (TMA-eligible for the PPO form), code 0 at E = 37 (VEC = 1).  A code outside
+    X.CODES is refused with STX_E_ARG and leaves the default selection in place for the next call."""
     from torch.autograd import DeviceType
     from torch.profiler import ProfilerActivity, profile
 
-    runs = [(code, 4, 48) for code in X.CODES] + [(0, 4, 37)]
+    runs = [(code, 4, 48) for code in X.CODES + REJECTED] + [(0, 4, 37)]
     cases = [(code, X.make_case(face, T, E)) for code, T, E in runs]
     for _, case in cases:
         _dev(case)
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         for code, case in cases:
-            tuning(code)
+            assert tuning(code) == (0 if code in X.CODES else STX_E_ARG), f"stx_gae_set_tuning({code})"
             _run(case)
             tuning(0)
             torch.cuda.synchronize()
@@ -294,5 +299,5 @@ def test_codes_launch_the_mirrored_kernels(face, tuning):
                      key=lambda e: e.time_range.start)
     got = [_kernel_form(e.name) for e in kernels]
     assert None not in got, f"unrecognised kernel names: {[e.name for e in kernels]}"
-    want = [(X.FACES[face], X.launch_form(face, code, case.E).name) for code, case in cases]
+    want = [(X.FACES[face], X.launch_form(face, code if code in X.CODES else 0, case.E).name) for code, case in cases]
     assert got == want, "\n".join(f"code {c} E={cs.E}: launched {g}, mirror {w}" for (c, cs), g, w in zip(cases, got, want) if g != w)

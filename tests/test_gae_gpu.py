@@ -101,7 +101,7 @@ def test_generic_form_array_lambda_and_truncation():
     np.testing.assert_allclose(tgt.cpu().numpy(), tgt_o, rtol=RTOL, atol=ATOL)
 
 
-@pytest.mark.parametrize("quads", [2, 4, 8, 16, 32, 216, 232, 308, 316, 332, 408, 416, 500, 501, 502])
+@pytest.mark.parametrize("quads", [2, 4, 8, 416, 500, 501])
 def test_every_block_shape_agrees(quads):
     import ctypes
 
@@ -113,14 +113,14 @@ def test_every_block_shape_agrees(quads):
     args = (_t(reward), _t(value), _t(boot), _t(done, torch.bool), _t(trunc, torch.bool), 0.99, 0.95, 1.0, 1)
     lib.stx_gae_set_tuning(0)
     a0, t0, s0 = ops.gae_ppo(*args)
-    lib.stx_gae_set_tuning(quads)
+    assert lib.stx_gae_set_tuning(quads) == 0
     try:
         a1, t1, s1 = ops.gae_ppo(*args)
     finally:
         lib.stx_gae_set_tuning(0)
-    if quads < 300 or quads in (408, 416, 500):  # same 4-step chunking (500 = the TMA-pipelined kernel, 32 x 128 tiles) -> bit-identical
+    if quads != 501:  # same 4-step chunking (500 = the TMA-pipelined kernel, 32 x 128 tiles) -> bit-identical
         assert torch.equal(a0, a1) and torch.equal(t0, t1)
-    else:            # 2-step chunking (3xx; 501 = TMA kernel with 64 x 64 tiles) re-associates the composition: equal to fp32 rounding
+    else:             # 2-step chunking (501 = TMA kernel with 64 x 64 tiles) re-associates the composition: equal to fp32 rounding
         np.testing.assert_allclose(a0.cpu().numpy(), a1.cpu().numpy(), rtol=1e-5, atol=1e-5)
         np.testing.assert_allclose(t0.cpu().numpy(), t1.cpu().numpy(), rtol=1e-5, atol=1e-5)
     np.testing.assert_allclose(s0.cpu().numpy(), s1.cpu().numpy(), rtol=1e-5)
@@ -128,7 +128,7 @@ def test_every_block_shape_agrees(quads):
 
 @pytest.mark.parametrize("T,E", [(128, 1024), (100, 48), (300, 1040), (1, 16), (129, 4112)])
 @pytest.mark.parametrize("standardize", [0, 1])
-@pytest.mark.parametrize("code", [500, 501, 502])
+@pytest.mark.parametrize("code", [500, 501])
 def test_tma_form_vs_oracle(T, E, standardize, code):
     """The TMA-pipelined persistent kernel (the default from E = 262144 up), forced at small shapes: ragged last segment
     (T % 128), ragged last env tile (E % 32), several segments per tile (carry across segments), one block walking many tiles."""
@@ -139,7 +139,7 @@ def test_tma_form_vs_oracle(T, E, standardize, code):
     lib = _lib.load()
     lib.stx_gae_set_tuning.argtypes = [ctypes.c_int]
     reward, value, boot, done, trunc = _random_ppo_inputs(T, E, seed=11, p_done=0.05, p_trunc=0.05)
-    lib.stx_gae_set_tuning(code)   # 500: 32 envs x 128 steps per tile, 501: 64 x 64
+    assert lib.stx_gae_set_tuning(code) == 0   # 500: 32 envs x 128 steps per tile, 501: 64 x 64
     try:
         adv, tgt, stats = ops.gae_ppo(_t(reward), _t(value), _t(boot), _t(done, torch.bool), _t(trunc, torch.bool), 0.99, 0.95, 1.0, standardize)
     finally:
