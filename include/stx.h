@@ -177,13 +177,9 @@ int stx_tc_debug_forward(const StxMlp* mlp, const void* x, int64_t ldx, int64_t 
  * kernel leaves idle) instead of queueing CTAs behind it.  Host-side state, read at launch time. */
 void stx_tc_set_forward_ctas(int n);
 
-/* Profiling hook kept for ABI compatibility: the K3a kernel of this build records no clock64() stamps, so the
- * buffer is left untouched.  Synchronous (not for capture). */
-int stx_tc_debug_set_clock_buffer(long long* buf);
-/* Profiling hook of the K3 launches: device buffer of [gridDim][8] int64 filled per CTA of K3a / K3b with
- * K3a {1, total cycles, -, tiles, -, -, -, -} and, overwriting it, K3b {2 + job, total cycles, cycles before the end of
- * griddepcontrol.wait, globaltimer (ns) after it, globaltimer at exit, chunks, -, -} (see stx_tc_ppo.cu g_prof_buf,
- * scripts/k3b_jobs.py); NULL disables. */
+/* Profiling hook of the K3b launches: device buffer of [gridDim][8] int64 filled per CTA of K3b with
+ * {2 + job, total cycles, cycles before the end of griddepcontrol.wait, globaltimer (ns) after it, globaltimer at exit,
+ * chunks, -, -} (see stx_tc_ppo.cu g_prof_buf, scripts/k3b_jobs.py); NULL disables.  Synchronous (not for capture). */
 int stx_tc_debug_set_prof_buffer(long long* buf);
 
 /* Categorical head ops on logits (E, A) -- tfd.Categorical (stoix/networks/heads.py:41) as used at

@@ -5,9 +5,7 @@ Workload: 64 minibatch steps of `ops.ppo_minibatch_grads` (K3a `tc_ppo_fwd_bwd_k
 for per-kernel device times, one with the profiler off for a CUDA-event time of the whole 64-step loop.  Achieved GB/s and TFLOP/s
 use the bytes and FLOPs the kernels need, computed from the shapes by `k3_accounting`.
 
-    python scripts/time_k3.py --out /tmp/time_k3.json [--split 19,13,15 --split 17,15,17]
-
-Each `--split w1,w2,w0` repeats the run in a child process with STX_DW_SPLIT set (the K3b CTA partition is read once per process).
+    python scripts/time_k3.py --out /tmp/time_k3.json
 """
 from __future__ import annotations
 
@@ -25,10 +23,10 @@ E, T, D, A, MB = 4096, 128, 64, 8, 32768
 H = 256
 STEPS = 64
 KERNELS = ("tc_ppo_fwd_bwd_kernel", "tc_dw_kernel", "tc_reduce_kernel", "clip_adam_kernel")
-DEFAULT_SPLIT = (19, 13, 15)
+DW_SPLIT = (19, 13, 15)  # K3b's split-K CTAs per dW1 half, dW2, dW0 (stx_tc_ppo.cu kDwCtasW1 / W2 / W0)
 
 
-def k3_accounting(mb: int = MB, d: int = D, split=DEFAULT_SPLIT, n_params: int = 0, rebuild: bool = True) -> dict:
+def k3_accounting(mb: int = MB, d: int = D, n_params: int = 0, rebuild: bool = True) -> dict:
     """HBM bytes and tensor FLOPs of one minibatch step, per kernel, from the shapes (both networks).
 
     Bytes are what each kernel has to move: the activations K3a writes and K3b reads in their stored widths (tiled bf16, dz
@@ -36,7 +34,7 @@ def k3_accounting(mb: int = MB, d: int = D, split=DEFAULT_SPLIT, n_params: int =
     rebuild=True is the current layout: K3b's dW1 half-jobs rebuild h1 and dh2 from x, dz and the mask, so those two never
     reach HBM.  rebuild=False is the earlier layout, where K3a stored h1 and dh2 and both dW1 half-jobs streamed all of h1
     and half of dh2.  FLOPs are the MMA work as executed (heads padded to N=16, the input layer to K=64)."""
-    w1, w2, w0 = split
+    w1, w2, w0 = DW_SPLIT
     x_row, act_row, dz_row, mask_row = 2 * d, 2 * H, 2 * 16, H // 8
     # K3a, per row: both nets gather x and read the index twice; the actor reads action, logp, adv, the critic value, target
     k3a_read = 2 * (x_row + 2 * 4) + 3 * 4 + 2 * 4
@@ -134,8 +132,7 @@ def run_once(rebuild: bool) -> dict:
             if k in ev.key:
                 dev_us[k] += ev.self_device_time_total
                 calls[k] += ev.count
-    split = tuple(int(s) for s in os.environ.get("STX_DW_SPLIT", ",".join(map(str, DEFAULT_SPLIT))).split(","))
-    acc = k3_accounting(split=split, n_params=n_params, rebuild=rebuild)
+    acc = k3_accounting(n_params=n_params, rebuild=rebuild)
     kernels = {}
     for k in KERNELS:
         us = dev_us[k] / STEPS
@@ -143,31 +140,18 @@ def run_once(rebuild: bool) -> dict:
         kernels[k] = {"us_per_step": round(us, 2), "launches": calls[k], "mbytes": round(b / 1e6, 2), "gflop": round(f / 1e9, 3),
                       "gb_per_s": round(b / (us * 1e-6) / 1e9, 1) if us > 0 else None,
                       "tflop_per_s": round(f / (us * 1e-6) / 1e12, 1) if us > 0 and f else None}
-    return {"split": list(split), "loop_us_per_step": round(loop_ms / STEPS * 1e3, 2), "steps": STEPS, "kernels": kernels,
+    return {"split": list(DW_SPLIT), "loop_us_per_step": round(loop_ms / STEPS * 1e3, 2), "steps": STEPS, "kernels": kernels,
             "sum_kernel_us_per_step": round(sum(v["us_per_step"] for v in kernels.values()), 2)}
 
 
 def main() -> None:
     ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
     ap.add_argument("--out", required=True, help="JSON output path")
-    ap.add_argument("--split", action="append", default=[], help="w1,w2,w0 (2 w1 + w2 + w0 = 66); repeatable; child process each")
     ap.add_argument("--layout", choices=("rebuild", "stored"), default="rebuild",
                     help="byte accounting of the build under test: rebuild (current) or stored (h1 and dh2 through HBM, earlier builds)")
-    ap.add_argument("--child", action="store_true", help=argparse.SUPPRESS)
     args = ap.parse_args()
-    rebuild = args.layout == "rebuild"
-    if args.child:
-        with open(args.out, "w") as f:
-            json.dump(run_once(rebuild), f)
-        return
-    res = {"gpu": _gpu_info(), "shape": {"E": E, "T": T, "D": D, "A": A, "mb": MB}, "layout": args.layout, "default": run_once(rebuild)}
-    for s in args.split:
-        child_out = args.out + f".split_{s.replace(',', '_')}.json"
-        env = dict(os.environ, STX_DW_SPLIT=s)
-        subprocess.run([sys.executable, os.path.abspath(__file__), "--child", "--layout", args.layout, "--out", child_out], env=env, check=True)
-        with open(child_out) as f:
-            res.setdefault("splits", {})[s] = json.load(f)
-        os.remove(child_out)
+    res = {"gpu": _gpu_info(), "shape": {"E": E, "T": T, "D": D, "A": A, "mb": MB}, "layout": args.layout,
+           "default": run_once(args.layout == "rebuild")}
     os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
     with open(args.out, "w") as f:
         json.dump(res, f, indent=1)

@@ -354,7 +354,6 @@ _SIGNATURES = {
     "stx_mlp_forward_workspace_bytes": (C.c_size_t, [C.POINTER(StxMlp), C.c_int64, C.c_int]),
     "stx_mlp_forward": (C.c_int, [C.POINTER(StxMlp), _P, C.c_int64, _P, C.c_int64, _P, C.c_int, _P, C.c_size_t, _P]),
     "stx_tc_debug_forward": (C.c_int, [C.POINTER(StxMlp), _P, C.c_int64, C.c_int64, _P, _P, _P, _P]),
-    "stx_tc_debug_set_clock_buffer": (C.c_int, [_P]),
     "stx_tc_debug_set_prof_buffer": (C.c_int, [_P]),
     "stx_tc_set_forward_ctas": (None, [C.c_int]),
     "stx_categorical": (C.c_int, [_P, C.c_int64, C.c_int, C.c_int, C.c_uint64, C.c_uint64, _P, _P, _P, _P, _P]),

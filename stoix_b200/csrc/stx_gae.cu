@@ -416,13 +416,7 @@ int launch_gae_tma_shape(const PpoIn& in, int T, int E, int want, float* adv, fl
     *ms = fresh;
   }
   const CUtensorMap &mr = ms->m[0], &mv = ms->m[1], &mvt = ms->m[2], &mdn = ms->m[3], &mtr = ms->m[4];
-  static unsigned long long opted = 0;
-  int dev = 0;
-  STX_CUDA_OK(cudaGetDevice(&dev));
-  if (dev >= 64 || !((opted >> dev) & 1ull)) {
-    STX_CUDA_OK(cudaFuncSetAttribute(gae_tma_kernel<kGE, kGT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGaeSmemBytes));
-    if (dev < 64) opted |= 1ull << dev;
-  }
+  STX_CUDA_OK(opt_in_smem<gae_tma_kernel<kGE, kGT>>(kGaeSmemBytes));
   if (int rc = tc::use_trap_record(st)) return rc;
   const int n_tiles = (E + kGE - 1) / kGE;
   const int grid = n_tiles < kNumSMs ? n_tiles : kNumSMs;

@@ -771,8 +771,6 @@ Form form_of(int T, int64_t E, int H) {
 
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_cluster2(void (*kernel)(KArgs...), unsigned clusters, int threads, size_t smem, cudaStream_t st, Args... args) {
-  cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemLimit);
-  if (e != cudaSuccess) return e;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(2 * clusters), cfg.blockDim = dim3(threads), cfg.dynamicSmemBytes = smem, cfg.stream = st;
   cudaLaunchAttribute attr[1];
@@ -780,12 +778,6 @@ inline cudaError_t launch_cluster2(void (*kernel)(KArgs...), unsigned clusters, 
   attr[0].val.clusterDim.x = 2, attr[0].val.clusterDim.y = 1, attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr, cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, args...);
-}
-
-template <typename K>
-inline int opt_in(K kernel) {
-  STX_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemLimit));
-  return STX_OK;
 }
 
 // ---- drivers ------------------------------------------------------------------------------------------------------------
@@ -808,6 +800,7 @@ int sequence_forward(const char* fn, const float* gi, const uint8_t* reset, cons
   const unsigned blocks = (unsigned)((eh + 255) / 256);
   switch (form_of<Cell>(T, E, H)) {
     case Form::kCluster:
+      STX_CUDA_OK(opt_in_smem<cluster_fwd_kernel<Cell>>(kSmemLimit));
       STX_CUDA_OK(launch_cluster2(cluster_fwd_kernel<Cell>, (unsigned)((E + kClusterR - 1) / kClusterR), cluster_threads<Cell>(H),
                                   ClusterSmem<Cell>::fwd_bytes(H), st, gi, reset, carry0, w_h, b_hn, T, E, H, h_seq, carry_last, ws.hp_seq, ws.cp_seq,
                                   ws.act));
@@ -816,11 +809,11 @@ int sequence_forward(const char* fn, const float* gi, const uint8_t* reset, cons
     case Form::kPersistent:
       if constexpr (Cell::kPersistent) {
         if (E >= 1024) {
-          if (int rc = opt_in(gru_seq_fwd_kernel<8, 1>)) return rc;
+          STX_CUDA_OK(opt_in_smem<gru_seq_fwd_kernel<8, 1>>(kSmemLimit));
           gru_seq_fwd_kernel<8, 1><<<(unsigned)((E + 7) / 8), gru_threads(H, 1), GruSmem<8, 1>::fwd_bytes(H), st>>>(gi, reset, carry0, w_h, b_hn, T, E, H,
                                                                                                                       h_seq, ws.hp_seq, ws.act);
         } else {
-          if (int rc = opt_in(gru_seq_fwd_kernel<4, 2>)) return rc;
+          STX_CUDA_OK(opt_in_smem<gru_seq_fwd_kernel<4, 2>>(kSmemLimit));
           gru_seq_fwd_kernel<4, 2><<<(unsigned)((E + 3) / 4), gru_threads(H, 2), GruSmem<4, 2>::fwd_bytes(H), st>>>(gi, reset, carry0, w_h, b_hn, T, E, H,
                                                                                                                       h_seq, ws.hp_seq, ws.act);
         }
@@ -864,6 +857,7 @@ int sequence_backward(const char* fn, const float* d_h_seq, const uint8_t* reset
   const float* carry_seq = Cell::kC ? ws.cp_seq : ws.hp_seq;     // the carry the cell's backward reads
   switch (form_of<Cell>(T, E, H)) {
     case Form::kCluster:
+      STX_CUDA_OK(opt_in_smem<cluster_bwd_kernel<Cell>>(kSmemLimit));
       STX_CUDA_OK(launch_cluster2(cluster_bwd_kernel<Cell>, (unsigned)((E + kClusterR - 1) / kClusterR), cluster_threads<Cell>(H),
                                   ClusterSmem<Cell>::bwd_bytes(H), st, d_h_seq, reset, w_h, T, E, H, carry_seq, ws.act, d_gi, ws.d_gh_seq, d_carry0));
       STX_LAUNCH_OK();
@@ -871,11 +865,11 @@ int sequence_backward(const char* fn, const float* d_h_seq, const uint8_t* reset
     case Form::kPersistent:
       if constexpr (Cell::kPersistent) {
         if (E >= 1024) {
-          if (int rc = opt_in(gru_seq_bwd_kernel<8, 1>)) return rc;
+          STX_CUDA_OK(opt_in_smem<gru_seq_bwd_kernel<8, 1>>(kSmemLimit));
           gru_seq_bwd_kernel<8, 1><<<(unsigned)((E + 7) / 8), gru_threads(H, 1), GruSmem<8, 1>::bwd_bytes(H), st>>>(d_h_seq, reset, w_h, T, E, H, ws.hp_seq,
                                                                                                                       ws.act, d_gi, ws.d_gh_seq, d_carry0);
         } else {
-          if (int rc = opt_in(gru_seq_bwd_kernel<4, 2>)) return rc;
+          STX_CUDA_OK(opt_in_smem<gru_seq_bwd_kernel<4, 2>>(kSmemLimit));
           gru_seq_bwd_kernel<4, 2><<<(unsigned)((E + 3) / 4), gru_threads(H, 2), GruSmem<4, 2>::bwd_bytes(H), st>>>(d_h_seq, reset, w_h, T, E, H, ws.hp_seq,
                                                                                                                       ws.act, d_gi, ws.d_gh_seq, d_carry0);
         }

@@ -102,27 +102,26 @@ __device__ __forceinline__ void store_out(const GemmArgs& g, int64_t m, int n, f
 }
 
 // Register-tiled GEMM, one shared-memory stage + register prefetch: the global loads of step k+1 are issued before the products
-// of step k and land in registers while the FMAs run; (BM, BN, BK, TM, TN) = (64, 64, 16, 4, 4) for mid-size grids and
-// (128, 128, 8, 8, 8) -- 64 accumulators per thread, 4 shared loads per 32 packed FMAs -- when that still fills the GPU.
-template <int MODE, int BM_, int BN_, int BK_, int TM_, int TN_>
-__global__ void __launch_bounds__((BM_ / TM_) * (BN_ / TN_)) gemm_kernel(GemmArgs g) {
-  constexpr int NT = (BM_ / TM_) * (BN_ / TN_);
-  constexpr int LA = BM_ * BK_ / NT, LB = BN_ * BK_ / NT;
-  static_assert(BM_ * BK_ % NT == 0 && BN_ * BK_ % NT == 0 && TN_ % 2 == 0 && TM_ % 4 == 0 && TN_ % 4 == 0, "tile shape");
-  __shared__ __align__(16) float As[BK_][BM_ + 4];
-  __shared__ __align__(16) float Bs[BK_][BN_ + 4];
+// of step k and land in registers while the FMAs run.  64x64 output tiles, 16 values of the reduction per step, 4x4 outputs
+// per thread.  (128x128 tiles with 8x8 outputs per thread measured slower.)
+template <int MODE>
+__global__ void __launch_bounds__(kThreads) gemm_kernel(GemmArgs g) {
+  constexpr int LA = BM * BK / kThreads, LB = BN * BK / kThreads;
+  static_assert(BM * BK % kThreads == 0 && BN * BK % kThreads == 0 && TN % 2 == 0 && TM % 4 == 0 && TN % 4 == 0, "tile shape");
+  __shared__ __align__(16) float As[BK][BM + 4];
+  __shared__ __align__(16) float Bs[BK][BN + 4];
   const int tid = threadIdx.x;
-  const int tx = tid % (BN_ / TN_), ty = tid / (BN_ / TN_);
-  const int64_t m0 = (int64_t)blockIdx.y * BM_;  // output row tile
-  const int n0 = blockIdx.x * BN_;               // output col tile
-  float2 acc[TM_][TN_ / 2];
+  const int tx = tid % (BN / TN), ty = tid / (BN / TN);
+  const int64_t m0 = (int64_t)blockIdx.y * BM;  // output row tile
+  const int n0 = blockIdx.x * BN;               // output col tile
+  float2 acc[TM][TN / 2];
 #pragma unroll
-  for (int i = 0; i < TM_; ++i)
+  for (int i = 0; i < TM; ++i)
 #pragma unroll
-    for (int j = 0; j < TN_ / 2; ++j) acc[i][j] = make_float2(0.f, 0.f);
-  float dbacc[TN_];
+    for (int j = 0; j < TN / 2; ++j) acc[i][j] = make_float2(0.f, 0.f);
+  float dbacc[TN];
 #pragma unroll
-  for (int j = 0; j < TN_; ++j) dbacc[j] = 0.f;
+  for (int j = 0; j < TN; ++j) dbacc[j] = 0.f;
 
   // reduction range
   int64_t r_begin = 0, r_end;
@@ -140,7 +139,7 @@ __global__ void __launch_bounds__((BM_ / TM_) * (BN_ / TN_)) gemm_kernel(GemmArg
     if (MODE == FWD || MODE == DX) {    // A[row(m)][r0 + kk]: kk fastest in memory -> As[kk][m]
 #pragma unroll
       for (int u = 0; u < LA; ++u) {
-        const int i = tid + u * NT, kk = i % BK_, mm = i / BK_;
+        const int i = tid + u * kThreads, kk = i % BK, mm = i / BK;
         const int64_t m = m0 + mm, k = r0 + kk;
         const bool ok = m < g.M && k < r_end;
         const int64_t row = ok ? ((MODE == FWD && g.rowidx) ? (int64_t)__ldg(g.rowidx + m) : m) : 0;
@@ -149,7 +148,7 @@ __global__ void __launch_bounds__((BM_ / TM_) * (BN_ / TN_)) gemm_kernel(GemmArg
     } else {                            // DW: A(f, r) = H[row(r)][f]; f (feature) fastest in memory. As[kk = r][mm = f]
 #pragma unroll
       for (int u = 0; u < LA; ++u) {
-        const int i = tid + u * NT, mm = i % BM_, kk = i / BM_;
+        const int i = tid + u * kThreads, mm = i % BM, kk = i / BM;
         const int64_t r = r0 + kk, f = m0 + mm;
         const bool ok = r < r_end && f < out_rows;
         const int64_t row = ok ? (g.rowidx ? (int64_t)__ldg(g.rowidx + r) : r) : 0;
@@ -158,14 +157,14 @@ __global__ void __launch_bounds__((BM_ / TM_) * (BN_ / TN_)) gemm_kernel(GemmArg
     }
 #pragma unroll
     for (int u = 0; u < LB; ++u) {
-      const int i = tid + u * NT;
+      const int i = tid + u * kThreads;
       if (MODE == DX) {                 // B(kk, j) = W[j][r0 + kk], W (Kout x Nr) row-major; reduction fastest in memory
-        const int kk = i % BK_, nn = i / BK_;
+        const int kk = i % BK, nn = i / BK;
         const int64_t k = r0 + kk;
         const int j = n0 + nn;
         vb[u] = (k < r_end && j < g.N) ? __ldg(g.B + (int64_t)j * g.K + k) : 0.f;
       } else {                          // FWD: W[k][n]; DW: dY[r][n]
-        const int nn = i % BN_, kk = i / BN_;
+        const int nn = i % BN, kk = i / BN;
         const int64_t k = r0 + kk;
         const int n = n0 + nn;
         vb[u] = (k < r_end && n < g.N) ? __ldg(g.B + k * g.N + n) : 0.f;
@@ -173,41 +172,41 @@ __global__ void __launch_bounds__((BM_ / TM_) * (BN_ / TN_)) gemm_kernel(GemmArg
     }
   };
   if (r_begin < r_end) load_tiles(r_begin);
-  for (int64_t r0 = r_begin; r0 < r_end; r0 += BK_) {
+  for (int64_t r0 = r_begin; r0 < r_end; r0 += BK) {
 #pragma unroll
     for (int u = 0; u < LA; ++u) {
-      const int i = tid + u * NT;
-      if (MODE == DW) As[i / BM_][i % BM_] = va[u];
-      else As[i % BK_][i / BK_] = va[u];
+      const int i = tid + u * kThreads;
+      if (MODE == DW) As[i / BM][i % BM] = va[u];
+      else As[i % BK][i / BK] = va[u];
     }
 #pragma unroll
     for (int u = 0; u < LB; ++u) {
-      const int i = tid + u * NT;
-      if (MODE == DX) Bs[i % BK_][i / BK_] = vb[u];
-      else Bs[i / BN_][i % BN_] = vb[u];
+      const int i = tid + u * kThreads;
+      if (MODE == DX) Bs[i % BK][i / BK] = vb[u];
+      else Bs[i / BN][i % BN] = vb[u];
     }
     __syncthreads();
-    if (r0 + BK_ < r_end) load_tiles(r0 + BK_);   // in flight under the products below
+    if (r0 + BK < r_end) load_tiles(r0 + BK);   // in flight under the products below
 #pragma unroll
-    for (int kk = 0; kk < BK_; ++kk) {
-      float a[TM_], b[TN_];
+    for (int kk = 0; kk < BK; ++kk) {
+      float a[TM], b[TN];
 #pragma unroll
-      for (int i = 0; i < TM_; i += 4) {
-        const float4 v = *reinterpret_cast<const float4*>(&As[kk][ty * TM_ + i]);
+      for (int i = 0; i < TM; i += 4) {
+        const float4 v = *reinterpret_cast<const float4*>(&As[kk][ty * TM + i]);
         a[i] = v.x, a[i + 1] = v.y, a[i + 2] = v.z, a[i + 3] = v.w;
       }
 #pragma unroll
-      for (int j = 0; j < TN_; j += 4) {
-        const float4 v = *reinterpret_cast<const float4*>(&Bs[kk][tx * TN_ + j]);
+      for (int j = 0; j < TN; j += 4) {
+        const float4 v = *reinterpret_cast<const float4*>(&Bs[kk][tx * TN + j]);
         b[j] = v.x, b[j + 1] = v.y, b[j + 2] = v.z, b[j + 3] = v.w;
       }
 #pragma unroll
-      for (int i = 0; i < TM_; ++i)
+      for (int i = 0; i < TM; ++i)
 #pragma unroll
-        for (int j = 0; j < TN_ / 2; ++j) fma2(acc[i][j], a[i], make_float2(b[2 * j], b[2 * j + 1]));
+        for (int j = 0; j < TN / 2; ++j) fma2(acc[i][j], a[i], make_float2(b[2 * j], b[2 * j + 1]));
       if (MODE == DW) {
 #pragma unroll
-        for (int j = 0; j < TN_; ++j) dbacc[j] += b[j];
+        for (int j = 0; j < TN; ++j) dbacc[j] += b[j];
       }
     }
     __syncthreads();
@@ -216,32 +215,32 @@ __global__ void __launch_bounds__((BM_ / TM_) * (BN_ / TN_)) gemm_kernel(GemmArg
   // ---- epilogue ----
   if (MODE != DW) {
 #pragma unroll
-    for (int i = 0; i < TM_; ++i) {
-      const int64_t m = m0 + ty * TM_ + i;
+    for (int i = 0; i < TM; ++i) {
+      const int64_t m = m0 + ty * TM + i;
       if (m >= g.M) continue;
 #pragma unroll
-      for (int j = 0; j < TN_; ++j) {
-        const int n = n0 + tx * TN_ + j;
+      for (int j = 0; j < TN; ++j) {
+        const int n = n0 + tx * TN + j;
         if (n < g.N) store_out<MODE>(g, m, n, (j & 1) ? acc[i][j / 2].y : acc[i][j / 2].x);
       }
     }
   } else {
     float* Cp = g.C + (int64_t)blockIdx.z * g.part_stride;
 #pragma unroll
-    for (int i = 0; i < TM_; ++i) {
-      const int64_t f = m0 + ty * TM_ + i;
+    for (int i = 0; i < TM; ++i) {
+      const int64_t f = m0 + ty * TM + i;
       if (f >= out_rows) continue;
 #pragma unroll
-      for (int j = 0; j < TN_; ++j) {
-        const int n = n0 + tx * TN_ + j;
+      for (int j = 0; j < TN; ++j) {
+        const int n = n0 + tx * TN + j;
         if (n < g.N) Cp[f * g.N + n] = (j & 1) ? acc[i][j / 2].y : acc[i][j / 2].x;
       }
     }
     if (blockIdx.y == 0 && ty == 0 && g.dbias) {
       float* dbp = g.dbias + (int64_t)blockIdx.z * g.dbias_stride;
 #pragma unroll
-      for (int j = 0; j < TN_; ++j) {
-        const int n = n0 + tx * TN_ + j;
+      for (int j = 0; j < TN; ++j) {
+        const int n = n0 + tx * TN + j;
         if (n < g.N) dbp[n] = dbacc[j];
       }
     }
@@ -430,29 +429,13 @@ template <int MODE>
 inline cudaError_t launch_gemm(const GemmArgs& g, int splits, cudaStream_t st) {
   const int64_t out_rows = (MODE == DW) ? g.K : g.M;
   const int64_t ctas64 = ((out_rows + BM - 1) / BM) * ((g.N + BN - 1) / BN) * (MODE == DW ? splits : 1);
-  const int64_t ctas128 = ((out_rows + 127) / 128) * ((g.N + 127) / 128) * (MODE == DW ? splits : 1);
-  // 128x128x8 tiles with 8x8 outputs per thread need ~136 registers -> one 256-thread block per SM; not dispatched by default
-  // (STX_GEMM_128=1 enables it).
-  static const bool big_tiles = [] { const char* e = getenv("STX_GEMM_128"); return e && e[0] == '1'; }();
-  if (big_tiles && ctas128 >= kPanelBelowCtas) {
-    dim3 grid((g.N + 127) / 128, (unsigned)((out_rows + 127) / 128), MODE == DW ? splits : 1);
-    gemm_kernel<MODE, 128, 128, 8, 8, 8><<<grid, 256, 0, st>>>(g);
-    return cudaGetLastError();
-  }
   if (ctas64 >= kPanelBelowCtas) {
     dim3 grid((g.N + BN - 1) / BN, (unsigned)((out_rows + BM - 1) / BM), MODE == DW ? splits : 1);
-    gemm_kernel<MODE, BM, BN, BK, TM, TN><<<grid, kThreads, 0, st>>>(g);
+    gemm_kernel<MODE><<<grid, kThreads, 0, st>>>(g);
     return cudaGetLastError();
   }
-  static unsigned long long opted = 0;  // bit d: dynamic shared memory opt-in done on device d (per instantiation)
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  cudaError_t e = opt_in_smem<gemm_panel_kernel<MODE>>(kPanelSmemBytes);
   if (e != cudaSuccess) return e;
-  if (dev >= 64 || !((opted >> dev) & 1ull)) {
-    e = cudaFuncSetAttribute(gemm_panel_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPanelSmemBytes);
-    if (e != cudaSuccess) return e;
-    if (dev < 64) opted |= 1ull << dev;
-  }
   dim3 grid((g.N + PN - 1) / PN, (unsigned)((out_rows + PM - 1) / PM), MODE == DW ? splits : 1);
   gemm_panel_kernel<MODE><<<grid, kPanelThreads, kPanelSmemBytes, st>>>(g);
   return cudaGetLastError();
@@ -551,20 +534,12 @@ static __global__ void __launch_bounds__(32 * kLnWarps) ln_backward_kernel(float
 
 // ln_backward_kernel takes kLnWarps * 2N floats of dynamic shared memory: 64 KiB at the widest width check_mlp accepts
 // (N = 32 * kLnMaxCols), more than the 48 KiB a launch may use without opting in (every width above 768).  The opt-in is made
-// once per device for the largest size, as launch_gemm does for the panel kernel; it is not a stream operation, so a launch
-// under stream capture may make it.
+// once per device for the largest size.
 constexpr uint32_t kLnMaxSmemBytes = sizeof(float) * kLnWarps * 2 * 32 * kLnMaxCols;
 static inline cudaError_t launch_ln_backward(float* D, const float* U, const float* stats, const float* gamma, const float* beta, int act, int64_t M,
                                       int N, int rows_per_block, int blocks, float* part, cudaStream_t st) {
-  static unsigned long long opted = 0;  // bit d: dynamic shared memory opt-in done on device d
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
+  cudaError_t e = opt_in_smem<ln_backward_kernel>(kLnMaxSmemBytes);
   if (e != cudaSuccess) return e;
-  if (dev >= 64 || !((opted >> dev) & 1ull)) {
-    e = cudaFuncSetAttribute(ln_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kLnMaxSmemBytes);
-    if (e != cudaSuccess) return e;
-    if (dev < 64) opted |= 1ull << dev;
-  }
   ln_backward_kernel<<<blocks, 32 * kLnWarps, sizeof(float) * kLnWarps * 2 * N, st>>>(D, U, stats, gamma, beta, act, M, N, rows_per_block, part);
   return cudaGetLastError();
 }

@@ -221,11 +221,7 @@ int tc_forward_impl(const StxMlp* m, const void* x, int64_t ldx, int64_t M, floa
   p.out = out, p.dbg_h1 = dbg_h1, p.dbg_h2 = dbg_h2, p.M = M, p.A = A;
   p.num_tiles = (int)((M + kTileM - 1) / kTileM);
   p.dev_rows = dev_rows;
-  static bool attr_set = false;
-  if (!attr_set) {
-    STX_CUDA_OK(cudaFuncSetAttribute(tc_mlp_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemBytes));
-    attr_set = true;
-  }
+  STX_CUDA_OK(opt_in_smem<tc_mlp_fwd_kernel>(kSmemBytes));
   if (int rc = use_trap_record(st)) return rc;
   int cap = (g_forward_ctas > 0 && g_forward_ctas < kNumSMs) ? g_forward_ctas : kNumSMs;
   if (max_ctas > 0 && max_ctas < cap) cap = max_ctas;

@@ -13,8 +13,9 @@
 //      MN-major B (forward) and K-major B (backward).  256-wide GEMMs run as two N=128 halves (64 accumulator
 //      registers).  The epilogues also emit h2, dh1, dz (bf16) and the h2 > 0 sign mask for the weight-gradient GEMMs,
 //      reduce the bias gradients (quad butterfly + per-warp smem slices, fixed order) and accumulate the loss metrics.
-//  tc_dw_kernel (K3b)  split-K GEMMs dW = A^T * B over the minibatch rows with both operands MN-major, two consumer
-//      warpgroups with fp32 register accumulators and a third warpgroup that feeds them:
+//  tc_dw_kernel (K3b)  split-K GEMMs dW = A^T * B over the minibatch rows with both operands MN-major, on a fixed plan of
+//      CTAs per job (kDwCtasW1 / W2 / W0), two consumer warpgroups with fp32 register accumulators and a third warpgroup that
+//      feeds them:
 //        dW2 = h2^T dz (N=16), dW0^T = dh1^T x (N=64): 4-stage TMA/mbarrier ring of A and B (one producer warp);
 //        dW1 = h1^T dh2 in two jobs of 128 hidden units (N=256): the third warpgroup rebuilds h1[:, half] = relu(x W0 + b0)
 //        and dh2 = (dz W2^T) * mask per 64-row chunk from x, dz and the mask (12 KB instead of 96 KB of stored h1 and dh2)
@@ -28,9 +29,6 @@
 // evict_first, partials / gradients evict_last L2 policies (see stx_common.cuh).
 #include <cuda.h>
 
-#include <cstdio>
-#include <cstdlib>
-
 #include "stx_common.cuh"
 #include "stx_tc_ptx.cuh"
 
@@ -41,8 +39,7 @@ int make_map_2d_pub(CUtensorMap* m, const void* base, uint64_t rows, uint64_t co
                     uint32_t box_cols);  // stx_tc_mlp.cu (SWIZZLE_128B bf16)
 int make_map_tiled(CUtensorMap* m, const void* base, uint64_t tiles, uint32_t colgroups, uint32_t box_cg);  // stx_tc_mlp.cu
 
-// optional instrumentation hooks of the C ABI (stx_tc_debug_set_*_buffer): [gridDim][8] per-CTA cycle counts
-__device__ long long* g_clock_buf = nullptr;
+// optional instrumentation hook of the C ABI (stx_tc_debug_set_prof_buffer): K3b's [gridDim][8] per-CTA profile record
 __device__ long long* g_prof_buf = nullptr;
 
 __device__ __forceinline__ long long globaltimer_ns() {
@@ -92,7 +89,6 @@ struct FbParams {
   int mb;
   float inv_m;              // 1 / mb, computed on the host (a device division would be a library call in this kernel)
   float clip_eps, ent_coef, vf_coef;
-  int act_policy;     // L2 policy of the activation stores: 0 evict_first (read once, after a kernel boundary), 1 normal, 2 evict_last
 };
 
 // Tiled activation layout shared by K3a (writer) and K3b (reader): element (row, col) of a [mb x 8*CG]
@@ -109,8 +105,10 @@ __device__ __forceinline__ int mask_word(int h, int i) { return 2 * h + (i >> 4)
 __device__ __forceinline__ uint32_t mask_bit(int i, int e) { return (uint32_t)(2 * (i & 15) + e); }
 
 // Stores half h of a packed 64 x 256 register operand (a: its 32 words of half h; rows row0, row0 + 8 of the thread, see
-// stx_tc_ptx.cuh) to the tiled layout.
-__device__ __forceinline__ void store_act(__nv_bfloat16* base, const uint32_t* a, int h, int64_t row0, int lane, uint64_t pol) {
+// stx_tc_ptx.cuh) to the tiled layout.  evict_first, like every activation store: K3b reads each activation once.  (The policy
+// is created per store site: one policy kept live across the whole K3a tile loop costs it spills.)
+__device__ __forceinline__ void store_act(__nv_bfloat16* base, const uint32_t* a, int h, int64_t row0, int lane) {
+  const uint64_t pol = l2_evict_first();
 #pragma unroll
   for (int i = 0; i < 32; ++i)
     st_hint(reinterpret_cast<uint32_t*>(tiled_ptr(base, row0 + 8 * (i & 1), 128 * h + 8 * (i >> 1) + 2 * (lane & 3), 32)), a[i], pol);
@@ -224,7 +222,6 @@ __global__ void __launch_bounds__(kFbThreads, 1)
   // align by OFFSET (not through an integer cast) so that the compiler keeps the shared address space: LDS/STS, not generic LD/ST
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const uint32_t sbase = smem_u32(smem);
-  const long long prof_t0 = clock64();
   float* s_b0 = reinterpret_cast<float*>(smem + kOffBias);
   float* s_b1 = s_b0 + 256;
   float* s_b2 = s_b1 + 256;
@@ -233,7 +230,6 @@ __global__ void __launch_bounds__(kFbThreads, 1)
 
   const int wg = threadIdx.x >> 7, t = threadIdx.x & 127, warp = threadIdx.x >> 5, wq = warp & 3, lane = threadIdx.x & 31;
   const int q4 = lane & 3;
-  const uint64_t pol_stream = l2_policy(p.act_policy);  // default evict_first: the activations are written once and read once (by K3b)
   const int which = (int)blockIdx.x < p.n_cta[0] ? 0 : 1;
   const FbNet& net = p.net[which];
   const int cta_in_net = which == 0 ? (int)blockIdx.x : (int)blockIdx.x - p.n_cta[0];
@@ -320,7 +316,7 @@ __global__ void __launch_bounds__(kFbThreads, 1)
       for (int cc = 0; cc < 4; ++cc) {
         const int c = hf * 4 + cc;
         const uint4 v = *reinterpret_cast<const uint4*>(smem + (xs - sbase) + r * 128 + ((c ^ (r & 7)) << 4));
-        st_hint(reinterpret_cast<uint4*>(tiled_ptr(p.xg, (int64_t)tile * kWTile + r, 8 * c, 8)), v, pol_stream);
+        st_hint(reinterpret_cast<uint4*>(tiled_ptr(p.xg, (int64_t)tile * kWTile + r, 8 * c, 8)), v, l2_evict_first());
       }
     }
     if (it + 1 < my_tiles) gather_tile(tile + n_wg, s ^ 1);
@@ -336,7 +332,7 @@ __global__ void __launch_bounds__(kFbThreads, 1)
     for (int h = 0; h < 2; ++h) {
       gemm_a_w1(acc, a1, sbase, h);
       epi_bias_relu(acc, s_b1, h, a2, lane);
-      store_act(net.h2, &a2[32 * h], h, row0, lane, pol_stream);
+      store_act(net.h2, &a2[32 * h], h, row0, lane);
     }
     // ---------------- G2 / E2: head + loss + d(head) ----------------
     float z[8];
@@ -377,7 +373,7 @@ __global__ void __launch_bounds__(kFbThreads, 1)
     for (int k = 0; k < 4; ++k) dzp[k] = pack_bf16(dz[2 * k], dz[2 * k + 1]);
 #pragma unroll
     for (int k = 0; k < 4; ++k)
-      st_hint(reinterpret_cast<uint32_t*>(tiled_ptr(net.dz, row0 + 8 * (k & 1), 8 * (k >> 1) + 2 * q4, 2)), dzp[k], pol_stream);
+      st_hint(reinterpret_cast<uint32_t*>(tiled_ptr(net.dz, row0 + 8 * (k & 1), 8 * (k >> 1) + 2 * q4, 2)), dzp[k], l2_evict_first());
     {  // head bias gradient: column sums of dz over the tile rows of this warp
       float cs[4];
 #pragma unroll
@@ -407,7 +403,7 @@ __global__ void __launch_bounds__(kFbThreads, 1)
       }
       colsum_half(acc, dbw + 256, h, lane);  // db1
     }
-    st_hint(net.mask + (int64_t)tile * 128 + t, make_uint4(mw[0], mw[1], mw[2], mw[3]), pol_stream);
+    st_hint(net.mask + (int64_t)tile * 128 + t, make_uint4(mw[0], mw[1], mw[2], mw[3]), l2_evict_first());
     // ---------------- G4 / E4: dh1 = (dh2 W1^T) * (h1 > 0) ----------------
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -420,7 +416,7 @@ __global__ void __launch_bounds__(kFbThreads, 1)
         const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(&pk);
         acc[2 * i] = __bfloat162float(v.x), acc[2 * i + 1] = __bfloat162float(v.y);  // db0 sums the bf16 dh1 that K3b's dW0 uses
       }
-      store_act(net.dh1, &a1[32 * h], h, row0, lane, pol_stream);
+      store_act(net.dh1, &a1[32 * h], h, row0, lane);
       colsum_half(acc, dbw, h, lane);  // db0
     }
   }
@@ -447,10 +443,6 @@ __global__ void __launch_bounds__(kFbThreads, 1)
         for (int w = 0; w < kFbThreads / 32; ++w) acc += s_mw[w][threadIdx.x];
       st_hint(&p.metric_part[(int64_t)blockIdx.x * 8 + threadIdx.x], acc, pol_keep);
     }
-  }
-  if (g_prof_buf != nullptr && threadIdx.x == 0) {
-    long long* pb = g_prof_buf + (int64_t)blockIdx.x * 8;
-    pb[0] = 1, pb[1] = clock64() - prof_t0, pb[3] = my_tiles;
   }
 }
 
@@ -498,7 +490,6 @@ struct DwJob {
 struct DwParams {
   DwJob job[kMaxJobs];
   int n_jobs;
-  int act_policy;
 };
 struct DwMaps {
   CUtensorMap a[kMaxJobs];  // tiled [mb x 256]: 2D u64 view {256 per (tile, colgroup), tiles*32}, box {128, 32}
@@ -711,13 +702,12 @@ __global__ void __launch_bounds__(kDwThreads, 1) tc_dw_kernel(const __grid_const
   griddep_launch();
   __syncthreads();
   griddep_wait();  // the activations are K3a's output; the partials written below were read by the previous reduce
-  // (the profile record is K3a's until K3a has finished: only written from here on)
   if (threadIdx.x == 0 && g_prof_buf != nullptr) {
     long long* prof = g_prof_buf + (int64_t)blockIdx.x * 8;
     prof[2] = clock64() - prof_t0, prof[3] = globaltimer_ns();
   }
 
-  const uint64_t pol_stream = l2_policy(p.act_policy);  // default evict_first: every activation tile is read exactly once
+  const uint64_t pol_stream = l2_evict_first();  // every activation tile is read exactly once
   if (job.rebuild) {
     // weights of the job's network (after griddep_wait: the previous optimiser step wrote them), as K3a stages them
     if (threadIdx.x == 256) {
@@ -877,22 +867,11 @@ struct TcWs {
 
 constexpr int kCtaPerNet = kNumSMs / 2;              // 66
 // Launch plan, per network (x 2 networks = 132 CTAs): K3a on 66 CTAs, then K3b with 19 + 19 / 13 / 15 split-K CTAs for
-// the two row halves of dW1 / dW2 / dW0.  Each dW1 CTA sums the same rows in the same order as the column-split jobs that
-// first set this plan, so the default keeps the gradients' rounding; the split decides which rows each partial holds.
-// Tuning switches: STX_DW_SPLIT="w1,w2,w0" (CTAs per dW1 half, dW2, dW0; 2 w1 + w2 + w0 = 66), STX_K3_POLICY (L2 policy
-// of the activation stream: 0 evict_first, 1 normal, 2 evict_last).
-struct K3Plan {
-  int w1 = 19, w2 = 13, w0 = 15;
-  int act_policy = 0;
-  K3Plan() {
-    int a, b, c;
-    const char* e = getenv("STX_DW_SPLIT");
-    if (e && sscanf(e, "%d,%d,%d", &a, &b, &c) == 3 && a > 0 && b > 0 && c > 0 && 2 * a + b + c == kCtaPerNet) w1 = a, w2 = b, w0 = c;
-    e = getenv("STX_K3_POLICY");
-    if (e) act_policy = atoi(e);
-  }
-};
-static const K3Plan g_plan;
+// the two row halves of dW1 / dW2 / dW0 (the fastest split of the sweeps in DESIGN.md).  Each dW1 CTA sums the same rows in
+// the same order as the column-split jobs that first set this plan, so the plan keeps the gradients' rounding; the split
+// decides which rows each partial holds.
+constexpr int kDwCtasW1 = 19, kDwCtasW2 = 13, kDwCtasW0 = 15;
+static_assert(2 * kDwCtasW1 + kDwCtasW2 + kDwCtasW0 == kCtaPerNet, "K3b's jobs of a network must take its 66 CTAs");
 
 TcWs carve_tc(int64_t mb, char* base) {
   TcWs w{};
@@ -908,9 +887,9 @@ TcWs carve_tc(int64_t mb, char* base) {
     w.dz[n] = (__nv_bfloat16*)take((size_t)mb * 16 * 2);
     w.mask[n] = (uint4*)take((size_t)mb * 256 / 8);
     // the dW1 half-jobs write both output halves: [1] must follow [0] directly (the size is a multiple of the alignment)
-    for (int hh = 0; hh < 2; ++hh) w.part_w1[n][hh] = (float*)take((size_t)g_plan.w1 * 256 * 128 * 4);
-    w.part_w2[n] = (float*)take((size_t)g_plan.w2 * 256 * 16 * 4);
-    w.part_w0[n] = (float*)take((size_t)g_plan.w0 * 256 * 64 * 4);
+    for (int hh = 0; hh < 2; ++hh) w.part_w1[n][hh] = (float*)take((size_t)kDwCtasW1 * 256 * 128 * 4);
+    w.part_w2[n] = (float*)take((size_t)kDwCtasW2 * 256 * 16 * 4);
+    w.part_w0[n] = (float*)take((size_t)kDwCtasW0 * 256 * 64 * 4);
     w.db_part[n] = (float*)take((size_t)kCtaPerNet * 528 * 4);
   }
   w.xg = (__nv_bfloat16*)take((size_t)mb * 64 * 2);
@@ -922,18 +901,6 @@ TcWs carve_tc(int64_t mb, char* base) {
 bool tc_ppo_shape_ok(const StxMlp* m) {
   return m->n_layers == 3 && m->sizes[1] == kH && m->sizes[2] == kH && m->sizes[0] <= 64 && m->sizes[0] % 8 == 0 &&
          m->sizes[3] >= 1 && m->sizes[3] <= 16 && m->activation == STX_ACT_RELU && !m->use_layer_norm;
-}
-
-// max dynamic shared memory opt-in, once per device and kernel
-template <typename K>
-static int opt_in_smem(K kernel, uint32_t bytes, int slot) {
-  static unsigned long long done[4] = {0, 0, 0, 0};  // bit d of done[slot]: set on device d
-  int dev = 0;
-  STX_CUDA_OK(cudaGetDevice(&dev));
-  if (dev < 64 && (done[slot] >> dev) & 1ull) return STX_OK;
-  STX_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-  if (dev < 64) done[slot] |= 1ull << dev;
-  return STX_OK;
 }
 
 }  // namespace tc
@@ -984,7 +951,6 @@ int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxP
   fp.adv_stats = h->standardize_advantages ? b->adv_stats : nullptr;
   fp.metric_part = ws.metric_part;
   fp.D = D, fp.mb = (int)mb, fp.inv_m = 1.0f / (float)mb, fp.clip_eps = h->clip_eps, fp.ent_coef = h->ent_coef, fp.vf_coef = h->vf_coef;
-  fp.act_policy = g_plan.act_policy;
 
   // ---- K3b parameters ----
   DwMaps maps;
@@ -1007,18 +973,18 @@ int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxP
       DwJob& j = dp.job[jn];
       if (int rc = make_map_tiled(&maps.a[jn], ws.xg, tiles, 8, 8)) return rc;
       if (int rc = make_map_tiled(&maps.b[jn], ws.dz[n], tiles, 2, 2)) return rc;
-      j.part = ws.part_w1[n][0], j.N = 256, j.map = jn, j.cta_begin = cta, j.n_cta = g_plan.w1, j.num_chunks = chunks;
+      j.part = ws.part_w1[n][0], j.N = 256, j.map = jn, j.cta_begin = cta, j.n_cta = kDwCtasW1, j.num_chunks = chunks;
       j.rebuild = 1, j.m0 = 128 * hh, j.net = n, j.A = fp.net[n].A, j.mask = ws.mask[n], j.w2 = fp.net[n].w2, j.b0 = fp.net[n].b0;
-      cta += g_plan.w1, ++jn;
+      cta += kDwCtasW1, ++jn;
     }
-    if (int rc = add_job(ws.part_w2[n], 16, ws.h2[n], ws.dz[n], 2, 0, g_plan.w2)) return rc;
-    if (int rc = add_job(ws.part_w0[n], 64, ws.dh1[n], ws.xg, 8, 0, g_plan.w0)) return rc;
+    if (int rc = add_job(ws.part_w2[n], 16, ws.h2[n], ws.dz[n], 2, 0, kDwCtasW2)) return rc;
+    if (int rc = add_job(ws.part_w0[n], 64, ws.dh1[n], ws.xg, 8, 0, kDwCtasW0)) return rc;
   }
-  dp.n_jobs = jn, dp.act_policy = g_plan.act_policy;
+  dp.n_jobs = jn;
 
   // ---- launches ----
-  if (int rc = opt_in_smem(tc_ppo_fwd_bwd_kernel, kFbSmemBytes, 0)) return rc;
-  if (int rc = opt_in_smem(tc_dw_kernel, kDwSmemBytes, 1)) return rc;
+  STX_CUDA_OK(opt_in_smem<tc_ppo_fwd_bwd_kernel>(kFbSmemBytes));
+  STX_CUDA_OK(opt_in_smem<tc_dw_kernel>(kDwSmemBytes));
   if (int rc = use_trap_record(st)) return rc;
   STX_CUDA_OK(launch_pdl(tc_ppo_fwd_bwd_kernel, dim3(2 * n_fb), dim3(kFbThreads), kFbSmemBytes, st, tmW0[0], tmW1[0], tmW0[1],
                          tmW1[1], fp));
@@ -1043,10 +1009,10 @@ int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxP
     const int A = nets[n]->sizes[3];
     const int64_t o_w0 = noff[n], o_b0 = o_w0 + (int64_t)D * kH, o_w1 = o_b0 + kH, o_b1 = o_w1 + (int64_t)kH * kH, o_w2 = o_b1 + kH,
                   o_b2 = o_w2 + (int64_t)kH * A;
-    add_seg(ws.part_w1[n][0], 256 * 128, g_plan.w1, kH, 128, 128, 0, kH, o_w1, n, 1);         // dW1[in][out], out 0..127
-    add_seg(ws.part_w1[n][1], 256 * 128, g_plan.w1, kH, 128, 128, 0, kH, o_w1 + 128, n, 1);   // out 128..255
-    add_seg(ws.part_w0[n], 256 * 64, g_plan.w0, kH, D, 64, 1, kH, o_w0, n, 1);      // part(j, d) -> W0[d][j]
-    add_seg(ws.part_w2[n], 256 * 16, g_plan.w2, kH, A, 16, 0, A, o_w2, n, 1);       // dW2[j][a]
+    add_seg(ws.part_w1[n][0], 256 * 128, kDwCtasW1, kH, 128, 128, 0, kH, o_w1, n, 1);         // dW1[in][out], out 0..127
+    add_seg(ws.part_w1[n][1], 256 * 128, kDwCtasW1, kH, 128, 128, 0, kH, o_w1 + 128, n, 1);   // out 128..255
+    add_seg(ws.part_w0[n], 256 * 64, kDwCtasW0, kH, D, 64, 1, kH, o_w0, n, 1);      // part(j, d) -> W0[d][j]
+    add_seg(ws.part_w2[n], 256 * 16, kDwCtasW2, kH, A, 16, 0, A, o_w2, n, 1);       // dW2[j][a]
     add_seg(ws.db_part[n], 528, n_fb, 1, kH, 528, 0, kH, o_b0, n, 0);
     add_seg(ws.db_part[n] + 256, 528, n_fb, 1, kH, 528, 0, kH, o_b1, n, 0);
     add_seg(ws.db_part[n] + 512, 528, n_fb, 1, A, 528, 0, A, o_b2, n, 0);
@@ -1069,10 +1035,5 @@ int tc_ppo_minibatch_grads(const StxMlp* actor, const StxMlp* critic, const StxP
 
 extern "C" int stx_tc_debug_set_prof_buffer(long long* buf) {
   cudaError_t e = cudaMemcpyToSymbol(stx::tc::g_prof_buf, &buf, sizeof(buf));
-  return e == cudaSuccess ? 0 : (int)e;
-}
-
-extern "C" int stx_tc_debug_set_clock_buffer(long long* buf) {
-  cudaError_t e = cudaMemcpyToSymbol(stx::tc::g_clock_buf, &buf, sizeof(buf));
   return e == cudaSuccess ? 0 : (int)e;
 }

@@ -241,11 +241,7 @@ extern "C" int stx_tc_rollout_policy(const StxMlp* actor, const void* obs, int32
   p.num_tiles = (int)((int64_t)T * E / ro::kTileM);
   p.action = action, p.log_prob = log_prob;
   p.cat_seed = cat_seed, p.cat_offset = cat_offset, p.cat_counter = cat_counter;
-  static bool attr_set = false;
-  if (!attr_set) {
-    STX_CUDA_OK(cudaFuncSetAttribute(ro::tc_rollout_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ro::kSmemBytes));
-    attr_set = true;
-  }
+  STX_CUDA_OK(stx::opt_in_smem<ro::tc_rollout_kernel>(ro::kSmemBytes));
   if (int rc = use_trap_record((cudaStream_t)stream)) return rc;
   const int cap = (max_ctas > 0 && max_ctas < kNumSMs) ? max_ctas : kNumSMs;
   const int grid = p.num_tiles < cap ? p.num_tiles : cap;

@@ -1,10 +1,10 @@
 """Exactly representable data for the fp32 CUDA-core MLP path -- TEST INFRASTRUCTURE (like exact_data.py).
 
 The fp32 path (stx_simt_gemm.cuh driven by simt_forward / simt_backward in stx_mlp.cu) accumulates in an order of its
-own: 64x64 tiles walking K in steps of 16, 32x32 panels walking it in 256-wide chunks split over even and odd k, a
-128x128 tiling behind STX_GEMM_128=1, weight gradients summed per split of the batch and then over the splits in a
-fixed order.  On random data that order shows in the last bits, so tolerance-based tests cannot see a fault confined to
-a small part of the gradient arena.  Here every value is a small integer times a power of two:
+own: 64x64 tiles walking K in steps of 16, 32x32 panels walking it in 256-wide chunks split over even and odd k, weight
+gradients summed per split of the batch and then over the splits in a fixed order.  On random data that order shows in
+the last bits, so tolerance-based tests cannot see a fault confined to a small part of the gradient arena.  Here every
+value is a small integer times a power of two:
 
 * observations in {-3..3}, weights in {-2..2}/4 (sparse), biases in {-2..2}/4, d(out) in {-3..3}/2^6, an overwrite=0
   starting gradient in {-3..3}/2^12 and grad_weight = 1/2; relu and identity networks only (every other activation is
@@ -61,7 +61,7 @@ CASES = [
     Case("k300", (300, 264, 5), "relu", 300),                         # panel K > 256 (FWD, d(input)); one split of 300 rows
     Case("cta131", (20, 64, 64, 1), "relu", 8384),                    # N = 64 at 131 CTAs: panel; DW splits of 262 rows
     Case("cta132", (20, 64, 64, 1), "relu", 8385, B=9000, ldx=24),    # 132 CTAs: 64x64, N = 1 head too; ragged last split
-    Case("bench", (64, 256, 256, 8), "relu", 32768),                  # 64x64 everywhere, 66 splits; reaches 128x128 tiles
+    Case("bench", (64, 256, 256, 8), "relu", 32768),                  # 64x64 everywhere, 66 splits
     Case("split128", (16, 128, 1), "identity", 32768, B=40000, ldx=20),  # 128 splits of 256 rows, 64x64 DW of layer 0
     Case("thin128", (16, 64, 1), "relu", 32768),                      # 128 splits on the panel DW
     Case("ragged", (48, 200, 3), "relu", 37000, B=37001, ldx=53),     # ragged tiles and splits, N = 200
@@ -81,14 +81,11 @@ def pick_splits(sizes, mb: int) -> int:
     return max(s, want)
 
 
-def tiling(mode: str, M: int, N: int, K: int, splits: int = 1, big_tiles: bool = False) -> str:
-    """'128', '64' or 'panel': the kernel launch_gemm<mode> picks."""
+def tiling(mode: str, M: int, N: int, K: int, splits: int = 1) -> str:
+    """'64' or 'panel': the kernel launch_gemm<mode> picks."""
     out_rows = K if mode == "DW" else M
     z = splits if mode == "DW" else 1
     ctas64 = -(-out_rows // 64) * -(-N // 64) * z
-    ctas128 = -(-out_rows // 128) * -(-N // 128) * z
-    if big_tiles and ctas128 >= NUM_SMS:
-        return "128"
     return "64" if ctas64 >= NUM_SMS else "panel"
 
 
@@ -102,7 +99,6 @@ class Launch:
     splits: int
     rows_per_split: int
     tile: str
-    tile128: str    # the tiling under STX_GEMM_128=1
 
     @property
     def chunks(self) -> int:
@@ -115,8 +111,7 @@ def launch_plan(sizes, M: int, d_input: bool = True) -> List[Launch]:
     """GEMM launches of stx_mlp_forward_train + stx_mlp_backward (net_grad and, if asked, d_input) in order."""
     n = len(sizes) - 1
     out = []
-    mk = lambda mode, layer, MM, N, K, s=1, rps=0: Launch(mode, layer, MM, N, K, s, rps, tiling(mode, MM, N, K, s),
-                                                          tiling(mode, MM, N, K, s, big_tiles=True))
+    mk = lambda mode, layer, MM, N, K, s=1, rps=0: Launch(mode, layer, MM, N, K, s, rps, tiling(mode, MM, N, K, s))
     for i in range(n):
         out.append(mk("FWD", i, M, sizes[i + 1], sizes[i]))
     splits = pick_splits(sizes, M)
@@ -128,10 +123,6 @@ def launch_plan(sizes, M: int, d_input: bool = True) -> List[Launch]:
         if i > 0:
             out.append(mk("DX", i, M, sizes[i], sizes[i + 1]))
     return out
-
-
-# the cases whose launches reach the 128x128 tiling when STX_GEMM_128=1 (run again in a child process with the switch)
-BIG_TILE_CASES = [c.name for c in CASES if any(l.tile128 == "128" for l in launch_plan(c.sizes, c.M))]
 
 
 # ---------------------------------------------------------------------------------------------------------------------

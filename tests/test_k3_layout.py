@@ -1,11 +1,20 @@
-"""CPU checks of the K3 data layout: the h2 sign-mask fragment order shared by K3a (writer) and K3b (reader), and the byte and
-FLOP accounting of scripts/time_k3.py."""
+"""CPU checks of the K3 data layout: the h2 sign-mask fragment order shared by K3a (writer) and K3b (reader), what K3b's
+launch plan does at the minibatches the GPU tests run, and the byte and FLOP accounting of scripts/time_k3.py."""
 import importlib.util
 import os
 
 import numpy as np
 
+from tests import exact_data as X
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+# K3b's launch plan (stx_tc_ppo.cu kDwCtasW1 / W2 / W0, kCtaPerNet, kDwStages): split-K CTAs of each job of one network
+# (dW1 runs as two row halves) and the stages of each job's input ring
+DW_CTAS = {"dW1 half": 19, "dW2": 13, "dW0": 15}
+DW_JOBS = ("dW1 half", "dW1 half", "dW2", "dW0")
+CTA_PER_NET = 66
+DW_STAGES = 4
 
 
 def _time_k3():
@@ -51,6 +60,27 @@ def test_mask_fragment_order_covers_the_tile_once_and_round_trips():
                     _, w, b = _mask_pos(t, h, i, e)
                     back[r, c] = (int(words[t, w]) >> b) & 1
     assert (back == h2).all()
+
+
+def _chunks_per_cta(mb, n_cta):
+    """64-row chunks of each CTA of a job: CTA c takes chunks c, c + n_cta, ... (my_chunks of tc_dw_kernel)."""
+    chunks = mb // 64
+    return [(chunks - c + n_cta - 1) // n_cta if c < chunks else 0 for c in range(n_cta)]
+
+
+def test_k3b_plan_at_the_dispatch_minibatches():
+    """The two minibatches of test_tc_exact_gpu.py's dispatch cases reach both ends of K3b's plan: at mb = 128 most CTAs
+    have no chunk, and at the benchmark minibatch every CTA of every job runs more chunks than its ring has stages, so
+    every ring wraps."""
+    assert sum(DW_CTAS[j] for j in DW_JOBS) == CTA_PER_NET
+    tk = _time_k3()
+    assert tk.DW_SPLIT == (DW_CTAS["dW1 half"], DW_CTAS["dW2"], DW_CTAS["dW0"])
+    small, bench = X.CRITIC_CASES[0][2], X.CRITIC_CASES[3][2]
+    assert small == 128 and bench == tk.MB
+    idle = sum(n == 0 for j in DW_JOBS for n in _chunks_per_cta(small, DW_CTAS[j]))
+    assert 2 * idle > CTA_PER_NET, f"mb = {small}: {idle} of {CTA_PER_NET} CTAs idle"
+    for j in DW_JOBS:
+        assert min(_chunks_per_cta(bench, DW_CTAS[j])) > DW_STAGES, f"mb = {bench}: a {j} CTA does not wrap its ring"
 
 
 def test_time_k3_accounting_matches_the_layouts():

@@ -27,7 +27,7 @@ def test_cases_cover_every_tiling_and_split_path():
     for name, p in plans.items():
         dw = next(l for l in p if l.mode == "DW")
         print(f"{name:9s} splits {dw.splits:3d} x {dw.rows_per_split:4d} rows: "
-              + " ".join(f"{l.mode}{l.layer}:{l.tile}{'/' + l.tile128 if l.tile128 == '128' else ''}" for l in p))
+              + " ".join(f"{l.mode}{l.layer}:{l.tile}" for l in p))
     for mode in ("FWD", "DX", "DW"):
         tiles = {l.tile for _, l in every if l.mode == mode}
         assert {"panel", "64"} <= tiles, f"{mode}: tilings reached {tiles}"
@@ -46,9 +46,6 @@ def test_cases_cover_every_tiling_and_split_path():
             ls = [l for _, l in every if l.mode == mode and l.tile == tile]
             assert any(l.K % 16 for l in ls) and any(l.N % 16 for l in ls), f"{mode} {tile}: K and N not multiples of 16"
     assert {1, 5} <= {c.M for c in S.CASES}
-    assert S.BIG_TILE_CASES, "no case reaches the 128x128 tiling under STX_GEMM_128=1"
-    for name in S.BIG_TILE_CASES:
-        assert any(l.tile128 == "128" for l in plans[name])
     assert any(c.gathered and c.ldx > c.sizes[0] for c in S.CASES)
 
 

@@ -3,7 +3,7 @@ references, in three tiers.
 
 A. Exact data (tests/simt_exact_data.py): every GEMM, split and reduction is exact in any order, so forward output,
    parameter gradients (overwrite 1 and 0), d(input), the d(input)-only call, gathered strided input and the inference
-   entry must equal the oracle bit for bit, on every tiling and split path, and again under STX_GEMM_128=1.
+   entry must equal the oracle bit for bit, on every tiling and split path.
 B. Element-wise epilogues: "identity sandwich" networks [N, N, N] with W0 = W1 = I and b1 = 0.  Each GEMM then adds
    exact zeros to one product, so the output IS the kernel's f(U) or f(LN(U)), d(input) IS its activation / LayerNorm
    backward of d(out), and the gradient arena holds the column sums (db0, or LayerNorm dgamma / dbeta).  Each element is
@@ -13,10 +13,6 @@ B. Element-wise epilogues: "identity sandwich" networks [N, N, N] with W0 = W1 =
 C. Composition at the shipped shapes against the fp64 oracle: per-element running error bounds where the forward is
    exact (relu at M = 32768), per-tensor norm-wise bounds for LayerNorm + silu and silu networks.
 """
-import os
-import subprocess
-import sys
-
 import numpy as np
 import pytest
 import torch
@@ -25,7 +21,6 @@ from oracle import ppo_oracle as O
 from tests import simt_exact_data as S
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 U = 2.0 ** -24
 ACTS = ["relu", "tanh", "silu", "elu", "gelu", "sigmoid", "softplus", "identity"]
 
@@ -96,26 +91,6 @@ def test_exact_case(name):
     again = _run_exact(pb)
     for k in got:
         assert np.array_equal(got[k], again[k]), f"{name}: {k} differs between two identical calls"
-
-
-def _big_tile_child(path: str) -> None:
-    np.savez(path, **{f"{n}.{k}": v for n in S.BIG_TILE_CASES for k, v in _run_exact(S.make_problem(S.CASE_BY_NAME[n])).items()})
-
-
-def test_exact_cases_under_128x128_tiles(tmp_path):
-    """STX_GEMM_128=1 (read once per process, hence a child): the cases whose launches reach 128x128 tiles give the
-    oracle's bits, i.e. the same bits as the default tilings."""
-    path = str(tmp_path / "big.npz")
-    code = ("import os; os.environ['STX_GEMM_128'] = '1'; import sys; sys.path.insert(0, os.getcwd());"
-            f"import tests.test_simt_mlp_gpu as m; m._big_tile_child({path!r}); print('child-ok')")
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=900, cwd=ROOT)
-    assert "child-ok" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
-    res = np.load(path)
-    for n in S.BIG_TILE_CASES:
-        c = S.CASE_BY_NAME[n]
-        print(f"{n}: 128x128 on " + " ".join(f"{l.mode}{l.layer}" for l in S.launch_plan(c.sizes, c.M) if l.tile128 == "128"))
-        _check_exact({k: res[f"{n}.{k}"] for k in ("out", "out_inf", "grad", "grad_acc", "d_input", "d_input_only")},
-                     S.reference(S.make_problem(c)), f"STX_GEMM_128=1 {n}")
 
 
 def test_layernorm_wider_than_1024_is_refused():

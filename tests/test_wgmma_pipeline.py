@@ -66,9 +66,8 @@ def test_kernel_has_no_call_and_pipelines_its_mma(compiled, src, kernel):
 
 
 def test_k3a_keeps_its_bias_gradient_butterfly_in_registers(compiled):
-    # K3a runs at the full register file: ptxas parks one 64-bit value, the profiling start clock, which is written at entry
-    # and read at exit (one STL.64 + one LDL.64).  Local memory inside the tile loop (the colsum_half butterfly in local memory
-    # was ~250 accesses per thread and tile) fails this.
+    # K3a runs at the full register file (255 registers) without local memory.  The colsum_half butterfly in local memory was
+    # ~250 accesses per thread and tile; one L2 policy kept live across the tile loop spills too (hence one per store site).
     sass = _sass(compiled["stx_tc_ppo.cu"][1], "tc_ppo_fwd_bwd_kernel")
     local = [ln.strip() for ln in sass if re.search(r"\b(LDL|STL)\b", ln)]
-    assert len(local) <= 2, f"K3a: {len(local)} local-memory accesses:\n" + "\n".join(local[:8])
+    assert not local, f"K3a: {len(local)} local-memory accesses:\n" + "\n".join(local[:8])
